@@ -1,6 +1,6 @@
 """Benchmark of the StreamYOLO hot path: frame-pairs/s of forward+loss (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model l] [--batch 8]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--model l] [--batch 8] [--dump-outputs DIR]
 
 One process per GPU (torchrun sets RANK/LOCAL_RANK/WORLD_SIZE for N > 1).  A "step" is one pass of
 the hot path -- DFPPAFPN (CSPDarknet + PAFPN on both frames, DFP fusion) + TALHead + SimOTA/TAL loss,
@@ -13,11 +13,14 @@ value      whole-job pairs/s with inputs resident in HBM, the step replayed as o
 e2e        same metric through the public API call ``model(x, targets)`` contract with HOST (pinned)
            inputs: every step copies the frame pairs + labels host->device (double buffered on a copy
            stream, like the reference's DataPrefetcher) and reads the 6 loss scalars back.
-roofline   dominant kernel (tcgen05 implicit-GEMM conv) timed alone, live, with CUDA events on its
+roofline   dominant kernel (wgmma implicit-GEMM conv) timed alone, live, with CUDA events on its
            heaviest layer shape; achieved algorithmic TFLOP/s vs the measured cuBLAS bf16 peak.
 cpu_baseline / --impl reference
            the CPU oracle (oracle/, a restatement of the reference's PyTorch path; the reference itself
            needs the un-installable yolox package) on the host cores, bounded sample.
+--dump-outputs DIR
+           after the timed steps, writes what the timed path returned in its last step -- the six loss scalars of
+           ``model(x, targets)`` -- as DIR/<name>.npy (float32).  The inputs are seeded, so two builds can be compared.
 """
 import argparse
 import json
@@ -42,13 +45,14 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return {"burst": d.get("bf16_tflops", 1590.0), "sustained": d.get("bf16_tflops_sustained", 1400.0),
-                "hbm": d.get("hbm_gbs", 6650.0), "source": "measured"}
-    return {"burst": 1590.0, "sustained": 1400.0, "hbm": 6650.0, "source": "fallback"}
+        return {"burst": d.get("bf16_tflops", 989.0), "sustained": d.get("bf16_tflops_sustained", 989.0),
+                "hbm": d.get("hbm_gbs", 3350.0), "source": "measured"}
+    # H100 SXM data sheet (dense bf16, HBM3), not a measurement
+    return {"burst": 989.0, "sustained": 989.0, "hbm": 3350.0, "source": "datasheet"}
 
 
 class ClockSampler:
-    """SM clock / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe): NVML polled every 2 ms
+    """SM clock / throttle reasons sampled DURING the timed region: NVML polled every 2 ms
     from a thread (the timed region can be shorter than nvidia-smi's start-up), `nvidia-smi -lms` as the fallback."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -152,7 +156,7 @@ def build_model(tag, device):
 
 def time_dominant_kernel(tag, batch, peaks):
     """The heaviest conv of the net (head tower 3x3 at stride 8) alone: a CUDA graph of 16 launches that rotate
-    over 8 input/output buffer sets (8 x 74 MB > the 126 MB L2, so every launch reads its operands from HBM and
+    over 8 input/output buffer sets (8 x 74 MB > the 50 MB L2, so every launch reads its operands from HBM and
     no host launch overhead is inside the timed region), CUDA events around the replay, best of 5."""
     from streamyolo_b200 import ops
     from streamyolo_b200.ops import View
@@ -190,14 +194,10 @@ def time_dominant_kernel(tag, batch, peaks):
     ms = best
     flops = 2.0 * n * h * w * c * c * 9
     ach = flops / (ms * 1e-3) / 1e12
-    return {"bound": "tensor", "kernel": f"conv_tc_kernel<{min(256, c)}> 3x3 s1 {c}->{c} @{n}x{h}x{w}",
+    return {"bound": "tensor", "kernel": f"conv_tc_kernel 3x3 s1 {c}->{c} @{n}x{h}x{w}",
             "achieved": round(ach, 1), "peak": peaks["burst"], "unit": "TFLOP/s", "frac": round(ach / peaks["burst"], 4),
             "peak_source": peaks["source"] + " cuBLAS bf16 burst", "ms_per_launch": round(ms, 4),
             "algorithmic_flop_per_launch": flops,
-            # dram__bytes_read.sum + dram__bytes_write.sum of this launch shape (8x75x120, 256->256) from the ncu --set full
-            # capture summarised in profiles/r01_ncu_full_summary.txt (38.12 MB read + 2.96 MB written; the 36.9 MB
-            # output is still L2-resident when the kernel ends).  Only meaningful for that shape.
-            "traffic": (41.07e6 if (n, c) == (8, 256) else None), "traffic_unit": "bytes/launch (ncu, r01)",
             "algorithmic_bytes_per_launch": 2 * n * h * w * c * 2 + 9 * c * c * 2,
             "how": "graph of 16 launches over 8 rotating buffer sets (operands > L2), CUDA events, best of 5"}
 
@@ -391,7 +391,7 @@ def measure_eval_modes(model, dev, batch, steps):
 def run_reference(args, rank):
     """--impl reference: the reference's own CPU path for this workload, timed on the host cores with EXACTLY the --steps /
     --warmup it prints.  It is the fp32 oracle (kind "port"): the reference's modules need the un-vendored yolox==0.3.0
-    package and /root/reference does not exist on the GPU box (DESIGN.md section 6); the oracle is pinned to outputs of the
+    package and the reference checkout is not needed at run time (DESIGN.md section 6); the oracle is pinned to outputs of the
     unmodified reference files (oracle/make_golden.py).  Each step = one forward+loss over a bounded sample of the per-GPU
     batch (2 frame pairs of the same 600x960 workload), so that the run stays within a few minutes."""
     if rank != 0:
@@ -410,7 +410,7 @@ def run_reference(args, rank):
                        "device": "host CPU cores (the reference's own CPU path: fp32 PyTorch)"},
             "cpu_baseline": {"value": round(v, 4), "unit": "pairs/s", "cores": torch.get_num_threads(), "kind": "port",
                              "sample": "%d pairs/step x %d steps (+%d warm-up), fp32 oracle restatement of the reference PyTorch "
-                                       "path (yolox not installable, /root/reference absent on the GPU box)" % (pairs, steps, warmup)},
+                                       "path (the yolox package is not installable)" % (pairs, steps, warmup)},
             "e2e": {"value": round(v, 4), "unit": "pairs/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
     emit(json.dumps(line))
 
@@ -447,7 +447,10 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-train", action="store_true", help="skip the training-step measurements (configs 2-4)")
     ap.add_argument("--no-extras", action="store_true", help="skip the sustained run, eval / on_pipe modes and the conv-family timing")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3)
 
     from streamyolo_b200 import dist as sydist
@@ -456,7 +459,7 @@ def main():
         run_reference(args, rank)
         return
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py --impl ours needs a B200 (no CPU path)")
+        raise SystemExit("bench.py --impl ours needs an H100 (no CPU path)")
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     # keep stdout to the one JSON line: whatever NCCL_DEBUG level the launcher asked for goes to a file (even WARN prints
@@ -525,6 +528,11 @@ def main():
         sydist.barrier()
         ms_total = sydist.max_over_ranks(e0.elapsed_time(e1), dev)
         clocks = sampler.stop()
+        if args.dump_outputs and rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            for name, v in zip(LOSS_KEYS, loss_vec.detach().float().cpu()):
+                np.save(os.path.join(args.dump_outputs, name + ".npy"), v.numpy().astype(np.float32).reshape(1))
         ms_step = ms_total / args.steps
         value = world * B / (ms_step * 1e-3)
 
@@ -647,7 +655,7 @@ def main():
                                "%d pairs/GPU" % (args.model, B),
                    "pairs_per_gpu": B, "global_pairs": world * B, "parallelism": "dp%d (no data-path collective)" % world,
                    "cuda_graph": not args.no_graph,
-                   "l2": "per-step inputs (%.0f MB) + activations (>1 GB) exceed the 126 MB L2" % (h2d / 1e6)},
+                   "l2": "per-step inputs (%.0f MB) + activations (>1 GB) exceed the 50 MB L2" % (h2d / 1e6)},
         "e2e": {"value": round(e2e_value, 2), "unit": "pairs/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 24,
                 "ms_per_step": round(e2e_ms, 4), "note": "pinned fp32 frames+labels copied every step on a copy stream "
                                                         "(double buffered), 6 loss scalars read back"},
@@ -679,11 +687,8 @@ def main():
                             "peak_source": peaks["source"] + " cuBLAS bf16 burst", "launches": fam_n,
                             "avg_launch_ms": round(fam_ms / fam_n, 5), "sum_launch_ms": round(fam_ms, 4),
                             "algorithmic_flop_per_step": B * gf * 1e9,
-                            # dram__bytes_read.sum + dram__bytes_write.sum per launch, averaged over the family's 114 launches of
-                            # one step (ncu launch list of this command, profiles/r02_launch_summary_final.txt; StreamYOLO-l, 8 pairs only)
-                            "traffic": (50.5e6 if (args.model, B) == ("l", 8) else None), "traffic_unit": "bytes/launch (ncu launch list profiles/r02_launch_summary_final.txt: 5761 MB DRAM read+written over the 114 conv launches)",
                             "how": "the step's conv launches re-issued alone, in order, as one CUDA graph on the step's own buffers; "
-                                   "CUDA events around the replay, best of 5; ncu launch list of the step: profiles/"}
+                                   "CUDA events around the replay, best of 5"}
     if not args.no_cpu_baseline:
         try:
             v, sec = cpu_oracle_run(args.model, 2, 2, 1)

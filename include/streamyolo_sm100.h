@@ -1,5 +1,5 @@
 /*
- * libstreamyolo_sm100.so -- C ABI of the B200-native StreamYOLO hot path.
+ * libstreamyolo_sm100.so -- C ABI of the H100-native StreamYOLO hot path.
  *
  * This is the drop-in boundary of SURVEY.md section 8(b): plain `extern "C"` entry
  * points, raw device pointers + sizes + a cudaStream_t, no torch types.  The host
@@ -16,7 +16,7 @@
  *     a channel slice of a wider concat buffer (pitch, slice offsets and c are
  *     multiples of 8 so that every pixel row is 16-byte aligned).
  *   - conv weights are bf16, packed [Cout][kh*kw][Cin] (K-major GEMM B operand).
- *   - the library requires an sm_100a device; there is no other code path.
+ *   - the library requires an sm_90a device; there is no other code path.
  *
  * Each entry point cites the reference interface it replaces (paths relative to
  * /root/reference; "[yolox]" = the un-vendored yolox==0.3.0 dependency).
@@ -36,7 +36,7 @@ typedef struct CUstream_st* sy_stream_t; /* == cudaStream_t */
 enum {
   SY_OK = 0,
   SY_EINVAL = 1,   /* bad shape / alignment / null pointer */
-  SY_EARCH = 2,    /* device is not sm_100 */
+  SY_EARCH = 2,    /* device is not sm_90 */
   SY_ELAUNCH = 3,  /* CUDA launch or driver error (see sy_last_error_string) */
   SY_EWORKSPACE = 4
 };
@@ -50,7 +50,7 @@ typedef struct {
 /* -------- runtime ---------------------------------------------------------- */
 const char* sy_last_error_string(void);
 int sy_version(void);
-/* 0 when the current device is sm_100 and the driver exposes cuTensorMapEncodeTiled. */
+/* 0 when the current device is sm_90 and the driver exposes cuTensorMapEncodeTiled. */
 int sy_check_device(void);
 
 /* Mark [ptr, ptr + bytes) as a persisting-L2 access window for the kernels subsequently launched on `stream` (inherited by
@@ -113,7 +113,7 @@ typedef struct {
 
 /* Rows of the statistics workspace (= SM count: one row per persistent CTA). */
 int sy_conv_stat_rows(void);
-/* tcgen05 implicit-GEMM kernel (TMA -> smem -> UMMA -> TMEM -> epilogue).  In RAW mode with
+/* wgmma implicit-GEMM kernel (TMA -> smem -> wgmma -> register accumulators -> epilogue).  In RAW mode with
  * stat_partials it also accumulates per-channel (sum, sum of squares) of the stored values per
  * statistics group, one partial row per CTA; with bn[] the persistent grid (all CTAs co-resident)
  * ends with a grid barrier and finalizes BatchNorm in parallel: batch statistics -> scale/shift,

@@ -24,7 +24,7 @@ extern "C" int sy_version(void) { return 100; }
 
 // L2 residency of the conv -> normalise hand-off: the raw conv output of a train-mode BaseConv is written by one kernel and
 // read back by the next (the BatchNorm statistics sit in between).  All layers whose raw tensor fits draw it from ONE arena;
-// marking that address window "persisting" on the launching stream keeps those lines in the set-aside part of the 126 MB L2,
+// marking that address window "persisting" on the launching stream keeps those lines in the set-aside part of the 50 MB L2,
 // so the normalise pass reads them from L2 and the next layer overwrites them before they are ever written back to HBM.
 // Returns the usable window size in *granted (0: the device grants no persisting L2).  bytes = 0 clears the window.
 extern "C" int sy_l2_persist_window(void* ptr, size_t bytes, float hit_ratio, size_t* granted, sy_stream_t stream_) {
@@ -63,8 +63,8 @@ extern "C" int sy_check_device(void) {
   int major = 0, minor = 0;
   SY_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   SY_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  SY_REQUIRE(major == 10 && minor == 0, SY_EARCH, "device %d is sm_%d%d; libstreamyolo_sm100 needs sm_100 (B200)", dev,
-             major, minor);
+  SY_REQUIRE(major == 9 && minor == 0, SY_EARCH, "device %d is sm_%d%d; libstreamyolo needs sm_90 (H100)", dev, major,
+             minor);
   void* ptr = nullptr;
   cudaDriverEntryPointQueryResult qres;
   SY_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres));

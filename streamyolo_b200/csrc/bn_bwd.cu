@@ -298,7 +298,7 @@ extern "C" int sy_bn_act_backward(const SyBnActBwdDesc* d, sy_stream_t stream_) 
   const int G = raw.c / 8, ppb = kBwdThreads / G;
   const int unroll_a = (var_a == 1 || var_a == 2) ? 2 : 4;
   long long blocks = (q.npix + (long long)ppb * unroll_a - 1) / ((long long)ppb * unroll_a);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   __nv_bfloat16* drp = reinterpret_cast<__nv_bfloat16*>(dr.ptr);
   switch (var_a) {
     case 1: bn_act_bwd_apply_kernel<2, 3><<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, drp, dr.pitch); break;

@@ -303,7 +303,7 @@ __global__ void copy_kernel(const __nv_bfloat16* __restrict__ x, long long xp, _
 
 static inline int grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
-  const long long cap = 148LL * 16;
+  const long long cap = (long long)sm_count() * 16;
   return (int)(b < cap ? (b < 1 ? 1 : b) : cap);
 }
 
@@ -359,8 +359,8 @@ extern "C" int sy_bn_act_apply(SyTensor x, const float* scale, const float* shif
   const int ppb = kApplyThreads / (x.c / 8);
   // enough blocks for one pass of kApplyUnroll pixels per thread, capped at one wave of 3 resident blocks per SM
   const long long want = (npix + (long long)ppb * kApplyUnroll - 1) / ((long long)ppb * kApplyUnroll);
-  long long cap = 148LL * 3;   // one wave of 3 resident blocks per SM (measured best: 6.188 vs 6.198 ms/step at 6 per SM)
-  if (const char* e = getenv("SY_APPLY_CAP")) cap = 148LL * (atoi(e) > 0 ? atoi(e) : 3);   // tuning aid: blocks per SM
+  long long cap = (long long)sm_count() * 3;   // one wave of 3 resident blocks per SM
+  if (const char* e = getenv("SY_APPLY_CAP")) cap = (long long)sm_count() * (atoi(e) > 0 ? atoi(e) : 3);   // tuning aid: blocks per SM
   const int grid = (int)(want < 1 ? 1 : (want < cap ? want : cap));
   const bool has_res = rp != nullptr;
   int hints = 0;
@@ -387,7 +387,7 @@ extern "C" int sy_upsample_nearest(SyTensor x, SyTensor y, sy_stream_t stream_) 
   const long long total = (long long)y.n * y.h * y.w * (y.c / 8);
   (void)total;
   const int up_rows = y.n * y.h;
-  upsample_nearest_kernel<<<up_rows < 148 * 8 ? up_rows : 148 * 8, 256, 0, stream>>>(CBF(x.ptr), x.pitch, x.n, x.h, x.w, BF(y.ptr),
+  upsample_nearest_kernel<<<up_rows < sm_count() * 8 ? up_rows : sm_count() * 8, 256, 0, stream>>>(CBF(x.ptr), x.pitch, x.n, x.h, x.w, BF(y.ptr),
                                                                                      y.pitch, y.h, y.w, x.c);
   return launch_status("upsample_nearest_kernel");
 }
@@ -417,7 +417,7 @@ extern "C" int sy_copy(SyTensor x, SyTensor y, sy_stream_t stream_) {
   {
     const int G = x.c / 8, ppb = G <= 256 ? 256 / G : 1;
     const long long want = (npix + 4LL * ppb - 1) / (4LL * ppb);
-    copy_kernel<<<(int)(want < 1 ? 1 : (want < 148 * 8 ? want : 148 * 8)), 256, 0, stream>>>(CBF(x.ptr), x.pitch, BF(y.ptr), y.pitch,
+    copy_kernel<<<(int)(want < 1 ? 1 : (want < sm_count() * 8 ? want : sm_count() * 8)), 256, 0, stream>>>(CBF(x.ptr), x.pitch, BF(y.ptr), y.pitch,
                                                                                           npix, x.c);
   }
   return launch_status("copy_kernel");

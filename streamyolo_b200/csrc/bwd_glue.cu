@@ -307,7 +307,7 @@ __global__ void spp_bwd_gather_kernel(const uint8_t* amax, const __nv_bfloat16* 
 
 static inline int grid_cap(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
-  return (int)(b < 1 ? 1 : (b < 148LL * 16 ? b : 148LL * 16));
+  return (int)(b < 1 ? 1 : (b < (long long)sm_count() * 16 ? b : (long long)sm_count() * 16));
 }
 
 }  // namespace sy

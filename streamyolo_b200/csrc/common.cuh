@@ -1,4 +1,4 @@
-// Shared helpers for libstreamyolo_sm100 (sm_100a only).
+// Shared helpers for libstreamyolo_sm100.so (built for sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -45,6 +45,20 @@ inline bool view_ok(const SyTensor& t) {
 }
 
 __host__ __device__ inline int cdiv(int a, int b) { return (a + b - 1) / b; }
+
+// SM count of the current device (cached; 132 = an H100 SXM when there is no device, for host-only queries).  Grid-stride
+// kernels cap their grids at a few waves of it.
+inline int sm_count() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      cudaGetLastError();
+      n = 132;
+    }
+  }
+  return n;
+}
 
 // ---- programmatic dependent launch (PDL) -------------------------------------------------
 // Kernels launched through launch_pdl() may be scheduled while their predecessor on the stream is still

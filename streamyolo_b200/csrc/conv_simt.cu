@@ -1,4 +1,4 @@
-// CUDA-core kernels: direct convolution (device-side cross-check of the tcgen05 kernel and
+// CUDA-core kernels: direct convolution (device-side cross-check of the wgmma kernel and
 // the path for shapes it rejects), the Focus stem, and per-channel statistic partials.
 #include "common.cuh"
 
@@ -173,7 +173,7 @@ extern "C" int sy_conv2d_simt(const SyConvDesc* d, sy_stream_t stream_) {
     p.res = reinterpret_cast<const __nv_bfloat16*>(d->res.ptr); p.res_pitch = d->res.pitch;
   }
   const long long total = (long long)p.N * p.Ho * p.Wo * (p.Cout / 8);
-  const int blocks = (int)((total + 127) / 128 < 148 * 16 ? (total + 127) / 128 : 148 * 16);
+  const int blocks = (int)((total + 127) / 128 < sm_count() * 16 ? (total + 127) / 128 : sm_count() * 16);
   conv_simt_kernel<<<blocks, 128, 0, stream>>>(p);
   return launch_status("conv_simt_kernel");
 }
@@ -187,7 +187,7 @@ extern "C" int sy_focus_pack(const float* x, int32_t b, int32_t in_ch, int32_t h
   SY_REQUIRE(y.n == frames * b && y.h == h / 2 && y.w == w_px / 2 && y.c == 64, SY_EINVAL,
              "focus_pack: output view must be [frames*b, h/2, w/2, 64]");
   const int rows = y.n * y.h;                                   // one block pass per output row
-  const int blocks = rows < 148 * 16 ? rows : 148 * 16;
+  const int blocks = rows < sm_count() * 16 ? rows : sm_count() * 16;
   focus_pack_kernel<<<blocks, 256, 0, stream>>>(x, b, in_ch, h, w_px, frames, reinterpret_cast<__nv_bfloat16*>(y.ptr),
                                                 y.pitch);
   return launch_status("focus_pack_kernel");

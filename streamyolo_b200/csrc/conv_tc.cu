@@ -1,37 +1,37 @@
-// Implicit-GEMM convolution on the Blackwell tensor cores (sm_100a).
+// Implicit-GEMM convolution on the Hopper tensor cores (sm_90a, wgmma).
 //
 //   M = 128 output pixels: 128 consecutive pixels of the flattened (n, oh, ow) space ("linear" tiles, the default), a
 //       TH x TW patch of one image, or a 16 x 8 patch with its input halo (template parameter AM, see below)
-//   N = output channels (BN = 64/128/256 per tile, chosen per layer)
+//   N = output channels (BN = 64/128 per tile, chosen per layer)
 //   K = taps * Cin, walked as (tap, 64-channel block)
 //
 // Operand movement is im2col-free: for every (tap, channel block) ONE TMA load (im2col mode for
 // linear tiles, tiled mode for patches) brings the shifted input pixels [128][64ch] straight from the NHWC tensor into a
 // 128B-swizzled shared-memory tile (out-of-bounds = zero padding = the conv padding;
 // stride-2 convs use the tensor map's element strides), and one 3-D TMA load brings the
-// [BN][64] weight slab.  A single elected thread issues tcgen05.mma (M=128, N=BN, K=16)
-// with both operands in shared memory and the fp32 accumulator in TMEM (double
-// buffered), so the epilogue of tile i overlaps the main loop of tile i+1.
+// [BN][64] weight slab.  Two consumer warpgroups issue wgmma.mma_async (M=64 each, N=BN, K=16) with both operands in
+// shared memory and the fp32 accumulators in registers.
 //
-// Warp roles (640 threads, persistent CTA, one per SM):
-//   warps 0-7   convert: per 64-column slab of the accumulator TMEM -> registers -> (raw | folded BN + SiLU + residual) ->
-//               bf16 -> 128B-swizzled shared staging tile (team mode: the two warpgroups take alternate slabs)
+// Warp roles (640 threads = five warpgroups, persistent CTA, one per SM):
+//   warps 0-7   MMA + convert: warpgroup wg computes rows [64 wg, +64) of the tile, then per 64-column slab converts its
+//               accumulators (raw | folded BN + SiLU + residual) to bf16 in a 128B-swizzled shared staging tile
 //   warps 8-15  statistics: per-channel (sum, sum of squares) of the staged tile in per-lane register accumulators that persist
 //               across slabs and tiles (overlaps the next slab's conversion)
 //   warp 16 TMA store (one 4-D store per slab; the tensor map clips the tile to the tensor / the channel slice)
-//   warp 17 TMEM alloc + weight (B) loads   warp 18 activation (A) loads   warp 19 MMA issuer
-// PAIR = true: the grid is launched as clusters of two CTAs sharing ONE tcgen05.mma.cta_group::2 stream (see below).
+//   warp 17 barrier init + weight (B) loads   warp 18 activation (A) loads   warp 19 idle
+// setmaxnreg moves registers from warps 16-19 to the MMA and statistics warpgroups (kRegs*).
+// BN = 256 is not offered: 64 x 256 fp32 accumulators are 128 registers per thread, more than the MMA warpgroups can hold.
 //
 // Train-mode BatchNorm is folded into this kernel as far as the grid-wide dependency allows:
 // every CTA accumulates per-channel (sum, sum of squares) of the values it stored, per
 // statistics group (current / support frames), and writes ONE partial row.  All CTAs of the
 // persistent grid are co-resident (one per SM), so the kernel ends with a grid-wide barrier after
-// which every CTA reduces a slice of the channels over the <= 148 rows in a fixed order
+// which every CTA reduces a slice of the channels over the rows (one per SM) in a fixed order
 // (deterministic), updates the running statistics and publishes scale/shift for the normalise+SiLU
 // pass.  (Two such kernels must not run concurrently on one GPU: the barrier needs the whole grid.)
 //
 // Replaces the cuDNN conv + ATen BN/SiLU triplet behind [yolox] BaseConv
-// (/root/reference/exps/model/darknet.py:115-165, dfp_pafpn.py:33-105, tal_head.py:55-104).
+// (exps/model/darknet.py:115-165, dfp_pafpn.py:33-105, tal_head.py:55-104 of StreamYOLO).
 #include <cuda.h>
 #include <stdio.h>
 
@@ -43,13 +43,19 @@ namespace tc {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;              // bf16 elements = one 128-byte swizzle row
-constexpr int kThreads = 640;
-constexpr int kEpiThreads = 256;    // convert warps 0-7
+constexpr int kThreads = 640;       // five warpgroups
+// registers per thread after setmaxnreg: the launch grants 96 x 640; the load/store warpgroup (warps 16-19) keeps 32 and
+// hands the rest to the MMA warpgroups (accumulators: BN / 2 registers) and the statistics warpgroups (per-lane sums)
+constexpr int kRegsLaunch = 96;
+constexpr int kRegsMma = 104;
+constexpr int kRegsStats = 120;
+constexpr int kRegsIo = 32;
+static_assert(2 * kRegsMma + 2 * kRegsStats + kRegsIo <= 5 * kRegsLaunch, "register budget of one CTA");
+constexpr int kEpiThreads = 256;    // MMA + convert warps 0-7
 constexpr int kTailThreads = 512;   // convert + statistics warps run the kernel tail (partials, grid barrier, finalize, apply)
 constexpr int kABytes = kBlockM * 128;   // 16 KiB per stage
 constexpr int kMaxStages = 8;
-// 64-deep K sub-blocks per pipeline stage: two (one barrier round per K = 128) halve the per-round hand-shake
-// cost, which dominates narrow tiles; BN = 256 keeps one so that four 48 KiB stages fit (ring depth matters more)
+// 64-deep K sub-blocks per pipeline stage: two (one barrier round per K = 128) halve the per-round hand-shake cost
 
 struct BnSeg {
   const float* gamma; const float* beta;
@@ -63,20 +69,15 @@ struct Params {
   int th, tw, tiles_x, tiles_y;
   int m_tiles, n_tiles, total_tiles;
   FastDiv fd_m_tiles, fd_per_img, fd_tiles_x, fd_tw;
-  // pair mode (cta_group::2): the tile loop walks PAIR tiles = 256 consecutive output pixels x BN channels; CTA rank r of the
-  // pair owns M tile 2 * m2 + r (it may lie past the end of the tensor: loads zero-fill, the store clips)
-  int m_tiles2, total_tiles2;
-  FastDiv fd_m_tiles2;
   // linear tiles (LIN): an M tile is 128 consecutive output pixels of the flattened (n, oh, ow) space
   int P_total;              // N * Ho * Wo
   int gp;                   // first output pixel of statistics group 1 (== P_total: single group)
   FastDiv fd_hw, fd_wo;
   int cblocks, kblocks, stages;
   int stage_tiles;          // 1 or 2 epilogue staging tiles
-  int team;                 // 1: the two convert warpgroups work on alternate slabs (needs stage_tiles == 2, RAW mode)
   // halo mode (AM == 2)
   int stagesA;              // halo ring depth
-  int halo_pitch;           // pixels per halo row in shared memory (16, or 10 with debug flag 128)
+  int halo_pitch;           // pixels per halo row in shared memory (10, or 16 with debug flag 128)
   int halo_bytes;           // stage stride (multiple of 1 KiB)
   int halo_tx;              // bytes one halo load delivers
   int mode, act;
@@ -104,7 +105,7 @@ struct Params {
   int ap_act;
   long long* timeline;      // debug: CTA 0 records (event id, clock) pairs; nullptr in production
   int timeline_cap;
-  int debug_flags;          // debug: 1 = skip the MMAs, 2 = skip the TMA loads (barriers still cycle)
+  int debug_flags;          // debug: 2 = skip the TMA loads (barriers still cycle)
   float* dbg_f32;           // validation: fp32 accumulators [pixel][Cout] written next to the stored result (nullptr in production)
 };
 
@@ -119,7 +120,6 @@ __device__ __forceinline__ void tl_rec(const Params& p, int& n, int role, int ph
 }
 
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-// staging-tile hand-off between the 8 epilogue warps and the store warp (warp 3): 256 + 32 threads
 // staging-tile hand-off between the 8 convert warps, the 8 statistics warps and the store warp: 256 + 256 + 32 threads
 // One or two staging tiles (Params::stage_tiles; slab j uses tile j & 1 when there are two, so that the TMA store /
 // statistics of one slab overlap the conversion of the next -- worth an operand stage only for epilogue-bound layers);
@@ -129,43 +129,16 @@ __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: 
 //               tile b are done; the convert warps WAIT on it before overwriting the tile
 //   staged(b) : convert warps arrive after writing tile b (+ proxy fence); store and statistics warps WAIT on it
 // so the convert warps never wait for the statistics arithmetic or the store issue, only for the tile to be read.
-// Team mode (Params::team, epilogue-bound RAW layers with two staging tiles): the two convert warpgroups stop sharing a slab;
-// warpgroup t converts every slab of parity t on its own, into staging tile t -- two slabs in flight, the latency chain
-// TMEM load -> pack -> wait free -> store -> fence -> arrive of one overlaps the other's.  The barriers of tile t then
-// count 128 + 256 + 32 = 416 threads.
 __device__ __forceinline__ void bar_free_wait(int b, int n = 544) { asm volatile("bar.sync %0, %1;" ::"r"(2 + 4 * b), "r"(n) : "memory"); }
 __device__ __forceinline__ void bar_free_arrive(int b, int n = 544) { asm volatile("bar.arrive %0, %1;" ::"r"(2 + 4 * b), "r"(n) : "memory"); }
 __device__ __forceinline__ void bar_staged_wait(int b, int n = 544) { asm volatile("bar.sync %0, %1;" ::"r"(3 + 4 * b), "r"(n) : "memory"); }
 __device__ __forceinline__ void bar_staged_arrive(int b, int n = 544) { asm volatile("bar.arrive %0, %1;" ::"r"(3 + 4 * b), "r"(n) : "memory"); }
 __device__ __forceinline__ void bar_stats_done() { asm volatile("bar.sync 5, 512;" ::: "memory"); }
 
-// K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row atoms 1024 bytes apart.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);   // start address      bits [0,14)
-  d |= (uint64_t)(1024u >> 4) << 32;          // stride byte offset  bits [32,46)
-  d |= (uint64_t)1 << 46;                     // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                     // SWIZZLE_128B
-  return d;
-}
-// general form: stride between 8-row atoms and the swizzle phase ("matrix base offset") of a start address that is not
-// 1024-byte aligned
-__device__ __forceinline__ uint64_t make_smem_desc_ex(uint32_t saddr, uint32_t sbo_bytes, uint32_t base_offset) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(base_offset & 7u) << 49;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// kind::f16 instruction descriptor: D=f32, A=B=bf16, both K-major, M=128.
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kBlockM >> 4) << 24);
-}
-
-__host__ __device__ constexpr uint32_t make_idesc_m(int n, int m) {      // M = 256: the cta_group::2 pair
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
+// K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row atoms `sbo` bytes apart (1 KiB for a TMA-written tile).
+// The leading byte offset is unused by K-major swizzled layouts.
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t sbo = 1024u, uint32_t base_offset = 0u) {
+  return make_gmma_desc(saddr, 16u, sbo, base_offset);
 }
 
 constexpr int kSlabCols = 64;                  // epilogue slab: 64 bf16 columns = one 128-byte swizzled row
@@ -174,8 +147,9 @@ constexpr int kSlabBytes = kBlockM * 128;      // 16 KiB staging tile
 template <int BN>
 struct Cfg {
   static constexpr int kBBytes = BN * 128;
-  static constexpr int kSub = (BN == 256) ? 1 : 2;
-  static constexpr int kTmemCols = 2 * BN;                          // double-buffered accumulator (power of two)
+  static constexpr int kSub = 1;                                    // 64-deep K blocks per ring stage (a fixed trip count keeps the
+                                                                    // wgmma stream asynchronous; a runtime-length loop serialises it)
+  static constexpr int kAcc = BN / 2;                               // fp32 accumulators per consumer thread (64 rows x BN)
   // fixed part of dynamic smem (everything but the A/B ring and the per-CTA statistic accumulators)
   // plus, after the barriers, ONE region that is scale/shift (FUSED, 2 KiB) or the statistic accumulators (RAW)
   static constexpr int kFixedBytes = 1024 /*align slack*/ + kSlabBytes + 256 /*barriers*/;
@@ -185,50 +159,27 @@ struct Cfg {
 //   0 patch  : TH x TW patch tiles, one tiled 4-D TMA load per (tap, channel block)
 //   1 linear : 128 consecutive output pixels, one im2col-mode TMA load per (tap, channel block)
 //   2 halo   : 16 x 8 patch tiles, ONE tiled load per channel block of the 18 x (8+2) input halo; the nine taps are nine
-//              shared-memory descriptors into that halo (row pitch 16 pixels = 2 KiB, so every 8-pixel swizzle atom of a
-//              tap view keeps the phase of its first row).  3x3 stride-1 only.  Each input pixel crosses L2 -> SM once
-//              per tile instead of nine times: the tap re-reads are what bounds the 3x3 layers otherwise.
-//
-// PAIR (cta_group::2, linear or halo tiles with a long main loop): the grid is launched as clusters of two CTAs (one TPC).  The
-// pair computes a 256-pixel x 256-channel tile with ONE tcgen05.mma.cta_group::2 stream issued by the leader (cluster rank 0):
-// every CTA stages its own 128 A rows and only its HALF of the weight slab (B rows [r * 128, +128) of the tile's 256 channels),
-// so a K block moves 32 KiB instead of 48 KiB through each SM's shared memory -- the operand bandwidth that holds the
-// single-CTA BN = 256 main loop at ~77 % of the tensor pipe -- and the ring gets six stages instead of four.  The
-// accumulator halves land in each CTA's own TMEM; epilogue, statistics and stores are those of two independent M tiles.
-//   full[s]   lives in the leader only: 4 arrivals (A and B producer of both CTAs; the peer's arrive remotely), the TMA
-//             loads of both CTAs complete their bytes there (.cta_group::2 load form)
-//   empty[s], tmem_full[a]   one per CTA, signalled together by the leader's multicast tcgen05.commit
-//   tmem_empty[a]   leader only: one elected arrival per convert warp of both CTAs (16)
-template <int BN, bool TL, int AM, bool PAIR = false>
+//              shared-memory descriptors into that halo (every 8-pixel swizzle atom of a tap view is one halo row).
+//              3x3 stride-1 only.  Each input pixel crosses L2 -> SM once per tile instead of nine times.
+template <int BN, bool TL, int AM>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmY, const Params p) {
   using C = Cfg<BN>;
   constexpr bool LIN = (AM == 1);
   constexpr bool HALO = (AM == 2);
-  static_assert(!PAIR || AM != 0, "pair mode: linear or halo tiles");
-  constexpr int kBB = PAIR ? C::kBBytes / 2 : C::kBBytes;   // weight bytes per 64-deep K block in THIS CTA's shared memory
-  const uint32_t crank = PAIR ? cluster_ctarank() : 0u;
-  // tile walk: (first, step, end) of this CTA's loop over tiles (pair mode: over pair tiles, shared by the two CTAs)
-  // (expressions, not variables: blockIdx / gridDim / kernel parameters cost no registers)
-#define SY_T_FIRST (PAIR ? (int)(blockIdx.x >> 1) : (int)blockIdx.x)
-#define SY_T_STEP (PAIR ? (int)(gridDim.x >> 1) : (int)gridDim.x)
-#define SY_T_END (PAIR ? p.total_tiles2 : p.total_tiles)
+  constexpr int kBB = C::kBBytes;
+  // tile walk of this CTA (expressions, not variables: blockIdx / gridDim / kernel parameters cost no registers)
+#define SY_T_FIRST ((int)blockIdx.x)
+#define SY_T_STEP ((int)gridDim.x)
+#define SY_T_END (p.total_tiles)
   auto tile_nm = [&](int tile, int& n_tile, int& m_tile) {
-    if constexpr (PAIR) {
-      n_tile = fdiv(tile, p.fd_m_tiles2);
-      m_tile = 2 * (tile - n_tile * p.m_tiles2) + (int)crank;
-    } else {
-      n_tile = fdiv(tile, p.fd_m_tiles);
-      m_tile = tile - n_tile * p.m_tiles;
-    }
+    n_tile = fdiv(tile, p.fd_m_tiles);
+    m_tile = tile - n_tile * p.m_tiles;
   };
   const int S = p.stages;                                  // patch/linear: A+B ring depth; halo: B ring depth
   // 64-deep K sub-blocks per ring stage; halo mode: filter taps per weight-ring stage (one barrier round per filter row)
-  // (pair mode: a stage is 32 KiB per sub-block, so two fit three deep -- and a producer warp needs ~300 cycles for the
-  // barrier round plus ~250 per load: one round per K = 128 keeps it below the MMA time of two K blocks)
-  constexpr int kSub = HALO ? (BN == 256 ? 1 : 3) : (PAIR ? 2 : C::kSub);
-  static_assert(!PAIR || C::kSub <= 2, "pair mode: the host sizes the ring for two sub-blocks per stage");
+  constexpr int kSub = HALO ? 3 : C::kSub;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms; plain pointer arithmetic keeps the shared address space
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -236,9 +187,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* sB = sA + (HALO ? p.stagesA * p.halo_bytes : S * kSub * kABytes);
   uint8_t* sStage = sB + S * kSub * kBB;                                 // 1024-aligned: the rings are multiples of 1 KiB
   uint64_t* bars = reinterpret_cast<uint64_t*>(sStage + p.stage_tiles * kSlabBytes);
-  const int sflip = p.stage_tiles - 1;                                          // slab parity toggles the tile iff there are two
-  // bars: [0,8) full, [8,16) empty, [16,18) tmem_full, [18,20) tmem_empty, then the tmem base slot
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
+  const int sflip = p.stage_tiles - 1;                                   // slab parity toggles the tile iff there are two
+  // bars: [0,8) full, [8,16) empty, [16,19) halo full, [19,22) halo empty
   float* sAcc = reinterpret_cast<float*>(bars + 32);                     // RAW:   [2 groups][2][Cout]
   float* sScale = sAcc;                                                  // FUSED: [256] scale, [256] shift
   float* sShift = sScale + 256;
@@ -251,54 +201,253 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const uint32_t bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (kMaxStages + s); };
-  auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * kMaxStages + a); };
-  auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * kMaxStages + 2 + a); };
-  auto fullA_bar = [&](int s) { return bar0 + 8u * (2 * kMaxStages + 6 + s); };      // halo ring (<= 3 stages)
-  auto emptyA_bar = [&](int s) { return bar0 + 8u * (2 * kMaxStages + 9 + s); };
+  auto fullA_bar = [&](int s) { return bar0 + 8u * (2 * kMaxStages + s); };          // halo ring (<= 3 stages)
+  auto emptyA_bar = [&](int s) { return bar0 + 8u * (2 * kMaxStages + 3 + s); };
 
-  if (threadIdx.x == 19 * 32) {
+  if (threadIdx.x == 17 * 32) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     prefetch_tmap(&tmY);
     for (int s = 0; s < S; ++s) {
-      mbar_init(full_bar(s), (HALO ? 1 : 2) * (PAIR ? 2 : 1));     // A producer + B producer (halo: B only; pair: of both CTAs)
-      mbar_init(empty_bar(s), 1);
+      mbar_init(full_bar(s), HALO ? 1 : 2);     // A producer + B producer (halo: B only)
+      mbar_init(empty_bar(s), 2);               // one arrival per consumer warpgroup
     }
     if (HALO) {
       for (int s = 0; s < p.stagesA; ++s) {
-        mbar_init(fullA_bar(s), PAIR ? 2 : 1);
-        mbar_init(emptyA_bar(s), 1);
+        mbar_init(fullA_bar(s), 1);
+        mbar_init(emptyA_bar(s), 2);
       }
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      // arrivals per accumulator hand-back: both convert warpgroups, except in team mode at BN = 64 (one slab per tile:
-      // only the warpgroup that owns the tile's slab ever reads the accumulator)
-      mbar_init(tempty_bar(a), PAIR ? 16 : ((p.team && BN == kSlabCols) ? kEpiThreads / 2 : kEpiThreads));
     }
     fence_barrier_init();
   }
-  if (warp == 17) {
-    if constexpr (PAIR) tmem_alloc_2cta(smem_u32(tmem_slot), C::kTmemCols);
-    else tmem_alloc(smem_u32(tmem_slot), C::kTmemCols);
-  }
-  tcgen05_fence_before();
-  if constexpr (PAIR) cluster_sync();     // both CTAs' barriers and TMEM exist before anybody signals / writes them
-  else __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // everything above touched only smem / TMEM / kernel parameters; from here on we read what the previous kernels wrote
+  __syncthreads();
+  // everything above touched only smem / kernel parameters; from here on we read what the previous kernels wrote
   pdl_wait();
   if (threadIdx.x == 16 * 32) tl_rec<TL>(p, tl_k, 4, 1, 0, 0);
 
   const uint32_t a_bytes = LIN ? (uint32_t)kABytes : (uint32_t)(p.th * p.tw) * 128u;
   const int per_img = p.tiles_x * p.tiles_y;
   const int hw = p.Ho * p.Wo;
-  int tl_epi = p.timeline_cap;           // debug-timeline cursor of thread 0, carried from the convert loop into the tail
+  int tl_epi = p.timeline_cap;           // debug-timeline cursor of thread 0, carried from the consumer loop into the tail
 
+  // ---------------------------------------------- per-CTA partial row, grid barrier, BatchNorm finalize, apply
+  // run by the 16 convert + statistics warps (512 threads); called from both of their branches so that each copy is
+  // compiled under that warpgroup's register budget
+  auto kernel_tail = [&]() {
+    const int et = threadIdx.x;                        // 0..511
+    const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
+    if (et == 0) tl_rec<TL>(p, tl_epi, 4, 2, 0, 0);
+    bar_stats_done();                                // every sAcc update is done; convert warps have seen the stores drain
+    if (do_stats) {
+      // partial row of this CTA, channel-major: the four sums of a channel are one 16-byte word (the finalize below loads
+      // one word per row and channel; with the shared-memory layout [4][Cout] in global memory it needed four loads, and the
+      // 640 sector requests per warp made the partial-row sums the longest part of the tail)
+      float4* mine = reinterpret_cast<float4*>(p.partials) + (size_t)blockIdx.x * p.Cout;
+      for (int c = et; c < p.Cout; c += kTailThreads)
+        mine[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
+      if (p.n_seg > 0) {
+        auto grid_barrier = [&](unsigned int* ctr) {    // all CTAs of the persistent grid are resident (1 per SM)
+          __threadfence();
+          bar_stats_done();
+          if (et == 0) {
+            atomicAdd(ctr, 1u);
+            while (ld_acquire_u32(ctr) < gridDim.x) __nanosleep(32);
+          }
+          bar_stats_done();
+        };
+        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 5, 0, 0);
+        // This CTA finalizes channels [b*cpc, (b+1)*cpc), one warp per channel.  The BatchNorm parameters and running
+        // statistics of the warp's first channel do not depend on the other CTAs: load them BEFORE the grid barrier (they
+        // come from DRAM -- behind the barrier their latency, twice in a row, was most of the finalize)
+        const int groups = p.split_n < p.N ? 2 : 1;
+        const int cpc = (p.Cout + (int)gridDim.x - 1) / (int)gridDim.x;
+        const int c_end = min(p.Cout, ((int)blockIdx.x + 1) * cpc);
+        const int c_first = (int)blockIdx.x * cpc + warp;
+        float pre_gamma = 1.f, pre_beta = 0.f, pre_rm = 0.f, pre_rv = 1.f;
+        if (c_first < c_end && lane < 2) {
+          const BnSeg& sg = (p.n_seg > 1 && c_first >= p.seg[1].c_begin) ? p.seg[1] : p.seg[0];
+          const int cs = c_first - sg.c_begin;
+          pre_gamma = sg.gamma[cs];
+          pre_beta = sg.beta[cs];
+          if (lane == 0) {
+            if (sg.rmean) pre_rm = sg.rmean[cs];
+            if (sg.rvar) pre_rv = sg.rvar[cs];
+          }
+        }
+        grid_barrier(&p.sync[0]);
+        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 6, 0, 0);
+        // exit ticket (the last CTA past the barriers re-arms the counters): taken as early as possible -- right after the
+        // last grid barrier -- so that the atomic's round trip overlaps the finalize instead of ending the kernel
+        unsigned int ticket = 0xffffffffu;
+        if (et == 0 && p.ap_y == nullptr) ticket = atomicAdd(&p.sync[2], 1u);
+        // one WARP per channel (no block barriers): lane l sums the partial rows l, l+32, ... in order, a fixed shuffle tree
+        // combines the lanes (deterministic), lanes 0 / 1 finalize one statistics group each.
+        for (int c = c_first; c < c_end; c += kTailThreads / 32) {
+          // all loads first (<= 160 rows: five per lane), then the sums in the same fixed order: one L2 round trip instead
+          // of five serialised ones (the fp64 adds used to sit between the loads of consecutive rows)
+          const float4* rows4 = reinterpret_cast<const float4*>(p.partials) + c;
+          float4 buf[5];
+#pragma unroll
+          for (int j = 0; j < 5; ++j) {
+            const int r = lane + 32 * j;
+            buf[j] = r < (int)gridDim.x ? __ldcg(rows4 + (size_t)r * p.Cout) : make_float4(0.f, 0.f, 0.f, 0.f);
+          }
+          double v[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+          for (int j = 0; j < 5; ++j) {
+            v[0] += (double)buf[j].x; v[1] += (double)buf[j].y; v[2] += (double)buf[j].z; v[3] += (double)buf[j].w;
+          }
+          if (et == 0) tl_rec<TL>(p, tl_epi, 4, 8, 0, 0);
+          for (int r = lane + 160; r < (int)gridDim.x; r += 32) {          // (more than 160 CTAs: not on an H100)
+            const float4 q = __ldcg(rows4 + (size_t)r * p.Cout);
+            v[0] += (double)q.x; v[1] += (double)q.y; v[2] += (double)q.z; v[3] += (double)q.w;
+          }
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+#pragma unroll
+            for (int m = 16; m >= 1; m >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], m);
+          }
+          if (et == 0) tl_rec<TL>(p, tl_epi, 4, 9, 0, 0);
+          // every lane holds the four sums: lane g finalizes statistics group g (fp64 only for mean / E[x^2] - mean^2; the
+          // reciprocal square root is IEEE fp32 -- the fp64 sqrt / divisions of the first version cost ~3 us per launch),
+          // lane 0 then folds both groups into the running statistics in order
+          const BnSeg& sg = (p.n_seg > 1 && c >= p.seg[1].c_begin) ? p.seg[1] : p.seg[0];
+          const int cs = c - sg.c_begin;
+          float mean_f = 0.f, var_f = 0.f;
+          if (lane < groups) {
+            const int g = lane;
+            const double s1 = g ? v[2] : v[0], s2 = g ? v[3] : v[1];
+            const double mean = s1 * p.inv_cnt[g];
+            double var = s2 * p.inv_cnt[g] - mean * mean;
+            if (var < 0.0) var = 0.0;
+            mean_f = (float)mean;
+            var_f = (float)var;
+            const float istd = 1.0f / sqrtf(var_f + p.eps);
+            const float sc = (c == c_first ? pre_gamma : sg.gamma[cs]) * istd;
+            p.ss[(0 * 2 + g) * p.Cout + c] = sc;
+            p.ss[(1 * 2 + g) * p.Cout + c] = (c == c_first ? pre_beta : sg.beta[cs]) - mean_f * sc;
+            if (p.mi != nullptr) {
+              p.mi[(0 * 2 + g) * p.Cout + c] = mean_f;
+              p.mi[(1 * 2 + g) * p.Cout + c] = istd;
+            }
+          }
+          const float mean1 = __shfl_sync(0xffffffffu, mean_f, 1), var1 = __shfl_sync(0xffffffffu, var_f, 1);
+          if (lane == 0) {
+            float rm = pre_rm, rv = pre_rv;
+            if (c != c_first) {
+              rm = sg.rmean ? sg.rmean[cs] : 0.f;
+              rv = sg.rvar ? sg.rvar[cs] : 1.f;
+            }
+            rm = (1.f - p.momentum) * rm + p.momentum * mean_f;
+            rv = (1.f - p.momentum) * rv + p.momentum * (var_f * p.unbias[0]);
+            if (groups == 2) {
+              rm = (1.f - p.momentum) * rm + p.momentum * mean1;
+              rv = (1.f - p.momentum) * rv + p.momentum * (var1 * p.unbias[1]);
+            }
+            if (sg.rmean) sg.rmean[cs] = rm;
+            if (sg.rvar) sg.rvar[cs] = rv;
+          }
+        }
+        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 7, 0, 0);
+        if (et == 0 && blockIdx.x == 0) {
+          for (int sgi = 0; sgi < p.n_seg; ++sgi)          // (a reduction: no round trip -- a load-add-store ended CTA 0 ~1 us late)
+            if (p.seg[sgi].nbt) atomicAdd(reinterpret_cast<unsigned long long*>(p.seg[sgi].nbt), (unsigned long long)groups);
+        }
+        if (p.ap_y != nullptr) {
+          // ---- second grid barrier: scale/shift of every channel are published; normalise this CTA's own tiles,
+          //      re-reading the raw bf16 values it just stored (L2 resident for all but the largest layers)
+          grid_barrier(&p.sync[1]);
+          for (int i = et; i < p.Cout; i += kTailThreads)          // [2 (scale|shift)][2 groups][Cout] -> smem (over sAcc)
+            reinterpret_cast<float4*>(sAcc)[i] = __ldcg(reinterpret_cast<const float4*>(p.ss) + i);
+          bar_stats_done();
+          constexpr int CPR = BN / 8;                              // 16-byte chunks per pixel row of a tile
+          constexpr int RPP = kTailThreads / CPR;                  // tile rows handled per pass of the 512 threads
+          const int chunk = et % CPR, r0 = et / CPR;
+          for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
+            int n_tile, m_tile;
+        tile_nm(tile, n_tile, m_tile);
+            const int cg = n_tile * BN + chunk * 8;
+            if (cg >= p.Cout) continue;
+            int img = 0, py = 0, px = 0;
+            if constexpr (!LIN) {
+              img = fdiv(m_tile, p.fd_per_img);
+              const int rem = m_tile - img * per_img;
+              py = fdiv(rem, p.fd_tiles_x); px = rem - py * p.tiles_x;
+            }
+            // batches of kAB rows: all loads first (the stores may alias the loads, so the compiler cannot hoist them)
+            constexpr int kAB = 4;
+            const int rows_in_patch = LIN ? kBlockM : p.th * p.tw;
+            for (int rb = r0; rb < rows_in_patch; rb += RPP * kAB) {
+              long long pixv[kAB];
+              uint4 u[kAB], rv[kAB];
+#pragma unroll
+              for (int j = 0; j < kAB; ++j) {
+                const int rr = rb + j * RPP;
+                if constexpr (LIN) {
+                  const long long pp = (long long)m_tile * kBlockM + rr;
+                  pixv[j] = (rr < kBlockM && pp < p.P_total) ? pp : -1;
+                } else {
+                  const int tyy = fdiv(rr, p.fd_tw), txx = rr - tyy * p.tw;
+                  const int oy = py * p.th + tyy, ox = px * p.tw + txx;
+                  pixv[j] = (rr < rows_in_patch && img < p.N && oy < p.Ho && ox < p.Wo) ? ((long long)img * p.Ho + oy) * p.Wo + ox : -1;
+                }
+              }
+#pragma unroll
+              for (int j = 0; j < kAB; ++j)
+                if (pixv[j] >= 0) u[j] = __ldcg(reinterpret_cast<const uint4*>(p.y + pixv[j] * p.y_pitch + cg));
+              if (p.ap_res != nullptr) {
+#pragma unroll
+                for (int j = 0; j < kAB; ++j)
+                  if (pixv[j] >= 0)
+                    rv[j] = *reinterpret_cast<const uint4*>(p.ap_res + pixv[j] * p.ap_res_pitch + cg +
+                                                            (pixv[j] >= p.gp ? p.ap_res_goff1 : 0));
+              }
+#pragma unroll
+              for (int j = 0; j < kAB; ++j) {
+                if (pixv[j] < 0) continue;
+                const int grp = pixv[j] >= p.gp ? 1 : 0;
+                const float* sc = sAcc + grp * p.Cout + cg;
+                const float* sh = sAcc + (2 + grp) * p.Cout + cg;
+                const float4 s0 = *reinterpret_cast<const float4*>(sc), s1 = *reinterpret_cast<const float4*>(sc + 4);
+                const float4 h0 = *reinterpret_cast<const float4*>(sh), h1 = *reinterpret_cast<const float4*>(sh + 4);
+                const float scv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+                const float shv[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
+                float f[8] = {bf16_lo(u[j].x), bf16_hi(u[j].x), bf16_lo(u[j].y), bf16_hi(u[j].y),
+                              bf16_lo(u[j].z), bf16_hi(u[j].z), bf16_lo(u[j].w), bf16_hi(u[j].w)};
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                  const float t = f[i] * scv[i] + shv[i];
+                  f[i] = p.ap_act ? silu_f(t) : t;
+                }
+                if (p.ap_res != nullptr) {
+                  f[0] += bf16_lo(rv[j].x); f[1] += bf16_hi(rv[j].x); f[2] += bf16_lo(rv[j].y); f[3] += bf16_hi(rv[j].y);
+                  f[4] += bf16_lo(rv[j].z); f[5] += bf16_hi(rv[j].z); f[6] += bf16_lo(rv[j].w); f[7] += bf16_hi(rv[j].w);
+                }
+                *reinterpret_cast<uint4*>(p.ap_y + pixv[j] * p.ap_y_pitch + cg + (grp ? p.ap_y_goff1 : 0)) =
+                    make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
+              }
+            }
+          }
+        }
+        if (et == 0) {
+          if (p.ap_y != nullptr) ticket = atomicAdd(&p.sync[2], 1u);
+          if (ticket == gridDim.x - 1) {            // every CTA is past both barriers: re-arm for the next launch
+            p.sync[0] = 0u;
+            p.sync[1] = 0u;
+            p.sync[2] = 0u;
+            __threadfence();
+          }
+        }
+      }
+    }
+  };
+  if (warp >= 16) {
+  // every role's branch starts with its warpgroup's setmaxnreg: the register budget of a code region is what ptxas can
+  // prove for every path into it
+  reg_dealloc<kRegsIo>();
   if (HALO && (warp == 18 || warp == 17)) {
     // ----------------------------------------------- halo mode producers
-    if (warp == 18) {                            // A: one halo box [18 rows][pitch px][64 ch] per (tile, channel block)
+    if (warp == 18) {                            // A: one halo box [TH + 2 rows][pitch px][64 ch] per (tile, channel block)
       int sa = 0;
       uint32_t pha = 0;
       for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
@@ -309,15 +458,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int cb = 0; cb < p.cblocks; ++cb) {
           mbar_wait(emptyA_bar(sa), pha ^ 1u);
           if (elect_one()) {
-            if constexpr (PAIR) {                // the leader's barrier collects the bytes of both CTAs' halos
-              const uint32_t fbar = mapa(fullA_bar(sa), 0u);
-              if (crank != 0u) mbar_arrive_cluster(fbar);
-              else mbar_expect_tx(fullA_bar(sa), 2u * (uint32_t)p.halo_tx);
-              tma_load_4d_2cta(smem_u32(sA + sa * p.halo_bytes), &tmA, fbar, cb * kBlockK, px * p.tw - 1, py * p.th - 1, img);
-            } else {
-              mbar_expect_tx(fullA_bar(sa), (uint32_t)p.halo_tx);
-              tma_load_4d(smem_u32(sA + sa * p.halo_bytes), &tmA, fullA_bar(sa), cb * kBlockK, px * p.tw - 1, py * p.th - 1, img);
-            }
+            mbar_expect_tx(fullA_bar(sa), (uint32_t)p.halo_tx);
+            tma_load_4d(smem_u32(sA + sa * p.halo_bytes), &tmA, fullA_bar(sa), cb * kBlockK, px * p.tw - 1, py * p.th - 1, img);
           }
           __syncwarp();
           if (++sa == p.stagesA) { sa = 0; pha ^= 1u; }
@@ -332,20 +474,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int cb = 0; cb < p.cblocks; ++cb) {
           for (int t0 = 0; t0 < 9; t0 += kSub) {
             mbar_wait(empty_bar(sb), phb ^ 1u);
-            const uint32_t fbar = PAIR ? mapa(full_bar(sb), 0u) : full_bar(sb);
             if (elect_one()) {
-              if (PAIR && crank != 0u) mbar_arrive_cluster(fbar);
-              else mbar_expect_tx(full_bar(sb), (uint32_t)(kSub * kBB) * (PAIR ? 2u : 1u));
-            }
+              mbar_expect_tx(full_bar(sb), (uint32_t)(kSub * kBB));
 #pragma unroll
-            for (int j = 0; j < kSub; ++j) {
-              if (elect_one()) {
-                if constexpr (PAIR)              // this CTA's half of the tile's weight rows
-                  tma_load_3d_2cta(smem_u32(sB + (sb * kSub + j) * kBB), &tmB, fbar, cb * kBlockK, t0 + j,
-                                   n_tile * BN + (int)crank * (BN / 2));
-                else
-                  tma_load_3d(smem_u32(sB + (sb * kSub + j) * kBB), &tmB, full_bar(sb), cb * kBlockK, t0 + j, n_tile * BN);
-              }
+              for (int j = 0; j < kSub; ++j)
+                tma_load_3d(smem_u32(sB + (sb * kSub + j) * kBB), &tmB, full_bar(sb), cb * kBlockK, t0 + j, n_tile * BN);
             }
             __syncwarp();
             if (++sb == S) { sb = 0; phb ^= 1u; }
@@ -353,62 +486,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (HALO && warp == 19) {
-    // ----------------------------------------------- halo mode MMA issuer: K order = (channel block, tap)
-    constexpr uint32_t idesc = PAIR ? make_idesc_m(BN, 2 * kBlockM) : make_idesc(BN);
-    int sa = 0, sb = 0, it = 0;
-    uint32_t pha = 0, phb = 0;
-    const uint32_t row_bytes = (uint32_t)p.halo_pitch * 128u;            // one halo row; also the stride between 8-pixel atoms
-    for (int tile = (PAIR && crank != 0u) ? SY_T_END : SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP, ++it) {   // pair: the leader issues
-      const int acc = it & 1;
-      const uint32_t acc_phase = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-      tcgen05_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-      for (int cb = 0; cb < p.cblocks; ++cb) {
-        mbar_wait(fullA_bar(sa), pha);
-        const uint32_t halo = smem_u32(sA + sa * p.halo_bytes);
-        for (int t0 = 0; t0 < 9; t0 += kSub) {
-          mbar_wait(full_bar(sb), phb);
-          tcgen05_fence_after();
-          if (elect_one()) {
-#pragma unroll
-            for (int j = 0; j < kSub; ++j) {
-              const int tap = t0 + j;
-              const int r = tap / 3, sx = tap - 3 * r;
-              const uint32_t a_addr = halo + (uint32_t)r * row_bytes + (uint32_t)sx * 128u;
-              const uint32_t boff = (p.debug_flags & 64) ? ((a_addr >> 7) & 7u) : 0u;
-              const uint64_t da = make_smem_desc_ex(a_addr, row_bytes, boff);
-              const uint64_t db = make_smem_desc(smem_u32(sB + (sb * kSub + j) * kBB));
-#pragma unroll
-              for (int k = 0; k < kBlockK / 16; ++k) {
-                if constexpr (PAIR) umma_bf16_2cta(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (cb | tap | k) != 0);
-                else umma_bf16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (cb | tap | k) != 0);
-              }
-            }
-            if constexpr (PAIR) {                             // (the same barrier offsets in both CTAs)
-              umma_commit_2cta(empty_bar(sb));
-              if (t0 + kSub >= 9) {
-                umma_commit_2cta(emptyA_bar(sa));
-                if (cb == p.cblocks - 1) umma_commit_2cta(tfull_bar(acc));
-              }
-            } else {
-              umma_commit(empty_bar(sb));                     // the weight slabs are free when these MMAs retire
-              if (t0 + kSub >= 9) {
-                umma_commit(emptyA_bar(sa));                  // ... and so is the halo after its ninth tap
-                if (cb == p.cblocks - 1) umma_commit(tfull_bar(acc));
-              }
-            }
-          }
-          __syncwarp();
-          if (++sb == S) { sb = 0; phb ^= 1u; }
-        }
-        if (++sa == p.stagesA) { sa = 0; pha ^= 1u; }
-      }
-    }
   } else if (warp == 18 || warp == 17) {
     // ----------------------------------------------- TMA producers: warp 18 loads A (activations), warp 17 loads B (weights)
-    // Two issuing threads because a single thread needs ~350 cycles per cp.async.bulk.tensor: the pair keeps a
+    // Two issuing threads because a single thread needs a few hundred cycles per cp.async.bulk.tensor: the pair keeps a
     // K block's issue time below its MMA time.  Both arrive (with their byte counts) on the same full barrier.
     {
       const bool is_a = (warp == 18);
@@ -436,32 +516,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int sb0 = 0; sb0 < p.kblocks; sb0 += kSub) {
           const int nsub = min(kSub, p.kblocks - sb0);
           mbar_wait(empty_bar(stage), phase ^ 1u);          // whole warp waits: control flow stays uniform
-          // pair mode: the full barrier is the LEADER's (cluster address); the leader's producers expect the bytes of both CTAs
-          const uint32_t fbar = PAIR ? mapa(full_bar(stage), 0u) : full_bar(stage);
           if (elect_one()) {
             tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 0, tile, sb0);
-            if constexpr (PAIR) {
-              if (crank != 0u || (p.debug_flags & 2)) mbar_arrive_cluster(fbar);
-              else mbar_expect_tx(full_bar(stage), 2u * (uint32_t)nsub * (is_a ? a_bytes : (uint32_t)kBB));
-            } else if (p.debug_flags & 2) {
-              mbar_arrive(full_bar(stage));
-            } else if (is_a) {
-              mbar_expect_tx(full_bar(stage), a_bytes * (uint32_t)nsub);
-            } else {
-              mbar_expect_tx(full_bar(stage), (uint32_t)(C::kBBytes * nsub));
-            }
+            if (p.debug_flags & 2) mbar_arrive(full_bar(stage));
+            else mbar_expect_tx(full_bar(stage), is_a ? a_bytes * (uint32_t)nsub : (uint32_t)(kBB * nsub));
             tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 1, tile, sb0);
           }
           for (int j = 0; j < nsub; ++j) {
             if (!(p.debug_flags & 2) && elect_one()) {
-              if constexpr (PAIR) {
-                if (is_a)
-                  tma_load_im2col_4d_2cta(smem_u32(sA + (stage * kSub + j) * kABytes), &tmA, fbar, cb * kBlockK, x0, y0, img, (uint16_t)sx,
-                                          (uint16_t)r);
-                else                        // this CTA's half of the tile's 256 weight rows
-                  tma_load_3d_2cta(smem_u32(sB + (stage * kSub + j) * kBB), &tmB, fbar, cb * kBlockK, r * p.kw + sx,
-                                   n_tile * BN + (int)crank * (BN / 2));
-              } else if (is_a) {
+              if (is_a) {
                 if constexpr (LIN)
                   tma_load_im2col_4d(smem_u32(sA + (stage * kSub + j) * kABytes), &tmA, full_bar(stage), cb * kBlockK, x0,
                                      y0, img, (uint16_t)sx, (uint16_t)r);
@@ -469,7 +532,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
                   tma_load_4d(smem_u32(sA + (stage * kSub + j) * kABytes), &tmA, full_bar(stage), cb * kBlockK, x0 + sx,
                               y0 + r, img);
               } else
-                tma_load_3d(smem_u32(sB + (stage * kSub + j) * C::kBBytes), &tmB, full_bar(stage), cb * kBlockK,
+                tma_load_3d(smem_u32(sB + (stage * kSub + j) * kBB), &tmB, full_bar(stage), cb * kBlockK,
                             r * p.kw + sx, n_tile * BN);
             }
             if (++cb == p.cblocks) { cb = 0; if (++sx == p.kw) { sx = 0; ++r; } }
@@ -480,53 +543,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 19) {
-    // -------------------------------------------------------------- MMA issuer
-    // The whole warp walks the pipeline (uniform control flow, operands in uniform registers); one elected
-    // lane issues the tcgen05 instructions.
-    constexpr uint32_t idesc = PAIR ? make_idesc_m(BN, 2 * kBlockM) : make_idesc(BN);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    int tl_n = p.timeline_cap / 4;
-    for (int tile = (PAIR && crank != 0u) ? SY_T_END : SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP, ++it) {   // pair: the leader issues
-      const int acc = it & 1;
-      const uint32_t acc_phase = (uint32_t)(it >> 1) & 1u;
-      mbar_wait(tempty_bar(acc), acc_phase ^ 1u);
-      tcgen05_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-      for (int sb0 = 0; sb0 < p.kblocks; sb0 += kSub) {
-        const int nsub = min(kSub, p.kblocks - sb0);
-        mbar_wait(full_bar(stage), phase);
-        tcgen05_fence_after();
-        if (elect_one()) {
-          tl_rec<TL>(p, tl_n, 1, 1, tile, sb0);
-          if (!(p.debug_flags & 1)) {
-            for (int j = 0; j < nsub; ++j) {
-              const uint64_t da = make_smem_desc(smem_u32(sA + (stage * kSub + j) * kABytes));
-              const uint64_t db = make_smem_desc(smem_u32(sB + (stage * kSub + j) * kBB));
-#pragma unroll
-              for (int k = 0; k < kBlockK / 16; ++k) {
-                // advance 16 bf16 = 32 bytes along K inside the swizzle row: +2 in the (addr >> 4) field
-                if constexpr (PAIR) umma_bf16_2cta(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (sb0 | j | k) != 0);
-                else umma_bf16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (sb0 | j | k) != 0);
-              }
-            }
-          }
-          tl_rec<TL>(p, tl_n, 1, 2, tile, sb0);
-          if constexpr (PAIR) {                     // the same barrier offsets in BOTH CTAs
-            umma_commit_2cta(empty_bar(stage));
-            if (sb0 + kSub >= p.kblocks) umma_commit_2cta(tfull_bar(acc));
-          } else {
-            umma_commit(empty_bar(stage));          // frees the smem slot when these MMAs retire
-            if (sb0 + kSub >= p.kblocks) umma_commit(tfull_bar(acc));
-          }
-          tl_rec<TL>(p, tl_n, 1, 3, tile, sb0);
-        }
-        __syncwarp();
-        if (++stage == S) { stage = 0; phase ^= 1u; }
-      }
-    }
   } else if (warp == 16) {
     // ------------------------------------------------------------- store warp
     // One 4-D TMA store per 64-column slab; the tensor map clips the patch to the image and to the
@@ -534,7 +550,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const uint32_t stage_base = smem_u32(sStage);
     int sbuf = 0, prev = -1;
     int tl_s = 7 * (p.timeline_cap / 8);
-    const int nbar = p.team ? 416 : 544;
+    const int nbar = 544;
     bar_free_arrive(0, nbar);                    // both tiles start out free
     if (sflip) bar_free_arrive(1, nbar);
     for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
@@ -585,10 +601,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     __syncwarp();
     asm volatile("bar.sync 4, 288;" ::: "memory");   // the epilogue warps may now re-read this CTA's own raw tiles
-  } else if (warp >= 8 && warp < 16) {
+  }
+  } else if (warp >= 8) {
+    reg_alloc<kRegsStats>();
     // ------------------------------------------------------------ statistics warps
     // Warp ew reduces columns [8*ew, 8*ew+8) of every staged 64-column slab while the convert warps already
-    // pull the next slab out of TMEM; one owner lane per (column, sum|sumsq) accumulates in fixed order.
+    // convert the next slab; one owner lane per (column, sum|sumsq) accumulates in fixed order.
     const int ew = warp - 8;
     const int st = threadIdx.x - 256;            // 0..255
     const uint32_t stage_base = smem_u32(sStage);
@@ -598,7 +616,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     int sbuf = 0;
     int tl_t = (st == 0) ? 5 * (p.timeline_cap / 8) : p.timeline_cap;
-    const int nbar = p.team ? 416 : 544;
+    const int nbar = 544;
     bar_free_arrive(0, nbar);                    // both tiles start out free
     if (sflip) bar_free_arrive(1, nbar);
     // Warp ew owns columns [8*ew, 8*ew+8) of every 64-column slab; lane l reads rows l, l+32, l+64, l+96 (one 16-byte
@@ -606,7 +624,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // -- one set per slab index of the tile -- and are only combined across the 32 lanes (recursive-halving shuffles) and
     // added to the CTA's shared-memory totals on a FLUSH: when the CTA moves to another n tile or statistics group, on a
     // tile that straddles the group boundary, and at the end.  (Per-slab shuffle reductions made the statistics warps the
-    // bottleneck of every epilogue-bound layer: ~1400 cycles per slab, profiles/r02_timeline_*.)
+    // bottleneck of every epilogue-bound layer: ~1400 cycles per slab.)
     constexpr int kSlabs = BN / kSlabCols;
     constexpr int kAccSlabs = (BN <= 128) ? kSlabs : 1;      // BN = 256: registers do not allow four sets; flush every slab
     float acc[kAccSlabs][16];
@@ -729,118 +747,52 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     if (do_stats) flush();
-  } else if (warp < 8) {
-    // ---------------------------------------------------------------- epilogue
-    const int q = warp & 3;                    // TMEM lane quarter this warp may read
-    const int half = warp >> 2;                // which 32 columns of a 64-column slab this warpgroup converts
-    const int row = q * 32 + lane;             // tile row == TMEM lane
-    const int et = threadIdx.x;                // 0..255
-    const int ty = LIN ? 0 : fdiv(row, p.fd_tw), tx = LIN ? 0 : row - ty * p.tw;
-    const bool in_patch = LIN ? true : row < p.th * p.tw;
+    kernel_tail();
+  } else {
+    reg_alloc<kRegsMma>();
+    // ---------------------------------------------------------------- MMA + convert warpgroups
+    // Warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile: it issues the wgmma stream for them (accumulators in
+    // registers), then converts its rows of every 64-column slab into the staging tile.  A ring stage is handed back to the
+    // producers one commit group late (wgmma.wait_group 1), so the next group's MMAs are queued while the last ones drain.
+    const int wg = warp >> 2;
+    const int et = threadIdx.x;                                    // 0..255
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);        // this thread's tile rows: r0 and r0 + 8
+    const int cq = 2 * (lane & 3);                                 // its first column in every 8-column group
     const uint32_t stage_base = smem_u32(sStage);
-    const uint32_t my_row = stage_base + (uint32_t)row * 128u;
-    const uint32_t rsw = (uint32_t)(row & 7);
-    const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
-    int it = 0;
-    int sbuf = 0;
+    const bool lead = (threadIdx.x & 127) == 0;                    // signals the warpgroup's ring releases
+    int ty[2], tx[2];
+    bool in_patch[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      ty[h] = LIN ? 0 : fdiv(row, p.fd_tw);
+      tx[h] = LIN ? 0 : row - ty[h] * p.tw;
+      in_patch[h] = LIN ? true : row < p.th * p.tw;
+    }
+    // halo mode: this warpgroup's 8 output rows start 8 halo rows further down
+    const uint32_t row_bytes = HALO ? (uint32_t)p.halo_pitch * 128u : 1024u;
+    const uint32_t a_off = HALO ? (uint32_t)(wg * 8) * row_bytes : (uint32_t)wg * 8192u;
+    float acc[C::kAcc];
+    int stage = 0, sa = 0, sbuf = 0;
+    uint32_t phase = 0, pha = 0;
     int tl_n = (et == 0) ? p.timeline_cap / 2 : p.timeline_cap;
-    if (p.team) {
-      // ------------------------------------------------------------ team mode (RAW only): warpgroup `half` owns the slabs
-      // of parity `half` (global slab counter of this CTA) and staging tile `half`, 64 columns = two TMEM loads per slab
-      const int team = half;
-      constexpr int kSlabs = BN / kSlabCols;
-      const uint32_t my_tile_row = my_row + (uint32_t)(team * kSlabBytes);
-      for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP, ++it) {
-        const int gs0 = it * kSlabs;                                   // global index of this tile's first slab
-        int first = ((gs0 & 1) == team) ? 0 : 1;                       // first slab of the tile this warpgroup owns
-        if (first >= kSlabs) continue;
-        int last = first;
-        while (last + 2 < kSlabs) last += 2;
-        const int acc = it & 1;
-        const uint32_t acc_phase = (uint32_t)(it >> 1) & 1u;
-        int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
-        bool valid;
-        long long pix;
+    for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
+      int n_tile, m_tile;
+      tile_nm(tile, n_tile, m_tile);
+      bool valid[2];
+      long long pix[2];                          // this thread's output pixels in the flattened (n, oh, ow) space
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
         if constexpr (LIN) {
-          pix = (long long)m_tile * kBlockM + row;
-          valid = pix < p.P_total;
+          pix[h] = (long long)m_tile * kBlockM + r0 + 8 * h;
+          valid[h] = pix[h] < p.P_total;
         } else {
           const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
           const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-          const int oy = py * p.th + ty, ox = px * p.tw + tx;
-          valid = in_patch && (oy < p.Ho) && (ox < p.Wo);
-          pix = ((long long)img * p.Ho + oy) * p.Wo + ox;
+          const int oy = py * p.th + ty[h], ox = px * p.tw + tx[h];
+          valid[h] = in_patch[h] && (oy < p.Ho) && (ox < p.Wo);
+          pix[h] = ((long long)img * p.Ho + oy) * p.Wo + ox;
         }
-        const int n0 = n_tile * BN;
-        tl_rec<TL>(p, tl_n, 2, 0, tile, 0);
-        mbar_wait(tfull_bar(acc), acc_phase);
-        tl_rec<TL>(p, tl_n, 2, 1, tile, 0);
-        tcgen05_fence_after();
-        const uint32_t taddr = tmem_base + (uint32_t)(acc * BN) + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-        for (int slab = first; slab < kSlabs; slab += 2) {
-          const int cl = slab * kSlabCols;
-          uint32_t v[32], packed[16];
-          tmem_ld32(taddr + (uint32_t)cl, v);
-          tmem_ld_wait();
-          if (p.dbg_f32 != nullptr && valid) {
-            float* o = p.dbg_f32 + pix * p.Cout + n0 + cl;
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (n0 + cl + i < p.Cout) o[i] = __uint_as_float(v[i]);
-          }
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            packed[i] = valid ? pack_bf16(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])) : 0u;
-          tmem_ld32(taddr + (uint32_t)(cl + 32), v);                  // second half of the slab: in flight during the stores
-          tl_rec<TL>(p, tl_n, 2, 2, tile, slab);
-          bar_free_wait(team, 416);                                    // staging tile free: its store has read it, statistics loaded
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-            sts128(my_tile_row + ((((uint32_t)g) ^ rsw) << 4), packed[4 * g], packed[4 * g + 1], packed[4 * g + 2], packed[4 * g + 3]);
-          tmem_ld_wait();
-          if (slab == last) {                                          // every TMEM read of this accumulator by this warpgroup is done
-            tcgen05_fence_before();
-            mbar_arrive(tempty_bar(acc));
-          }
-          if (p.dbg_f32 != nullptr && valid) {
-            float* o = p.dbg_f32 + pix * p.Cout + n0 + cl + 32;
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (n0 + cl + 32 + i < p.Cout) o[i] = __uint_as_float(v[i]);
-          }
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            packed[i] = valid ? pack_bf16(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])) : 0u;
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-            sts128(my_tile_row + ((((uint32_t)(4 + g)) ^ rsw) << 4), packed[4 * g], packed[4 * g + 1], packed[4 * g + 2], packed[4 * g + 3]);
-          fence_proxy_async();
-          bar_staged_arrive(team, 416);
-          tl_rec<TL>(p, tl_n, 2, 3, tile, slab);
-        }
-      }
-      tl_epi = tl_n;
-      bar_free_wait(team, 416);                                        // drain the last arrivals of this warpgroup's tile
-      asm volatile("bar.sync 4, 288;" ::: "memory");
-    } else {
-    for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (uint32_t)(it >> 1) & 1u;
-      int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
-      bool valid;
-      long long pix;                             // this thread's output pixel in the flattened (n, oh, ow) space
-      if constexpr (LIN) {
-        pix = (long long)m_tile * kBlockM + row;
-        valid = pix < p.P_total;
-      } else {
-        const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
-        const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-        const int oy = py * p.th + ty, ox = px * p.tw + tx;
-        valid = in_patch && (oy < p.Ho) && (ox < p.Wo);
-        pix = ((long long)img * p.Ho + oy) * p.Wo + ox;
       }
       const int n0 = n_tile * BN;
       tl_rec<TL>(p, tl_n, 2, 0, tile, 0);
@@ -853,305 +805,112 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         epi_bar();
       }
-      mbar_wait(tfull_bar(acc), acc_phase);
-      tl_rec<TL>(p, tl_n, 2, 1, tile, 0);
-      tcgen05_fence_after();
-      const uint32_t taddr = tmem_base + (uint32_t)(acc * BN) + ((uint32_t)(q * 32) << 16);
-      // software pipeline: the TMEM load of slab s+1 is in flight while slab s is staged (debug flag 32: off)
-      const bool pf = !(p.debug_flags & 32);
-      uint32_t v[32];
-      tmem_ld32(taddr + (uint32_t)(half * 32), v);
-#pragma unroll 1
-      for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
-        const int cl = slab * kSlabCols + half * 32;     // first of this thread's 32 accumulator columns
-        if (!pf && slab > 0) tmem_ld32(taddr + (uint32_t)cl, v);
-        tmem_ld_wait();
-        if (slab == BN / kSlabCols - 1) {
-          // every TMEM read of this accumulator is complete: hand it back to the MMA warp
-          tcgen05_fence_before();
-          if constexpr (PAIR) {                      // ... of the leader: one arrival per warp
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa(tempty_bar(acc), 0u));
-          } else {
-            mbar_arrive(tempty_bar(acc));
-          }
+      // ---- main loop
+      int pend_b = -1, pend_a = -1;              // ring stages read by the commit group still in flight
+      auto release = [&]() {
+        if (lead) {
+          if (pend_b >= 0) mbar_arrive(empty_bar(pend_b));
+          if (pend_a >= 0) mbar_arrive(emptyA_bar(pend_a));
         }
-        if (p.dbg_f32 != nullptr && valid) {       // validation only: the accumulators before any rounding
-          float* o = p.dbg_f32 + pix * p.Cout + n0 + cl;
-#pragma unroll                                   // (static indices: v[] must stay in registers)
-          for (int i = 0; i < 32; ++i)
-            if (n0 + cl + i < p.Cout) o[i] = __uint_as_float(v[i]);
-        }
-        uint32_t packed[16];
-        if (p.mode == SY_CONV_RAW) {
+      };
+      if constexpr (HALO) {                      // K order = (channel block, tap)
+        for (int cb = 0; cb < p.cblocks; ++cb) {
+          mbar_wait(fullA_bar(sa), pha);
+          const uint32_t halo = smem_u32(sA + sa * p.halo_bytes) + a_off;
+          for (int t0 = 0; t0 < 9; t0 += kSub) {
+            mbar_wait(full_bar(stage), phase);
+            wgmma_fence_operand(acc);
+            wgmma_fence();
 #pragma unroll
-          for (int i = 0; i < 16; ++i)
-            packed[i] = valid ? pack_bf16(__uint_as_float(v[2 * i]), __uint_as_float(v[2 * i + 1])) : 0u;
-        } else {
-          float f[32];
+            for (int j = 0; j < kSub; ++j) {
+              const int tap = t0 + j;
+              const int r = tap / 3, sx = tap - 3 * r;
+              const uint32_t a_addr = halo + (uint32_t)r * row_bytes + (uint32_t)sx * 128u;
+              const uint32_t boff = (p.debug_flags & 64) ? ((a_addr >> 7) & 7u) : 0u;
+              const uint64_t da = make_smem_desc(a_addr, row_bytes, boff);
+              const uint64_t db = make_smem_desc(smem_u32(sB + (stage * kSub + j) * kBB));
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            float t = __uint_as_float(v[i]) * sScale[cl + i] + sShift[cl + i];
-            f[i] = p.act ? silu_f(t) : t;
-          }
-          if (p.res != nullptr && valid) {
-            const __nv_bfloat16* rp = p.res + pix * p.res_pitch + n0 + cl;
-#pragma unroll
-            for (int g = 0; g < 4; ++g) {
-              if (n0 + cl + g * 8 < p.Cout) {
-                const uint4 rv = *reinterpret_cast<const uint4*>(rp + g * 8);
-                f[g * 8 + 0] += bf16_lo(rv.x); f[g * 8 + 1] += bf16_hi(rv.x);
-                f[g * 8 + 2] += bf16_lo(rv.y); f[g * 8 + 3] += bf16_hi(rv.y);
-                f[g * 8 + 4] += bf16_lo(rv.z); f[g * 8 + 5] += bf16_hi(rv.z);
-                f[g * 8 + 6] += bf16_lo(rv.w); f[g * 8 + 7] += bf16_hi(rv.w);
-              }
+              for (int k = 0; k < kBlockK / 16; ++k)   // 16 bf16 = 32 bytes along K inside the swizzle row: +2 in (addr >> 4)
+                Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (cb | tap | k) != 0);
             }
+            wgmma_commit();
+            wgmma_fence_operand(acc);
+            wgmma_wait<1>();
+            release();
+            pend_b = stage;
+            pend_a = (t0 + kSub >= 9) ? sa : -1;     // the halo is free after its ninth tap
+            if (++stage == S) { stage = 0; phase ^= 1u; }
           }
-#pragma unroll
-          for (int i = 0; i < 16; ++i) packed[i] = valid ? pack_bf16(f[2 * i], f[2 * i + 1]) : 0u;
+          if (++sa == p.stagesA) { sa = 0; pha ^= 1u; }
         }
-        if (pf && slab + 1 < BN / kSlabCols) tmem_ld32(taddr + (uint32_t)(cl + kSlabCols), v);   // v is dead: prefetch the next slab
+      } else {
+        static_assert(kSub == 1, "one K block per stage");
+        for (int kb = 0; kb < p.kblocks; ++kb) {
+          mbar_wait(full_bar(stage), phase);
+          wgmma_fence_operand(acc);
+          wgmma_fence();
+          const uint64_t da = make_smem_desc(smem_u32(sA + stage * kABytes) + a_off);
+          const uint64_t db = make_smem_desc(smem_u32(sB + stage * kBB));
+#pragma unroll
+          for (int k = 0; k < kBlockK / 16; ++k)
+            Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
+          wgmma_commit();
+          wgmma_fence_operand(acc);
+          wgmma_wait<1>();
+          release();
+          pend_b = stage;
+          if (++stage == S) { stage = 0; phase ^= 1u; }
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      release();
+      tl_rec<TL>(p, tl_n, 2, 1, tile, 0);
+      // ---- epilogue: per 64-column slab, registers -> (raw | folded BN + SiLU + residual) -> bf16 -> staging tile
+#pragma unroll
+      for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
         tl_rec<TL>(p, tl_n, 2, 2, tile, slab);
         bar_free_wait(sbuf);                     // (A) staging tile free: its store has read it, the statistics loads are done
-        const uint32_t my_tile_row = my_row + (uint32_t)(sbuf * kSlabBytes);
+        const uint32_t tb = stage_base + (uint32_t)(sbuf * kSlabBytes) + (uint32_t)cq * 2u;
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {            // 16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) << 4)
-          const uint32_t j = (uint32_t)(half * 4 + g);
-          sts128(my_tile_row + ((j ^ rsw) << 4), packed[4 * g], packed[4 * g + 1], packed[4 * g + 2], packed[4 * g + 3]);
+        for (int j = 0; j < 8; ++j) {
+          const int J = slab * 8 + j;
+          const int cl = slab * kSlabCols + j * 8 + cq;          // tile column of this thread's first value
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float v0 = acc[4 * J + 2 * h], v1 = acc[4 * J + 2 * h + 1];
+            const bool inb = valid[h] && n0 + cl < p.Cout;
+            if (p.dbg_f32 != nullptr && inb)     // validation only: the accumulators before any rounding
+              *reinterpret_cast<float2*>(p.dbg_f32 + pix[h] * p.Cout + n0 + cl) = make_float2(v0, v1);
+            if (p.mode != SY_CONV_RAW) {
+              v0 = v0 * sScale[cl] + sShift[cl];
+              v1 = v1 * sScale[cl + 1] + sShift[cl + 1];
+              if (p.act) { v0 = silu_f(v0); v1 = silu_f(v1); }
+              if (p.res != nullptr && inb) {
+                const uint32_t rv = *reinterpret_cast<const uint32_t*>(p.res + pix[h] * p.res_pitch + n0 + cl);
+                v0 += bf16_lo(rv);
+                v1 += bf16_hi(rv);
+              }
+            }
+            // 16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) << 4)
+            const uint32_t row = (uint32_t)(r0 + 8 * h);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + row * 128u + ((((uint32_t)j) ^ (row & 7u)) << 4)),
+                         "r"(valid[h] ? pack_bf16(v0, v1) : 0u) : "memory");
+          }
         }
         fence_proxy_async();                     // generic-proxy writes -> visible to the TMA (async proxy)
         bar_staged_arrive(sbuf);                 // (B) staging tile complete: store + statistics warps take it from here
         tl_rec<TL>(p, tl_n, 2, 3, tile, slab);
-        tl_rec<TL>(p, tl_n, 2, 4, tile, slab);
       }
     }
     tl_epi = tl_n;
     bar_free_wait(0);                                // drain the last arrivals (balanced barriers at exit)
     if (sflip) bar_free_wait(1);
     asm volatile("bar.sync 4, 288;" ::: "memory");   // store warp: all TMA stores of this CTA are complete
-    }
+    kernel_tail();
   }
-  if (warp < 16) {
-    // ---------------------------------------------- per-CTA partial row, grid barrier, BatchNorm finalize, apply
-    // run by the 16 convert + statistics warps (512 threads)
-    const int et = threadIdx.x;                        // 0..511
-    const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
-    if (et == 0) tl_rec<TL>(p, tl_epi, 4, 2, 0, 0);
-    bar_stats_done();                                // every sAcc update is done; convert warps have seen the stores drain
-    if (do_stats) {
-      // partial row of this CTA, channel-major: the four sums of a channel are one 16-byte word (the finalize below loads
-      // one word per row and channel; with the shared-memory layout [4][Cout] in global memory it needed four loads, and the
-      // 640 sector requests per warp made the partial-row sums the longest part of the tail)
-      float4* mine = reinterpret_cast<float4*>(p.partials) + (size_t)blockIdx.x * p.Cout;
-      for (int c = et; c < p.Cout; c += kTailThreads)
-        mine[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
-      if (p.n_seg > 0) {
-        auto grid_barrier = [&](unsigned int* ctr) {    // all CTAs of the persistent grid are resident (1 per SM)
-          __threadfence();
-          bar_stats_done();
-          if (et == 0) {
-            atomicAdd(ctr, 1u);
-            while (ld_acquire_u32(ctr) < gridDim.x) __nanosleep(32);
-          }
-          bar_stats_done();
-        };
-        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 5, 0, 0);
-        // This CTA finalizes channels [b*cpc, (b+1)*cpc), one warp per channel.  The BatchNorm parameters and running
-        // statistics of the warp's first channel do not depend on the other CTAs: load them BEFORE the grid barrier (they
-        // come from DRAM -- behind the barrier their latency, twice in a row, was most of the finalize)
-        const int groups = p.split_n < p.N ? 2 : 1;
-        const int cpc = (p.Cout + (int)gridDim.x - 1) / (int)gridDim.x;
-        const int c_end = min(p.Cout, ((int)blockIdx.x + 1) * cpc);
-        const int c_first = (int)blockIdx.x * cpc + warp;
-        float pre_gamma = 1.f, pre_beta = 0.f, pre_rm = 0.f, pre_rv = 1.f;
-        if (c_first < c_end && lane < 2) {
-          const BnSeg& sg = (p.n_seg > 1 && c_first >= p.seg[1].c_begin) ? p.seg[1] : p.seg[0];
-          const int cs = c_first - sg.c_begin;
-          pre_gamma = sg.gamma[cs];
-          pre_beta = sg.beta[cs];
-          if (lane == 0) {
-            if (sg.rmean) pre_rm = sg.rmean[cs];
-            if (sg.rvar) pre_rv = sg.rvar[cs];
-          }
-        }
-        grid_barrier(&p.sync[0]);
-        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 6, 0, 0);
-        // exit ticket (the last CTA past the barriers re-arms the counters): taken as early as possible -- right after the
-        // last grid barrier -- so that the atomic's round trip overlaps the finalize instead of ending the kernel
-        unsigned int ticket = 0xffffffffu;
-        if (et == 0 && p.ap_y == nullptr) ticket = atomicAdd(&p.sync[2], 1u);
-        // one WARP per channel (no block barriers): lane l sums the partial rows l, l+32, ... in order, a fixed shuffle tree
-        // combines the lanes (deterministic), lanes 0 / 1 finalize one statistics group each.
-        for (int c = c_first; c < c_end; c += kTailThreads / 32) {
-          // all loads first (<= 148 rows: five per lane), then the sums in the same fixed order: one L2 round trip instead
-          // of five serialised ones (the fp64 adds used to sit between the loads of consecutive rows)
-          const float4* rows4 = reinterpret_cast<const float4*>(p.partials) + c;
-          float4 buf[5];
-#pragma unroll
-          for (int j = 0; j < 5; ++j) {
-            const int r = lane + 32 * j;
-            buf[j] = r < (int)gridDim.x ? __ldcg(rows4 + (size_t)r * p.Cout) : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          double v[4] = {0.0, 0.0, 0.0, 0.0};
-#pragma unroll
-          for (int j = 0; j < 5; ++j) {
-            v[0] += (double)buf[j].x; v[1] += (double)buf[j].y; v[2] += (double)buf[j].z; v[3] += (double)buf[j].w;
-          }
-          if (et == 0) tl_rec<TL>(p, tl_epi, 4, 8, 0, 0);
-          for (int r = lane + 160; r < (int)gridDim.x; r += 32) {          // (more than 160 CTAs: not on a B200)
-            const float4 q = __ldcg(rows4 + (size_t)r * p.Cout);
-            v[0] += (double)q.x; v[1] += (double)q.y; v[2] += (double)q.z; v[3] += (double)q.w;
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-#pragma unroll
-            for (int m = 16; m >= 1; m >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], m);
-          }
-          if (et == 0) tl_rec<TL>(p, tl_epi, 4, 9, 0, 0);
-          // every lane holds the four sums: lane g finalizes statistics group g (fp64 only for mean / E[x^2] - mean^2; the
-          // reciprocal square root is IEEE fp32 -- the fp64 sqrt / divisions of the first version cost ~3 us per launch),
-          // lane 0 then folds both groups into the running statistics in order
-          const BnSeg& sg = (p.n_seg > 1 && c >= p.seg[1].c_begin) ? p.seg[1] : p.seg[0];
-          const int cs = c - sg.c_begin;
-          float mean_f = 0.f, var_f = 0.f;
-          if (lane < groups) {
-            const int g = lane;
-            const double s1 = g ? v[2] : v[0], s2 = g ? v[3] : v[1];
-            const double mean = s1 * p.inv_cnt[g];
-            double var = s2 * p.inv_cnt[g] - mean * mean;
-            if (var < 0.0) var = 0.0;
-            mean_f = (float)mean;
-            var_f = (float)var;
-            const float istd = 1.0f / sqrtf(var_f + p.eps);
-            const float sc = (c == c_first ? pre_gamma : sg.gamma[cs]) * istd;
-            p.ss[(0 * 2 + g) * p.Cout + c] = sc;
-            p.ss[(1 * 2 + g) * p.Cout + c] = (c == c_first ? pre_beta : sg.beta[cs]) - mean_f * sc;
-            if (p.mi != nullptr) {
-              p.mi[(0 * 2 + g) * p.Cout + c] = mean_f;
-              p.mi[(1 * 2 + g) * p.Cout + c] = istd;
-            }
-          }
-          const float mean1 = __shfl_sync(0xffffffffu, mean_f, 1), var1 = __shfl_sync(0xffffffffu, var_f, 1);
-          if (lane == 0) {
-            float rm = pre_rm, rv = pre_rv;
-            if (c != c_first) {
-              rm = sg.rmean ? sg.rmean[cs] : 0.f;
-              rv = sg.rvar ? sg.rvar[cs] : 1.f;
-            }
-            rm = (1.f - p.momentum) * rm + p.momentum * mean_f;
-            rv = (1.f - p.momentum) * rv + p.momentum * (var_f * p.unbias[0]);
-            if (groups == 2) {
-              rm = (1.f - p.momentum) * rm + p.momentum * mean1;
-              rv = (1.f - p.momentum) * rv + p.momentum * (var1 * p.unbias[1]);
-            }
-            if (sg.rmean) sg.rmean[cs] = rm;
-            if (sg.rvar) sg.rvar[cs] = rv;
-          }
-        }
-        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 7, 0, 0);
-        if (et == 0 && blockIdx.x == 0) {
-          for (int sgi = 0; sgi < p.n_seg; ++sgi)          // (a reduction: no round trip -- a load-add-store ended CTA 0 ~1 us late)
-            if (p.seg[sgi].nbt) atomicAdd(reinterpret_cast<unsigned long long*>(p.seg[sgi].nbt), (unsigned long long)groups);
-        }
-        if (p.ap_y != nullptr) {
-          // ---- second grid barrier: scale/shift of every channel are published; normalise this CTA's own tiles,
-          //      re-reading the raw bf16 values it just stored (L2 resident for all but the largest layers)
-          grid_barrier(&p.sync[1]);
-          for (int i = et; i < p.Cout; i += kTailThreads)          // [2 (scale|shift)][2 groups][Cout] -> smem (over sAcc)
-            reinterpret_cast<float4*>(sAcc)[i] = __ldcg(reinterpret_cast<const float4*>(p.ss) + i);
-          bar_stats_done();
-          constexpr int CPR = BN / 8;                              // 16-byte chunks per pixel row of a tile
-          constexpr int RPP = kTailThreads / CPR;                  // tile rows handled per pass of the 512 threads
-          const int chunk = et % CPR, r0 = et / CPR;
-          for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-            int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
-            const int cg = n_tile * BN + chunk * 8;
-            if (cg >= p.Cout) continue;
-            int img = 0, py = 0, px = 0;
-            if constexpr (!LIN) {
-              img = fdiv(m_tile, p.fd_per_img);
-              const int rem = m_tile - img * per_img;
-              py = fdiv(rem, p.fd_tiles_x); px = rem - py * p.tiles_x;
-            }
-            // batches of kAB rows: all loads first (the stores may alias the loads, so the compiler cannot hoist them)
-            constexpr int kAB = 4;
-            const int rows_in_patch = LIN ? kBlockM : p.th * p.tw;
-            for (int rb = r0; rb < rows_in_patch; rb += RPP * kAB) {
-              long long pixv[kAB];
-              uint4 u[kAB], rv[kAB];
-#pragma unroll
-              for (int j = 0; j < kAB; ++j) {
-                const int rr = rb + j * RPP;
-                if constexpr (LIN) {
-                  const long long pp = (long long)m_tile * kBlockM + rr;
-                  pixv[j] = (rr < kBlockM && pp < p.P_total) ? pp : -1;
-                } else {
-                  const int tyy = fdiv(rr, p.fd_tw), txx = rr - tyy * p.tw;
-                  const int oy = py * p.th + tyy, ox = px * p.tw + txx;
-                  // (img >= N: the second M tile of the last pair may lie past the end of the tensor)
-                  pixv[j] = (rr < rows_in_patch && img < p.N && oy < p.Ho && ox < p.Wo) ? ((long long)img * p.Ho + oy) * p.Wo + ox : -1;
-                }
-              }
-#pragma unroll
-              for (int j = 0; j < kAB; ++j)
-                if (pixv[j] >= 0) u[j] = __ldcg(reinterpret_cast<const uint4*>(p.y + pixv[j] * p.y_pitch + cg));
-              if (p.ap_res != nullptr) {
-#pragma unroll
-                for (int j = 0; j < kAB; ++j)
-                  if (pixv[j] >= 0)
-                    rv[j] = *reinterpret_cast<const uint4*>(p.ap_res + pixv[j] * p.ap_res_pitch + cg +
-                                                            (pixv[j] >= p.gp ? p.ap_res_goff1 : 0));
-              }
-#pragma unroll
-              for (int j = 0; j < kAB; ++j) {
-                if (pixv[j] < 0) continue;
-                const int grp = pixv[j] >= p.gp ? 1 : 0;
-                const float* sc = sAcc + grp * p.Cout + cg;
-                const float* sh = sAcc + (2 + grp) * p.Cout + cg;
-                const float4 s0 = *reinterpret_cast<const float4*>(sc), s1 = *reinterpret_cast<const float4*>(sc + 4);
-                const float4 h0 = *reinterpret_cast<const float4*>(sh), h1 = *reinterpret_cast<const float4*>(sh + 4);
-                const float scv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-                const float shv[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-                float f[8] = {bf16_lo(u[j].x), bf16_hi(u[j].x), bf16_lo(u[j].y), bf16_hi(u[j].y),
-                              bf16_lo(u[j].z), bf16_hi(u[j].z), bf16_lo(u[j].w), bf16_hi(u[j].w)};
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const float t = f[i] * scv[i] + shv[i];
-                  f[i] = p.ap_act ? silu_f(t) : t;
-                }
-                if (p.ap_res != nullptr) {
-                  f[0] += bf16_lo(rv[j].x); f[1] += bf16_hi(rv[j].x); f[2] += bf16_lo(rv[j].y); f[3] += bf16_hi(rv[j].y);
-                  f[4] += bf16_lo(rv[j].z); f[5] += bf16_hi(rv[j].z); f[6] += bf16_lo(rv[j].w); f[7] += bf16_hi(rv[j].w);
-                }
-                *reinterpret_cast<uint4*>(p.ap_y + pixv[j] * p.ap_y_pitch + cg + (grp ? p.ap_y_goff1 : 0)) =
-                    make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-              }
-            }
-          }
-        }
-        if (et == 0) {
-          if (p.ap_y != nullptr) ticket = atomicAdd(&p.sync[2], 1u);
-          if (ticket == gridDim.x - 1) {            // every CTA is past both barriers: re-arm for the next launch
-            p.sync[0] = 0u;
-            p.sync[1] = 0u;
-            p.sync[2] = 0u;
-            __threadfence();
-          }
-        }
-      }
-    }
-  }
-  tcgen05_fence_before();
-  if constexpr (PAIR) cluster_sync();     // the peer's MMAs read this CTA's operands and write its TMEM: leave together
-  else __syncthreads();
+  __syncthreads();
   if (threadIdx.x == 16 * 32) tl_rec<TL>(p, tl_k, 4, 3, 0, 0);
-  if (warp == 17) {
-    tcgen05_fence_after();
-    if constexpr (PAIR) tmem_dealloc_2cta(tmem_base, C::kTmemCols);
-    else tmem_dealloc(tmem_base, C::kTmemCols);
-  }
-  if (threadIdx.x == 17 * 32) { int k2 = tl_k + 8; tl_rec<TL>(p, k2, 4, 4, 0, 0); }
 }
 
 #undef SY_T_FIRST
@@ -1186,45 +945,37 @@ static void pick_patch(int ho, int wo, int* th, int* tw) {
 }
 
 
-// Tile width heuristic from measured costs (B200, 1.965 GHz): one 64-deep K block of a 128-row tile costs about
-// 665 / 515 / 560 cycles at BN = 256 / 128 / 64 (MMA issue + barrier hand-shake + operand supply; the MMA itself
-// would need 512 / 256 / 128), the epilogue about 1900 cycles per 64-column slab and overlaps the next tile's main
-// loop, and the persistent grid runs ceil(tiles / SMs) rounds -- so wide tiles win unless they add a round.
-// epilogue cost per 64-column slab used by the tile-width / staging heuristics.  The timelines say ~1000 cycles at BN <= 128
-// (register statistics, two slabs in flight) and ~1400 at BN = 256, but refitting the heuristic to those numbers moved the
-// 256->256 1x1 layers to BN = 128 and made them SLOWER in-graph (36 -> 44 us at 16x75x120, profiles/r02_layers_in_graph_*):
-// the round-1 constant stays.
+// Tile width heuristic from a per-K-block cost model: one 64-deep K block of a 128-row tile costs about kbc[] cycles
+// (MMA + barrier hand-shake + operand supply), the epilogue about epi_cycles_per_slab() per 64-column slab, and the
+// persistent grid runs ceil(tiles / SMs) rounds -- so wide tiles win unless they add a round.  The constants are a model,
+// not H100 measurements; SY_EPI_CYCLES / SY_CONV_BN let a tuning run override them.
 static double epi_cycles_per_slab(int bn) {
-  if (const char* e = getenv("SY_EPI_CYCLES")) {          // tuning aid "c64,c128,c256": the heuristics' epilogue cost per slab
-    int c64 = 0, c128 = 0, c256 = 0;
-    if (sscanf(e, "%d,%d,%d", &c64, &c128, &c256) == 3) return (double)(bn == 64 ? c64 : (bn == 128 ? c128 : c256));
+  if (const char* e = getenv("SY_EPI_CYCLES")) {          // tuning aid "c64,c128": the heuristics' epilogue cost per slab
+    int c64 = 0, c128 = 0;
+    if (sscanf(e, "%d,%d", &c64, &c128) == 2) return (double)(bn == 64 ? c64 : c128);
   }
-  // BN = 256: 1000 (measured on the whole step, profiles/r02_ab_epi_cycles.txt: 5.432 -> 5.405 ms; it makes the 1x1 layers with
-  // 448 - 704 input channels "main-loop bound": one staging tile, pair mode); BN <= 128: lower values were slower
-  return bn == 256 ? 1000.0 : 1900.0;
+  return 1900.0;
 }
+
+static double kblock_cycles(int bn) { return bn == 128 ? 515.0 : 560.0; }
 
 static int pick_bn(int cout, int m_tiles, int kblocks) {
   if (const char* e = getenv("SY_CONV_BN")) {            // tuning / test aid: force the tile width
     const int v = atoi(e);
-    if (v == 64 || v == 128 || v == 256) return v;
+    if (v == 64 || v == 128) return v;
   }
-  if (const char* e = getenv("SY_BN128_RULE")) {         // tuning aid "max_m_tiles,max_kblocks": short-K wide layers on few tiles
-    int mt = 0, kb = 0;                                  // take BN = 128 (their epilogue, not the main loop, sets the time)
-    if (sscanf(e, "%d,%d", &mt, &kb) == 2 && cout >= 256 && m_tiles <= mt && kblocks <= kb) return 128;
-  }
-  const int cands[3] = {256, 128, 64};
-  const double kbc[3] = {665.0, 515.0, 560.0};
+  const int cands[2] = {128, 64};
   int best_bn = 64;
   double best = 1e30;
-  for (int i = 0; i < 3; ++i) {
+  for (int i = 0; i < 2; ++i) {
     const int bn = cands[i];
     if (bn > 64 && bn / 2 >= cout) continue;          // a narrower tile already covers every channel
     const int tiles = m_tiles * cdiv(cout, bn);
     const int rounds = cdiv(tiles, num_sms());
-    const double main_c = kblocks * kbc[i];
+    const double main_c = kblocks * kblock_cycles(bn);
     const double epi = epi_cycles_per_slab(bn) * (bn / 64);
-    const double t = rounds * ((main_c > epi ? main_c : epi) + 400.0) + (main_c < epi ? main_c : epi);
+    // the epilogue of a tile does not overlap the main loop of the next one (the accumulators are the consumers' registers)
+    const double t = rounds * (main_c + epi + 400.0);
     if (t < best) { best = t; best_bn = bn; }
   }
   return best_bn;
@@ -1234,142 +985,60 @@ static const int kSmemLimit = 232448;   // 227 KiB opt-in maximum per CTA
 
 struct Plan {
   int smem, grid;
-  bool pair;
 };
 
-template <int BN, int AM, bool PAIR>
+template <int BN, int AM>
 static bool set_smem_attr() {
   static int state = 0;                 // 0 = not tried, 1 = ok, -1 = failed
   if (state == 0) {
     const bool ok =
-        cudaFuncSetAttribute(conv_tc_kernel<BN, false, AM, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess &&
-        cudaFuncSetAttribute(conv_tc_kernel<BN, true, AM, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess;
+        cudaFuncSetAttribute(conv_tc_kernel<BN, false, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess &&
+        cudaFuncSetAttribute(conv_tc_kernel<BN, true, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess;
     if (!ok) cudaGetLastError();
     state = ok ? 1 : -1;
   }
   return state == 1;
 }
 
-// How many 2-CTA clusters of the pair kernel can be resident at once (the BatchNorm tail's grid barrier needs all of them;
-// 74 on a B200: 148 SMs in TPC pairs).  0 = clusters cannot be launched.
-template <int BN, int AM>
-static int resident_pairs(size_t smem) {
-  if constexpr (AM == 0) {
-    return 0;
-  } else {
-    static size_t seen_smem[4] = {0, 0, 0, 0};
-    static int seen_n[4] = {0, 0, 0, 0};
-    for (int i = 0; i < 4; ++i)
-      if (seen_smem[i] == smem) return seen_n[i];
-    if (!set_smem_attr<BN, AM, true>()) return 0;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(num_sms() & ~1);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, conv_tc_kernel<BN, false, AM, true>, &cfg) != cudaSuccess) {
-      cudaGetLastError();
-      n = 0;
-    }
-    for (int i = 0; i < 4; ++i)
-      if (seen_smem[i] == 0) { seen_smem[i] = smem; seen_n[i] = n; break; }
-    return n;
-  }
-}
-
-// Ring depth, staging tiles, shared-memory size and grid of one launch; decides pair mode (cta_group::2).
-// Pair mode is for main-loop-bound layers (the epilogue of a tile hides behind the next tile's K loop), and only when pairing
-// the M tiles does not add a round of the persistent grid.  SY_CONV_PAIR=0 disables it, =1 forces it on every layer with
-// linear or halo tiles.
+// Ring depth, staging tiles, shared-memory size and grid of one launch.
 template <int BN, int AM>
 static int make_plan(Params& p, Plan* out) {
   const int acc_bytes = (p.mode == SY_CONV_RAW && p.partials) ? 16 * p.Cout : 2048;
   // epilogue-bound layers (main loop of a tile shorter than its epilogue: 1x1 convs with few input channels, the
   // stem) get a second staging tile: the store + statistics of a slab then overlap the conversion of the next
-  const double kbc = BN == 256 ? 665.0 : (BN == 128 ? 515.0 : 560.0);
-  const bool main_loop_bound = !(p.kblocks * kbc < epi_cycles_per_slab(BN) * (BN / 64));
-  bool pair = false;
-  if (AM != 0) {
-    const char* e = getenv("SY_CONV_PAIR");
-    const bool off = e != nullptr && e[0] == '0', force = e != nullptr && e[0] == '1';
-    // (the in-kernel normalise pass works on pair tiles too; SY_PAIR_APPLY=1 lets such launches pair up -- A/B switch)
-    const char* pa = getenv("SY_PAIR_APPLY");
-    const bool pair_apply = pa != nullptr && pa[0] == '1';
-    pair = !off && (force || (main_loop_bound && (p.ap_y == nullptr || pair_apply)));
+  const bool main_loop_bound = !(p.kblocks * kblock_cycles(BN) < epi_cycles_per_slab(BN) * (BN / 64));
+  p.stage_tiles = main_loop_bound ? 1 : 2;
+  if (const char* e = getenv("SY_STAGE_TILES")) p.stage_tiles = (e[0] == '2') ? 2 : 1;   // tuning aid
+  const int bbytes = Cfg<BN>::kBBytes;
+  const int fixed_bytes = Cfg<BN>::kFixedBytes + (p.stage_tiles - 1) * kSlabBytes;
+  int smem;
+  if (AM == 2) {
+    // halo ring (2-3 stages of 23 KiB) + weight-slab ring (the rest, three taps per stage)
+    const int taps = 3;                                          // filter taps per weight-ring stage (kernel: kSub)
+    p.stagesA = (BN == 64 && p.cblocks > 1) ? 3 : 2;
+    int stages = (kSmemLimit - fixed_bytes - acc_bytes - p.stagesA * p.halo_bytes) / (taps * bbytes);
+    if (stages > kMaxStages) stages = kMaxStages;
+    SY_REQUIRE(stages >= 2, SY_EINVAL, "conv2d_tc(halo): Cout=%d leaves no room for the weight ring", p.Cout);
+    p.stages = stages;
+    smem = fixed_bytes + acc_bytes + p.stagesA * p.halo_bytes + stages * taps * bbytes;
+  } else {
+    const int stage_bytes = Cfg<BN>::kSub * (kABytes + bbytes);
+    int stages = (kSmemLimit - fixed_bytes - acc_bytes) / stage_bytes;
+    if (stages > kMaxStages) stages = kMaxStages;
+    if ((p.debug_flags >> 8) & 15) stages = min(stages, (p.debug_flags >> 8) & 15);   // debug: cap the ring depth
+    SY_REQUIRE(stages >= 2, SY_EINVAL, "conv2d_tc: Cout=%d leaves no room for the operand ring", p.Cout);
+    p.stages = stages;
+    smem = fixed_bytes + acc_bytes + stages * stage_bytes;
   }
-  for (int attempt = 0; attempt < 2; ++attempt) {
-    p.stage_tiles = main_loop_bound ? 1 : 2;
-    if (const char* e = getenv("SY_STAGE_TILES")) p.stage_tiles = (e[0] == '2') ? 2 : 1;   // tuning aid
-    // epilogue-bound layers in RAW mode: the two convert warpgroups take alternate slabs (SY_CONV_TEAM=0 turns it off)
-    p.team = (p.stage_tiles == 2 && p.mode == SY_CONV_RAW) ? 1 : 0;
-    if (const char* e = getenv("SY_CONV_TEAM")) p.team = (e[0] != '0' && p.stage_tiles == 2 && p.mode == SY_CONV_RAW) ? 1 : 0;
-    if (pair) { p.stage_tiles = 1; p.team = 0; }
-    const int bbytes = Cfg<BN>::kBBytes / (pair ? 2 : 1);          // weight bytes per 64-deep K block in one CTA
-    const int fixed_bytes = Cfg<BN>::kFixedBytes + (p.stage_tiles - 1) * kSlabBytes;
-    int smem;
-    if (AM == 2) {
-      // halo ring (2-3 stages of 23 KiB) + weight-slab ring (the rest, `taps` slabs per stage)
-      const int taps = (BN == 256) ? 1 : 3;                        // filter taps per weight-ring stage (kernel: kSub)
-      p.stagesA = (BN == 64 && p.cblocks > 1) ? 3 : 2;
-      int stages = (kSmemLimit - fixed_bytes - acc_bytes - p.stagesA * p.halo_bytes) / (taps * bbytes);
-      if (stages > kMaxStages) stages = kMaxStages;
-      SY_REQUIRE(stages >= 2, SY_EINVAL, "conv2d_tc(halo): Cout=%d leaves no room for the weight ring", p.Cout);
-      p.stages = stages;
-      smem = fixed_bytes + acc_bytes + p.stagesA * p.halo_bytes + stages * taps * bbytes;
-    } else {
-      const int ksub = pair ? 2 : Cfg<BN>::kSub;                   // 64-deep sub-blocks per stage (kernel: kSub)
-      const int stage_bytes = ksub * (kABytes + bbytes);
-      int stages = (kSmemLimit - fixed_bytes - acc_bytes) / stage_bytes;
-      if (stages > kMaxStages) stages = kMaxStages;
-      if ((p.debug_flags >> 8) & 15) stages = min(stages, (p.debug_flags >> 8) & 15);   // debug: cap the ring depth
-      SY_REQUIRE(stages >= 2, SY_EINVAL, "conv2d_tc: Cout=%d leaves no room for the operand ring", p.Cout);
-      p.stages = stages;
-      smem = fixed_bytes + acc_bytes + stages * stage_bytes;
-    }
-    out->smem = smem;
-    out->pair = pair;
-    if (!pair) {
-      out->grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
-      return SY_OK;
-    }
-    // pair tiles: CTA rank r of a pair owns M tile 2 * m2 + r
-    const int m2 = cdiv(p.m_tiles, 2), total2 = m2 * p.n_tiles;
-    const int pairs = resident_pairs<BN, AM>((size_t)smem);
-    const bool forced = getenv("SY_CONV_PAIR") != nullptr;
-    if (pairs < 1 || (!forced && cdiv(total2, pairs) > cdiv(p.total_tiles, num_sms()))) {
-      pair = false;                                                // not launchable / would add a round: plan again without
-      continue;
-    }
-    p.m_tiles2 = m2;
-    p.total_tiles2 = total2;
-    p.fd_m_tiles2 = make_fastdiv((uint32_t)m2);
-    out->grid = 2 * (total2 < pairs ? total2 : pairs);
-    return SY_OK;
-  }
+  out->smem = smem;
+  out->grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
   return SY_OK;
 }
 
 template <int BN, int AM>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, Params& p, const Plan& pl, cudaStream_t stream) {
   const int smem = pl.smem, grid = pl.grid;
-  if (pl.pair) {
-    if constexpr (AM != 0) {
-      // (co-residency of the clusters was checked by make_plan: grid <= 2 * resident pairs)
-      if (p.timeline != nullptr)
-        SY_CUDA(launch_pdl_cluster(conv_tc_kernel<BN, true, AM, true>, 2, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
-      else
-        SY_CUDA(launch_pdl_cluster(conv_tc_kernel<BN, false, AM, true>, 2, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
-      return launch_status("conv_tc_kernel(pair)");
-    } else {
-      SY_REQUIRE(false, SY_EINVAL, "conv2d_tc: pair mode needs linear or halo tiles");
-    }
-  }
-  SY_REQUIRE((set_smem_attr<BN, AM, false>()), SY_ELAUNCH, "conv2d_tc: cannot opt in to %d bytes of shared memory", kSmemLimit);
+  SY_REQUIRE((set_smem_attr<BN, AM>()), SY_ELAUNCH, "conv2d_tc: cannot opt in to %d bytes of shared memory", kSmemLimit);
   if (p.n_seg > 0) {
     // The BatchNorm tail ends in a grid-wide barrier: every CTA of this launch must be resident at once.  The launch is
     // not a cooperative launch (it carries the programmatic-dependent-launch attribute instead), so check what a
@@ -1379,7 +1048,7 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
     for (int i = 0; i < 8; ++i) seen = seen || ok_smem[i] == smem;
     if (!seen) {
       int per_sm = 0;
-      SY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_tc_kernel<BN, false, AM, false>, kThreads, (size_t)smem));
+      SY_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, conv_tc_kernel<BN, false, AM>, kThreads, (size_t)smem));
       SY_REQUIRE(per_sm >= 1 && per_sm * num_sms() >= grid, SY_ELAUNCH,
                  "conv2d_tc: %d CTAs cannot be co-resident (%d per SM x %d SMs): the BatchNorm grid barrier would hang", grid,
                  per_sm, num_sms());
@@ -1388,34 +1057,26 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
     }
   }
   if (p.timeline != nullptr)
-    SY_CUDA(launch_pdl(conv_tc_kernel<BN, true, AM, false>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
+    SY_CUDA(launch_pdl(conv_tc_kernel<BN, true, AM>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
   else
-    SY_CUDA(launch_pdl(conv_tc_kernel<BN, false, AM, false>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
+    SY_CUDA(launch_pdl(conv_tc_kernel<BN, false, AM>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
   return launch_status("conv_tc_kernel");
 }
 
 template <int AM>
 static int plan_bn(int bn, Params& p, Plan* out) {
-  switch (bn) {
-    case 64: return make_plan<64, AM>(p, out);
-    case 128: return make_plan<128, AM>(p, out);
-    default: return make_plan<256, AM>(p, out);
-  }
+  return bn == 64 ? make_plan<64, AM>(p, out) : make_plan<128, AM>(p, out);
 }
 
 template <int AM>
 static int launch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, Params& p, const Plan& pl,
                      cudaStream_t stream) {
-  switch (bn) {
-    case 64: return launch<64, AM>(ta, tb, ty, p, pl, stream);
-    case 128: return launch<128, AM>(ta, tb, ty, p, pl, stream);
-    default: return launch<256, AM>(ta, tb, ty, p, pl, stream);
-  }
+  return bn == 64 ? launch<64, AM>(ta, tb, ty, p, pl, stream) : launch<128, AM>(ta, tb, ty, p, pl, stream);
 }
 
 // Halo mode (conv_tc_kernel, AM = 2) for a 3x3 stride-1 convolution?  It needs 16 x 8 patch tiles (more tiles than the
-// linear tiling on small feature maps) and pays off where the tap re-reads bound the main loop, i.e. at BN <= 128.
-// Measured per-K-block costs on B200 (cycles): linear 515 / 560, halo 430 / 370 at BN = 128 / 64; equal at BN = 256.
+// linear tiling on small feature maps) and pays off where the tap re-reads bound the main loop.  Modelled per-K-block
+// costs (cycles): linear 515 / 560, halo 430 / 370 at BN = 128 / 64.
 // SY_CONV_A=halo forces it (every eligible conv), SY_CONV_A=off disables it.
 static bool use_halo(int n, int ho, int wo, int cout, int kblocks) {
   const char* e = getenv("SY_CONV_A");
@@ -1423,7 +1084,6 @@ static bool use_halo(int n, int ho, int wo, int cout, int kblocks) {
   if (e != nullptr && e[0] == 'o') return false;
   const int tiles_l = cdiv(n * ho * wo, kBlockM), tiles_h = n * cdiv(ho, 16) * cdiv(wo, 8);
   const int bn = pick_bn(cout, tiles_l, kblocks);
-  if (bn > 128) return false;
   const double lin_c = bn == 128 ? 515.0 : 560.0, halo_c = bn == 128 ? 430.0 : 370.0;
   const int nt = cdiv(cout, bn);
   return cdiv(tiles_h * nt, num_sms()) * halo_c < cdiv(tiles_l * nt, num_sms()) * lin_c;
@@ -1468,8 +1128,7 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     p.th = 16; p.tw = 8;                                          // one 8-pixel swizzle atom per patch row
     // halo rows are stored densely (TW + 2 pixels = 1280 bytes apart): the MMA's swizzle follows the absolute shared
     // address bits, exactly like the TMA that wrote the tile, so neither the atoms' stride nor their start need 1 KiB
-    // alignment (verified on B200; debug flag 128 selects a 2 KiB row pitch instead, flag 64 sets the descriptor's
-    // base-offset field -- which breaks the result, i.e. the field must stay 0).
+    // alignment (debug flag 128 selects a 2 KiB row pitch instead, flag 64 sets the descriptor's base-offset field).
     p.halo_pitch = (p.debug_flags & 128) ? 16 : p.tw + 2;
     p.halo_tx = (p.th + 2) * p.halo_pitch * 128;
     p.halo_bytes = (p.halo_tx + 1023) / 1024 * 1024;
@@ -1554,7 +1213,6 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     const int rc = halo ? tc::plan_bn<2>(bn, p, &pl) : (lin ? tc::plan_bn<1>(bn, p, &pl) : tc::plan_bn<0>(bn, p, &pl));
     if (rc != SY_OK) return rc;
   }
-  const bool pair = pl.pair;
   if (d->rows_written) *d->rows_written = pl.grid;
 
   // A: input view as (C, W, H, N), box (64, TW*s, TH*s, 1) traversed with element strides (1, s, s, 1)
@@ -1603,7 +1261,7 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     const int taps = d->kh * d->kw;
     cuuint64_t dims[3] = {(cuuint64_t)x.c, (cuuint64_t)taps, (cuuint64_t)y.c};
     cuuint64_t strides[2] = {(cuuint64_t)x.c * 2, (cuuint64_t)x.c * 2 * taps};
-    cuuint32_t box[3] = {(cuuint32_t)tc::kBlockK, 1, (cuuint32_t)(pair ? bn / 2 : bn)};   // pair: each CTA loads half a slab
+    cuuint32_t box[3] = {(cuuint32_t)tc::kBlockK, 1, (cuuint32_t)bn};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&tb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d->w), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,

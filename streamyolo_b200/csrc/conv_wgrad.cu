@@ -1,20 +1,20 @@
-// Weight gradient of a convolution on the Blackwell tensor cores (sm_100a):
+// Weight gradient of a convolution on the Hopper tensor cores (sm_90a, wgmma):
 //
 //   dW[co][tap][ci] = sum over output pixels p of  dy[p][co] * x[p @ tap][ci]
 //
-// as one GEMM per filter tap with  M = output channels (128 per tile, one TMEM lane each),  N = input channels (BN),
-// K = output pixels.  In NHWC both operands have K (pixels) as the strided dimension, so they are staged "MN-major":
-// every shared-memory row is one pixel holding 64 contiguous channels -- exactly what a TMA load of a [64 px][64 ch]
-// box with the 128B swizzle writes.  Verified with tools/mn_probe.cu: descriptor LBO = 8192 B (next 64-channel box),
-// SBO = 1024 B (next 8 pixels), +2048 B per K = 16 step, instruction-descriptor bits 15/16 (A/B MN-major).
+// as one GEMM per filter tap with  M = output channels (128 per tile, 64 per consumer warpgroup),  N = input channels (BN),
+// K = output pixels.  In NHWC both operands have K (pixels) as the strided dimension, so they are staged "MN-major"
+// (wgmma's transposed operand form): every shared-memory row is one pixel holding 64 contiguous channels -- exactly what a
+// TMA load of a [64 px][64 ch] box with the 128B swizzle writes.  Descriptor LBO = 8192 B (next 64-channel box),
+// SBO = 1024 B (next 8 pixels), +2048 B per K = 16 step.
 //   * dy tile: plain 2-D TMA boxes of the [pixels][Cout] view;
 //   * x tile for tap (r, s): im2col-mode TMA (the forward kernel's loader) of the same 64 output pixels' input positions
 //     shifted by the tap -- stride-2 convs and the zero padding come for free.
 // The pixel range is split over CTAs (split-K); every CTA writes an fp32 partial [128][BN] per work item and a second
 // kernel reduces the partials in a fixed order (deterministic) into the optimizer's fp32 OIHW layout.
 //
-// Replaces the cuDNN backward-filter call behind loss.backward() (/root/reference/exps/train_utils/double_trainer.py:114)
-// for every [yolox] BaseConv (/root/reference/exps/model/darknet.py:115-165, dfp_pafpn.py:33-105, tal_head.py:55-104).
+// Replaces the cuDNN backward-filter call behind loss.backward() (exps/train_utils/double_trainer.py:114 of StreamYOLO)
+// for every [yolox] BaseConv (exps/model/darknet.py:115-165, dfp_pafpn.py:33-105, tal_head.py:55-104).
 #include <cuda.h>
 
 #include "common.cuh"
@@ -25,7 +25,7 @@ namespace wg {
 
 using namespace tc;
 
-constexpr int kThreads = 192;            // warps 0-3 epilogue (TMEM lanes 0..127), warp 4 TMA producer, warp 5 MMA issuer
+constexpr int kThreads = 288;            // warps 0-7: two MMA + epilogue warpgroups (rows 0-63, 64-127), warp 8: TMA producer
 constexpr int kPixK = 64;                // pixels per pipeline stage (K block)
 constexpr int kBoxBytes = kPixK * 128;   // one [64 px][64 ch] box
 constexpr int kMaxStages = 8;
@@ -45,19 +45,7 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
 // MN-major, 128B-swizzled operand: rows = K (pixels) of 128 bytes, 8-row groups 1 KiB apart, 64-channel boxes 8 KiB apart
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)(kBoxBytes >> 4) << 16;       // leading byte offset
-  d |= (uint64_t)(1024u >> 4) << 32;           // stride byte offset
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// D f32, A = B = bf16, both MN-major, M = 128
-__host__ __device__ constexpr uint32_t make_idesc_mn(int n) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
+__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr) { return make_gmma_desc(saddr, kBoxBytes, 1024u); }
 
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -68,36 +56,21 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int S = p.stages;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + S * kStageBytes);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kMaxStages + 4);
   const uint32_t bar0 = smem_u32(bars);
   auto full_bar = [&](int s) { return bar0 + 8u * s; };
   auto empty_bar = [&](int s) { return bar0 + 8u * (kMaxStages + s); };
-  // two accumulators (2 x BN TMEM columns): the epilogue of work item i (TMEM -> 128 x BN fp32 partial in global memory)
-  // overlaps the main loop of item i + 1 (with one accumulator the MMA warp idled through every epilogue)
-  auto tfull_bar = [&](int a) { return bar0 + 8u * (2 * kMaxStages + a); };
-  auto tempty_bar = [&](int a) { return bar0 + 8u * (2 * kMaxStages + 2 + a); };
-  constexpr int kTmemCols = 2 * BN;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  (void)lane;
 
-  if (threadIdx.x == 5 * 32) {
+  if (threadIdx.x == 8 * 32) {
     prefetch_tmap(&tmDY);
     prefetch_tmap(&tmX);
     for (int s = 0; s < S; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull_bar(a), 1);
-      mbar_init(tempty_bar(a), 128);
+      mbar_init(empty_bar(s), 2);                // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(smem_u32(tmem_slot), kTmemCols);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int hw = p.Ho * p.Wo;
 
   auto decode = [&](int item, int& m_tile, int& n_tile, int& tap, int& kb0, int& kb1) {
@@ -110,7 +83,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     kb1 = min(kb0 + p.kb_per_split, p.kb_total);
   };
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer
     int stage = 0;
     uint32_t phase = 0;
@@ -124,80 +97,61 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
         const int oh = fdiv(rem, p.fd_wo), ow = rem - oh * p.Wo;
         mbar_wait(empty_bar(stage), phase ^ 1u);
         uint8_t* st = smem + stage * kStageBytes;
-        if (elect_one()) mbar_expect_tx(full_bar(stage), (uint32_t)kStageBytes);
+        if (elect_one()) {
+          mbar_expect_tx(full_bar(stage), (uint32_t)kStageBytes);
 #pragma unroll
-        for (int j = 0; j < 2; ++j)
-          if (elect_one()) tma_load_2d(smem_u32(st + j * kBoxBytes), &tmDY, full_bar(stage), m_tile * 128 + j * 64, p0);
+          for (int j = 0; j < 2; ++j) tma_load_2d(smem_u32(st + j * kBoxBytes), &tmDY, full_bar(stage), m_tile * 128 + j * 64, p0);
 #pragma unroll
-        for (int j = 0; j < kXBoxes; ++j)
-          if (elect_one())
+          for (int j = 0; j < kXBoxes; ++j)
             tma_load_im2col_4d(smem_u32(st + (2 + j) * kBoxBytes), &tmX, full_bar(stage), n_tile * BN + j * 64,
                                ow * p.stride - p.pad_w, oh * p.stride - p.pad_h, img, (uint16_t)sx, (uint16_t)r);
-        __syncwarp();
-        if (++stage == S) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp == 5) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = make_idesc_mn(BN);
-    int stage = 0, it = 0;
-    uint32_t phase = 0;
-    for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
-      int m_tile, n_tile, tap, kb0, kb1;
-      decode(item, m_tile, n_tile, tap, kb0, kb1);
-      const int acc = it & 1;
-      mbar_wait(tempty_bar(acc), (((uint32_t)it >> 1) & 1u) ^ 1u);   // the epilogue has drained this accumulator
-      tcgen05_fence_after();
-      const uint32_t tmem_d = tmem_base + (uint32_t)(acc * BN);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(full_bar(stage), phase);
-        tcgen05_fence_after();
-        if (elect_one()) {
-          const uint32_t a0 = smem_u32(smem + stage * kStageBytes), b0 = a0 + 2 * kBoxBytes;
-#pragma unroll
-          for (int k = 0; k < kPixK / 16; ++k)
-            umma_bf16(tmem_d, make_desc_mn(a0 + k * 2048), make_desc_mn(b0 + k * 2048), idesc, (kb != kb0) || (k != 0));
-          umma_commit(empty_bar(stage));
-          if (kb == kb1 - 1) umma_commit(tfull_bar(acc));
         }
         __syncwarp();
         if (++stage == S) { stage = 0; phase ^= 1u; }
       }
-      if (kb1 <= kb0 && elect_one()) umma_commit(tfull_bar(acc));     // empty split (cannot happen with the host's ksplit; keeps the protocol safe)
-      __syncwarp();
     }
   } else {
-    // ------------------------------------------------------------------ epilogue: TMEM -> fp32 partial [128][BN]
-    int it = 0;
-    for (int item = blockIdx.x; item < p.items; item += gridDim.x, ++it) {
+    // ------------------------------------------------------------------ MMA + epilogue: registers -> fp32 partial [128][BN]
+    // Warpgroup g computes output channels [64 g, 64 g + 64) of the tile (its dy box); a ring stage goes back to the producer
+    // one commit group late, so the next group's MMAs are queued while the last ones drain.
+    const int g = warp >> 2;
+    const bool lead = (threadIdx.x & 127) == 0;
+    const int row0 = g * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    float acc[BN / 2];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = blockIdx.x; item < p.items; item += gridDim.x) {
       int m_tile, n_tile, tap, kb0, kb1;
       decode(item, m_tile, n_tile, tap, kb0, kb1);
-      const int acc = it & 1;
-      mbar_wait(tfull_bar(acc), ((uint32_t)it >> 1) & 1u);
-      tcgen05_fence_after();
-      const int row = warp * 32 + lane;
-      float* dst = p.partial + ((size_t)item * 128 + row) * BN;
-      const bool empty = kb1 <= kb0;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(acc * BN + c0), v);
-        tmem_ld_wait();
+      int pend = -1;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t a0 = smem_u32(smem + stage * kStageBytes) + (uint32_t)(g * kBoxBytes), b0 = smem_u32(smem + stage * kStageBytes) + 2 * kBoxBytes;
+        wgmma_fence_operand(acc);
+        wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 32; i += 4)
-          *reinterpret_cast<float4*>(dst + c0 + i) =
-              empty ? make_float4(0.f, 0.f, 0.f, 0.f)
-                    : make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
+        for (int k = 0; k < kPixK / 16; ++k)
+          Wgmma<BN, 1, 1>::mma(acc, make_desc_mn(a0 + k * 2048), make_desc_mn(b0 + k * 2048), (kb != kb0) || (k != 0));
+        wgmma_commit();
+        wgmma_fence_operand(acc);
+        wgmma_wait<1>();
+        if (lead && pend >= 0) mbar_arrive(empty_bar(pend));
+        pend = stage;
+        if (++stage == S) { stage = 0; phase ^= 1u; }
       }
-      tcgen05_fence_before();
-      mbar_arrive(tempty_bar(acc));
+      wgmma_wait<0>();
+      wgmma_fence_operand(acc);
+      if (lead && pend >= 0) mbar_arrive(empty_bar(pend));
+      const bool empty = kb1 <= kb0;             // (cannot happen with the host's ksplit; keeps the output defined)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float* dst = p.partial + ((size_t)item * 128 + row0 + 8 * h) * BN + cq;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j)
+          *reinterpret_cast<float2*>(dst + 8 * j) = empty ? make_float2(0.f, 0.f) : make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -302,7 +256,7 @@ static int launch(const CUtensorMap& tdy, const CUtensorMap& tx, WParams& p, cud
   int stages = (kSmemLimit - 1024 - 512) / stage_bytes;
   if (stages > kMaxStages) stages = kMaxStages;
   p.stages = stages;
-  const int smem = 1024 + 512 + stages * stage_bytes;
+  const int smem = 1024 + 512 + stages * stage_bytes;   // align slack + barriers + ring
   const int grid = p.items < num_sms() ? p.items : num_sms();
   conv_wgrad_kernel<BN><<<grid, kThreads, smem, stream>>>(tdy, tx, p);
   return launch_status("conv_wgrad_kernel");
@@ -372,14 +326,14 @@ extern "C" int sy_conv2d_wgrad_tc(const SyConvWgradDesc* d, sy_stream_t stream_)
   }
   if (lrc != SY_OK) return lrc;
   const long long total = (long long)dy.c * x.c * pl.taps;
-  // split groups per output: enough threads to cover the GPU (~148 x 2048) and at least 8 splits per group
+  // split groups per output: enough threads to cover the GPU (SMs x 2048) and at least 8 splits per group
   int sg = 1;
   if (getenv("SY_WGRAD_SG1") == nullptr) {
-    while (sg < 8 && total * sg < 148LL * 2048 && pl.ksplit >= 16 * sg) sg *= 2;
+    while (sg < 8 && total * sg < (long long)tc::num_sms() * 2048 && pl.ksplit >= 16 * sg) sg *= 2;
   }
   const long long per_block = 256 / sg;
   const long long want = (total + per_block - 1) / per_block;
-  const int blocks = (int)(want < 148 * 8 ? want : 148 * 8);
+  const int blocks = (int)(want < tc::num_sms() * 8 ? want : tc::num_sms() * 8);
   switch (sg) {
     case 8: wg::wgrad_reduce_kernel<8><<<blocks, 256, 0, stream>>>(p.partial, pl.bn, pl.m_tiles, pl.n_tiles, pl.taps, pl.ksplit, dy.c, x.c, d->dw, d->accumulate); break;
     case 4: wg::wgrad_reduce_kernel<4><<<blocks, 256, 0, stream>>>(p.partial, pl.bn, pl.m_tiles, pl.n_tiles, pl.taps, pl.ksplit, dy.c, x.c, d->dw, d->accumulate); break;

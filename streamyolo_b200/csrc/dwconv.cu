@@ -94,7 +94,7 @@ extern "C" int sy_dwconv2d(const SyConvDesc* d, sy_stream_t stream_) {
   p.mode = d->mode; p.act = d->act;
   const long long total = (long long)x.n * ho * wo * (x.c / 8);
   long long blocks = (total + 255) / 256;
-  if (blocks > 148ll * 32) blocks = 148ll * 32;
+  if (blocks > (long long)sm_count() * 32) blocks = (long long)sm_count() * 32;
   if (blocks < 1) blocks = 1;
   switch (d->kh) {
     case 1: dwconv_kernel<1><<<(int)blocks, 256, 0, stream>>>(p); break;

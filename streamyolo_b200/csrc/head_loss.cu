@@ -210,7 +210,7 @@ static int launch_head_pred_pt(const SyHeadPredDesc* d, const SyTensor& f, cudaS
     SY_CUDA(cudaFuncSetAttribute(head_pred_kernel<NO, PT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const long long npix = (long long)f.n * f.h * f.w;
   int blocks = (int)((npix + 64 * PT - 1) / (64 * PT));
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   head_pred_kernel<NO, PT><<<blocks, 256, smem, stream>>>(*d, f.n, f.h, f.w, f.c);
   return launch_status("head_pred_kernel");
 }
@@ -231,7 +231,7 @@ static int launch_head_pred_generic(const SyHeadPredDesc* d, const SyTensor& f, 
     SY_CUDA(cudaFuncSetAttribute(head_pred_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const long long npix = (long long)f.n * f.h * f.w;
   int blocks = (int)((npix + 63) / 64);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   head_pred_generic_kernel<<<blocks, 256, smem, stream>>>(*d, f.n, f.h, f.w, f.c, NO);
   return launch_status("head_pred_generic_kernel");
 }

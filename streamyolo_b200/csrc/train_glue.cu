@@ -211,7 +211,7 @@ __global__ void scale_labels_kernel(float* lab, long long rows, int cols, float 
 
 static int grid_for(long long total, int block) {
   long long g = (total + block - 1) / block;
-  if (g > 148ll * 16) g = 148ll * 16;
+  if (g > (long long)sm_count() * 16) g = (long long)sm_count() * 16;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -238,7 +238,7 @@ extern "C" int64_t sy_pack_item_tiles(int32_t cout, int32_t cin, int32_t mode) {
 extern "C" int sy_pack_conv_weights_batch(const SyPackItem* items_dev, int32_t n_items, int64_t total, sy_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   SY_REQUIRE(items_dev != nullptr && n_items > 0 && total > 0, SY_EINVAL, "pack_conv_weights_batch: bad arguments");
-  const int grid = (int)(total < 148ll * 8 ? total : 148ll * 8);
+  const int grid = (int)(total < (long long)sm_count() * 8 ? total : (long long)sm_count() * 8);
   pack_weights_batch_kernel<<<grid, 256, 0, stream>>>(items_dev, n_items, total);
   return launch_status("pack_weights_batch_kernel");
 }

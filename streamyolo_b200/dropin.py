@@ -1,5 +1,5 @@
 """Make ``from exps.model.yolox import YOLOX`` (what the reference's cfgs/*.py do,
-/root/reference/cfgs/s_s50_onex_dfp_tal_flip.py:35-37) resolve to the B200 implementation.
+/root/reference/cfgs/s_s50_onex_dfp_tal_flip.py:35-37) resolve to this implementation.
 
     import streamyolo_b200.dropin; streamyolo_b200.dropin.install()     # before get_exp(...)
 

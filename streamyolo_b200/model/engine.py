@@ -1,6 +1,6 @@
 """Layer executor: walks the module tree with NHWC bf16 views and launches the CUDA ops.
 
-Train mode (``model.training``): every BaseConv = tcgen05 conv writing the raw bf16 result + per-tile
+Train mode (``model.training``): every BaseConv = wgmma conv writing the raw bf16 result + per-tile
 statistic partials  ->  bn_finalize (batch statistics, running-stat update)  ->  bn_act_apply
 (normalise + SiLU + optional residual, written straight into its consumer's concat slice).
 The two frames of a pair are batched through the shared-weight backbone as 2B images with
@@ -19,9 +19,8 @@ from .. import ops
 from ..ops import View
 
 
-# normalise pass inside the conv launch (1 launch / BaseConv).  For every layer it was measured SLOWER on B200 (11.7 vs
-# 8.2 ms/step: one CTA per SM cannot keep enough bytes in flight on the big tensors), so SY_FUSE_APPLY=1 is a debug
-# switch; SY_FUSE_APPLY_MAX_MB fuses only the layers whose raw output is at most that many MB (L2 resident, launch-bound)
+# normalise pass inside the conv launch (1 launch / BaseConv).  One CTA per SM keeps fewer bytes in flight on the big tensors
+# than the separate pass (not measured on H100), so SY_FUSE_APPLY=1 is a debug switch; SY_FUSE_APPLY_MAX_MB fuses only the layers whose raw output is at most that many MB (L2 resident, launch-bound)
 FUSE_APPLY = os.environ.get("SY_FUSE_APPLY", "0") != "0"
 FUSE_APPLY_MAX_BYTES = float(os.environ.get("SY_FUSE_APPLY_MAX_MB", "0")) * 1e6
 WEIGHT_EPOCH = 0  # bumped by whoever updates parameters through raw pointers (train.Trainer's fused optimiser kernel does
@@ -192,7 +191,7 @@ def graph_capture_stream(device):
 
 
 def _dbg_skip_apply(nbytes):
-    """timing experiments only (tools/ab_step.py): SY_DBG_SKIP_APPLY="lo:hi" (MB) drops the normalise pass of the layers whose
+    """timing experiments only: SY_DBG_SKIP_APPLY="lo:hi" (MB) drops the normalise pass of the layers whose
     raw output size lies in [lo, hi) -- the results are garbage, the step time shows what those launches really cost"""
     e = os.environ.get("SY_DBG_SKIP_APPLY")
     if not e:

@@ -1,5 +1,5 @@
 """TALHead: decoupled YOLOX head + SimOTA + Trend-Aware Loss (mirror of
-/root/reference/exps/model/tal_head.py).  Towers run on the tcgen05 conv kernel, the three
+/root/reference/exps/model/tal_head.py).  Towers run on the wgmma conv kernel, the three
 prediction convs + box decode are one kernel per level writing [B, A, 5+ncls] directly, and the
 whole of get_losses/get_assignments/dynamic_k_matching is ``sy_tal_loss`` (no host sync)."""
 import math

@@ -1,7 +1,7 @@
 """ctypes binding of libstreamyolo_sm100.so (include/streamyolo_sm100.h) + NHWC view helper.
 
 The library is the product; there is NO fallback: if it is missing or the device is not an
-sm_100 part, every op raises RuntimeError.
+sm_90 part, every op raises RuntimeError.
 """
 import ctypes as C
 import os
@@ -186,12 +186,12 @@ def load_library():
 
 
 def lib():
-    """Library handle for compute calls: also insists on a CUDA sm_100 device."""
+    """Library handle for compute calls: also insists on a CUDA sm_90 device."""
     global _device_ok
     l = load_library()
     if not _device_ok:
         if not torch.cuda.is_available():
-            raise RuntimeError("streamyolo_b200 needs a CUDA sm_100 (B200) device; there is no CPU path")
+            raise RuntimeError("streamyolo_b200 needs a CUDA sm_90 (H100) device; there is no CPU path")
         rc = l.sy_check_device()
         if rc != 0:
             raise RuntimeError("streamyolo_b200: " + l.sy_last_error_string().decode())

@@ -6,7 +6,7 @@
     plain PyTorch -- the drop-in path, used when the reference's own Trainer drives ``model(inps, targets)`` /
     ``loss.backward()`` (the training forward returns a loss with a grad_fn, model/backward.py) -- and the bit-level
     reference of the fused kernel.
-  * ``Trainer``: the B200-native step.  Parameters, gradients, momentum and the EMA copy live in FLAT fp32 buffers laid out in
+  * ``Trainer``: the H100-native step.  Parameters, gradients, momentum and the EMA copy live in FLAT fp32 buffers laid out in
     the order in which the backward walk finishes the gradients; every ``nn.Parameter`` / BatchNorm buffer of the model is a
     view into them (state_dict, checkpoints and ``model.parameters()`` are unchanged).
       - the weight-gradient / BatchNorm-gradient kernels write straight into the flat gradient buffer (``FlatSink``);
@@ -305,7 +305,7 @@ class FlatSink:
 
 
 class Trainer:
-    """B200-native training loop body for YOLOX(DFPPAFPN, TALHead): ``step(x, targets, lr)``."""
+    """H100-native training loop body for YOLOX(DFPPAFPN, TALHead): ``step(x, targets, lr)``."""
 
     def __init__(self, model, lr=0.01, momentum=0.9, weight_decay=5e-4, ema_decay=0.9998, use_ema=True,
                  bucket_bytes=25 << 20, overlap=True):

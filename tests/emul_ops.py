@@ -1,6 +1,6 @@
 """CPU emulation of the ``streamyolo_b200.ops`` entry points in plain PyTorch -- TEST INFRASTRUCTURE ONLY.
 
-The product has no CPU path (``ops.lib()`` raises without the CUDA library and an sm_100 device).  The host-side logic above
+The product has no CPU path (``ops.lib()`` raises without the CUDA library and an sm_90 device).  The host-side logic above
 the C ABI -- which buffers feed which kernel, in-place concat slices, gradient routing of the backward walk -- is plain
 Python, though, and can be checked without a GPU if every kernel call is replaced by a few lines of torch with the same
 contract (same arguments, same bf16 rounding points).  ``install(monkeypatch)`` swaps the functions of ``ops`` for these;
@@ -42,7 +42,7 @@ def _unpack(wpk, kh, kw):
 
 
 def conv_stat_rows():
-    return 148
+    return 132
 
 
 def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=None, partials=None, split_n=0,
@@ -91,7 +91,7 @@ def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=
                     nbt.add_(1)
         PTRS[scale_shift[0].data_ptr()] = scale_shift[0]
         PTRS[scale_shift[1].data_ptr()] = scale_shift[1]
-    return 148
+    return 132
 
 
 def _strided(v: View, img0, nimg, goff):

@@ -1,4 +1,4 @@
-"""CPU: the B200-native training step (streamyolo_b200/train.py: flat fp32 state, gradient sink writing into the flat
+"""CPU: the H100-native training step (streamyolo_b200/train.py: flat fp32 state, gradient sink writing into the flat
 buffer in walk order, bucketed all-reduce launched from the walk, fused optimiser step) with every kernel replaced by its
 torch emulation (tests/emul_ops.py), against the same step made of stock PyTorch pieces (torch.optim.SGD with the
 reference's three parameter groups, the Python ModelEMA, a post-hoc all-reduce) -- the semantics of the reference's trainer

@@ -319,7 +319,7 @@ def test_loss_backward_vs_oracle_autograd():
 def test_forward_backward_vs_oracle_autograd():
     """streamyolo_b200.model.backward.forward_backward on the GPU against autograd through the oracle with bf16 storage
     (which tests/test_oracle_golden.py pins to the reference's loss.backward()).  A random-init train-mode BatchNorm net is
-    chaotic under bf16 storage (tools/diag_bwd.py, profiles/r02_backward_noise_floor.txt: nudging the inputs by half a bf16
+    chaotic under bf16 storage (tests/tools/diag_bwd.py: nudging the inputs by half a bf16
     ulp decorrelates the stride-32 gradients of the ORACLE ITSELF at 120x160, rel ~1.0), so the element-wise bar lives in
     tests/test_gpu_train.py::test_walk_in_situ_every_conv_backward (identical inputs per op); here, on a larger map where
     the noise is moderate, every parameter gradient must be finite, point the right way and have the right size:

@@ -26,7 +26,7 @@ from test_gpu_ops import bf, check_close, rand_w  # noqa: E402
 
 DEV = "cuda"
 
-# (n, cin, cout, h, w, k, stride, conv1|conv2 pair) -- profiles/r01_conv_plan_l_b8.txt, distinct rows
+# (n, cin, cout, h, w, k, stride, conv1|conv2 pair) -- the distinct conv shapes of StreamYOLO-l at 8 pairs
 L_SHAPES = [
     (16, 64, 128, 300, 480, 3, 2, False),
     (16, 128, 128, 150, 240, 1, 1, True),

@@ -1,4 +1,4 @@
-"""The same-box LIBRARY bar (SURVEY section 2.1: "whatever cuDNN / ATen picks on B200 ... is the bar on the same box"):
+"""The same-box LIBRARY bar (SURVEY section 2.1: "whatever cuDNN / ATen picks on the GPU ... is the bar on the same box"):
 the reference's network (CSPDarknet + PAFPN on both frames with shared weights, DFP fusion, TALHead towers and prediction
 convs -- /root/reference/exps/model/{darknet,dfp_pafpn,tal_head}.py) assembled from the in-repo stand-in of the yolox 0.3.0
 blocks (oracle/ref_shim: nn.Conv2d + nn.BatchNorm2d + nn.SiLU), run the way the reference trains on GPUs: CUDA, bf16

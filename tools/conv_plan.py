@@ -1,6 +1,6 @@
 """Per-layer tiling plan of one training-forward step (no GPU needed): dry-runs the engine with the kernels mocked
 (tools/op_sequence.py) and asks the library's host-only planner (sy_conv2d_plan) what sy_conv2d_tc does for each conv:
-A-operand mode (patch / linear = im2col-mode TMA / halo), tile width, tiles, rounds of the 148-CTA persistent grid.
+A-operand mode (patch / linear = im2col-mode TMA / halo), tile width, tiles, rounds of the persistent grid (one CTA per SM).
 
     python tools/conv_plan.py [model] [pairs]"""
 import os
@@ -26,7 +26,7 @@ for s in seq:
     n, h, w, ci, co, kh, kw, st = map(int, m.groups())
     p = plan(n, h, w, ci, co, (kh, kw), st)
     tiles = p["m_tiles"] * p["n_tiles"]
-    fill = tiles / (p["rounds"] * 148)
+    fill = tiles / (p["rounds"] * ops.conv_stat_rows())
     tot[MODE[p["mode"]]] = tot.get(MODE[p["mode"]], 0) + 1
     print(f"{s['name'][-50:]:50s} {s['shape']:34s} {MODE[p['mode']]:7s} {p['bn']:4d} {tiles:6d} {p['rounds']:6d} {p['kblocks']:6d} {fill:5.2f}")
 print("launches per mode:", tot)

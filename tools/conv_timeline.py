@@ -1,4 +1,4 @@
-"""Pipeline timeline of CTA 0 of the tcgen05 conv kernel (debug instrumentation) + event timing.
+"""Pipeline timeline of CTA 0 of the wgmma conv kernel (debug instrumentation) + event timing.
 usage: python tools/conv_timeline.py n cin cout h w k s [reps]"""
 import os
 import sys

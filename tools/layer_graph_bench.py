@@ -1,5 +1,5 @@
 """Per-layer time INSIDE a CUDA graph (what the step really pays), for every distinct BaseConv launch of the benchmark
-workload: the train-mode conv (tcgen05 kernel with statistics + BatchNorm finalize) and its normalise pass, each replayed
+workload: the train-mode conv (wgmma kernel with statistics + BatchNorm finalize) and its normalise pass, each replayed
 R times back to back in one graph (PDL edges like the real step), next to the layer's roofline time
 max(FLOPs / tensor peak, algorithmic bytes / HBM peak).  The sum over the step's launches is compared with bench.py.
 
