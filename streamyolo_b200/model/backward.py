@@ -5,9 +5,10 @@
 What ``loss.backward()`` does for the reference (/root/reference/exps/train_utils/double_trainer.py:110-114) through
 exps/model/{yolox,dfp_pafpn,darknet,tal_head}.py, expressed over the kernels of libstreamyolo_sm100 (DESIGN.md 4.3):
 
-  * the forward is the product's forward (same kernels, same batching of the two frames with grouped BatchNorm statistics)
-    with two differences that a backward pass needs: nothing is updated in place (every conv keeps its input, its raw
-    output and the batch statistics), and the DFP fusion runs its two jian convs as two launches;
+  * the forward is the engine's walk of the product's forward (model/engine.py: same kernels, same batching of the two
+    frames with grouped BatchNorm statistics) run with a ``Tape``, which makes the two differences a backward pass needs:
+    nothing is updated in place (every conv keeps its input, its raw output and the batch statistics), and the DFP fusion
+    runs its two jian convs as two launches;
   * every recorded op then runs its backward in reverse order.  Gradients of activations live in bf16 buffers that mirror
     the activation buffers (a channel / image slice of an activation is the same slice of its gradient buffer) and are
     *accumulated*: a tensor read by several consumers (Bottleneck shortcuts, FPN features, the concat buffers) simply
@@ -27,6 +28,7 @@ mode with gradients enabled returns ``loss_with_autograd`` (the step as one auto
 import torch
 
 from . import engine
+from .tal_head import _f32
 from .. import ops
 from ..ops import View
 
@@ -266,169 +268,6 @@ class TensorSink:
         return self.views.get(id(p))
 
 
-# ------------------------------------------------------------------------------------------------ recording forward
-def conv_rec(T: Tape, mods, x: View, wpk, k, s, y: View, split, res: View = None, act=1, kind="normal"):
-    """conv -> train-mode BatchNorm (statistics groups split at image ``split``; 0 = one group) -> act (+ res) into ``y``;
-    keeps what the backward needs.  ``mods``: one BaseConv, or the conv1 | conv2 pair of a CSPLayer (one GEMM)."""
-    kh, kw = (k, k) if isinstance(k, int) else k
-    ho = (x.h + 2 * ((kh - 1) // 2) - kh) // s + 1
-    wo = (x.w + 2 * ((kw - 1) // 2) - kw) // s + 1
-    cout = sum(m.conv.out_channels for m in mods)
-    dev = T.device
-    raw = View.empty(x.n, ho, wo, cout, dev)
-    bn0 = mods[0].bn
-    mom = float(0.1 if bn0.momentum is None else bn0.momentum)
-    for m in mods:
-        m._stats_epoch = getattr(m, "_stats_epoch", 0) + 1
-    partials = torch.empty((ops.conv_stat_rows(), 4 * cout), dtype=torch.float32, device=dev)
-    segs, c0 = [], 0
-    for m in mods:
-        segs.append(engine._bn_seg(m, c0))
-        c0 += m.conv.out_channels
-    ss = torch.empty((2, 2, cout), dtype=torch.float32, device=dev)
-    mi = torch.empty((2, 2, cout), dtype=torch.float32, device=dev)
-    ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl="tc", partials=partials, split_n=split, bn=segs, momentum=mom,
-               eps=float(bn0.eps), scale_shift=ss, sync=engine._sync(mods[0], dev), mean_invstd=mi)
-    ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), split if split else x.n, act, res, y)
-    T.rec(t="conv", mods=mods, x=x, k=(kh, kw), s=s, raw=raw, y=y, res=res, ss=ss, mi=mi, split=split, act=act, kind=kind)
-    T.uses[id(mods[0])] = T.uses.get(id(mods[0]), 0) + 1
-    return y
-
-
-def base_conv_rec(T, m, x, split, y=None, res=None):
-    k, s = m.ksize, m.stride
-    ho, wo = ops.conv_out_hw(x.h, x.w, k, s)
-    if y is None:
-        y = View.empty(x.n, ho, wo, m.conv.out_channels, T.device)
-    return conv_rec(T, (m,), x, engine._packed(m), k, s, y, split, res, 1 if m.act_name == "silu" else 0)
-
-
-def csp_rec(T, m, x, split, out=None):
-    """CSPLayer without in-place updates: conv1 | conv2 as one GEMM into ``u0``; the bottleneck chain in fresh buffers, its
-    last output straight into the concat buffer ``u``; conv2's half copied next to it; conv3."""
-    hid = m.conv1.conv.out_channels
-    dev = T.device
-    u0 = View.empty(x.n, x.h, x.w, 2 * hid, dev)
-    conv_rec(T, (m.conv1, m.conv2), x, engine._packed_pair(m.conv1, m.conv2), 1, 1, u0, split)
-    u = View.empty(x.n, x.h, x.w, 2 * hid, dev)
-    a = u0.ch(0, hid)
-    nblk = len(m.m)
-    for i, blk in enumerate(m.m):
-        t = base_conv_rec(T, blk.conv1, a, split)
-        dst = u.ch(0, hid) if i == nblk - 1 else View.empty(x.n, x.h, x.w, hid, dev)
-        base_conv_rec(T, blk.conv2, t, split, dst, res=a if blk.use_add else None)
-        a = dst
-    if nblk == 0:
-        ops.copy(a, u.ch(0, hid))
-        T.rec(t="copy", src=a, dst=u.ch(0, hid))
-    ops.copy(u0.ch(hid, hid), u.ch(hid, hid))
-    T.rec(t="copy", src=u0.ch(hid, hid), dst=u.ch(hid, hid))
-    return base_conv_rec(T, m.conv3, u, split, out)
-
-
-def pafpn_rec(T, net, x, frames, split):
-    """engine.pafpn_frames in recording mode (same buffers / concat slices, no in-place bottleneck chain)."""
-    bb = net.backbone
-    dev = T.device
-    c3 = net.C3_p3.conv3.conv.out_channels
-    c4 = net.C3_p4.conv3.conv.out_channels
-    b, ch, h, w = x.shape
-    n = frames * b
-    stem = bb.stem.conv
-    xin = View.empty(n, h // 2, w // 2, 64, dev)
-    ops.focus_pack(x, frames, xin)
-    t = View.empty(n, h // 2, w // 2, stem.conv.out_channels, dev)
-    conv_rec(T, (stem,), xin, engine._packed_stem(stem), ops.STEM_K, 1, t, split, kind="stem")
-    t = base_conv_rec(T, bb.dark2[0], t, split)
-    t = csp_rec(T, bb.dark2[1], t, split)
-    t = base_conv_rec(T, bb.dark3[0], t, split)
-    h8, w8 = t.h, t.w
-    f1 = View.empty(n, h8, w8, 2 * c3, dev)              # cat(up(fpn_out1), dark3)
-    x2 = csp_rec(T, bb.dark3[1], t, split, f1.ch(c3, c3))
-    t = base_conv_rec(T, bb.dark4[0], x2, split)
-    h16, w16 = t.h, t.w
-    f0 = View.empty(n, h16, w16, 2 * c4, dev)            # cat(up(fpn_out0), dark4)
-    x1 = csp_rec(T, bb.dark4[1], t, split, f0.ch(c4, c4))
-    t = base_conv_rec(T, bb.dark5[0], x1, split)
-    h32, w32 = t.h, t.w
-    spp = bb.dark5[1]
-    hid = spp.conv1.conv.out_channels
-    sbuf = View.empty(n, h32, w32, 4 * hid, dev)
-    base_conv_rec(T, spp.conv1, t, split, sbuf.ch(0, hid))
-    ops.spp_maxpool(sbuf.ch(0, hid), sbuf.ch(hid, hid), sbuf.ch(2 * hid, hid), sbuf.ch(3 * hid, hid))
-    T.rec(t="spp", x=sbuf.ch(0, hid), y5=sbuf.ch(hid, hid), y9=sbuf.ch(2 * hid, hid), y13=sbuf.ch(3 * hid, hid))
-    t = base_conv_rec(T, spp.conv2, sbuf, split)
-    x0 = csp_rec(T, bb.dark5[2], t, split)
-    z0 = View.empty(n, h32, w32, 2 * c4, dev)            # cat(bu_conv1, fpn_out0)
-    fpn0 = base_conv_rec(T, net.lateral_conv0, x0, split, z0.ch(c4, c4))
-    ops.upsample_nearest(fpn0, f0.ch(0, c4))
-    T.rec(t="upsample", x=fpn0, y=f0.ch(0, c4))
-    fo0 = csp_rec(T, net.C3_p4, f0, split)
-    z1 = View.empty(n, h16, w16, 2 * c3, dev)            # cat(bu_conv2, fpn_out1)
-    fpn1 = base_conv_rec(T, net.reduce_conv1, fo0, split, z1.ch(c3, c3))
-    ops.upsample_nearest(fpn1, f1.ch(0, c3))
-    T.rec(t="upsample", x=fpn1, y=f1.ch(0, c3))
-    pan2 = csp_rec(T, net.C3_p3, f1, split)
-    base_conv_rec(T, net.bu_conv2, pan2, split, z1.ch(0, c3))
-    pan1 = csp_rec(T, net.C3_n3, z1, split)
-    base_conv_rec(T, net.bu_conv1, pan1, split, z0.ch(0, c4))
-    pan0 = csp_rec(T, net.C3_n4, z0, split)
-    return pan2, pan1, pan0
-
-
-def dfp_rec(T, net, cur, sup):
-    """out = cat(jian(cur), jian(sup)) + cur (dfp_pafpn.py:168-170); two launches per level, one statistics group each,
-    like the reference's two jian calls."""
-    outs = []
-    for m, c, s in zip((net.jian2, net.jian1, net.jian0), cur, sup):
-        half = m.conv.out_channels
-        out = View.empty(c.n, c.h, c.w, 2 * half, T.device)
-        wpk = engine._packed(m)
-        conv_rec(T, (m,), c, wpk, 1, 1, out.ch(0, half), 0, res=c.ch(0, half))
-        conv_rec(T, (m,), s, wpk, 1, 1, out.ch(half, half), 0, res=c.ch(half, half))
-        outs.append(out)
-    return outs
-
-
-def _f32(p):
-    return p.detach().float().contiguous().view(p.shape[0], -1) if p.dim() > 1 else p.detach().float().contiguous()
-
-
-def head_rec(T, head, fused, labels):
-    dev = T.device
-    b = fused[0].n
-    hw = [(v.h, v.w) for v in fused]
-    head.hw = hw
-    a_total = sum(h * w for h, w in hw)
-    no = 5 + head.num_classes
-    out = torch.empty((b, a_total, no), dtype=torch.float32, device=dev)
-    origin = torch.empty((b, a_total, 4), dtype=torch.float32, device=dev)
-    off = 0
-    levels = []
-    for k, v in enumerate(fused):
-        x = base_conv_rec(T, head.stems[k], v, 0)
-        c0, r0 = head.cls_convs[k][0], head.reg_convs[k][0]          # same input: one launch (engine.conv_pair)
-        hw_c = c0.conv.out_channels
-        u = View.empty(x.n, x.h, x.w, 2 * hw_c, dev)
-        conv_rec(T, (c0, r0), x, engine._packed_pair(c0, r0), c0.ksize, c0.stride, u, 0)
-        cf = base_conv_rec(T, head.cls_convs[k][1], u.ch(0, hw_c), 0)
-        rf = base_conv_rec(T, head.reg_convs[k][1], u.ch(hw_c, hw_c), 0)
-        ops.head_pred_decode(cf, rf, _f32(head.reg_preds[k].weight), _f32(head.reg_preds[k].bias),
-                             _f32(head.obj_preds[k].weight), _f32(head.obj_preds[k].bias), _f32(head.cls_preds[k].weight),
-                             _f32(head.cls_preds[k].bias), head.strides[k], off, a_total, out, origin, sigmoid=False, decode=True)
-        levels.append((k, cf, rf, off))
-        off += v.h * v.w
-    fut = labels[0][..., :5].to(dev, torch.float32).contiguous()
-    cur = labels[1][..., :5].to(dev, torch.float32).contiguous()
-    wsb = ops.tal_loss_workspace_bytes(b, a_total, fut.shape[1], head.num_classes)
-    ws = torch.empty((wsb + 255) // 256 * 256, dtype=torch.uint8, device=dev)
-    loss = torch.empty(6, dtype=torch.float32, device=dev)
-    ops.tal_loss(out, origin, fut, cur, hw, head.strides, float(head.gamma), float(head.ignore_thr), float(head.ignore_value),
-                 True, ws, loss)
-    T.rec(t="head", levels=levels, out=out, origin=origin, fut=fut, ws=ws, hw=hw, a_total=a_total)
-    return loss
-
-
 # ------------------------------------------------------------------------------------------------ reverse walk
 def _conv_backward(T: Tape, r, sink):
     mods, x, raw, y, res = r["mods"], r["x"], r["raw"], r["y"], r["res"]
@@ -473,7 +312,8 @@ def _conv_backward(T: Tape, r, sink):
         src = View.empty(x.n, x.h, x.w, cout, dev)
         ops.dilate2(draw, src)
     # data gradient: gx = conv(src, flipped / transposed filter) * 1 + 0 (+ gx: accumulated in place through the residual input)
-    ops.conv2d(src, engine._packed_dgrad(mods), gx, (kh, kw), 1, ops.SY_CONV_FUSED, scale=one, shift=zero, act=0,
+    wpk = engine.packed_operand(mods[0], "_pkd", [m.conv.weight for m in mods], ops.pack_conv_weight_dgrad)
+    ops.conv2d(src, wpk, gx, (kh, kw), 1, ops.SY_CONV_FUSED, scale=one, shift=zero, act=0,
                res=shortcut if shortcut is not None else (None if fresh else gx))
     if DEBUG_HOOK is not None:
         DEBUG_HOOK("post", r, draw=draw, dgamma=dgamma, dbeta=dbeta, dw=dw, gx=gx)
@@ -541,16 +381,18 @@ def _record(model, x, targets):
     assert model.training and model.head.use_l1
     if any(getattr(m, "groups", 1) > 1 for m in model.modules() if isinstance(m, torch.nn.Conv2d)):
         raise NotImplementedError("the training backward does not cover depthwise convolutions (depthwise=True): forward only")
-    net, head = model.backbone, model.head
+    net = model.backbone
     xin = x.float().contiguous()
     b = xin.shape[0]
-    T = Tape(xin.device)
-    with torch.no_grad(), engine.forward_scope(xin.device):
-        pans = pafpn_rec(T, net, xin, 2, b)
+    dev = xin.device
+    T = Tape(dev)
+    with torch.no_grad(), engine.forward_scope(dev):
+        pans = engine.pafpn_frames(engine.Ctx(True, 2 * b, b, dev, T), net, xin, 2)
         cur = tuple(p.imgs(0, b) for p in pans)
         sup = tuple(p.imgs(b, b) for p in pans)
-        fused = dfp_rec(T, net, cur, sup)
-        loss = head_rec(T, head, fused, targets)
+        ctx = engine.Ctx(True, b, b, dev, T)
+        fused = engine.dfp_fuse(ctx, net, cur, sup)
+        loss = model.head.run(ctx, fused, targets)
     return T, loss
 
 

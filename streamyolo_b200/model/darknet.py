@@ -30,14 +30,7 @@ class CSPDarknet(nn.Module):
         """Standalone use: NCHW 3-channel float input -> {name: NCHW tensor}."""
         x = x.float().contiguous()
         ctx = engine.Ctx(self.training, x.shape[0], x.shape[0], x.device)
-        with torch.no_grad():
-            t = engine.focus_stem(ctx, self.stem, x, 1)
-            outs = {"stem": t}
-            for name in ("dark2", "dark3", "dark4"):
-                blk = getattr(self, name)
-                t = engine.csp_layer(ctx, blk[1], engine.base_conv(ctx, blk[0], t))
-                outs[name] = t
-            t = engine.base_conv(ctx, self.dark5[0], t)
-            t = engine.spp_bottleneck(ctx, self.dark5[1], t)
-            outs["dark5"] = engine.csp_layer(ctx, self.dark5[2], t)
-        return {k: engine.as_nchw(v) for k, v in outs.items() if k in self.out_features}
+        with torch.no_grad(), engine.forward_scope(x.device):
+            outs = engine.darknet(ctx, self, x, 1)
+        names = ("stem", "dark2", "dark3", "dark4", "dark5")
+        return {k: engine.as_nchw(v) for k, v in zip(names, outs) if k in self.out_features}

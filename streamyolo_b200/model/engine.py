@@ -10,6 +10,9 @@ including the order of the two running-statistic updates.
 
 Eval mode: BatchNorm is folded into a per-channel scale/shift applied in the conv epilogue
 together with SiLU and the residual (what yolox ``fuse_model`` + ``fuseforward`` achieve).
+
+The recording forward of a training step (model/backward.py) is this same walk with a tape in the ``Ctx``: nothing is
+updated in place, every op keeps what its backward needs and is recorded on the tape.
 """
 import os
 
@@ -39,45 +42,36 @@ def _trace(m, y):
 
 
 class Ctx:
-    """Per-forward execution context."""
+    """Per-forward execution context.  ``tape`` (a ``backward.Tape``): the recording forward of a training step -- every op
+    keeps what its backward needs and is recorded on the tape; None: the plain forward."""
 
-    def __init__(self, train, n, split, device):
+    def __init__(self, train, n, split, device, tape=None):
         self.train = train
         self.n = n              # images in the batched tensor
         self.split = split      # first image of statistics group 1 (== n: single group)
         self.groups = 2 if split < n else 1
         self.device = device
-        self.impl = os.environ.get("SY_CONV_IMPL", "tc")
+        self.tape = tape
+        self.impl = "tc" if tape is not None else os.environ.get("SY_CONV_IMPL", "tc")
+
+    def rec(self, **kw):
+        if self.tape is not None:
+            self.tape.rec(**kw)
 
 
-def _packed(m):
-    w = m.conv.weight
-    key = (w._version, w.data_ptr(), w.device, WEIGHT_EPOCH)
-    if getattr(m, "_pk_key", None) != key:
-        m._pk = ops.pack_conv_weight(w)
-        m._pk_key = key
-    return m._pk
-
-
-def _packed_dw(m):
-    """depthwise BaseConv: bf16 [k*k][C]"""
-    w = m.conv.weight
-    key = (w._version, w.data_ptr(), w.device, WEIGHT_EPOCH)
-    if getattr(m, "_pk_key", None) != key:
-        m._pk = ops.pack_dw_weight(w)
-        m._pk_key = key
-    return m._pk
-
-
-def _packed_dgrad(mods):
-    """Data-gradient operand (flipped taps, transposed channels) of one BaseConv or of a conv1 | conv2 pair."""
-    ws = [m.conv.weight for m in mods]
-    key = tuple((w._version, w.data_ptr()) for w in ws) + (WEIGHT_EPOCH,)
-    m0 = mods[0]
-    if getattr(m0, "_pkd_key", None) != key:
-        m0._pkd = ops.pack_conv_weight_dgrad(*ws)
-        m0._pkd_key = key
-    return m0._pkd
+def packed_operand(m, slot, ws, pack, value=None):
+    """The conv operand held in attribute ``slot`` of module ``m`` ("_pk": its own forward operand, "_pk2": the conv1 | conv2
+    pair it leads, "_pkd": the data-gradient operand): ``pack(*ws)``, cached until one of the weights ``ws`` changes (torch
+    version counter, storage, device) or WEIGHT_EPOCH moves.  ``value``: install that buffer as the operand of the current
+    weights instead of packing (train.Trainer's batched re-pack)."""
+    key = tuple((w._version, w.data_ptr(), w.device) for w in ws) + (WEIGHT_EPOCH,)
+    if value is not None:
+        setattr(m, slot, value)
+        setattr(m, slot + "_key", key)
+    elif getattr(m, slot + "_key", None) != key:
+        setattr(m, slot, pack(*ws))
+        setattr(m, slot + "_key", key)
+    return getattr(m, slot)
 
 
 def _folded(m):
@@ -200,16 +194,20 @@ def _dbg_skip_apply(nbytes):
     return lo * 1e6 <= nbytes < hi * 1e6
 
 
-def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, act=1, y_goff1=0, res_goff1=0, impl=None):
+def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, act=1, y_goff1=0, res_goff1=0, impl=None,
+                kind="normal"):
     """Train mode: conv -> batch statistics -> BatchNorm (running-stat update) -> act (+res) into ``y``.
     Tensor-core path = 2 launches: the conv writes the raw bf16 result, accumulates the statistics and
     (grid barrier + parallel reduce in its tail) publishes scale/shift; then the normalise pass.  ``mods``: one BaseConv, or two whose
-    outputs are concatenated along channels (CSPLayer conv1 | conv2)."""
+    outputs are concatenated along channels (CSPLayer conv1 | conv2).  With a tape the raw output goes to a fresh buffer
+    and the conv also writes the batch mean / inverse std: the backward reads both.  ``kind="stem"``: the Focus stem, whose
+    input needs no gradient."""
     kh, kw = (k, k) if isinstance(k, int) else k
     ho = (x.h + 2 * ((kh - 1) // 2) - kh) // s + 1
     wo = (x.w + 2 * ((kw - 1) // 2) - kw) // s + 1
     cout = sum(m.conv.out_channels for m in mods)
-    raw = _raw_view(ctx, x.n, ho, wo, cout)
+    T = ctx.tape
+    raw = _raw_view(ctx, x.n, ho, wo, cout) if T is None else View.empty(x.n, ho, wo, cout, ctx.device)
     bn0 = mods[0].bn
     mom = float(0.1 if bn0.momentum is None else bn0.momentum)
     n = x.n
@@ -224,16 +222,21 @@ def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, a
             segs.append(_bn_seg(m, c0))
             c0 += m.conv.out_channels
         ss = torch.empty((2, 2, cout), dtype=torch.float32, device=ctx.device)
-        if FUSE_APPLY or n * ho * wo * cout * 2 <= FUSE_APPLY_MAX_BYTES:
+        mi = None if T is None else torch.empty((2, 2, cout), dtype=torch.float32, device=ctx.device)
+        if T is None and (FUSE_APPLY or n * ho * wo * cout * 2 <= FUSE_APPLY_MAX_BYTES):
             ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl="tc", partials=partials, split_n=split, bn=segs,
                        momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device), act=act,
                        apply_y=y, apply_res=res, y_goff1=y_goff1, res_goff1=res_goff1)
         else:
             ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl="tc", partials=partials, split_n=split, bn=segs,
-                       momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device))
-            if not _dbg_skip_apply(n * ho * wo * cout * 2):
+                       momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device), mean_invstd=mi)
+            if T is not None or not _dbg_skip_apply(n * ho * wo * cout * 2):
                 ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), split if split else n, act, res, y, y_goff1,
                                  res_goff1)
+        if T is not None:
+            T.rec(t="conv", mods=mods, x=x, k=(kh, kw), s=s, raw=raw, y=y, res=res, ss=ss, mi=mi, split=split, act=act,
+                  kind=kind)
+            T.uses[id(mods[0])] = T.uses.get(id(mods[0]), 0) + 1
         return
     # CUDA-core path (cross-check of the tensor-core kernel; depthwise convs): conv, separate statistics pass, separate
     # finalize per module, apply
@@ -275,7 +278,7 @@ def base_conv(ctx: Ctx, m, x: View, y: View = None, res: View = None) -> View:
     if y is None:
         y = View.empty(x.n, ho, wo, cout, ctx.device)
     dw = m.conv.groups > 1
-    wpk = _packed_dw(m) if dw else _packed(m)
+    wpk = packed_operand(m, "_pk", [m.conv.weight], ops.pack_dw_weight if dw else ops.pack_conv_weight)
     impl = "dw" if dw else ctx.impl
     act = 1 if m.act_name == "silu" else 0
     if not ctx.train:
@@ -285,16 +288,6 @@ def base_conv(ctx: Ctx, m, x: View, y: View = None, res: View = None) -> View:
         conv_bn_act(ctx, (m,), x, wpk, k, s, y, res, act, impl=impl)
     _trace(m, y)
     return y
-
-
-def _packed_pair(m1, m2):
-    """conv1 | conv2 of a CSPLayer as one [2*hidden][1][Cin] GEMM operand."""
-    w1, w2 = m1.conv.weight, m2.conv.weight
-    key = (w1._version, w2._version, w1.data_ptr(), w2.data_ptr(), w1.device, WEIGHT_EPOCH)
-    if getattr(m1, "_pk2_key", None) != key:
-        m1._pk2 = ops.pack_conv_weight(w1, w2)
-        m1._pk2_key = key
-    return m1._pk2
 
 
 def _folded_pair(m1, m2):
@@ -320,7 +313,7 @@ def conv_pair(ctx: Ctx, m1, m2, x: View) -> View:
     assert (m2.ksize, m2.stride, m2.conv.in_channels) == (k, s, m1.conv.in_channels)
     ho, wo = ops.conv_out_hw(x.h, x.w, k, s)
     u = View.empty(x.n, ho, wo, c1 + c2, ctx.device)
-    wpk = _packed_pair(m1, m2)
+    wpk = packed_operand(m1, "_pk2", [m1.conv.weight, m2.conv.weight], ops.pack_conv_weight)
     if not ctx.train:
         scale, shift = _folded_pair(m1, m2)
         ops.conv2d(x, wpk, u, k, s, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=1)
@@ -334,31 +327,33 @@ def conv_pair(ctx: Ctx, m1, m2, x: View) -> View:
 def csp_layer(ctx: Ctx, m, x: View, out: View = None) -> View:
     """[yolox] CSPLayer: conv3(cat(m(conv1 x), conv2 x)).  conv1 and conv2 read the same input, so they
     run as ONE GEMM with 2*hidden output channels written straight into the concat buffer; the
-    bottleneck chain then updates the first half in place.  No concat copy ever happens."""
+    bottleneck chain then updates the first half in place.  No concat copy ever happens -- except with a tape: the
+    backward needs every input kept, so the chain runs in fresh buffers, its last output lands in a second concat buffer
+    and conv2's half is copied next to it."""
     hid = m.conv1.conv.out_channels
-    u = View.empty(x.n, x.h, x.w, 2 * hid, ctx.device)
+    u = conv_pair(ctx, m.conv1, m.conv2, x)
     a = u.ch(0, hid)
-    wpk = _packed_pair(m.conv1, m.conv2)
-    if not ctx.train:
-        scale, shift = _folded_pair(m.conv1, m.conv2)
-        ops.conv2d(x, wpk, u, 1, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=1)
-    else:
-        conv_bn_act(ctx, (m.conv1, m.conv2), x, wpk, 1, 1, u)
-    _trace(m.conv1, a)
-    _trace(m.conv2, u.ch(hid, hid))
-    for blk in m.m:
+    keep = ctx.tape is not None
+    if keep:
+        u2 = View.empty(x.n, x.h, x.w, 2 * hid, ctx.device)
+    for i, blk in enumerate(m.m):
         t = base_conv(ctx, blk.conv1, a)
-        base_conv(ctx, blk.conv2, t, a, res=a if blk.use_add else None)
+        dst = a
+        if keep:
+            dst = u2.ch(0, hid) if i == len(m.m) - 1 else View.empty(x.n, x.h, x.w, hid, ctx.device)
+        base_conv(ctx, blk.conv2, t, dst, res=a if blk.use_add else None)
+        a = dst
+    if keep:
+        if len(m.m) == 0:
+            copy(ctx, a, u2.ch(0, hid))
+        copy(ctx, u.ch(hid, hid), u2.ch(hid, hid))
+        u = u2
     return base_conv(ctx, m.conv3, u, out)
 
 
-def _packed_stem(bc):
-    w = bc.conv.weight
-    key = (w._version, w.data_ptr(), w.device, WEIGHT_EPOCH)
-    if getattr(bc, "_pk_key", None) != key:
-        bc._pk = ops.pack_stem_weight(w)
-        bc._pk_key = key
-    return bc._pk
+def copy(ctx: Ctx, src: View, dst: View):
+    ops.copy(src, dst)
+    ctx.rec(t="copy", src=src, dst=dst)
 
 
 def focus_stem(ctx: Ctx, m, x, frames) -> View:
@@ -370,13 +365,13 @@ def focus_stem(ctx: Ctx, m, x, frames) -> View:
     n = frames * b
     xin = View.empty(n, h // 2, w // 2, 64, ctx.device)
     ops.focus_pack(x, frames, xin)
-    wpk = _packed_stem(bc)
+    wpk = packed_operand(bc, "_pk", [bc.conv.weight], ops.pack_stem_weight)
     y = View.empty(n, h // 2, w // 2, cout, ctx.device)
     if not ctx.train:
         scale, shift = _folded(bc)
         ops.conv2d(xin, wpk, y, ops.STEM_K, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=1)
     else:
-        conv_bn_act(ctx, (bc,), xin, wpk, ops.STEM_K, 1, y)
+        conv_bn_act(ctx, (bc,), xin, wpk, ops.STEM_K, 1, y, kind="stem")
     _trace(bc, y)
     return y
 
@@ -386,38 +381,50 @@ def spp_bottleneck(ctx: Ctx, m, x: View) -> View:
     s = View.empty(x.n, x.h, x.w, 4 * hid, ctx.device)
     base_conv(ctx, m.conv1, x, s.ch(0, hid))
     ops.spp_maxpool(s.ch(0, hid), s.ch(hid, hid), s.ch(2 * hid, hid), s.ch(3 * hid, hid))
+    ctx.rec(t="spp", x=s.ch(0, hid), y5=s.ch(hid, hid), y9=s.ch(2 * hid, hid), y13=s.ch(3 * hid, hid))
     return base_conv(ctx, m.conv2, s)
+
+
+def upsample(ctx: Ctx, x: View, y: View):
+    ops.upsample_nearest(x, y)
+    ctx.rec(t="upsample", x=x, y=y)
+
+
+def darknet(ctx: Ctx, bb, x, frames, dark3: View = None, dark4: View = None):
+    """CSPDarknet stem -> dark5 for ``frames`` x B images (/root/reference/exps/model/darknet.py:167-179).  ``dark3`` /
+    ``dark4``: where the dark3 / dark4 outputs go (e.g. slices of the PAFPN's concat buffers).  Returns the (stem, dark2,
+    dark3, dark4, dark5) views."""
+    outs = [focus_stem(ctx, bb.stem, x, frames)]
+    for blk, dst in ((bb.dark2, None), (bb.dark3, dark3), (bb.dark4, dark4)):
+        outs.append(csp_layer(ctx, blk[1], base_conv(ctx, blk[0], outs[-1]), dst))
+    t = base_conv(ctx, bb.dark5[0], outs[-1])
+    t = spp_bottleneck(ctx, bb.dark5[1], t)
+    outs.append(csp_layer(ctx, bb.dark5[2], t))
+    return outs
 
 
 def pafpn_frames(ctx: Ctx, net, x, frames):
     """CSPDarknet + PAFPN for ``frames`` x B images (/root/reference/exps/model/darknet.py:167-179,
     dfp_pafpn.py:120-140).  Returns the un-fused (pan_out2, pan_out1, pan_out0) views."""
-    bb = net.backbone
     dev = ctx.device
     c3 = net.C3_p3.conv3.conv.out_channels
     c4 = net.C3_p4.conv3.conv.out_channels
-    t = focus_stem(ctx, bb.stem, x, frames)
-    t = base_conv(ctx, bb.dark2[0], t)
-    t = csp_layer(ctx, bb.dark2[1], t)
-    t = base_conv(ctx, bb.dark3[0], t)
-    n, h8, w8 = t.n, t.h, t.w
+    n = frames * x.shape[0]
+    h8, w8 = x.shape[2] // 2, x.shape[3] // 2                       # Focus, then the 3x3 stride-2 convs of dark2, dark3
+    for _ in range(2):
+        h8, w8 = ops.conv_out_hw(h8, w8, 3, 2)
+    h16, w16 = ops.conv_out_hw(h8, w8, 3, 2)
     f1 = View.empty(n, h8, w8, 2 * c3, dev)              # cat(up(fpn_out1), dark3)
-    x2 = csp_layer(ctx, bb.dark3[1], t, f1.ch(c3, c3))
-    t = base_conv(ctx, bb.dark4[0], x2)
-    h16, w16 = t.h, t.w
     f0 = View.empty(n, h16, w16, 2 * c4, dev)            # cat(up(fpn_out0), dark4)
-    x1 = csp_layer(ctx, bb.dark4[1], t, f0.ch(c4, c4))
-    t = base_conv(ctx, bb.dark5[0], x1)
-    h32, w32 = t.h, t.w
-    t = spp_bottleneck(ctx, bb.dark5[1], t)
-    x0 = csp_layer(ctx, bb.dark5[2], t)
+    x0 = darknet(ctx, net.backbone, x, frames, f1.ch(c3, c3), f0.ch(c4, c4))[-1]
+    h32, w32 = x0.h, x0.w
     z0 = View.empty(n, h32, w32, 2 * c4, dev)            # cat(bu_conv1, fpn_out0)
     fpn0 = base_conv(ctx, net.lateral_conv0, x0, z0.ch(c4, c4))
-    ops.upsample_nearest(fpn0, f0.ch(0, c4))
+    upsample(ctx, fpn0, f0.ch(0, c4))
     fo0 = csp_layer(ctx, net.C3_p4, f0)
     z1 = View.empty(n, h16, w16, 2 * c3, dev)            # cat(bu_conv2, fpn_out1)
     fpn1 = base_conv(ctx, net.reduce_conv1, fo0, z1.ch(c3, c3))
-    ops.upsample_nearest(fpn1, f1.ch(0, c3))
+    upsample(ctx, fpn1, f1.ch(0, c3))
     pan2 = csp_layer(ctx, net.C3_p3, f1)
     base_conv(ctx, net.bu_conv2, pan2, z1.ch(0, c3))
     pan1 = csp_layer(ctx, net.C3_n3, z1)
@@ -436,14 +443,14 @@ def dfp_fuse(ctx: Ctx, net, cur, sup):
         if hasattr(m, "dconv"):                               # depthwise=True: jian is a DWConv (dfp_pafpn.py:83-105)
             half = m.pconv.conv.out_channels
             out = View.empty(nb, c.h, c.w, 2 * half, ctx.device)
-            sub = Ctx(ctx.train, nb, nb, ctx.device)          # two calls = two BatchNorm batches, like the reference
+            sub = Ctx(ctx.train, nb, nb, ctx.device, ctx.tape)    # two calls = two BatchNorm batches, like the reference
             base_conv(sub, m, c, out.ch(0, half), res=c.ch(0, half))
             base_conv(sub, m, s, out.ch(half, half), res=c.ch(half, half))
             outs.append(out)
             continue
         half = m.conv.out_channels
         out = View.empty(nb, c.h, c.w, 2 * half, ctx.device)
-        wpk = _packed(m)
+        wpk = packed_operand(m, "_pk", [m.conv.weight], ops.pack_conv_weight)
         if not ctx.train:
             scale, shift = _folded(m)
             ops.conv2d(c, wpk, out.ch(0, half), 1, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift,
@@ -452,9 +459,10 @@ def dfp_fuse(ctx: Ctx, net, cur, sup):
                        shift=shift, act=1, res=c.ch(half, half))
         else:
             # the reference runs jian(cur) then jian(sup): two BN batches, two running-stat updates.
-            # Batched here (grouped statistics) when cur/sup are the two halves of one buffer.
+            # Batched here (grouped statistics) when cur/sup are the two halves of one buffer -- not with a tape: the
+            # backward takes one statistics group per launch.
             same = (c.buf is s.buf) and s.n0 == c.n0 + nb and c.c0 == s.c0 and c.c == s.c
-            if same:
+            if same and ctx.tape is None:
                 both = View(c.buf, c.c0, c.c, c.n0, 2 * nb)
                 sub = Ctx(True, 2 * nb, nb, ctx.device)
                 # group 1 (support frames, images nb..2nb-1) lands in channels [half, 2*half) of image n - nb
@@ -463,7 +471,7 @@ def dfp_fuse(ctx: Ctx, net, cur, sup):
                 conv_bn_act(sub, (m,), both, wpk, 1, 1, yv, rv, 1,
                             y_goff1=half - nb * yv.img_elems(), res_goff1=half - nb * rv.img_elems())
             else:
-                sub = Ctx(True, nb, nb, ctx.device)
+                sub = Ctx(True, nb, nb, ctx.device, ctx.tape)
                 for src, dst, r in ((c, out.ch(0, half), c.ch(0, half)), (s, out.ch(half, half), c.ch(half, half))):
                     conv_bn_act(sub, (m,), src, wpk, 1, 1, dst, r, 1)
         outs.append(out)

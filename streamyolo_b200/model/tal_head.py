@@ -52,39 +52,49 @@ class TALHead(nn.Module):
             conv.bias = torch.nn.Parameter(b.view(-1), requires_grad=True)
 
     # ------------------------------------------------------------------
-    def _f32(self, p):
-        return p.detach().float().contiguous().view(p.shape[0], -1) if p.dim() > 1 else p.detach().float().contiguous()
-
     def forward(self, xin, labels=None, imgs=None):
         views = [engine.as_view(x) for x in xin]
         dev = views[0].buf.device
         b = views[0].n
         ctx = engine.Ctx(self.training, b, b, dev)
+        with torch.no_grad(), engine.forward_scope(dev):
+            r = self.run(ctx, views, labels)
+        return tuple(r) if self.training else r
+
+    def run(self, ctx, views, labels=None):
+        """The head on the per-level views: eval -> the [B, A, 5+ncls] outputs; train -> the loss vector [total, iou, conf,
+        cls, l1, num_fg].  With a tape (the recording forward) the prediction / decode / loss launches are recorded as
+        one ``head`` op."""
+        dev = ctx.device
+        b = views[0].n
+        train = ctx.train
         self.hw = [(v.h, v.w) for v in views]
         a_total = sum(h * w for h, w in self.hw)
         no = 5 + self.num_classes
-        train = self.training
-        with torch.no_grad(), engine.forward_scope(dev):
-            out = torch.empty((b, a_total, no), dtype=torch.float32, device=dev)
-            origin = torch.empty((b, a_total, 4), dtype=torch.float32, device=dev) if (train and self.use_l1) else None
-            off = 0
-            for k, v in enumerate(views):
-                x = engine.base_conv(ctx, self.stems[k], v)
-                # cls_convs[k][0] and reg_convs[k][0] read the same stem output (tal_head.py:159-171): ONE conv launch with
-                # 2 x hw output channels and two BatchNorm segments, like the conv1 | conv2 pair of a CSPLayer
-                u = engine.conv_pair(ctx, self.cls_convs[k][0], self.reg_convs[k][0], x)
-                hw_c = u.c // 2
-                cf = engine.base_conv(ctx, self.cls_convs[k][1], u.ch(0, hw_c))
-                rf = engine.base_conv(ctx, self.reg_convs[k][1], u.ch(hw_c, hw_c))
-                ops.head_pred_decode(cf, rf, self._f32(self.reg_preds[k].weight), self._f32(self.reg_preds[k].bias),
-                                     self._f32(self.obj_preds[k].weight), self._f32(self.obj_preds[k].bias),
-                                     self._f32(self.cls_preds[k].weight), self._f32(self.cls_preds[k].bias),
-                                     self.strides[k], off, a_total, out, origin,
-                                     sigmoid=not train, decode=train or self.decode_in_inference)
-                off += v.h * v.w
-            if not train:
-                return out
-            return self.get_losses(out, origin, labels)
+        out = torch.empty((b, a_total, no), dtype=torch.float32, device=dev)
+        origin = torch.empty((b, a_total, 4), dtype=torch.float32, device=dev) if (train and self.use_l1) else None
+        off = 0
+        levels = []
+        for k, v in enumerate(views):
+            x = engine.base_conv(ctx, self.stems[k], v)
+            # cls_convs[k][0] and reg_convs[k][0] read the same stem output (tal_head.py:159-171): ONE conv launch with
+            # 2 x hw output channels and two BatchNorm segments, like the conv1 | conv2 pair of a CSPLayer
+            u = engine.conv_pair(ctx, self.cls_convs[k][0], self.reg_convs[k][0], x)
+            hw_c = u.c // 2
+            cf = engine.base_conv(ctx, self.cls_convs[k][1], u.ch(0, hw_c))
+            rf = engine.base_conv(ctx, self.reg_convs[k][1], u.ch(hw_c, hw_c))
+            ops.head_pred_decode(cf, rf, _f32(self.reg_preds[k].weight), _f32(self.reg_preds[k].bias),
+                                 _f32(self.obj_preds[k].weight), _f32(self.obj_preds[k].bias),
+                                 _f32(self.cls_preds[k].weight), _f32(self.cls_preds[k].bias),
+                                 self.strides[k], off, a_total, out, origin,
+                                 sigmoid=not train, decode=train or self.decode_in_inference)
+            levels.append((k, cf, rf, off))
+            off += v.h * v.w
+        if not train:
+            return out
+        loss, fut, ws = self._loss(out, origin, labels)
+        ctx.rec(t="head", levels=levels, out=out, origin=origin, fut=fut, ws=ws, hw=self.hw, a_total=a_total)
+        return loss
 
     def decode_outputs(self, outputs, dtype=None):
         """Decode raw [B, A, 5+ncls] outputs (tools/eval.py:188 path when decode_in_inference is False)."""
@@ -98,7 +108,8 @@ class TALHead(nn.Module):
         outputs[..., 2:4] = torch.exp(outputs[..., 2:4]) * gs[:, None]
         return outputs
 
-    def get_losses(self, outputs, origin, labels):
+    def _loss(self, outputs, origin, labels):
+        """-> (loss vector, future labels, workspace): the last two are what the loss backward reads"""
         if not self.use_l1:
             # the reference dereferences origin_preds unconditionally (tal_head.py:435) and raises; every
             # shipped schedule sets use_l1 = True (double_trainer.py:209-216)
@@ -119,4 +130,9 @@ class TALHead(nn.Module):
                      float(self.ignore_value), self.use_l1, ws, loss, **dumps)
         if self.keep_assignment:
             self.last_assignment = dict(dumps, outputs=outputs, origin=origin)
-        return loss[0], loss[1], loss[2], loss[3], loss[4], loss[5]
+        return loss, fut, ws
+
+
+def _f32(p):
+    """fp32 operand of a prediction conv: weight [O][C], bias [O]"""
+    return p.detach().float().contiguous().view(p.shape[0], -1) if p.dim() > 1 else p.detach().float().contiguous()

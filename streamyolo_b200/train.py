@@ -82,8 +82,9 @@ def train_step(model, optimizer, x, targets, ema=None, grad_scale=1.0):
 
 # ------------------------------------------------------------------------------------------------ flat state
 def conv_groups_forward_order(model):
-    """The BaseConv launch groups of one training forward in launch order (model/backward.py: pafpn_rec, dfp_rec,
-    head_rec): a CSPLayer's conv1 | conv2 run as one GEMM, everything else alone."""
+    """The BaseConv launch groups of one training forward in launch order (the recording forward: model/engine.py
+    pafpn_frames, dfp_fuse and TALHead.run with a tape): a CSPLayer's conv1 | conv2 and the first cls | reg tower convs of
+    a head level run as one GEMM, everything else alone."""
     net, head = model.backbone, model.head
     bb = net.backbone
     out = []
@@ -349,18 +350,13 @@ class Trainer:
     def _repack(self):
         """run the batched pack and hand the buffers to the engine's operand caches (keys of the current WEIGHT_EPOCH)"""
         self.pack.run()
-        ep = engine.WEIGHT_EPOCH
         for g, fwd, dg in self._packed_groups:
             ws = [m.conv.weight for m in g]
-            if dg is None:                                  # stem
-                g[0]._pk, g[0]._pk_key = fwd, (ws[0]._version, ws[0].data_ptr(), ws[0].device, ep)
+            if dg is None:
+                engine.packed_operand(g[0], "_pk", ws, ops.pack_stem_weight, value=fwd)
                 continue
-            if len(g) == 1:
-                g[0]._pk, g[0]._pk_key = fwd, (ws[0]._version, ws[0].data_ptr(), ws[0].device, ep)
-            else:
-                g[0]._pk2 = fwd
-                g[0]._pk2_key = (ws[0]._version, ws[1]._version, ws[0].data_ptr(), ws[1].data_ptr(), ws[0].device, ep)
-            g[0]._pkd, g[0]._pkd_key = dg, tuple((w._version, w.data_ptr()) for w in ws) + (ep,)
+            engine.packed_operand(g[0], "_pk" if len(g) == 1 else "_pk2", ws, ops.pack_conv_weight, value=fwd)
+            engine.packed_operand(g[0], "_pkd", ws, ops.pack_conv_weight_dgrad, value=dg)
 
     def forward_backward(self, x, targets, loss_scale=1.0):
         T, loss = backward._record(self.model, x, targets)

@@ -14,7 +14,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import emul_ops  # noqa: E402
 import test_cpu_backward as T  # noqa: E402
 from oracle.make_golden import CASES  # noqa: E402
-from streamyolo_b200 import synth, train  # noqa: E402
+from streamyolo_b200 import ops, synth, train  # noqa: E402
+from streamyolo_b200.model import backward, engine  # noqa: E402
 
 
 def test_flat_state_keeps_the_module_surface(monkeypatch):
@@ -48,6 +49,28 @@ def test_flat_state_keeps_the_module_surface(monkeypatch):
     assert sorted(ids) == sorted(id(p) for p in model.parameters())
 
 
+@pytest.mark.parametrize("name", ["tiny_120x160", "l_depth_64x96"])
+def test_launch_plan_matches_recording_forward(name, monkeypatch):
+    """train.conv_groups_forward_order -- the list FlatState's layout, the gradient buckets and the batched re-pack are built
+    from -- is the conv launch groups of the recording forward in order of first launch; every group runs once except the
+    DFP jian convs (jian(cur) and jian(sup): two launches)."""
+    emul_ops.install(monkeypatch, exact=True)
+    c = CASES[name] if name in CASES else T.DEPTH_CASES[name]
+    model = T.build_product(c)
+    x = synth.synth_frames(c["B"], c["H"], c["W"])
+    tape, _ = backward._record(model, x, synth.synth_labels(c["B"], c["H"], c["W"]))
+    seen, recorded = set(), []
+    for r in tape.ops:
+        if r["t"] == "conv" and id(r["mods"][0]) not in seen:
+            seen.add(id(r["mods"][0]))
+            recorded.append(tuple(map(id, r["mods"])))
+    plan = train.conv_groups_forward_order(model)
+    assert recorded == [tuple(map(id, g)) for g in plan]
+    net = model.backbone
+    jian = {id(net.jian2), id(net.jian1), id(net.jian0)}
+    assert {id(g[0]): tape.uses[id(g[0])] for g in plan} == {id(g[0]): 2 if id(g[0]) in jian else 1 for g in plan}
+
+
 def test_trainer_step_matches_stock_pytorch_step(monkeypatch):
     """Three steps of train.Trainer (flat state + fused kernel emulation) == three steps of train.train_step (torch SGD
     nesterov with weight-decay groups + Python ModelEMA): losses, every parameter, the EMA copy and the BatchNorm buffers."""
@@ -67,6 +90,8 @@ def test_trainer_step_matches_stock_pytorch_step(monkeypatch):
         got = tr.step(x, tg)
         d3 = model.backbone.backbone.dark3[0]
         assert any(g[0] is d3 and d3._pk is fwd for g, fwd, _ in tr._packed_groups)      # the batched re-pack feeds the forward
+        # ... under the key the forward looks it up with (a lookup with any other key would re-pack)
+        assert engine.packed_operand(d3, "_pk", [d3.conv.weight], ops.pack_conv_weight) is d3._pk
         assert abs(float(got["total_loss"]) - float(want["total_loss"])) <= 1e-5 * abs(float(want["total_loss"])), i
     assert tr.sink.launched and sum(b - a for a, b in tr.sink.launched) == tr.fs.n_param      # every gradient in one bucket
     for (k, p), q in zip(model.named_parameters(), ref.parameters()):

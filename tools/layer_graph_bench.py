@@ -30,12 +30,12 @@ calls = []
 orig = engine.conv_bn_act
 
 
-def spy(ctx, mods, xv, wpk, k, s, y, res=None, act=1, y_goff1=0, res_goff1=0, impl=None):
-    kh, kw = (k, k) if isinstance(k, int) else k
+def spy(ctx, mods, xv, wpk, k, s, y, res=None, act=1, y_goff1=0, res_goff1=0, **kw):
+    kh, kw_ = (k, k) if isinstance(k, int) else k
     calls.append(dict(name="|".join(getattr(m, "_sy_name", "?") for m in mods), n=xv.n, h=xv.h, w=xv.w, cin=xv.c,
-                      cout=sum(m.conv.out_channels for m in mods), k=(kh, kw), s=s, res=res is not None, split=ctx.split if ctx.groups == 2 else 0,
+                      cout=sum(m.conv.out_channels for m in mods), k=(kh, kw_), s=s, res=res is not None, split=ctx.split if ctx.groups == 2 else 0,
                       mods=mods, wpk=wpk, goff=y_goff1 != 0))
-    return orig(ctx, mods, xv, wpk, k, s, y, res, act, y_goff1, res_goff1, impl)
+    return orig(ctx, mods, xv, wpk, k, s, y, res, act, y_goff1, res_goff1, **kw)
 
 
 engine.conv_bn_act = spy
