@@ -104,7 +104,7 @@ typedef struct {
   /* ---- debugging only: CTA 0 records (event, clock64) int64 pairs of its three pipeline roles ---- */
   void* debug_timeline;  /* device buffer of 2*debug_timeline_events int64, or NULL */
   int32_t debug_timeline_events;
-  int32_t debug_flags;   /* 0 in production; 1 = skip MMAs, 2 = skip TMA loads (pipeline dissection, results invalid) */
+  int32_t debug_flags;   /* 0 in production; 2 = skip TMA loads (pipeline dissection, results invalid) */
   /* ---- validation only: the fp32 accumulators themselves, before the bf16 rounding of the stored result:
    * debug_f32[pixel][Cout] (pixel = flattened (n, oh, ow)), written next to the normal output.  This is where
    * north_star's "within 1e-3 of the reference" is literal (tests/test_gpu_ops.py::test_conv_fp32_accumulators). ---- */

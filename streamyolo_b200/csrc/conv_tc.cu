@@ -55,6 +55,10 @@ constexpr int kEpiThreads = 256;    // MMA + convert warps 0-7
 constexpr int kTailThreads = 512;   // convert + statistics warps run the kernel tail (partials, grid barrier, finalize, apply)
 constexpr int kABytes = kBlockM * 128;   // 16 KiB per stage
 constexpr int kMaxStages = 8;
+// Linear / patch tiles: a ring of four A+B stages (four 64-deep K blocks in flight), not as many as shared memory holds.
+// bench.py's forward+loss step on an H100 80GB HBM3 at 700 W, ring depth capped at 3 / 4 / 5 / none (= 6 stages at
+// BN = 128): 405 / 416 / 404 / 387 pairs/s.  Why deeper rings are slower has not been isolated; four is the measured optimum.
+constexpr int kRingStages = 4;
 // 64-deep K sub-blocks per pipeline stage: two (one barrier round per K = 128) halve the per-round hand-shake cost
 
 struct BnSeg {
@@ -458,8 +462,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         for (int cb = 0; cb < p.cblocks; ++cb) {
           mbar_wait(emptyA_bar(sa), pha ^ 1u);
           if (elect_one()) {
-            mbar_expect_tx(fullA_bar(sa), (uint32_t)p.halo_tx);
-            tma_load_4d(smem_u32(sA + sa * p.halo_bytes), &tmA, fullA_bar(sa), cb * kBlockK, px * p.tw - 1, py * p.th - 1, img);
+            if (p.debug_flags & 2) {
+              mbar_arrive(fullA_bar(sa));
+            } else {
+              mbar_expect_tx(fullA_bar(sa), (uint32_t)p.halo_tx);
+              tma_load_4d(smem_u32(sA + sa * p.halo_bytes), &tmA, fullA_bar(sa), cb * kBlockK, px * p.tw - 1, py * p.th - 1, img);
+            }
           }
           __syncwarp();
           if (++sa == p.stagesA) { sa = 0; pha ^= 1u; }
@@ -475,10 +483,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int t0 = 0; t0 < 9; t0 += kSub) {
             mbar_wait(empty_bar(sb), phb ^ 1u);
             if (elect_one()) {
-              mbar_expect_tx(full_bar(sb), (uint32_t)(kSub * kBB));
+              if (p.debug_flags & 2) {
+                mbar_arrive(full_bar(sb));
+              } else {
+                mbar_expect_tx(full_bar(sb), (uint32_t)(kSub * kBB));
 #pragma unroll
-              for (int j = 0; j < kSub; ++j)
-                tma_load_3d(smem_u32(sB + (sb * kSub + j) * kBB), &tmB, full_bar(sb), cb * kBlockK, t0 + j, n_tile * BN);
+                for (int j = 0; j < kSub; ++j)
+                  tma_load_3d(smem_u32(sB + (sb * kSub + j) * kBB), &tmB, full_bar(sb), cb * kBlockK, t0 + j, n_tile * BN);
+              }
             }
             __syncwarp();
             if (++sb == S) { sb = 0; phb ^= 1u; }
@@ -1023,9 +1035,9 @@ static int make_plan(Params& p, Plan* out) {
     smem = fixed_bytes + acc_bytes + p.stagesA * p.halo_bytes + stages * taps * bbytes;
   } else {
     const int stage_bytes = Cfg<BN>::kSub * (kABytes + bbytes);
-    int stages = (kSmemLimit - fixed_bytes - acc_bytes) / stage_bytes;
-    if (stages > kMaxStages) stages = kMaxStages;
-    if ((p.debug_flags >> 8) & 15) stages = min(stages, (p.debug_flags >> 8) & 15);   // debug: cap the ring depth
+    const int fit = min(kMaxStages, (kSmemLimit - fixed_bytes - acc_bytes) / stage_bytes);
+    int stages = min(fit, kRingStages);
+    if ((p.debug_flags >> 8) & 15) stages = min(fit, (p.debug_flags >> 8) & 15);     // debug: set the ring depth
     SY_REQUIRE(stages >= 2, SY_EINVAL, "conv2d_tc: Cout=%d leaves no room for the operand ring", p.Cout);
     p.stages = stages;
     smem = fixed_bytes + acc_bytes + stages * stage_bytes;

@@ -1,5 +1,8 @@
 """Dissect the conv pipeline: time a shape (CUDA graph of 20 back-to-back launches, so host launch cost is
-excluded) with the MMAs and/or the TMA loads switched off.   usage: python tools/conv_dissect.py"""
+excluded) as it runs and with the TMA loads switched off (debug flag 2: the barriers still cycle, the MMAs read stale
+shared memory).  The gap between the two is what operand supply costs the shape.  The plan column is the A mode
+(0 patch, 1 linear, 2 halo) and the tile width.
+    usage: python tools/conv_dissect.py"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -36,14 +39,16 @@ if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "stages":
     for shape in [(16, 128, 128, 75, 120, 3, 1), (8, 256, 256, 75, 120, 3, 1), (16, 64, 64, 150, 240, 3, 1)]:
         row = []
         for st in (2, 3, 4, 6, 8):
-            row.append((st, run(*shape, (st << 8)), run(*shape, 3 | (st << 8))))
-        print(shape, " ".join(f"S={a}: full {b:.1f} skel {c:.1f} |" for a, b, c in row))
+            row.append((st, run(*shape, (st << 8)), run(*shape, 2 | (st << 8))))
+        print(shape, " ".join(f"S={a}: full {b:.1f} no-TMA {c:.1f} |" for a, b, c in row))
     sys.exit(0)
 if __name__ == "__main__":
     for shape in SHAPES:
-        t = [run(*shape, f) for f in (0, 1, 2, 3)]
+        t = [run(*shape, f) for f in (0, 2)]
         n, ci, co, h, w, k, s = shape
         ho, wo = ops.conv_out_hw(h, w, k, s)
+        pl = ops.conv2d_plan(n, h, w, ci, co, k, s)
         fl = 2.0 * n * ho * wo * co * ci * k * k
         by = 2.0 * n * (h * w * ci + ho * wo * co)
-        print(f"{str(shape):38s} full {t[0]:6.1f} us {fl / t[0] / 1e6:7.0f} TF/s {by / t[0] / 1e3:6.0f} GB/s | no-MMA {t[1]:6.1f} | no-TMA {t[2]:6.1f} | neither {t[3]:6.1f}")
+        print(f"{str(shape):38s} A{pl['mode']} BN{pl['bn']:<4d} full {t[0]:6.1f} us {fl / t[0] / 1e6:7.0f} TF/s {by / t[0] / 1e3:6.0f} GB/s"
+              f" | no-TMA {t[1]:6.1f} us | supply {t[0] - t[1]:6.1f} us ({(t[0] - t[1]) / t[0] * 100:3.0f} %)", flush=True)
