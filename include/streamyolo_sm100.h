@@ -121,9 +121,10 @@ int sy_conv_stat_rows(void);
  * run two such launches concurrently on one GPU (the barrier needs every SM). */
 int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream);
 /* Host-only query (no launch, no GPU needed): the tiling sy_conv2d_tc chooses for a layer shape -- A-operand mode
- * (0 patch tiles, 1 linear tiles / im2col-mode TMA, 2 halo), tile width BN, tiles and rounds of the persistent grid. */
+ * (0 patch tiles, 1 linear tiles / im2col-mode TMA, 2 halo), tile width BN, tiles and rounds of the persistent grid,
+ * tile walk (0 N-major, 1 M-band: each CTA keeps one N tile) and grid size. */
 typedef struct SyConvPlan {
-  int32_t mode, bn, m_tiles, n_tiles, rounds, kblocks, patch_h, patch_w;
+  int32_t mode, bn, m_tiles, n_tiles, rounds, kblocks, patch_h, patch_w, walk, grid;
 } SyConvPlan;
 int sy_conv2d_plan(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride,
                    SyConvPlan* out);

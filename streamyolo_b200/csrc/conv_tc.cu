@@ -73,6 +73,10 @@ struct Params {
   int th, tw, tiles_x, tiles_y;
   int m_tiles, n_tiles, total_tiles;
   FastDiv fd_m_tiles, fd_per_img, fd_tiles_x, fd_tw;
+  // tile walk (pick_walk; see tile_nm in the kernel) and the statistics rows it fills
+  int band, t_end, cls_step, cls_tiles;
+  int stat_rows;            // partial rows the finalize sums (N-major: one per CTA; M-band: one per class)
+  FastDiv fd_band, fd_cls_tiles;
   // linear tiles (LIN): an M tile is 128 consecutive output pixels of the flattened (n, oh, ow) space
   int P_total;              // N * Ho * Wo
   int gp;                   // first output pixel of statistics group 1 (== P_total: single group)
@@ -173,13 +177,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   constexpr bool LIN = (AM == 1);
   constexpr bool HALO = (AM == 2);
   constexpr int kBB = C::kBBytes;
-  // tile walk of this CTA (expressions, not variables: blockIdx / gridDim / kernel parameters cost no registers)
-#define SY_T_FIRST ((int)blockIdx.x)
-#define SY_T_STEP ((int)gridDim.x)
-#define SY_T_END (p.total_tiles)
-  auto tile_nm = [&](int tile, int& n_tile, int& m_tile) {
-    n_tile = fdiv(tile, p.fd_m_tiles);
-    m_tile = tile - n_tile * p.m_tiles;
+  // tile walk of this CTA (expressions, not variables: blockIdx / kernel parameters cost no registers; see pick_walk).
+  // band == 1 (N-major): walk index = tile index, M fastest.  band == n_tiles (M-band): CTA b = slot * band + N tile;
+  // walk index w = class * cls_tiles + k visits M tile rho + k * stat_rows of class rho = slot + class * cls_step.
+  // tile_nm is false for walk indices that name no tile (every role skips them alike).
+#define SY_T_FIRST (p.band > 1 ? 0 : (int)blockIdx.x)
+#define SY_T_STEP (p.band > 1 ? 1 : (int)gridDim.x)
+#define SY_T_END (p.t_end)
+  auto tile_nm = [&](int tile, int& n_tile, int& m_tile) -> bool {
+    if (p.band == 1) {
+      n_tile = fdiv(tile, p.fd_m_tiles);
+      m_tile = tile - n_tile * p.m_tiles;
+      return true;
+    }
+    const int slot = fdiv((int)blockIdx.x, p.fd_band);
+    n_tile = (int)blockIdx.x - slot * p.band;
+    const int cls = fdiv(tile, p.fd_cls_tiles);
+    const int rho = slot + cls * p.cls_step;
+    m_tile = rho + (tile - cls * p.cls_tiles) * p.stat_rows;
+    return rho < p.stat_rows && m_tile < p.m_tiles;
   };
   const int S = p.stages;                                  // patch/linear: A+B ring depth; halo: B ring depth
   // 64-deep K sub-blocks per ring stage; halo mode: filter taps per weight-ring stage (one barrier round per filter row)
@@ -246,9 +262,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       // partial row of this CTA, channel-major: the four sums of a channel are one 16-byte word (the finalize below loads
       // one word per row and channel; with the shared-memory layout [4][Cout] in global memory it needed four loads, and the
       // 640 sector requests per warp made the partial-row sums the longest part of the tail)
-      float4* mine = reinterpret_cast<float4*>(p.partials) + (size_t)blockIdx.x * p.Cout;
-      for (int c = et; c < p.Cout; c += kTailThreads)
-        mine[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
+      // (M-band walk: the statistics warps wrote this CTA's class rows already)
+      if (p.band == 1) {
+        float4* mine = reinterpret_cast<float4*>(p.partials) + (size_t)blockIdx.x * p.Cout;
+        for (int c = et; c < p.Cout; c += kTailThreads)
+          mine[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
+      }
       if (p.n_seg > 0) {
         auto grid_barrier = [&](unsigned int* ctr) {    // all CTAs of the persistent grid are resident (1 per SM)
           __threadfence();
@@ -294,7 +313,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll
           for (int j = 0; j < 5; ++j) {
             const int r = lane + 32 * j;
-            buf[j] = r < (int)gridDim.x ? __ldcg(rows4 + (size_t)r * p.Cout) : make_float4(0.f, 0.f, 0.f, 0.f);
+            buf[j] = r < p.stat_rows ? __ldcg(rows4 + (size_t)r * p.Cout) : make_float4(0.f, 0.f, 0.f, 0.f);
           }
           double v[4] = {0.0, 0.0, 0.0, 0.0};
 #pragma unroll
@@ -302,7 +321,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             v[0] += (double)buf[j].x; v[1] += (double)buf[j].y; v[2] += (double)buf[j].z; v[3] += (double)buf[j].w;
           }
           if (et == 0) tl_rec<TL>(p, tl_epi, 4, 8, 0, 0);
-          for (int r = lane + 160; r < (int)gridDim.x; r += 32) {          // (more than 160 CTAs: not on an H100)
+          for (int r = lane + 160; r < p.stat_rows; r += 32) {            // (more than 160 rows: not on an H100)
             const float4 q = __ldcg(rows4 + (size_t)r * p.Cout);
             v[0] += (double)q.x; v[1] += (double)q.y; v[2] += (double)q.z; v[3] += (double)q.w;
           }
@@ -369,7 +388,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           const int chunk = et % CPR, r0 = et / CPR;
           for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
             int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
+        if (!tile_nm(tile, n_tile, m_tile)) continue;
             const int cg = n_tile * BN + chunk * 8;
             if (cg >= p.Cout) continue;
             int img = 0, py = 0, px = 0;
@@ -456,7 +475,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       uint32_t pha = 0;
       for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
         int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
+        if (!tile_nm(tile, n_tile, m_tile)) continue;
         const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
         const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
         for (int cb = 0; cb < p.cblocks; ++cb) {
@@ -478,7 +497,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       uint32_t phb = 0;
       for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
         int n_tile, m_tile_unused;
-        tile_nm(tile, n_tile, m_tile_unused);
+        if (!tile_nm(tile, n_tile, m_tile_unused)) continue;
         for (int cb = 0; cb < p.cblocks; ++cb) {
           for (int t0 = 0; t0 < 9; t0 += kSub) {
             mbar_wait(empty_bar(sb), phb ^ 1u);
@@ -509,7 +528,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       int tl_n = is_a ? 0 : p.timeline_cap / 8;
       for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
         int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
+        if (!tile_nm(tile, n_tile, m_tile)) continue;
         int img, y0, x0;
         if constexpr (LIN) {
           const int p0 = m_tile * kBlockM;
@@ -567,7 +586,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (sflip) bar_free_arrive(1, nbar);
     for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
       int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
+        if (!tile_nm(tile, n_tile, m_tile)) continue;
       int c1, c2, c3;                            // store coordinates below the channel: (x, y, image) | (pixel, 0, 0)
       if constexpr (LIN) {
         c1 = m_tile * kBlockM; c2 = 0; c3 = 0;
@@ -634,8 +653,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // Warp ew owns columns [8*ew, 8*ew+8) of every 64-column slab; lane l reads rows l, l+32, l+64, l+96 (one 16-byte
     // chunk each).  The per-lane partial sums (8 columns x {sum, sum of squares}) stay in REGISTERS across slabs and tiles
     // -- one set per slab index of the tile -- and are only combined across the 32 lanes (recursive-halving shuffles) and
-    // added to the CTA's shared-memory totals on a FLUSH: when the CTA moves to another n tile or statistics group, on a
-    // tile that straddles the group boundary, and at the end.  (Per-slab shuffle reductions made the statistics warps the
+    // added to the CTA's shared-memory totals on a FLUSH: when the CTA moves to another n tile (N-major walk only) or
+    // statistics group, on a tile that straddles the group boundary, and at the end.  (Per-slab shuffle reductions made the statistics warps the
     // bottleneck of every epilogue-bound layer: ~1400 cycles per slab.)
     constexpr int kSlabs = BN / kSlabCols;
     constexpr int kAccSlabs = (BN <= 128) ? kSlabs : 1;      // BN = 256: registers do not allow four sets; flush every slab
@@ -691,9 +710,35 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int j = 0; j < kAccSlabs; ++j) reduce_store(acc[j], pend_grp, pend_n0 + j * kSlabCols);
       pend_grp = -1;
     };
+    // M-band walk: the CTA's tiles of one class rho are exactly those that one CTA of the N-major walk took for this N tile,
+    // in the same order, so this CTA's sums of a class are that CTA's partial row for these BN columns, bit for bit.  The
+    // row of class rho is the N-major walk's CTA (n_tile * m_tiles + rho) mod stat_rows; classes without tiles write zeros.
+#define SY_BAND (do_stats && p.band > 1)
+    auto write_class = [&](int cls, bool zero) {                 // all 256 statistics threads
+      const int my_slot = fdiv((int)blockIdx.x, p.fd_band), my_n = (int)blockIdx.x - my_slot * p.band;
+      const int row = (int)(((long long)my_n * p.m_tiles + my_slot + cls * p.cls_step) % p.stat_rows);
+      float4* dst = reinterpret_cast<float4*>(p.partials) + (size_t)row * p.Cout;
+      const int c = my_n * BN + st;
+      if (zero) {
+        if (st < BN && c < p.Cout) dst[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+        return;
+      }
+      asm volatile("bar.sync 8, 256;" ::: "memory");          // the owner lanes' shared-memory sums are complete
+      if (st < BN && c < p.Cout) {
+        dst[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
+        sAcc[c] = 0.f; sAcc[p.Cout + c] = 0.f; sAcc[2 * p.Cout + c] = 0.f; sAcc[3 * p.Cout + c] = 0.f;
+      }
+      asm volatile("bar.sync 8, 256;" ::: "memory");
+    };
+    int pend_cls = -1;                                           // class whose sums sAcc holds (M-band walk)
+    if (SY_BAND) {
+      const int my_slot = fdiv((int)blockIdx.x, p.fd_band);
+      for (int cls = 0; my_slot + cls * p.cls_step < p.stat_rows; ++cls)
+        if (my_slot + cls * p.cls_step >= p.m_tiles) write_class(cls, true);
+    }
     for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
       int n_tile, m_tile;
-        tile_nm(tile, n_tile, m_tile);
+        if (!tile_nm(tile, n_tile, m_tile)) continue;
       const int n0 = n_tile * BN;
       // rows [0, cut) of the tile belong to statistics group 0, rows [cut, 128) to group 1 (a patch tile lies in one
       // image = one group; a linear tile can straddle the boundary; rows past the end of the tensor were staged as zeros)
@@ -705,6 +750,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
       const bool pure = (cut <= 0) || (cut >= kBlockM);
       const int tgrp = cut <= 0 ? 1 : 0;
+      if (SY_BAND) {                                             // warp-uniform
+        const int cls = fdiv(tile, p.fd_cls_tiles);
+        if (pend_cls >= 0 && cls != pend_cls) {
+          flush();
+          write_class(pend_cls, false);
+        }
+        pend_cls = cls;
+      }
       if (do_stats && kAccSlabs == kSlabs && (!pure || pend_grp != tgrp || pend_n0 != n0)) flush();     // warp-uniform
       for (int slab = 0; slab < kSlabs; ++slab, sbuf ^= sflip) {
         bar_staged_wait(sbuf, nbar);
@@ -759,6 +812,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
     if (do_stats) flush();
+    if (SY_BAND && pend_cls >= 0) write_class(pend_cls, false);
+#undef SY_BAND
     kernel_tail();
   } else {
     reg_alloc<kRegsMma>();
@@ -790,7 +845,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     int tl_n = (et == 0) ? p.timeline_cap / 2 : p.timeline_cap;
     for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
       int n_tile, m_tile;
-      tile_nm(tile, n_tile, m_tile);
+      if (!tile_nm(tile, n_tile, m_tile)) continue;
       bool valid[2];
       long long pix[2];                          // this thread's output pixels in the flattened (n, oh, ow) space
 #pragma unroll
@@ -995,6 +1050,37 @@ static int pick_bn(int cout, int m_tiles, int kblocks) {
 
 static const int kSmemLimit = 232448;   // 227 KiB opt-in maximum per CTA
 
+// Order in which the persistent grid walks the (N tile, M tile) space.
+//   N-major (band 1): CTA b takes tiles b, b + G, ... numbered M fastest.  The whole grid works on one or two N tiles at a
+//     time, so every N tile re-streams the whole A tensor, from HBM whenever A does not fit in L2.
+//   M-band (band n_tiles, S = SMs / n_tiles slots, grid S * n_tiles): CTA b = slot * n_tiles + N tile keeps its N tile for
+//     its whole life.  The M tiles fall into SMs classes rho = m mod SMs; slot j owns the classes j, j + S, j + 2S, ... < SMs
+//     and walks them one after the other, each class in increasing m.  The n_tiles CTAs of a slot walk the same M tiles at
+//     about the same time, so A crosses HBM -> L2 about once per layer.
+// One class of one N tile holds exactly the tiles that one CTA of the N-major walk (grid = SMs) takes for that N tile, in the
+// same order, so the M-band walk writes the N-major walk's statistics rows bit for bit (statistics warps, write_class).
+// M-band is taken whenever it does not add a round of the persistent grid (it never saves one).
+struct Walk {
+  int band, grid, t_end, stat_rows, cls_step, cls_tiles;
+};
+static Walk pick_walk(int m_tiles, int n_tiles) {
+  const int sms = num_sms(), total = m_tiles * n_tiles;
+  const int grid = min(total, sms);
+  const Walk nmajor{1, grid, total, grid, 0, 1};
+  if (n_tiles == 1 || total <= sms) return nmajor;
+  const int slots = sms / n_tiles;
+  int worst = 0;                                   // tiles of the busiest slot
+  for (int j = 0; j < slots; ++j) {
+    int w = 0;
+    for (int rho = j; rho < sms; rho += slots)
+      if (rho < m_tiles) w += cdiv(m_tiles - rho, sms);
+    worst = max(worst, w);
+  }
+  if (worst > cdiv(total, sms)) return nmajor;
+  const int cls_tiles = cdiv(m_tiles, sms);
+  return {n_tiles, slots * n_tiles, cdiv(sms, slots) * cls_tiles, sms, slots, cls_tiles};
+}
+
 struct Plan {
   int smem, grid;
 };
@@ -1043,7 +1129,11 @@ static int make_plan(Params& p, Plan* out) {
     smem = fixed_bytes + acc_bytes + stages * stage_bytes;
   }
   out->smem = smem;
-  out->grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
+  const Walk wk = pick_walk(p.m_tiles, p.n_tiles);
+  p.band = wk.band; p.t_end = wk.t_end; p.stat_rows = wk.stat_rows; p.cls_step = wk.cls_step; p.cls_tiles = wk.cls_tiles;
+  p.fd_band = make_fastdiv((uint32_t)wk.band);
+  p.fd_cls_tiles = make_fastdiv((uint32_t)wk.cls_tiles);
+  out->grid = wk.grid;
   return SY_OK;
 }
 
@@ -1225,7 +1315,7 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     const int rc = halo ? tc::plan_bn<2>(bn, p, &pl) : (lin ? tc::plan_bn<1>(bn, p, &pl) : tc::plan_bn<0>(bn, p, &pl));
     if (rc != SY_OK) return rc;
   }
-  if (d->rows_written) *d->rows_written = pl.grid;
+  if (d->rows_written) *d->rows_written = p.stat_rows;
 
   // A: input view as (C, W, H, N), box (64, TW*s, TH*s, 1) traversed with element strides (1, s, s, 1)
   CUtensorMap ta, tb, ty;
@@ -1327,6 +1417,9 @@ extern "C" int sy_conv2d_plan(int32_t n, int32_t h, int32_t w, int32_t cin, int3
   out->m_tiles = m_tiles;
   out->n_tiles = cdiv(cout, bn);
   out->rounds = cdiv(m_tiles * out->n_tiles, tc::num_sms());
+  const tc::Walk wk = tc::pick_walk(m_tiles, out->n_tiles);
+  out->walk = wk.band > 1 ? 1 : 0;
+  out->grid = wk.grid;
   out->kblocks = kblocks;
   out->patch_h = lin ? 0 : th;
   out->patch_w = lin ? 0 : tw;

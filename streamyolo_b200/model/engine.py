@@ -23,7 +23,9 @@ from ..ops import View
 
 
 # normalise pass inside the conv launch (1 launch / BaseConv).  One CTA per SM keeps fewer bytes in flight on the big tensors
-# than the separate pass (not measured on H100), so SY_FUSE_APPLY=1 is a debug switch; SY_FUSE_APPLY_MAX_MB fuses only the layers whose raw output is at most that many MB (L2 resident, launch-bound)
+# than the separate pass, so SY_FUSE_APPLY=1 is a debug switch; SY_FUSE_APPLY_MAX_MB fuses only the layers whose raw output
+# is at most that many MB.  Off by default: bench.py's forward+loss step on an H100 80GB HBM3 at 400 W ran as fast or slower
+# with it (8 / 24 MB: 427 / 424 pairs/s against 427 with the 40 MB arena; 8 MB without the arena: 548 against 552-556)
 FUSE_APPLY = os.environ.get("SY_FUSE_APPLY", "0") != "0"
 FUSE_APPLY_MAX_BYTES = float(os.environ.get("SY_FUSE_APPLY_MAX_MB", "0")) * 1e6
 WEIGHT_EPOCH = 0  # bumped by whoever updates parameters through raw pointers (train.Trainer's fused optimiser kernel does
@@ -140,8 +142,12 @@ def _bn_seg(m, c_begin=0):
     return (bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.num_batches_tracked, c_begin)
 
 
-# raw conv outputs of the plain (non-recording) train-mode forward: one arena per (device, stream), marked persisting in L2
-RAW_ARENA_MB = float(os.environ.get("SY_RAW_ARENA_MB", "40"))
+# raw conv outputs of the plain (non-recording) train-mode forward: one arena per (device, stream), marked persisting in L2.
+# Off by default on H100: the persisting set-aside (at most 32.8 MB of the 50 MB L2) is taken from every other kernel's L2,
+# and the convs' operand re-reads lose more than the normalise passes gain.  bench.py's forward+loss step on an H100 80GB
+# HBM3 at 400 W, arena 0 / 24 / 40 MB: 526 / 476 / 399 pairs/s with the N-major tile walk; with a first version of the
+# M-band walk, 0 / 8 / 16 / 24 / 40 MB: 552-556 / 553 / 539 / 508 / 427 pairs/s (profiles/h100_l2_sweep.txt).
+RAW_ARENA_MB = float(os.environ.get("SY_RAW_ARENA_MB", "0"))
 _RAW_ARENAS = {}
 
 

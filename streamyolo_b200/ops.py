@@ -101,7 +101,8 @@ class SyPackItem(C.Structure):
 
 
 class SyConvPlan(C.Structure):
-    _fields_ = [(n, C.c_int32) for n in ("mode", "bn", "m_tiles", "n_tiles", "rounds", "kblocks", "patch_h", "patch_w")]
+    _fields_ = [(n, C.c_int32) for n in ("mode", "bn", "m_tiles", "n_tiles", "rounds", "kblocks", "patch_h", "patch_w",
+                                               "walk", "grid")]
 
 
 class SyTalLossBwdDesc(C.Structure):

@@ -19,8 +19,10 @@ batch = int(sys.argv[2]) if len(sys.argv) > 2 else 8
 seq = [s for s in op_sequence.sequence(model, batch) if s["kind"] == "conv"]
 MODE = {0: "patch", 1: "linear", 2: "halo"}
 print(f"StreamYOLO-{model}, {batch} frame pairs: {len(seq)} conv launches per step")
-print(f"{'layer':50s} {'shape':34s} {'mode':7s} {'BN':>4s} {'tiles':>6s} {'rounds':>6s} {'K blk':>6s} {'fill':>5s}")
-tot = {}
+WALK = {0: "N-major", 1: "M-band"}
+print(f"{'layer':50s} {'shape':34s} {'mode':7s} {'BN':>4s} {'tiles':>6s} {'rounds':>6s} {'K blk':>6s} {'fill':>5s} "
+      f"{'walk':8s} {'grid':>4s}")
+tot, walks = {}, {}
 for s in seq:
     m = re.match(r"(\d+)x(\d+)x(\d+) (\d+)->(\d+) k(\d+)x(\d+)s(\d+)", s["shape"])
     n, h, w, ci, co, kh, kw, st = map(int, m.groups())
@@ -28,5 +30,8 @@ for s in seq:
     tiles = p["m_tiles"] * p["n_tiles"]
     fill = tiles / (p["rounds"] * ops.conv_stat_rows())
     tot[MODE[p["mode"]]] = tot.get(MODE[p["mode"]], 0) + 1
-    print(f"{s['name'][-50:]:50s} {s['shape']:34s} {MODE[p['mode']]:7s} {p['bn']:4d} {tiles:6d} {p['rounds']:6d} {p['kblocks']:6d} {fill:5.2f}")
+    walks[WALK[p["walk"]]] = walks.get(WALK[p["walk"]], 0) + 1
+    print(f"{s['name'][-50:]:50s} {s['shape']:34s} {MODE[p['mode']]:7s} {p['bn']:4d} {tiles:6d} {p['rounds']:6d} {p['kblocks']:6d} {fill:5.2f} "
+          f"{WALK[p['walk']]:8s} {p['grid']:4d}")
 print("launches per mode:", tot)
+print("launches per walk:", walks)
