@@ -846,21 +846,24 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
       int n_tile, m_tile;
       if (!tile_nm(tile, n_tile, m_tile)) continue;
-      bool valid[2];
-      long long pix[2];                          // this thread's output pixels in the flattened (n, oh, ow) space
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
+      // this thread's output pixels in the flattened (n, oh, ow) space (evaluated where they are used: only the
+      // validity flags stay live across the main loop)
+      auto pixel = [&](int h, bool& ok) -> long long {
         if constexpr (LIN) {
-          pix[h] = (long long)m_tile * kBlockM + r0 + 8 * h;
-          valid[h] = pix[h] < p.P_total;
+          const long long px = (long long)m_tile * kBlockM + r0 + 8 * h;
+          ok = px < p.P_total;
+          return px;
         } else {
           const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
           const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
           const int oy = py * p.th + ty[h], ox = px * p.tw + tx[h];
-          valid[h] = in_patch[h] && (oy < p.Ho) && (ox < p.Wo);
-          pix[h] = ((long long)img * p.Ho + oy) * p.Wo + ox;
+          ok = in_patch[h] && (oy < p.Ho) && (ox < p.Wo);
+          return ((long long)img * p.Ho + oy) * p.Wo + ox;
         }
-      }
+      };
+      bool valid[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) pixel(h, valid[h]);
       const int n0 = n_tile * BN;
       tl_rec<TL>(p, tl_n, 2, 0, tile, 0);
       if (p.mode == SY_CONV_FUSED) {
@@ -938,31 +941,50 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
         tl_rec<TL>(p, tl_n, 2, 2, tile, slab);
         bar_free_wait(sbuf);                     // (A) staging tile free: its store has read it, the statistics loads are done
-        const uint32_t tb = stage_base + (uint32_t)(sbuf * kSlabBytes) + (uint32_t)cq * 2u;
+        // 16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) << 4); this thread's rows r0 and r0 + 8 share r & 7,
+        // so the chunk offset is (j << 4) ^ sw: one logic op, nothing kept live across the main loop
+        const uint32_t tb = stage_base + (uint32_t)(sbuf * kSlabBytes) + (uint32_t)cq * 2u + (uint32_t)r0 * 128u;
+        const uint32_t sw = ((uint32_t)r0 & 7u) << 4;
+        if (p.mode == SY_CONV_RAW && p.dbg_f32 == nullptr) {
+          // raw values (every conv of a training step): round, pack and stage -- no per-value pixel or column arithmetic
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const int J = slab * 8 + j;
-          const int cl = slab * kSlabCols + j * 8 + cq;          // tile column of this thread's first value
+          for (int j = 0; j < 8; ++j) {
+            const int J = slab * 8 + j;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
+                           "r"(valid[h] ? pack_bf16(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]) : 0u) : "memory");
+          }
+        } else {
+          long long pix[2];
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            float v0 = acc[4 * J + 2 * h], v1 = acc[4 * J + 2 * h + 1];
-            const bool inb = valid[h] && n0 + cl < p.Cout;
-            if (p.dbg_f32 != nullptr && inb)     // validation only: the accumulators before any rounding
-              *reinterpret_cast<float2*>(p.dbg_f32 + pix[h] * p.Cout + n0 + cl) = make_float2(v0, v1);
-            if (p.mode != SY_CONV_RAW) {
-              v0 = v0 * sScale[cl] + sShift[cl];
-              v1 = v1 * sScale[cl + 1] + sShift[cl + 1];
-              if (p.act) { v0 = silu_f(v0); v1 = silu_f(v1); }
-              if (p.res != nullptr && inb) {
-                const uint32_t rv = *reinterpret_cast<const uint32_t*>(p.res + pix[h] * p.res_pitch + n0 + cl);
-                v0 += bf16_lo(rv);
-                v1 += bf16_hi(rv);
+            bool ok;
+            pix[h] = pixel(h, ok);
+          }
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const int J = slab * 8 + j;
+            const int cl = slab * kSlabCols + j * 8 + cq;          // tile column of this thread's first value
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float v0 = acc[4 * J + 2 * h], v1 = acc[4 * J + 2 * h + 1];
+              const bool inb = valid[h] && n0 + cl < p.Cout;
+              if (p.dbg_f32 != nullptr && inb)     // validation only: the accumulators before any rounding
+                *reinterpret_cast<float2*>(p.dbg_f32 + pix[h] * p.Cout + n0 + cl) = make_float2(v0, v1);
+              if (p.mode != SY_CONV_RAW) {
+                v0 = v0 * sScale[cl] + sShift[cl];
+                v1 = v1 * sScale[cl + 1] + sShift[cl + 1];
+                if (p.act) { v0 = silu_f(v0); v1 = silu_f(v1); }
+                if (p.res != nullptr && inb) {
+                  const uint32_t rv = *reinterpret_cast<const uint32_t*>(p.res + pix[h] * p.res_pitch + n0 + cl);
+                  v0 += bf16_lo(rv);
+                  v1 += bf16_hi(rv);
+                }
               }
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
+                           "r"(valid[h] ? pack_bf16(v0, v1) : 0u) : "memory");
             }
-            // 16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) << 4)
-            const uint32_t row = (uint32_t)(r0 + 8 * h);
-            asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + row * 128u + ((((uint32_t)j) ^ (row & 7u)) << 4)),
-                         "r"(valid[h] ? pack_bf16(v0, v1) : 0u) : "memory");
           }
         }
         fence_proxy_async();                     // generic-proxy writes -> visible to the TMA (async proxy)
