@@ -53,12 +53,6 @@ int sy_version(void);
 /* 0 when the current device is sm_90 and the driver exposes cuTensorMapEncodeTiled. */
 int sy_check_device(void);
 
-/* Mark [ptr, ptr + bytes) as a persisting-L2 access window for the kernels subsequently launched on `stream` (inherited by
- * the kernel nodes of a stream capture); bytes = 0 clears it.  *granted = the window the device allows (0: none).  The host
- * side (engine.py) draws the raw conv outputs of all train-mode BaseConvs that fit from one arena inside this window: the
- * normalise pass then reads them from L2 and the next layer overwrites them before they reach HBM. */
-int sy_l2_persist_window(void* ptr, size_t bytes, float hit_ratio, size_t* granted, sy_stream_t stream);
-
 /* -------- convolution (replaces [yolox] BaseConv.conv / nn.Conv2d, e.g.
  * exps/model/darknet.py:115-165, exps/model/dfp_pafpn.py:33-105,
  * exps/model/tal_head.py:55-104) ------------------------------------------------- */
@@ -94,17 +88,13 @@ typedef struct {
   float* scale_shift;    /* [2 (scale|shift)][2 groups][Cout]: y = x*scale + shift, ready when the kernel ends */
   float* mean_invstd;    /* optional [2 (mean|invstd)][2 groups][Cout]: the batch statistics themselves, saved for
                           * sy_bn_act_backward (NULL: not written) */
-  uint32_t* sync;        /* four zero-initialised counters (grid barriers); the kernel leaves them at zero */
-  /* With bn[]: optional normalise + act (+ residual) pass INSIDE the same launch (after a second grid barrier
-   * every CTA re-reads the raw tiles it stored -- L2 resident -- and writes apply_y = act(y*scale+shift) (+ apply_res)).
-   * apply_y.ptr == NULL: leave it to sy_bn_act_apply.  The *_group1_offset are element offsets added to the
-   * addresses of statistics-group-1 images (DFP fusion, see sy_bn_act_apply). */
-  SyTensor apply_y, apply_res;
-  int64_t apply_y_group1_offset, apply_res_group1_offset;
+  uint32_t* sync;        /* two zero-initialised counters (grid barrier + exit ticket); the kernel leaves them at zero.
+                          * The normalise + act pass is sy_bn_act_apply, launched after the conv. */
   /* ---- debugging only: CTA 0 records (event, clock64) int64 pairs of its three pipeline roles ---- */
   void* debug_timeline;  /* device buffer of 2*debug_timeline_events int64, or NULL */
   int32_t debug_timeline_events;
-  int32_t debug_flags;   /* 0 in production; 2 = skip TMA loads (pipeline dissection, results invalid) */
+  int32_t debug_flags;   /* 0 in production; 2 = skip TMA loads (pipeline dissection, results invalid);
+                          * bits 8-11 = operand ring depth of linear tiles (0: default) */
   /* ---- validation only: the fp32 accumulators themselves, before the bf16 rounding of the stored result:
    * debug_f32[pixel][Cout] (pixel = flattened (n, oh, ow)), written next to the normal output.  This is where
    * north_star's "within 1e-3 of the reference" is literal (tests/test_gpu_ops.py::test_conv_fp32_accumulators). ---- */
@@ -121,8 +111,9 @@ int sy_conv_stat_rows(void);
  * run two such launches concurrently on one GPU (the barrier needs every SM). */
 int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream);
 /* Host-only query (no launch, no GPU needed): the tiling sy_conv2d_tc chooses for a layer shape -- A-operand mode
- * (0 patch tiles, 1 linear tiles / im2col-mode TMA, 2 halo), tile width BN, tiles and rounds of the persistent grid,
- * tile walk (0 N-major, 1 M-band: each CTA keeps one N tile) and grid size. */
+ * (1 linear tiles / im2col-mode TMA, 2 halo: 16 x 8 patches, the only mode with patch_h x patch_w, else 0 x 0), tile
+ * width BN, tiles and rounds of the persistent grid, tile walk (0 N-major, 1 M-band: each CTA keeps one N tile) and grid
+ * size. */
 typedef struct SyConvPlan {
   int32_t mode, bn, m_tiles, n_tiles, rounds, kblocks, patch_h, patch_w, walk, grid;
 } SyConvPlan;

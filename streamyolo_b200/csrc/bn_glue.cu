@@ -64,40 +64,6 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
   return make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
 }
 
-// first version (one 16-byte chunk per loop trip, 64-bit index division): kept for A/B runs (SY_APPLY=v1)
-__global__ void bn_act_apply_v1_kernel(const __nv_bfloat16* __restrict__ x, long long xp, const float* __restrict__ scale,
-                                    const float* __restrict__ shift, long long split_pix, int act,
-                                    const __nv_bfloat16* res, long long rp, __nv_bfloat16* y, long long yp,
-                                    long long npix, int C, long long y_goff1, long long r_goff1) {
-  const int G = C / 8;
-  const long long total = npix * G;
-  for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-       idx += (long long)gridDim.x * blockDim.x) {
-    const int g = (int)(idx % G);
-    const long long pix = idx / G;
-    const int grp = pix >= split_pix ? 1 : 0;
-    float f[8], r[8];
-    unpack8(*reinterpret_cast<const uint4*>(x + pix * xp + g * 8), f);
-    const float4 s0 = *reinterpret_cast<const float4*>(scale + grp * C + g * 8);
-    const float4 s1 = *reinterpret_cast<const float4*>(scale + grp * C + g * 8 + 4);
-    const float4 h0 = *reinterpret_cast<const float4*>(shift + grp * C + g * 8);
-    const float4 h1 = *reinterpret_cast<const float4*>(shift + grp * C + g * 8 + 4);
-    const float sc[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-    const float sh[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float t = f[i] * sc[i] + sh[i];
-      f[i] = act ? silu_f(t) : t;
-    }
-    if (res != nullptr) {
-      unpack8(*reinterpret_cast<const uint4*>(res + pix * rp + g * 8 + (grp ? r_goff1 : 0)), r);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) f[i] += r[i];
-    }
-    *reinterpret_cast<uint4*>(y + pix * yp + g * 8 + (grp ? y_goff1 : 0)) = pack8(f);
-  }
-}
-
 // y = act(x * scale[grp] + shift[grp]) (+ res), 16 bytes (8 channels) per thread and pixel.
 // A thread keeps ONE channel chunk for its whole life (scale/shift of both statistics groups live in registers, no
 // per-element index division) and walks the pixels with kApplyUnroll independent 16-byte loads in flight.
@@ -108,7 +74,7 @@ __global__ void __launch_bounds__(kApplyThreads, 3)
 bn_act_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xp, const float* __restrict__ scale,
                     const float* __restrict__ shift, long long split_pix, int act,
                     const __nv_bfloat16* res, long long rp, __nv_bfloat16* y, long long yp,
-                    long long npix, int C, long long y_goff1, long long r_goff1, int hints) {
+                    long long npix, int C, long long y_goff1, long long r_goff1) {
   pdl_launch_dependents();
   const int G = C >> 3;                           // 16-byte chunks per pixel (<= 256)
   const int ppb = kApplyThreads / G;              // pixels per block pass
@@ -136,8 +102,7 @@ bn_act_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xp, const flo
 #pragma unroll
     for (int j = 0; j < kApplyUnroll; ++j) {
       const long long pix = pix0 + j * step;
-      // hints & 1: the raw tensor is dead after this pass -- read it with the streaming (evict-first) policy (A/B switch)
-      if (pix < npix) v[j] = (hints & 1) ? __ldcs(reinterpret_cast<const uint4*>(xg + pix * xp)) : *reinterpret_cast<const uint4*>(xg + pix * xp);
+      if (pix < npix) v[j] = *reinterpret_cast<const uint4*>(xg + pix * xp);
     }
     if (RES) {
 #pragma unroll
@@ -165,8 +130,7 @@ bn_act_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xp, const flo
 #pragma unroll
         for (int i = 0; i < 8; ++i) f[i] += r[i];
       }
-      if (hints & 2) __stcg(reinterpret_cast<uint4*>(yg + pix * yp + (g1 ? y_goff1 : 0)), pack8(f));
-      else *reinterpret_cast<uint4*>(yg + pix * yp + (g1 ? y_goff1 : 0)) = pack8(f);
+      *reinterpret_cast<uint4*>(yg + pix * yp + (g1 ? y_goff1 : 0)) = pack8(f);
     }
   }
 }
@@ -346,32 +310,20 @@ extern "C" int sy_bn_act_apply(SyTensor x, const float* scale, const float* shif
   }
   const long long npix = (long long)x.n * x.h * x.w;
   const long long split_pix = (long long)split_n * x.h * x.w;
-  {
-    const char* e = getenv("SY_APPLY");
-    if (e != nullptr && e[0] == 'v' && e[1] == '1') {
-      bn_act_apply_v1_kernel<<<grid_for(npix * (x.c / 8), 256), 256, 0, stream>>>(
-          CBF(x.ptr), x.pitch, scale, shift, split_pix, act, rp, rpitch, BF(y.ptr), y.pitch, npix, x.c, (long long)y_goff1,
-          (long long)r_goff1);
-      return launch_status("bn_act_apply_v1_kernel");
-    }
-  }
   SY_REQUIRE(x.c <= 8 * kApplyThreads, SY_EINVAL, "bn_act_apply: C=%d > %d", x.c, 8 * kApplyThreads);
   const int ppb = kApplyThreads / (x.c / 8);
   // enough blocks for one pass of kApplyUnroll pixels per thread, capped at one wave of 3 resident blocks per SM
   const long long want = (npix + (long long)ppb * kApplyUnroll - 1) / ((long long)ppb * kApplyUnroll);
-  long long cap = (long long)sm_count() * 3;   // one wave of 3 resident blocks per SM
-  if (const char* e = getenv("SY_APPLY_CAP")) cap = (long long)sm_count() * (atoi(e) > 0 ? atoi(e) : 3);   // tuning aid: blocks per SM
+  const long long cap = (long long)sm_count() * 3;
   const int grid = (int)(want < 1 ? 1 : (want < cap ? want : cap));
   const bool has_res = rp != nullptr;
-  int hints = 0;
-  if (const char* e = getenv("SY_APPLY_HINTS")) hints = atoi(e);                             // tuning aid: cache-policy bits
   auto launch = [&](auto kernel) -> int {
     // L1/shared split: measured on the whole step (StreamYOLO-l, 8 pairs): carveout 0 (all L1) 6.40 ms, default and
     // 100 (all shared, the conv kernels' split) 6.51 ms.
     SY_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
     SY_CUDA(launch_pdl(kernel, dim3(grid), dim3(kApplyThreads), 0, stream, CBF(x.ptr), (long long)x.pitch, scale, shift,
                        split_pix, act, rp, rpitch, BF(y.ptr), (long long)y.pitch, npix, x.c, (long long)y_goff1,
-                       (long long)r_goff1, hints));
+                       (long long)r_goff1));
     return SY_OK;
   };
   int rc;

@@ -1,14 +1,13 @@
 // Implicit-GEMM convolution on the Hopper tensor cores (sm_90a, wgmma).
 //
-//   M = 128 output pixels: 128 consecutive pixels of the flattened (n, oh, ow) space ("linear" tiles, the default), a
-//       TH x TW patch of one image, or a 16 x 8 patch with its input halo (template parameter AM, see below)
+//   M = 128 output pixels: 128 consecutive pixels of the flattened (n, oh, ow) space ("linear" tiles, the default), or a
+//       16 x 8 patch of one image with its input halo (3x3 stride-1 convs; template parameter AM, see below)
 //   N = output channels (BN = 64/128 per tile, chosen per layer)
 //   K = taps * Cin, walked as (tap, 64-channel block)
 //
-// Operand movement is im2col-free: for every (tap, channel block) ONE TMA load (im2col mode for
-// linear tiles, tiled mode for patches) brings the shifted input pixels [128][64ch] straight from the NHWC tensor into a
-// 128B-swizzled shared-memory tile (out-of-bounds = zero padding = the conv padding;
-// stride-2 convs use the tensor map's element strides), and one 3-D TMA load brings the
+// Operand movement is im2col-free: for linear tiles ONE im2col-mode TMA load per (tap, channel block) brings the shifted
+// input pixels [128][64ch] straight from the NHWC tensor into a 128B-swizzled shared-memory tile (out-of-bounds = zero
+// padding = the conv padding; stride-2 convs use the tensor map's element strides), and one 3-D TMA load brings the
 // [BN][64] weight slab.  Two consumer warpgroups issue wgmma.mma_async (M=64 each, N=BN, K=16) with both operands in
 // shared memory and the fp32 accumulators in registers.
 //
@@ -52,14 +51,22 @@ constexpr int kRegsStats = 120;
 constexpr int kRegsIo = 32;
 static_assert(2 * kRegsMma + 2 * kRegsStats + kRegsIo <= 5 * kRegsLaunch, "register budget of one CTA");
 constexpr int kEpiThreads = 256;    // MMA + convert warps 0-7
-constexpr int kTailThreads = 512;   // convert + statistics warps run the kernel tail (partials, grid barrier, finalize, apply)
+constexpr int kTailThreads = 512;   // convert + statistics warps run the kernel tail (partials, grid barrier, finalize)
 constexpr int kABytes = kBlockM * 128;   // 16 KiB per stage
 constexpr int kMaxStages = 8;
-// Linear / patch tiles: a ring of four A+B stages (four 64-deep K blocks in flight), not as many as shared memory holds.
+// Linear tiles: a ring of four A+B stages (four 64-deep K blocks in flight), not as many as shared memory holds.
 // bench.py's forward+loss step on an H100 80GB HBM3 at 700 W, ring depth capped at 3 / 4 / 5 / none (= 6 stages at
 // BN = 128): 405 / 416 / 404 / 387 pairs/s.  Why deeper rings are slower has not been isolated; four is the measured optimum.
 constexpr int kRingStages = 4;
-// 64-deep K sub-blocks per pipeline stage: two (one barrier round per K = 128) halve the per-round hand-shake cost
+// Halo tiles: a 16 x 8 output patch (one 8-pixel swizzle atom per patch row) and its 18 x 10 input halo, stored densely
+// (kHaloPitch pixels = 1280 bytes per halo row: the MMA's swizzle follows the absolute shared address bits, exactly like the
+// TMA that wrote the tile, so neither the atoms' stride nor their start needs 1 KiB alignment); three filter taps per
+// weight-ring stage (one barrier round per filter row)
+constexpr int kHaloTH = 16, kHaloTW = 8;
+constexpr int kHaloPitch = kHaloTW + 2;
+constexpr int kHaloTx = (kHaloTH + 2) * kHaloPitch * 128;           // bytes one halo load delivers
+constexpr int kHaloBytes = (kHaloTx + 1023) / 1024 * 1024;          // halo ring stage stride (multiple of 1 KiB)
+constexpr int kHaloTaps = 3;
 
 struct BnSeg {
   const float* gamma; const float* beta;
@@ -70,9 +77,9 @@ struct BnSeg {
 struct Params {
   int N, Ho, Wo, Cout, Cin;
   int kh, kw, stride, pad_h, pad_w;
-  int th, tw, tiles_x, tiles_y;
-  int m_tiles, n_tiles, total_tiles;
-  FastDiv fd_m_tiles, fd_per_img, fd_tiles_x, fd_tw;
+  int tiles_x, tiles_y;     // halo mode: 16 x 8 patches per image row / column
+  int m_tiles, n_tiles;
+  FastDiv fd_m_tiles, fd_per_img, fd_tiles_x;
   // tile walk (pick_walk; see tile_nm in the kernel) and the statistics rows it fills
   int band, t_end, cls_step, cls_tiles;
   int stat_rows;            // partial rows the finalize sums (N-major: one per CTA; M-band: one per class)
@@ -83,11 +90,7 @@ struct Params {
   FastDiv fd_hw, fd_wo;
   int cblocks, kblocks, stages;
   int stage_tiles;          // 1 or 2 epilogue staging tiles
-  // halo mode (AM == 2)
-  int stagesA;              // halo ring depth
-  int halo_pitch;           // pixels per halo row in shared memory (10, or 16 with debug flag 128)
-  int halo_bytes;           // stage stride (multiple of 1 KiB)
-  int halo_tx;              // bytes one halo load delivers
+  int stagesA;              // halo mode: halo ring depth
   int mode, act;
   __nv_bfloat16* y;
   long long y_pitch;
@@ -105,12 +108,7 @@ struct Params {
   float unbias[2];          // cnt / (cnt - 1) of each group: biased -> unbiased variance for the running statistics
   float* ss;                // [2 (scale|shift)][2 groups][Cout]
   float* mi;                // optional [2 (mean|invstd)][2 groups][Cout] for the backward pass
-  unsigned int* sync;       // three counters (two grid barriers + exit ticket), zero between launches
-  // normalise + act (+ residual) pass done by this kernel after the statistics are final (nullptr: separate launch)
-  __nv_bfloat16* ap_y; long long ap_y_pitch;
-  const __nv_bfloat16* ap_res; long long ap_res_pitch;
-  long long ap_y_goff1, ap_res_goff1;
-  int ap_act;
+  unsigned int* sync;       // two counters (grid barrier + exit ticket), zero between launches
   long long* timeline;      // debug: CTA 0 records (event id, clock) pairs; nullptr in production
   int timeline_cap;
   int debug_flags;          // debug: 2 = skip the TMA loads (barriers still cycle)
@@ -155,8 +153,6 @@ constexpr int kSlabBytes = kBlockM * 128;      // 16 KiB staging tile
 template <int BN>
 struct Cfg {
   static constexpr int kBBytes = BN * 128;
-  static constexpr int kSub = 1;                                    // 64-deep K blocks per ring stage (a fixed trip count keeps the
-                                                                    // wgmma stream asynchronous; a runtime-length loop serialises it)
   static constexpr int kAcc = BN / 2;                               // fp32 accumulators per consumer thread (64 rows x BN)
   // fixed part of dynamic smem (everything but the A/B ring and the per-CTA statistic accumulators)
   // plus, after the barriers, ONE region that is scale/shift (FUSED, 2 KiB) or the statistic accumulators (RAW)
@@ -164,7 +160,6 @@ struct Cfg {
 };
 
 // AM = how the A operand (activations) reaches shared memory:
-//   0 patch  : TH x TW patch tiles, one tiled 4-D TMA load per (tap, channel block)
 //   1 linear : 128 consecutive output pixels, one im2col-mode TMA load per (tap, channel block)
 //   2 halo   : 16 x 8 patch tiles, ONE tiled load per channel block of the 18 x (8+2) input halo; the nine taps are nine
 //              shared-memory descriptors into that halo (every 8-pixel swizzle atom of a tap view is one halo row).
@@ -197,14 +192,14 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     m_tile = rho + (tile - cls * p.cls_tiles) * p.stat_rows;
     return rho < p.stat_rows && m_tile < p.m_tiles;
   };
-  const int S = p.stages;                                  // patch/linear: A+B ring depth; halo: B ring depth
-  // 64-deep K sub-blocks per ring stage; halo mode: filter taps per weight-ring stage (one barrier round per filter row)
-  constexpr int kSub = HALO ? 3 : C::kSub;
+  const int S = p.stages;                                  // linear: A+B ring depth; halo: B ring depth
+  // weight slabs per ring stage: one 64-deep K block; halo mode: kHaloTaps filter taps
+  constexpr int kSub = HALO ? kHaloTaps : 1;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms; plain pointer arithmetic keeps the shared address space
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
-  uint8_t* sB = sA + (HALO ? p.stagesA * p.halo_bytes : S * kSub * kABytes);
+  uint8_t* sB = sA + (HALO ? p.stagesA * kHaloBytes : S * kABytes);
   uint8_t* sStage = sB + S * kSub * kBB;                                 // 1024-aligned: the rings are multiples of 1 KiB
   uint64_t* bars = reinterpret_cast<uint64_t*>(sStage + p.stage_tiles * kSlabBytes);
   const int sflip = p.stage_tiles - 1;                                   // slab parity toggles the tile iff there are two
@@ -245,19 +240,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   pdl_wait();
   if (threadIdx.x == 16 * 32) tl_rec<TL>(p, tl_k, 4, 1, 0, 0);
 
-  const uint32_t a_bytes = LIN ? (uint32_t)kABytes : (uint32_t)(p.th * p.tw) * 128u;
   const int per_img = p.tiles_x * p.tiles_y;
   const int hw = p.Ho * p.Wo;
   int tl_epi = p.timeline_cap;           // debug-timeline cursor of thread 0, carried from the consumer loop into the tail
 
-  // ---------------------------------------------- per-CTA partial row, grid barrier, BatchNorm finalize, apply
+  // ---------------------------------------------- per-CTA partial row, grid barrier, BatchNorm finalize
   // run by the 16 convert + statistics warps (512 threads); called from both of their branches so that each copy is
   // compiled under that warpgroup's register budget
   auto kernel_tail = [&]() {
     const int et = threadIdx.x;                        // 0..511
     const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
     if (et == 0) tl_rec<TL>(p, tl_epi, 4, 2, 0, 0);
-    bar_stats_done();                                // every sAcc update is done; convert warps have seen the stores drain
+    bar_stats_done();                                // every sAcc update is done
     if (do_stats) {
       // partial row of this CTA, channel-major: the four sums of a channel are one 16-byte word (the finalize below loads
       // one word per row and channel; with the shared-memory layout [4][Cout] in global memory it needed four loads, and the
@@ -269,15 +263,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           mine[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
       }
       if (p.n_seg > 0) {
-        auto grid_barrier = [&](unsigned int* ctr) {    // all CTAs of the persistent grid are resident (1 per SM)
-          __threadfence();
-          bar_stats_done();
-          if (et == 0) {
-            atomicAdd(ctr, 1u);
-            while (ld_acquire_u32(ctr) < gridDim.x) __nanosleep(32);
-          }
-          bar_stats_done();
-        };
         if (et == 0) tl_rec<TL>(p, tl_epi, 4, 5, 0, 0);
         // This CTA finalizes channels [b*cpc, (b+1)*cpc), one warp per channel.  The BatchNorm parameters and running
         // statistics of the warp's first channel do not depend on the other CTAs: load them BEFORE the grid barrier (they
@@ -297,12 +282,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (sg.rvar) pre_rv = sg.rvar[cs];
           }
         }
-        grid_barrier(&p.sync[0]);
+        // grid barrier: all CTAs of the persistent grid are resident (1 per SM)
+        __threadfence();
+        bar_stats_done();
+        if (et == 0) {
+          atomicAdd(&p.sync[0], 1u);
+          while (ld_acquire_u32(&p.sync[0]) < gridDim.x) __nanosleep(32);
+        }
+        bar_stats_done();
         if (et == 0) tl_rec<TL>(p, tl_epi, 4, 6, 0, 0);
-        // exit ticket (the last CTA past the barriers re-arms the counters): taken as early as possible -- right after the
-        // last grid barrier -- so that the atomic's round trip overlaps the finalize instead of ending the kernel
+        // exit ticket (the last CTA past the barrier re-arms the counters): taken as early as possible -- right after the
+        // barrier -- so that the atomic's round trip overlaps the finalize instead of ending the kernel
         unsigned int ticket = 0xffffffffu;
-        if (et == 0 && p.ap_y == nullptr) ticket = atomicAdd(&p.sync[2], 1u);
+        if (et == 0) ticket = atomicAdd(&p.sync[1], 1u);
         // one WARP per channel (no block barriers): lane l sums the partial rows l, l+32, ... in order, a fixed shuffle tree
         // combines the lanes (deterministic), lanes 0 / 1 finalize one statistics group each.
         for (int c = c_first; c < c_end; c += kTailThreads / 32) {
@@ -376,90 +368,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int sgi = 0; sgi < p.n_seg; ++sgi)          // (a reduction: no round trip -- a load-add-store ended CTA 0 ~1 us late)
             if (p.seg[sgi].nbt) atomicAdd(reinterpret_cast<unsigned long long*>(p.seg[sgi].nbt), (unsigned long long)groups);
         }
-        if (p.ap_y != nullptr) {
-          // ---- second grid barrier: scale/shift of every channel are published; normalise this CTA's own tiles,
-          //      re-reading the raw bf16 values it just stored (L2 resident for all but the largest layers)
-          grid_barrier(&p.sync[1]);
-          for (int i = et; i < p.Cout; i += kTailThreads)          // [2 (scale|shift)][2 groups][Cout] -> smem (over sAcc)
-            reinterpret_cast<float4*>(sAcc)[i] = __ldcg(reinterpret_cast<const float4*>(p.ss) + i);
-          bar_stats_done();
-          constexpr int CPR = BN / 8;                              // 16-byte chunks per pixel row of a tile
-          constexpr int RPP = kTailThreads / CPR;                  // tile rows handled per pass of the 512 threads
-          const int chunk = et % CPR, r0 = et / CPR;
-          for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-            int n_tile, m_tile;
-        if (!tile_nm(tile, n_tile, m_tile)) continue;
-            const int cg = n_tile * BN + chunk * 8;
-            if (cg >= p.Cout) continue;
-            int img = 0, py = 0, px = 0;
-            if constexpr (!LIN) {
-              img = fdiv(m_tile, p.fd_per_img);
-              const int rem = m_tile - img * per_img;
-              py = fdiv(rem, p.fd_tiles_x); px = rem - py * p.tiles_x;
-            }
-            // batches of kAB rows: all loads first (the stores may alias the loads, so the compiler cannot hoist them)
-            constexpr int kAB = 4;
-            const int rows_in_patch = LIN ? kBlockM : p.th * p.tw;
-            for (int rb = r0; rb < rows_in_patch; rb += RPP * kAB) {
-              long long pixv[kAB];
-              uint4 u[kAB], rv[kAB];
-#pragma unroll
-              for (int j = 0; j < kAB; ++j) {
-                const int rr = rb + j * RPP;
-                if constexpr (LIN) {
-                  const long long pp = (long long)m_tile * kBlockM + rr;
-                  pixv[j] = (rr < kBlockM && pp < p.P_total) ? pp : -1;
-                } else {
-                  const int tyy = fdiv(rr, p.fd_tw), txx = rr - tyy * p.tw;
-                  const int oy = py * p.th + tyy, ox = px * p.tw + txx;
-                  pixv[j] = (rr < rows_in_patch && img < p.N && oy < p.Ho && ox < p.Wo) ? ((long long)img * p.Ho + oy) * p.Wo + ox : -1;
-                }
-              }
-#pragma unroll
-              for (int j = 0; j < kAB; ++j)
-                if (pixv[j] >= 0) u[j] = __ldcg(reinterpret_cast<const uint4*>(p.y + pixv[j] * p.y_pitch + cg));
-              if (p.ap_res != nullptr) {
-#pragma unroll
-                for (int j = 0; j < kAB; ++j)
-                  if (pixv[j] >= 0)
-                    rv[j] = *reinterpret_cast<const uint4*>(p.ap_res + pixv[j] * p.ap_res_pitch + cg +
-                                                            (pixv[j] >= p.gp ? p.ap_res_goff1 : 0));
-              }
-#pragma unroll
-              for (int j = 0; j < kAB; ++j) {
-                if (pixv[j] < 0) continue;
-                const int grp = pixv[j] >= p.gp ? 1 : 0;
-                const float* sc = sAcc + grp * p.Cout + cg;
-                const float* sh = sAcc + (2 + grp) * p.Cout + cg;
-                const float4 s0 = *reinterpret_cast<const float4*>(sc), s1 = *reinterpret_cast<const float4*>(sc + 4);
-                const float4 h0 = *reinterpret_cast<const float4*>(sh), h1 = *reinterpret_cast<const float4*>(sh + 4);
-                const float scv[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-                const float shv[8] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w};
-                float f[8] = {bf16_lo(u[j].x), bf16_hi(u[j].x), bf16_lo(u[j].y), bf16_hi(u[j].y),
-                              bf16_lo(u[j].z), bf16_hi(u[j].z), bf16_lo(u[j].w), bf16_hi(u[j].w)};
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                  const float t = f[i] * scv[i] + shv[i];
-                  f[i] = p.ap_act ? silu_f(t) : t;
-                }
-                if (p.ap_res != nullptr) {
-                  f[0] += bf16_lo(rv[j].x); f[1] += bf16_hi(rv[j].x); f[2] += bf16_lo(rv[j].y); f[3] += bf16_hi(rv[j].y);
-                  f[4] += bf16_lo(rv[j].z); f[5] += bf16_hi(rv[j].z); f[6] += bf16_lo(rv[j].w); f[7] += bf16_hi(rv[j].w);
-                }
-                *reinterpret_cast<uint4*>(p.ap_y + pixv[j] * p.ap_y_pitch + cg + (grp ? p.ap_y_goff1 : 0)) =
-                    make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-              }
-            }
-          }
-        }
-        if (et == 0) {
-          if (p.ap_y != nullptr) ticket = atomicAdd(&p.sync[2], 1u);
-          if (ticket == gridDim.x - 1) {            // every CTA is past both barriers: re-arm for the next launch
-            p.sync[0] = 0u;
-            p.sync[1] = 0u;
-            p.sync[2] = 0u;
-            __threadfence();
-          }
+        if (et == 0 && ticket == gridDim.x - 1) {   // every CTA is past the barrier: re-arm for the next launch
+          p.sync[0] = 0u;
+          p.sync[1] = 0u;
+          __threadfence();
         }
       }
     }
@@ -470,7 +382,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   reg_dealloc<kRegsIo>();
   if (HALO && (warp == 18 || warp == 17)) {
     // ----------------------------------------------- halo mode producers
-    if (warp == 18) {                            // A: one halo box [TH + 2 rows][pitch px][64 ch] per (tile, channel block)
+    if (warp == 18) {                            // A: one halo box [18 rows][10 px][64 ch] per (tile, channel block)
       int sa = 0;
       uint32_t pha = 0;
       for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
@@ -484,8 +396,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             if (p.debug_flags & 2) {
               mbar_arrive(fullA_bar(sa));
             } else {
-              mbar_expect_tx(fullA_bar(sa), (uint32_t)p.halo_tx);
-              tma_load_4d(smem_u32(sA + sa * p.halo_bytes), &tmA, fullA_bar(sa), cb * kBlockK, px * p.tw - 1, py * p.th - 1, img);
+              mbar_expect_tx(fullA_bar(sa), (uint32_t)kHaloTx);
+              tma_load_4d(smem_u32(sA + sa * kHaloBytes), &tmA, fullA_bar(sa), cb * kBlockK, px * kHaloTW - 1, py * kHaloTH - 1, img);
             }
           }
           __syncwarp();
@@ -529,46 +441,30 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
         int n_tile, m_tile;
         if (!tile_nm(tile, n_tile, m_tile)) continue;
-        int img, y0, x0;
-        if constexpr (LIN) {
-          const int p0 = m_tile * kBlockM;
-          img = fdiv(p0, p.fd_hw);
-          const int rem = p0 - img * hw;
-          const int oh = fdiv(rem, p.fd_wo), ow = rem - oh * p.Wo;
-          y0 = oh * p.stride - p.pad_h; x0 = ow * p.stride - p.pad_w;
-        } else {
-          img = fdiv(m_tile, p.fd_per_img);
-          const int rem = m_tile - img * per_img;
-          const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-          y0 = py * p.th * p.stride - p.pad_h; x0 = px * p.tw * p.stride - p.pad_w;
-        }
-        // walk the (tap, channel block) sub-blocks kSub at a time: one barrier round per stage
+        const int p0 = m_tile * kBlockM;
+        const int img = fdiv(p0, p.fd_hw);
+        const int rem = p0 - img * hw;
+        const int oh = fdiv(rem, p.fd_wo), ow = rem - oh * p.Wo;
+        const int y0 = oh * p.stride - p.pad_h, x0 = ow * p.stride - p.pad_w;
+        // walk the (tap, channel block) K blocks, one per ring stage
         int r = 0, sx = 0, cb = 0;
-        for (int sb0 = 0; sb0 < p.kblocks; sb0 += kSub) {
-          const int nsub = min(kSub, p.kblocks - sb0);
+        for (int kb = 0; kb < p.kblocks; ++kb) {
           mbar_wait(empty_bar(stage), phase ^ 1u);          // whole warp waits: control flow stays uniform
           if (elect_one()) {
-            tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 0, tile, sb0);
+            tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 0, tile, kb);
             if (p.debug_flags & 2) mbar_arrive(full_bar(stage));
-            else mbar_expect_tx(full_bar(stage), is_a ? a_bytes * (uint32_t)nsub : (uint32_t)(kBB * nsub));
-            tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 1, tile, sb0);
+            else mbar_expect_tx(full_bar(stage), is_a ? (uint32_t)kABytes : (uint32_t)kBB);
+            tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 1, tile, kb);
           }
-          for (int j = 0; j < nsub; ++j) {
-            if (!(p.debug_flags & 2) && elect_one()) {
-              if (is_a) {
-                if constexpr (LIN)
-                  tma_load_im2col_4d(smem_u32(sA + (stage * kSub + j) * kABytes), &tmA, full_bar(stage), cb * kBlockK, x0,
-                                     y0, img, (uint16_t)sx, (uint16_t)r);
-                else
-                  tma_load_4d(smem_u32(sA + (stage * kSub + j) * kABytes), &tmA, full_bar(stage), cb * kBlockK, x0 + sx,
-                              y0 + r, img);
-              } else
-                tma_load_3d(smem_u32(sB + (stage * kSub + j) * kBB), &tmB, full_bar(stage), cb * kBlockK,
-                            r * p.kw + sx, n_tile * BN);
-            }
-            if (++cb == p.cblocks) { cb = 0; if (++sx == p.kw) { sx = 0; ++r; } }
+          if (!(p.debug_flags & 2) && elect_one()) {
+            if (is_a)
+              tma_load_im2col_4d(smem_u32(sA + stage * kABytes), &tmA, full_bar(stage), cb * kBlockK, x0, y0, img,
+                                 (uint16_t)sx, (uint16_t)r);
+            else
+              tma_load_3d(smem_u32(sB + stage * kBB), &tmB, full_bar(stage), cb * kBlockK, r * p.kw + sx, n_tile * BN);
           }
-          if (TL && elect_one()) tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 2, tile, sb0);
+          if (++cb == p.cblocks) { cb = 0; if (++sx == p.kw) { sx = 0; ++r; } }
+          if (TL && elect_one()) tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 2, tile, kb);
           __syncwarp();
           if (++stage == S) { stage = 0; phase ^= 1u; }
         }
@@ -593,7 +489,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       } else {
         const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
         const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-        c1 = px * p.tw; c2 = py * p.th; c3 = img;
+        c1 = px * kHaloTW; c2 = py * kHaloTH; c3 = img;
       }
       for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
         bar_staged_wait(sbuf, nbar);
@@ -622,16 +518,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       __syncwarp();
       bar_free_arrive(prev, nbar);
     }
-    if (lane == 0) {
-      if (p.ap_y != nullptr) {
-        bulk_wait_all();                         // the fused normalise pass re-reads this CTA's raw tiles from global
-        asm volatile("fence.proxy.async;" ::: "memory");
-      } else {
-        bulk_wait_read();                        // smem has been read; the writes complete with the grid
-      }
-    }
+    // the stores have read the staging tiles before the CTA's final __syncthreads; their writes complete with the grid
+    if (lane == 0) bulk_wait_read();
     __syncwarp();
-    asm volatile("bar.sync 4, 288;" ::: "memory");   // the epilogue warps may now re-read this CTA's own raw tiles
   }
   } else if (warp >= 8) {
     reg_alloc<kRegsStats>();
@@ -657,10 +546,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     // statistics group, on a tile that straddles the group boundary, and at the end.  (Per-slab shuffle reductions made the statistics warps the
     // bottleneck of every epilogue-bound layer: ~1400 cycles per slab.)
     constexpr int kSlabs = BN / kSlabCols;
-    constexpr int kAccSlabs = (BN <= 128) ? kSlabs : 1;      // BN = 256: registers do not allow four sets; flush every slab
-    float acc[kAccSlabs][16];
+    float acc[kSlabs][16];
 #pragma unroll
-    for (int j = 0; j < kAccSlabs; ++j)
+    for (int j = 0; j < kSlabs; ++j)
 #pragma unroll
       for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
     int pend_grp = -1, pend_n0 = 0;                          // what the register sums belong to (-1: nothing pending)
@@ -707,7 +595,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     auto flush = [&]() {
       if (pend_grp < 0) return;
 #pragma unroll
-      for (int j = 0; j < kAccSlabs; ++j) reduce_store(acc[j], pend_grp, pend_n0 + j * kSlabCols);
+      for (int j = 0; j < kSlabs; ++j) reduce_store(acc[j], pend_grp, pend_n0 + j * kSlabCols);
       pend_grp = -1;
     };
     // M-band walk: the CTA's tiles of one class rho are exactly those that one CTA of the N-major walk took for this N tile,
@@ -740,7 +628,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       int n_tile, m_tile;
         if (!tile_nm(tile, n_tile, m_tile)) continue;
       const int n0 = n_tile * BN;
-      // rows [0, cut) of the tile belong to statistics group 0, rows [cut, 128) to group 1 (a patch tile lies in one
+      // rows [0, cut) of the tile belong to statistics group 0, rows [cut, 128) to group 1 (a halo tile lies in one
       // image = one group; a linear tile can straddle the boundary; rows past the end of the tensor were staged as zeros)
       int cut;
       if constexpr (LIN) {
@@ -758,7 +646,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
         pend_cls = cls;
       }
-      if (do_stats && kAccSlabs == kSlabs && (!pure || pend_grp != tgrp || pend_n0 != n0)) flush();     // warp-uniform
+      if (do_stats && (!pure || pend_grp != tgrp || pend_n0 != n0)) flush();     // warp-uniform
       for (int slab = 0; slab < kSlabs; ++slab, sbuf ^= sflip) {
         bar_staged_wait(sbuf, nbar);
         tl_rec<TL>(p, tl_t, 5, 0, tile, slab);
@@ -777,25 +665,21 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         tl_rec<TL>(p, tl_t, 5, 1, tile, slab);
         if (do_stats) {
           if (pure) {
-            float (&a)[16] = acc[kAccSlabs == kSlabs ? slab : 0];
+            float (&a)[16] = acc[slab];
 #pragma unroll
             for (int rr = 0; rr < 4; ++rr) {
 #pragma unroll
               for (int i = 0; i < 8; ++i) { a[i] += x[rr][i]; a[8 + i] += x[rr][i] * x[rr][i]; }
             }
-            if (kAccSlabs == kSlabs) {
-              pend_grp = tgrp; pend_n0 = n0;
-            } else {
-              reduce_store(a, tgrp, n0 + slab * kSlabCols);
-            }
+            pend_grp = tgrp; pend_n0 = n0;
           } else {
-            // the tile straddles the group boundary (at most one M tile per layer and N tile): masked, reduced at once
+            // the tile straddles the group boundary (at most one M tile per layer and N tile): masked, reduced at once.
+            // The sums go through acc[slab]: the flush before this tile left it zero, and reduce_store zeroes it again
+            // (a separate scratch array made the BN = 64 statistics warps spill)
 #pragma unroll 1
             for (int grp = 0; grp < 2; ++grp) {
               const int lo = grp ? cut : 0, hi = grp ? kBlockM : cut;
-              float a[16];
-#pragma unroll
-              for (int i = 0; i < 16; ++i) a[i] = 0.f;
+              float (&a)[16] = acc[slab];
 #pragma unroll
               for (int rr = 0; rr < 4; ++rr) {
                 const int r = lane + 32 * rr;
@@ -827,17 +711,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     const int cq = 2 * (lane & 3);                                 // its first column in every 8-column group
     const uint32_t stage_base = smem_u32(sStage);
     const bool lead = (threadIdx.x & 127) == 0;                    // signals the warpgroup's ring releases
-    int ty[2], tx[2];
-    bool in_patch[2];
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int row = r0 + 8 * h;
-      ty[h] = LIN ? 0 : fdiv(row, p.fd_tw);
-      tx[h] = LIN ? 0 : row - ty[h] * p.tw;
-      in_patch[h] = LIN ? true : row < p.th * p.tw;
-    }
     // halo mode: this warpgroup's 8 output rows start 8 halo rows further down
-    const uint32_t row_bytes = HALO ? (uint32_t)p.halo_pitch * 128u : 1024u;
+    constexpr uint32_t row_bytes = HALO ? (uint32_t)kHaloPitch * 128u : 1024u;
     const uint32_t a_off = HALO ? (uint32_t)(wg * 8) * row_bytes : (uint32_t)wg * 8192u;
     float acc[C::kAcc];
     int stage = 0, sa = 0, sbuf = 0;
@@ -856,8 +731,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         } else {
           const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
           const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-          const int oy = py * p.th + ty[h], ox = px * p.tw + tx[h];
-          ok = in_patch[h] && (oy < p.Ho) && (ox < p.Wo);
+          const int row = r0 + 8 * h;
+          const int oy = py * kHaloTH + row / kHaloTW, ox = px * kHaloTW + row % kHaloTW;
+          ok = (oy < p.Ho) && (ox < p.Wo);
           return ((long long)img * p.Ho + oy) * p.Wo + ox;
         }
       };
@@ -886,7 +762,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       if constexpr (HALO) {                      // K order = (channel block, tap)
         for (int cb = 0; cb < p.cblocks; ++cb) {
           mbar_wait(fullA_bar(sa), pha);
-          const uint32_t halo = smem_u32(sA + sa * p.halo_bytes) + a_off;
+          const uint32_t halo = smem_u32(sA + sa * kHaloBytes) + a_off;
           for (int t0 = 0; t0 < 9; t0 += kSub) {
             mbar_wait(full_bar(stage), phase);
             wgmma_fence_operand(acc);
@@ -896,8 +772,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               const int tap = t0 + j;
               const int r = tap / 3, sx = tap - 3 * r;
               const uint32_t a_addr = halo + (uint32_t)r * row_bytes + (uint32_t)sx * 128u;
-              const uint32_t boff = (p.debug_flags & 64) ? ((a_addr >> 7) & 7u) : 0u;
-              const uint64_t da = make_smem_desc(a_addr, row_bytes, boff);
+              const uint64_t da = make_smem_desc(a_addr, row_bytes);
               const uint64_t db = make_smem_desc(smem_u32(sB + (stage * kSub + j) * kBB));
 #pragma unroll
               for (int k = 0; k < kBlockK / 16; ++k)   // 16 bf16 = 32 bytes along K inside the swizzle row: +2 in (addr >> 4)
@@ -914,7 +789,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           if (++sa == p.stagesA) { sa = 0; pha ^= 1u; }
         }
       } else {
-        static_assert(kSub == 1, "one K block per stage");
         for (int kb = 0; kb < p.kblocks; ++kb) {
           mbar_wait(full_bar(stage), phase);
           wgmma_fence_operand(acc);
@@ -995,7 +869,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     tl_epi = tl_n;
     bar_free_wait(0);                                // drain the last arrivals (balanced barriers at exit)
     if (sflip) bar_free_wait(1);
-    asm volatile("bar.sync 4, 288;" ::: "memory");   // store warp: all TMA stores of this CTA are complete
     kernel_tail();
   }
   __syncthreads();
@@ -1008,43 +881,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
 // ------------------------------------------------------------------ host side
 
-// M tiling: "linear" = 128 consecutive output pixels of the flattened (n, oh, ow) space, fetched with im2col-mode TMA
-// (no partial tiles except the very last: 10-20 % fewer tiles than rectangular patches on 38x60 / 19x30 maps, which is
-// often a whole round of the persistent grid); SY_CONV_TILES=patch selects the rectangular TH x TW patches.
-static bool linear_tiles() {
-  const char* e = getenv("SY_CONV_TILES");
-  return !(e != nullptr && e[0] == 'p');
-}
-
-// choose the TH x TW output patch (<= 128 pixels) that needs the fewest tiles
-static void pick_patch(int ho, int wo, int* th, int* tw) {
-  long best = -1;
-  for (int w = 1; w <= 128 && w <= ((wo + 7) / 8) * 8; ++w) {
-    int h = 128 / w;
-    if (h < 1) break;
-    if (h > ho) h = ho;
-    long tiles = (long)cdiv(ho, h) * cdiv(wo, w);
-    long score = tiles * 1000 - (long)h * w;   // fewer tiles first, then fuller tiles
-    if (best < 0 || score < best) {
-      best = score;
-      *th = h;
-      *tw = w;
-    }
-  }
-}
-
-
-// Tile width heuristic from a per-K-block cost model: one 64-deep K block of a 128-row tile costs about kbc[] cycles
-// (MMA + barrier hand-shake + operand supply), the epilogue about epi_cycles_per_slab() per 64-column slab, and the
+// Tile width heuristic from a per-K-block cost model: one 64-deep K block of a 128-row tile costs about kblock_cycles()
+// (MMA + barrier hand-shake + operand supply), the epilogue about kEpiCyclesPerSlab per 64-column slab, and the
 // persistent grid runs ceil(tiles / SMs) rounds -- so wide tiles win unless they add a round.  The constants are a model,
-// not H100 measurements; SY_EPI_CYCLES / SY_CONV_BN let a tuning run override them.
-static double epi_cycles_per_slab(int bn) {
-  if (const char* e = getenv("SY_EPI_CYCLES")) {          // tuning aid "c64,c128": the heuristics' epilogue cost per slab
-    int c64 = 0, c128 = 0;
-    if (sscanf(e, "%d,%d", &c64, &c128) == 2) return (double)(bn == 64 ? c64 : c128);
-  }
-  return 1900.0;
-}
+// not H100 measurements; SY_CONV_BN forces the width.
+constexpr double kEpiCyclesPerSlab = 1900.0;
 
 static double kblock_cycles(int bn) { return bn == 128 ? 515.0 : 560.0; }
 
@@ -1062,7 +903,7 @@ static int pick_bn(int cout, int m_tiles, int kblocks) {
     const int tiles = m_tiles * cdiv(cout, bn);
     const int rounds = cdiv(tiles, num_sms());
     const double main_c = kblocks * kblock_cycles(bn);
-    const double epi = epi_cycles_per_slab(bn) * (bn / 64);
+    const double epi = kEpiCyclesPerSlab * (bn / 64);
     // the epilogue of a tile does not overlap the main loop of the next one (the accumulators are the consumers' registers)
     const double t = rounds * (main_c + epi + 400.0);
     if (t < best) { best = t; best_bn = bn; }
@@ -1126,23 +967,21 @@ static int make_plan(Params& p, Plan* out) {
   const int acc_bytes = (p.mode == SY_CONV_RAW && p.partials) ? 16 * p.Cout : 2048;
   // epilogue-bound layers (main loop of a tile shorter than its epilogue: 1x1 convs with few input channels, the
   // stem) get a second staging tile: the store + statistics of a slab then overlap the conversion of the next
-  const bool main_loop_bound = !(p.kblocks * kblock_cycles(BN) < epi_cycles_per_slab(BN) * (BN / 64));
+  const bool main_loop_bound = !(p.kblocks * kblock_cycles(BN) < kEpiCyclesPerSlab * (BN / 64));
   p.stage_tiles = main_loop_bound ? 1 : 2;
-  if (const char* e = getenv("SY_STAGE_TILES")) p.stage_tiles = (e[0] == '2') ? 2 : 1;   // tuning aid
   const int bbytes = Cfg<BN>::kBBytes;
   const int fixed_bytes = Cfg<BN>::kFixedBytes + (p.stage_tiles - 1) * kSlabBytes;
   int smem;
   if (AM == 2) {
-    // halo ring (2-3 stages of 23 KiB) + weight-slab ring (the rest, three taps per stage)
-    const int taps = 3;                                          // filter taps per weight-ring stage (kernel: kSub)
+    // halo ring (2-3 stages of 23 KiB) + weight-slab ring (the rest, kHaloTaps taps per stage)
     p.stagesA = (BN == 64 && p.cblocks > 1) ? 3 : 2;
-    int stages = (kSmemLimit - fixed_bytes - acc_bytes - p.stagesA * p.halo_bytes) / (taps * bbytes);
+    int stages = (kSmemLimit - fixed_bytes - acc_bytes - p.stagesA * kHaloBytes) / (kHaloTaps * bbytes);
     if (stages > kMaxStages) stages = kMaxStages;
     SY_REQUIRE(stages >= 2, SY_EINVAL, "conv2d_tc(halo): Cout=%d leaves no room for the weight ring", p.Cout);
     p.stages = stages;
-    smem = fixed_bytes + acc_bytes + p.stagesA * p.halo_bytes + stages * taps * bbytes;
+    smem = fixed_bytes + acc_bytes + p.stagesA * kHaloBytes + stages * kHaloTaps * bbytes;
   } else {
-    const int stage_bytes = Cfg<BN>::kSub * (kABytes + bbytes);
+    const int stage_bytes = kABytes + bbytes;
     const int fit = min(kMaxStages, (kSmemLimit - fixed_bytes - acc_bytes) / stage_bytes);
     int stages = min(fit, kRingStages);
     if ((p.debug_flags >> 8) & 15) stages = min(fit, (p.debug_flags >> 8) & 15);     // debug: set the ring depth
@@ -1213,6 +1052,25 @@ static bool use_halo(int n, int ho, int wo, int cout, int kblocks) {
   return cdiv(tiles_h * nt, num_sms()) * halo_c < cdiv(tiles_l * nt, num_sms()) * lin_c;
 }
 
+// The tiling of one layer shape, shared by sy_conv2d_tc and the host-only sy_conv2d_plan: halo mode where use_halo
+// takes it, linear tiles otherwise.  The tile width is chosen on the linear tiling (the halo decision assumed that width).
+struct Tiling {
+  bool halo;
+  int bn, m_tiles, tiles_x, tiles_y, cblocks, kblocks;
+};
+static Tiling pick_tiling(int n, int ho, int wo, int cin, int cout, int kh, int kw, int stride) {
+  Tiling t{};
+  t.cblocks = cdiv(cin, kBlockK);
+  t.kblocks = kh * kw * t.cblocks;
+  t.halo = kh == 3 && kw == 3 && stride == 1 && use_halo(n, ho, wo, cout, t.kblocks);
+  t.tiles_y = cdiv(ho, kHaloTH);
+  t.tiles_x = cdiv(wo, kHaloTW);
+  const int lin_tiles = cdiv(n * ho * wo, kBlockM);
+  t.m_tiles = t.halo ? n * t.tiles_y * t.tiles_x : lin_tiles;
+  t.bn = pick_bn(cout, lin_tiles, t.kblocks);
+  return t;
+}
+
 }  // namespace tc
 }  // namespace sy
 
@@ -1242,35 +1100,21 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   if (const char* e = getenv("SY_CONV_DEBUG")) p.debug_flags |= atoi(e);    // tuning aid (see Params::debug_flags)
   p.N = x.n; p.Ho = ho; p.Wo = wo; p.Cout = y.c; p.Cin = x.c;
   p.kh = d->kh; p.kw = d->kw; p.stride = d->stride; p.pad_h = ph; p.pad_w = pw;
-  const bool halo = d->kh == 3 && d->kw == 3 && d->stride == 1 && tc::linear_tiles() &&
-                    tc::use_halo(x.n, ho, wo, y.c, 9 * cdiv(x.c, tc::kBlockK));
-  const bool lin = !halo && tc::linear_tiles();
   SY_REQUIRE((long long)x.n * ho * wo < (1ll << 31) - 256, SY_EINVAL, "conv2d_tc: too many output pixels");
+  const tc::Tiling t = tc::pick_tiling(x.n, ho, wo, x.c, y.c, d->kh, d->kw, d->stride);
+  const bool halo = t.halo;
+  const int bn = t.bn;
   p.P_total = x.n * ho * wo;
-  tc::pick_patch(ho, wo, &p.th, &p.tw);
-  if (halo) {
-    p.th = 16; p.tw = 8;                                          // one 8-pixel swizzle atom per patch row
-    // halo rows are stored densely (TW + 2 pixels = 1280 bytes apart): the MMA's swizzle follows the absolute shared
-    // address bits, exactly like the TMA that wrote the tile, so neither the atoms' stride nor their start need 1 KiB
-    // alignment (debug flag 128 selects a 2 KiB row pitch instead, flag 64 sets the descriptor's base-offset field).
-    p.halo_pitch = (p.debug_flags & 128) ? 16 : p.tw + 2;
-    p.halo_tx = (p.th + 2) * p.halo_pitch * 128;
-    p.halo_bytes = (p.halo_tx + 1023) / 1024 * 1024;
-  }
-  p.tiles_y = cdiv(ho, p.th); p.tiles_x = cdiv(wo, p.tw);
-  p.m_tiles = lin ? cdiv(p.P_total, tc::kBlockM) : x.n * p.tiles_y * p.tiles_x;
+  p.tiles_y = t.tiles_y; p.tiles_x = t.tiles_x;
+  p.m_tiles = t.m_tiles;
   p.fd_hw = tc::make_fastdiv((uint32_t)(ho * wo));
   p.fd_wo = tc::make_fastdiv((uint32_t)wo);
-  p.cblocks = cdiv(x.c, tc::kBlockK);
-  p.kblocks = d->kh * d->kw * p.cblocks;
-  // tile width: chosen on the linear tiling (the halo decision above assumed that width)
-  const int bn = tc::pick_bn(y.c, halo ? cdiv(p.P_total, tc::kBlockM) : p.m_tiles, p.kblocks);
+  p.cblocks = t.cblocks;
+  p.kblocks = t.kblocks;
   p.n_tiles = cdiv(y.c, bn);
-  p.total_tiles = p.m_tiles * p.n_tiles;
   p.fd_m_tiles = tc::make_fastdiv((uint32_t)p.m_tiles);
   p.fd_per_img = tc::make_fastdiv((uint32_t)(p.tiles_x * p.tiles_y));
   p.fd_tiles_x = tc::make_fastdiv((uint32_t)p.tiles_x);
-  p.fd_tw = tc::make_fastdiv((uint32_t)p.tw);
   p.mode = d->mode; p.act = d->act;
   p.y = reinterpret_cast<__nv_bfloat16*>(y.ptr); p.y_pitch = y.pitch;
   p.res = nullptr; p.res_pitch = 0;
@@ -1317,41 +1161,27 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     p.ss = d->scale_shift;
     p.mi = d->mean_invstd;
     p.sync = d->sync;
-    if (d->apply_y.ptr != nullptr) {
-      const SyTensor& ay = d->apply_y;
-      SY_REQUIRE(view_ok(ay) && ay.h == ho && ay.w == wo && ay.c == y.c, SY_EINVAL, "conv2d_tc: apply_y view mismatch");
-      SY_REQUIRE((d->apply_y_group1_offset % 8) == 0 && (d->apply_res_group1_offset % 8) == 0, SY_EINVAL,
-                 "conv2d_tc: group offsets must be multiples of 8");
-      p.ap_y = reinterpret_cast<__nv_bfloat16*>(ay.ptr); p.ap_y_pitch = ay.pitch;
-      p.ap_act = d->act;
-      p.ap_y_goff1 = d->apply_y_group1_offset; p.ap_res_goff1 = d->apply_res_group1_offset;
-      if (d->apply_res.ptr != nullptr) {
-        SY_REQUIRE(view_ok(d->apply_res) && d->apply_res.h == ho && d->apply_res.w == wo && d->apply_res.c == y.c, SY_EINVAL,
-                   "conv2d_tc: apply_res view mismatch");
-        p.ap_res = reinterpret_cast<const __nv_bfloat16*>(d->apply_res.ptr); p.ap_res_pitch = d->apply_res.pitch;
-      }
-    }
   }
   tc::Plan pl{};
   {
-    const int rc = halo ? tc::plan_bn<2>(bn, p, &pl) : (lin ? tc::plan_bn<1>(bn, p, &pl) : tc::plan_bn<0>(bn, p, &pl));
+    const int rc = halo ? tc::plan_bn<2>(bn, p, &pl) : tc::plan_bn<1>(bn, p, &pl);
     if (rc != SY_OK) return rc;
   }
   if (d->rows_written) *d->rows_written = p.stat_rows;
 
-  // A: input view as (C, W, H, N), box (64, TW*s, TH*s, 1) traversed with element strides (1, s, s, 1)
+  // A: input view as (C, W, H, N)
   CUtensorMap ta, tb, ty;
   if (halo) {
-    // A, halo mode: box (64 ch, pitch px, TH + 2 rows, 1 image) at (x0 - 1, y0 - 1): out of bounds = zero padding
+    // A, halo mode: box (64 ch, 10 px, 18 rows, 1 image) at (x0 - 1, y0 - 1): out of bounds = zero padding
     cuuint64_t dims[4] = {(cuuint64_t)x.c, (cuuint64_t)x.w, (cuuint64_t)x.h, (cuuint64_t)x.n};
     cuuint64_t strides[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.pitch * 2 * x.w, (cuuint64_t)x.pitch * 2 * x.w * x.h};
-    cuuint32_t box[4] = {(cuuint32_t)tc::kBlockK, (cuuint32_t)p.halo_pitch, (cuuint32_t)(p.th + 2), 1};
+    cuuint32_t box[4] = {(cuuint32_t)tc::kBlockK, (cuuint32_t)tc::kHaloPitch, (cuuint32_t)(tc::kHaloTH + 2), 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = enc(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x.ptr, dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(A halo) failed: %d", (int)r);
-  } else if (lin) {
+  } else {
     // A, im2col mode: tensor (C, W, H, N); the bounding box of base pixels is [-pad, dim + pad - (k - 1)) per spatial
     // dim, walked with the conv stride; one load = 128 consecutive base pixels x 64 channels, shifted by the tap offset
     tc::EncodeIm2colFn enc2 = tc::get_encode_im2col();
@@ -1360,26 +1190,12 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     cuuint64_t strides[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.pitch * 2 * x.w, (cuuint64_t)x.pitch * 2 * x.w * x.h};
     int lower[2] = {-pw, -ph};                                   // {W, H}
     int upper[2] = {pw - (d->kw - 1), ph - (d->kh - 1)};
-    if (getenv("SY_IM2COL_HW") != nullptr) {                     // bring-up switch: corners in {H, W} order
-      int t = lower[0]; lower[0] = lower[1]; lower[1] = t;
-      t = upper[0]; upper[0] = upper[1]; upper[1] = t;
-    }
     cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
     CUresult r = enc2(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x.ptr, dims, strides, lower, upper, (cuuint32_t)tc::kBlockK,
                       (cuuint32_t)tc::kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeIm2col(A) failed: %d (c=%d w=%d h=%d n=%d pitch=%lld k=%dx%d s=%d)",
                (int)r, x.c, x.w, x.h, x.n, (long long)x.pitch, d->kh, d->kw, d->stride);
-  } else {
-    cuuint64_t dims[4] = {(cuuint64_t)x.c, (cuuint64_t)x.w, (cuuint64_t)x.h, (cuuint64_t)x.n};
-    cuuint64_t strides[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.pitch * 2 * x.w, (cuuint64_t)x.pitch * 2 * x.w * x.h};
-    cuuint32_t box[4] = {(cuuint32_t)tc::kBlockK, (cuuint32_t)(p.tw * d->stride), (cuuint32_t)(p.th * d->stride), 1};
-    cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
-    CUresult r = enc(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x.ptr, dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(A) failed: %d (c=%d w=%d h=%d n=%d pitch=%lld box=%u,%u,%u)",
-               (int)r, x.c, x.w, x.h, x.n, (long long)x.pitch, box[0], box[1], box[2]);
   }
   {
     const int taps = d->kh * d->kw;
@@ -1392,7 +1208,7 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
-  if (lin) {
+  if (!halo) {
     // Y: output view as (C, pixels, 1, 1), box (64, 128, 1, 1): the TMA store clips the last tile / the channel slice
     cuuint64_t dims[4] = {(cuuint64_t)y.c, (cuuint64_t)p.P_total, 1, 1};
     cuuint64_t strides[3] = {(cuuint64_t)y.pitch * 2, (cuuint64_t)y.pitch * 2 * p.P_total, (cuuint64_t)y.pitch * 2 * p.P_total};
@@ -1403,22 +1219,21 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(Y linear) failed: %d", (int)r);
   } else {
-    // Y: output view as (C, W, H, N), box (64, TW, TH, 1): the TMA store clips the patch to the image / slice
+    // Y: output view as (C, W, H, N), box (64, 8, 16, 1): the TMA store clips the patch to the image / slice
     cuuint64_t dims[4] = {(cuuint64_t)y.c, (cuuint64_t)y.w, (cuuint64_t)y.h, (cuuint64_t)y.n};
     cuuint64_t strides[3] = {(cuuint64_t)y.pitch * 2, (cuuint64_t)y.pitch * 2 * y.w, (cuuint64_t)y.pitch * 2 * y.w * y.h};
-    cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)p.tw, (cuuint32_t)p.th, 1};
+    cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)tc::kHaloTW, (cuuint32_t)tc::kHaloTH, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
     CUresult r = enc(&ty, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, y.ptr, dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(Y) failed: %d", (int)r);
   }
-  if (halo) return tc::launch_bn<2>(bn, ta, tb, ty, p, pl, stream);
-  if (lin) return tc::launch_bn<1>(bn, ta, tb, ty, p, pl, stream);
-  return tc::launch_bn<0>(bn, ta, tb, ty, p, pl, stream);
+  return halo ? tc::launch_bn<2>(bn, ta, tb, ty, p, pl, stream) : tc::launch_bn<1>(bn, ta, tb, ty, p, pl, stream);
 }
 
-// Host-only query (no launch, works without a GPU): the tiling decisions sy_conv2d_tc takes for a layer shape.
+// Host-only query (no launch, works without a GPU): the tiling decisions sy_conv2d_tc takes for a layer shape
+// (both go through pick_tiling and pick_walk).
 extern "C" int sy_conv2d_plan(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride,
                               SyConvPlan* out) {
   SY_REQUIRE(out != nullptr && n > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, SY_EINVAL, "conv2d_plan: bad arguments");
@@ -1426,24 +1241,18 @@ extern "C" int sy_conv2d_plan(int32_t n, int32_t h, int32_t w, int32_t cin, int3
              "conv2d_plan: kernel %dx%d stride %d unsupported", kh, kw, stride);
   const int ph = (kh - 1) / 2, pw = (kw - 1) / 2;
   const int ho = (h + 2 * ph - kh) / stride + 1, wo = (w + 2 * pw - kw) / stride + 1;
-  const int cblocks = cdiv(cin, tc::kBlockK), kblocks = kh * kw * cblocks;
-  const bool halo = kh == 3 && kw == 3 && stride == 1 && tc::linear_tiles() && tc::use_halo(n, ho, wo, cout, kblocks);
-  const bool lin = !halo && tc::linear_tiles();
-  int th = 16, tw = 8;
-  if (!halo) tc::pick_patch(ho, wo, &th, &tw);
-  const int lin_tiles = cdiv(n * ho * wo, tc::kBlockM);
-  const int m_tiles = lin ? lin_tiles : n * cdiv(ho, th) * cdiv(wo, tw);
-  const int bn = tc::pick_bn(cout, halo ? lin_tiles : m_tiles, kblocks);
-  out->mode = halo ? 2 : (lin ? 1 : 0);
-  out->bn = bn;
+  const tc::Tiling t = tc::pick_tiling(n, ho, wo, cin, cout, kh, kw, stride);
+  const int m_tiles = t.m_tiles;
+  out->mode = t.halo ? 2 : 1;
+  out->bn = t.bn;
   out->m_tiles = m_tiles;
-  out->n_tiles = cdiv(cout, bn);
+  out->n_tiles = cdiv(cout, t.bn);
   out->rounds = cdiv(m_tiles * out->n_tiles, tc::num_sms());
   const tc::Walk wk = tc::pick_walk(m_tiles, out->n_tiles);
   out->walk = wk.band > 1 ? 1 : 0;
   out->grid = wk.grid;
-  out->kblocks = kblocks;
-  out->patch_h = lin ? 0 : th;
-  out->patch_w = lin ? 0 : tw;
+  out->kblocks = t.kblocks;
+  out->patch_h = t.halo ? tc::kHaloTH : 0;
+  out->patch_w = t.halo ? tc::kHaloTW : 0;
   return SY_OK;
 }

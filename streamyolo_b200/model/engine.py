@@ -22,12 +22,6 @@ from .. import ops
 from ..ops import View
 
 
-# normalise pass inside the conv launch (1 launch / BaseConv).  One CTA per SM keeps fewer bytes in flight on the big tensors
-# than the separate pass, so SY_FUSE_APPLY=1 is a debug switch; SY_FUSE_APPLY_MAX_MB fuses only the layers whose raw output
-# is at most that many MB.  Off by default: bench.py's forward+loss step on an H100 80GB HBM3 at 400 W ran as fast or slower
-# with it (8 / 24 MB: 427 / 424 pairs/s against 427 with the 40 MB arena; 8 MB without the arena: 548 against 552-556)
-FUSE_APPLY = os.environ.get("SY_FUSE_APPLY", "0") != "0"
-FUSE_APPLY_MAX_BYTES = float(os.environ.get("SY_FUSE_APPLY_MAX_MB", "0")) * 1e6
 WEIGHT_EPOCH = 0  # bumped by whoever updates parameters through raw pointers (train.Trainer's fused optimiser kernel does
                   # not touch torch's version counters): part of every packed-operand cache key
 TRACE = None      # debugging: set to a dict to capture every BaseConv's stored output by module name
@@ -91,14 +85,14 @@ def _folded(m):
 
 
 SYNC_SLOTS = 1024
-_SYNC_POOLS = {}      # (device, stream) -> [int32 tensor of 4 * SYNC_SLOTS counters, next slot, scope depth]
+_SYNC_POOLS = {}      # (device, stream) -> [int32 tensor of 2 * SYNC_SLOTS counters, next slot, scope depth]
 
 
 def _sync_pool(device):
     key = (str(device), torch.cuda.current_stream().cuda_stream if torch.device(device).type == "cuda" else 0)
     st = _SYNC_POOLS.get(key)
     if st is None:
-        st = [torch.zeros(4 * SYNC_SLOTS, dtype=torch.int32, device=device), 0, 0]
+        st = [torch.zeros(2 * SYNC_SLOTS, dtype=torch.int32, device=device), 0, 0]
         _SYNC_POOLS[key] = st
     return st
 
@@ -118,7 +112,6 @@ class forward_scope:
     def __enter__(self):
         if self.st[2] == 0:
             self.st[1] = 0
-            _arm_raw_window(self.device)
         self.st[2] += 1
         return self
 
@@ -128,13 +121,13 @@ class forward_scope:
 
 
 def _sync(m, device):
-    """Four zeroed counters for one train-mode conv launch (two grid barriers + exit ticket), from the stream's pool."""
+    """Two zeroed counters for one train-mode conv launch (grid barrier + exit ticket), from the stream's pool."""
     st = _sync_pool(device)
     if st[1] == 0:
         st[0].zero_()
     i = st[1]
     st[1] = (i + 1) % SYNC_SLOTS
-    return st[0][4 * i:4 * i + 4]
+    return st[0][2 * i:2 * i + 2]
 
 
 def _bn_seg(m, c_begin=0):
@@ -142,62 +135,16 @@ def _bn_seg(m, c_begin=0):
     return (bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.num_batches_tracked, c_begin)
 
 
-# raw conv outputs of the plain (non-recording) train-mode forward: one arena per (device, stream), marked persisting in L2.
-# Off by default on H100: the persisting set-aside (at most 32.8 MB of the 50 MB L2) is taken from every other kernel's L2,
-# and the convs' operand re-reads lose more than the normalise passes gain.  bench.py's forward+loss step on an H100 80GB
-# HBM3 at 400 W, arena 0 / 24 / 40 MB: 526 / 476 / 399 pairs/s with the N-major tile walk; with a first version of the
-# M-band walk, 0 / 8 / 16 / 24 / 40 MB: 552-556 / 553 / 539 / 508 / 427 pairs/s (profiles/h100_l2_sweep.txt).
-RAW_ARENA_MB = float(os.environ.get("SY_RAW_ARENA_MB", "0"))
-_RAW_ARENAS = {}
-
-
-def _raw_view(ctx, n, h, w, c):
-    """The raw bf16 conv output of a train-mode BaseConv: dead as soon as its normalise pass has run, so every layer whose
-    tensor fits aliases ONE arena that the launching stream treats as a persisting-L2 window (sy_l2_persist_window)."""
-    nbytes = n * h * w * c * 2
-    if RAW_ARENA_MB <= 0 or torch.device(ctx.device).type != "cuda" or nbytes > RAW_ARENA_MB * 1e6:
-        return View.empty(n, h, w, c, ctx.device)
-    key = str(ctx.device)
-    st = _RAW_ARENAS.get(key)
-    if st is None:
-        if torch.cuda.is_current_stream_capturing():       # the device limit / stream attribute cannot be set during capture
-            return View.empty(n, h, w, c, ctx.device)
-        arena = torch.empty(int(RAW_ARENA_MB * 1e6) // 256 * 256, dtype=torch.uint8, device=ctx.device)
-        st = _RAW_ARENAS[key] = [arena, ops.l2_persist_window(arena)]
-    return View(st[0][:nbytes].view(torch.bfloat16).view(n, h, w, c))
-
-
-def _arm_raw_window(device):
-    """(re)apply the persisting window on the CURRENT stream (a forward may run on another stream than the one the arena was
-    created on).  Not during stream capture: capture on ``graph_capture_stream()``, which carries the window already."""
-    st = _RAW_ARENAS.get(str(device))
-    if st is not None and st[1] > 0 and not torch.cuda.is_current_stream_capturing():
-        ops.l2_persist_window(st[0])
-
-
 _CAPTURE_STREAMS = {}
 
 
 def graph_capture_stream(device):
-    """A side stream to capture CUDA graphs of the forward on (``torch.cuda.graph(g, stream=...)``): the persisting-L2 window of
-    the raw arena is set on it BEFORE the capture starts, so the captured kernel nodes inherit it."""
+    """The side stream to capture CUDA graphs of the forward on (``torch.cuda.graph(g, stream=...)``), one per device.  The
+    same stream on every call: the grid-barrier counter pool is kept per stream, so repeated captures share one pool."""
     key = str(device)
     if key not in _CAPTURE_STREAMS:
         _CAPTURE_STREAMS[key] = torch.cuda.Stream(device=device)
-    st = _CAPTURE_STREAMS[key]
-    with torch.cuda.stream(st):
-        _arm_raw_window(device)
-    return st
-
-
-def _dbg_skip_apply(nbytes):
-    """timing experiments only: SY_DBG_SKIP_APPLY="lo:hi" (MB) drops the normalise pass of the layers whose
-    raw output size lies in [lo, hi) -- the results are garbage, the step time shows what those launches really cost"""
-    e = os.environ.get("SY_DBG_SKIP_APPLY")
-    if not e:
-        return False
-    lo, hi = (float(v) for v in e.split(":"))
-    return lo * 1e6 <= nbytes < hi * 1e6
+    return _CAPTURE_STREAMS[key]
 
 
 def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, act=1, y_goff1=0, res_goff1=0, impl=None,
@@ -205,15 +152,15 @@ def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, a
     """Train mode: conv -> batch statistics -> BatchNorm (running-stat update) -> act (+res) into ``y``.
     Tensor-core path = 2 launches: the conv writes the raw bf16 result, accumulates the statistics and
     (grid barrier + parallel reduce in its tail) publishes scale/shift; then the normalise pass.  ``mods``: one BaseConv, or two whose
-    outputs are concatenated along channels (CSPLayer conv1 | conv2).  With a tape the raw output goes to a fresh buffer
-    and the conv also writes the batch mean / inverse std: the backward reads both.  ``kind="stem"``: the Focus stem, whose
+    outputs are concatenated along channels (CSPLayer conv1 | conv2).  With a tape the conv also writes the batch mean /
+    inverse std: the backward reads them and the raw output.  ``kind="stem"``: the Focus stem, whose
     input needs no gradient."""
     kh, kw = (k, k) if isinstance(k, int) else k
     ho = (x.h + 2 * ((kh - 1) // 2) - kh) // s + 1
     wo = (x.w + 2 * ((kw - 1) // 2) - kw) // s + 1
     cout = sum(m.conv.out_channels for m in mods)
     T = ctx.tape
-    raw = _raw_view(ctx, x.n, ho, wo, cout) if T is None else View.empty(x.n, ho, wo, cout, ctx.device)
+    raw = View.empty(x.n, ho, wo, cout, ctx.device)
     bn0 = mods[0].bn
     mom = float(0.1 if bn0.momentum is None else bn0.momentum)
     n = x.n
@@ -229,16 +176,9 @@ def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, a
             c0 += m.conv.out_channels
         ss = torch.empty((2, 2, cout), dtype=torch.float32, device=ctx.device)
         mi = None if T is None else torch.empty((2, 2, cout), dtype=torch.float32, device=ctx.device)
-        if T is None and (FUSE_APPLY or n * ho * wo * cout * 2 <= FUSE_APPLY_MAX_BYTES):
-            ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl="tc", partials=partials, split_n=split, bn=segs,
-                       momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device), act=act,
-                       apply_y=y, apply_res=res, y_goff1=y_goff1, res_goff1=res_goff1)
-        else:
-            ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl="tc", partials=partials, split_n=split, bn=segs,
-                       momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device), mean_invstd=mi)
-            if T is not None or not _dbg_skip_apply(n * ho * wo * cout * 2):
-                ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), split if split else n, act, res, y, y_goff1,
-                                 res_goff1)
+        ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl="tc", partials=partials, split_n=split, bn=segs,
+                   momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device), mean_invstd=mi)
+        ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), split if split else n, act, res, y, y_goff1, res_goff1)
         if T is not None:
             T.rec(t="conv", mods=mods, x=x, k=(kh, kw), s=s, raw=raw, y=y, res=res, ss=ss, mi=mi, split=split, act=act,
                   kind=kind)

@@ -30,10 +30,7 @@ class SyConvDesc(C.Structure):
                 ("shift", C.c_void_p), ("res", SyTensor), ("split_n", C.c_int32), ("stat_partials", C.c_void_p),
                 ("n_partials", C.c_int32), ("rows_written", C.POINTER(C.c_int32)), ("bn", SyBnSegment * 2),
                 ("momentum", C.c_float), ("eps", C.c_float), ("scale_shift", C.c_void_p), ("mean_invstd", C.c_void_p),
-                ("sync", C.c_void_p),
-                ("apply_y", SyTensor), ("apply_res", SyTensor), ("apply_y_group1_offset", C.c_int64),
-                ("apply_res_group1_offset", C.c_int64),
-                ("debug_timeline", C.c_void_p),
+                ("sync", C.c_void_p), ("debug_timeline", C.c_void_p),
                 ("debug_timeline_events", C.c_int32), ("debug_flags", C.c_int32), ("debug_f32", C.c_void_p)]
 
 
@@ -120,7 +117,6 @@ _SIG = {
     "sy_version": (C.c_int, []),
     "sy_check_device": (C.c_int, []),
     "sy_conv_stat_rows": (C.c_int, []),
-    "sy_l2_persist_window": (C.c_int, [C.c_void_p, C.c_size_t, C.c_float, C.POINTER(C.c_size_t), C.c_void_p]),
     "sy_conv2d_tc": (C.c_int, [C.POINTER(SyConvDesc), C.c_void_p]),
     "sy_conv2d_plan": (C.c_int, [C.c_int32] * 8 + [C.POINTER(SyConvPlan)]),
     "sy_conv2d_simt": (C.c_int, [C.POINTER(SyConvDesc), C.c_void_p]),
@@ -303,7 +299,7 @@ def conv_stat_rows():
 
 def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None, act=1, res: View = None,
            partials=None, split_n=0, timeline=None, debug_flags=0, bn=None, momentum=0.03, eps=1e-3, scale_shift=None,
-           sync=None, apply_y: View = None, apply_res: View = None, y_goff1=0, res_goff1=0, mean_invstd=None, debug_f32=None):
+           sync=None, mean_invstd=None, debug_f32=None):
     """``k`` is an int (square) or (kh, kw).  With ``partials`` (RAW mode, tensor-core path) returns the number
     of per-CTA statistic rows the launch writes."""
     d = SyConvDesc()
@@ -330,10 +326,6 @@ def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None,
         d.momentum, d.eps = momentum, eps
         d.scale_shift, d.sync = scale_shift.data_ptr(), sync.data_ptr()
         d.mean_invstd = mean_invstd.data_ptr() if mean_invstd is not None else None
-        if apply_y is not None:
-            d.apply_y = apply_y.st()
-            d.apply_res = apply_res.st() if apply_res is not None else NULL_T
-            d.apply_y_group1_offset, d.apply_res_group1_offset = y_goff1, res_goff1
     d.debug_flags = debug_flags
     d.debug_f32 = debug_f32.data_ptr() if debug_f32 is not None else None
     if timeline is not None:
@@ -614,17 +606,6 @@ def scale_labels_(labels, sx, sy):
     cols = labels.shape[-1]
     _check(lib().sy_scale_labels(labels.data_ptr(), labels.numel() // cols, cols, sx, sy, _stream()))
     return labels
-
-
-def l2_persist_window(t, hit_ratio=1.0):
-    """Persisting-L2 window over tensor ``t`` (None: clear) for the kernels launched on the current stream; returns the
-    number of bytes the device granted."""
-    got = C.c_size_t(0)
-    if t is None:
-        _check(lib().sy_l2_persist_window(None, 0, 0.0, C.byref(got), _stream()), kernels=0)
-        return 0
-    _check(lib().sy_l2_persist_window(t.data_ptr(), t.numel() * t.element_size(), hit_ratio, C.byref(got), _stream()), kernels=0)
-    return got.value
 
 
 class PackBatch:

@@ -145,22 +145,24 @@ def test_struct_layouts_match_header(tmp_path):
         assert int(v) == want, f"{n}.{f}: header {v}, ctypes {want}"
 
 
-def test_conv_plan_query_without_gpu(monkeypatch):
+def test_conv_tiling_plan_without_gpu(monkeypatch):
     """sy_conv2d_plan is host-only: the tiling decisions of the tensor-core conv can be inspected (and are pinned here for the
     layers that motivated them) without a device.  132 SMs (an H100 SXM) are assumed when no GPU is present."""
-    monkeypatch.delenv("SY_CONV_TILES", raising=False)
     monkeypatch.delenv("SY_CONV_A", raising=False)
-    p = ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1)          # linear tiles: 285 x 2 tiles = 5 rounds (patch tiles: 304 x 2)
+    p = ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1)          # linear tiles: 285 x 2 tiles = 5 rounds
     assert (p["mode"], p["bn"], p["m_tiles"], p["rounds"]) == (1, 128, 285, 5)
     p = ops.conv2d_plan(16, 19, 30, 512, 512, 3, 1)          # 72 x 4 tiles: three rounds
     assert (p["mode"], p["bn"], p["rounds"]) == (1, 128, 3)
     p = ops.conv2d_plan(16, 75, 120, 128, 128, 3, 1)         # BN = 128 on a large map: halo mode, 16 x 8 patches
     assert (p["mode"], p["bn"], p["patch_h"], p["patch_w"], p["kblocks"]) == (2, 128, 16, 8, 18)
     p = ops.conv2d_plan(16, 75, 120, 128, 128, 1, 1)         # 1x1: never halo
-    assert p["mode"] == 1 and p["kblocks"] == 2
-    monkeypatch.setenv("SY_CONV_TILES", "patch")
+    assert (p["mode"], p["kblocks"], p["patch_h"], p["patch_w"]) == (1, 2, 0, 0)
+    monkeypatch.setenv("SY_CONV_A", "off")                    # halo disabled: the halo layer above on linear tiles
+    p = ops.conv2d_plan(16, 75, 120, 128, 128, 3, 1)
+    assert (p["mode"], p["m_tiles"], p["patch_h"], p["patch_w"]) == (1, (16 * 75 * 120 + 127) // 128, 0, 0)
+    monkeypatch.setenv("SY_CONV_A", "halo")                   # halo forced: 16 x 8 patches of the 38 x 60 map
     p = ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1)
-    assert p["mode"] == 0 and p["m_tiles"] == 304 and p["rounds"] == 5
+    assert (p["mode"], p["m_tiles"], p["patch_h"], p["patch_w"]) == (2, 16 * 3 * 8, 16, 8)
     with pytest.raises(RuntimeError):
         ops.conv2d_plan(1, 8, 8, 8, 8, 5, 1)
 

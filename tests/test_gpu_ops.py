@@ -48,18 +48,20 @@ def check_close(got, ref, what, ulp=2.0 ** -7):
     return rel
 
 
-# SY_TEST_TILES=linear|patch|halo restricts the tensor-core variants under test (bring-up aid); default: all
+# SY_TEST_TILES=linear|halo restricts the tensor-core variants under test (bring-up aid); default: all
 _T = os.environ.get("SY_TEST_TILES", "all")
-_ALL = {"tc": "linear", "tc_patch": "patch", "tc_halo": "halo"}
+_ALL = {"tc": "linear", "tc_bn64": "linear", "tc_halo": "halo"}
 TC_IMPLS = [i for i, t in _ALL.items() if _T in ("all", "both", t)]
 
 
 def tc_impl(impl, monkeypatch):
-    """'tc' = linear M tiles (im2col-mode TMA, the default), 'tc_patch' = rectangular patch tiles, 'tc_halo' = one halo
-    load per tile and channel block for the 3x3 stride-1 convs (linear tiles elsewhere); all are product paths."""
+    """'tc' = linear M tiles (im2col-mode TMA, the default), 'tc_bn64' = linear tiles with the tile width forced to 64
+    (the BN = 64 kernel on layers the planner gives BN = 128, i.e. several N tiles and the M-band walk), 'tc_halo' = one
+    halo load per tile and channel block for the 3x3 stride-1 convs (linear tiles elsewhere); all are product paths."""
     if impl.startswith("tc"):
-        monkeypatch.setenv("SY_CONV_TILES", "patch" if impl == "tc_patch" else "linear")
         monkeypatch.setenv("SY_CONV_A", "halo" if impl == "tc_halo" else "off")
+        if impl == "tc_bn64":
+            monkeypatch.setenv("SY_CONV_BN", "64")
         return "tc"
     return impl
 
@@ -118,7 +120,7 @@ def test_conv_raw(case, impl, monkeypatch):
 
 
 @pytest.mark.parametrize("tiles", TC_IMPLS)
-def test_conv_tc_bn_finalize_then_apply(tiles, monkeypatch):
+def test_conv_tc_bn_finalize_then_separate_apply(tiles, monkeypatch):
     tc_impl(tiles, monkeypatch)
     _bn_finalize_then_apply()
 
@@ -126,7 +128,8 @@ def test_conv_tc_bn_finalize_then_apply(tiles, monkeypatch):
 def _bn_finalize_then_apply():
     """RAW conv that also finalizes BatchNorm in its tail (grid barrier + parallel reduce; two groups, two
     parameter segments, running statistics), then the normalise pass with SiLU + residual; against
-    F.batch_norm on the stored conv output.  The sync counters must come back to zero (graph replay safe)."""
+    F.batch_norm on the stored conv output.  Three launches in a row: the sync counters must come back to zero after each
+    (graph replay safe) and num_batches_tracked must count two statistics groups per launch."""
     n, ci, co, h, w = 4, 64, 128, 19, 30
     x, wt = rand_act(n, ci, h, w, 61), rand_w(co, ci, 1, 62)
     g = torch.Generator().manual_seed(63)
@@ -142,19 +145,16 @@ def _bn_finalize_then_apply():
     resid = rand_act(n, co, h, w, 64)
     partials = torch.empty((ops.conv_stat_rows(), 4 * co), device=DEV)
     ss = torch.empty((2, 2, co), device=DEV)
-    sync = torch.zeros(4, dtype=torch.int32, device=DEV)
+    sync = torch.zeros(2, dtype=torch.int32, device=DEV)
     resid_v, x_v = ops.from_nchw(resid), ops.from_nchw(x)
     for rep in range(3):
-        fused = rep == 2        # last repetition: normalise pass inside the conv launch
         y.buf.fill_(float("nan"))
         rows = ops.conv2d(x_v, ops.pack_conv_weight(wt), raw, 1, 1, ops.SY_CONV_RAW, partials=partials,
-                          split_n=2, bn=segs, momentum=0.03, eps=1e-3, scale_shift=ss, sync=sync, act=1,
-                          apply_y=y if fused else None, apply_res=resid_v if fused else None)
+                          split_n=2, bn=segs, momentum=0.03, eps=1e-3, scale_shift=ss, sync=sync, act=1)
         assert 1 <= rows <= ops.conv_stat_rows()
-        if not fused:
-            ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), 2, 1, resid_v, y)
+        ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), 2, 1, resid_v, y)
         torch.cuda.synchronize()
-        assert sync.tolist() == [0, 0, 0, 0]
+        assert sync.tolist() == [0, 0]
         rawf = raw.nchw_float()
         refs = []
         for gi in range(2):
@@ -420,7 +420,7 @@ def test_baseconv_backward_chain(case):
     raw2 = View.empty(n, h, w, co, DEV)
     ops.conv2d(xv, ops.pack_conv_weight(wt), raw2, k, 1, ops.SY_CONV_RAW, split_n=split,
                partials=torch.empty((ops.conv_stat_rows(), 4 * co), device=DEV), bn=[(gamma, beta, rm, rv, nbt, 0)],
-               momentum=0.03, eps=eps, scale_shift=ss, sync=torch.zeros(4, dtype=torch.int32, device=DEV), mean_invstd=mi)
+               momentum=0.03, eps=eps, scale_shift=ss, sync=torch.zeros(2, dtype=torch.int32, device=DEV), mean_invstd=mi)
     torch.cuda.synchronize()
     ng = len(groups)
     assert torch.equal(raw2.torch(), raw.torch())

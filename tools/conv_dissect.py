@@ -1,12 +1,11 @@
 """Dissect the conv pipeline: time a shape (CUDA graph of 20 back-to-back launches, so host launch cost is
 excluded) as it runs and with the TMA loads switched off (debug flag 2: the barriers still cycle, the MMAs read stale
 shared memory).  The gap between the two is what operand supply costs the shape.  The plan column is the A mode
-(0 patch, 1 linear, 2 halo) and the tile width.
-L2 state: no model runs first.  With SY_RAW_ARENA_MB > 0 (the step's default) the output is drawn from the step's
-raw-output arena when it fits and the graphs are captured on the stream that carries its persisting window, as in the
-step; SY_RAW_ARENA_MB=0 times with no persisting set-aside.  The header line states what was granted.
+(1 linear, 2 halo) and the tile width.
+L2 state: no model runs first, and there is no persisting-L2 set-aside (the library never asks for one).  The graphs are
+captured on the step's capture stream.
     usage: python tools/conv_dissect.py"""
-import os, sys, types
+import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from streamyolo_b200 import ops
@@ -19,7 +18,7 @@ def run(n, ci, co, h, w, k, s, flags, mode=ops.SY_CONV_RAW):
     x = View(torch.randn((n, h, w, ci), device="cuda").to(torch.bfloat16))
     wt = ops.pack_conv_weight(torch.randn((co, ci, k, k), device="cuda") * 0.05)
     ho, wo = ops.conv_out_hw(h, w, k, s)
-    y = engine._raw_view(types.SimpleNamespace(device=DEV), n, ho, wo, co)
+    y = View.empty(n, ho, wo, co, DEV)
     part = torch.empty((ops.conv_stat_rows(), 4 * co), device="cuda") if mode == ops.SY_CONV_RAW else None
     def go():
         ops.conv2d(x, wt, y, k, s, mode, partials=part, split_n=n // 2, debug_flags=flags)
@@ -49,10 +48,6 @@ if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "stages":
         print(shape, " ".join(f"S={a}: full {b:.1f} no-TMA {c:.1f} |" for a, b, c in row))
     sys.exit(0)
 if __name__ == "__main__":
-    run(*SHAPES[0], 0)                                      # creates the arena (if any) before the header reports it
-    arena = engine._RAW_ARENAS.get(str(DEV))
-    print(f"L2 state: no model run; raw-output arena {engine.RAW_ARENA_MB:g} MB, persisting window granted "
-          f"{arena[1] if arena else 0} bytes")
     for shape in SHAPES:
         t = [run(*shape, f) for f in (0, 2)]
         n, ci, co, h, w, k, s = shape

@@ -1,6 +1,6 @@
 """Per-layer tiling plan of one training-forward step (no GPU needed): dry-runs the engine with the kernels mocked
 (tools/op_sequence.py) and asks the library's host-only planner (sy_conv2d_plan) what sy_conv2d_tc does for each conv:
-A-operand mode (patch / linear = im2col-mode TMA / halo), tile width, tiles, rounds of the persistent grid (one CTA per SM).
+A-operand mode (linear = im2col-mode TMA / halo), tile width, tiles, rounds of the persistent grid (one CTA per SM).
 
     python tools/conv_plan.py [model] [pairs]"""
 import os
@@ -17,7 +17,7 @@ import op_sequence  # noqa: E402
 model = sys.argv[1] if len(sys.argv) > 1 else "l"
 batch = int(sys.argv[2]) if len(sys.argv) > 2 else 8
 seq = [s for s in op_sequence.sequence(model, batch) if s["kind"] == "conv"]
-MODE = {0: "patch", 1: "linear", 2: "halo"}
+MODE = {1: "linear", 2: "halo"}
 print(f"StreamYOLO-{model}, {batch} frame pairs: {len(seq)} conv launches per step")
 WALK = {0: "N-major", 1: "M-band"}
 print(f"{'layer':50s} {'shape':34s} {'mode':7s} {'BN':>4s} {'tiles':>6s} {'rounds':>6s} {'K blk':>6s} {'fill':>5s} "

@@ -3,16 +3,13 @@ workload: the train-mode conv (wgmma kernel with statistics + BatchNorm finalize
 R times back to back in one graph (PDL edges like the real step), next to the layer's roofline time
 max(FLOPs / tensor peak, algorithmic bytes / HBM peak).  The sum over the step's launches is compared with bench.py.
 
-L2 state: the same as bench.py's step.  The model's forward runs first (it creates the raw-output arena, and with it the
-device's persisting-L2 set-aside); every raw conv output that fits is drawn from that arena, and the graphs are captured
-on engine.graph_capture_stream, which carries the arena's persisting window.  SY_RAW_ARENA_MB sets the arena as it does
-for the step (0: no arena, no set-aside).  The header line states what was granted.
+L2 state: the same as bench.py's step.  The model's forward runs first, there is no persisting-L2 set-aside (the library
+never asks for one), and the graphs are captured on engine.graph_capture_stream like the step's.
 
     python tools/layer_graph_bench.py [model] [pairs] [reps]"""
 import collections
 import os
 import sys
-import types
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -79,9 +76,6 @@ for c in calls:
     groups.setdefault(key, []).append(c)
 
 print(f"StreamYOLO-{tag}, {B} pairs: {len(calls)} BaseConv launches, {len(groups)} distinct; in-graph us per launch ({R} reps back to back)")
-arena = engine._RAW_ARENAS.get(str(dev))
-print(f"L2 state: model forward ran first; raw-output arena {engine.RAW_ARENA_MB:g} MB, persisting window granted "
-      f"{arena[1] if arena else 0} bytes; graphs captured on the step's capture stream")
 print(f"{'shape':44s} {'x':>3s} {'conv':>8s} {'apply':>8s} {'both':>8s} {'roof':>7s} {'TF/s':>7s} {'GB/s':>6s}  first layer")
 tot = dict(conv=0.0, apply=0.0, both=0.0, roof=0.0)
 for key, cs in groups.items():
@@ -89,7 +83,7 @@ for key, cs in groups.items():
     n, h, w, cin, cout, (kh, kw), s = c["n"], c["h"], c["w"], c["cin"], c["cout"], c["k"], c["s"]
     ho, wo = (h + 2 * ((kh - 1) // 2) - kh) // s + 1, (w + 2 * ((kw - 1) // 2) - kw) // s + 1
     xin = View(torch.randn((n, h, w, cin), device=dev).to(torch.bfloat16))
-    raw, y = engine._raw_view(types.SimpleNamespace(device=dev), n, ho, wo, cout), View.empty(n, ho, wo, cout, dev)
+    raw, y = View.empty(n, ho, wo, cout, dev), View.empty(n, ho, wo, cout, dev)
     resv = View(torch.randn((n, ho, wo, cout), device=dev).to(torch.bfloat16)) if c["res"] else None
     mods, wpk = c["mods"], c["wpk"]
     partials = torch.empty((ops.conv_stat_rows(), 4 * cout), dtype=torch.float32, device=dev)
