@@ -385,6 +385,42 @@ int sy_resize_bilinear(const float* x, int32_t nc, int32_t hi, int32_t wi, float
                        sy_stream_t stream);
 int sy_scale_labels(float* labels, int64_t rows, int32_t cols, float sx, float sy, sy_stream_t stream);
 
+/* -------- input transforms (streamyolo_b200/csrc/input.cu) ------------------------------------------------------ */
+/* Label half of DoubleTrainTransform(max_labels, hsv=False, flip) (exps/data/data_augment_flip.py:141-148, 176-234) for
+ * n_items frame pairs, one warp per frame, in fp64 with one final cast to fp32: mirror the boxes (x1' = width - x2,
+ * x2' = width - x1) when flip && mirror[item] && the frame has rows, xyxy -> cxcywh, * r, keep rows with min(w, h) > 1;
+ * if none survive, the unmirrored, unfiltered rows instead.  Rows past max_labels are dropped, the rest is zero.
+ * flags_out receives each frame's effective mirror bit, which sy_letterbox reads: launch this first on the same stream. */
+typedef struct SyPairLabelsDesc {
+  const double* ann;       /* [n_items][2][max_rows][5] x1, y1, x2, y2, cls (frame 0 = current image, future boxes) */
+  const int32_t* counts;   /* [n_items][2] valid rows of each frame (clamped to [0, max_rows]) */
+  const int32_t* mirror;   /* [n_items] the pair's mirror bit (may be NULL when flip == 0) */
+  int32_t n_items, max_rows, max_labels, flip;
+  int32_t width;           /* width of the frame entering the transform: the mirror axis */
+  double r;                /* letterbox scale min(H / h, W / w) */
+  float* labels_fut;       /* [n_items][max_labels][5] cls, cx, cy, w, h of frame 0 */
+  float* labels_cur;       /* [n_items][max_labels][5] of frame 1 */
+  int32_t* flags_out;      /* [n_items][2] */
+} SyPairLabelsDesc;
+int sy_pair_labels(const SyPairLabelsDesc* d, sy_stream_t stream);
+
+/* Image half: uint8 HWC BGR frames [n][h][w][3] -> fp32 planar [n][3][out_h][out_w] (a [B][6][H][W] pair batch when
+ * n = 2B).  Each frame goes through cv2.resize(INTER_LINEAR) h x w -> mid_h x mid_w (load_resized_img,
+ * exps/dataset/tal_flip_one_future_argoversedataset.py:179-187; none when mid == h x w), the mirror when flags[i] is
+ * set, cv2.resize mid -> dst_h x dst_w (preproc, data_augment_flip.py:151-167; none when dst == mid), top-left on a canvas
+ * of 114, bit-identical to OpenCV's 8-bit fixed-point bilinear resize.  With dst == out and no flags it is the streaming
+ * driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60, 176-181). */
+typedef struct SyLetterboxDesc {
+  const uint8_t* src;      /* [n][h][w][3] */
+  int32_t n, h, w;
+  int32_t mid_h, mid_w;
+  int32_t dst_h, dst_w;
+  int32_t out_h, out_w;
+  const int32_t* flags;    /* [n] mirror bits, or NULL */
+  float* out;              /* [n][3][out_h][out_w] */
+} SyLetterboxDesc;
+int sy_letterbox(const SyLetterboxDesc* d, sy_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

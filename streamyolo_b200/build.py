@@ -17,7 +17,7 @@ NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = "arch=compute_90a,code=sm_90a"      # H100 (Hopper): wgmma, TMA, mbarrier
 COMMON = ["-gencode", ARCH, "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
           "--use_fast_math=false" if False else "-DSY_BUILD", "-Xptxas", "-v"]
-# per-file extra flags: the loss/decode unit must evaluate reference expressions without FMA contraction
+# per-file extra flags: the loss/decode and input-transform units must evaluate reference expressions without FMA contraction
 SOURCES = {
     "api.cu": [],
     "conv_tc.cu": [],
@@ -30,6 +30,7 @@ SOURCES = {
     "train_glue.cu": [],
     "head_loss.cu": ["-fmad=false"],
     "postprocess.cu": ["-fmad=false"],
+    "input.cu": ["-fmad=false"],
 }
 
 

@@ -1,0 +1,66 @@
+"""The data loader's image transforms on the device, from the uint8 BGR frames the dataset holds to the model's input.
+
+``pair_transform`` = DoubleTrainTransform(max_labels, hsv=False, flip) / DoubleValTransform
+(/root/reference/exps/data/data_augment_flip.py:141-234) for a batch of frame pairs, ``stream_frame`` = the streaming
+driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60, 176-181).  Both are bit-identical to the cv2 / numpy host code
+they replace (sy_pair_labels, sy_letterbox); INTEGRATION.md shows where they plug in.
+"""
+import torch
+
+from . import ops
+
+
+def _fit(h, w, size):
+    """the scale and (int-truncated) size of an h x w image fitted into ``size`` (preproc, load_resized_img)"""
+    r = min(size[0] / h, size[1] / w)
+    return r, (int(h * r), int(w * r))
+
+
+def pair_transform(frames, ann, counts, mirror, input_size, max_labels=50, flip=True, raw=False, hsv=False, out=None):
+    """Train / validation transform of a batch of frame pairs.
+
+    frames  uint8 CUDA [B, 2, h, w, 3], BGR, current frame first: the two images of ``pull_item`` (``raw=True``: what
+            cv2.imread returned, and load_resized_img's resize runs first)
+    ann     float64 [B, 2, M, 5] rows x1, y1, x2, y2, cls as ``pull_item`` scales them (frame 0: the future boxes), or None
+            for the validation transform (no labels, no mirror)
+    counts  int32 [B, 2] valid rows of ``ann``
+    mirror  int32 [B] the pair's random mirror bit (``random.randrange(2)`` of DoubleTrainTransform)
+    out     ``(x, (labels_fut, labels_cur))`` of an earlier call to write into (static buffers for CUDA-graph capture)
+
+    -> ``(x, (labels_fut, labels_cur))``: x fp32 [B, 6, H, W], labels fp32 [B, max_labels, 5] (cls, cx, cy, w, h), or
+    ``(x, None)`` without annotations.  Nothing is read back to the host."""
+    if hsv:
+        raise NotImplementedError("pair_transform: HSV augmentation has no device implementation (no TAL cfg enables it)")
+    ops._require(torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 5 and frames.shape[1] == 2
+                 and frames.shape[4] == 3 and frames.is_contiguous(), "pair_transform: frames must be contiguous uint8 [B, 2, h, w, 3]")
+    b, _, h, w, _ = frames.shape
+    mid = _fit(h, w, input_size)[1] if raw else (h, w)
+    r, dst = _fit(mid[0], mid[1], input_size)
+    if out is None:
+        x = torch.empty((b, 6, input_size[0], input_size[1]), dtype=torch.float32, device=frames.device)
+        labels = None
+        if ann is not None:
+            labels = tuple(torch.empty((b, max_labels, 5), dtype=torch.float32, device=frames.device) for _ in range(2))
+    else:
+        x, labels = out
+    ops._require(tuple(x.shape) == (b, 6, input_size[0], input_size[1]), "pair_transform: out image must be [B, 6, H, W]")
+    flags = None
+    if ann is not None:
+        ops._require(labels is not None and labels[0].shape[1] == max_labels, "pair_transform: out labels must be [B, max_labels, 5]")
+        flags = torch.empty((b, 2), dtype=torch.int32, device=frames.device)
+        ops.pair_labels(ann, counts, mirror if flip else None, flip, mid[1], r, labels[0], labels[1], flags)
+    ops.letterbox(frames.view(2 * b, h, w, 3), mid, dst, x, flags)
+    return x, labels
+
+
+def stream_frame(frame, size=(600, 960), out=None):
+    """streamyolo_det.preproc(frame, size) followed by torch.from_numpy(.).float()[None]: uint8 CUDA [h, w, 3] BGR ->
+    fp32 [1, 3, H, W], a plain (possibly non-uniform) cv2-exact resize without pad or mirror."""
+    ops._require(torch.is_tensor(frame) and frame.dtype == torch.uint8 and frame.dim() == 3 and frame.shape[2] == 3
+                 and frame.is_contiguous(), "stream_frame: frame must be contiguous uint8 [h, w, 3]")
+    h, w, _ = frame.shape
+    if out is None:
+        out = torch.empty((1, 3, size[0], size[1]), dtype=torch.float32, device=frame.device)
+    ops._require(tuple(out.shape) == (1, 3, size[0], size[1]), "stream_frame: out must be [1, 3, H, W]")
+    ops.letterbox(frame.view(1, h, w, 3), (h, w), size, out)
+    return out

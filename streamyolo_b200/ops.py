@@ -111,6 +111,18 @@ class SyTalLossBwdDesc(C.Structure):
                 ("grad_outputs", C.c_void_p), ("grad_origin", C.c_void_p), ("grad_raw", C.c_void_p)]
 
 
+class SyPairLabelsDesc(C.Structure):
+    _fields_ = [("ann", C.c_void_p), ("counts", C.c_void_p), ("mirror", C.c_void_p), ("n_items", C.c_int32),
+                ("max_rows", C.c_int32), ("max_labels", C.c_int32), ("flip", C.c_int32), ("width", C.c_int32),
+                ("r", C.c_double), ("labels_fut", C.c_void_p), ("labels_cur", C.c_void_p), ("flags_out", C.c_void_p)]
+
+
+class SyLetterboxDesc(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("mid_h", C.c_int32),
+                ("mid_w", C.c_int32), ("dst_h", C.c_int32), ("dst_w", C.c_int32), ("out_h", C.c_int32),
+                ("out_w", C.c_int32), ("flags", C.c_void_p), ("out", C.c_void_p)]
+
+
 # every symbol include/streamyolo_sm100.h declares: (restype, argtypes)
 _SIG = {
     "sy_last_error_string": (C.c_char_p, []),
@@ -159,6 +171,8 @@ _SIG = {
     "sy_resize_bilinear": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                                      C.c_void_p]),
     "sy_scale_labels": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_float, C.c_void_p]),
+    "sy_pair_labels": (C.c_int, [C.POINTER(SyPairLabelsDesc), C.c_void_p]),
+    "sy_letterbox": (C.c_int, [C.POINTER(SyLetterboxDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
 
@@ -606,6 +620,52 @@ def scale_labels_(labels, sx, sy):
     cols = labels.shape[-1]
     _check(lib().sy_scale_labels(labels.data_ptr(), labels.numel() // cols, cols, sx, sy, _stream()))
     return labels
+
+
+def _require(cond, msg):
+    if not cond:
+        raise RuntimeError(msg)
+
+
+def _tensor_ok(t, dtype, dim):
+    return torch.is_tensor(t) and t.dtype == dtype and t.dim() == dim and t.is_contiguous()
+
+
+def pair_labels(ann, counts, mirror, flip, width, r, labels_fut, labels_cur, flags):
+    """Label half of DoubleTrainTransform on the device (sy_pair_labels): ``ann`` fp64 [B, 2, M, 5] (x1, y1, x2, y2, cls),
+    ``counts`` int32 [B, 2], ``mirror`` int32 [B] (or None without flip); writes fp32 [B, max_labels, 5] ``labels_fut`` /
+    ``labels_cur`` and the int32 [B, 2] effective mirror bits ``flags``."""
+    _require(_tensor_ok(ann, torch.float64, 4) and ann.shape[1] == 2 and ann.shape[3] == 5,
+             "pair_labels: annotations must be contiguous float64 [B, 2, M, 5]")
+    b = ann.shape[0]
+    _require(_tensor_ok(counts, torch.int32, 2) and tuple(counts.shape) == (b, 2), "pair_labels: counts must be int32 [B, 2]")
+    _require(mirror is None or (_tensor_ok(mirror, torch.int32, 1) and mirror.shape[0] == b),
+             "pair_labels: mirror must be int32 [B]")
+    for t in (labels_fut, labels_cur):
+        _require(_tensor_ok(t, torch.float32, 3) and t.shape[0] == b and t.shape[2] == 5 and t.shape == labels_fut.shape,
+                 "pair_labels: labels must be float32 [B, max_labels, 5]")
+    _require(_tensor_ok(flags, torch.int32, 2) and tuple(flags.shape) == (b, 2), "pair_labels: flags must be int32 [B, 2]")
+    d = SyPairLabelsDesc()
+    d.ann, d.counts = ann.data_ptr(), counts.data_ptr()
+    d.mirror = mirror.data_ptr() if mirror is not None else None
+    d.n_items, d.max_rows, d.max_labels, d.flip = b, ann.shape[2], labels_fut.shape[1], int(flip)
+    d.width, d.r = width, r
+    d.labels_fut, d.labels_cur, d.flags_out = labels_fut.data_ptr(), labels_cur.data_ptr(), flags.data_ptr()
+    _check(lib().sy_pair_labels(C.byref(d), _stream()))
+
+
+def letterbox(src, mid, dst, out, flags=None):
+    """uint8 [n, h, w, 3] frames -> fp32 [n * 3 / C, C, H, W] ``out`` (sy_letterbox): cv2-exact resize to ``mid`` (h, w),
+    mirror where int32 ``flags[i]`` is set, cv2-exact resize to ``dst``, top-left on a canvas of 114."""
+    _require(_tensor_ok(src, torch.uint8, 4) and src.shape[3] == 3, "letterbox: frames must be contiguous uint8 [n, h, w, 3]")
+    n, h, w, _ = src.shape
+    _require(_tensor_ok(out, torch.float32, 4) and out.numel() == n * 3 * out.shape[2] * out.shape[3],
+             "letterbox: out must be contiguous float32 holding [n, 3, H, W]")
+    _require(flags is None or (torch.is_tensor(flags) and flags.dtype == torch.int32 and flags.is_contiguous()
+                               and flags.numel() == n), "letterbox: flags must be int32 [n]")
+    d = SyLetterboxDesc(src.data_ptr(), n, h, w, mid[0], mid[1], dst[0], dst[1], out.shape[2], out.shape[3],
+                        flags.data_ptr() if flags is not None else None, out.data_ptr())
+    _check(lib().sy_letterbox(C.byref(d), _stream()))
 
 
 class PackBatch:

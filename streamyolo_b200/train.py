@@ -388,12 +388,13 @@ class Trainer:
         return backward._loss_dict(loss)
 
     # ---- the whole step as CUDA graph(s) (the eager step is bound by the host's launch rate: ~800-1300 launches)
-    def capture(self, x, targets, loss_scale=1.0):
+    def capture(self, x, targets, loss_scale=1.0, prologue=None):
         """Capture forward + backward + weight re-pack + optimiser step on static input buffers (``x`` / ``targets`` become the
         graph's inputs: copy new data into them, then ``replay(lr)``).  One process: ONE graph.  Several ranks: the walk is cut
         into one graph segment per gradient bucket; between two segments the host enqueues that bucket's NCCL all-reduce on the
         communication stream, where it overlaps the following segments (the collectives themselves stay outside the
-        captured graphs); a last segment holds the optimiser step."""
+        captured graphs); a last segment holds the optimiser step.  ``prologue``: a callable captured at the front of the
+        graph, e.g. ``data.pair_transform(..., out=(x, targets))`` so that the static inputs are the uint8 frames."""
         dev = self.fs.state.device
         self._hyper = torch.zeros(8, dtype=torch.float32, device=dev)
         self._hyper_host = torch.zeros(8, dtype=torch.float32).pin_memory()
@@ -401,6 +402,8 @@ class Trainer:
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):                      # warm-up on a side stream (allocator, lazy module attributes)
+            if prologue is not None:
+                prologue()
             self._set_hyper(None)
             self.forward_backward(x, targets, loss_scale)
             self.optimizer_step(hyper=self._hyper)
@@ -423,6 +426,8 @@ class Trainer:
         self.sink.on_bucket = cut if self.world > 1 else None
         with torch.cuda.stream(side):
             begin()
+            if prologue is not None:
+                prologue()
             loss = self.forward_backward(x, targets, loss_scale)
             if self.world > 1:                             # the optimiser step waits for the collectives: its own segment
                 cur[0].capture_end()
