@@ -93,12 +93,14 @@ typedef struct {
   /* ---- debugging only: CTA 0 records (event, clock64) int64 pairs of its three pipeline roles ---- */
   void* debug_timeline;  /* device buffer of 2*debug_timeline_events int64, or NULL */
   int32_t debug_timeline_events;
-  int32_t debug_flags;   /* 0 in production; 2 = skip TMA loads (pipeline dissection, results invalid);
-                          * bits 8-11 = operand ring depth of linear tiles (0: default) */
+  int32_t debug_flags;   /* 0 in production; 2 = skip TMA loads (pipeline dissection, results invalid); other values: SY_EINVAL */
   /* ---- validation only: the fp32 accumulators themselves, before the bf16 rounding of the stored result:
    * debug_f32[pixel][Cout] (pixel = flattened (n, oh, ow)), written next to the normal output.  This is where
    * north_star's "within 1e-3 of the reference" is literal (tests/test_gpu_ops.py::test_conv_fp32_accumulators). ---- */
   float* debug_f32;
+  /* ---- tiling override (sy_conv2d_tc only; 0 = the planner's choice) ---- */
+  int32_t tile_mode;     /* 1 = linear tiles, 2 = halo where the conv is 3x3 stride 1 (linear elsewhere); as SyConvPlan.mode */
+  int32_t tile_bn;       /* tile width 64 or 128 */
 } SyConvDesc;
 
 /* Rows of the statistics workspace (= SM count: one row per persistent CTA). */
@@ -110,15 +112,15 @@ int sy_conv_stat_rows(void);
  * running statistics (group 0 then group 1, unbiased variance, momentum).  Deterministic.  Do not
  * run two such launches concurrently on one GPU (the barrier needs every SM). */
 int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream);
-/* Host-only query (no launch, no GPU needed): the tiling sy_conv2d_tc chooses for a layer shape -- A-operand mode
- * (1 linear tiles / im2col-mode TMA, 2 halo: 16 x 8 patches, the only mode with patch_h x patch_w, else 0 x 0), tile
- * width BN, tiles and rounds of the persistent grid, tile walk (0 N-major, 1 M-band: each CTA keeps one N tile) and grid
- * size. */
+/* Host-only query (no launch, no GPU needed): the tiling sy_conv2d_tc chooses for a layer shape and the descriptor's
+ * tile_mode / tile_bn -- A-operand mode (1 linear tiles / im2col-mode TMA, 2 halo: 16 x 8 patches, the only mode with
+ * patch_h x patch_w, else 0 x 0), tile width BN, tiles and rounds of the persistent grid, tile walk (0 N-major, 1 M-band:
+ * each CTA keeps one N tile) and grid size. */
 typedef struct SyConvPlan {
   int32_t mode, bn, m_tiles, n_tiles, rounds, kblocks, patch_h, patch_w, walk, grid;
 } SyConvPlan;
 int sy_conv2d_plan(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride,
-                   SyConvPlan* out);
+                   int32_t tile_mode, int32_t tile_bn, SyConvPlan* out);
 /* plain CUDA-core direct convolution with the same x/y/w/FUSED contract (no statistics):
  * device-side cross-check of the tensor-core kernel. */
 int sy_conv2d_simt(const SyConvDesc* d, sy_stream_t stream);

@@ -1,6 +1,5 @@
 // Runtime entry points: error text, version, device check.
 #include <stdarg.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -12,15 +11,10 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-// read on every launch (a getenv is ~100 ns) so that a process can switch it between two measurements
-bool pdl_enabled() {
-  const char* e = getenv("SY_PDL");
-  return !(e != nullptr && e[0] == '0');
-}
 }  // namespace sy
 
 extern "C" const char* sy_last_error_string(void) { return sy::g_err; }
-extern "C" int sy_version(void) { return 100; }
+extern "C" int sy_version(void) { return 101; }
 
 extern "C" int sy_check_device(void) {
   int dev = 0;

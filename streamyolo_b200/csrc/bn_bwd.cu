@@ -45,8 +45,7 @@ struct BwdArgs {
 // Partial rows [rows0 + rows1][2 (sum dz | sum dz * xhat)][C].  Row r of a group covers an equal share of the group's
 // pixels; inside the block a thread owns one 8-channel chunk and every (256 / G)-th pixel (kBwdUnroll 16-byte load pairs in
 // flight), then the pixel lanes are combined through shared memory in a fixed order (deterministic).
-template <int UNROLL, int MINB>
-__global__ void __launch_bounds__(kBwdThreads, MINB) bn_act_bwd_reduce_kernel(const BwdArgs q, float* partials) {
+__global__ void __launch_bounds__(kBwdThreads, 2) bn_act_bwd_reduce_kernel(const BwdArgs q, float* partials) {
   __shared__ float red[kBwdThreads][17];
   const int grp = (int)blockIdx.x >= q.rows0 ? 1 : 0;
   const int row = grp ? (int)blockIdx.x - q.rows0 : (int)blockIdx.x, nrows = grp ? q.rows1 : q.rows0;
@@ -72,10 +71,10 @@ __global__ void __launch_bounds__(kBwdThreads, MINB) bn_act_bwd_reduce_kernel(co
       }
       const __nv_bfloat16* rp = q.raw + g * 8;
       const __nv_bfloat16* dp = q.dy + g * 8;
-      for (long long pp = p0 + pl; pp < p1; pp += (long long)PL * UNROLL) {
-        uint4 rv[UNROLL], dv[UNROLL];
+      for (long long pp = p0 + pl; pp < p1; pp += (long long)PL * kBwdUnroll) {
+        uint4 rv[kBwdUnroll], dv[kBwdUnroll];
 #pragma unroll
-        for (int j = 0; j < UNROLL; ++j) {
+        for (int j = 0; j < kBwdUnroll; ++j) {
           const long long pix = pp + (long long)j * PL;
           if (pix < p1) {
             rv[j] = *reinterpret_cast<const uint4*>(rp + pix * q.raw_pitch);
@@ -83,7 +82,7 @@ __global__ void __launch_bounds__(kBwdThreads, MINB) bn_act_bwd_reduce_kernel(co
           }
         }
 #pragma unroll
-        for (int j = 0; j < UNROLL; ++j) {
+        for (int j = 0; j < kBwdUnroll; ++j) {
           if (pp + (long long)j * PL >= p1) continue;
           float r[8], d[8];
           unpack8b(rv[j], r);
@@ -178,9 +177,8 @@ __global__ void __launch_bounds__(256) bn_act_bwd_finalize_kernel(const float* _
 
 // draw = A * dz + C1 * r + C0 (bf16), dz = dy * silu'(r * A + B).  Same thread mapping as the forward normalise pass: a
 // thread owns one 8-channel chunk for its whole life (coefficients in registers), kBwdUnroll load pairs in flight.
-template <int UNROLL, int MINB>
-__global__ void __launch_bounds__(kBwdThreads, MINB) bn_act_bwd_apply_kernel(const BwdArgs q, const float* __restrict__ coef,
-                                                                          __nv_bfloat16* draw, long long draw_pitch) {
+__global__ void __launch_bounds__(kBwdThreads, 2) bn_act_bwd_apply_kernel(const BwdArgs q, const float* __restrict__ coef,
+                                                                       __nv_bfloat16* draw, long long draw_pitch) {
   const int C = q.C, G = C >> 3;
   const int ppb = kBwdThreads / G;
   const int prow = (int)threadIdx.x / G, g = (int)threadIdx.x - prow * G;
@@ -199,10 +197,10 @@ __global__ void __launch_bounds__(kBwdThreads, MINB) bn_act_bwd_apply_kernel(con
   const __nv_bfloat16* rp = q.raw + g * 8;
   const __nv_bfloat16* dp = q.dy + g * 8;
   __nv_bfloat16* op = draw + g * 8;
-  for (long long pix0 = (long long)blockIdx.x * ppb + prow; pix0 < q.npix; pix0 += step * UNROLL) {
-    uint4 rv[UNROLL], dv[UNROLL];
+  for (long long pix0 = (long long)blockIdx.x * ppb + prow; pix0 < q.npix; pix0 += step * kBwdUnroll) {
+    uint4 rv[kBwdUnroll], dv[kBwdUnroll];
 #pragma unroll
-    for (int j = 0; j < UNROLL; ++j) {
+    for (int j = 0; j < kBwdUnroll; ++j) {
       const long long pix = pix0 + j * step;
       if (pix < q.npix) {
         rv[j] = *reinterpret_cast<const uint4*>(rp + pix * q.raw_pitch);
@@ -210,7 +208,7 @@ __global__ void __launch_bounds__(kBwdThreads, MINB) bn_act_bwd_apply_kernel(con
       }
     }
 #pragma unroll
-    for (int j = 0; j < UNROLL; ++j) {
+    for (int j = 0; j < kBwdUnroll; ++j) {
       const long long pix = pix0 + j * step;
       if (pix >= q.npix) continue;
       const int grp = pix >= q.split_pix ? 1 : 0;
@@ -275,20 +273,7 @@ extern "C" int sy_bn_act_backward(const SyBnActBwdDesc* d, sy_stream_t stream_) 
   q.rows0 = bwd_rows_for(q.split_pix, raw.c); q.rows1 = bwd_rows_for(q.npix - q.split_pix, raw.c);
   const int rows = q.rows0 + q.rows1;
   SY_REQUIRE(d->n_partials >= rows, SY_EWORKSPACE, "bn_act_backward: %d partial rows, need %d", d->n_partials, rows);
-  // tuning aid: SY_BNBWD = <reduce variant><apply variant>, each 0 (4 loads pairs in flight, 2 blocks / SM: the default),
-  // 1 (2 pairs, 3 blocks), 2 (2 pairs, 4 blocks), 3 (4 pairs, 3 blocks)
-  static int var_r = -1, var_a = -1;
-  if (var_r < 0) {
-    const char* e = getenv("SY_BNBWD");
-    var_r = (e && e[0] >= '0' && e[0] <= '3') ? e[0] - '0' : 0;
-    var_a = (e && e[0] && e[1] >= '0' && e[1] <= '3') ? e[1] - '0' : 0;
-  }
-  switch (var_r) {
-    case 1: bn_act_bwd_reduce_kernel<2, 3><<<rows, kBwdThreads, 0, stream>>>(q, d->partials); break;
-    case 2: bn_act_bwd_reduce_kernel<2, 4><<<rows, kBwdThreads, 0, stream>>>(q, d->partials); break;
-    case 3: bn_act_bwd_reduce_kernel<4, 3><<<rows, kBwdThreads, 0, stream>>>(q, d->partials); break;
-    default: bn_act_bwd_reduce_kernel<4, 2><<<rows, kBwdThreads, 0, stream>>>(q, d->partials); break;
-  }
+  bn_act_bwd_reduce_kernel<<<rows, kBwdThreads, 0, stream>>>(q, d->partials);
   const double inv0 = q.split_pix > 0 ? 1.0 / (double)q.split_pix : 0.0;
   const double inv1 = q.npix - q.split_pix > 0 ? 1.0 / (double)(q.npix - q.split_pix) : 0.0;
   // (plain launches: programmatic dependent launch of the backward kernels was measured SLOWER -- 17.16 vs 16.39 ms per
@@ -296,15 +281,9 @@ extern "C" int sy_bn_act_backward(const SyBnActBwdDesc* d, sy_stream_t stream_) 
   bn_act_bwd_finalize_kernel<<<cdiv(raw.c, 8), 256, 0, stream>>>(d->partials, q.rows0, q.rows1, inv0, inv1, raw.c, d->scale, d->shift, d->mean,
                                                                  d->invstd, d->dgamma, d->dbeta, d->accumulate, d->coef);
   const int G = raw.c / 8, ppb = kBwdThreads / G;
-  const int unroll_a = (var_a == 1 || var_a == 2) ? 2 : 4;
-  long long blocks = (q.npix + (long long)ppb * unroll_a - 1) / ((long long)ppb * unroll_a);
+  long long blocks = (q.npix + (long long)ppb * kBwdUnroll - 1) / ((long long)ppb * kBwdUnroll);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  __nv_bfloat16* drp = reinterpret_cast<__nv_bfloat16*>(dr.ptr);
-  switch (var_a) {
-    case 1: bn_act_bwd_apply_kernel<2, 3><<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, drp, dr.pitch); break;
-    case 2: bn_act_bwd_apply_kernel<2, 4><<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, drp, dr.pitch); break;
-    case 3: bn_act_bwd_apply_kernel<4, 3><<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, drp, dr.pitch); break;
-    default: bn_act_bwd_apply_kernel<4, 2><<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, drp, dr.pitch); break;
-  }
+  bn_act_bwd_apply_kernel<<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, reinterpret_cast<__nv_bfloat16*>(dr.ptr),
+                                                                 dr.pitch);
   return launch_status("bn_act_backward kernels");
 }

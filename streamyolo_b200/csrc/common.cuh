@@ -64,10 +64,9 @@ inline int sm_count() {
 // Kernels launched through launch_pdl() may be scheduled while their predecessor on the stream is still
 // draining: they call pdl_launch_dependents() first thing (lets the *next* kernel do the same) and pdl_wait()
 // before their first access to global memory (returns once every prerequisite grid has completed and its
-// writes are visible).  Both are no-ops for a normally launched grid.  SY_PDL=0 turns the attribute off.
+// writes are visible).  Both are no-ops for a normally launched grid.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-bool pdl_enabled();
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
@@ -79,29 +78,9 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.stream = stream;
   cudaLaunchAttribute at[1];
   at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = at;
   cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-// the same, as thread-block clusters of `cluster_x` consecutive CTAs (grid.x must be a multiple of it)
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), int cluster_x, dim3 grid, dim3 block, size_t smem,
-                                      cudaStream_t stream, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-  at[1].id = cudaLaunchAttributeClusterDimension;
-  at[1].val.clusterDim.x = (unsigned)cluster_x;
-  at[1].val.clusterDim.y = 1;
-  at[1].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 2;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

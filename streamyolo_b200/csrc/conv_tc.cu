@@ -884,16 +884,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // Tile width heuristic from a per-K-block cost model: one 64-deep K block of a 128-row tile costs about kblock_cycles()
 // (MMA + barrier hand-shake + operand supply), the epilogue about kEpiCyclesPerSlab per 64-column slab, and the
 // persistent grid runs ceil(tiles / SMs) rounds -- so wide tiles win unless they add a round.  The constants are a model,
-// not H100 measurements; SY_CONV_BN forces the width.
+// not H100 measurements; a tile_bn override (SyConvDesc) forces the width.
 constexpr double kEpiCyclesPerSlab = 1900.0;
 
 static double kblock_cycles(int bn) { return bn == 128 ? 515.0 : 560.0; }
 
-static int pick_bn(int cout, int m_tiles, int kblocks) {
-  if (const char* e = getenv("SY_CONV_BN")) {            // tuning / test aid: force the tile width
-    const int v = atoi(e);
-    if (v == 64 || v == 128) return v;
-  }
+static int pick_bn(int cout, int m_tiles, int kblocks, int tile_bn) {
+  if (tile_bn != 0) return tile_bn;
   const int cands[2] = {128, 64};
   int best_bn = 64;
   double best = 1e30;
@@ -983,8 +980,7 @@ static int make_plan(Params& p, Plan* out) {
   } else {
     const int stage_bytes = kABytes + bbytes;
     const int fit = min(kMaxStages, (kSmemLimit - fixed_bytes - acc_bytes) / stage_bytes);
-    int stages = min(fit, kRingStages);
-    if ((p.debug_flags >> 8) & 15) stages = min(fit, (p.debug_flags >> 8) & 15);     // debug: set the ring depth
+    const int stages = min(fit, kRingStages);
     SY_REQUIRE(stages >= 2, SY_EINVAL, "conv2d_tc: Cout=%d leaves no room for the operand ring", p.Cout);
     p.stages = stages;
     smem = fixed_bytes + acc_bytes + stages * stage_bytes;
@@ -1040,13 +1036,11 @@ static int launch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const
 // Halo mode (conv_tc_kernel, AM = 2) for a 3x3 stride-1 convolution?  It needs 16 x 8 patch tiles (more tiles than the
 // linear tiling on small feature maps) and pays off where the tap re-reads bound the main loop.  Modelled per-K-block
 // costs (cycles): linear 515 / 560, halo 430 / 370 at BN = 128 / 64.
-// SY_CONV_A=halo forces it (every eligible conv), SY_CONV_A=off disables it.
-static bool use_halo(int n, int ho, int wo, int cout, int kblocks) {
-  const char* e = getenv("SY_CONV_A");
-  if (e != nullptr && e[0] == 'h') return true;
-  if (e != nullptr && e[0] == 'o') return false;
+// tile_mode 2 forces it (every eligible conv), 1 disables it.
+static bool use_halo(int n, int ho, int wo, int cout, int kblocks, int tile_mode, int tile_bn) {
+  if (tile_mode != 0) return tile_mode == 2;
   const int tiles_l = cdiv(n * ho * wo, kBlockM), tiles_h = n * cdiv(ho, 16) * cdiv(wo, 8);
-  const int bn = pick_bn(cout, tiles_l, kblocks);
+  const int bn = pick_bn(cout, tiles_l, kblocks, tile_bn);
   const double lin_c = bn == 128 ? 515.0 : 560.0, halo_c = bn == 128 ? 430.0 : 370.0;
   const int nt = cdiv(cout, bn);
   return cdiv(tiles_h * nt, num_sms()) * halo_c < cdiv(tiles_l * nt, num_sms()) * lin_c;
@@ -1054,20 +1048,24 @@ static bool use_halo(int n, int ho, int wo, int cout, int kblocks) {
 
 // The tiling of one layer shape, shared by sy_conv2d_tc and the host-only sy_conv2d_plan: halo mode where use_halo
 // takes it, linear tiles otherwise.  The tile width is chosen on the linear tiling (the halo decision assumed that width).
+// tile_mode / tile_bn (SyConvDesc; 0 = planner) override the choices; they are plan inputs only and never reach Params.
 struct Tiling {
   bool halo;
   int bn, m_tiles, tiles_x, tiles_y, cblocks, kblocks;
 };
-static Tiling pick_tiling(int n, int ho, int wo, int cin, int cout, int kh, int kw, int stride) {
+static bool tiling_override_ok(int tile_mode, int tile_bn) {
+  return tile_mode >= 0 && tile_mode <= 2 && (tile_bn == 0 || tile_bn == 64 || tile_bn == 128);
+}
+static Tiling pick_tiling(int n, int ho, int wo, int cin, int cout, int kh, int kw, int stride, int tile_mode, int tile_bn) {
   Tiling t{};
   t.cblocks = cdiv(cin, kBlockK);
   t.kblocks = kh * kw * t.cblocks;
-  t.halo = kh == 3 && kw == 3 && stride == 1 && use_halo(n, ho, wo, cout, t.kblocks);
+  t.halo = kh == 3 && kw == 3 && stride == 1 && use_halo(n, ho, wo, cout, t.kblocks, tile_mode, tile_bn);
   t.tiles_y = cdiv(ho, kHaloTH);
   t.tiles_x = cdiv(wo, kHaloTW);
   const int lin_tiles = cdiv(n * ho * wo, kBlockM);
   t.m_tiles = t.halo ? n * t.tiles_y * t.tiles_x : lin_tiles;
-  t.bn = pick_bn(cout, lin_tiles, t.kblocks);
+  t.bn = pick_bn(cout, lin_tiles, t.kblocks, tile_bn);
   return t;
 }
 
@@ -1092,16 +1090,18 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
              y.n, y.h, y.w, x.n, ho, wo);
   SY_REQUIRE(((uintptr_t)d->w % 16) == 0, SY_EINVAL, "conv2d_tc: weights not 16B aligned");
   SY_REQUIRE(y.c <= 2048, SY_EINVAL, "conv2d_tc: Cout=%d > 2048", y.c);
+  SY_REQUIRE(d->debug_flags == 0 || d->debug_flags == 2, SY_EINVAL, "conv2d_tc: debug_flags %d unsupported", d->debug_flags);
+  SY_REQUIRE(tc::tiling_override_ok(d->tile_mode, d->tile_bn), SY_EINVAL, "conv2d_tc: tile_mode %d / tile_bn %d unsupported",
+             d->tile_mode, d->tile_bn);
   tc::EncodeTiledFn enc = tc::get_encode();
   SY_REQUIRE(enc != nullptr, SY_EARCH, "cuTensorMapEncodeTiled not available from the driver");
 
   tc::Params p{};
   p.debug_flags = d->debug_flags;
-  if (const char* e = getenv("SY_CONV_DEBUG")) p.debug_flags |= atoi(e);    // tuning aid (see Params::debug_flags)
   p.N = x.n; p.Ho = ho; p.Wo = wo; p.Cout = y.c; p.Cin = x.c;
   p.kh = d->kh; p.kw = d->kw; p.stride = d->stride; p.pad_h = ph; p.pad_w = pw;
   SY_REQUIRE((long long)x.n * ho * wo < (1ll << 31) - 256, SY_EINVAL, "conv2d_tc: too many output pixels");
-  const tc::Tiling t = tc::pick_tiling(x.n, ho, wo, x.c, y.c, d->kh, d->kw, d->stride);
+  const tc::Tiling t = tc::pick_tiling(x.n, ho, wo, x.c, y.c, d->kh, d->kw, d->stride, d->tile_mode, d->tile_bn);
   const bool halo = t.halo;
   const int bn = t.bn;
   p.P_total = x.n * ho * wo;
@@ -1232,16 +1232,18 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   return halo ? tc::launch_bn<2>(bn, ta, tb, ty, p, pl, stream) : tc::launch_bn<1>(bn, ta, tb, ty, p, pl, stream);
 }
 
-// Host-only query (no launch, works without a GPU): the tiling decisions sy_conv2d_tc takes for a layer shape
-// (both go through pick_tiling and pick_walk).
+// Host-only query (no launch, works without a GPU): the tiling decisions sy_conv2d_tc takes for a layer shape and
+// tiling override (both go through pick_tiling and pick_walk).
 extern "C" int sy_conv2d_plan(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride,
-                              SyConvPlan* out) {
+                              int32_t tile_mode, int32_t tile_bn, SyConvPlan* out) {
   SY_REQUIRE(out != nullptr && n > 0 && h > 0 && w > 0 && cin > 0 && cout > 0, SY_EINVAL, "conv2d_plan: bad arguments");
   SY_REQUIRE((kh == 1 || kh == 3) && (kw == 1 || kw == 3) && (stride == 1 || stride == 2), SY_EINVAL,
              "conv2d_plan: kernel %dx%d stride %d unsupported", kh, kw, stride);
+  SY_REQUIRE(tc::tiling_override_ok(tile_mode, tile_bn), SY_EINVAL, "conv2d_plan: tile_mode %d / tile_bn %d unsupported",
+             tile_mode, tile_bn);
   const int ph = (kh - 1) / 2, pw = (kw - 1) / 2;
   const int ho = (h + 2 * ph - kh) / stride + 1, wo = (w + 2 * pw - kw) / stride + 1;
-  const tc::Tiling t = tc::pick_tiling(n, ho, wo, cin, cout, kh, kw, stride);
+  const tc::Tiling t = tc::pick_tiling(n, ho, wo, cin, cout, kh, kw, stride, tile_mode, tile_bn);
   const int m_tiles = t.m_tiles;
   out->mode = t.halo ? 2 : 1;
   out->bn = t.bn;

@@ -229,12 +229,7 @@ static int make_plan(const SyConvWgradDesc* d, Plan* pl) {
   pl->taps = d->kh * d->kw;
   pl->kb_total = cdiv(x.n * pl->ho * pl->wo, kPixK);
   const int base = pl->m_tiles * pl->n_tiles * pl->taps;
-  int waves = 2;                                            // about two waves of work items
-  if (const char* e = getenv("SY_WGRAD_WAVES")) {           // tuning aid: fewer waves = less split-K partial traffic
-    const int v = atoi(e);
-    if (v >= 1 && v <= 8) waves = v;
-  }
-  int ks = cdiv(waves * num_sms(), base);
+  int ks = cdiv(2 * num_sms(), base);                      // about two waves of work items
   const int ks_max = pl->kb_total / 8 > 1 ? pl->kb_total / 8 : 1;   // at least 8 K blocks per split
   if (ks > ks_max) ks = ks_max;
   if (ks < 1) ks = 1;
@@ -328,9 +323,7 @@ extern "C" int sy_conv2d_wgrad_tc(const SyConvWgradDesc* d, sy_stream_t stream_)
   const long long total = (long long)dy.c * x.c * pl.taps;
   // split groups per output: enough threads to cover the GPU (SMs x 2048) and at least 8 splits per group
   int sg = 1;
-  if (getenv("SY_WGRAD_SG1") == nullptr) {
-    while (sg < 8 && total * sg < (long long)tc::num_sms() * 2048 && pl.ksplit >= 16 * sg) sg *= 2;
-  }
+  while (sg < 8 && total * sg < (long long)tc::num_sms() * 2048 && pl.ksplit >= 16 * sg) sg *= 2;
   const long long per_block = 256 / sg;
   const long long want = (total + per_block - 1) / per_block;
   const int blocks = (int)(want < tc::num_sms() * 8 ? want : tc::num_sms() * 8);

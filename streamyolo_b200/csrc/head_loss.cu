@@ -196,10 +196,6 @@ head_pred_generic_kernel(const SyHeadPredDesc d, int B, int H, int W, int C, int
 }
 
 static int head_pixels_per_thread(long long npix) {
-  if (const char* e = getenv("SY_HEAD_PT")) {            // tuning aid
-    const int v = atoi(e);
-    if (v == 1 || v == 2 || v == 4) return v;
-  }
   return npix >= 32768 ? 2 : 1;                          // small levels: more blocks matter more than the weight reuse
 }
 
@@ -217,11 +213,8 @@ static int launch_head_pred_pt(const SyHeadPredDesc* d, const SyTensor& f, cudaS
 
 template <int NO>
 static int launch_head_pred(const SyHeadPredDesc* d, const SyTensor& f, cudaStream_t stream) {
-  switch (head_pixels_per_thread((long long)f.n * f.h * f.w)) {
-    case 4: return launch_head_pred_pt<NO, 4>(d, f, stream);
-    case 2: return launch_head_pred_pt<NO, 2>(d, f, stream);
-    default: return launch_head_pred_pt<NO, 1>(d, f, stream);
-  }
+  if (head_pixels_per_thread((long long)f.n * f.h * f.w) == 2) return launch_head_pred_pt<NO, 2>(d, f, stream);
+  return launch_head_pred_pt<NO, 1>(d, f, stream);
 }
 
 static int launch_head_pred_generic(const SyHeadPredDesc* d, const SyTensor& f, cudaStream_t stream) {

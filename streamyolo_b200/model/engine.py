@@ -14,8 +14,6 @@ together with SiLU and the residual (what yolox ``fuse_model`` + ``fuseforward``
 The recording forward of a training step (model/backward.py) is this same walk with a tape in the ``Ctx``: nothing is
 updated in place, every op keeps what its backward needs and is recorded on the tape.
 """
-import os
-
 import torch
 
 from .. import ops
@@ -25,6 +23,7 @@ from ..ops import View
 WEIGHT_EPOCH = 0  # bumped by whoever updates parameters through raw pointers (train.Trainer's fused optimiser kernel does
                   # not touch torch's version counters): part of every packed-operand cache key
 TRACE = None      # debugging: set to a dict to capture every BaseConv's stored output by module name
+CONV_IMPL = "tc"  # conv of the plain forward: "tc" (wgmma kernel) or "simt" (CUDA-core cross-check); a tape always runs "tc"
 
 
 def name_modules(model):
@@ -48,7 +47,7 @@ class Ctx:
         self.groups = 2 if split < n else 1
         self.device = device
         self.tape = tape
-        self.impl = "tc" if tape is not None else os.environ.get("SY_CONV_IMPL", "tc")
+        self.impl = "tc" if tape is not None else CONV_IMPL
 
     def rec(self, **kw):
         if self.tape is not None:

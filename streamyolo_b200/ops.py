@@ -31,7 +31,8 @@ class SyConvDesc(C.Structure):
                 ("n_partials", C.c_int32), ("rows_written", C.POINTER(C.c_int32)), ("bn", SyBnSegment * 2),
                 ("momentum", C.c_float), ("eps", C.c_float), ("scale_shift", C.c_void_p), ("mean_invstd", C.c_void_p),
                 ("sync", C.c_void_p), ("debug_timeline", C.c_void_p),
-                ("debug_timeline_events", C.c_int32), ("debug_flags", C.c_int32), ("debug_f32", C.c_void_p)]
+                ("debug_timeline_events", C.c_int32), ("debug_flags", C.c_int32), ("debug_f32", C.c_void_p),
+                ("tile_mode", C.c_int32), ("tile_bn", C.c_int32)]
 
 
 class SyHeadPredDesc(C.Structure):
@@ -130,7 +131,7 @@ _SIG = {
     "sy_check_device": (C.c_int, []),
     "sy_conv_stat_rows": (C.c_int, []),
     "sy_conv2d_tc": (C.c_int, [C.POINTER(SyConvDesc), C.c_void_p]),
-    "sy_conv2d_plan": (C.c_int, [C.c_int32] * 8 + [C.POINTER(SyConvPlan)]),
+    "sy_conv2d_plan": (C.c_int, [C.c_int32] * 10 + [C.POINTER(SyConvPlan)]),
     "sy_conv2d_simt": (C.c_int, [C.POINTER(SyConvDesc), C.c_void_p]),
     "sy_dwconv2d": (C.c_int, [C.POINTER(SyConvDesc), C.c_void_p]),
     "sy_focus_pack": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, SyTensor,
@@ -313,9 +314,10 @@ def conv_stat_rows():
 
 def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None, act=1, res: View = None,
            partials=None, split_n=0, timeline=None, debug_flags=0, bn=None, momentum=0.03, eps=1e-3, scale_shift=None,
-           sync=None, mean_invstd=None, debug_f32=None):
+           sync=None, mean_invstd=None, debug_f32=None, tile_mode=0, tile_bn=0):
     """``k`` is an int (square) or (kh, kw).  With ``partials`` (RAW mode, tensor-core path) returns the number
-    of per-CTA statistic rows the launch writes."""
+    of per-CTA statistic rows the launch writes.  ``tile_mode`` / ``tile_bn`` override the tensor-core tiling
+    (0 = planner; see conv2d_plan)."""
     d = SyConvDesc()
     d.x, d.y = x.st(), y.st()
     d.w = wpk.data_ptr()
@@ -341,6 +343,7 @@ def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None,
         d.scale_shift, d.sync = scale_shift.data_ptr(), sync.data_ptr()
         d.mean_invstd = mean_invstd.data_ptr() if mean_invstd is not None else None
     d.debug_flags = debug_flags
+    d.tile_mode, d.tile_bn = tile_mode, tile_bn
     d.debug_f32 = debug_f32.data_ptr() if debug_f32 is not None else None
     if timeline is not None:
         d.debug_timeline, d.debug_timeline_events = timeline.data_ptr(), timeline.numel() // 2
@@ -580,11 +583,12 @@ def spp_maxpool_backward(x: View, d5: View, d9: View, d13: View, dx: View):
            kernels=2)
 
 
-def conv2d_plan(n, h, w, cin, cout, k, s):
-    """Tiling decisions of the tensor-core conv for a layer shape (host-only: works without a GPU)."""
+def conv2d_plan(n, h, w, cin, cout, k, s, tile_mode=0, tile_bn=0):
+    """Tiling decisions of the tensor-core conv for a layer shape (host-only: works without a GPU).  ``tile_mode``:
+    0 = planner, 1 = linear tiles, 2 = halo where the conv is 3x3 stride 1; ``tile_bn``: 0 = planner, 64 or 128."""
     kh, kw = (k, k) if isinstance(k, int) else k
     p = SyConvPlan()
-    rc = load_library().sy_conv2d_plan(n, h, w, cin, cout, kh, kw, s, C.byref(p))
+    rc = load_library().sy_conv2d_plan(n, h, w, cin, cout, kh, kw, s, tile_mode, tile_bn, C.byref(p))
     if rc != 0:
         raise RuntimeError("conv2d_plan: " + (load_library().sy_last_error_string() or b"").decode())
     return {f: getattr(p, f) for f, _ in SyConvPlan._fields_}

@@ -47,7 +47,7 @@ def conv_stat_rows():
 
 def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=None, partials=None, split_n=0,
            timeline=None, debug_flags=0, bn=None, momentum=0.03, eps=1e-3, scale_shift=None, sync=None, mean_invstd=None,
-           debug_f32=None):
+           debug_f32=None, tile_mode=0, tile_bn=0):
     kh, kw = (k, k) if isinstance(k, int) else k
     if impl == "dw":                                # depthwise: wpk [kh*kw][C]
         c = wpk.shape[1]

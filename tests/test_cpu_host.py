@@ -145,10 +145,10 @@ def test_struct_layouts_match_header(tmp_path):
         assert int(v) == want, f"{n}.{f}: header {v}, ctypes {want}"
 
 
-def test_conv_tiling_plan_without_gpu(monkeypatch):
+def test_conv_tiling_plan_and_overrides_without_gpu():
     """sy_conv2d_plan is host-only: the tiling decisions of the tensor-core conv can be inspected (and are pinned here for the
-    layers that motivated them) without a device.  132 SMs (an H100 SXM) are assumed when no GPU is present."""
-    monkeypatch.delenv("SY_CONV_A", raising=False)
+    layers that motivated them) without a device, with and without the tile_mode / tile_bn overrides; out-of-range
+    overrides are rejected.  132 SMs (an H100 SXM) are assumed when no GPU is present."""
     p = ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1)          # linear tiles: 285 x 2 tiles = 5 rounds
     assert (p["mode"], p["bn"], p["m_tiles"], p["rounds"]) == (1, 128, 285, 5)
     p = ops.conv2d_plan(16, 19, 30, 512, 512, 3, 1)          # 72 x 4 tiles: three rounds
@@ -157,14 +157,16 @@ def test_conv_tiling_plan_without_gpu(monkeypatch):
     assert (p["mode"], p["bn"], p["patch_h"], p["patch_w"], p["kblocks"]) == (2, 128, 16, 8, 18)
     p = ops.conv2d_plan(16, 75, 120, 128, 128, 1, 1)         # 1x1: never halo
     assert (p["mode"], p["kblocks"], p["patch_h"], p["patch_w"]) == (1, 2, 0, 0)
-    monkeypatch.setenv("SY_CONV_A", "off")                    # halo disabled: the halo layer above on linear tiles
-    p = ops.conv2d_plan(16, 75, 120, 128, 128, 3, 1)
+    p = ops.conv2d_plan(16, 75, 120, 128, 128, 3, 1, tile_mode=1)   # linear forced: the halo layer above on linear tiles
     assert (p["mode"], p["m_tiles"], p["patch_h"], p["patch_w"]) == (1, (16 * 75 * 120 + 127) // 128, 0, 0)
-    monkeypatch.setenv("SY_CONV_A", "halo")                   # halo forced: 16 x 8 patches of the 38 x 60 map
-    p = ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1)
+    p = ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1, tile_mode=2)    # halo forced: 16 x 8 patches of the 38 x 60 map
     assert (p["mode"], p["m_tiles"], p["patch_h"], p["patch_w"]) == (2, 16 * 3 * 8, 16, 8)
+    p = ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1, tile_mode=1, tile_bn=64)   # width forced: 4 N tiles
+    assert (p["mode"], p["bn"], p["n_tiles"]) == (1, 64, 4)
     with pytest.raises(RuntimeError):
         ops.conv2d_plan(1, 8, 8, 8, 8, 5, 1)
+    with pytest.raises(RuntimeError):
+        ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1, tile_bn=96)
 
 
 def test_pack_batch_tile_table():

@@ -24,7 +24,7 @@ pytestmark = pytest.mark.gpu
 from oracle.make_golden import CASES  # noqa: E402
 from oracle.streamyolo_oracle import OracleCfg, StreamYoloOracle, bf16_round, model_shapes  # noqa: E402
 from streamyolo_b200 import ops, synth  # noqa: E402
-from streamyolo_b200.model import DFPPAFPN, TALHead, YOLOX  # noqa: E402
+from streamyolo_b200.model import DFPPAFPN, TALHead, YOLOX, engine  # noqa: E402
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 ORDER = ["total_loss", "iou_loss", "l1_loss", "conf_loss", "cls_loss", "num_fg"]
@@ -56,7 +56,7 @@ def rel(a, b):
 
 @pytest.fixture(params=["tc", "simt"])
 def impl(request, monkeypatch):
-    monkeypatch.setenv("SY_CONV_IMPL", request.param)
+    monkeypatch.setattr(engine, "CONV_IMPL", request.param)
     return request.param
 
 

@@ -6,8 +6,6 @@ Tolerances (written here once):
   * statistic partial sums (fp32): relative 2e-3 of sqrt(count)*rms
   * integer / index / max-pool / copy results: bit exact
 """
-import os
-
 import numpy as np
 import pytest
 import torch
@@ -48,22 +46,16 @@ def check_close(got, ref, what, ulp=2.0 ** -7):
     return rel
 
 
-# SY_TEST_TILES=linear|halo restricts the tensor-core variants under test (bring-up aid); default: all
-_T = os.environ.get("SY_TEST_TILES", "all")
-_ALL = {"tc": "linear", "tc_bn64": "linear", "tc_halo": "halo"}
-TC_IMPLS = [i for i, t in _ALL.items() if _T in ("all", "both", t)]
+TC_IMPLS = ["tc", "tc_bn64", "tc_halo"]
 
 
-def tc_impl(impl, monkeypatch):
-    """'tc' = linear M tiles (im2col-mode TMA, the default), 'tc_bn64' = linear tiles with the tile width forced to 64
-    (the BN = 64 kernel on layers the planner gives BN = 128, i.e. several N tiles and the M-band walk), 'tc_halo' = one
-    halo load per tile and channel block for the 3x3 stride-1 convs (linear tiles elsewhere); all are product paths."""
-    if impl.startswith("tc"):
-        monkeypatch.setenv("SY_CONV_A", "halo" if impl == "tc_halo" else "off")
-        if impl == "tc_bn64":
-            monkeypatch.setenv("SY_CONV_BN", "64")
-        return "tc"
-    return impl
+def tc_impl(impl):
+    """ops.conv2d's ``impl`` and tiling keywords of a variant under test.  'tc' = linear M tiles (im2col-mode TMA, the
+    default), 'tc_bn64' = linear tiles with the tile width forced to 64 (the BN = 64 kernel on layers the planner gives
+    BN = 128, i.e. several N tiles and the M-band walk), 'tc_halo' = one halo load per tile and channel block for the 3x3
+    stride-1 convs (linear tiles elsewhere); all are product paths."""
+    return {"tc": ("tc", dict(tile_mode=1)), "tc_bn64": ("tc", dict(tile_mode=1, tile_bn=64)),
+            "tc_halo": ("tc", dict(tile_mode=2))}.get(impl, (impl, {}))
 
 
 CONV_CASES = [
@@ -87,9 +79,9 @@ CONV_CASES = [
 
 @pytest.mark.parametrize("impl", ["simt"] + TC_IMPLS)
 @pytest.mark.parametrize("case", CONV_CASES, ids=lambda c: "x".join(map(str, c)))
-def test_conv_raw(case, impl, monkeypatch):
+def test_conv_raw(case, impl):
     n, ci, co, h, w, k, s = case
-    impl = tc_impl(impl, monkeypatch)
+    impl, tiling = tc_impl(impl)
     if impl == "simt" and ci * co * h * w * k * k * n > 3e10:
         pytest.skip("too slow on the CUDA-core cross-check kernel")
     x = rand_act(n, ci, h, w, 1)
@@ -102,7 +94,8 @@ def test_conv_raw(case, impl, monkeypatch):
     rows = ops.conv_stat_rows()
     partials = torch.full((rows, 4 * co), float("nan"), device=DEV) if impl == "tc" else None
     split = 1 if n > 1 else 0
-    ops.conv2d(xv, ops.pack_conv_weight(wt), y, k, s, ops.SY_CONV_RAW, impl=impl, partials=partials, split_n=split)
+    ops.conv2d(xv, ops.pack_conv_weight(wt), y, k, s, ops.SY_CONV_RAW, impl=impl, partials=partials, split_n=split,
+               **tiling)
     torch.cuda.synchronize()
     got = y.nchw_float()
     check_close(got, ref, f"conv_{impl}{case}")
@@ -120,12 +113,11 @@ def test_conv_raw(case, impl, monkeypatch):
 
 
 @pytest.mark.parametrize("tiles", TC_IMPLS)
-def test_conv_tc_bn_finalize_then_separate_apply(tiles, monkeypatch):
-    tc_impl(tiles, monkeypatch)
-    _bn_finalize_then_apply()
+def test_conv_tc_bn_finalize_then_separate_apply(tiles):
+    _bn_finalize_then_apply(**tc_impl(tiles)[1])
 
 
-def _bn_finalize_then_apply():
+def _bn_finalize_then_apply(**tiling):
     """RAW conv that also finalizes BatchNorm in its tail (grid barrier + parallel reduce; two groups, two
     parameter segments, running statistics), then the normalise pass with SiLU + residual; against
     F.batch_norm on the stored conv output.  Three launches in a row: the sync counters must come back to zero after each
@@ -150,7 +142,7 @@ def _bn_finalize_then_apply():
     for rep in range(3):
         y.buf.fill_(float("nan"))
         rows = ops.conv2d(x_v, ops.pack_conv_weight(wt), raw, 1, 1, ops.SY_CONV_RAW, partials=partials,
-                          split_n=2, bn=segs, momentum=0.03, eps=1e-3, scale_shift=ss, sync=sync, act=1)
+                          split_n=2, bn=segs, momentum=0.03, eps=1e-3, scale_shift=ss, sync=sync, act=1, **tiling)
         assert 1 <= rows <= ops.conv_stat_rows()
         ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), 2, 1, resid_v, y)
         torch.cuda.synchronize()
@@ -166,9 +158,9 @@ def _bn_finalize_then_apply():
 
 
 @pytest.mark.parametrize("impl", ["simt"] + TC_IMPLS)
-def test_conv_fused_residual_slices(impl, monkeypatch):
+def test_conv_fused_residual_slices(impl):
     """FUSED epilogue (scale, shift, SiLU, residual) reading and writing channel slices, in place."""
-    impl = tc_impl(impl, monkeypatch)
+    impl, tiling = tc_impl(impl)
     n, ci, co, h, w = 2, 64, 64, 19, 30
     x = rand_act(n, ci, h, w, 3)
     wt = rand_w(co, ci, 3, 4)
@@ -186,7 +178,7 @@ def test_conv_fused_residual_slices(impl, monkeypatch):
     yv = big_out.ch(co, co)
     yv.torch().copy_(resid.permute(0, 2, 3, 1))      # residual lives where the output goes (in place)
     ops.conv2d(xin, ops.pack_conv_weight(wt), yv, 3, 1, ops.SY_CONV_FUSED, impl=impl, scale=scale, shift=shift,
-               act=1, res=yv)
+               act=1, res=yv, **tiling)
     torch.cuda.synchronize()
     check_close(yv.nchw_float(), ref, f"conv_fused_{impl}")
     assert (big_out.ch(0, co).torch() == -3.0).all(), "neighbouring slice was overwritten"
@@ -207,8 +199,8 @@ def test_conv_tc_matches_simt_bitwise_mostly():
 
 
 @pytest.mark.parametrize("impl", ["simt"] + TC_IMPLS)
-def test_stem_focus(impl, monkeypatch):
-    impl = tc_impl(impl, monkeypatch)
+def test_stem_focus(impl):
+    impl, tiling = tc_impl(impl)
     b, h, w, co = 2, 120, 160, 16
     g = torch.Generator().manual_seed(0)
     x = (torch.rand(b, 6, h, w, generator=g) * 255).to(DEV)
@@ -216,7 +208,7 @@ def test_stem_focus(impl, monkeypatch):
     xin = View.empty(2 * b, h // 2, w // 2, 64, DEV)
     ops.focus_pack(x, 2, xin)
     y = View.empty(2 * b, h // 2, w // 2, co, DEV)
-    ops.conv2d(xin, ops.pack_stem_weight(wt), y, ops.STEM_K, 1, ops.SY_CONV_RAW, impl=impl)
+    ops.conv2d(xin, ops.pack_stem_weight(wt), y, ops.STEM_K, 1, ops.SY_CONV_RAW, impl=impl, **tiling)
     torch.cuda.synchronize()
     xs = bf(torch.cat([x[:, 0:3], x[:, 3:6]], 0))
     foc = torch.cat([xs[..., ::2, ::2], xs[..., 1::2, ::2], xs[..., ::2, 1::2], xs[..., 1::2, 1::2]], 1)
@@ -283,10 +275,11 @@ def test_spp_and_copy_exact():
 
 @pytest.mark.parametrize("shape", [(2, 64, 15, 20, 8), (2, 64, 15, 20, 3), (1, 32, 9, 11, 80), (8, 256, 75, 120, 8)],
                          ids=["nc8", "nc3-generic", "nc80-generic", "level0-l"])
-def test_head_pred_decode(shape, monkeypatch):
+def test_head_pred_decode(shape):
     """Prediction convs + decode against F.conv2d.  Class counts without a compiled instantiation take the generic kernel
-    (the reference head accepts any num_classes, tal_head.py:27); the benchmark's level-0 shape takes the two-pixels-per-thread
-    variant, whose output must be bit-identical to the one-pixel variant (same per-pixel arithmetic)."""
+    (the reference head accepts any num_classes, tal_head.py:27); the benchmark's level-0 shape (72 000 pixels) takes the
+    two-pixels-per-thread variant, whose output must be bit-identical to the one-pixel variant that one image of it
+    (9 000 pixels) takes (same per-pixel arithmetic)."""
     b, c, h, w, nc = shape
     cf, rf = rand_act(b, c, h, w, 51), rand_act(b, c, h, w, 52)
     g = torch.Generator().manual_seed(53)
@@ -316,16 +309,12 @@ def test_head_pred_decode(shape, monkeypatch):
             assert torch.allclose(origin[:, off:], raw[..., :4], rtol=1e-4, atol=1e-5)
         assert (out[:, :off] == 0).all()
         if nc == 8:
-            outs = []
-            for pt in ("1", "2", "4"):
-                monkeypatch.setenv("SY_HEAD_PT", pt)
-                o2 = torch.zeros((b, a_total, 5 + nc), device=DEV)
-                ops.head_pred_decode(ops.from_nchw(cf), ops.from_nchw(rf), wr, br, wo_, bo, wc, bc, stride, off, a_total, o2,
-                                     None, sigmoid=not train, decode=True)
-                torch.cuda.synchronize()
-                outs.append(o2)
-            monkeypatch.delenv("SY_HEAD_PT")
-            assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2]) and torch.equal(outs[0], out)
+            o1 = torch.zeros((b, a_total, 5 + nc), device=DEV)
+            for i in range(b):                         # one image at a time: the one-pixel-per-thread variant
+                ops.head_pred_decode(ops.from_nchw(cf[i:i + 1]), ops.from_nchw(rf[i:i + 1]), wr, br, wo_, bo, wc, bc, stride,
+                                     off, a_total, o1[i:i + 1], None, sigmoid=not train, decode=True)
+            torch.cuda.synchronize()
+            assert torch.equal(o1, out)
 
 
 # ---------------------------------------------------------------------------------------------- backward bricks (SURVEY 8 row a19)

@@ -40,13 +40,6 @@ def run(n, ci, co, h, w, k, s, flags, mode=ops.SY_CONV_RAW):
 SHAPES = [(8, 256, 256, 75, 120, 3, 1), (16, 128, 128, 75, 120, 3, 1), (16, 64, 64, 150, 240, 3, 1), (16, 256, 256, 38, 60, 3, 1),
           (16, 512, 512, 19, 30, 3, 1), (8, 256, 256, 19, 30, 3, 1), (16, 128, 128, 75, 120, 1, 1), (16, 512, 512, 38, 60, 1, 1),
           (16, 64, 128, 300, 480, 3, 2), (16, 1024, 1024, 19, 30, 1, 1)]
-if __name__ == "__main__" and len(sys.argv) > 1 and sys.argv[1] == "stages":
-    for shape in [(16, 128, 128, 75, 120, 3, 1), (8, 256, 256, 75, 120, 3, 1), (16, 64, 64, 150, 240, 3, 1)]:
-        row = []
-        for st in (2, 3, 4, 6, 8):
-            row.append((st, run(*shape, (st << 8)), run(*shape, 2 | (st << 8))))
-        print(shape, " ".join(f"S={a}: full {b:.1f} no-TMA {c:.1f} |" for a, b, c in row))
-    sys.exit(0)
 if __name__ == "__main__":
     for shape in SHAPES:
         t = [run(*shape, f) for f in (0, 2)]

@@ -13,14 +13,14 @@ SHAPES = [(16, 128, 128, 75, 120), (8, 256, 256, 75, 120), (16, 64, 64, 150, 240
           (16, 512, 512, 19, 30), (8, 256, 256, 38, 60), (8, 256, 256, 19, 30)]
 
 
-def run(n, ci, co, h, w, sets=4):
+def run(n, ci, co, h, w, tile_mode, sets=4):
     xs = [View(torch.randn((n, h, w, ci), device="cuda").to(torch.bfloat16)) for _ in range(sets)]
     ys = [View.empty(n, h, w, co, "cuda") for _ in range(sets)]
     wt = ops.pack_conv_weight(torch.randn((co, ci, 3, 3), device="cuda") * 0.05)
     part = torch.empty((ops.conv_stat_rows(), 4 * co), device="cuda")
 
     def go(i):
-        ops.conv2d(xs[i % sets], wt, ys[i % sets], 3, 1, ops.SY_CONV_RAW, partials=part, split_n=n // 2)
+        ops.conv2d(xs[i % sets], wt, ys[i % sets], 3, 1, ops.SY_CONV_RAW, partials=part, split_n=n // 2, tile_mode=tile_mode)
     go(0)
     torch.cuda.synchronize()
     g = torch.cuda.CUDAGraph()
@@ -40,10 +40,8 @@ def run(n, ci, co, h, w, sets=4):
 
 
 for shape in SHAPES:
-    os.environ["SY_CONV_A"] = "off"
-    t_lin, y_lin = run(*shape)
-    os.environ["SY_CONV_A"] = "halo"
-    t_halo, y_halo = run(*shape)
+    t_lin, y_lin = run(*shape, tile_mode=1)
+    t_halo, y_halo = run(*shape, tile_mode=2)
     n, ci, co, h, w = shape
     fl = 2.0 * n * h * w * co * ci * 9
     print(f"{str(shape):28s} linear {t_lin:6.1f} us {fl / t_lin / 1e6:6.0f} TF/s | halo {t_halo:6.1f} us {fl / t_halo / 1e6:6.0f} TF/s | x{t_lin / t_halo:.2f}", flush=True)

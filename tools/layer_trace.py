@@ -13,7 +13,7 @@ from streamyolo_b200.model import DFPPAFPN, TALHead, YOLOX, engine
 a = sys.argv[1:]
 depth, width = float(a[0]) if a else 0.33, float(a[1]) if len(a) > 1 else 0.125
 H, W, B = (int(a[2]), int(a[3]), int(a[4])) if len(a) > 4 else (120, 160, 2)
-os.environ["SY_CONV_IMPL"] = a[5] if len(a) > 5 else "tc"
+engine.CONV_IMPL = a[5] if len(a) > 5 else "tc"
 train = (a[6] if len(a) > 6 else "train") == "train"
 torch.backends.cudnn.allow_tf32 = False
 ch = [256, 512, 1024]
