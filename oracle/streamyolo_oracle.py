@@ -330,18 +330,21 @@ class StreamYoloOracle:
         v = self.pairwise_iou_cxcywh(gt, sup_gt).max(1).values
         return torch.where(v < self.cfg.ignore_thr, torch.full_like(v, self.cfg.ignore_value), v)
 
-    def losses(self, outputs, origin, grid, targets, return_aux=False):
-        """get_losses (tal_head.py:262-470).  targets = (future[B,120,5], current[B,120,5])."""
+    def losses(self, outputs, origin, grid, targets, return_aux=False, dtype=torch.float32):
+        """get_losses (tal_head.py:262-470).  targets = (future[B,120,5], current[B,120,5]).  ``dtype``: precision of the
+        labels, the TAL weights and the loss terms (outputs, origin and grid are expected in it).  The SimOTA assignment is
+        a no-grad constant and always runs in fp32, so a float64 evaluation differentiates the fp32 assignment."""
         c = self.cfg
-        fut, cur = targets[0][..., :5].float(), targets[1][..., :5].float()
+        fut, cur = targets[0][..., :5].to(dtype), targets[1][..., :5].to(dtype)
         B, A, _ = outputs.shape
         gx, gy, gs = grid
+        grid32 = tuple(t.float() for t in grid)
         nl = (fut.sum(2) > 0).sum(1)
         sl = (cur.sum(2) > 0).sum(1)
         fg_all = torch.zeros(B, A, dtype=torch.bool)
         match_all = torch.full((B, A), -1, dtype=torch.int64)
         piou_all = torch.zeros(B, A)
-        tiou_all = torch.zeros(B, A)
+        tiou_all = torch.zeros(B, A, dtype=dtype)
         num_gts = 0
         for b in range(B):
             G, Gs = int(nl[b]), int(sl[b])
@@ -350,18 +353,18 @@ class StreamYoloOracle:
                 continue
             gt, gcls = fut[b, :G, 1:5], fut[b, :G, 0]
             with torch.no_grad():
-                fg, m, pi = self.assign(gt, gcls, outputs[b, :, :4].detach(), outputs[b, :, 4].detach(),
-                                        outputs[b, :, 5:].detach(), grid)
+                fg, m, pi = self.assign(gt.float(), gcls.float(), outputs[b, :, :4].detach().float(),
+                                        outputs[b, :, 4].detach().float(), outputs[b, :, 5:].detach().float(), grid32)
             fg_all[b], match_all[b], piou_all[b] = fg, m, pi
             tio = self.tal_gt_iou(gt, cur[b, :Gs, 1:5])
-            tiou_all[b] = torch.where(fg, tio[m.clamp(min=0)], torch.zeros(A))
+            tiou_all[b] = torch.where(fg, tio[m.clamp(min=0)], torch.zeros(A, dtype=dtype))
         n_fg_raw = int(fg_all.sum())
         num_fg = max(n_fg_raw, 1)
         # gather foreground rows in (image, anchor) order like the reference's torch.cat
         bi, ai = fg_all.nonzero(as_tuple=True)
         gtm = match_all[bi, ai]
         reg_t = fut[bi, gtm, 1:5]
-        cls_t = F.one_hot(fut[bi, gtm, 0].to(torch.int64), c.num_classes).float() * piou_all[bi, ai][:, None]
+        cls_t = F.one_hot(fut[bi, gtm, 0].to(torch.int64), c.num_classes).to(dtype) * piou_all[bi, ai][:, None].to(dtype)
         s, xs, ys = gs[ai], gx[ai], gy[ai]
         l1_t = torch.stack([reg_t[:, 0] / s - xs, reg_t[:, 1] / s - ys,
                             torch.log(reg_t[:, 2] / s + 1e-8), torch.log(reg_t[:, 3] / s + 1e-8)], 1)
@@ -373,9 +376,9 @@ class StreamYoloOracle:
         w4 = w[:, None].expand(-1, 4)
         l1_w = ((w4 * l1_l.sum()) / (w4 * l1_l).sum()).detach()
         loss_iou = (iou_w * iou_l).sum() / num_fg
-        loss_obj = F.binary_cross_entropy_with_logits(outputs[..., 4], fg_all.float(), reduction="sum") / num_fg
+        loss_obj = F.binary_cross_entropy_with_logits(outputs[..., 4], fg_all.to(dtype), reduction="sum") / num_fg
         loss_cls = F.binary_cross_entropy_with_logits(outputs[bi, ai, 5:], cls_t, reduction="sum") / num_fg
-        loss_l1 = (l1_w * l1_l).sum() / num_fg if self.use_l1 else torch.zeros(())
+        loss_l1 = (l1_w * l1_l).sum() / num_fg if self.use_l1 else torch.zeros((), dtype=dtype)
         total = 5.0 * loss_iou + loss_obj + loss_cls + loss_l1
         res = {"total_loss": total, "iou_loss": 5.0 * loss_iou, "l1_loss": loss_l1,
                "conf_loss": loss_obj, "cls_loss": loss_cls, "num_fg": num_fg / max(num_gts, 1)}

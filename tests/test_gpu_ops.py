@@ -273,8 +273,9 @@ def test_spp_and_copy_exact():
     assert torch.equal(s.nchw_float(), ref)
 
 
-@pytest.mark.parametrize("shape", [(2, 64, 15, 20, 8), (2, 64, 15, 20, 3), (1, 32, 9, 11, 80), (8, 256, 75, 120, 8)],
-                         ids=["nc8", "nc3-generic", "nc80-generic", "level0-l"])
+@pytest.mark.parametrize("shape", [(2, 64, 15, 20, 8), (2, 64, 15, 20, 3), (1, 32, 9, 11, 80), (8, 256, 75, 120, 8),
+                                   (2, 64, 15, 20, 1), (2, 64, 15, 20, 20)],
+                         ids=["nc8", "nc3-generic", "nc80-generic", "level0-l", "nc1", "nc20"])
 def test_head_pred_decode(shape):
     """Prediction convs + decode against F.conv2d.  Class counts without a compiled instantiation take the generic kernel
     (the reference head accepts any num_classes, tal_head.py:27); the benchmark's level-0 shape (72 000 pixels) takes the

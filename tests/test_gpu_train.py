@@ -148,79 +148,16 @@ def test_trainer_steps_reduce_the_loss_on_gpu():
 def test_walk_in_situ_every_conv_backward():
     """The assembled backward on the GPU, checked op by op INSIDE the walk: for every recorded BaseConv launch (73 modules,
     DFP jian twice) the BatchNorm+SiLU gradient, the weight gradient and the (accumulated) data gradient the kernels produce
-    are compared with fp32 torch on the very tensors the kernels read (the gradient buffer as it stood, the saved raw
-    output / statistics, the bf16 weights).  Identical inputs per step: no chaos amplification, so bf16-ulp tolerances hold.
+    are compared with float64 torch on the very tensors the kernels read (the gradient buffer as it stood, the saved raw
+    output / statistics, the bf16 weights).  Identical inputs per step: no chaos amplification, so bf16-ulp and fp32-reduction
+    tolerances hold (the checker and its bars: tests/test_gpu_parity_bwd.py, which runs it at the benchmarked sizes).
     Together with the exact routing test on CPU (tests/test_cpu_backward.py) this pins the walk on hardware."""
-    from test_gpu_ops import check_close
+    from test_gpu_parity_bwd import run_walk_checked
     c = CASES["tiny_120x160"]
     x = synth.synth_frames(c["B"], c["H"], c["W"]).cuda()
     tg = tuple(t.cuda() for t in synth.synth_labels(c["B"], c["H"], c["W"]))
     m = build_product(c["depth"], c["width"]).train()
-    snap, seen = {}, []
-
-    def nchw(v):
-        return v.torch().permute(0, 3, 1, 2).float()
-
-    def hook(stage, r, **kw):
-        if stage == "pre":
-            snap["gy"] = nchw(kw["gy"]).clone()
-            snap["dg"] = kw["dgamma"].clone() if kw["acc_bn"] else None
-            snap["db"] = kw["dbeta"].clone() if kw["acc_bn"] else None
-            return
-        if stage == "pre_w":
-            snap["dw"] = kw["dw"].clone() if kw["acc_w"] else None
-            # gx is None when this launch is the first contribution to its input's gradient (written, not accumulated)
-            snap["gx"] = nchw(kw["gx"]).clone() if kw["gx"] is not None else 0.0
-            return
-        mods, raw, xin = r["mods"], nchw(r["raw"]), nchw(r["x"])
-        name = getattr(mods[0], "_sy_name", "?")
-        kh, kw_ = r["k"]
-        s, act = r["s"], r["act"]
-        n = raw.shape[0]
-        sp = r["split"] if 0 < r["split"] < n else n
-        groups = [(0, sp, 0), (sp, n, 1)] if sp < n else [(0, n, 0)]
-        ss, mi, gy = r["ss"], r["mi"], snap["gy"]
-        draw_ref = torch.empty_like(raw)
-        dg, db = torch.zeros(raw.shape[1], device="cuda"), torch.zeros(raw.shape[1], device="cuda")
-        for a, b, g in groups:
-            sc, sh, mu, iv = (t[None, :, None, None] for t in (ss[0, g], ss[1, g], mi[0, g], mi[1, g]))
-            z = raw[a:b] * sc + sh
-            sg = torch.sigmoid(z)
-            dz = gy[a:b] * (sg * (1 + z * (1 - sg))) if act else gy[a:b]
-            xh = (raw[a:b] - mu) * iv
-            m1, m2 = dz.mean((0, 2, 3), keepdim=True), (dz * xh).mean((0, 2, 3), keepdim=True)
-            draw_ref[a:b] = sc * (dz - m1 - xh * m2)
-            dg += (dz * xh).sum((0, 2, 3))
-            db += dz.sum((0, 2, 3))
-        if snap["dg"] is not None:
-            dg, db = dg + snap["dg"], db + snap["db"]
-        draw = nchw(kw["draw"])
-        check_close(draw, draw_ref, f"{name}: d raw", ulp=2.0 ** -6)
-        for got, want, what in ((kw["dgamma"], dg, "dgamma"), (kw["dbeta"], db, "dbeta")):
-            assert torch.allclose(got, want, rtol=5e-3, atol=5e-3 * float(want.abs().max()) + 1e-6), f"{name}: {what}"
-        pad = ((kh - 1) // 2, (kw_ - 1) // 2)
-        dw_ref = torch.nn.grad.conv2d_weight(xin, kw["dw"].shape, draw, stride=s, padding=pad)
-        if snap["dw"] is not None:
-            dw_ref = dw_ref + snap["dw"]
-        scale = float(dw_ref.abs().max()) + 1e-12
-        assert float((kw["dw"] - dw_ref).abs().max()) <= 2e-3 * scale, f"{name}: dw"
-        wq = torch.cat([mm.conv.weight.detach() for mm in mods], 0).to(torch.bfloat16).float()
-        dx_ref = torch.nn.grad.conv2d_input(xin.shape, wq, draw, stride=s, padding=pad) + snap["gx"]
-        check_close(nchw(kw["gx"]), dx_ref, f"{name}: dx (accumulated)", ulp=2.0 ** -6)
-        seen.append(name)
-
-    from streamyolo_b200.model import engine
-    engine.name_modules(m)
-    backward.DEBUG_HOOK = hook
-    backward.POISON = True        # the gradient arena starts as NaN: a region read before it was written would show up
-    try:
-        backward.forward_backward(m, x, tg)
-        torch.cuda.synchronize()
-    finally:
-        backward.DEBUG_HOOK = None
-        backward.POISON = False
-    for n_, p_ in m.named_parameters():
-        assert p_.grad is not None and bool(torch.isfinite(p_.grad).all()), n_
+    seen = run_walk_checked(m, x, tg)
     # 77 BaseConvs: 8 CSP conv2 ride with their conv1, 3 head reg towers with their cls twin, jian x2, the stem has no dx
     assert len(seen) == 77 - 8 - 3 + 3 - 1, len(seen)
 
