@@ -91,7 +91,6 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 p = __floats2bfloat162_rn(a, b);  // .x = a (low half), .y = b
   return *reinterpret_cast<uint32_t*>(&p);
 }
-__device__ __forceinline__ float round_bf16(float a) { return __bfloat162float(__float2bfloat16_rn(a)); }
 
 // SiLU = v * rcp(1 + 2^(-v * log2 e)) on the two approximate SFU ops (ex2.approx, rcp.approx: ~2 ulp fp32, far below
 // the bf16 output rounding) = 5 instructions per value; the normalise pass is issue-bound otherwise (a correctly

@@ -11,14 +11,18 @@
 // [BN][64] weight slab.  Two consumer warpgroups issue wgmma.mma_async (M=64 each, N=BN, K=16) with both operands in
 // shared memory and the fp32 accumulators in registers.
 //
-// Warp roles (640 threads = five warpgroups, persistent CTA, one per SM):
-//   warps 0-7   MMA + convert: warpgroup wg computes rows [64 wg, +64) of the tile, then per 64-column slab converts its
+// Warp roles (640 threads = five warpgroups, persistent CTA, one per SM), one function each:
+//   warps 0-7   mma_convert: warpgroup wg computes rows [64 wg, +64) of the tile, then per 64-column slab converts its
 //               accumulators (raw | folded BN + SiLU + residual) to bf16 in a 128B-swizzled shared staging tile
 //   warps 8-15  statistics: per-channel (sum, sum of squares) of the staged tile in per-lane register accumulators that persist
 //               across slabs and tiles (overlaps the next slab's conversion)
-//   warp 16 TMA store (one 4-D store per slab; the tensor map clips the tile to the tensor / the channel slice)
-//   warp 17 barrier init + weight (B) loads   warp 18 activation (A) loads   warp 19 idle
-// setmaxnreg moves registers from warps 16-19 to the MMA and statistics warpgroups (kRegs*).
+//   warps 0-15  bn_tail after either role: partial row, grid barrier, BatchNorm finalize
+//   warp 16 store_slabs: TMA store (one 4-D store per slab; the tensor map clips the tile to the tensor / the channel slice)
+//   warp 17 barrier init + weight (B) loads   warp 18 activation (A) loads: load_linear | load_halo_b, load_halo_a
+//   warp 19 idle
+// The kernel body carves up shared memory, initialises the barriers and dispatches the roles; every role walks the tiles
+// through TileWalk.  setmaxnreg at the start of each branch moves registers from warps 16-19 to the MMA and statistics
+// warpgroups (kRegs*).
 // BN = 256 is not offered: 64 x 256 fp32 accumulators are 128 registers per thread, more than the MMA warpgroups can hold.
 //
 // Train-mode BatchNorm is folded into this kernel as far as the grid-wide dependency allows:
@@ -75,12 +79,12 @@ struct BnSeg {
 };
 
 struct Params {
-  int N, Ho, Wo, Cout, Cin;
-  int kh, kw, stride, pad_h, pad_w;
+  int N, Ho, Wo, Cout;
+  int kw, stride, pad_h, pad_w;
   int tiles_x, tiles_y;     // halo mode: 16 x 8 patches per image row / column
   int m_tiles, n_tiles;
   FastDiv fd_m_tiles, fd_per_img, fd_tiles_x;
-  // tile walk (pick_walk; see tile_nm in the kernel) and the statistics rows it fills
+  // tile walk (pick_walk; see TileWalk) and the statistics rows it fills
   int band, t_end, cls_step, cls_tiles;
   int stat_rows;            // partial rows the finalize sums (N-major: one per CTA; M-band: one per class)
   FastDiv fd_band, fd_cls_tiles;
@@ -92,8 +96,6 @@ struct Params {
   int stage_tiles;          // 1 or 2 epilogue staging tiles
   int stagesA;              // halo mode: halo ring depth
   int mode, act;
-  __nv_bfloat16* y;
-  long long y_pitch;
   const __nv_bfloat16* res;
   long long res_pitch;
   const float* scale;
@@ -159,6 +161,737 @@ struct Cfg {
   static constexpr int kFixedBytes = 1024 /*align slack*/ + kSlabBytes + 256 /*barriers*/;
 };
 
+// Tile walk of this CTA (pick_walk).  Every member is an expression of the kernel parameters and blockIdx, not a stored
+// value: those cost no registers.
+//   band == 1 (N-major): walk index = tile index, M fastest.
+//   band == n_tiles (M-band): CTA b = slot * band + N tile; walk index t = class * cls_tiles + k visits M tile rho + k *
+//   stat_rows of class rho = slot + class * cls_step.
+// decode() is false for walk indices that name no tile (every role skips them alike).
+struct TileWalk {
+  const Params& p;
+  __device__ __forceinline__ int first() const { return p.band > 1 ? 0 : (int)blockIdx.x; }
+  __device__ __forceinline__ int step() const { return p.band > 1 ? 1 : (int)gridDim.x; }
+  __device__ __forceinline__ int end() const { return p.t_end; }
+  __device__ __forceinline__ bool mband() const { return p.band > 1; }
+  // M-band walk: this CTA's slot (a fast division: callers evaluate it once) and N tile, the class of walk index t
+  __device__ __forceinline__ int slot() const { return fdiv((int)blockIdx.x, p.fd_band); }
+  __device__ __forceinline__ int band_n_tile(int slot) const { return (int)blockIdx.x - slot * p.band; }
+  __device__ __forceinline__ int cls(int t) const { return fdiv(t, p.fd_cls_tiles); }
+  // partial row of class cls (M-tile class rho = slot + cls * cls_step): the N-major walk's CTA (n_tile * m_tiles + rho)
+  // mod stat_rows
+  __device__ __forceinline__ int class_row(int slot, int cls) const {
+    return (int)(((long long)band_n_tile(slot) * p.m_tiles + slot + cls * p.cls_step) % p.stat_rows);
+  }
+  __device__ __forceinline__ bool decode(int t, int& n_tile, int& m_tile) const {
+    if (p.band == 1) {
+      n_tile = fdiv(t, p.fd_m_tiles);
+      m_tile = t - n_tile * p.m_tiles;
+      return true;
+    }
+    const int s = slot();
+    n_tile = band_n_tile(s);
+    const int c = cls(t);
+    const int r = s + c * p.cls_step;
+    m_tile = r + (t - c * p.cls_tiles) * p.stat_rows;
+    return r < p.stat_rows && m_tile < p.m_tiles;
+  }
+};
+
+// position in a ring of mbarrier-guarded stages: the stage and the parity of its current phase
+struct RingCursor {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance(int depth) {
+    if (++stage == depth) { stage = 0; phase ^= 1u; }
+  }
+};
+
+// first output pixel of an M tile as (image, row, column): the top-left corner of a halo patch, the first of 128
+// consecutive pixels of a linear tile
+struct TileOrigin {
+  int img, y, x;
+};
+__device__ __forceinline__ TileOrigin halo_origin(const Params& p, int m_tile) {
+  const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * (p.tiles_x * p.tiles_y);
+  const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
+  return {img, py * kHaloTH, px * kHaloTW};
+}
+__device__ __forceinline__ TileOrigin linear_origin(const Params& p, int m_tile) {
+  const int p0 = m_tile * kBlockM;
+  const int img = fdiv(p0, p.fd_hw);
+  const int rem = p0 - img * (p.Ho * p.Wo);
+  const int oh = fdiv(rem, p.fd_wo), ow = rem - oh * p.Wo;
+  return {img, oh, ow};
+}
+
+// the BatchNorm (segment) that channel c belongs to
+__device__ __forceinline__ const BnSeg& bn_seg(const Params& p, int c) {
+  return (p.n_seg > 1 && c >= p.seg[1].c_begin) ? p.seg[1] : p.seg[0];
+}
+
+// Shared memory of a CTA as the roles see it (carved up in conv_tc_kernel)
+struct Smem {
+  uint8_t* a;            // A ring: linear stages of kABytes | halo stages of kHaloBytes
+  uint8_t* b;            // B ring: one weight slab per stage | halo mode: kHaloTaps slabs per stage
+  uint8_t* stage;        // Params::stage_tiles epilogue staging tiles (1024-aligned: the rings are multiples of 1 KiB)
+  float* acc;            // RAW: statistic accumulators [2 groups][2][Cout]; FUSED: [256] scale, [256] shift
+  uint32_t bar0;         // mbarriers: [0,8) full, [8,16) empty, [16,19) halo full, [19,22) halo empty
+  int sflip;             // slab parity toggles the staging tile iff there are two
+  __device__ __forceinline__ uint32_t full(int s) const { return bar0 + 8u * s; }
+  __device__ __forceinline__ uint32_t empty(int s) const { return bar0 + 8u * (kMaxStages + s); }
+  __device__ __forceinline__ uint32_t full_a(int s) const { return bar0 + 8u * (2 * kMaxStages + s); }   // halo ring (<= 3)
+  __device__ __forceinline__ uint32_t empty_a(int s) const { return bar0 + 8u * (2 * kMaxStages + 3 + s); }
+};
+
+// ---------------------------------------------------------------- warp 18, halo mode: activation (A) loads
+// one halo box [18 rows][10 px][64 ch] per (tile, channel block)
+__device__ __forceinline__ void load_halo_a(const Params& p, const Smem& sm, const CUtensorMap& tmA) {
+  const TileWalk w{p};
+  RingCursor ra;
+  for (int tile = w.first(); tile < w.end(); tile += w.step()) {
+    int n_tile, m_tile;
+    if (!w.decode(tile, n_tile, m_tile)) continue;
+    const TileOrigin o = halo_origin(p, m_tile);
+    for (int cb = 0; cb < p.cblocks; ++cb) {
+      mbar_wait(sm.empty_a(ra.stage), ra.phase ^ 1u);
+      if (elect_one()) {
+        if (p.debug_flags & 2) {
+          mbar_arrive(sm.full_a(ra.stage));
+        } else {
+          mbar_expect_tx(sm.full_a(ra.stage), (uint32_t)kHaloTx);
+          tma_load_4d(smem_u32(sm.a + ra.stage * kHaloBytes), &tmA, sm.full_a(ra.stage), cb * kBlockK, o.x - 1, o.y - 1, o.img);
+        }
+      }
+      __syncwarp();
+      ra.advance(p.stagesA);
+    }
+  }
+}
+
+// ---------------------------------------------------------------- warp 17, halo mode: weight (B) loads
+// kHaloTaps [BN][64] weight slabs (one filter row) per (channel block, ring stage)
+template <int BN>
+__device__ __forceinline__ void load_halo_b(const Params& p, const Smem& sm, const CUtensorMap& tmB) {
+  constexpr int kBB = Cfg<BN>::kBBytes;
+  const TileWalk w{p};
+  RingCursor rb;
+  for (int tile = w.first(); tile < w.end(); tile += w.step()) {
+    int n_tile, m_tile_unused;
+    if (!w.decode(tile, n_tile, m_tile_unused)) continue;
+    for (int cb = 0; cb < p.cblocks; ++cb) {
+      for (int t0 = 0; t0 < 9; t0 += kHaloTaps) {
+        mbar_wait(sm.empty(rb.stage), rb.phase ^ 1u);
+        if (elect_one()) {
+          if (p.debug_flags & 2) {
+            mbar_arrive(sm.full(rb.stage));
+          } else {
+            mbar_expect_tx(sm.full(rb.stage), (uint32_t)(kHaloTaps * kBB));
+#pragma unroll
+            for (int j = 0; j < kHaloTaps; ++j)
+              tma_load_3d(smem_u32(sm.b + (rb.stage * kHaloTaps + j) * kBB), &tmB, sm.full(rb.stage), cb * kBlockK, t0 + j,
+                          n_tile * BN);
+          }
+        }
+        __syncwarp();
+        rb.advance(p.stages);
+      }
+    }
+  }
+}
+
+// ---------------------------------------------------------------- warps 17 / 18, linear tiles: B / A loads
+// Two issuing threads because a single thread needs a few hundred cycles per cp.async.bulk.tensor: the pair keeps a
+// K block's issue time below its MMA time.  Both arrive (with their byte counts) on the same full barrier.
+template <int BN, bool TL>
+__device__ __forceinline__ void load_linear(const Params& p, const Smem& sm, const CUtensorMap& tmA, const CUtensorMap& tmB,
+                                            bool is_a) {
+  constexpr int kBB = Cfg<BN>::kBBytes;
+  const TileWalk w{p};
+  RingCursor ring;
+  int tl_n = is_a ? 0 : p.timeline_cap / 8;
+  for (int tile = w.first(); tile < w.end(); tile += w.step()) {
+    int n_tile, m_tile;
+    if (!w.decode(tile, n_tile, m_tile)) continue;
+    const TileOrigin o = linear_origin(p, m_tile);
+    const int y0 = o.y * p.stride - p.pad_h, x0 = o.x * p.stride - p.pad_w;
+    // walk the (tap, channel block) K blocks, one per ring stage
+    int r = 0, sx = 0, cb = 0;
+    for (int kb = 0; kb < p.kblocks; ++kb) {
+      mbar_wait(sm.empty(ring.stage), ring.phase ^ 1u);          // whole warp waits: control flow stays uniform
+      if (elect_one()) {
+        tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 0, tile, kb);
+        if (p.debug_flags & 2) mbar_arrive(sm.full(ring.stage));
+        else mbar_expect_tx(sm.full(ring.stage), is_a ? (uint32_t)kABytes : (uint32_t)kBB);
+        tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 1, tile, kb);
+      }
+      if (!(p.debug_flags & 2) && elect_one()) {
+        if (is_a)
+          tma_load_im2col_4d(smem_u32(sm.a + ring.stage * kABytes), &tmA, sm.full(ring.stage), cb * kBlockK, x0, y0, o.img,
+                             (uint16_t)sx, (uint16_t)r);
+        else
+          tma_load_3d(smem_u32(sm.b + ring.stage * kBB), &tmB, sm.full(ring.stage), cb * kBlockK, r * p.kw + sx, n_tile * BN);
+      }
+      if (++cb == p.cblocks) { cb = 0; if (++sx == p.kw) { sx = 0; ++r; } }
+      if (TL && elect_one()) tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 2, tile, kb);
+      __syncwarp();
+      ring.advance(p.stages);
+    }
+  }
+}
+
+// ---------------------------------------------------------------- warp 16: TMA store
+// One 4-D TMA store per 64-column slab; the tensor map clips the patch to the image and to the
+// channel slice.  Issuing it here keeps its issue + drain latency off the epilogue warps' path.
+template <int BN, bool TL, int AM>
+__device__ __forceinline__ void store_slabs(const Params& p, const Smem& sm, const CUtensorMap& tmY, int tid) {
+  const int lane = tid & 31;
+  const TileWalk w{p};
+  const int sflip = sm.sflip;
+  const uint32_t stage_base = smem_u32(sm.stage);
+  int sbuf = 0, prev = -1;
+  int tl_s = 7 * (p.timeline_cap / 8);
+  const int nbar = 544;
+  bar_free_arrive(0, nbar);                    // both tiles start out free
+  if (sflip) bar_free_arrive(1, nbar);
+  for (int tile = w.first(); tile < w.end(); tile += w.step()) {
+    int n_tile, m_tile;
+    if (!w.decode(tile, n_tile, m_tile)) continue;
+    int c1, c2, c3;                            // store coordinates below the channel: (x, y, image) | (pixel, 0, 0)
+    if constexpr (AM == 1) {
+      c1 = m_tile * kBlockM; c2 = 0; c3 = 0;
+    } else {
+      const TileOrigin o = halo_origin(p, m_tile);
+      c1 = o.x; c2 = o.y; c3 = o.img;
+    }
+    for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
+      bar_staged_wait(sbuf, nbar);
+      if (lane == 0) tl_rec<TL>(p, tl_s, 6, 0, tile, slab);
+      if (elect_one()) {
+        tma_store_4d(&tmY, stage_base + (uint32_t)(sbuf * kSlabBytes), n_tile * BN + slab * kSlabCols, c1, c2, c3);
+        bulk_commit();
+        if (sflip) {
+          if (prev >= 0) bulk_wait_read1();    // two tiles: the previous slab's store has read ITS tile
+        } else {
+          bulk_wait_read();                    // one tile: wait until this store has read it
+        }
+      }
+      __syncwarp();
+      if (lane == 0) tl_rec<TL>(p, tl_s, 6, 1, tile, slab);
+      if (sflip) {
+        if (prev >= 0) bar_free_arrive(prev, nbar);
+        prev = sbuf;
+      } else {
+        bar_free_arrive(0, nbar);
+      }
+    }
+  }
+  if (sflip && prev >= 0) {
+    if (elect_one()) bulk_wait_read();
+    __syncwarp();
+    bar_free_arrive(prev, nbar);
+  }
+  // the stores have read the staging tiles before the CTA's final __syncthreads; their writes complete with the grid
+  if (lane == 0) bulk_wait_read();
+  __syncwarp();
+}
+
+// ---------------------------------------------------------------- warps 8-15: statistics
+// Warp ew reduces columns [8*ew, 8*ew+8) of every staged 64-column slab while the convert warps already
+// convert the next slab; one owner lane per (column, sum|sumsq) accumulates in fixed order.
+template <int BN, bool TL, int AM>
+__device__ __forceinline__ void statistics(const Params& p, const Smem& sm, int tid) {
+  const int warp = tid >> 5, lane = tid & 31;
+  const TileWalk w{p};
+  float* sAcc = sm.acc;
+  const int sflip = sm.sflip;
+  const int ew = warp - 8;
+  const int st = tid - 256;                    // 0..255
+  const uint32_t stage_base = smem_u32(sm.stage);
+  const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
+  if (do_stats) {
+    for (int i = st; i < 4 * p.Cout; i += 256) sAcc[i] = 0.f;
+  }
+  int sbuf = 0;
+  int tl_t = (st == 0) ? 5 * (p.timeline_cap / 8) : p.timeline_cap;
+  const int nbar = 544;
+  bar_free_arrive(0, nbar);                    // both tiles start out free
+  if (sflip) bar_free_arrive(1, nbar);
+  // Warp ew owns columns [8*ew, 8*ew+8) of every 64-column slab; lane l reads rows l, l+32, l+64, l+96 (one 16-byte
+  // chunk each).  The per-lane partial sums (8 columns x {sum, sum of squares}) stay in REGISTERS across slabs and tiles
+  // -- one set per slab index of the tile -- and are only combined across the 32 lanes (recursive-halving shuffles) and
+  // added to the CTA's shared-memory totals on a FLUSH: when the CTA moves to another n tile (N-major walk only) or
+  // statistics group, on a tile that straddles the group boundary, and at the end.  (Per-slab shuffle reductions made the statistics warps the
+  // bottleneck of every epilogue-bound layer: ~1400 cycles per slab.)
+  constexpr int kSlabs = BN / kSlabCols;
+  float acc[kSlabs][16];
+#pragma unroll
+  for (int j = 0; j < kSlabs; ++j)
+#pragma unroll
+    for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
+  int pend_grp = -1, pend_n0 = 0;                          // what the register sums belong to (-1: nothing pending)
+  // lanes combine a[16] (fixed shuffle tree: deterministic) and the 16 owner lanes add into the shared totals
+  auto reduce_store = [&](float (&a)[16], int grp, int col_base) {
+    float b8[8], c4[4], d2[2], e1;
+    {
+      const bool up = (lane & 16) != 0;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        const float send = up ? a[i] : a[8 + i], keep = up ? a[8 + i] : a[i];
+        b8[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
+      }
+    }
+    {
+      const bool up = (lane & 8) != 0;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float send = up ? b8[i] : b8[4 + i], keep = up ? b8[4 + i] : b8[i];
+        c4[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
+      }
+    }
+    {
+      const bool up = (lane & 4) != 0;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float send = up ? c4[i] : c4[2 + i], keep = up ? c4[2 + i] : c4[i];
+        d2[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
+      }
+    }
+    {
+      const bool up = (lane & 2) != 0;
+      const float send = up ? d2[0] : d2[1], keep = up ? d2[1] : d2[0];
+      e1 = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+    }
+    e1 += __shfl_xor_sync(0xffffffffu, e1, 1);
+    if ((lane & 1) == 0) {               // 16 owner lanes: bit4 = sum | sumsq, bits 3..1 = column in the group
+      const int col = col_base + ew * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
+      if (col < p.Cout) sAcc[(grp * 2 + (lane >> 4)) * p.Cout + col] += e1;
+    }
+#pragma unroll
+    for (int i = 0; i < 16; ++i) a[i] = 0.f;
+  };
+  auto flush = [&]() {
+    if (pend_grp < 0) return;
+#pragma unroll
+    for (int j = 0; j < kSlabs; ++j) reduce_store(acc[j], pend_grp, pend_n0 + j * kSlabCols);
+    pend_grp = -1;
+  };
+  // M-band walk: the CTA's tiles of one class rho are exactly those that one CTA of the N-major walk took for this N tile,
+  // in the same order, so this CTA's sums of a class are that CTA's partial row for these BN columns, bit for bit.  The
+  // row of class rho is the N-major walk's CTA (n_tile * m_tiles + rho) mod stat_rows; classes without tiles write zeros.
+  auto write_class = [&](int cls, bool zero) {                 // all 256 statistics threads
+    const int my_slot = w.slot();
+    float4* dst = reinterpret_cast<float4*>(p.partials) + (size_t)w.class_row(my_slot, cls) * p.Cout;
+    const int c = w.band_n_tile(my_slot) * BN + st;
+    if (zero) {
+      if (st < BN && c < p.Cout) dst[c] = make_float4(0.f, 0.f, 0.f, 0.f);
+      return;
+    }
+    asm volatile("bar.sync 8, 256;" ::: "memory");          // the owner lanes' shared-memory sums are complete
+    if (st < BN && c < p.Cout) {
+      dst[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
+      sAcc[c] = 0.f; sAcc[p.Cout + c] = 0.f; sAcc[2 * p.Cout + c] = 0.f; sAcc[3 * p.Cout + c] = 0.f;
+    }
+    asm volatile("bar.sync 8, 256;" ::: "memory");
+  };
+  int pend_cls = -1;                                           // class whose sums sAcc holds (M-band walk)
+  if (do_stats && w.mband()) {
+    const int my_slot = w.slot();
+    for (int cls = 0; my_slot + cls * p.cls_step < p.stat_rows; ++cls)
+      if (my_slot + cls * p.cls_step >= p.m_tiles) write_class(cls, true);
+  }
+  for (int tile = w.first(); tile < w.end(); tile += w.step()) {
+    int n_tile, m_tile;
+    if (!w.decode(tile, n_tile, m_tile)) continue;
+    const int n0 = n_tile * BN;
+    // rows [0, cut) of the tile belong to statistics group 0, rows [cut, 128) to group 1 (a halo tile lies in one
+    // image = one group; a linear tile can straddle the boundary; rows past the end of the tensor were staged as zeros)
+    int cut;
+    if constexpr (AM == 1) {
+      cut = min(max(p.gp - m_tile * kBlockM, 0), kBlockM);
+    } else {
+      cut = fdiv(m_tile, p.fd_per_img) >= p.split_n ? 0 : kBlockM;
+    }
+    const bool pure = (cut <= 0) || (cut >= kBlockM);
+    const int tgrp = cut <= 0 ? 1 : 0;
+    if (do_stats && w.mband()) {                               // warp-uniform
+      const int cls = w.cls(tile);
+      if (pend_cls >= 0 && cls != pend_cls) {
+        flush();
+        write_class(pend_cls, false);
+      }
+      pend_cls = cls;
+    }
+    if (do_stats && (!pure || pend_grp != tgrp || pend_n0 != n0)) flush();     // warp-uniform
+    for (int slab = 0; slab < kSlabs; ++slab, sbuf ^= sflip) {
+      bar_staged_wait(sbuf, nbar);
+      tl_rec<TL>(p, tl_t, 5, 0, tile, slab);
+      const uint32_t tile_base = stage_base + (uint32_t)(sbuf * kSlabBytes);
+      float x[4][8];
+      if (do_stats) {
+#pragma unroll
+        for (int rr = 0; rr < 4; ++rr) {
+          const uint32_t r = (uint32_t)(lane + 32 * rr);
+          const uint4 u = lds128(tile_base + r * 128u + ((((uint32_t)ew) ^ (r & 7u)) << 4));
+          x[rr][0] = bf16_lo(u.x); x[rr][1] = bf16_hi(u.x); x[rr][2] = bf16_lo(u.y); x[rr][3] = bf16_hi(u.y);
+          x[rr][4] = bf16_lo(u.z); x[rr][5] = bf16_hi(u.z); x[rr][6] = bf16_lo(u.w); x[rr][7] = bf16_hi(u.w);
+        }
+      }
+      bar_free_arrive(sbuf, nbar);             // the values are in registers: the tile may be overwritten
+      tl_rec<TL>(p, tl_t, 5, 1, tile, slab);
+      if (do_stats) {
+        if (pure) {
+          float (&a)[16] = acc[slab];
+#pragma unroll
+          for (int rr = 0; rr < 4; ++rr) {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) { a[i] += x[rr][i]; a[8 + i] += x[rr][i] * x[rr][i]; }
+          }
+          pend_grp = tgrp; pend_n0 = n0;
+        } else {
+          // the tile straddles the group boundary (at most one M tile per layer and N tile): masked, reduced at once.
+          // The sums go through acc[slab]: the flush before this tile left it zero, and reduce_store zeroes it again
+          // (a separate scratch array made the BN = 64 statistics warps spill)
+#pragma unroll 1
+          for (int grp = 0; grp < 2; ++grp) {
+            const int lo = grp ? cut : 0, hi = grp ? kBlockM : cut;
+            float (&a)[16] = acc[slab];
+#pragma unroll
+            for (int rr = 0; rr < 4; ++rr) {
+              const int r = lane + 32 * rr;
+              if (r >= lo && r < hi) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) { a[i] += x[rr][i]; a[8 + i] += x[rr][i] * x[rr][i]; }
+              }
+            }
+            reduce_store(a, grp, n0 + slab * kSlabCols);
+          }
+        }
+      }
+      tl_rec<TL>(p, tl_t, 5, 2, tile, slab);
+    }
+  }
+  if (do_stats) flush();
+  if (do_stats && w.mband() && pend_cls >= 0) write_class(pend_cls, false);
+}
+
+// ---------------------------------------------------------------- warps 0-7: MMA + convert
+// Warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile: it issues the wgmma stream for them (accumulators in
+// registers), then converts its rows of every 64-column slab into the staging tile.  A ring stage is handed back to the
+// producers one commit group late (wgmma.wait_group 1), so the next group's MMAs are queued while the last ones drain.
+// Returns the debug-timeline cursor of thread 0, which the kernel tail carries on.
+template <int BN, bool TL, int AM>
+__device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int tid) {
+  // the compiler knows this range for threadIdx.x but not for the argument; with it the FUSED scale/shift fill below is
+  // one guarded pass instead of a loop
+  __builtin_assume(tid >= 0 && tid < kThreads);
+  using C = Cfg<BN>;
+  constexpr bool LIN = (AM == 1);
+  constexpr bool HALO = (AM == 2);
+  constexpr int kBB = C::kBBytes;
+  const TileWalk w{p};
+  const int sflip = sm.sflip;
+  float* sScale = sm.acc;
+  float* sShift = sScale + 256;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;
+  const int et = tid;                                            // 0..255
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);        // this thread's tile rows: r0 and r0 + 8
+  const int cq = 2 * (lane & 3);                                 // its first column in every 8-column group
+  const uint32_t stage_base = smem_u32(sm.stage);
+  const bool lead = (tid & 127) == 0;                            // signals the warpgroup's ring releases
+  // halo mode: this warpgroup's 8 output rows start 8 halo rows further down
+  constexpr uint32_t row_bytes = HALO ? (uint32_t)kHaloPitch * 128u : 1024u;
+  const uint32_t a_off = HALO ? (uint32_t)(wg * 8) * row_bytes : (uint32_t)wg * 8192u;
+  float acc[C::kAcc];
+  RingCursor ring, ring_a;                                       // B ring (linear: A+B ring) | halo ring
+  int sbuf = 0;
+  int tl_n = (et == 0) ? p.timeline_cap / 2 : p.timeline_cap;
+  for (int tile = w.first(); tile < w.end(); tile += w.step()) {
+    int n_tile, m_tile;
+    if (!w.decode(tile, n_tile, m_tile)) continue;
+    // this thread's output pixels in the flattened (n, oh, ow) space (evaluated where they are used: only the
+    // validity flags stay live across the main loop)
+    auto pixel = [&](int h, bool& ok) -> long long {
+      if constexpr (LIN) {
+        const long long px = (long long)m_tile * kBlockM + r0 + 8 * h;
+        ok = px < p.P_total;
+        return px;
+      } else {
+        const TileOrigin o = halo_origin(p, m_tile);
+        const int row = r0 + 8 * h;
+        const int oy = o.y + row / kHaloTW, ox = o.x + row % kHaloTW;
+        ok = (oy < p.Ho) && (ox < p.Wo);
+        return ((long long)o.img * p.Ho + oy) * p.Wo + ox;
+      }
+    };
+    bool valid[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) pixel(h, valid[h]);
+    const int n0 = n_tile * BN;
+    tl_rec<TL>(p, tl_n, 2, 0, tile, 0);
+    if (p.mode == SY_CONV_FUSED) {
+      epi_bar();                               // previous tile's readers of sScale/sShift are done
+      for (int c = et; c < BN; c += kEpiThreads) {
+        const int cg = n0 + c;
+        sScale[c] = (cg < p.Cout && p.scale) ? p.scale[cg] : 1.0f;
+        sShift[c] = (cg < p.Cout && p.shift) ? p.shift[cg] : 0.0f;
+      }
+      epi_bar();
+    }
+    // ---- main loop
+    int pend_b = -1, pend_a = -1;              // ring stages read by the commit group still in flight
+    auto release = [&]() {
+      if (lead) {
+        if (pend_b >= 0) mbar_arrive(sm.empty(pend_b));
+        if (pend_a >= 0) mbar_arrive(sm.empty_a(pend_a));
+      }
+    };
+    if constexpr (HALO) {                      // K order = (channel block, tap)
+      for (int cb = 0; cb < p.cblocks; ++cb) {
+        mbar_wait(sm.full_a(ring_a.stage), ring_a.phase);
+        const uint32_t halo = smem_u32(sm.a + ring_a.stage * kHaloBytes) + a_off;
+        for (int t0 = 0; t0 < 9; t0 += kHaloTaps) {
+          mbar_wait(sm.full(ring.stage), ring.phase);
+          wgmma_fence_operand(acc);
+          wgmma_fence();
+#pragma unroll
+          for (int j = 0; j < kHaloTaps; ++j) {
+            const int tap = t0 + j;
+            const int r = tap / 3, sx = tap - 3 * r;
+            const uint32_t a_addr = halo + (uint32_t)r * row_bytes + (uint32_t)sx * 128u;
+            const uint64_t da = make_smem_desc(a_addr, row_bytes);
+            const uint64_t db = make_smem_desc(smem_u32(sm.b + (ring.stage * kHaloTaps + j) * kBB));
+#pragma unroll
+            for (int k = 0; k < kBlockK / 16; ++k)   // 16 bf16 = 32 bytes along K inside the swizzle row: +2 in (addr >> 4)
+              Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (cb | tap | k) != 0);
+          }
+          wgmma_commit();
+          wgmma_fence_operand(acc);
+          wgmma_wait<1>();
+          release();
+          pend_b = ring.stage;
+          pend_a = (t0 + kHaloTaps >= 9) ? ring_a.stage : -1;     // the halo is free after its ninth tap
+          ring.advance(p.stages);
+        }
+        ring_a.advance(p.stagesA);
+      }
+    } else {
+      for (int kb = 0; kb < p.kblocks; ++kb) {
+        mbar_wait(sm.full(ring.stage), ring.phase);
+        wgmma_fence_operand(acc);
+        wgmma_fence();
+        const uint64_t da = make_smem_desc(smem_u32(sm.a + ring.stage * kABytes) + a_off);
+        const uint64_t db = make_smem_desc(smem_u32(sm.b + ring.stage * kBB));
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k)
+          Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
+        wgmma_commit();
+        wgmma_fence_operand(acc);
+        wgmma_wait<1>();
+        release();
+        pend_b = ring.stage;
+        ring.advance(p.stages);
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_operand(acc);
+    release();
+    tl_rec<TL>(p, tl_n, 2, 1, tile, 0);
+    // ---- epilogue: per 64-column slab, registers -> (raw | folded BN + SiLU + residual) -> bf16 -> staging tile
+#pragma unroll
+    for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
+      tl_rec<TL>(p, tl_n, 2, 2, tile, slab);
+      bar_free_wait(sbuf);                     // (A) staging tile free: its store has read it, the statistics loads are done
+      // 16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) << 4); this thread's rows r0 and r0 + 8 share r & 7,
+      // so the chunk offset is (j << 4) ^ sw: one logic op, nothing kept live across the main loop
+      const uint32_t tb = stage_base + (uint32_t)(sbuf * kSlabBytes) + (uint32_t)cq * 2u + (uint32_t)r0 * 128u;
+      const uint32_t sw = ((uint32_t)r0 & 7u) << 4;
+      if (p.mode == SY_CONV_RAW && p.dbg_f32 == nullptr) {
+        // raw values (every conv of a training step): round, pack and stage -- no per-value pixel or column arithmetic
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int J = slab * 8 + j;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
+                         "r"(valid[h] ? pack_bf16(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]) : 0u) : "memory");
+        }
+      } else {
+        long long pix[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          bool ok;
+          pix[h] = pixel(h, ok);
+        }
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int J = slab * 8 + j;
+          const int cl = slab * kSlabCols + j * 8 + cq;          // tile column of this thread's first value
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float v0 = acc[4 * J + 2 * h], v1 = acc[4 * J + 2 * h + 1];
+            const bool inb = valid[h] && n0 + cl < p.Cout;
+            if (p.dbg_f32 != nullptr && inb)     // validation only: the accumulators before any rounding
+              *reinterpret_cast<float2*>(p.dbg_f32 + pix[h] * p.Cout + n0 + cl) = make_float2(v0, v1);
+            if (p.mode != SY_CONV_RAW) {
+              v0 = v0 * sScale[cl] + sShift[cl];
+              v1 = v1 * sScale[cl + 1] + sShift[cl + 1];
+              if (p.act) { v0 = silu_f(v0); v1 = silu_f(v1); }
+              if (p.res != nullptr && inb) {
+                const uint32_t rv = *reinterpret_cast<const uint32_t*>(p.res + pix[h] * p.res_pitch + n0 + cl);
+                v0 += bf16_lo(rv);
+                v1 += bf16_hi(rv);
+              }
+            }
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
+                         "r"(valid[h] ? pack_bf16(v0, v1) : 0u) : "memory");
+          }
+        }
+      }
+      fence_proxy_async();                     // generic-proxy writes -> visible to the TMA (async proxy)
+      bar_staged_arrive(sbuf);                 // (B) staging tile complete: store + statistics warps take it from here
+      tl_rec<TL>(p, tl_n, 2, 3, tile, slab);
+    }
+  }
+  bar_free_wait(0);                                // drain the last arrivals (balanced barriers at exit)
+  if (sflip) bar_free_wait(1);
+  return tl_n;
+}
+
+// ---------------------------------------------------------------- warps 0-15: per-CTA partial row, grid barrier, BatchNorm finalize
+// Run by the 16 convert + statistics warps (512 threads), called at the end of both of their roles so that each copy is
+// compiled under that warpgroup's register budget.  tl: debug-timeline cursor (thread 0 records).
+template <bool TL>
+__device__ __forceinline__ void bn_tail(const Params& p, const Smem& sm, int tid, int& tl) {
+  const int warp = tid >> 5, lane = tid & 31;
+  const float* sAcc = sm.acc;
+  const int et = tid;                                // 0..511
+  const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
+  if (et == 0) tl_rec<TL>(p, tl, 4, 2, 0, 0);
+  bar_stats_done();                                // every sAcc update is done
+  if (!do_stats) return;
+  // partial row of this CTA, channel-major: the four sums of a channel are one 16-byte word (the finalize below loads
+  // one word per row and channel; with the shared-memory layout [4][Cout] in global memory it needed four loads, and the
+  // 640 sector requests per warp made the partial-row sums the longest part of the tail)
+  // (M-band walk: the statistics warps wrote this CTA's class rows already)
+  if (p.band == 1) {
+    float4* mine = reinterpret_cast<float4*>(p.partials) + (size_t)blockIdx.x * p.Cout;
+    for (int c = et; c < p.Cout; c += kTailThreads)
+      mine[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
+  }
+  if (p.n_seg == 0) return;
+  if (et == 0) tl_rec<TL>(p, tl, 4, 5, 0, 0);
+  // This CTA finalizes channels [b*cpc, (b+1)*cpc), one warp per channel.  The BatchNorm parameters and running
+  // statistics of the warp's first channel do not depend on the other CTAs: load them BEFORE the grid barrier (they
+  // come from DRAM -- behind the barrier their latency, twice in a row, was most of the finalize)
+  const int groups = p.split_n < p.N ? 2 : 1;
+  const int cpc = (p.Cout + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int c_end = min(p.Cout, ((int)blockIdx.x + 1) * cpc);
+  const int c_first = (int)blockIdx.x * cpc + warp;
+  float pre_gamma = 1.f, pre_beta = 0.f, pre_rm = 0.f, pre_rv = 1.f;
+  if (c_first < c_end && lane < 2) {
+    const BnSeg& sg = bn_seg(p, c_first);
+    const int cs = c_first - sg.c_begin;
+    pre_gamma = sg.gamma[cs];
+    pre_beta = sg.beta[cs];
+    if (lane == 0) {
+      if (sg.rmean) pre_rm = sg.rmean[cs];
+      if (sg.rvar) pre_rv = sg.rvar[cs];
+    }
+  }
+  // grid barrier: all CTAs of the persistent grid are resident (1 per SM)
+  __threadfence();
+  bar_stats_done();
+  if (et == 0) {
+    atomicAdd(&p.sync[0], 1u);
+    while (ld_acquire_u32(&p.sync[0]) < gridDim.x) __nanosleep(32);
+  }
+  bar_stats_done();
+  if (et == 0) tl_rec<TL>(p, tl, 4, 6, 0, 0);
+  // exit ticket (the last CTA past the barrier re-arms the counters): taken as early as possible -- right after the
+  // barrier -- so that the atomic's round trip overlaps the finalize instead of ending the kernel
+  unsigned int ticket = 0xffffffffu;
+  if (et == 0) ticket = atomicAdd(&p.sync[1], 1u);
+  // one WARP per channel (no block barriers): lane l sums the partial rows l, l+32, ... in order, a fixed shuffle tree
+  // combines the lanes (deterministic), lanes 0 / 1 finalize one statistics group each.
+  for (int c = c_first; c < c_end; c += kTailThreads / 32) {
+    // all loads first (<= 160 rows: five per lane), then the sums in the same fixed order: one L2 round trip instead
+    // of five serialised ones (the fp64 adds used to sit between the loads of consecutive rows)
+    const float4* rows4 = reinterpret_cast<const float4*>(p.partials) + c;
+    float4 buf[5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      const int r = lane + 32 * j;
+      buf[j] = r < p.stat_rows ? __ldcg(rows4 + (size_t)r * p.Cout) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    double v[4] = {0.0, 0.0, 0.0, 0.0};
+#pragma unroll
+    for (int j = 0; j < 5; ++j) {
+      v[0] += (double)buf[j].x; v[1] += (double)buf[j].y; v[2] += (double)buf[j].z; v[3] += (double)buf[j].w;
+    }
+    if (et == 0) tl_rec<TL>(p, tl, 4, 8, 0, 0);
+    for (int r = lane + 160; r < p.stat_rows; r += 32) {            // (more than 160 rows: not on an H100)
+      const float4 q = __ldcg(rows4 + (size_t)r * p.Cout);
+      v[0] += (double)q.x; v[1] += (double)q.y; v[2] += (double)q.z; v[3] += (double)q.w;
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+      for (int m = 16; m >= 1; m >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], m);
+    }
+    if (et == 0) tl_rec<TL>(p, tl, 4, 9, 0, 0);
+    // every lane holds the four sums: lane g finalizes statistics group g (fp64 only for mean / E[x^2] - mean^2; the
+    // reciprocal square root is IEEE fp32 -- the fp64 sqrt / divisions of the first version cost ~3 us per launch),
+    // lane 0 then folds both groups into the running statistics in order
+    const BnSeg& sg = bn_seg(p, c);
+    const int cs = c - sg.c_begin;
+    float mean_f = 0.f, var_f = 0.f;
+    if (lane < groups) {
+      const int g = lane;
+      const double s1 = g ? v[2] : v[0], s2 = g ? v[3] : v[1];
+      const double mean = s1 * p.inv_cnt[g];
+      double var = s2 * p.inv_cnt[g] - mean * mean;
+      if (var < 0.0) var = 0.0;
+      mean_f = (float)mean;
+      var_f = (float)var;
+      const float istd = 1.0f / sqrtf(var_f + p.eps);
+      const float sc = (c == c_first ? pre_gamma : sg.gamma[cs]) * istd;
+      p.ss[(0 * 2 + g) * p.Cout + c] = sc;
+      p.ss[(1 * 2 + g) * p.Cout + c] = (c == c_first ? pre_beta : sg.beta[cs]) - mean_f * sc;
+      if (p.mi != nullptr) {
+        p.mi[(0 * 2 + g) * p.Cout + c] = mean_f;
+        p.mi[(1 * 2 + g) * p.Cout + c] = istd;
+      }
+    }
+    const float mean1 = __shfl_sync(0xffffffffu, mean_f, 1), var1 = __shfl_sync(0xffffffffu, var_f, 1);
+    if (lane == 0) {
+      float rm = pre_rm, rv = pre_rv;
+      if (c != c_first) {
+        rm = sg.rmean ? sg.rmean[cs] : 0.f;
+        rv = sg.rvar ? sg.rvar[cs] : 1.f;
+      }
+      rm = (1.f - p.momentum) * rm + p.momentum * mean_f;
+      rv = (1.f - p.momentum) * rv + p.momentum * (var_f * p.unbias[0]);
+      if (groups == 2) {
+        rm = (1.f - p.momentum) * rm + p.momentum * mean1;
+        rv = (1.f - p.momentum) * rv + p.momentum * (var1 * p.unbias[1]);
+      }
+      if (sg.rmean) sg.rmean[cs] = rm;
+      if (sg.rvar) sg.rvar[cs] = rv;
+    }
+  }
+  if (et == 0) tl_rec<TL>(p, tl, 4, 7, 0, 0);
+  if (et == 0 && blockIdx.x == 0) {
+    for (int sgi = 0; sgi < p.n_seg; ++sgi)          // (a reduction: no round trip -- a load-add-store ended CTA 0 ~1 us late)
+      if (p.seg[sgi].nbt) atomicAdd(reinterpret_cast<unsigned long long*>(p.seg[sgi].nbt), (unsigned long long)groups);
+  }
+  if (et == 0 && ticket == gridDim.x - 1) {   // every CTA is past the barrier: re-arm for the next launch
+    p.sync[0] = 0u;
+    p.sync[1] = 0u;
+    __threadfence();
+  }
+}
+
 // AM = how the A operand (activations) reaches shared memory:
 //   1 linear : 128 consecutive output pixels, one im2col-mode TMA load per (tap, channel block)
 //   2 halo   : 16 x 8 patch tiles, ONE tiled load per channel block of the 18 x (8+2) input halo; the nine taps are nine
@@ -168,30 +901,7 @@ template <int BN, bool TL, int AM>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmY, const Params p) {
-  using C = Cfg<BN>;
-  constexpr bool LIN = (AM == 1);
   constexpr bool HALO = (AM == 2);
-  constexpr int kBB = C::kBBytes;
-  // tile walk of this CTA (expressions, not variables: blockIdx / kernel parameters cost no registers; see pick_walk).
-  // band == 1 (N-major): walk index = tile index, M fastest.  band == n_tiles (M-band): CTA b = slot * band + N tile;
-  // walk index w = class * cls_tiles + k visits M tile rho + k * stat_rows of class rho = slot + class * cls_step.
-  // tile_nm is false for walk indices that name no tile (every role skips them alike).
-#define SY_T_FIRST (p.band > 1 ? 0 : (int)blockIdx.x)
-#define SY_T_STEP (p.band > 1 ? 1 : (int)gridDim.x)
-#define SY_T_END (p.t_end)
-  auto tile_nm = [&](int tile, int& n_tile, int& m_tile) -> bool {
-    if (p.band == 1) {
-      n_tile = fdiv(tile, p.fd_m_tiles);
-      m_tile = tile - n_tile * p.m_tiles;
-      return true;
-    }
-    const int slot = fdiv((int)blockIdx.x, p.fd_band);
-    n_tile = (int)blockIdx.x - slot * p.band;
-    const int cls = fdiv(tile, p.fd_cls_tiles);
-    const int rho = slot + cls * p.cls_step;
-    m_tile = rho + (tile - cls * p.cls_tiles) * p.stat_rows;
-    return rho < p.stat_rows && m_tile < p.m_tiles;
-  };
   const int S = p.stages;                                  // linear: A+B ring depth; halo: B ring depth
   // weight slabs per ring stage: one 64-deep K block; halo mode: kHaloTaps filter taps
   constexpr int kSub = HALO ? kHaloTaps : 1;
@@ -200,37 +910,27 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* sA = smem;
   uint8_t* sB = sA + (HALO ? p.stagesA * kHaloBytes : S * kABytes);
-  uint8_t* sStage = sB + S * kSub * kBB;                                 // 1024-aligned: the rings are multiples of 1 KiB
+  uint8_t* sStage = sB + S * kSub * Cfg<BN>::kBBytes;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sStage + p.stage_tiles * kSlabBytes);
-  const int sflip = p.stage_tiles - 1;                                   // slab parity toggles the tile iff there are two
-  // bars: [0,8) full, [8,16) empty, [16,19) halo full, [19,22) halo empty
-  float* sAcc = reinterpret_cast<float*>(bars + 32);                     // RAW:   [2 groups][2][Cout]
-  float* sScale = sAcc;                                                  // FUSED: [256] scale, [256] shift
-  float* sShift = sScale + 256;
 
   const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   pdl_launch_dependents();               // the next kernel on the stream may start its own prologue
   int tl_k = 3 * (p.timeline_cap / 4);
   if (threadIdx.x == 16 * 32) tl_rec<TL>(p, tl_k, 4, 0, 0, 0);
-  const uint32_t bar0 = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (kMaxStages + s); };
-  auto fullA_bar = [&](int s) { return bar0 + 8u * (2 * kMaxStages + s); };          // halo ring (<= 3 stages)
-  auto emptyA_bar = [&](int s) { return bar0 + 8u * (2 * kMaxStages + 3 + s); };
+  const Smem sm{sA, sB, sStage, reinterpret_cast<float*>(bars + 32), smem_u32(bars), p.stage_tiles - 1};
 
   if (threadIdx.x == 17 * 32) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     prefetch_tmap(&tmY);
     for (int s = 0; s < S; ++s) {
-      mbar_init(full_bar(s), HALO ? 1 : 2);     // A producer + B producer (halo: B only)
-      mbar_init(empty_bar(s), 2);               // one arrival per consumer warpgroup
+      mbar_init(sm.full(s), HALO ? 1 : 2);     // A producer + B producer (halo: B only)
+      mbar_init(sm.empty(s), 2);               // one arrival per consumer warpgroup
     }
     if (HALO) {
       for (int s = 0; s < p.stagesA; ++s) {
-        mbar_init(fullA_bar(s), 1);
-        mbar_init(emptyA_bar(s), 2);
+        mbar_init(sm.full_a(s), 1);
+        mbar_init(sm.empty_a(s), 2);
       }
     }
     fence_barrier_init();
@@ -240,644 +940,33 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   pdl_wait();
   if (threadIdx.x == 16 * 32) tl_rec<TL>(p, tl_k, 4, 1, 0, 0);
 
-  const int per_img = p.tiles_x * p.tiles_y;
-  const int hw = p.Ho * p.Wo;
-  int tl_epi = p.timeline_cap;           // debug-timeline cursor of thread 0, carried from the consumer loop into the tail
-
-  // ---------------------------------------------- per-CTA partial row, grid barrier, BatchNorm finalize
-  // run by the 16 convert + statistics warps (512 threads); called from both of their branches so that each copy is
-  // compiled under that warpgroup's register budget
-  auto kernel_tail = [&]() {
-    const int et = threadIdx.x;                        // 0..511
-    const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
-    if (et == 0) tl_rec<TL>(p, tl_epi, 4, 2, 0, 0);
-    bar_stats_done();                                // every sAcc update is done
-    if (do_stats) {
-      // partial row of this CTA, channel-major: the four sums of a channel are one 16-byte word (the finalize below loads
-      // one word per row and channel; with the shared-memory layout [4][Cout] in global memory it needed four loads, and the
-      // 640 sector requests per warp made the partial-row sums the longest part of the tail)
-      // (M-band walk: the statistics warps wrote this CTA's class rows already)
-      if (p.band == 1) {
-        float4* mine = reinterpret_cast<float4*>(p.partials) + (size_t)blockIdx.x * p.Cout;
-        for (int c = et; c < p.Cout; c += kTailThreads)
-          mine[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
-      }
-      if (p.n_seg > 0) {
-        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 5, 0, 0);
-        // This CTA finalizes channels [b*cpc, (b+1)*cpc), one warp per channel.  The BatchNorm parameters and running
-        // statistics of the warp's first channel do not depend on the other CTAs: load them BEFORE the grid barrier (they
-        // come from DRAM -- behind the barrier their latency, twice in a row, was most of the finalize)
-        const int groups = p.split_n < p.N ? 2 : 1;
-        const int cpc = (p.Cout + (int)gridDim.x - 1) / (int)gridDim.x;
-        const int c_end = min(p.Cout, ((int)blockIdx.x + 1) * cpc);
-        const int c_first = (int)blockIdx.x * cpc + warp;
-        float pre_gamma = 1.f, pre_beta = 0.f, pre_rm = 0.f, pre_rv = 1.f;
-        if (c_first < c_end && lane < 2) {
-          const BnSeg& sg = (p.n_seg > 1 && c_first >= p.seg[1].c_begin) ? p.seg[1] : p.seg[0];
-          const int cs = c_first - sg.c_begin;
-          pre_gamma = sg.gamma[cs];
-          pre_beta = sg.beta[cs];
-          if (lane == 0) {
-            if (sg.rmean) pre_rm = sg.rmean[cs];
-            if (sg.rvar) pre_rv = sg.rvar[cs];
-          }
-        }
-        // grid barrier: all CTAs of the persistent grid are resident (1 per SM)
-        __threadfence();
-        bar_stats_done();
-        if (et == 0) {
-          atomicAdd(&p.sync[0], 1u);
-          while (ld_acquire_u32(&p.sync[0]) < gridDim.x) __nanosleep(32);
-        }
-        bar_stats_done();
-        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 6, 0, 0);
-        // exit ticket (the last CTA past the barrier re-arms the counters): taken as early as possible -- right after the
-        // barrier -- so that the atomic's round trip overlaps the finalize instead of ending the kernel
-        unsigned int ticket = 0xffffffffu;
-        if (et == 0) ticket = atomicAdd(&p.sync[1], 1u);
-        // one WARP per channel (no block barriers): lane l sums the partial rows l, l+32, ... in order, a fixed shuffle tree
-        // combines the lanes (deterministic), lanes 0 / 1 finalize one statistics group each.
-        for (int c = c_first; c < c_end; c += kTailThreads / 32) {
-          // all loads first (<= 160 rows: five per lane), then the sums in the same fixed order: one L2 round trip instead
-          // of five serialised ones (the fp64 adds used to sit between the loads of consecutive rows)
-          const float4* rows4 = reinterpret_cast<const float4*>(p.partials) + c;
-          float4 buf[5];
-#pragma unroll
-          for (int j = 0; j < 5; ++j) {
-            const int r = lane + 32 * j;
-            buf[j] = r < p.stat_rows ? __ldcg(rows4 + (size_t)r * p.Cout) : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          double v[4] = {0.0, 0.0, 0.0, 0.0};
-#pragma unroll
-          for (int j = 0; j < 5; ++j) {
-            v[0] += (double)buf[j].x; v[1] += (double)buf[j].y; v[2] += (double)buf[j].z; v[3] += (double)buf[j].w;
-          }
-          if (et == 0) tl_rec<TL>(p, tl_epi, 4, 8, 0, 0);
-          for (int r = lane + 160; r < p.stat_rows; r += 32) {            // (more than 160 rows: not on an H100)
-            const float4 q = __ldcg(rows4 + (size_t)r * p.Cout);
-            v[0] += (double)q.x; v[1] += (double)q.y; v[2] += (double)q.z; v[3] += (double)q.w;
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-#pragma unroll
-            for (int m = 16; m >= 1; m >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], m);
-          }
-          if (et == 0) tl_rec<TL>(p, tl_epi, 4, 9, 0, 0);
-          // every lane holds the four sums: lane g finalizes statistics group g (fp64 only for mean / E[x^2] - mean^2; the
-          // reciprocal square root is IEEE fp32 -- the fp64 sqrt / divisions of the first version cost ~3 us per launch),
-          // lane 0 then folds both groups into the running statistics in order
-          const BnSeg& sg = (p.n_seg > 1 && c >= p.seg[1].c_begin) ? p.seg[1] : p.seg[0];
-          const int cs = c - sg.c_begin;
-          float mean_f = 0.f, var_f = 0.f;
-          if (lane < groups) {
-            const int g = lane;
-            const double s1 = g ? v[2] : v[0], s2 = g ? v[3] : v[1];
-            const double mean = s1 * p.inv_cnt[g];
-            double var = s2 * p.inv_cnt[g] - mean * mean;
-            if (var < 0.0) var = 0.0;
-            mean_f = (float)mean;
-            var_f = (float)var;
-            const float istd = 1.0f / sqrtf(var_f + p.eps);
-            const float sc = (c == c_first ? pre_gamma : sg.gamma[cs]) * istd;
-            p.ss[(0 * 2 + g) * p.Cout + c] = sc;
-            p.ss[(1 * 2 + g) * p.Cout + c] = (c == c_first ? pre_beta : sg.beta[cs]) - mean_f * sc;
-            if (p.mi != nullptr) {
-              p.mi[(0 * 2 + g) * p.Cout + c] = mean_f;
-              p.mi[(1 * 2 + g) * p.Cout + c] = istd;
-            }
-          }
-          const float mean1 = __shfl_sync(0xffffffffu, mean_f, 1), var1 = __shfl_sync(0xffffffffu, var_f, 1);
-          if (lane == 0) {
-            float rm = pre_rm, rv = pre_rv;
-            if (c != c_first) {
-              rm = sg.rmean ? sg.rmean[cs] : 0.f;
-              rv = sg.rvar ? sg.rvar[cs] : 1.f;
-            }
-            rm = (1.f - p.momentum) * rm + p.momentum * mean_f;
-            rv = (1.f - p.momentum) * rv + p.momentum * (var_f * p.unbias[0]);
-            if (groups == 2) {
-              rm = (1.f - p.momentum) * rm + p.momentum * mean1;
-              rv = (1.f - p.momentum) * rv + p.momentum * (var1 * p.unbias[1]);
-            }
-            if (sg.rmean) sg.rmean[cs] = rm;
-            if (sg.rvar) sg.rvar[cs] = rv;
-          }
-        }
-        if (et == 0) tl_rec<TL>(p, tl_epi, 4, 7, 0, 0);
-        if (et == 0 && blockIdx.x == 0) {
-          for (int sgi = 0; sgi < p.n_seg; ++sgi)          // (a reduction: no round trip -- a load-add-store ended CTA 0 ~1 us late)
-            if (p.seg[sgi].nbt) atomicAdd(reinterpret_cast<unsigned long long*>(p.seg[sgi].nbt), (unsigned long long)groups);
-        }
-        if (et == 0 && ticket == gridDim.x - 1) {   // every CTA is past the barrier: re-arm for the next launch
-          p.sync[0] = 0u;
-          p.sync[1] = 0u;
-          __threadfence();
-        }
-      }
-    }
-  };
-  if (warp >= 16) {
   // every role's branch starts with its warpgroup's setmaxnreg: the register budget of a code region is what ptxas can
   // prove for every path into it
-  reg_dealloc<kRegsIo>();
-  if (HALO && (warp == 18 || warp == 17)) {
-    // ----------------------------------------------- halo mode producers
-    if (warp == 18) {                            // A: one halo box [18 rows][10 px][64 ch] per (tile, channel block)
-      int sa = 0;
-      uint32_t pha = 0;
-      for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-        int n_tile, m_tile;
-        if (!tile_nm(tile, n_tile, m_tile)) continue;
-        const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
-        const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-        for (int cb = 0; cb < p.cblocks; ++cb) {
-          mbar_wait(emptyA_bar(sa), pha ^ 1u);
-          if (elect_one()) {
-            if (p.debug_flags & 2) {
-              mbar_arrive(fullA_bar(sa));
-            } else {
-              mbar_expect_tx(fullA_bar(sa), (uint32_t)kHaloTx);
-              tma_load_4d(smem_u32(sA + sa * kHaloBytes), &tmA, fullA_bar(sa), cb * kBlockK, px * kHaloTW - 1, py * kHaloTH - 1, img);
-            }
-          }
-          __syncwarp();
-          if (++sa == p.stagesA) { sa = 0; pha ^= 1u; }
-        }
-      }
-    } else {                                     // B: one [BN][64] weight slab per (channel block, tap)
-      int sb = 0;
-      uint32_t phb = 0;
-      for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-        int n_tile, m_tile_unused;
-        if (!tile_nm(tile, n_tile, m_tile_unused)) continue;
-        for (int cb = 0; cb < p.cblocks; ++cb) {
-          for (int t0 = 0; t0 < 9; t0 += kSub) {
-            mbar_wait(empty_bar(sb), phb ^ 1u);
-            if (elect_one()) {
-              if (p.debug_flags & 2) {
-                mbar_arrive(full_bar(sb));
-              } else {
-                mbar_expect_tx(full_bar(sb), (uint32_t)(kSub * kBB));
-#pragma unroll
-                for (int j = 0; j < kSub; ++j)
-                  tma_load_3d(smem_u32(sB + (sb * kSub + j) * kBB), &tmB, full_bar(sb), cb * kBlockK, t0 + j, n_tile * BN);
-              }
-            }
-            __syncwarp();
-            if (++sb == S) { sb = 0; phb ^= 1u; }
-          }
-        }
-      }
-    }
-  } else if (warp == 18 || warp == 17) {
-    // ----------------------------------------------- TMA producers: warp 18 loads A (activations), warp 17 loads B (weights)
-    // Two issuing threads because a single thread needs a few hundred cycles per cp.async.bulk.tensor: the pair keeps a
-    // K block's issue time below its MMA time.  Both arrive (with their byte counts) on the same full barrier.
-    {
-      const bool is_a = (warp == 18);
-      int stage = 0;
-      uint32_t phase = 0;
-      int tl_n = is_a ? 0 : p.timeline_cap / 8;
-      for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-        int n_tile, m_tile;
-        if (!tile_nm(tile, n_tile, m_tile)) continue;
-        const int p0 = m_tile * kBlockM;
-        const int img = fdiv(p0, p.fd_hw);
-        const int rem = p0 - img * hw;
-        const int oh = fdiv(rem, p.fd_wo), ow = rem - oh * p.Wo;
-        const int y0 = oh * p.stride - p.pad_h, x0 = ow * p.stride - p.pad_w;
-        // walk the (tap, channel block) K blocks, one per ring stage
-        int r = 0, sx = 0, cb = 0;
-        for (int kb = 0; kb < p.kblocks; ++kb) {
-          mbar_wait(empty_bar(stage), phase ^ 1u);          // whole warp waits: control flow stays uniform
-          if (elect_one()) {
-            tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 0, tile, kb);
-            if (p.debug_flags & 2) mbar_arrive(full_bar(stage));
-            else mbar_expect_tx(full_bar(stage), is_a ? (uint32_t)kABytes : (uint32_t)kBB);
-            tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 1, tile, kb);
-          }
-          if (!(p.debug_flags & 2) && elect_one()) {
-            if (is_a)
-              tma_load_im2col_4d(smem_u32(sA + stage * kABytes), &tmA, full_bar(stage), cb * kBlockK, x0, y0, img,
-                                 (uint16_t)sx, (uint16_t)r);
-            else
-              tma_load_3d(smem_u32(sB + stage * kBB), &tmB, full_bar(stage), cb * kBlockK, r * p.kw + sx, n_tile * BN);
-          }
-          if (++cb == p.cblocks) { cb = 0; if (++sx == p.kw) { sx = 0; ++r; } }
-          if (TL && elect_one()) tl_rec<TL>(p, tl_n, is_a ? 0 : 3, 2, tile, kb);
-          __syncwarp();
-          if (++stage == S) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 16) {
-    // ------------------------------------------------------------- store warp
-    // One 4-D TMA store per 64-column slab; the tensor map clips the patch to the image and to the
-    // channel slice.  Issuing it here keeps its issue + drain latency off the epilogue warps' path.
-    const uint32_t stage_base = smem_u32(sStage);
-    int sbuf = 0, prev = -1;
-    int tl_s = 7 * (p.timeline_cap / 8);
-    const int nbar = 544;
-    bar_free_arrive(0, nbar);                    // both tiles start out free
-    if (sflip) bar_free_arrive(1, nbar);
-    for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-      int n_tile, m_tile;
-        if (!tile_nm(tile, n_tile, m_tile)) continue;
-      int c1, c2, c3;                            // store coordinates below the channel: (x, y, image) | (pixel, 0, 0)
-      if constexpr (LIN) {
-        c1 = m_tile * kBlockM; c2 = 0; c3 = 0;
+  if (warp >= 16) {
+    reg_dealloc<kRegsIo>();
+    if (warp == 18 || warp == 17) {
+      if constexpr (HALO) {
+        if (warp == 18) load_halo_a(p, sm, tmA);
+        else load_halo_b<BN>(p, sm, tmB);
       } else {
-        const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
-        const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-        c1 = px * kHaloTW; c2 = py * kHaloTH; c3 = img;
+        load_linear<BN, TL>(p, sm, tmA, tmB, warp == 18);
       }
-      for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
-        bar_staged_wait(sbuf, nbar);
-        if (lane == 0) tl_rec<TL>(p, tl_s, 6, 0, tile, slab);
-        if (elect_one()) {
-          tma_store_4d(&tmY, stage_base + (uint32_t)(sbuf * kSlabBytes), n_tile * BN + slab * kSlabCols, c1, c2, c3);
-          bulk_commit();
-          if (sflip) {
-            if (prev >= 0) bulk_wait_read1();    // two tiles: the previous slab's store has read ITS tile
-          } else {
-            bulk_wait_read();                    // one tile: wait until this store has read it
-          }
-        }
-        __syncwarp();
-        if (lane == 0) tl_rec<TL>(p, tl_s, 6, 1, tile, slab);
-        if (sflip) {
-          if (prev >= 0) bar_free_arrive(prev, nbar);
-          prev = sbuf;
-        } else {
-          bar_free_arrive(0, nbar);
-        }
-      }
+    } else if (warp == 16) {
+      store_slabs<BN, TL, AM>(p, sm, tmY, threadIdx.x);
     }
-    if (sflip && prev >= 0) {
-      if (elect_one()) bulk_wait_read();
-      __syncwarp();
-      bar_free_arrive(prev, nbar);
-    }
-    // the stores have read the staging tiles before the CTA's final __syncthreads; their writes complete with the grid
-    if (lane == 0) bulk_wait_read();
-    __syncwarp();
-  }
   } else if (warp >= 8) {
     reg_alloc<kRegsStats>();
-    // ------------------------------------------------------------ statistics warps
-    // Warp ew reduces columns [8*ew, 8*ew+8) of every staged 64-column slab while the convert warps already
-    // convert the next slab; one owner lane per (column, sum|sumsq) accumulates in fixed order.
-    const int ew = warp - 8;
-    const int st = threadIdx.x - 256;            // 0..255
-    const uint32_t stage_base = smem_u32(sStage);
-    const bool do_stats = (p.mode == SY_CONV_RAW) && (p.partials != nullptr);
-    if (do_stats) {
-      for (int i = st; i < 4 * p.Cout; i += 256) sAcc[i] = 0.f;
-    }
-    int sbuf = 0;
-    int tl_t = (st == 0) ? 5 * (p.timeline_cap / 8) : p.timeline_cap;
-    const int nbar = 544;
-    bar_free_arrive(0, nbar);                    // both tiles start out free
-    if (sflip) bar_free_arrive(1, nbar);
-    // Warp ew owns columns [8*ew, 8*ew+8) of every 64-column slab; lane l reads rows l, l+32, l+64, l+96 (one 16-byte
-    // chunk each).  The per-lane partial sums (8 columns x {sum, sum of squares}) stay in REGISTERS across slabs and tiles
-    // -- one set per slab index of the tile -- and are only combined across the 32 lanes (recursive-halving shuffles) and
-    // added to the CTA's shared-memory totals on a FLUSH: when the CTA moves to another n tile (N-major walk only) or
-    // statistics group, on a tile that straddles the group boundary, and at the end.  (Per-slab shuffle reductions made the statistics warps the
-    // bottleneck of every epilogue-bound layer: ~1400 cycles per slab.)
-    constexpr int kSlabs = BN / kSlabCols;
-    float acc[kSlabs][16];
-#pragma unroll
-    for (int j = 0; j < kSlabs; ++j)
-#pragma unroll
-      for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
-    int pend_grp = -1, pend_n0 = 0;                          // what the register sums belong to (-1: nothing pending)
-    // lanes combine a[16] (fixed shuffle tree: deterministic) and the 16 owner lanes add into the shared totals
-    auto reduce_store = [&](float (&a)[16], int grp, int col_base) {
-      float b8[8], c4[4], d2[2], e1;
-      {
-        const bool up = (lane & 16) != 0;
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float send = up ? a[i] : a[8 + i], keep = up ? a[8 + i] : a[i];
-          b8[i] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-        }
-      }
-      {
-        const bool up = (lane & 8) != 0;
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float send = up ? b8[i] : b8[4 + i], keep = up ? b8[4 + i] : b8[i];
-          c4[i] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-        }
-      }
-      {
-        const bool up = (lane & 4) != 0;
-#pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const float send = up ? c4[i] : c4[2 + i], keep = up ? c4[2 + i] : c4[i];
-          d2[i] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-        }
-      }
-      {
-        const bool up = (lane & 2) != 0;
-        const float send = up ? d2[0] : d2[1], keep = up ? d2[1] : d2[0];
-        e1 = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-      }
-      e1 += __shfl_xor_sync(0xffffffffu, e1, 1);
-      if ((lane & 1) == 0) {               // 16 owner lanes: bit4 = sum | sumsq, bits 3..1 = column in the group
-        const int col = col_base + ew * 8 + ((lane >> 3) & 1) * 4 + ((lane >> 2) & 1) * 2 + ((lane >> 1) & 1);
-        if (col < p.Cout) sAcc[(grp * 2 + (lane >> 4)) * p.Cout + col] += e1;
-      }
-#pragma unroll
-      for (int i = 0; i < 16; ++i) a[i] = 0.f;
-    };
-    auto flush = [&]() {
-      if (pend_grp < 0) return;
-#pragma unroll
-      for (int j = 0; j < kSlabs; ++j) reduce_store(acc[j], pend_grp, pend_n0 + j * kSlabCols);
-      pend_grp = -1;
-    };
-    // M-band walk: the CTA's tiles of one class rho are exactly those that one CTA of the N-major walk took for this N tile,
-    // in the same order, so this CTA's sums of a class are that CTA's partial row for these BN columns, bit for bit.  The
-    // row of class rho is the N-major walk's CTA (n_tile * m_tiles + rho) mod stat_rows; classes without tiles write zeros.
-#define SY_BAND (do_stats && p.band > 1)
-    auto write_class = [&](int cls, bool zero) {                 // all 256 statistics threads
-      const int my_slot = fdiv((int)blockIdx.x, p.fd_band), my_n = (int)blockIdx.x - my_slot * p.band;
-      const int row = (int)(((long long)my_n * p.m_tiles + my_slot + cls * p.cls_step) % p.stat_rows);
-      float4* dst = reinterpret_cast<float4*>(p.partials) + (size_t)row * p.Cout;
-      const int c = my_n * BN + st;
-      if (zero) {
-        if (st < BN && c < p.Cout) dst[c] = make_float4(0.f, 0.f, 0.f, 0.f);
-        return;
-      }
-      asm volatile("bar.sync 8, 256;" ::: "memory");          // the owner lanes' shared-memory sums are complete
-      if (st < BN && c < p.Cout) {
-        dst[c] = make_float4(sAcc[c], sAcc[p.Cout + c], sAcc[2 * p.Cout + c], sAcc[3 * p.Cout + c]);
-        sAcc[c] = 0.f; sAcc[p.Cout + c] = 0.f; sAcc[2 * p.Cout + c] = 0.f; sAcc[3 * p.Cout + c] = 0.f;
-      }
-      asm volatile("bar.sync 8, 256;" ::: "memory");
-    };
-    int pend_cls = -1;                                           // class whose sums sAcc holds (M-band walk)
-    if (SY_BAND) {
-      const int my_slot = fdiv((int)blockIdx.x, p.fd_band);
-      for (int cls = 0; my_slot + cls * p.cls_step < p.stat_rows; ++cls)
-        if (my_slot + cls * p.cls_step >= p.m_tiles) write_class(cls, true);
-    }
-    for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-      int n_tile, m_tile;
-        if (!tile_nm(tile, n_tile, m_tile)) continue;
-      const int n0 = n_tile * BN;
-      // rows [0, cut) of the tile belong to statistics group 0, rows [cut, 128) to group 1 (a halo tile lies in one
-      // image = one group; a linear tile can straddle the boundary; rows past the end of the tensor were staged as zeros)
-      int cut;
-      if constexpr (LIN) {
-        cut = min(max(p.gp - m_tile * kBlockM, 0), kBlockM);
-      } else {
-        cut = fdiv(m_tile, p.fd_per_img) >= p.split_n ? 0 : kBlockM;
-      }
-      const bool pure = (cut <= 0) || (cut >= kBlockM);
-      const int tgrp = cut <= 0 ? 1 : 0;
-      if (SY_BAND) {                                             // warp-uniform
-        const int cls = fdiv(tile, p.fd_cls_tiles);
-        if (pend_cls >= 0 && cls != pend_cls) {
-          flush();
-          write_class(pend_cls, false);
-        }
-        pend_cls = cls;
-      }
-      if (do_stats && (!pure || pend_grp != tgrp || pend_n0 != n0)) flush();     // warp-uniform
-      for (int slab = 0; slab < kSlabs; ++slab, sbuf ^= sflip) {
-        bar_staged_wait(sbuf, nbar);
-        tl_rec<TL>(p, tl_t, 5, 0, tile, slab);
-        const uint32_t tile_base = stage_base + (uint32_t)(sbuf * kSlabBytes);
-        float x[4][8];
-        if (do_stats) {
-#pragma unroll
-          for (int rr = 0; rr < 4; ++rr) {
-            const uint32_t r = (uint32_t)(lane + 32 * rr);
-            const uint4 u = lds128(tile_base + r * 128u + ((((uint32_t)ew) ^ (r & 7u)) << 4));
-            x[rr][0] = bf16_lo(u.x); x[rr][1] = bf16_hi(u.x); x[rr][2] = bf16_lo(u.y); x[rr][3] = bf16_hi(u.y);
-            x[rr][4] = bf16_lo(u.z); x[rr][5] = bf16_hi(u.z); x[rr][6] = bf16_lo(u.w); x[rr][7] = bf16_hi(u.w);
-          }
-        }
-        bar_free_arrive(sbuf, nbar);             // the values are in registers: the tile may be overwritten
-        tl_rec<TL>(p, tl_t, 5, 1, tile, slab);
-        if (do_stats) {
-          if (pure) {
-            float (&a)[16] = acc[slab];
-#pragma unroll
-            for (int rr = 0; rr < 4; ++rr) {
-#pragma unroll
-              for (int i = 0; i < 8; ++i) { a[i] += x[rr][i]; a[8 + i] += x[rr][i] * x[rr][i]; }
-            }
-            pend_grp = tgrp; pend_n0 = n0;
-          } else {
-            // the tile straddles the group boundary (at most one M tile per layer and N tile): masked, reduced at once.
-            // The sums go through acc[slab]: the flush before this tile left it zero, and reduce_store zeroes it again
-            // (a separate scratch array made the BN = 64 statistics warps spill)
-#pragma unroll 1
-            for (int grp = 0; grp < 2; ++grp) {
-              const int lo = grp ? cut : 0, hi = grp ? kBlockM : cut;
-              float (&a)[16] = acc[slab];
-#pragma unroll
-              for (int rr = 0; rr < 4; ++rr) {
-                const int r = lane + 32 * rr;
-                if (r >= lo && r < hi) {
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) { a[i] += x[rr][i]; a[8 + i] += x[rr][i] * x[rr][i]; }
-                }
-              }
-              reduce_store(a, grp, n0 + slab * kSlabCols);
-            }
-          }
-        }
-        tl_rec<TL>(p, tl_t, 5, 2, tile, slab);
-      }
-    }
-    if (do_stats) flush();
-    if (SY_BAND && pend_cls >= 0) write_class(pend_cls, false);
-#undef SY_BAND
-    kernel_tail();
+    statistics<BN, TL, AM>(p, sm, threadIdx.x);
+    int tl = p.timeline_cap;
+    bn_tail<TL>(p, sm, threadIdx.x, tl);
   } else {
     reg_alloc<kRegsMma>();
-    // ---------------------------------------------------------------- MMA + convert warpgroups
-    // Warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile: it issues the wgmma stream for them (accumulators in
-    // registers), then converts its rows of every 64-column slab into the staging tile.  A ring stage is handed back to the
-    // producers one commit group late (wgmma.wait_group 1), so the next group's MMAs are queued while the last ones drain.
-    const int wg = warp >> 2;
-    const int et = threadIdx.x;                                    // 0..255
-    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);        // this thread's tile rows: r0 and r0 + 8
-    const int cq = 2 * (lane & 3);                                 // its first column in every 8-column group
-    const uint32_t stage_base = smem_u32(sStage);
-    const bool lead = (threadIdx.x & 127) == 0;                    // signals the warpgroup's ring releases
-    // halo mode: this warpgroup's 8 output rows start 8 halo rows further down
-    constexpr uint32_t row_bytes = HALO ? (uint32_t)kHaloPitch * 128u : 1024u;
-    const uint32_t a_off = HALO ? (uint32_t)(wg * 8) * row_bytes : (uint32_t)wg * 8192u;
-    float acc[C::kAcc];
-    int stage = 0, sa = 0, sbuf = 0;
-    uint32_t phase = 0, pha = 0;
-    int tl_n = (et == 0) ? p.timeline_cap / 2 : p.timeline_cap;
-    for (int tile = SY_T_FIRST; tile < SY_T_END; tile += SY_T_STEP) {
-      int n_tile, m_tile;
-      if (!tile_nm(tile, n_tile, m_tile)) continue;
-      // this thread's output pixels in the flattened (n, oh, ow) space (evaluated where they are used: only the
-      // validity flags stay live across the main loop)
-      auto pixel = [&](int h, bool& ok) -> long long {
-        if constexpr (LIN) {
-          const long long px = (long long)m_tile * kBlockM + r0 + 8 * h;
-          ok = px < p.P_total;
-          return px;
-        } else {
-          const int img = fdiv(m_tile, p.fd_per_img), rem = m_tile - img * per_img;
-          const int py = fdiv(rem, p.fd_tiles_x), px = rem - py * p.tiles_x;
-          const int row = r0 + 8 * h;
-          const int oy = py * kHaloTH + row / kHaloTW, ox = px * kHaloTW + row % kHaloTW;
-          ok = (oy < p.Ho) && (ox < p.Wo);
-          return ((long long)img * p.Ho + oy) * p.Wo + ox;
-        }
-      };
-      bool valid[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) pixel(h, valid[h]);
-      const int n0 = n_tile * BN;
-      tl_rec<TL>(p, tl_n, 2, 0, tile, 0);
-      if (p.mode == SY_CONV_FUSED) {
-        epi_bar();                               // previous tile's readers of sScale/sShift are done
-        for (int c = et; c < BN; c += kEpiThreads) {
-          const int cg = n0 + c;
-          sScale[c] = (cg < p.Cout && p.scale) ? p.scale[cg] : 1.0f;
-          sShift[c] = (cg < p.Cout && p.shift) ? p.shift[cg] : 0.0f;
-        }
-        epi_bar();
-      }
-      // ---- main loop
-      int pend_b = -1, pend_a = -1;              // ring stages read by the commit group still in flight
-      auto release = [&]() {
-        if (lead) {
-          if (pend_b >= 0) mbar_arrive(empty_bar(pend_b));
-          if (pend_a >= 0) mbar_arrive(emptyA_bar(pend_a));
-        }
-      };
-      if constexpr (HALO) {                      // K order = (channel block, tap)
-        for (int cb = 0; cb < p.cblocks; ++cb) {
-          mbar_wait(fullA_bar(sa), pha);
-          const uint32_t halo = smem_u32(sA + sa * kHaloBytes) + a_off;
-          for (int t0 = 0; t0 < 9; t0 += kSub) {
-            mbar_wait(full_bar(stage), phase);
-            wgmma_fence_operand(acc);
-            wgmma_fence();
-#pragma unroll
-            for (int j = 0; j < kSub; ++j) {
-              const int tap = t0 + j;
-              const int r = tap / 3, sx = tap - 3 * r;
-              const uint32_t a_addr = halo + (uint32_t)r * row_bytes + (uint32_t)sx * 128u;
-              const uint64_t da = make_smem_desc(a_addr, row_bytes);
-              const uint64_t db = make_smem_desc(smem_u32(sB + (stage * kSub + j) * kBB));
-#pragma unroll
-              for (int k = 0; k < kBlockK / 16; ++k)   // 16 bf16 = 32 bytes along K inside the swizzle row: +2 in (addr >> 4)
-                Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (cb | tap | k) != 0);
-            }
-            wgmma_commit();
-            wgmma_fence_operand(acc);
-            wgmma_wait<1>();
-            release();
-            pend_b = stage;
-            pend_a = (t0 + kSub >= 9) ? sa : -1;     // the halo is free after its ninth tap
-            if (++stage == S) { stage = 0; phase ^= 1u; }
-          }
-          if (++sa == p.stagesA) { sa = 0; pha ^= 1u; }
-        }
-      } else {
-        for (int kb = 0; kb < p.kblocks; ++kb) {
-          mbar_wait(full_bar(stage), phase);
-          wgmma_fence_operand(acc);
-          wgmma_fence();
-          const uint64_t da = make_smem_desc(smem_u32(sA + stage * kABytes) + a_off);
-          const uint64_t db = make_smem_desc(smem_u32(sB + stage * kBB));
-#pragma unroll
-          for (int k = 0; k < kBlockK / 16; ++k)
-            Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
-          wgmma_commit();
-          wgmma_fence_operand(acc);
-          wgmma_wait<1>();
-          release();
-          pend_b = stage;
-          if (++stage == S) { stage = 0; phase ^= 1u; }
-        }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_operand(acc);
-      release();
-      tl_rec<TL>(p, tl_n, 2, 1, tile, 0);
-      // ---- epilogue: per 64-column slab, registers -> (raw | folded BN + SiLU + residual) -> bf16 -> staging tile
-#pragma unroll
-      for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
-        tl_rec<TL>(p, tl_n, 2, 2, tile, slab);
-        bar_free_wait(sbuf);                     // (A) staging tile free: its store has read it, the statistics loads are done
-        // 16-byte chunk j of row r lives at r*128 + ((j ^ (r & 7)) << 4); this thread's rows r0 and r0 + 8 share r & 7,
-        // so the chunk offset is (j << 4) ^ sw: one logic op, nothing kept live across the main loop
-        const uint32_t tb = stage_base + (uint32_t)(sbuf * kSlabBytes) + (uint32_t)cq * 2u + (uint32_t)r0 * 128u;
-        const uint32_t sw = ((uint32_t)r0 & 7u) << 4;
-        if (p.mode == SY_CONV_RAW && p.dbg_f32 == nullptr) {
-          // raw values (every conv of a training step): round, pack and stage -- no per-value pixel or column arithmetic
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int J = slab * 8 + j;
-#pragma unroll
-            for (int h = 0; h < 2; ++h)
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
-                           "r"(valid[h] ? pack_bf16(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]) : 0u) : "memory");
-          }
-        } else {
-          long long pix[2];
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            bool ok;
-            pix[h] = pixel(h, ok);
-          }
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int J = slab * 8 + j;
-            const int cl = slab * kSlabCols + j * 8 + cq;          // tile column of this thread's first value
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              float v0 = acc[4 * J + 2 * h], v1 = acc[4 * J + 2 * h + 1];
-              const bool inb = valid[h] && n0 + cl < p.Cout;
-              if (p.dbg_f32 != nullptr && inb)     // validation only: the accumulators before any rounding
-                *reinterpret_cast<float2*>(p.dbg_f32 + pix[h] * p.Cout + n0 + cl) = make_float2(v0, v1);
-              if (p.mode != SY_CONV_RAW) {
-                v0 = v0 * sScale[cl] + sShift[cl];
-                v1 = v1 * sScale[cl + 1] + sShift[cl + 1];
-                if (p.act) { v0 = silu_f(v0); v1 = silu_f(v1); }
-                if (p.res != nullptr && inb) {
-                  const uint32_t rv = *reinterpret_cast<const uint32_t*>(p.res + pix[h] * p.res_pitch + n0 + cl);
-                  v0 += bf16_lo(rv);
-                  v1 += bf16_hi(rv);
-                }
-              }
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
-                           "r"(valid[h] ? pack_bf16(v0, v1) : 0u) : "memory");
-            }
-          }
-        }
-        fence_proxy_async();                     // generic-proxy writes -> visible to the TMA (async proxy)
-        bar_staged_arrive(sbuf);                 // (B) staging tile complete: store + statistics warps take it from here
-        tl_rec<TL>(p, tl_n, 2, 3, tile, slab);
-      }
-    }
-    tl_epi = tl_n;
-    bar_free_wait(0);                                // drain the last arrivals (balanced barriers at exit)
-    if (sflip) bar_free_wait(1);
-    kernel_tail();
+    int tl = mma_convert<BN, TL, AM>(p, sm, threadIdx.x);
+    bn_tail<TL>(p, sm, threadIdx.x, tl);
   }
   __syncthreads();
   if (threadIdx.x == 16 * 32) tl_rec<TL>(p, tl_k, 4, 3, 0, 0);
 }
-
-#undef SY_T_FIRST
-#undef SY_T_STEP
-#undef SY_T_END
 
 // ------------------------------------------------------------------ host side
 
@@ -1093,13 +1182,12 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   SY_REQUIRE(d->debug_flags == 0 || d->debug_flags == 2, SY_EINVAL, "conv2d_tc: debug_flags %d unsupported", d->debug_flags);
   SY_REQUIRE(tc::tiling_override_ok(d->tile_mode, d->tile_bn), SY_EINVAL, "conv2d_tc: tile_mode %d / tile_bn %d unsupported",
              d->tile_mode, d->tile_bn);
-  tc::EncodeTiledFn enc = tc::get_encode();
-  SY_REQUIRE(enc != nullptr, SY_EARCH, "cuTensorMapEncodeTiled not available from the driver");
+  SY_REQUIRE(tc::get_encode() != nullptr, SY_EARCH, "cuTensorMapEncodeTiled not available from the driver");
 
   tc::Params p{};
   p.debug_flags = d->debug_flags;
-  p.N = x.n; p.Ho = ho; p.Wo = wo; p.Cout = y.c; p.Cin = x.c;
-  p.kh = d->kh; p.kw = d->kw; p.stride = d->stride; p.pad_h = ph; p.pad_w = pw;
+  p.N = x.n; p.Ho = ho; p.Wo = wo; p.Cout = y.c;
+  p.kw = d->kw; p.stride = d->stride; p.pad_h = ph; p.pad_w = pw;
   SY_REQUIRE((long long)x.n * ho * wo < (1ll << 31) - 256, SY_EINVAL, "conv2d_tc: too many output pixels");
   const tc::Tiling t = tc::pick_tiling(x.n, ho, wo, x.c, y.c, d->kh, d->kw, d->stride, d->tile_mode, d->tile_bn);
   const bool halo = t.halo;
@@ -1116,7 +1204,6 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   p.fd_per_img = tc::make_fastdiv((uint32_t)(p.tiles_x * p.tiles_y));
   p.fd_tiles_x = tc::make_fastdiv((uint32_t)p.tiles_x);
   p.mode = d->mode; p.act = d->act;
-  p.y = reinterpret_cast<__nv_bfloat16*>(y.ptr); p.y_pitch = y.pitch;
   p.res = nullptr; p.res_pitch = 0;
   if (d->mode == SY_CONV_FUSED && d->res.ptr != nullptr) {
     SY_REQUIRE(view_ok(d->res) && d->res.n == y.n && d->res.h == ho && d->res.w == wo && d->res.c == y.c, SY_EINVAL,
@@ -1169,64 +1256,43 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   }
   if (d->rows_written) *d->rows_written = p.stat_rows;
 
-  // A: input view as (C, W, H, N)
   CUtensorMap ta, tb, ty;
   if (halo) {
-    // A, halo mode: box (64 ch, 10 px, 18 rows, 1 image) at (x0 - 1, y0 - 1): out of bounds = zero padding
-    cuuint64_t dims[4] = {(cuuint64_t)x.c, (cuuint64_t)x.w, (cuuint64_t)x.h, (cuuint64_t)x.n};
-    cuuint64_t strides[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.pitch * 2 * x.w, (cuuint64_t)x.pitch * 2 * x.w * x.h};
-    cuuint32_t box[4] = {(cuuint32_t)tc::kBlockK, (cuuint32_t)tc::kHaloPitch, (cuuint32_t)(tc::kHaloTH + 2), 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x.ptr, dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    // A, halo mode: input view as (C, W, H, N), box (64 ch, 10 px, 18 rows, 1 image) at (x0 - 1, y0 - 1): out of bounds
+    // = zero padding
+    cuuint64_t dims[4], strides[3];
+    tc::nhwc_dims(x, dims, strides);
+    const cuuint32_t box[4] = {(cuuint32_t)tc::kBlockK, (cuuint32_t)tc::kHaloPitch, (cuuint32_t)(tc::kHaloTH + 2), 1};
+    const CUresult r = tc::encode_tiled_bf16(&ta, 4, x.ptr, dims, strides, box);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(A halo) failed: %d", (int)r);
   } else {
-    // A, im2col mode: tensor (C, W, H, N); the bounding box of base pixels is [-pad, dim + pad - (k - 1)) per spatial
-    // dim, walked with the conv stride; one load = 128 consecutive base pixels x 64 channels, shifted by the tap offset
-    tc::EncodeIm2colFn enc2 = tc::get_encode_im2col();
-    SY_REQUIRE(enc2 != nullptr, SY_EARCH, "cuTensorMapEncodeIm2col not available from the driver");
-    cuuint64_t dims[4] = {(cuuint64_t)x.c, (cuuint64_t)x.w, (cuuint64_t)x.h, (cuuint64_t)x.n};
-    cuuint64_t strides[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.pitch * 2 * x.w, (cuuint64_t)x.pitch * 2 * x.w * x.h};
-    int lower[2] = {-pw, -ph};                                   // {W, H}
-    int upper[2] = {pw - (d->kw - 1), ph - (d->kh - 1)};
-    cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
-    CUresult r = enc2(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x.ptr, dims, strides, lower, upper, (cuuint32_t)tc::kBlockK,
-                      (cuuint32_t)tc::kBlockM, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    // A, im2col mode: one load = 128 consecutive base pixels x 64 channels, shifted by the tap offset
+    SY_REQUIRE(tc::get_encode_im2col() != nullptr, SY_EARCH, "cuTensorMapEncodeIm2col not available from the driver");
+    const CUresult r = tc::encode_im2col_nhwc(&ta, x, d->kh, d->kw, d->stride, tc::kBlockM);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeIm2col(A) failed: %d (c=%d w=%d h=%d n=%d pitch=%lld k=%dx%d s=%d)",
                (int)r, x.c, x.w, x.h, x.n, (long long)x.pitch, d->kh, d->kw, d->stride);
   }
   {
     const int taps = d->kh * d->kw;
-    cuuint64_t dims[3] = {(cuuint64_t)x.c, (cuuint64_t)taps, (cuuint64_t)y.c};
-    cuuint64_t strides[2] = {(cuuint64_t)x.c * 2, (cuuint64_t)x.c * 2 * taps};
-    cuuint32_t box[3] = {(cuuint32_t)tc::kBlockK, 1, (cuuint32_t)bn};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&tb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d->w), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[3] = {(cuuint64_t)x.c, (cuuint64_t)taps, (cuuint64_t)y.c};
+    const cuuint64_t strides[2] = {(cuuint64_t)x.c * 2, (cuuint64_t)x.c * 2 * taps};
+    const cuuint32_t box[3] = {(cuuint32_t)tc::kBlockK, 1, (cuuint32_t)bn};
+    const CUresult r = tc::encode_tiled_bf16(&tb, 3, d->w, dims, strides, box);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
   if (!halo) {
     // Y: output view as (C, pixels, 1, 1), box (64, 128, 1, 1): the TMA store clips the last tile / the channel slice
-    cuuint64_t dims[4] = {(cuuint64_t)y.c, (cuuint64_t)p.P_total, 1, 1};
-    cuuint64_t strides[3] = {(cuuint64_t)y.pitch * 2, (cuuint64_t)y.pitch * 2 * p.P_total, (cuuint64_t)y.pitch * 2 * p.P_total};
-    cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)tc::kBlockM, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&ty, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, y.ptr, dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[4] = {(cuuint64_t)y.c, (cuuint64_t)p.P_total, 1, 1};
+    const cuuint64_t strides[3] = {(cuuint64_t)y.pitch * 2, (cuuint64_t)y.pitch * 2 * p.P_total, (cuuint64_t)y.pitch * 2 * p.P_total};
+    const cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)tc::kBlockM, 1, 1};
+    const CUresult r = tc::encode_tiled_bf16(&ty, 4, y.ptr, dims, strides, box);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(Y linear) failed: %d", (int)r);
   } else {
     // Y: output view as (C, W, H, N), box (64, 8, 16, 1): the TMA store clips the patch to the image / slice
-    cuuint64_t dims[4] = {(cuuint64_t)y.c, (cuuint64_t)y.w, (cuuint64_t)y.h, (cuuint64_t)y.n};
-    cuuint64_t strides[3] = {(cuuint64_t)y.pitch * 2, (cuuint64_t)y.pitch * 2 * y.w, (cuuint64_t)y.pitch * 2 * y.w * y.h};
-    cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)tc::kHaloTW, (cuuint32_t)tc::kHaloTH, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&ty, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, y.ptr, dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    cuuint64_t dims[4], strides[3];
+    tc::nhwc_dims(y, dims, strides);
+    const cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)tc::kHaloTW, (cuuint32_t)tc::kHaloTH, 1};
+    const CUresult r = tc::encode_tiled_bf16(&ty, 4, y.ptr, dims, strides, box);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(Y) failed: %d", (int)r);
   }
   return halo ? tc::launch_bn<2>(bn, ta, tb, ty, p, pl, stream) : tc::launch_bn<1>(bn, ta, tb, ty, p, pl, stream);

@@ -279,9 +279,8 @@ extern "C" int sy_conv2d_wgrad_tc(const SyConvWgradDesc* d, sy_stream_t stream_)
   SY_REQUIRE(((uintptr_t)d->workspace % 16) == 0, SY_EINVAL, "conv2d_wgrad: workspace must be 16B aligned");
   const SyTensor& x = d->x;
   const SyTensor& dy = d->dy;
-  tc::EncodeTiledFn enc = tc::get_encode();
-  tc::EncodeIm2colFn enc2 = tc::get_encode_im2col();
-  SY_REQUIRE(enc != nullptr && enc2 != nullptr, SY_EARCH, "tensor-map encoders not available from the driver");
+  SY_REQUIRE(tc::get_encode() != nullptr && tc::get_encode_im2col() != nullptr, SY_EARCH,
+             "tensor-map encoders not available from the driver");
   const int ph = (d->kh - 1) / 2, pw = (d->kw - 1) / 2;
   wg::WParams p{};
   p.P_total = x.n * pl.ho * pl.wo; p.Ho = pl.ho; p.Wo = pl.wo; p.stride = d->stride; p.pad_h = ph; p.pad_w = pw; p.kw = d->kw;
@@ -294,23 +293,15 @@ extern "C" int sy_conv2d_wgrad_tc(const SyConvWgradDesc* d, sy_stream_t stream_)
   CUtensorMap tdy, tx;
   {
     // dy as (C, pixels): box (64 ch, 64 px); pixels past the end / channels past Cout read as zero
-    cuuint64_t dims[2] = {(cuuint64_t)dy.c, (cuuint64_t)p.P_total};
-    cuuint64_t strides[1] = {(cuuint64_t)dy.pitch * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)wg::kPixK}, estr[2] = {1, 1};
-    CUresult r = enc(&tdy, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dy.ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[2] = {(cuuint64_t)dy.c, (cuuint64_t)p.P_total};
+    const cuuint64_t strides[1] = {(cuuint64_t)dy.pitch * 2};
+    const cuuint32_t box[2] = {64, (cuuint32_t)wg::kPixK};
+    const CUresult r = tc::encode_tiled_bf16(&tdy, 2, dy.ptr, dims, strides, box);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(dy) failed: %d", (int)r);
   }
   {
     // x in im2col mode, 64 base pixels per load (same bounding box as the forward kernel's linear tiles)
-    cuuint64_t dims[4] = {(cuuint64_t)x.c, (cuuint64_t)x.w, (cuuint64_t)x.h, (cuuint64_t)x.n};
-    cuuint64_t strides[3] = {(cuuint64_t)x.pitch * 2, (cuuint64_t)x.pitch * 2 * x.w, (cuuint64_t)x.pitch * 2 * x.w * x.h};
-    int lower[2] = {-pw, -ph};
-    int upper[2] = {pw - (d->kw - 1), ph - (d->kh - 1)};
-    cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
-    CUresult r = enc2(&tx, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x.ptr, dims, strides, lower, upper, 64, (cuuint32_t)wg::kPixK, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const CUresult r = tc::encode_im2col_nhwc(&tx, x, d->kh, d->kw, d->stride, wg::kPixK);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeIm2col(x) failed: %d", (int)r);
   }
   int lrc;

@@ -110,27 +110,11 @@ __device__ __forceinline__ void tma_store_4d(const CUtensorMap* map, uint32_t sr
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void sts128(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
 __device__ __forceinline__ uint4 lds128(uint32_t addr) {
   uint4 v;
   asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
   return v;
-}
-// two 8x8 b16 matrices, transposed: thread t receives M^T[t / 4][2 (t % 4) .. +1] = M[2 (t % 4) .. +1][t / 4]; lanes 0-7 give
-// the row addresses of matrix 0, lanes 8-15 those of matrix 1
-__device__ __forceinline__ void ldmatrix_x2_trans(uint32_t& r0, uint32_t& r1, uint32_t addr) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x2.trans.shared.b16 {%0, %1}, [%2];" : "=r"(r0), "=r"(r1) : "r"(addr) : "memory");
-}
-// legacy tensor path (HMMA): D[16x8] += A[16x16] * B[16x8], bf16 in, fp32 accumulate
-__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                               uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-               : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 __device__ __forceinline__ unsigned int ld_acquire_u32(const unsigned int* p) {
   unsigned int v;
@@ -282,6 +266,41 @@ static EncodeIm2colFn get_encode_im2col() {
       fn = reinterpret_cast<EncodeIm2colFn>(ptr);
   }
   return fn;
+}
+
+// ---- tensor maps of bf16 tensors: 128B swizzle, 256-byte L2 promotion, out-of-bounds elements read as zero.  Both
+// encoders need their driver entry point (get_encode / get_encode_im2col), which the caller checks first.
+
+// an NHWC view as the 4-D tensor (C, W, H, N): dimension sizes and the byte strides of W, H, N
+static void nhwc_dims(const SyTensor& t, cuuint64_t (&dims)[4], cuuint64_t (&strides)[3]) {
+  dims[0] = (cuuint64_t)t.c; dims[1] = (cuuint64_t)t.w; dims[2] = (cuuint64_t)t.h; dims[3] = (cuuint64_t)t.n;
+  strides[0] = (cuuint64_t)t.pitch * 2;
+  strides[1] = (cuuint64_t)t.pitch * 2 * t.w;
+  strides[2] = (cuuint64_t)t.pitch * 2 * t.w * t.h;
+}
+
+// tiled map of a rank-`rank` tensor (innermost dimension first), box `box`, unit element strides
+static CUresult encode_tiled_bf16(CUtensorMap* map, cuuint32_t rank, const void* ptr, const cuuint64_t* dims,
+                                  const cuuint64_t* strides, const cuuint32_t* box) {
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  return get_encode()(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(ptr), dims, strides, box, estr,
+                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+// im2col map of the input view x of a kh x kw convolution (padding (k - 1) / 2, stride `stride`): the bounding box of
+// base pixels is [-pad, dim + pad - (k - 1)) per spatial dim, walked with the stride; one load brings `pixels`
+// consecutive base pixels x 64 channels (one 128-byte swizzle row), shifted by the filter tap
+static CUresult encode_im2col_nhwc(CUtensorMap* map, const SyTensor& x, int kh, int kw, int stride, int pixels) {
+  cuuint64_t dims[4], strides[3];
+  nhwc_dims(x, dims, strides);
+  const int ph = (kh - 1) / 2, pw = (kw - 1) / 2;
+  int lower[2] = {-pw, -ph};                                   // {W, H}
+  int upper[2] = {pw - (kw - 1), ph - (kh - 1)};
+  const cuuint32_t estr[4] = {1, (cuuint32_t)stride, (cuuint32_t)stride, 1};
+  return get_encode_im2col()(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, x.ptr, dims, strides, lower, upper, 64,
+                             (cuuint32_t)pixels, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
 static int num_sms() { return sm_count(); }

@@ -169,6 +169,35 @@ def test_conv_tiling_plan_and_overrides_without_gpu():
         ops.conv2d_plan(16, 38, 60, 256, 256, 3, 1, tile_bn=96)
 
 
+def test_conv_kernels_compile_without_spills(tmp_path):
+    """The tensor-core conv kernels fit their register budgets: ptxas reports 0 spill bytes for every production
+    instantiation of conv_tc_kernel (TL = false) and for every conv_wgrad_kernel, and prints no warning (e.g. C7520,
+    serialised wgmma) for either unit.  A spill costs speed silently; this is where a schedule change shows it first."""
+    import shutil
+    from streamyolo_b200 import build
+    if not os.path.exists(build.NVCC) and shutil.which("nvcc") is None:
+        pytest.skip("no nvcc")
+    nvcc = build.NVCC if os.path.exists(build.NVCC) else shutil.which("nvcc")
+    procs = {src: subprocess.Popen([nvcc] + build.COMMON + ["-c", os.path.join(build.CSRC, src), "-o",
+                                                            str(tmp_path / src.replace(".cu", ".o"))],
+                                   stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
+             for src in ("conv_tc.cu", "conv_wgrad.cu")}
+    checked = []
+    for src, proc in procs.items():
+        out = proc.communicate(timeout=600)[0]
+        assert proc.returncode == 0, out
+        assert not [ln for ln in out.splitlines() if ln.startswith("ptxas") and "warning" in ln.lower()], out
+        # "Compiling entry function '<mangled>'", "Function properties for <mangled>", "N bytes stack frame, S bytes spill
+        # stores, L bytes spill loads"
+        for name, st, ld in re.findall(r"Compiling entry function '(\w+)'[^\n]*\n[^\n]*\n\s*\d+ bytes stack frame, "
+                                       r"(\d+) bytes spill stores, (\d+) bytes spill loads", out):
+            if re.search(r"conv_tc_kernelILi\d+ELb0E|conv_wgrad_kernel", name):
+                checked.append(name)
+                assert (int(st), int(ld)) == (0, 0), f"{name}: {st} bytes spill stores, {ld} bytes spill loads"
+    assert sum("conv_tc_kernel" in n for n in checked) == 4, checked       # BN = 64 / 128 x linear / halo
+    assert sum("conv_wgrad_kernel" in n for n in checked) == 3, checked    # BN = 64 / 128 / 256
+
+
 def test_pack_batch_tile_table():
     """Host side of sy_pack_conv_weights_batch: items are laid out in work TILES (64 output x 32 input channels; 64 outputs of a
     stem item), `begin` is the prefix sum of sy_pack_item_tiles (a host-only entry point: no GPU needed)."""
