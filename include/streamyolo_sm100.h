@@ -63,7 +63,7 @@ enum { SY_CONV_RAW = 0, SY_CONV_FUSED = 1 };
 typedef struct {
   const float* gamma; const float* beta;          /* [c] */
   float* running_mean; float* running_var;        /* [c], updated in place (may be NULL) */
-  int64_t* num_batches_tracked;                   /* += number of statistic groups (may be NULL) */
+  int64_t* num_batches_tracked;                   /* += number of running-statistics updates (may be NULL) */
   int32_t c_begin;
 } SyBnSegment;
 
@@ -101,6 +101,11 @@ typedef struct {
   /* ---- tiling override (sy_conv2d_tc only; 0 = the planner's choice) ---- */
   int32_t tile_mode;     /* 1 = linear tiles, 2 = halo where the conv is 3x3 stride 1 (linear elsewhere); as SyConvPlan.mode */
   int32_t tile_bn;       /* tile width 64 or 128 */
+  /* ---- running-statistics updates per statistics group (sy_conv2d_tc only) ---- */
+  int32_t stat_updates;  /* 0 or 1: one update per group.  2: the launch's single group is folded into the running
+                          * statistics twice, in the order and roundings of a two-group launch whose groups have equal
+                          * statistics, and num_batches_tracked += 2 -- one pass over a batch that stands for two identical
+                          * passes (a still frame duplicated into a pair).  Needs bn[] and one group; other values: SY_EINVAL */
 } SyConvDesc;
 
 /* Rows of the statistics workspace (= SM count: one row per persistent CTA). */
@@ -405,6 +410,21 @@ typedef struct SyPairLabelsDesc {
   int32_t* flags_out;      /* [n_items][2] */
 } SyPairLabelsDesc;
 int sy_pair_labels(const SyPairLabelsDesc* d, sy_stream_t stream);
+
+/* The same for n independent frames: the label half of TrainTransform(max_labels, hsv=False, flip)
+ * (exps/data/data_augment_flip.py:170-234), the dataset transform of the still-image baseline.  Per frame the rules of
+ * sy_pair_labels; flags_out[i] is frame i's effective mirror bit for sy_letterbox over the same n frames. */
+typedef struct SyFrameLabelsDesc {
+  const double* ann;       /* [n][max_rows][5] x1, y1, x2, y2, cls */
+  const int32_t* counts;   /* [n] valid rows (clamped to [0, max_rows]) */
+  const int32_t* mirror;   /* [n] mirror bits (may be NULL when flip == 0) */
+  int32_t n, max_rows, max_labels, flip;
+  int32_t width;           /* width of the frame entering the transform: the mirror axis */
+  double r;                /* letterbox scale min(H / h, W / w) */
+  float* labels;           /* [n][max_labels][5] cls, cx, cy, w, h */
+  int32_t* flags_out;      /* [n] */
+} SyFrameLabelsDesc;
+int sy_frame_labels(const SyFrameLabelsDesc* d, sy_stream_t stream);
 
 /* Image half: uint8 HWC BGR frames [n][h][w][3] -> fp32 planar [n][3][out_h][out_w] (a [B][6][H][W] pair batch when
  * n = 2B).  Each frame goes through cv2.resize(INTER_LINEAR) h x w -> mid_h x mid_w (load_resized_img,

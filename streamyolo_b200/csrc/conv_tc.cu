@@ -108,6 +108,7 @@ struct Params {
   float momentum, eps;
   double inv_cnt[2];        // 1 / (values per channel) of statistics group 0 | 1 (host-computed: no fp64 division in the tail)
   float unbias[2];          // cnt / (cnt - 1) of each group: biased -> unbiased variance for the running statistics
+  int updates;              // running-statistics updates per channel: 1, or 2 (two groups, or one group applied twice)
   float* ss;                // [2 (scale|shift)][2 groups][Cout]
   float* mi;                // optional [2 (mean|invstd)][2 groups][Cout] for the backward pass
   unsigned int* sync;       // two counters (grid barrier + exit ticket), zero between launches
@@ -863,7 +864,8 @@ __device__ __forceinline__ void bn_tail(const Params& p, const Smem& sm, int tid
         p.mi[(1 * 2 + g) * p.Cout + c] = istd;
       }
     }
-    const float mean1 = __shfl_sync(0xffffffffu, mean_f, 1), var1 = __shfl_sync(0xffffffffu, var_f, 1);
+    // the second update: group 1's statistics, or group 0's again when the launch repeats its single group
+    const float mean1 = __shfl_sync(0xffffffffu, mean_f, groups - 1), var1 = __shfl_sync(0xffffffffu, var_f, groups - 1);
     if (lane == 0) {
       float rm = pre_rm, rv = pre_rv;
       if (c != c_first) {
@@ -872,7 +874,7 @@ __device__ __forceinline__ void bn_tail(const Params& p, const Smem& sm, int tid
       }
       rm = (1.f - p.momentum) * rm + p.momentum * mean_f;
       rv = (1.f - p.momentum) * rv + p.momentum * (var_f * p.unbias[0]);
-      if (groups == 2) {
+      if (p.updates == 2) {
         rm = (1.f - p.momentum) * rm + p.momentum * mean1;
         rv = (1.f - p.momentum) * rv + p.momentum * (var1 * p.unbias[1]);
       }
@@ -883,7 +885,7 @@ __device__ __forceinline__ void bn_tail(const Params& p, const Smem& sm, int tid
   if (et == 0) tl_rec<TL>(p, tl, 4, 7, 0, 0);
   if (et == 0 && blockIdx.x == 0) {
     for (int sgi = 0; sgi < p.n_seg; ++sgi)          // (a reduction: no round trip -- a load-add-store ended CTA 0 ~1 us late)
-      if (p.seg[sgi].nbt) atomicAdd(reinterpret_cast<unsigned long long*>(p.seg[sgi].nbt), (unsigned long long)groups);
+      if (p.seg[sgi].nbt) atomicAdd(reinterpret_cast<unsigned long long*>(p.seg[sgi].nbt), (unsigned long long)p.updates);
   }
   if (et == 0 && ticket == gridDim.x - 1) {   // every CTA is past the barrier: re-arm for the next launch
     p.sync[0] = 0u;
@@ -1182,6 +1184,16 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   SY_REQUIRE(d->debug_flags == 0 || d->debug_flags == 2, SY_EINVAL, "conv2d_tc: debug_flags %d unsupported", d->debug_flags);
   SY_REQUIRE(tc::tiling_override_ok(d->tile_mode, d->tile_bn), SY_EINVAL, "conv2d_tc: tile_mode %d / tile_bn %d unsupported",
              d->tile_mode, d->tile_bn);
+  {
+    const bool one_group = !(d->split_n > 0 && d->split_n < x.n);
+    SY_REQUIRE(d->stat_updates >= 0 && d->stat_updates <= 2, SY_EINVAL, "conv2d_tc: stat_updates %d unsupported (0, 1 or 2)",
+               d->stat_updates);
+    SY_REQUIRE(d->stat_updates < 2 || (d->mode == SY_CONV_RAW && d->stat_partials != nullptr && d->bn[0].gamma != nullptr),
+               SY_EINVAL, "conv2d_tc: stat_updates = 2 needs the BatchNorm finalize (RAW mode, stat_partials and bn[])");
+    SY_REQUIRE(d->stat_updates < 2 || one_group, SY_EINVAL,
+               "conv2d_tc: stat_updates = 2 repeats a single statistics group, but split_n = %d splits %d images in two",
+               d->split_n, x.n);
+  }
   SY_REQUIRE(tc::get_encode() != nullptr, SY_EARCH, "cuTensorMapEncodeTiled not available from the driver");
 
   tc::Params p{};
@@ -1244,6 +1256,8 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
         p.inv_cnt[g] = cnt > 0.0 ? 1.0 / cnt : 0.0;
         p.unbias[g] = cnt > 1.0 ? (float)(cnt / (cnt - 1.0)) : 1.0f;
       }
+      p.updates = (groups == 2 || d->stat_updates == 2) ? 2 : 1;
+      if (groups == 1) p.unbias[1] = p.unbias[0];      // a repeated update uses group 0's count
     }
     p.ss = d->scale_shift;
     p.mi = d->mean_invstd;

@@ -2,6 +2,7 @@
 //   * sy_pair_labels   the label half of DoubleTrainTransform (/root/reference/exps/data/data_augment_flip.py:176-234):
 //                      mirror, xyxy -> cxcywh, * r, the min(w, h) > 1 filter and its all-filtered fallback, padding to
 //                      max_labels; also the per-frame mirror bit the image kernel applies
+//   * sy_frame_labels  the same per frame for single frames: the label half of TrainTransform (data_augment_flip.py:170-234)
 //   * sy_letterbox     the image half: cv2.resize(INTER_LINEAR) on uint8 (OpenCV's 11-bit fixed-point bilinear), the
 //                      mirror, the 114 pad and HWC uint8 -> CHW fp32; optionally preceded by load_resized_img's resize
 //                      (tal_flip_one_future_argoversedataset.py:179-187).  With no pad and no flags it is the streaming
@@ -119,16 +120,12 @@ __device__ __forceinline__ void frame_box(const double* row, bool mirror, double
   v[3] = h * r;
 }
 
-__global__ void __launch_bounds__(128) pair_labels_kernel(SyPairLabelsDesc d) {
+// The label transform of one frame, run by one warp (every lane takes part in the ballots): ``ann`` [n][5] rows, ``want`` =
+// the frame's mirror was drawn and flip is on; writes [max_labels][5] ``out`` and the effective mirror bit.
+__device__ __forceinline__ void frame_labels_warp(const double* __restrict__ ann, int n, bool want, double width, double r,
+                                                  int max_labels, float* __restrict__ out, int32_t* flag_out) {
   const int lane = threadIdx.x & 31;
-  const int fi = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // (item, frame) = (fi >> 1, fi & 1)
-  if (fi >= 2 * d.n_items) return;
-  const int item = fi >> 1, frame = fi & 1;
-  const double* ann = d.ann + (long long)fi * d.max_rows * 5;
-  const int n = min(max(d.counts[fi], 0), d.max_rows);
-  const bool a = d.flip != 0 && d.mirror != nullptr && d.mirror[item] != 0 && n > 0;
-  const double width = (double)d.width, r = d.r;
-  float* out = (frame == 0 ? d.labels_fut : d.labels_cur) + (long long)item * d.max_labels * 5;
+  const bool a = want && n > 0;
   int kept = 0;                                    // rows that survive the min(w, h) > 1 filter
   for (int i0 = 0; i0 < n; i0 += 32) {
     bool keep = false;
@@ -142,7 +139,7 @@ __global__ void __launch_bounds__(128) pair_labels_kernel(SyPairLabelsDesc d) {
   const bool fallback = kept == 0;                 // nothing left: the unmirrored frame and all rows, unfiltered
   const bool mirror = a && !fallback;
   int written = 0;
-  for (int i0 = 0; i0 < n && written < d.max_labels; i0 += 32) {
+  for (int i0 = 0; i0 < n && written < max_labels; i0 += 32) {
     const int i = i0 + lane;
     double v[4];
     bool keep = false;
@@ -152,15 +149,36 @@ __global__ void __launch_bounds__(128) pair_labels_kernel(SyPairLabelsDesc d) {
     }
     const unsigned m = __ballot_sync(0xffffffffu, keep);
     const int slot = written + __popc(m & ((1u << lane) - 1u));
-    if (keep && slot < d.max_labels) {
+    if (keep && slot < max_labels) {
       float* q = out + slot * 5;
       q[0] = (float)ann[i * 5 + 4];
       q[1] = (float)v[0], q[2] = (float)v[1], q[3] = (float)v[2], q[4] = (float)v[3];
     }
     written += __popc(m);
   }
-  for (int e = min(written, d.max_labels) * 5 + lane; e < d.max_labels * 5; e += 32) out[e] = 0.f;
-  if (lane == 0) d.flags_out[fi] = mirror ? 1 : 0;
+  for (int e = min(written, max_labels) * 5 + lane; e < max_labels * 5; e += 32) out[e] = 0.f;
+  if (lane == 0) *flag_out = mirror ? 1 : 0;
+}
+
+__global__ void __launch_bounds__(128) pair_labels_kernel(SyPairLabelsDesc d) {
+  const int fi = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;     // (item, frame) = (fi >> 1, fi & 1)
+  if (fi >= 2 * d.n_items) return;
+  const int item = fi >> 1, frame = fi & 1;
+  const int n = min(max(d.counts[fi], 0), d.max_rows);
+  const bool want = d.flip != 0 && d.mirror != nullptr && d.mirror[item] != 0;
+  float* out = (frame == 0 ? d.labels_fut : d.labels_cur) + (long long)item * d.max_labels * 5;
+  frame_labels_warp(d.ann + (long long)fi * d.max_rows * 5, n, want, (double)d.width, d.r, d.max_labels, out,
+                    d.flags_out + fi);
+}
+
+// One warp per frame of a single-frame batch (TrainTransform).
+__global__ void __launch_bounds__(128) frame_labels_kernel(SyFrameLabelsDesc d) {
+  const int fi = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (fi >= d.n) return;
+  const int n = min(max(d.counts[fi], 0), d.max_rows);
+  const bool want = d.flip != 0 && d.mirror != nullptr && d.mirror[fi] != 0;
+  frame_labels_warp(d.ann + (long long)fi * d.max_rows * 5, n, want, (double)d.width, d.r, d.max_labels,
+                    d.labels + (long long)fi * d.max_labels * 5, d.flags_out + fi);
 }
 
 }  // namespace sy
@@ -178,6 +196,18 @@ extern "C" int sy_pair_labels(const SyPairLabelsDesc* d, sy_stream_t stream_) {
   const int warps = 2 * d->n_items;
   pair_labels_kernel<<<cdiv(warps, 4), 128, 0, stream>>>(*d);
   return launch_status("pair_labels_kernel");
+}
+
+extern "C" int sy_frame_labels(const SyFrameLabelsDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr && d->ann != nullptr && d->counts != nullptr && d->labels != nullptr && d->flags_out != nullptr,
+             SY_EINVAL, "frame_labels: null pointer");
+  SY_REQUIRE(d->n > 0 && d->max_rows > 0 && d->max_labels > 0 && d->width > 0 && d->r > 0.0, SY_EINVAL,
+             "frame_labels: bad sizes (frames %d, rows %d, max_labels %d, width %d)", d->n, d->max_rows, d->max_labels,
+             d->width);
+  SY_REQUIRE(d->flip == 0 || d->mirror != nullptr, SY_EINVAL, "frame_labels: flip without mirror bits");
+  frame_labels_kernel<<<cdiv(d->n, 4), 128, 0, stream>>>(*d);
+  return launch_status("frame_labels_kernel");
 }
 
 extern "C" int sy_letterbox(const SyLetterboxDesc* d, sy_stream_t stream_) {

@@ -1,9 +1,10 @@
 """The data loader's image transforms on the device, from the uint8 BGR frames the dataset holds to the model's input.
 
 ``pair_transform`` = DoubleTrainTransform(max_labels, hsv=False, flip) / DoubleValTransform
-(/root/reference/exps/data/data_augment_flip.py:141-234) for a batch of frame pairs, ``stream_frame`` = the streaming
+(/root/reference/exps/data/data_augment_flip.py:141-234) for a batch of frame pairs, ``frame_transform`` =
+TrainTransform / ValTransform (:170-263) for a batch of single frames, ``stream_frame`` = the streaming
 driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60, 176-181).  Both are bit-identical to the cv2 / numpy host code
-they replace (sy_pair_labels, sy_letterbox); INTEGRATION.md shows where they plug in.
+they replace (sy_pair_labels, sy_frame_labels, sy_letterbox); INTEGRATION.md shows where they plug in.
 """
 import torch
 
@@ -50,6 +51,43 @@ def pair_transform(frames, ann, counts, mirror, input_size, max_labels=50, flip=
         flags = torch.empty((b, 2), dtype=torch.int32, device=frames.device)
         ops.pair_labels(ann, counts, mirror if flip else None, flip, mid[1], r, labels[0], labels[1], flags)
     ops.letterbox(frames.view(2 * b, h, w, 3), mid, dst, x, flags)
+    return x, labels
+
+
+def frame_transform(frames, ann, counts, mirror, input_size, max_labels=50, flip=True, raw=False, out=None):
+    """Train / validation transform of a batch of single frames: TrainTransform(max_labels, hsv=False, flip) / ValTransform
+    (/root/reference/exps/data/data_augment_flip.py:170-263), the dataset transform of the still-image baseline
+    (cfgs/l_s50_still_dfp_flip.py).
+
+    frames  uint8 CUDA [B, h, w, 3], BGR (``raw=True``: what cv2.imread returned, and load_resized_img's resize runs first)
+    ann     float64 [B, M, 5] rows x1, y1, x2, y2, cls, or None for the validation transform (no labels, no mirror)
+    counts  int32 [B] valid rows of ``ann``
+    mirror  int32 [B] each frame's random mirror bit (``random.randrange(2)`` of TrainTransform)
+    out     ``(x, labels)`` of an earlier call to write into (static buffers for CUDA-graph capture)
+
+    -> ``(x, labels)``: x fp32 [B, 3, H, W], labels fp32 [B, max_labels, 5] (cls, cx, cy, w, h), or ``(x, None)`` without
+    annotations.  Nothing is read back to the host."""
+    ops._require(torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+                 and frames.is_contiguous(), "frame_transform: frames must be contiguous uint8 [B, h, w, 3]")
+    b, h, w, _ = frames.shape
+    mid = _fit(h, w, input_size)[1] if raw else (h, w)
+    r, dst = _fit(mid[0], mid[1], input_size)
+    if out is None:
+        x = torch.empty((b, 3, input_size[0], input_size[1]), dtype=torch.float32, device=frames.device)
+        labels = None
+        if ann is not None:
+            labels = torch.empty((b, max_labels, 5), dtype=torch.float32, device=frames.device)
+    else:
+        x, labels = out
+    ops._require(torch.is_tensor(x) and tuple(x.shape) == (b, 3, input_size[0], input_size[1]),
+                 "frame_transform: out image must be [B, 3, H, W]")
+    flags = None
+    if ann is not None:
+        ops._require(torch.is_tensor(labels) and labels.dim() == 3 and labels.shape[1] == max_labels,
+                     "frame_transform: out labels must be [B, max_labels, 5]")
+        flags = torch.empty((b,), dtype=torch.int32, device=frames.device)
+        ops.frame_labels(ann, counts, mirror if flip else None, flip, mid[1], r, labels, flags)
+    ops.letterbox(frames, mid, dst, x, flags)
     return x, labels
 
 

@@ -28,6 +28,7 @@ mode with gradients enabled returns ``loss_with_autograd`` (the step as one auto
 import torch
 
 from . import engine
+from .pipe_head import PIPEHead
 from .tal_head import _f32
 from .. import ops
 from ..ops import View
@@ -376,22 +377,49 @@ def _walk(T: Tape, head, grad_scale, sink):
     sink.finish()
 
 
+def label_pair(model, targets):
+    """(future, current) labels of a training batch.  A ``PIPEHead`` (the still-image baseline,
+    /root/reference/exps/model/pipe_head.py) takes ONE label tensor and uses it for both, as ``PIPEHead.forward`` does; the
+    TAL head needs the pair (indexing a single tensor would take the labels of images 0 and 1)."""
+    if not torch.is_tensor(targets):
+        return targets
+    if not isinstance(model.head, PIPEHead):
+        raise TypeError(f"{type(model.head).__name__} trains on (future labels, current labels); got one label tensor "
+                        f"{tuple(targets.shape)} (only PIPEHead takes a single tensor)")
+    return targets, targets
+
+
 def _record(model, x, targets):
-    """Recording forward of YOLOX(DFPPAFPN, TALHead) in train mode; returns (tape, loss vector [total, iou, conf, cls, l1, num_fg])."""
+    """Recording forward of YOLOX(DFPPAFPN, TALHead / PIPEHead) in train mode; returns (tape, loss vector [total, iou, conf,
+    cls, l1, num_fg]).
+
+    ``x`` [B, 6, H, W]: frame pairs, the two frames batched as 2B images with grouped statistics.  ``x`` [B, 3, H, W]: still
+    frames.  The reference duplicates them into identical pairs (dfp_pafpn.py:236-238), so its second backbone + PAFPN pass
+    repeats the first: same activations, same batch statistics, a second running-statistics update, and a backward that
+    is linear in the incoming gradient.  Here ONE pass runs over the B frames with each BatchNorm's running update applied
+    twice (stat_updates=2), and the DFP fusion reads that pass as both cur and sup, so the gradients of the two branches
+    meet in the same buffer."""
     assert model.training and model.head.use_l1
     if any(getattr(m, "groups", 1) > 1 for m in model.modules() if isinstance(m, torch.nn.Conv2d)):
         raise NotImplementedError("the training backward does not cover depthwise convolutions (depthwise=True): forward only")
+    targets = label_pair(model, targets)
     net = model.backbone
     xin = x.float().contiguous()
     b = xin.shape[0]
+    if xin.shape[1] not in (3, 6):
+        raise ValueError(f"training input must be [B, 6, H, W] frame pairs or [B, 3, H, W] still frames, got {tuple(xin.shape)}")
     dev = xin.device
     T = Tape(dev)
     with torch.no_grad(), engine.forward_scope(dev):
-        pans = engine.pafpn_frames(engine.Ctx(True, 2 * b, b, dev, T), net, xin, 2)
-        cur = tuple(p.imgs(0, b) for p in pans)
-        sup = tuple(p.imgs(b, b) for p in pans)
+        if xin.shape[1] == 3:
+            pans = engine.pafpn_frames(engine.Ctx(True, b, b, dev, T, stat_updates=2), net, xin, 1)
+            cur = sup = pans
+        else:
+            pans = engine.pafpn_frames(engine.Ctx(True, 2 * b, b, dev, T), net, xin, 2)
+            cur = tuple(p.imgs(0, b) for p in pans)
+            sup = tuple(p.imgs(b, b) for p in pans)
         ctx = engine.Ctx(True, b, b, dev, T)
-        fused = engine.dfp_fuse(ctx, net, cur, sup)
+        fused = engine.dfp_fuse(ctx, net, cur, sup)       # jian: two launches, one running update each (as the reference)
         loss = model.head.run(ctx, fused, targets)
     return T, loss
 
@@ -402,7 +430,8 @@ def _loss_dict(loss):
 
 
 def forward_backward(model, x, targets, grad_scale=1.0, sink=None):
-    """One training forward + backward of YOLOX(DFPPAFPN, TALHead) in train mode on a frame-pair batch ``x`` [B, 6, H, W].
+    """One training forward + backward of YOLOX(DFPPAFPN, TALHead) in train mode on a frame-pair batch ``x`` [B, 6, H, W]
+    (or of a still model, YOLOX(DFPPAFPN, PIPEHead), on ``x`` [B, 3, H, W] and one label tensor; see ``_record``).
     Returns the loss dict of YOLOX.forward (0-dim tensors).  Without ``sink`` the gradients are accumulated into ``p.grad``
     of every parameter (like autograd); with a sink (train.FlatSink) they are written where the sink says."""
     T, loss = _record(model, x, targets)
@@ -447,7 +476,8 @@ class _TrainLoss(torch.autograd.Function):
 def loss_with_autograd(model, x, targets):
     """Loss dict whose ``total_loss`` carries a grad_fn (see _TrainLoss); the other entries are detached values."""
     params = tuple(p for p in model.parameters() if p.requires_grad)
-    total, loss = _TrainLoss.apply(model, x, targets[0], targets[1], *params)
+    fut, cur = label_pair(model, targets)
+    total, loss = _TrainLoss.apply(model, x, fut, cur, *params)
     d = _loss_dict(loss)
     d["total_loss"] = total
     return d

@@ -38,15 +38,18 @@ def _trace(m, y):
 
 class Ctx:
     """Per-forward execution context.  ``tape`` (a ``backward.Tape``): the recording forward of a training step -- every op
-    keeps what its backward needs and is recorded on the tape; None: the plain forward."""
+    keeps what its backward needs and is recorded on the tape; None: the plain forward.  ``stat_updates=2``: every train-mode
+    conv of this context applies its (single-group) batch statistics to the running statistics twice -- one pass over a
+    batch standing for the reference's two identical passes over it (a still frame duplicated into a pair)."""
 
-    def __init__(self, train, n, split, device, tape=None):
+    def __init__(self, train, n, split, device, tape=None, stat_updates=1):
         self.train = train
         self.n = n              # images in the batched tensor
         self.split = split      # first image of statistics group 1 (== n: single group)
         self.groups = 2 if split < n else 1
         self.device = device
         self.tape = tape
+        self.stat_updates = stat_updates
         self.impl = "tc" if tape is not None else CONV_IMPL
 
     def rec(self, **kw):
@@ -175,8 +178,11 @@ def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, a
             c0 += m.conv.out_channels
         ss = torch.empty((2, 2, cout), dtype=torch.float32, device=ctx.device)
         mi = None if T is None else torch.empty((2, 2, cout), dtype=torch.float32, device=ctx.device)
+        # the keyword only where it is not the default: every other launch is issued exactly as before it existed
+        repeat = {} if ctx.stat_updates == 1 else {"stat_updates": ctx.stat_updates}
         ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl="tc", partials=partials, split_n=split, bn=segs,
-                   momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device), mean_invstd=mi)
+                   momentum=mom, eps=float(bn0.eps), scale_shift=ss, sync=_sync(mods[0], ctx.device), mean_invstd=mi,
+                   **repeat)
         ops.bn_act_apply(raw, ss[0].data_ptr(), ss[1].data_ptr(), split if split else n, act, res, y, y_goff1, res_goff1)
         if T is not None:
             T.rec(t="conv", mods=mods, x=x, k=(kh, kw), s=s, raw=raw, y=y, res=res, ss=ss, mi=mi, split=split, act=act,
@@ -185,6 +191,8 @@ def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, a
         return
     # CUDA-core path (cross-check of the tensor-core kernel; depthwise convs): conv, separate statistics pass, separate
     # finalize per module, apply
+    if ctx.stat_updates != 1:
+        raise NotImplementedError(f"repeated running-statistics updates run on the tensor-core conv only, not impl={impl!r}")
     ops.conv2d(x, wpk, raw, k, s, ops.SY_CONV_RAW, impl=impl)
     sc = torch.empty((2, 2, cout), dtype=torch.float32, device=ctx.device)
     sp = split if split else n

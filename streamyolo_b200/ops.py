@@ -32,7 +32,7 @@ class SyConvDesc(C.Structure):
                 ("momentum", C.c_float), ("eps", C.c_float), ("scale_shift", C.c_void_p), ("mean_invstd", C.c_void_p),
                 ("sync", C.c_void_p), ("debug_timeline", C.c_void_p),
                 ("debug_timeline_events", C.c_int32), ("debug_flags", C.c_int32), ("debug_f32", C.c_void_p),
-                ("tile_mode", C.c_int32), ("tile_bn", C.c_int32)]
+                ("tile_mode", C.c_int32), ("tile_bn", C.c_int32), ("stat_updates", C.c_int32)]
 
 
 class SyHeadPredDesc(C.Structure):
@@ -118,6 +118,12 @@ class SyPairLabelsDesc(C.Structure):
                 ("r", C.c_double), ("labels_fut", C.c_void_p), ("labels_cur", C.c_void_p), ("flags_out", C.c_void_p)]
 
 
+class SyFrameLabelsDesc(C.Structure):
+    _fields_ = [("ann", C.c_void_p), ("counts", C.c_void_p), ("mirror", C.c_void_p), ("n", C.c_int32),
+                ("max_rows", C.c_int32), ("max_labels", C.c_int32), ("flip", C.c_int32), ("width", C.c_int32),
+                ("r", C.c_double), ("labels", C.c_void_p), ("flags_out", C.c_void_p)]
+
+
 class SyLetterboxDesc(C.Structure):
     _fields_ = [("src", C.c_void_p), ("n", C.c_int32), ("h", C.c_int32), ("w", C.c_int32), ("mid_h", C.c_int32),
                 ("mid_w", C.c_int32), ("dst_h", C.c_int32), ("dst_w", C.c_int32), ("out_h", C.c_int32),
@@ -173,6 +179,7 @@ _SIG = {
                                      C.c_void_p]),
     "sy_scale_labels": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_float, C.c_void_p]),
     "sy_pair_labels": (C.c_int, [C.POINTER(SyPairLabelsDesc), C.c_void_p]),
+    "sy_frame_labels": (C.c_int, [C.POINTER(SyFrameLabelsDesc), C.c_void_p]),
     "sy_letterbox": (C.c_int, [C.POINTER(SyLetterboxDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
@@ -314,10 +321,11 @@ def conv_stat_rows():
 
 def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None, act=1, res: View = None,
            partials=None, split_n=0, timeline=None, debug_flags=0, bn=None, momentum=0.03, eps=1e-3, scale_shift=None,
-           sync=None, mean_invstd=None, debug_f32=None, tile_mode=0, tile_bn=0):
+           sync=None, mean_invstd=None, debug_f32=None, tile_mode=0, tile_bn=0, stat_updates=1):
     """``k`` is an int (square) or (kh, kw).  With ``partials`` (RAW mode, tensor-core path) returns the number
     of per-CTA statistic rows the launch writes.  ``tile_mode`` / ``tile_bn`` override the tensor-core tiling
-    (0 = planner; see conv2d_plan)."""
+    (0 = planner; see conv2d_plan).  ``stat_updates=2``: the single statistics group updates the running statistics
+    twice (one pass standing for two identical ones; SyConvDesc.stat_updates)."""
     d = SyConvDesc()
     d.x, d.y = x.st(), y.st()
     d.w = wpk.data_ptr()
@@ -344,6 +352,7 @@ def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None,
         d.mean_invstd = mean_invstd.data_ptr() if mean_invstd is not None else None
     d.debug_flags = debug_flags
     d.tile_mode, d.tile_bn = tile_mode, tile_bn
+    d.stat_updates = stat_updates
     d.debug_f32 = debug_f32.data_ptr() if debug_f32 is not None else None
     if timeline is not None:
         d.debug_timeline, d.debug_timeline_events = timeline.data_ptr(), timeline.numel() // 2
@@ -656,6 +665,28 @@ def pair_labels(ann, counts, mirror, flip, width, r, labels_fut, labels_cur, fla
     d.width, d.r = width, r
     d.labels_fut, d.labels_cur, d.flags_out = labels_fut.data_ptr(), labels_cur.data_ptr(), flags.data_ptr()
     _check(lib().sy_pair_labels(C.byref(d), _stream()))
+
+
+def frame_labels(ann, counts, mirror, flip, width, r, labels, flags):
+    """Label half of TrainTransform on the device (sy_frame_labels): ``ann`` fp64 [B, M, 5] (x1, y1, x2, y2, cls),
+    ``counts`` int32 [B], ``mirror`` int32 [B] (or None without flip); writes fp32 [B, max_labels, 5] ``labels`` and the
+    int32 [B] effective mirror bits ``flags``."""
+    _require(_tensor_ok(ann, torch.float64, 3) and ann.shape[2] == 5,
+             "frame_labels: annotations must be contiguous float64 [B, M, 5]")
+    b = ann.shape[0]
+    _require(_tensor_ok(counts, torch.int32, 1) and counts.shape[0] == b, "frame_labels: counts must be int32 [B]")
+    _require(mirror is None or (_tensor_ok(mirror, torch.int32, 1) and mirror.shape[0] == b),
+             "frame_labels: mirror must be int32 [B]")
+    _require(_tensor_ok(labels, torch.float32, 3) and labels.shape[0] == b and labels.shape[2] == 5,
+             "frame_labels: labels must be float32 [B, max_labels, 5]")
+    _require(_tensor_ok(flags, torch.int32, 1) and flags.shape[0] == b, "frame_labels: flags must be int32 [B]")
+    d = SyFrameLabelsDesc()
+    d.ann, d.counts = ann.data_ptr(), counts.data_ptr()
+    d.mirror = mirror.data_ptr() if mirror is not None else None
+    d.n, d.max_rows, d.max_labels, d.flip = b, ann.shape[1], labels.shape[1], int(flip)
+    d.width, d.r = width, r
+    d.labels, d.flags_out = labels.data_ptr(), flags.data_ptr()
+    _check(lib().sy_frame_labels(C.byref(d), _stream()))
 
 
 def letterbox(src, mid, dst, out, flags=None):

@@ -306,7 +306,9 @@ class FlatSink:
 
 
 class Trainer:
-    """H100-native training loop body for YOLOX(DFPPAFPN, TALHead): ``step(x, targets, lr)``."""
+    """H100-native training loop body for YOLOX(DFPPAFPN, TALHead): ``step(x, targets, lr)`` on frame pairs ``x``
+    [B, 6, H, W] and (future, current) labels; for the still-image baseline YOLOX(DFPPAFPN, PIPEHead) also on still frames
+    [B, 3, H, W] and one label tensor (one backbone pass, model/backward.py ``_record``)."""
 
     def __init__(self, model, lr=0.01, momentum=0.9, weight_decay=5e-4, ema_decay=0.9998, use_ema=True,
                  bucket_bytes=25 << 20, overlap=True):
