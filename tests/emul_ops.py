@@ -47,7 +47,7 @@ def conv_stat_rows():
 
 def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=None, partials=None, split_n=0,
            timeline=None, debug_flags=0, bn=None, momentum=0.03, eps=1e-3, scale_shift=None, sync=None, mean_invstd=None,
-           debug_f32=None, tile_mode=0, tile_bn=0):
+           debug_f32=None, tile_mode=0, tile_bn=0, stat_updates=1):
     kh, kw = (k, k) if isinstance(k, int) else k
     if impl == "dw":                                # depthwise: wpk [kh*kw][C]
         c = wpk.shape[1]
@@ -84,11 +84,12 @@ def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=
                 if mean_invstd is not None:
                     mean_invstd[0, gi, sl] = mean[sl]
                     mean_invstd[1, gi, sl] = invstd[sl]
-                if rm is not None:
-                    rm.mul_(1 - momentum).add_(momentum * mean[sl])
-                    rv.mul_(1 - momentum).add_(momentum * var[sl] * (cnt / max(cnt - 1, 1)))
-                if nbt is not None:
-                    nbt.add_(1)
+                for _ in range(stat_updates):
+                    if rm is not None:
+                        rm.mul_(1 - momentum).add_(momentum * mean[sl])
+                        rv.mul_(1 - momentum).add_(momentum * var[sl] * (cnt / max(cnt - 1, 1)))
+                    if nbt is not None:
+                        nbt.add_(1)
         PTRS[scale_shift[0].data_ptr()] = scale_shift[0]
         PTRS[scale_shift[1].data_ptr()] = scale_shift[1]
     return 132
