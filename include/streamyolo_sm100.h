@@ -11,7 +11,8 @@
  *     never synchronises the device and never throws; it returns 0 or an SY_E*
  *     status and `sy_last_error_string()` describes the last failure of the
  *     calling thread.  The caller owns every buffer (PyTorch caching allocator).
- *   - activations are NHWC bf16 "views" (SyTensor): pixel (n,y,x) channel c lives
+ *   - activations are NHWC 16-bit "views" (SyTensor), bf16 unless an entry point says otherwise (SyConvDesc.storage,
+ *     SyHeadPredDesc.storage, the *_f16 entry points): pixel (n,y,x) channel c lives
  *     at ptr + (((n*h + y)*w + x)*pitch + c) elements; pitch >= c lets a view be
  *     a channel slice of a wider concat buffer (pitch, slice offsets and c are
  *     multiples of 8 so that every pixel row is 16-byte aligned).
@@ -41,8 +42,11 @@ enum {
   SY_EWORKSPACE = 4
 };
 
+/* 16-bit activation storage of a launch (SyConvDesc.storage, SyHeadPredDesc.storage) */
+enum { SY_STORAGE_BF16 = 0, SY_STORAGE_F16 = 1 };
+
 typedef struct {
-  void* ptr;      /* bf16 */
+  void* ptr;      /* bf16 (fp16 where the entry point stores fp16) */
   int32_t n, h, w, c;
   int64_t pitch;  /* elements between consecutive pixels */
 } SyTensor;
@@ -106,6 +110,10 @@ typedef struct {
                           * statistics twice, in the order and roundings of a two-group launch whose groups have equal
                           * statistics, and num_batches_tracked += 2 -- one pass over a batch that stands for two identical
                           * passes (a still frame duplicated into a pair).  Needs bn[] and one group; other values: SY_EINVAL */
+  /* ---- activation storage (sy_conv2d_tc, sy_dwconv2d; sy_conv2d_simt takes bf16 only) ---- */
+  int32_t storage;       /* SY_STORAGE_BF16 (0): x, y, res and w are bf16.  SY_STORAGE_F16 (1): all four are IEEE fp16
+                          * (fp32 accumulation, one fp16 rounding of the stored result); FUSED mode only, without statistics,
+                          * bn[] or the debug timeline (SY_EINVAL otherwise); debug_f32 works as with bf16 */
 } SyConvDesc;
 
 /* Rows of the statistics workspace (= SM count: one row per persistent CTA). */
@@ -127,13 +135,14 @@ typedef struct SyConvPlan {
 int sy_conv2d_plan(int32_t n, int32_t h, int32_t w, int32_t cin, int32_t cout, int32_t kh, int32_t kw, int32_t stride,
                    int32_t tile_mode, int32_t tile_bn, SyConvPlan* out);
 /* plain CUDA-core direct convolution with the same x/y/w/FUSED contract (no statistics):
- * device-side cross-check of the tensor-core kernel. */
+ * device-side cross-check of the tensor-core kernel.  bf16 storage only (storage != 0: SY_EINVAL). */
 int sy_conv2d_simt(const SyConvDesc* d, sy_stream_t stream);
 
 /* Depthwise k x k convolution (groups = channels, k in {1, 3, 5}, stride 1 / 2): the first half of [yolox] DWConv, selected
  * by depthwise=True at exps/model/darknet.py:109, dfp_pafpn.py:31, tal_head.py:53.  Same descriptor and RAW / FUSED contract
  * as sy_conv2d_tc with x.c == y.c and w = bf16 [kh*kw][C]; the statistics fields are ignored (train-mode BatchNorm runs
- * through sy_channel_stats / sy_bn_finalize / sy_bn_act_apply).  Coalesced, vectorised CUDA-core kernel (HBM-bound). */
+ * through sy_channel_stats / sy_bn_finalize / sy_bn_act_apply).  Coalesced, vectorised CUDA-core kernel (HBM-bound).
+ * storage = SY_STORAGE_F16: x, y, res and w fp16, FUSED mode only. */
 int sy_dwconv2d(const SyConvDesc* d, sy_stream_t stream);
 
 /* Focus stem, part 1: [yolox] Focus space-to-depth (TL/BL/TR/BR channel order), used at
@@ -146,6 +155,9 @@ int sy_dwconv2d(const SyConvDesc* d, sy_stream_t stream);
  * [cout][3][64]. */
 int sy_focus_pack(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w_px, int32_t frames,
                   SyTensor y, sy_stream_t stream);
+/* The same with y in fp16 (input pixels rounded to fp16), for the stem conv of an fp16-storage forward. */
+int sy_focus_pack_f16(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w_px, int32_t frames,
+                      SyTensor y, sy_stream_t stream);
 
 /* -------- BatchNorm (train mode) + SiLU (replaces nn.BatchNorm2d + nn.SiLU inside
  * [yolox] BaseConv; eps/momentum from cfgs/s_s50_onex_dfp_tal_flip.py:40-44) ---------- */
@@ -177,7 +189,10 @@ int sy_upsample_nearest(SyTensor x, SyTensor y, sy_stream_t stream);
 /* [yolox] SPPBottleneck pooling (exps/model/darknet.py:156): y5,y9,y13 = stride-1
  * same-padded max pools (k = 5, 9, 13; -inf padding) of x. */
 int sy_spp_maxpool(SyTensor x, SyTensor y5, SyTensor y9, SyTensor y13, sy_stream_t stream);
-/* strided copy of a view (used for 3-channel duplicates and buffers). */
+/* The same on fp16 views (the maximum of fp16 values: a different bit order from bf16). */
+int sy_spp_maxpool_f16(SyTensor x, SyTensor y5, SyTensor y9, SyTensor y13, sy_stream_t stream);
+/* strided copy of a view (used for 3-channel duplicates and buffers).  sy_upsample_nearest and sy_copy only move
+ * 16-bit values, so they serve fp16 views unchanged. */
 int sy_copy(SyTensor x, SyTensor y, sy_stream_t stream);
 
 /* -------- head: prediction convs + decode (exps/model/tal_head.py:105-131,167-171,
@@ -195,6 +210,7 @@ typedef struct {
   int32_t decode;          /* xy = (xy + grid) * stride, wh = exp(wh) * stride */
   float* out;              /* [b, a_total, 5+ncls] float32 */
   float* origin;           /* [b, a_total, 4] raw reg (tal_head.py:185-194) or NULL */
+  int32_t storage;         /* SY_STORAGE_BF16 (0): cls_feat / reg_feat are bf16; SY_STORAGE_F16 (1): fp16 */
 } SyHeadPredDesc;
 int sy_head_pred_decode(const SyHeadPredDesc* d, sy_stream_t stream);
 
@@ -342,8 +358,10 @@ int sy_postprocess_nms(const SyNmsDesc* d, sy_stream_t stream);
  *   mode 1  out[i][taps-1-(r*kw+s)][co_offset + o] = w[o][i][r][s]     data-gradient operand (flipped taps, transposed
  *           channels; rows of out_pitch elements so that the conv1 | conv2 pair of a CSPLayer packs into one operand)
  *   mode 2  out[o][r][s*16 + i] = w[o][i][r][s], 64 columns per (o, r) Focus stem (see sy_focus_pack)
+ *   mode 0 | SY_PACK_F16, mode 2 | SY_PACK_F16: the same layouts in fp16 (operands of fp16-storage forwards)
  * Replaces the weight.to(bf16).permute chain a PyTorch host would run after every optimizer.step()
  * (exps/train_utils/double_trainer.py:119-121). */
+enum { SY_PACK_F16 = 0x100 };
 int sy_pack_conv_weight(const float* w, int32_t cout, int32_t cin, int32_t kh, int32_t kw, int32_t mode, void* out,
                         int64_t out_pitch, int32_t co_offset, sy_stream_t stream);
 

@@ -1,7 +1,10 @@
 // BatchNorm(train) finalize / apply+SiLU, nearest upsample, SPP max pools, strided copy:
-// vectorised (16-byte) HBM-bound kernels over NHWC bf16 views.
+// vectorised (16-byte) HBM-bound kernels over NHWC bf16 views.  The upsample and the copy only move 16-bit values and
+// serve fp16 views unchanged; the SPP max pools compare values and have an fp16 instantiation (sy_spp_maxpool_f16).
 #include <math.h>
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -156,11 +159,14 @@ __global__ void upsample_nearest_kernel(const __nv_bfloat16* __restrict__ x, lon
   }
 }
 
+// element-wise maximum of eight packed bf16 (F16: fp16) values
+template <bool F16>
 __device__ __forceinline__ uint4 bmax(const uint4 a, const uint4 b) {
+  using T2 = typename std::conditional<F16, __half2, __nv_bfloat162>::type;
   uint4 r;
-  const __nv_bfloat162* pa = reinterpret_cast<const __nv_bfloat162*>(&a);
-  const __nv_bfloat162* pb = reinterpret_cast<const __nv_bfloat162*>(&b);
-  __nv_bfloat162* pr = reinterpret_cast<__nv_bfloat162*>(&r);
+  const T2* pa = reinterpret_cast<const T2*>(&a);
+  const T2* pb = reinterpret_cast<const T2*>(&b);
+  T2* pr = reinterpret_cast<T2*>(&r);
 #pragma unroll
   for (int i = 0; i < 4; ++i) pr[i] = __hmax2(pa[i], pb[i]);
   return r;
@@ -168,8 +174,9 @@ __device__ __forceinline__ uint4 bmax(const uint4 a, const uint4 b) {
 
 // stride-1 same-padded max pools k = 5, 9, 13 (-inf padding) as a cascade of separable 5-wide pools
 // (5 o 5 = 9, 5 o 5 o 5 = 13 for max with -inf padding).  One block = one (image, 8-channel group) plane
-// held in shared memory; every pass is a 5-tap row or column max on packed bf16 (exact).
+// held in shared memory; every pass is a 5-tap row or column max on packed bf16 | fp16 (exact).
 constexpr int kSppMaxPix = 1024;
+template <bool F16>
 __global__ void __launch_bounds__(256)
 spp_maxpool_kernel(const __nv_bfloat16* __restrict__ x, long long xp, int H, int W, int C,
                    __nv_bfloat16* y5, long long p5, __nv_bfloat16* y9, long long p9,
@@ -191,7 +198,7 @@ spp_maxpool_kernel(const __nv_bfloat16* __restrict__ x, long long xp, int H, int
       uint4 m = bufA[i];
 #pragma unroll
       for (int d = -2; d <= 2; ++d)
-        if (d != 0 && xx + d >= 0 && xx + d < W) m = bmax(m, bufA[i + d]);
+        if (d != 0 && xx + d >= 0 && xx + d < W) m = bmax<F16>(m, bufA[i + d]);
       bufB[i] = m;
     }
     __syncthreads();
@@ -200,7 +207,7 @@ spp_maxpool_kernel(const __nv_bfloat16* __restrict__ x, long long xp, int H, int
       uint4 m = bufB[i];
 #pragma unroll
       for (int d = -2; d <= 2; ++d)
-        if (d != 0 && yy + d >= 0 && yy + d < H) m = bmax(m, bufB[i + d * W]);
+        if (d != 0 && yy + d >= 0 && yy + d < H) m = bmax<F16>(m, bufB[i + d * W]);
       bufA[i] = m;
       *reinterpret_cast<uint4*>(outs[lvl] + (base + i) * pitches[lvl] + g * 8) = m;
     }
@@ -209,6 +216,7 @@ spp_maxpool_kernel(const __nv_bfloat16* __restrict__ x, long long xp, int H, int
 }
 
 // large planes (not used by the 600x960 configs): direct nested-window version
+template <bool F16>
 __global__ void spp_maxpool_direct_kernel(const __nv_bfloat16* __restrict__ x, long long xp, int N, int H, int W, int C,
                                           __nv_bfloat16* y5, long long p5, __nv_bfloat16* y9, long long p9,
                                           __nv_bfloat16* y13, long long p13) {
@@ -228,10 +236,10 @@ __global__ void spp_maxpool_direct_kernel(const __nv_bfloat16* __restrict__ x, l
         const int ix = ox + dx;
         if (ix < 0 || ix >= W) continue;
         const uint4 v = *reinterpret_cast<const uint4*>(x + (((long long)n * H + iy) * W + ix) * xp + g * 8);
-        m13 = bmax(m13, v);
+        m13 = bmax<F16>(m13, v);
         const int ad = max(abs(dy), abs(dx));
-        if (ad <= 4) m9 = bmax(m9, v);
-        if (ad <= 2) m5 = bmax(m5, v);
+        if (ad <= 4) m9 = bmax<F16>(m9, v);
+        if (ad <= 2) m5 = bmax<F16>(m5, v);
       }
     }
     *reinterpret_cast<uint4*>(y5 + pix * p5 + g * 8) = m5;
@@ -344,21 +352,30 @@ extern "C" int sy_upsample_nearest(SyTensor x, SyTensor y, sy_stream_t stream_) 
   return launch_status("upsample_nearest_kernel");
 }
 
-extern "C" int sy_spp_maxpool(SyTensor x, SyTensor y5, SyTensor y9, SyTensor y13, sy_stream_t stream_) {
+template <bool F16>
+static int spp_maxpool(SyTensor x, SyTensor y5, SyTensor y9, SyTensor y13, sy_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   SY_REQUIRE(view_ok(x) && view_ok(y5) && view_ok(y9) && view_ok(y13), SY_EINVAL, "spp: bad views");
   SY_REQUIRE(y5.c == x.c && y9.c == x.c && y13.c == x.c && y5.h == x.h && y5.w == x.w && y5.n == x.n, SY_EINVAL,
              "spp: shape mismatch");
   if (x.h * x.w <= kSppMaxPix) {
-    spp_maxpool_kernel<<<x.n * (x.c / 8), 256, 0, stream>>>(CBF(x.ptr), x.pitch, x.h, x.w, x.c, BF(y5.ptr), y5.pitch,
+    spp_maxpool_kernel<F16><<<x.n * (x.c / 8), 256, 0, stream>>>(CBF(x.ptr), x.pitch, x.h, x.w, x.c, BF(y5.ptr), y5.pitch,
                                                             BF(y9.ptr), y9.pitch, BF(y13.ptr), y13.pitch);
   } else {
     const long long total = (long long)x.n * x.h * x.w * (x.c / 8);
-    spp_maxpool_direct_kernel<<<grid_for(total, 128), 128, 0, stream>>>(CBF(x.ptr), x.pitch, x.n, x.h, x.w, x.c,
+    spp_maxpool_direct_kernel<F16><<<grid_for(total, 128), 128, 0, stream>>>(CBF(x.ptr), x.pitch, x.n, x.h, x.w, x.c,
                                                                         BF(y5.ptr), y5.pitch, BF(y9.ptr), y9.pitch,
                                                                         BF(y13.ptr), y13.pitch);
   }
   return launch_status("spp_maxpool_kernel");
+}
+
+extern "C" int sy_spp_maxpool(SyTensor x, SyTensor y5, SyTensor y9, SyTensor y13, sy_stream_t stream) {
+  return spp_maxpool<false>(x, y5, y9, y13, stream);
+}
+
+extern "C" int sy_spp_maxpool_f16(SyTensor x, SyTensor y5, SyTensor y9, SyTensor y13, sy_stream_t stream) {
+  return spp_maxpool<true>(x, y5, y9, y13, stream);
 }
 
 extern "C" int sy_copy(SyTensor x, SyTensor y, sy_stream_t stream_) {

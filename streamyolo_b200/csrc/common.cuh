@@ -1,6 +1,7 @@
 // Shared helpers for libstreamyolo_sm100.so (built for sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -90,6 +91,33 @@ __device__ __forceinline__ float bf16_hi(uint32_t v) { return __uint_as_float(v 
 __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
   __nv_bfloat162 p = __floats2bfloat162_rn(a, b);  // .x = a (low half), .y = b
   return *reinterpret_cast<uint32_t*>(&p);
+}
+
+// ---- fp16 pack helpers (SY_STORAGE_F16: the eval / streaming forwards with IEEE half activations) ----------------
+__device__ __forceinline__ float f16_lo(uint32_t v) { return __half2float(__ushort_as_half((unsigned short)(v & 0xffffu))); }
+__device__ __forceinline__ float f16_hi(uint32_t v) { return __half2float(__ushort_as_half((unsigned short)(v >> 16))); }
+__device__ __forceinline__ uint32_t pack_f16(float a, float b) {
+  __half2 p = __floats2half2_rn(a, b);             // .x = a (low half), .y = b
+  return *reinterpret_cast<uint32_t*>(&p);
+}
+// the 16-bit activation storage type as a template flag: F16 = IEEE half, otherwise bf16
+template <bool F16>
+__device__ __forceinline__ float st_lo(uint32_t v) {
+  if constexpr (F16) return f16_lo(v); else return bf16_lo(v);
+}
+template <bool F16>
+__device__ __forceinline__ float st_hi(uint32_t v) {
+  if constexpr (F16) return f16_hi(v); else return bf16_hi(v);
+}
+template <bool F16>
+__device__ __forceinline__ uint32_t st_pack(float a, float b) {
+  if constexpr (F16) return pack_f16(a, b); else return pack_bf16(a, b);
+}
+// eight 16-bit values of one 16-byte chunk as floats
+template <bool F16>
+__device__ __forceinline__ void st_unpack8(const uint4& u, float (&v)[8]) {
+  v[0] = st_lo<F16>(u.x); v[1] = st_hi<F16>(u.x); v[2] = st_lo<F16>(u.y); v[3] = st_hi<F16>(u.y);
+  v[4] = st_lo<F16>(u.z); v[5] = st_hi<F16>(u.z); v[6] = st_lo<F16>(u.w); v[7] = st_hi<F16>(u.w);
 }
 
 // SiLU = v * rcp(1 + 2^(-v * log2 e)) on the two approximate SFU ops (ex2.approx, rcp.approx: ~2 ulp fp32, far below

@@ -72,11 +72,12 @@ __global__ void conv_simt_kernel(const SimtConvParams p) {
 // 12 focus channels + 4 zero channels, plus 16 zero channels = 64 channels = one 128-byte row per pixel (TMA boxes
 // whose inner extent runs past a 96-byte pixel were measured 2.6x slower: 354 vs 133 us for the stem conv), so that
 // the stem is a 3x1 conv with three 64-deep K blocks for the tensor-core kernel.  thread = (pixel, tap | pad).
-// Input pixels are rounded to bf16.
+// Input pixels are rounded to bf16 (F16: to fp16, for the stem of an fp16-storage forward).
 // One block pass per output row (image, oy); threads walk (ox, tap) with shifts only (the first version resolved
 // (tap, ox, oy, image, frame) from a flat index with five 64-bit divisions per thread).
+template <bool F16>
 __global__ void focus_pack_kernel(const float* __restrict__ x, int B, int in_ch, int H, int W, int frames,
-                                  __nv_bfloat16* y, long long y_pitch) {
+                                  uint16_t* y, long long y_pitch) {
   const int Ho = H / 2, Wo = W / 2;
   const int rows = frames * B * Ho;
   for (int row = blockIdx.x; row < rows; row += gridDim.x) {
@@ -99,8 +100,9 @@ __global__ void focus_pack_kernel(const float* __restrict__ x, int B, int in_ch,
         for (int fc = 0; fc < 12; ++fc) v[fc] = 0.f;
       }
       uint4* dst = reinterpret_cast<uint4*>(y + ((long long)row * Wo + ox) * y_pitch + s * 16);
-      dst[0] = make_uint4(pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
-      dst[1] = make_uint4(pack_bf16(v[8], v[9]), pack_bf16(v[10], v[11]), 0u, 0u);
+      dst[0] = make_uint4(st_pack<F16>(v[0], v[1]), st_pack<F16>(v[2], v[3]), st_pack<F16>(v[4], v[5]),
+                          st_pack<F16>(v[6], v[7]));
+      dst[1] = make_uint4(st_pack<F16>(v[8], v[9]), st_pack<F16>(v[10], v[11]), 0u, 0u);
     }
   }
 }
@@ -157,6 +159,7 @@ extern "C" int sy_conv2d_simt(const SyConvDesc* d, sy_stream_t stream_) {
   SY_REQUIRE(view_ok(x) && view_ok(y) && d->w != nullptr, SY_EINVAL, "conv2d_simt: bad x/y view or null weights");
   SY_REQUIRE((d->kh == 1 || d->kh == 3) && (d->kw == 1 || d->kw == 3) && (d->stride == 1 || d->stride == 2), SY_EINVAL,
              "conv2d_simt: kernel %dx%d stride %d unsupported", d->kh, d->kw, d->stride);
+  SY_REQUIRE(d->storage == SY_STORAGE_BF16, SY_EINVAL, "conv2d_simt: bf16 storage only (storage %d)", d->storage);
   SimtConvParams p{};
   p.pad_h = (d->kh - 1) / 2; p.pad_w = (d->kw - 1) / 2;
   p.N = x.n; p.H = x.h; p.W = x.w; p.Cin = x.c; p.Cout = y.c; p.kh = d->kh; p.kw = d->kw; p.stride = d->stride;
@@ -178,8 +181,9 @@ extern "C" int sy_conv2d_simt(const SyConvDesc* d, sy_stream_t stream_) {
   return launch_status("conv_simt_kernel");
 }
 
-extern "C" int sy_focus_pack(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w_px, int32_t frames,
-                             SyTensor y, sy_stream_t stream_) {
+template <bool F16>
+static int focus_pack(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w_px, int32_t frames, SyTensor y,
+                      sy_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   SY_REQUIRE(x && view_ok(y), SY_EINVAL, "focus_pack: null input or bad output view");
   SY_REQUIRE(h % 2 == 0 && w_px % 2 == 0 && frames >= 1 && frames * 3 <= in_ch, SY_EINVAL,
@@ -188,9 +192,19 @@ extern "C" int sy_focus_pack(const float* x, int32_t b, int32_t in_ch, int32_t h
              "focus_pack: output view must be [frames*b, h/2, w/2, 64]");
   const int rows = y.n * y.h;                                   // one block pass per output row
   const int blocks = rows < sm_count() * 16 ? rows : sm_count() * 16;
-  focus_pack_kernel<<<blocks, 256, 0, stream>>>(x, b, in_ch, h, w_px, frames, reinterpret_cast<__nv_bfloat16*>(y.ptr),
-                                                y.pitch);
+  focus_pack_kernel<F16><<<blocks, 256, 0, stream>>>(x, b, in_ch, h, w_px, frames, reinterpret_cast<uint16_t*>(y.ptr),
+                                                     y.pitch);
   return launch_status("focus_pack_kernel");
+}
+
+extern "C" int sy_focus_pack(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w_px, int32_t frames,
+                             SyTensor y, sy_stream_t stream) {
+  return focus_pack<false>(x, b, in_ch, h, w_px, frames, y, stream);
+}
+
+extern "C" int sy_focus_pack_f16(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w_px, int32_t frames,
+                                 SyTensor y, sy_stream_t stream) {
+  return focus_pack<true>(x, b, in_ch, h, w_px, frames, y, stream);
 }
 
 extern "C" int sy_stats_num_partials(int32_t n, int32_t hw) { return n * cdiv(hw, kStatChunk); }

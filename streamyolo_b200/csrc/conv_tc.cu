@@ -33,6 +33,10 @@
 // (deterministic), updates the running statistics and publishes scale/shift for the normalise+SiLU
 // pass.  (Two such kernels must not run concurrently on one GPU: the barrier needs the whole grid.)
 //
+// Activation storage: conv_tc_kernel reads and writes bf16 (every mode).  conv_tc_f16_kernel runs the same roles on fp16
+// activations and weights (wgmma .f16 inputs, fp16 tensor maps, fp16 epilogue pack / residual): the FUSED epilogue of the
+// eval and streaming forwards only, so its statistics warps just cycle the staging-tile barriers and its tail is empty.
+//
 // Replaces the cuDNN conv + ATen BN/SiLU triplet behind [yolox] BaseConv
 // (exps/model/darknet.py:115-165, dfp_pafpn.py:33-105, tal_head.py:55-104 of StreamYOLO).
 #include <cuda.h>
@@ -45,7 +49,7 @@ namespace sy {
 namespace tc {
 
 constexpr int kBlockM = 128;
-constexpr int kBlockK = 64;              // bf16 elements = one 128-byte swizzle row
+constexpr int kBlockK = 64;              // 16-bit elements = one 128-byte swizzle row
 constexpr int kThreads = 640;       // five warpgroups
 // registers per thread after setmaxnreg: the launch grants 96 x 640; the load/store warpgroup (warps 16-19) keeps 32 and
 // hands the rest to the MMA warpgroups (accumulators: BN / 2 registers) and the statistics warpgroups (per-lane sums)
@@ -96,7 +100,7 @@ struct Params {
   int stage_tiles;          // 1 or 2 epilogue staging tiles
   int stagesA;              // halo mode: halo ring depth
   int mode, act;
-  const __nv_bfloat16* res;
+  const uint16_t* res;      // 16-bit elements of the kernel's storage type (bf16 | fp16)
   long long res_pitch;
   const float* scale;
   const float* shift;
@@ -579,8 +583,8 @@ __device__ __forceinline__ void statistics(const Params& p, const Smem& sm, int 
 // Warpgroup wg owns rows [64 wg, 64 wg + 64) of the tile: it issues the wgmma stream for them (accumulators in
 // registers), then converts its rows of every 64-column slab into the staging tile.  A ring stage is handed back to the
 // producers one commit group late (wgmma.wait_group 1), so the next group's MMAs are queued while the last ones drain.
-// Returns the debug-timeline cursor of thread 0, which the kernel tail carries on.
-template <int BN, bool TL, int AM>
+// Returns the debug-timeline cursor of thread 0, which the kernel tail carries on.  F16: fp16 operands and output.
+template <int BN, bool TL, int AM, bool F16>
 __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int tid) {
   // the compiler knows this range for threadIdx.x but not for the argument; with it the FUSED scale/shift fill below is
   // one guarded pass instead of a loop
@@ -664,7 +668,7 @@ __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int 
             const uint64_t db = make_smem_desc(smem_u32(sm.b + (ring.stage * kHaloTaps + j) * kBB));
 #pragma unroll
             for (int k = 0; k < kBlockK / 16; ++k)   // 16 bf16 = 32 bytes along K inside the swizzle row: +2 in (addr >> 4)
-              Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (cb | tap | k) != 0);
+              Wgmma<BN, 0, 0, F16>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (cb | tap | k) != 0);
           }
           wgmma_commit();
           wgmma_fence_operand(acc);
@@ -685,7 +689,7 @@ __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int 
         const uint64_t db = make_smem_desc(smem_u32(sm.b + ring.stage * kBB));
 #pragma unroll
         for (int k = 0; k < kBlockK / 16; ++k)
-          Wgmma<BN, 0, 0>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
+          Wgmma<BN, 0, 0, F16>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
         wgmma_commit();
         wgmma_fence_operand(acc);
         wgmma_wait<1>();
@@ -698,7 +702,7 @@ __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int 
     wgmma_fence_operand(acc);
     release();
     tl_rec<TL>(p, tl_n, 2, 1, tile, 0);
-    // ---- epilogue: per 64-column slab, registers -> (raw | folded BN + SiLU + residual) -> bf16 -> staging tile
+    // ---- epilogue: per 64-column slab, registers -> (raw | folded BN + SiLU + residual) -> bf16 | fp16 -> staging tile
 #pragma unroll
     for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
       tl_rec<TL>(p, tl_n, 2, 2, tile, slab);
@@ -708,14 +712,16 @@ __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int 
       const uint32_t tb = stage_base + (uint32_t)(sbuf * kSlabBytes) + (uint32_t)cq * 2u + (uint32_t)r0 * 128u;
       const uint32_t sw = ((uint32_t)r0 & 7u) << 4;
       if (p.mode == SY_CONV_RAW && p.dbg_f32 == nullptr) {
-        // raw values (every conv of a training step): round, pack and stage -- no per-value pixel or column arithmetic
+        // raw values (every conv of a training step): round, pack and stage -- no per-value pixel or column arithmetic.
+        // (The host never runs the fp16 kernel in RAW mode; compiling the branch out of it made ptxas spill 32 bytes in
+        // the BN = 128 halo instantiation.)
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int J = slab * 8 + j;
 #pragma unroll
           for (int h = 0; h < 2; ++h)
             asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
-                         "r"(valid[h] ? pack_bf16(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]) : 0u) : "memory");
+                         "r"(valid[h] ? st_pack<F16>(acc[4 * J + 2 * h], acc[4 * J + 2 * h + 1]) : 0u) : "memory");
         }
       } else {
         long long pix[2];
@@ -740,12 +746,12 @@ __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int 
               if (p.act) { v0 = silu_f(v0); v1 = silu_f(v1); }
               if (p.res != nullptr && inb) {
                 const uint32_t rv = *reinterpret_cast<const uint32_t*>(p.res + pix[h] * p.res_pitch + n0 + cl);
-                v0 += bf16_lo(rv);
-                v1 += bf16_hi(rv);
+                v0 += st_lo<F16>(rv);
+                v1 += st_hi<F16>(rv);
               }
             }
             asm volatile("st.shared.b32 [%0], %1;" ::"r"(tb + (uint32_t)h * 1024u + ((((uint32_t)j) << 4) ^ sw)),
-                         "r"(valid[h] ? pack_bf16(v0, v1) : 0u) : "memory");
+                         "r"(valid[h] ? st_pack<F16>(v0, v1) : 0u) : "memory");
           }
         }
       }
@@ -899,10 +905,10 @@ __device__ __forceinline__ void bn_tail(const Params& p, const Smem& sm, int tid
 //   2 halo   : 16 x 8 patch tiles, ONE tiled load per channel block of the 18 x (8+2) input halo; the nine taps are nine
 //              shared-memory descriptors into that halo (every 8-pixel swizzle atom of a tap view is one halo row).
 //              3x3 stride-1 only.  Each input pixel crosses L2 -> SM once per tile instead of nine times.
-template <int BN, bool TL, int AM>
-__global__ void __launch_bounds__(kThreads, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmY, const Params p) {
+// The body of both kernels below: carves up shared memory, initialises the barriers, dispatches the warp roles.
+template <int BN, bool TL, int AM, bool F16>
+__device__ __forceinline__ void conv_tc_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmY,
+                                             const Params& p) {
   constexpr bool HALO = (AM == 2);
   const int S = p.stages;                                  // linear: A+B ring depth; halo: B ring depth
   // weight slabs per ring stage: one 64-deep K block; halo mode: kHaloTaps filter taps
@@ -963,11 +969,28 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     bn_tail<TL>(p, sm, threadIdx.x, tl);
   } else {
     reg_alloc<kRegsMma>();
-    int tl = mma_convert<BN, TL, AM>(p, sm, threadIdx.x);
+    int tl = mma_convert<BN, TL, AM, F16>(p, sm, threadIdx.x);
     bn_tail<TL>(p, sm, threadIdx.x, tl);
   }
   __syncthreads();
   if (threadIdx.x == 16 * 32) tl_rec<TL>(p, tl_k, 4, 3, 0, 0);
+}
+
+// bf16 activations, every mode (TL: debug timeline)
+template <int BN, bool TL, int AM>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+               const __grid_constant__ CUtensorMap tmY, const Params p) {
+  conv_tc_body<BN, TL, AM, false>(tmA, tmB, tmY, p);
+}
+
+// fp16 activations and weights, FUSED mode only (a kernel of its own: the bf16 kernel's name and instantiations stay as
+// they are)
+template <int BN, int AM>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_tc_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                   const __grid_constant__ CUtensorMap tmY, const Params p) {
+  conv_tc_body<BN, false, AM, true>(tmA, tmB, tmY, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -1036,13 +1059,16 @@ struct Plan {
   int smem, grid;
 };
 
-template <int BN, int AM>
+template <int BN, int AM, bool F16>
 static bool set_smem_attr() {
   static int state = 0;                 // 0 = not tried, 1 = ok, -1 = failed
   if (state == 0) {
-    const bool ok =
-        cudaFuncSetAttribute(conv_tc_kernel<BN, false, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess &&
-        cudaFuncSetAttribute(conv_tc_kernel<BN, true, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess;
+    bool ok;
+    if constexpr (F16)
+      ok = cudaFuncSetAttribute(conv_tc_f16_kernel<BN, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess;
+    else
+      ok = cudaFuncSetAttribute(conv_tc_kernel<BN, false, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess &&
+           cudaFuncSetAttribute(conv_tc_kernel<BN, true, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess;
     if (!ok) cudaGetLastError();
     state = ok ? 1 : -1;
   }
@@ -1085,10 +1111,10 @@ static int make_plan(Params& p, Plan* out) {
   return SY_OK;
 }
 
-template <int BN, int AM>
+template <int BN, int AM, bool F16>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, Params& p, const Plan& pl, cudaStream_t stream) {
   const int smem = pl.smem, grid = pl.grid;
-  SY_REQUIRE((set_smem_attr<BN, AM>()), SY_ELAUNCH, "conv2d_tc: cannot opt in to %d bytes of shared memory", kSmemLimit);
+  SY_REQUIRE((set_smem_attr<BN, AM, F16>()), SY_ELAUNCH, "conv2d_tc: cannot opt in to %d bytes of shared memory", kSmemLimit);
   if (p.n_seg > 0) {
     // The BatchNorm tail ends in a grid-wide barrier: every CTA of this launch must be resident at once.  The launch is
     // not a cooperative launch (it carries the programmatic-dependent-launch attribute instead), so check what a
@@ -1106,6 +1132,10 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
         if (ok_smem[i] == 0) { ok_smem[i] = smem; break; }
     }
   }
+  if constexpr (F16) {                  // (no statistics, no timeline: the host side refused them)
+    SY_CUDA(launch_pdl(conv_tc_f16_kernel<BN, AM>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
+    return launch_status("conv_tc_f16_kernel");
+  }
   if (p.timeline != nullptr)
     SY_CUDA(launch_pdl(conv_tc_kernel<BN, true, AM>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
   else
@@ -1118,10 +1148,10 @@ static int plan_bn(int bn, Params& p, Plan* out) {
   return bn == 64 ? make_plan<64, AM>(p, out) : make_plan<128, AM>(p, out);
 }
 
-template <int AM>
+template <int AM, bool F16>
 static int launch_bn(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& ty, Params& p, const Plan& pl,
                      cudaStream_t stream) {
-  return bn == 64 ? launch<64, AM>(ta, tb, ty, p, pl, stream) : launch<128, AM>(ta, tb, ty, p, pl, stream);
+  return bn == 64 ? launch<64, AM, F16>(ta, tb, ty, p, pl, stream) : launch<128, AM, F16>(ta, tb, ty, p, pl, stream);
 }
 
 // Halo mode (conv_tc_kernel, AM = 2) for a 3x3 stride-1 convolution?  It needs 16 x 8 patch tiles (more tiles than the
@@ -1184,6 +1214,12 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   SY_REQUIRE(d->debug_flags == 0 || d->debug_flags == 2, SY_EINVAL, "conv2d_tc: debug_flags %d unsupported", d->debug_flags);
   SY_REQUIRE(tc::tiling_override_ok(d->tile_mode, d->tile_bn), SY_EINVAL, "conv2d_tc: tile_mode %d / tile_bn %d unsupported",
              d->tile_mode, d->tile_bn);
+  SY_REQUIRE(d->storage == SY_STORAGE_BF16 || d->storage == SY_STORAGE_F16, SY_EINVAL, "conv2d_tc: storage %d unsupported",
+             d->storage);
+  const bool f16 = d->storage == SY_STORAGE_F16;
+  SY_REQUIRE(!f16 || (d->mode == SY_CONV_FUSED && d->stat_partials == nullptr && d->bn[0].gamma == nullptr &&
+                      d->debug_timeline == nullptr),
+             SY_EINVAL, "conv2d_tc: fp16 storage runs the FUSED mode only (no statistics, BatchNorm finalize or timeline)");
   {
     const bool one_group = !(d->split_n > 0 && d->split_n < x.n);
     SY_REQUIRE(d->stat_updates >= 0 && d->stat_updates <= 2, SY_EINVAL, "conv2d_tc: stat_updates %d unsupported (0, 1 or 2)",
@@ -1220,7 +1256,7 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   if (d->mode == SY_CONV_FUSED && d->res.ptr != nullptr) {
     SY_REQUIRE(view_ok(d->res) && d->res.n == y.n && d->res.h == ho && d->res.w == wo && d->res.c == y.c, SY_EINVAL,
                "conv2d_tc: residual view mismatch");
-    p.res = reinterpret_cast<const __nv_bfloat16*>(d->res.ptr); p.res_pitch = d->res.pitch;
+    p.res = reinterpret_cast<const uint16_t*>(d->res.ptr); p.res_pitch = d->res.pitch;
   }
   p.scale = d->scale; p.shift = d->shift;
   p.split_n = (d->split_n > 0 && d->split_n < x.n) ? d->split_n : x.n;
@@ -1271,18 +1307,19 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
   if (d->rows_written) *d->rows_written = p.stat_rows;
 
   CUtensorMap ta, tb, ty;
+  const CUtensorMapDataType dt = f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   if (halo) {
     // A, halo mode: input view as (C, W, H, N), box (64 ch, 10 px, 18 rows, 1 image) at (x0 - 1, y0 - 1): out of bounds
     // = zero padding
     cuuint64_t dims[4], strides[3];
     tc::nhwc_dims(x, dims, strides);
     const cuuint32_t box[4] = {(cuuint32_t)tc::kBlockK, (cuuint32_t)tc::kHaloPitch, (cuuint32_t)(tc::kHaloTH + 2), 1};
-    const CUresult r = tc::encode_tiled_bf16(&ta, 4, x.ptr, dims, strides, box);
+    const CUresult r = tc::encode_tiled(&ta, 4, x.ptr, dims, strides, box, dt);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(A halo) failed: %d", (int)r);
   } else {
     // A, im2col mode: one load = 128 consecutive base pixels x 64 channels, shifted by the tap offset
     SY_REQUIRE(tc::get_encode_im2col() != nullptr, SY_EARCH, "cuTensorMapEncodeIm2col not available from the driver");
-    const CUresult r = tc::encode_im2col_nhwc(&ta, x, d->kh, d->kw, d->stride, tc::kBlockM);
+    const CUresult r = tc::encode_im2col_nhwc(&ta, x, d->kh, d->kw, d->stride, tc::kBlockM, dt);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeIm2col(A) failed: %d (c=%d w=%d h=%d n=%d pitch=%lld k=%dx%d s=%d)",
                (int)r, x.c, x.w, x.h, x.n, (long long)x.pitch, d->kh, d->kw, d->stride);
   }
@@ -1291,7 +1328,7 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     const cuuint64_t dims[3] = {(cuuint64_t)x.c, (cuuint64_t)taps, (cuuint64_t)y.c};
     const cuuint64_t strides[2] = {(cuuint64_t)x.c * 2, (cuuint64_t)x.c * 2 * taps};
     const cuuint32_t box[3] = {(cuuint32_t)tc::kBlockK, 1, (cuuint32_t)bn};
-    const CUresult r = tc::encode_tiled_bf16(&tb, 3, d->w, dims, strides, box);
+    const CUresult r = tc::encode_tiled(&tb, 3, d->w, dims, strides, box, dt);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(B) failed: %d", (int)r);
   }
   if (!halo) {
@@ -1299,17 +1336,18 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
     const cuuint64_t dims[4] = {(cuuint64_t)y.c, (cuuint64_t)p.P_total, 1, 1};
     const cuuint64_t strides[3] = {(cuuint64_t)y.pitch * 2, (cuuint64_t)y.pitch * 2 * p.P_total, (cuuint64_t)y.pitch * 2 * p.P_total};
     const cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)tc::kBlockM, 1, 1};
-    const CUresult r = tc::encode_tiled_bf16(&ty, 4, y.ptr, dims, strides, box);
+    const CUresult r = tc::encode_tiled(&ty, 4, y.ptr, dims, strides, box, dt);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(Y linear) failed: %d", (int)r);
   } else {
     // Y: output view as (C, W, H, N), box (64, 8, 16, 1): the TMA store clips the patch to the image / slice
     cuuint64_t dims[4], strides[3];
     tc::nhwc_dims(y, dims, strides);
     const cuuint32_t box[4] = {(cuuint32_t)tc::kSlabCols, (cuuint32_t)tc::kHaloTW, (cuuint32_t)tc::kHaloTH, 1};
-    const CUresult r = tc::encode_tiled_bf16(&ty, 4, y.ptr, dims, strides, box);
+    const CUresult r = tc::encode_tiled(&ty, 4, y.ptr, dims, strides, box, dt);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(Y) failed: %d", (int)r);
   }
-  return halo ? tc::launch_bn<2>(bn, ta, tb, ty, p, pl, stream) : tc::launch_bn<1>(bn, ta, tb, ty, p, pl, stream);
+  if (f16) return halo ? tc::launch_bn<2, true>(bn, ta, tb, ty, p, pl, stream) : tc::launch_bn<1, true>(bn, ta, tb, ty, p, pl, stream);
+  return halo ? tc::launch_bn<2, false>(bn, ta, tb, ty, p, pl, stream) : tc::launch_bn<1, false>(bn, ta, tb, ty, p, pl, stream);
 }
 
 // Host-only query (no launch, works without a GPU): the tiling decisions sy_conv2d_tc takes for a layer shape and

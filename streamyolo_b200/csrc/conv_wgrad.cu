@@ -296,7 +296,7 @@ extern "C" int sy_conv2d_wgrad_tc(const SyConvWgradDesc* d, sy_stream_t stream_)
     const cuuint64_t dims[2] = {(cuuint64_t)dy.c, (cuuint64_t)p.P_total};
     const cuuint64_t strides[1] = {(cuuint64_t)dy.pitch * 2};
     const cuuint32_t box[2] = {64, (cuuint32_t)wg::kPixK};
-    const CUresult r = tc::encode_tiled_bf16(&tdy, 2, dy.ptr, dims, strides, box);
+    const CUresult r = tc::encode_tiled(&tdy, 2, dy.ptr, dims, strides, box);
     SY_REQUIRE(r == CUDA_SUCCESS, SY_ELAUNCH, "cuTensorMapEncodeTiled(dy) failed: %d", (int)r);
   }
   {

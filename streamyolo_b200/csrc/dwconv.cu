@@ -4,21 +4,24 @@
 // this is a coalesced, vectorised HBM kernel on the CUDA cores: NHWC bf16, one thread = one output pixel x 8 channels, every
 // tap one 16-byte load (neighbouring pixels / rows come from L1/L2), weights [taps][C] bf16, fp32 accumulation in tap
 // order.  Same RAW / FUSED epilogue contract as sy_conv2d_tc (RAW: bf16 conv result for the train-mode BatchNorm passes;
-// FUSED: act(acc * scale + shift) (+ residual) for eval with folded BatchNorm).
+// FUSED: act(acc * scale + shift) (+ residual) for eval with folded BatchNorm).  F16: activations, residual and weights in
+// fp16 (the eval / streaming forwards with fp16 storage; FUSED only).
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace sy {
 
-struct DwParams {
-  const __nv_bfloat16* x; long long x_pitch;
-  const __nv_bfloat16* w;                  // [taps][C]
-  __nv_bfloat16* y; long long y_pitch;
-  const __nv_bfloat16* res; long long res_pitch;
+struct DwParams {                          // 16-bit elements of the kernel's storage type (bf16 | fp16)
+  const uint16_t* x; long long x_pitch;
+  const uint16_t* w;                       // [taps][C]
+  uint16_t* y; long long y_pitch;
+  const uint16_t* res; long long res_pitch;
   const float* scale; const float* shift;
   int N, H, W, C, Ho, Wo, k, stride, pad, mode, act;
 };
 
-template <int K>
+template <int K, bool F16>
 __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
   const int G = p.C >> 3;
   const long long total = (long long)p.N * p.Ho * p.Wo * G;
@@ -38,10 +41,11 @@ __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
         if (ix < 0 || ix >= p.W) continue;
         const uint4 xv = *reinterpret_cast<const uint4*>(p.x + (((long long)n * p.H + iy) * p.W + ix) * p.x_pitch + g * 8);
         const uint4 wv = __ldg(reinterpret_cast<const uint4*>(p.w + (long long)(r * K + s) * p.C + g * 8));
-        acc[0] += bf16_lo(xv.x) * bf16_lo(wv.x); acc[1] += bf16_hi(xv.x) * bf16_hi(wv.x);
-        acc[2] += bf16_lo(xv.y) * bf16_lo(wv.y); acc[3] += bf16_hi(xv.y) * bf16_hi(wv.y);
-        acc[4] += bf16_lo(xv.z) * bf16_lo(wv.z); acc[5] += bf16_hi(xv.z) * bf16_hi(wv.z);
-        acc[6] += bf16_lo(xv.w) * bf16_lo(wv.w); acc[7] += bf16_hi(xv.w) * bf16_hi(wv.w);
+        float xf[8], wf[8];
+        st_unpack8<F16>(xv, xf);
+        st_unpack8<F16>(wv, wf);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] += xf[i] * wf[i];
       }
     }
     if (p.mode == SY_CONV_FUSED) {
@@ -53,12 +57,15 @@ __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
       }
       if (p.res != nullptr) {
         const uint4 rv = *reinterpret_cast<const uint4*>(p.res + pix * p.res_pitch + g * 8);
-        acc[0] += bf16_lo(rv.x); acc[1] += bf16_hi(rv.x); acc[2] += bf16_lo(rv.y); acc[3] += bf16_hi(rv.y);
-        acc[4] += bf16_lo(rv.z); acc[5] += bf16_hi(rv.z); acc[6] += bf16_lo(rv.w); acc[7] += bf16_hi(rv.w);
+        float rf[8];
+        st_unpack8<F16>(rv, rf);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] += rf[i];
       }
     }
     *reinterpret_cast<uint4*>(p.y + pix * p.y_pitch + g * 8) =
-        make_uint4(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]), pack_bf16(acc[4], acc[5]), pack_bf16(acc[6], acc[7]));
+        make_uint4(st_pack<F16>(acc[0], acc[1]), st_pack<F16>(acc[2], acc[3]), st_pack<F16>(acc[4], acc[5]),
+                   st_pack<F16>(acc[6], acc[7]));
   }
 }
 
@@ -79,15 +86,17 @@ extern "C" int sy_dwconv2d(const SyConvDesc* d, sy_stream_t stream_) {
   SY_REQUIRE(y.n == x.n && y.h == ho && y.w == wo && y.c == x.c, SY_EINVAL, "dwconv2d: output view %dx%dx%dx%d, expected %dx%dx%dx%d",
              y.n, y.h, y.w, y.c, x.n, ho, wo, x.c);
   SY_REQUIRE(((uintptr_t)d->w % 16) == 0, SY_EINVAL, "dwconv2d: weights not 16B aligned");
+  SY_REQUIRE(d->storage == SY_STORAGE_BF16 || (d->storage == SY_STORAGE_F16 && d->mode == SY_CONV_FUSED), SY_EINVAL,
+             "dwconv2d: storage %d in mode %d unsupported (fp16: FUSED only)", d->storage, d->mode);
   DwParams p{};
-  p.x = reinterpret_cast<const __nv_bfloat16*>(x.ptr); p.x_pitch = x.pitch;
-  p.w = reinterpret_cast<const __nv_bfloat16*>(d->w);
-  p.y = reinterpret_cast<__nv_bfloat16*>(y.ptr); p.y_pitch = y.pitch;
+  p.x = reinterpret_cast<const uint16_t*>(x.ptr); p.x_pitch = x.pitch;
+  p.w = reinterpret_cast<const uint16_t*>(d->w);
+  p.y = reinterpret_cast<uint16_t*>(y.ptr); p.y_pitch = y.pitch;
   p.res = nullptr;
   if (d->mode == SY_CONV_FUSED && d->res.ptr != nullptr) {
     SY_REQUIRE(view_ok(d->res) && d->res.n == y.n && d->res.h == ho && d->res.w == wo && d->res.c == y.c, SY_EINVAL,
                "dwconv2d: residual view mismatch");
-    p.res = reinterpret_cast<const __nv_bfloat16*>(d->res.ptr); p.res_pitch = d->res.pitch;
+    p.res = reinterpret_cast<const uint16_t*>(d->res.ptr); p.res_pitch = d->res.pitch;
   }
   p.scale = d->scale; p.shift = d->shift;
   p.N = x.n; p.H = x.h; p.W = x.w; p.C = x.c; p.Ho = ho; p.Wo = wo; p.k = d->kh; p.stride = d->stride; p.pad = pad;
@@ -96,10 +105,15 @@ extern "C" int sy_dwconv2d(const SyConvDesc* d, sy_stream_t stream_) {
   long long blocks = (total + 255) / 256;
   if (blocks > (long long)sm_count() * 32) blocks = (long long)sm_count() * 32;
   if (blocks < 1) blocks = 1;
-  switch (d->kh) {
-    case 1: dwconv_kernel<1><<<(int)blocks, 256, 0, stream>>>(p); break;
-    case 3: dwconv_kernel<3><<<(int)blocks, 256, 0, stream>>>(p); break;
-    default: dwconv_kernel<5><<<(int)blocks, 256, 0, stream>>>(p); break;
-  }
+  auto go = [&](auto f16) {
+    constexpr bool F16 = decltype(f16)::value;
+    switch (d->kh) {
+      case 1: dwconv_kernel<1, F16><<<(int)blocks, 256, 0, stream>>>(p); break;
+      case 3: dwconv_kernel<3, F16><<<(int)blocks, 256, 0, stream>>>(p); break;
+      default: dwconv_kernel<5, F16><<<(int)blocks, 256, 0, stream>>>(p); break;
+    }
+  };
+  if (d->storage == SY_STORAGE_F16) go(std::true_type{});
+  else go(std::false_type{});
   return launch_status("dwconv_kernel");
 }

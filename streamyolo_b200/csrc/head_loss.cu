@@ -20,8 +20,8 @@ constexpr int kMaxPred = 5 + 32;
 // PT pixels per thread (64 * PT pixels per block and pass): every weight chunk read from shared memory is used for PT
 // pixels.  With one pixel per thread the kernel was bound by its shared-memory weight reads (26 LDS.128 per 104 FMAs: 51 us
 // for the 73 MB of level-0 features = 1.4 TB/s); the per-pixel arithmetic (order of the products and sums) is unchanged, so
-// the results are bit-identical for every PT.
-template <int NO, int PT>
+// the results are bit-identical for every PT.  F16: the tower features are fp16 (SyHeadPredDesc.storage).
+template <int NO, int PT, bool F16>
 __global__ void __launch_bounds__(256)
 head_pred_kernel(const SyHeadPredDesc d, int B, int H, int W, int C) {
   extern __shared__ float wsm[];   // [NO][C] : reg(4), obj(1), cls(NO-5)
@@ -60,9 +60,7 @@ head_pred_kernel(const SyHeadPredDesc d, int B, int H, int W, int C) {
         float v[PT][8];
 #pragma unroll
         for (int j = 0; j < PT; ++j) {
-          const uint4 u = part == 0 ? rv[j] : cv[j];
-          v[j][0] = bf16_lo(u.x); v[j][1] = bf16_hi(u.x); v[j][2] = bf16_lo(u.y); v[j][3] = bf16_hi(u.y);
-          v[j][4] = bf16_lo(u.z); v[j][5] = bf16_hi(u.z); v[j][6] = bf16_lo(u.w); v[j][7] = bf16_hi(u.w);
+          st_unpack8<F16>(part == 0 ? rv[j] : cv[j], v[j]);
         }
 #pragma unroll
         for (int o = (part == 0 ? 0 : 5); o < (part == 0 ? 5 : NO); ++o) {
@@ -121,6 +119,7 @@ head_pred_kernel(const SyHeadPredDesc d, int B, int H, int W, int C) {
 
 // Any class count (the reference head takes `num_classes` freely, tal_head.py:27): the outputs are walked in groups of eight
 // compile-time accumulators, re-reading the pixel's features (L1 / L2) for every group.  Same per-output arithmetic as above.
+template <bool F16>
 __global__ void __launch_bounds__(256)
 head_pred_generic_kernel(const SyHeadPredDesc d, int B, int H, int W, int C, int NO) {
   extern __shared__ float wsm[];   // [NO][C]
@@ -148,10 +147,9 @@ head_pred_generic_kernel(const SyHeadPredDesc d, int B, int H, int W, int C, int
         for (int ch = ks; ch < chunks; ch += 4) {
           const uint4 rv = *reinterpret_cast<const uint4*>(rf + pix * d.reg_feat.pitch + ch * 8);
           const uint4 cv = *reinterpret_cast<const uint4*>(cf + pix * d.cls_feat.pitch + ch * 8);
-          const float r[8] = {bf16_lo(rv.x), bf16_hi(rv.x), bf16_lo(rv.y), bf16_hi(rv.y),
-                              bf16_lo(rv.z), bf16_hi(rv.z), bf16_lo(rv.w), bf16_hi(rv.w)};
-          const float c[8] = {bf16_lo(cv.x), bf16_hi(cv.x), bf16_lo(cv.y), bf16_hi(cv.y),
-                              bf16_lo(cv.z), bf16_hi(cv.z), bf16_lo(cv.w), bf16_hi(cv.w)};
+          float r[8], c[8];
+          st_unpack8<F16>(rv, r);
+          st_unpack8<F16>(cv, c);
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
             const int o = o0 + i;
@@ -199,34 +197,46 @@ static int head_pixels_per_thread(long long npix) {
   return npix >= 32768 ? 2 : 1;                          // small levels: more blocks matter more than the weight reuse
 }
 
-template <int NO, int PT>
+template <int NO, int PT, bool F16>
 static int launch_head_pred_pt(const SyHeadPredDesc* d, const SyTensor& f, cudaStream_t stream) {
   const size_t smem = sizeof(float) * NO * f.c;
   if (smem > 48 * 1024)
-    SY_CUDA(cudaFuncSetAttribute(head_pred_kernel<NO, PT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SY_CUDA(cudaFuncSetAttribute(head_pred_kernel<NO, PT, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const long long npix = (long long)f.n * f.h * f.w;
   int blocks = (int)((npix + 64 * PT - 1) / (64 * PT));
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  head_pred_kernel<NO, PT><<<blocks, 256, smem, stream>>>(*d, f.n, f.h, f.w, f.c);
+  head_pred_kernel<NO, PT, F16><<<blocks, 256, smem, stream>>>(*d, f.n, f.h, f.w, f.c);
   return launch_status("head_pred_kernel");
 }
 
-template <int NO>
+template <int NO, bool F16>
 static int launch_head_pred(const SyHeadPredDesc* d, const SyTensor& f, cudaStream_t stream) {
-  if (head_pixels_per_thread((long long)f.n * f.h * f.w) == 2) return launch_head_pred_pt<NO, 2>(d, f, stream);
-  return launch_head_pred_pt<NO, 1>(d, f, stream);
+  if (head_pixels_per_thread((long long)f.n * f.h * f.w) == 2) return launch_head_pred_pt<NO, 2, F16>(d, f, stream);
+  return launch_head_pred_pt<NO, 1, F16>(d, f, stream);
 }
 
+template <bool F16>
 static int launch_head_pred_generic(const SyHeadPredDesc* d, const SyTensor& f, cudaStream_t stream) {
   const int NO = 5 + d->num_classes;
   const size_t smem = sizeof(float) * NO * f.c;
   if (smem > 48 * 1024)
-    SY_CUDA(cudaFuncSetAttribute(head_pred_generic_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    SY_CUDA(cudaFuncSetAttribute(head_pred_generic_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const long long npix = (long long)f.n * f.h * f.w;
   int blocks = (int)((npix + 63) / 64);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  head_pred_generic_kernel<<<blocks, 256, smem, stream>>>(*d, f.n, f.h, f.w, f.c, NO);
+  head_pred_generic_kernel<F16><<<blocks, 256, smem, stream>>>(*d, f.n, f.h, f.w, f.c, NO);
   return launch_status("head_pred_generic_kernel");
+}
+
+template <bool F16>
+static int launch_head_pred_classes(const SyHeadPredDesc* d, const SyTensor& f, cudaStream_t stream) {
+  switch (d->num_classes) {           // compile-time output counts for the class counts in use (Argoverse-HD: 8); any other: generic
+    case 8: return launch_head_pred<13, F16>(d, f, stream);
+    case 1: return launch_head_pred<6, F16>(d, f, stream);
+    case 20: return launch_head_pred<25, F16>(d, f, stream);
+    default: break;
+  }
+  return launch_head_pred_generic<F16>(d, f, stream);
 }
 
 // ======================================================================= loss
@@ -740,13 +750,9 @@ extern "C" int sy_head_pred_decode(const SyHeadPredDesc* d, sy_stream_t stream_)
   SY_REQUIRE(d->anchor_offset >= 0 && d->anchor_offset + f.h * f.w <= d->a_total, SY_EINVAL, "head_pred: anchor range");
   SY_REQUIRE((f.c % 8) == 0 && sizeof(float) * (5 + d->num_classes) * f.c <= 200 * 1024, SY_EINVAL,
              "head_pred: %d channels x %d outputs do not fit the shared-memory weight tile", f.c, 5 + d->num_classes);
-  switch (d->num_classes) {           // compile-time output counts for the class counts in use (Argoverse-HD: 8); any other: generic
-    case 8: return launch_head_pred<13>(d, f, stream);
-    case 1: return launch_head_pred<6>(d, f, stream);
-    case 20: return launch_head_pred<25>(d, f, stream);
-    default: break;
-  }
-  return launch_head_pred_generic(d, f, stream);
+  SY_REQUIRE(d->storage == SY_STORAGE_BF16 || d->storage == SY_STORAGE_F16, SY_EINVAL, "head_pred: storage %d unsupported",
+             d->storage);
+  return d->storage == SY_STORAGE_F16 ? launch_head_pred_classes<true>(d, f, stream) : launch_head_pred_classes<false>(d, f, stream);
 }
 
 extern "C" size_t sy_tal_loss_workspace_bytes(int32_t b, int32_t a_total, int32_t max_labels, int32_t num_classes) {

@@ -1,6 +1,7 @@
 // Kernels around the training step that are neither convolutions nor BatchNorm:
 //   * sy_pack_conv_weight      fp32 OIHW parameter -> bf16 GEMM operand of the tensor-core kernels (forward layout
-//                              [Cout][taps][Cin], data-gradient layout = flipped taps + transposed channels, Focus-stem layout):
+//                              [Cout][taps][Cin], data-gradient layout = flipped taps + transposed channels, Focus-stem layout;
+//                              the forward and stem layouts also in fp16 with SY_PACK_F16):
 //                              one launch per parameter per optimiser step instead of an ATen permute + cast chain
 //   * sy_sgd_nesterov_ema_step the optimiser step of the reference trainer as ONE launch over flat fp32 buffers:
 //                              GradScaler unscale + weight decay + SGD momentum (nesterov) + ModelEMA
@@ -10,6 +11,8 @@
 //                              F.interpolate(mode="bilinear", align_corners=False)) + sy_scale_labels for the box rescale
 #include <math.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace sy {
@@ -17,7 +20,14 @@ namespace sy {
 // mode 0: out[o][t][i]                      = w[o][i][r][s],               t = r * kw + s                (forward B operand)
 // mode 1: out[i][(kh-1-r)*kw + (kw-1-s)][o] = w[o][i][r][s]   (row pitch out_pitch, column offset co_off: data gradient)
 // mode 2: out[o][r][s * 16 + i]             = w[o][i][r][s], i < 12, 64 columns per (o, r), rest zero     (Focus stem)
-__global__ void pack_weight_kernel(const float* __restrict__ w, int O, int I, int kh, int kw, int mode, __nv_bfloat16* out,
+// T: the operand's element type (bf16, or __half for SY_PACK_F16)
+template <typename T>
+__device__ __forceinline__ T round_to(float v) {
+  if constexpr (std::is_same<T, __half>::value) return __float2half_rn(v); else return __float2bfloat16_rn(v);
+}
+
+template <typename T>
+__global__ void pack_weight_kernel(const float* __restrict__ w, int O, int I, int kh, int kw, int mode, T* out,
                                    long long out_pitch, int co_off) {
   const int taps = kh * kw;
   if (mode == 2) {
@@ -29,7 +39,7 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, int O, int I, in
       const int s = col >> 4, i = col & 15;
       float v = 0.f;
       if (s < kw && i < I) v = w[(((long long)o * I + i) * kh + r) * kw + s];
-      out[idx] = __float2bfloat16_rn(v);
+      out[idx] = round_to<T>(v);
     }
     return;
   }
@@ -39,13 +49,13 @@ __global__ void pack_weight_kernel(const float* __restrict__ w, int O, int I, in
       const int i = (int)(idx % I);
       const int t = (int)((idx / I) % taps);
       const int o = (int)(idx / ((long long)I * taps));
-      out[idx] = __float2bfloat16_rn(w[((long long)o * I + i) * taps + t]);
+      out[idx] = round_to<T>(w[((long long)o * I + i) * taps + t]);
     } else {                               // idx walks (i, t', o), o fastest
       const int o = (int)(idx % O);
       const int t2 = (int)((idx / O) % taps);
       const int i = (int)(idx / ((long long)O * taps));
       const int t = taps - 1 - t2;         // (kh-1-r)*kw + (kw-1-s) = taps - 1 - (r*kw + s)
-      out[((long long)i * taps + t2) * out_pitch + co_off + o] = __float2bfloat16_rn(w[((long long)o * I + i) * taps + t]);
+      out[((long long)i * taps + t2) * out_pitch + co_off + o] = round_to<T>(w[((long long)o * I + i) * taps + t]);
     }
   }
 }
@@ -224,12 +234,19 @@ extern "C" int sy_pack_conv_weight(const float* w, int32_t cout, int32_t cin, in
                                    int64_t out_pitch, int32_t co_offset, sy_stream_t stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   SY_REQUIRE(w != nullptr && out != nullptr && cout > 0 && cin > 0 && kh > 0 && kw > 0, SY_EINVAL, "pack_conv_weight: bad arguments");
-  SY_REQUIRE(mode >= 0 && mode <= 2, SY_EINVAL, "pack_conv_weight: mode %d", mode);
+  const bool f16 = (mode & SY_PACK_F16) != 0;
+  mode &= ~SY_PACK_F16;
+  SY_REQUIRE(mode >= 0 && mode <= 2 && !(f16 && mode == 1), SY_EINVAL, "pack_conv_weight: mode %d%s", mode,
+             f16 ? " | SY_PACK_F16 (fp16: forward and stem layouts only)" : "");
   if (mode == 1) SY_REQUIRE(out_pitch >= co_offset + cout, SY_EINVAL, "pack_conv_weight: pitch %lld < %d + %d", (long long)out_pitch, co_offset, cout);
   if (mode == 2) SY_REQUIRE(cin <= 16 && kw <= 4, SY_EINVAL, "pack_conv_weight(stem): cin %d kw %d", cin, kw);
   const long long total = mode == 2 ? (long long)cout * kh * 64 : (long long)cout * cin * kh * kw;
-  pack_weight_kernel<<<grid_for(total, 256), 256, 0, stream>>>(w, cout, cin, kh, kw, mode, reinterpret_cast<__nv_bfloat16*>(out),
-                                                              out_pitch, co_offset);
+  if (f16)
+    pack_weight_kernel<<<grid_for(total, 256), 256, 0, stream>>>(w, cout, cin, kh, kw, mode, reinterpret_cast<__half*>(out),
+                                                                out_pitch, co_offset);
+  else
+    pack_weight_kernel<<<grid_for(total, 256), 256, 0, stream>>>(w, cout, cin, kh, kw, mode,
+                                                                reinterpret_cast<__nv_bfloat16*>(out), out_pitch, co_offset);
   return launch_status("pack_weight_kernel");
 }
 

@@ -402,6 +402,7 @@ def _record(model, x, targets):
     assert model.training and model.head.use_l1
     if any(getattr(m, "groups", 1) > 1 for m in model.modules() if isinstance(m, torch.nn.Conv2d)):
         raise NotImplementedError("the training backward does not cover depthwise convolutions (depthwise=True): forward only")
+    engine.require_bf16_training(model)
     targets = label_pair(model, targets)
     net = model.backbone
     xin = x.float().contiguous()

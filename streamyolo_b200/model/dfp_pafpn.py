@@ -2,7 +2,8 @@
 
 Same constructor, sub-module names and forward(input, buffer, mode) contract; outputs are
 NCHW-shaped bf16 tensors (channels-last memory, i.e. zero-copy views of the NHWC buffers the
-kernels write)."""
+kernels write).  ``activation_dtype = torch.float16`` (eval only): every activation, the outputs and the on_pipe
+buffers are fp16 instead."""
 import torch
 from torch import nn
 
@@ -34,12 +35,13 @@ class DFPPAFPN(nn.Module):
         self.jian2 = Conv(c3, c3 // 2, 1, 1, act=act)
         self.jian1 = Conv(c4, c4 // 2, 1, 1, act=act)
         self.jian0 = Conv(c5, c5 // 2, 1, 1, act=act)
+        self.activation_dtype = torch.bfloat16      # activation storage: bf16, or fp16 in eval mode (engine.Ctx)
 
     # ---- reference: off_forward (:109-175)
     def off_forward(self, input):
         x = input.float().contiguous()
         b = x.shape[0]
-        ctx = engine.Ctx(self.training, 2 * b, b, x.device)
+        ctx = engine.Ctx(self.training, 2 * b, b, x.device, dtype=self.activation_dtype)
         with torch.no_grad(), engine.forward_scope(x.device):
             pans = engine.pafpn_frames(ctx, self, x, 2)
             cur = tuple(p.imgs(0, b) for p in pans)
@@ -51,10 +53,15 @@ class DFPPAFPN(nn.Module):
     def online_forward(self, input, buffer=None, node="star"):
         x = input.float().contiguous()
         b = x.shape[0]
-        ctx = engine.Ctx(self.training, b, b, x.device)
+        ctx = engine.Ctx(self.training, b, b, x.device, dtype=self.activation_dtype)
         with torch.no_grad(), engine.forward_scope(x.device):
             cur = engine.pafpn_frames(ctx, self, x, 1)
-            sup = cur if node == "star" else tuple(engine.as_view(t) for t in buffer)
+            if node == "star":
+                sup = cur
+            elif ctx.f16:
+                sup = tuple(engine.as_view(t, torch.float16) for t in buffer)
+            else:
+                sup = tuple(engine.as_view(t) for t in buffer)
             fused = engine.dfp_fuse(ctx, self, cur, sup)
         return tuple(engine.as_nchw(v) for v in fused), tuple(engine.as_nchw(v) for v in cur)
 

@@ -13,6 +13,12 @@ together with SiLU and the residual (what yolox ``fuse_model`` + ``fuseforward``
 
 The recording forward of a training step (model/backward.py) is this same walk with a tape in the ``Ctx``: nothing is
 updated in place, every op keeps what its backward needs and is recorded on the tape.
+
+Activation storage: bf16 everywhere by default.  An eval-mode ``Ctx`` may store every activation and pack every conv
+operand in fp16 instead (``dtype=torch.float16``, what ``model.activation_dtype = torch.float16`` selects): 11 significant
+bits instead of 8, the precision of the reference's half-precision inference.  The fp16 operands live in their own cache
+slots ("_pkh", "_pk2h") next to the bf16 ones, so switching back and forth re-packs nothing and leaves the bf16 operands
+(and train.Trainer's re-packed ones) alone.
 """
 import torch
 
@@ -36,13 +42,29 @@ def _trace(m, y):
         TRACE[getattr(m, "_sy_name", str(id(m)))] = y.torch().permute(0, 3, 1, 2).float().cpu()
 
 
+ACTIVATION_DTYPES = (torch.bfloat16, torch.float16)
+
+
+def check_activation_dtype(dtype):
+    if dtype not in ACTIVATION_DTYPES:
+        raise ValueError(f"activation_dtype must be torch.bfloat16 or torch.float16, not {dtype}")
+    return dtype
+
+
+def require_bf16_training(model):
+    """training stores bf16 activations: refuse a model (or any of its modules) switched to fp16 storage"""
+    if any(getattr(m, "activation_dtype", torch.bfloat16) != torch.bfloat16 for m in model.modules()):
+        raise NotImplementedError("fp16 activation storage runs the eval / streaming forwards only (training stores bf16)")
+
+
 class Ctx:
     """Per-forward execution context.  ``tape`` (a ``backward.Tape``): the recording forward of a training step -- every op
     keeps what its backward needs and is recorded on the tape; None: the plain forward.  ``stat_updates=2``: every train-mode
     conv of this context applies its (single-group) batch statistics to the running statistics twice -- one pass over a
-    batch standing for the reference's two identical passes over it (a still frame duplicated into a pair)."""
+    batch standing for the reference's two identical passes over it (a still frame duplicated into a pair).  ``dtype``: the
+    activation storage, bf16 or (eval, tensor-core conv only) fp16."""
 
-    def __init__(self, train, n, split, device, tape=None, stat_updates=1):
+    def __init__(self, train, n, split, device, tape=None, stat_updates=1, dtype=torch.bfloat16):
         self.train = train
         self.n = n              # images in the batched tensor
         self.split = split      # first image of statistics group 1 (== n: single group)
@@ -51,10 +73,32 @@ class Ctx:
         self.tape = tape
         self.stat_updates = stat_updates
         self.impl = "tc" if tape is not None else CONV_IMPL
+        self.dtype = check_activation_dtype(dtype)
+        self.f16 = dtype == torch.float16
+        if self.f16 and (train or tape is not None):
+            raise NotImplementedError("fp16 activation storage runs the eval / streaming forwards only (training stores bf16)")
+        if self.f16 and self.impl != "tc":
+            raise NotImplementedError(f"fp16 activation storage runs on the tensor-core conv only, not CONV_IMPL={self.impl!r}")
 
     def rec(self, **kw):
         if self.tape is not None:
             self.tape.rec(**kw)
+
+    def empty(self, n, h, w, c) -> View:
+        """a fresh activation buffer in the storage dtype (the dtype is passed only where it is not the default)"""
+        if self.f16:
+            return View.empty(n, h, w, c, self.device, torch.float16)
+        return View.empty(n, h, w, c, self.device)
+
+    def slot(self, name):
+        """the packed-operand cache slot of this storage: fp16 operands are kept next to the bf16 ones, not over them"""
+        return name + "h" if self.f16 else name
+
+    def pack(self, fn):
+        """the packing function ``fn`` (ops.pack_*) producing operands in the storage dtype"""
+        if self.f16:
+            return lambda *ws: fn(*ws, dtype=torch.float16)
+        return fn
 
 
 def packed_operand(m, slot, ws, pack, value=None):
@@ -229,9 +273,9 @@ def base_conv(ctx: Ctx, m, x: View, y: View = None, res: View = None) -> View:
     ho, wo = ops.conv_out_hw(x.h, x.w, k, s)
     cout = m.conv.out_channels
     if y is None:
-        y = View.empty(x.n, ho, wo, cout, ctx.device)
+        y = ctx.empty(x.n, ho, wo, cout)
     dw = m.conv.groups > 1
-    wpk = packed_operand(m, "_pk", [m.conv.weight], ops.pack_dw_weight if dw else ops.pack_conv_weight)
+    wpk = packed_operand(m, ctx.slot("_pk"), [m.conv.weight], ctx.pack(ops.pack_dw_weight if dw else ops.pack_conv_weight))
     impl = "dw" if dw else ctx.impl
     act = 1 if m.act_name == "silu" else 0
     if not ctx.train:
@@ -257,7 +301,7 @@ def conv_pair(ctx: Ctx, m1, m2, x: View) -> View:
     parameter segment per module (CSPLayer conv1 | conv2; the first cls / reg tower convs of a head level)."""
     if hasattr(m1, "dconv") or hasattr(m2, "dconv"):          # depthwise variants: two ordinary launches into one buffer
         c1, c2 = m1.pconv.conv.out_channels, m2.pconv.conv.out_channels
-        u = View.empty(x.n, x.h, x.w, c1 + c2, ctx.device)
+        u = ctx.empty(x.n, x.h, x.w, c1 + c2)
         base_conv(ctx, m1, x, u.ch(0, c1))
         base_conv(ctx, m2, x, u.ch(c1, c2))
         return u
@@ -265,8 +309,8 @@ def conv_pair(ctx: Ctx, m1, m2, x: View) -> View:
     k, s = m1.ksize, m1.stride
     assert (m2.ksize, m2.stride, m2.conv.in_channels) == (k, s, m1.conv.in_channels)
     ho, wo = ops.conv_out_hw(x.h, x.w, k, s)
-    u = View.empty(x.n, ho, wo, c1 + c2, ctx.device)
-    wpk = packed_operand(m1, "_pk2", [m1.conv.weight, m2.conv.weight], ops.pack_conv_weight)
+    u = ctx.empty(x.n, ho, wo, c1 + c2)
+    wpk = packed_operand(m1, ctx.slot("_pk2"), [m1.conv.weight, m2.conv.weight], ctx.pack(ops.pack_conv_weight))
     if not ctx.train:
         scale, shift = _folded_pair(m1, m2)
         ops.conv2d(x, wpk, u, k, s, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=1)
@@ -316,10 +360,10 @@ def focus_stem(ctx: Ctx, m, x, frames) -> View:
     bc = m.conv
     cout = bc.conv.out_channels
     n = frames * b
-    xin = View.empty(n, h // 2, w // 2, 64, ctx.device)
+    xin = ctx.empty(n, h // 2, w // 2, 64)
     ops.focus_pack(x, frames, xin)
-    wpk = packed_operand(bc, "_pk", [bc.conv.weight], ops.pack_stem_weight)
-    y = View.empty(n, h // 2, w // 2, cout, ctx.device)
+    wpk = packed_operand(bc, ctx.slot("_pk"), [bc.conv.weight], ctx.pack(ops.pack_stem_weight))
+    y = ctx.empty(n, h // 2, w // 2, cout)
     if not ctx.train:
         scale, shift = _folded(bc)
         ops.conv2d(xin, wpk, y, ops.STEM_K, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=1)
@@ -331,7 +375,7 @@ def focus_stem(ctx: Ctx, m, x, frames) -> View:
 
 def spp_bottleneck(ctx: Ctx, m, x: View) -> View:
     hid = m.conv1.conv.out_channels
-    s = View.empty(x.n, x.h, x.w, 4 * hid, ctx.device)
+    s = ctx.empty(x.n, x.h, x.w, 4 * hid)
     base_conv(ctx, m.conv1, x, s.ch(0, hid))
     ops.spp_maxpool(s.ch(0, hid), s.ch(hid, hid), s.ch(2 * hid, hid), s.ch(3 * hid, hid))
     ctx.rec(t="spp", x=s.ch(0, hid), y5=s.ch(hid, hid), y9=s.ch(2 * hid, hid), y13=s.ch(3 * hid, hid))
@@ -359,7 +403,6 @@ def darknet(ctx: Ctx, bb, x, frames, dark3: View = None, dark4: View = None):
 def pafpn_frames(ctx: Ctx, net, x, frames):
     """CSPDarknet + PAFPN for ``frames`` x B images (/root/reference/exps/model/darknet.py:167-179,
     dfp_pafpn.py:120-140).  Returns the un-fused (pan_out2, pan_out1, pan_out0) views."""
-    dev = ctx.device
     c3 = net.C3_p3.conv3.conv.out_channels
     c4 = net.C3_p4.conv3.conv.out_channels
     n = frames * x.shape[0]
@@ -367,15 +410,15 @@ def pafpn_frames(ctx: Ctx, net, x, frames):
     for _ in range(2):
         h8, w8 = ops.conv_out_hw(h8, w8, 3, 2)
     h16, w16 = ops.conv_out_hw(h8, w8, 3, 2)
-    f1 = View.empty(n, h8, w8, 2 * c3, dev)              # cat(up(fpn_out1), dark3)
-    f0 = View.empty(n, h16, w16, 2 * c4, dev)            # cat(up(fpn_out0), dark4)
+    f1 = ctx.empty(n, h8, w8, 2 * c3)                    # cat(up(fpn_out1), dark3)
+    f0 = ctx.empty(n, h16, w16, 2 * c4)                  # cat(up(fpn_out0), dark4)
     x0 = darknet(ctx, net.backbone, x, frames, f1.ch(c3, c3), f0.ch(c4, c4))[-1]
     h32, w32 = x0.h, x0.w
-    z0 = View.empty(n, h32, w32, 2 * c4, dev)            # cat(bu_conv1, fpn_out0)
+    z0 = ctx.empty(n, h32, w32, 2 * c4)                  # cat(bu_conv1, fpn_out0)
     fpn0 = base_conv(ctx, net.lateral_conv0, x0, z0.ch(c4, c4))
     upsample(ctx, fpn0, f0.ch(0, c4))
     fo0 = csp_layer(ctx, net.C3_p4, f0)
-    z1 = View.empty(n, h16, w16, 2 * c3, dev)            # cat(bu_conv2, fpn_out1)
+    z1 = ctx.empty(n, h16, w16, 2 * c3)                  # cat(bu_conv2, fpn_out1)
     fpn1 = base_conv(ctx, net.reduce_conv1, fo0, z1.ch(c3, c3))
     upsample(ctx, fpn1, f1.ch(0, c3))
     pan2 = csp_layer(ctx, net.C3_p3, f1)
@@ -395,15 +438,15 @@ def dfp_fuse(ctx: Ctx, net, cur, sup):
         nb = c.n
         if hasattr(m, "dconv"):                               # depthwise=True: jian is a DWConv (dfp_pafpn.py:83-105)
             half = m.pconv.conv.out_channels
-            out = View.empty(nb, c.h, c.w, 2 * half, ctx.device)
-            sub = Ctx(ctx.train, nb, nb, ctx.device, ctx.tape)    # two calls = two BatchNorm batches, like the reference
+            out = ctx.empty(nb, c.h, c.w, 2 * half)
+            sub = Ctx(ctx.train, nb, nb, ctx.device, ctx.tape, dtype=ctx.dtype)   # two calls = two BatchNorm batches, like the reference
             base_conv(sub, m, c, out.ch(0, half), res=c.ch(0, half))
             base_conv(sub, m, s, out.ch(half, half), res=c.ch(half, half))
             outs.append(out)
             continue
         half = m.conv.out_channels
-        out = View.empty(nb, c.h, c.w, 2 * half, ctx.device)
-        wpk = packed_operand(m, "_pk", [m.conv.weight], ops.pack_conv_weight)
+        out = ctx.empty(nb, c.h, c.w, 2 * half)
+        wpk = packed_operand(m, ctx.slot("_pk"), [m.conv.weight], ctx.pack(ops.pack_conv_weight))
         if not ctx.train:
             scale, shift = _folded(m)
             ops.conv2d(c, wpk, out.ch(0, half), 1, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift,
@@ -431,14 +474,14 @@ def dfp_fuse(ctx: Ctx, net, cur, sup):
     return tuple(outs)
 
 
-def as_view(t) -> View:
-    """Accept a View or an NCHW-shaped torch tensor (zero-copy when it is channels-last bf16)."""
+def as_view(t, dtype=torch.bfloat16) -> View:
+    """Accept a View or an NCHW-shaped torch tensor (zero-copy when it is channels-last ``dtype``, bf16 or fp16)."""
     if isinstance(t, View):
         return t
     p = t.permute(0, 2, 3, 1)
-    if t.dtype == torch.bfloat16 and p.is_contiguous():
+    if t.dtype == dtype and p.is_contiguous():
         return View(p)
-    return View(p.contiguous().to(torch.bfloat16))
+    return View(p.contiguous().to(dtype))
 
 
 def as_nchw(v: View):

@@ -43,6 +43,7 @@ class TALHead(nn.Module):
         self.hw = None
         self.last_assignment = None     # optional debug dumps (set ``keep_assignment = True``)
         self.keep_assignment = False
+        self.activation_dtype = torch.bfloat16      # storage of the tower activations: bf16, or fp16 in eval mode (engine.Ctx)
 
     def initialize_biases(self, prior_prob):
         v = -math.log((1 - prior_prob) / prior_prob)
@@ -53,10 +54,13 @@ class TALHead(nn.Module):
 
     # ------------------------------------------------------------------
     def forward(self, xin, labels=None, imgs=None):
-        views = [engine.as_view(x) for x in xin]
+        dt = engine.check_activation_dtype(self.activation_dtype)
+        if dt != torch.bfloat16 and self.training:
+            raise NotImplementedError("fp16 activation storage runs the eval / streaming forwards only (training stores bf16)")
+        views = [engine.as_view(x, dt) if dt != torch.bfloat16 else engine.as_view(x) for x in xin]
         dev = views[0].buf.device
         b = views[0].n
-        ctx = engine.Ctx(self.training, b, b, dev)
+        ctx = engine.Ctx(self.training, b, b, dev, dtype=dt)
         with torch.no_grad(), engine.forward_scope(dev):
             r = self.run(ctx, views, labels)
         return tuple(r) if self.training else r

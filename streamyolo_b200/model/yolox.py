@@ -15,6 +15,21 @@ class YOLOX(nn.Module):
         # trainer's scaler.scale(loss).backward() works unchanged; False = always the plain (no-gradient) forward
         self.train_with_autograd = True
 
+    @property
+    def activation_dtype(self):
+        """Storage of every activation and conv operand: torch.bfloat16 (default), or torch.float16 for the eval and
+        on_pipe forwards (11 significant bits instead of 8, like the reference's half-precision inference; head outputs stay
+        fp32, the on_pipe buffers are fp16).  Setting it sets the backbone's and the head's.  Training runs bf16 only:
+        a train-mode forward with fp16 raises NotImplementedError.  ``model.half()`` does not change it."""
+        return getattr(self.backbone, "activation_dtype", torch.bfloat16)
+
+    @activation_dtype.setter
+    def activation_dtype(self, dtype):
+        from . import engine
+        engine.check_activation_dtype(dtype)
+        self.backbone.activation_dtype = dtype
+        self.head.activation_dtype = dtype
+
     def forward(self, x, targets=None, buffer=None, mode="off_pipe"):
         from . import engine
         with engine.forward_scope(x.device):       # one grid-barrier counter pool rewind for backbone + head
@@ -22,6 +37,8 @@ class YOLOX(nn.Module):
 
     def _forward(self, x, targets=None, buffer=None, mode="off_pipe"):
         assert mode in ["off_pipe", "on_pipe"]
+        if self.training and self.activation_dtype != torch.bfloat16:
+            raise NotImplementedError("fp16 activation storage runs the eval / streaming forwards only (training stores bf16)")
         if mode == "off_pipe":
             if self.training and self.train_with_autograd and torch.is_grad_enabled():
                 # /root/reference/exps/train_utils/double_trainer.py:108-116: outputs = model(inps, targets); loss.backward()

@@ -12,6 +12,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "lib", "libstreamyolo_sm100.so")
 
 SY_CONV_RAW, SY_CONV_FUSED = 0, 1
+SY_STORAGE_BF16, SY_STORAGE_F16 = 0, 1
+SY_PACK_F16 = 0x100
+STORAGE = {torch.bfloat16: SY_STORAGE_BF16, torch.float16: SY_STORAGE_F16}    # activation dtype -> SyConvDesc.storage
 
 
 class SyTensor(C.Structure):
@@ -32,7 +35,7 @@ class SyConvDesc(C.Structure):
                 ("momentum", C.c_float), ("eps", C.c_float), ("scale_shift", C.c_void_p), ("mean_invstd", C.c_void_p),
                 ("sync", C.c_void_p), ("debug_timeline", C.c_void_p),
                 ("debug_timeline_events", C.c_int32), ("debug_flags", C.c_int32), ("debug_f32", C.c_void_p),
-                ("tile_mode", C.c_int32), ("tile_bn", C.c_int32), ("stat_updates", C.c_int32)]
+                ("tile_mode", C.c_int32), ("tile_bn", C.c_int32), ("stat_updates", C.c_int32), ("storage", C.c_int32)]
 
 
 class SyHeadPredDesc(C.Structure):
@@ -41,7 +44,7 @@ class SyHeadPredDesc(C.Structure):
                 ("w_cls", C.c_void_p), ("b_cls", C.c_void_p),
                 ("num_classes", C.c_int32), ("stride", C.c_int32), ("anchor_offset", C.c_int32),
                 ("a_total", C.c_int32), ("sigmoid", C.c_int32), ("decode", C.c_int32),
-                ("out", C.c_void_p), ("origin", C.c_void_p)]
+                ("out", C.c_void_p), ("origin", C.c_void_p), ("storage", C.c_int32)]
 
 
 class SyTalLossDesc(C.Structure):
@@ -142,6 +145,8 @@ _SIG = {
     "sy_dwconv2d": (C.c_int, [C.POINTER(SyConvDesc), C.c_void_p]),
     "sy_focus_pack": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, SyTensor,
                                 C.c_void_p]),
+    "sy_focus_pack_f16": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, SyTensor,
+                                    C.c_void_p]),
     "sy_stats_num_partials": (C.c_int, [C.c_int32, C.c_int32]),
     "sy_channel_stats": (C.c_int, [SyTensor, C.c_void_p, C.c_int32, C.c_void_p]),
     "sy_bn_finalize": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int64, C.c_int32, C.c_void_p,
@@ -151,6 +156,7 @@ _SIG = {
                                   C.c_int64, C.c_int64, C.c_void_p]),
     "sy_upsample_nearest": (C.c_int, [SyTensor, SyTensor, C.c_void_p]),
     "sy_spp_maxpool": (C.c_int, [SyTensor, SyTensor, SyTensor, SyTensor, C.c_void_p]),
+    "sy_spp_maxpool_f16": (C.c_int, [SyTensor, SyTensor, SyTensor, SyTensor, C.c_void_p]),
     "sy_copy": (C.c_int, [SyTensor, SyTensor, C.c_void_p]),
     "sy_head_pred_decode": (C.c_int, [C.POINTER(SyHeadPredDesc), C.c_void_p]),
     "sy_tal_loss_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
@@ -233,18 +239,23 @@ NULL_T = SyTensor(None, 0, 0, 0, 0, 0)
 
 
 class View:
-    """Channel-slice / image-slice view of an NHWC bf16 buffer ``buf[N,H,W,Ctot]``."""
+    """Channel-slice / image-slice view of an NHWC 16-bit buffer ``buf[N,H,W,Ctot]``: bf16, or fp16 for the eval /
+    streaming forwards with fp16 activation storage."""
     __slots__ = ("buf", "n0", "n", "c0", "c", "off")
 
     def __init__(self, buf, c0=0, c=None, n0=0, n=None):
-        assert buf.dtype == torch.bfloat16 and buf.dim() == 4 and buf.is_contiguous()
+        assert buf.dtype in STORAGE and buf.dim() == 4 and buf.is_contiguous()
         self.buf, self.c0, self.n0, self.off = buf, c0, n0, 0
         self.c = buf.shape[3] - c0 if c is None else c
         self.n = buf.shape[0] - n0 if n is None else n
 
     @staticmethod
-    def empty(n, h, w, c, device):
-        return View(torch.empty((n, h, w, c), dtype=torch.bfloat16, device=device))
+    def empty(n, h, w, c, device, dtype=torch.bfloat16):
+        return View(torch.empty((n, h, w, c), dtype=dtype, device=device))
+
+    @property
+    def dtype(self):
+        return self.buf.dtype
 
     @property
     def h(self):
@@ -295,17 +306,24 @@ def _w32(w):
     return w
 
 
-def pack_conv_weight(*ws):
-    """OIHW fp32 parameter(s) -> bf16 [sum O][kh*kw][I] contiguous (GEMM B operand, K-major), packed on the device
+def _pack_flag(dtype):
+    if dtype not in STORAGE:
+        raise ValueError(f"conv operands are bf16 or fp16, not {dtype}")
+    return SY_PACK_F16 if dtype == torch.float16 else 0
+
+
+def pack_conv_weight(*ws, dtype=torch.bfloat16):
+    """OIHW fp32 parameter(s) -> bf16 (or fp16) [sum O][kh*kw][I] contiguous (GEMM B operand, K-major), packed on the device
     (sy_pack_conv_weight).  Several weights with the same [I, kh, kw] (CSPLayer conv1 | conv2) land in one operand."""
     _, i, kh, kw = ws[0].shape
-    out = torch.empty((sum(w.shape[0] for w in ws), kh * kw, i), dtype=torch.bfloat16, device=ws[0].device)
+    flag = _pack_flag(dtype)
+    out = torch.empty((sum(w.shape[0] for w in ws), kh * kw, i), dtype=dtype, device=ws[0].device)
     o0 = 0
     for w in ws:
         w = _w32(w)
         assert tuple(w.shape[1:]) == (i, kh, kw)
-        _check(lib().sy_pack_conv_weight(w.data_ptr(), w.shape[0], i, kh, kw, 0, out.data_ptr() + 2 * o0 * kh * kw * i, 0, 0,
-                                         _stream()))
+        _check(lib().sy_pack_conv_weight(w.data_ptr(), w.shape[0], i, kh, kw, flag, out.data_ptr() + 2 * o0 * kh * kw * i, 0,
+                                         0, _stream()))
         o0 += w.shape[0]
     return out
 
@@ -325,7 +343,11 @@ def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None,
     """``k`` is an int (square) or (kh, kw).  With ``partials`` (RAW mode, tensor-core path) returns the number
     of per-CTA statistic rows the launch writes.  ``tile_mode`` / ``tile_bn`` override the tensor-core tiling
     (0 = planner; see conv2d_plan).  ``stat_updates=2``: the single statistics group updates the running statistics
-    twice (one pass standing for two identical ones; SyConvDesc.stat_updates)."""
+    twice (one pass standing for two identical ones; SyConvDesc.stat_updates).  The activation storage (bf16 | fp16) is
+    that of the views: x, y, res and the packed weights must all have it."""
+    dtypes = {x.dtype, y.dtype, wpk.dtype} | ({res.dtype} if res is not None else set())
+    if len(dtypes) != 1:
+        raise ValueError(f"conv2d: x, y, res and the packed weights must share one storage dtype, got {sorted(map(str, dtypes))}")
     d = SyConvDesc()
     d.x, d.y = x.st(), y.st()
     d.w = wpk.data_ptr()
@@ -353,6 +375,7 @@ def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None,
     d.debug_flags = debug_flags
     d.tile_mode, d.tile_bn = tile_mode, tile_bn
     d.stat_updates = stat_updates
+    d.storage = STORAGE[x.dtype]
     d.debug_f32 = debug_f32.data_ptr() if debug_f32 is not None else None
     if timeline is not None:
         d.debug_timeline, d.debug_timeline_events = timeline.data_ptr(), timeline.numel() // 2
@@ -362,27 +385,32 @@ def conv2d(x: View, wpk, y: View, k, s, mode, impl="tc", scale=None, shift=None,
 
 
 def focus_pack(x, frames, y: View):
+    """Focus space-to-depth of the float frames into ``y`` (bf16, or fp16 for an fp16-storage forward)."""
     assert x.dtype == torch.float32 and x.is_contiguous()
     b, ch, h, w = x.shape
-    _check(lib().sy_focus_pack(x.data_ptr(), b, ch, h, w, frames, y.st(), _stream()))
+    fn = lib().sy_focus_pack_f16 if y.dtype == torch.float16 else lib().sy_focus_pack
+    _check(fn(x.data_ptr(), b, ch, h, w, frames, y.st(), _stream()))
 
 
 STEM_K = (3, 1)      # the stem runs as a 3x1 conv over the W-gathered 64-channel focus tensor
 
 
-def pack_dw_weight(w):
-    """depthwise [C, 1, k, k] fp32 parameter -> bf16 [k*k][C] (sy_pack_conv_weight mode 0 on the [1, C, k, k] view)."""
+def pack_dw_weight(w, dtype=torch.bfloat16):
+    """depthwise [C, 1, k, k] fp32 parameter -> bf16 (or fp16) [k*k][C] (sy_pack_conv_weight mode 0 on the [1, C, k, k]
+    view)."""
     c, one, kh, kw = w.shape
     assert one == 1
-    return pack_conv_weight(_w32(w).view(1, c, kh, kw)).view(kh * kw, c)
+    return pack_conv_weight(_w32(w).view(1, c, kh, kw), dtype=dtype).view(kh * kw, c)
 
 
-def pack_stem_weight(w):
-    """[O,12,3,3] float -> bf16 [O][3 (row)][64 = 3 taps x (12 focus + 4 zero) + 16 zero] (sy_pack_conv_weight, mode 2)."""
+def pack_stem_weight(w, dtype=torch.bfloat16):
+    """[O,12,3,3] float -> bf16 (or fp16) [O][3 (row)][64 = 3 taps x (12 focus + 4 zero) + 16 zero] (sy_pack_conv_weight,
+    mode 2)."""
     w = _w32(w)
     o, i, kh, kw = w.shape
-    out = torch.empty((o, kh, 64), dtype=torch.bfloat16, device=w.device)
-    _check(lib().sy_pack_conv_weight(w.data_ptr(), o, i, kh, kw, 2, out.data_ptr(), 0, 0, _stream()))
+    flag = _pack_flag(dtype)
+    out = torch.empty((o, kh, 64), dtype=dtype, device=w.device)
+    _check(lib().sy_pack_conv_weight(w.data_ptr(), o, i, kh, kw, 2 | flag, out.data_ptr(), 0, 0, _stream()))
     return out
 
 
@@ -412,22 +440,35 @@ def bn_act_apply(x: View, scale_ptr, shift_ptr, split_n, act, res, y: View, y_go
                                  res.st() if res is not None else NULL_T, y.st(), y_goff1, res_goff1, _stream()))
 
 
+def _same_dtype(what, *views):
+    if len({v.dtype for v in views}) != 1:
+        raise ValueError(f"{what}: the views must share one storage dtype")
+
+
 def upsample_nearest(x: View, y: View):
+    """(moves 16-bit values: bf16 and fp16 views alike)"""
+    _same_dtype("upsample_nearest", x, y)
     _check(lib().sy_upsample_nearest(x.st(), y.st(), _stream()))
 
 
 def spp_maxpool(x: View, y5: View, y9: View, y13: View):
-    _check(lib().sy_spp_maxpool(x.st(), y5.st(), y9.st(), y13.st(), _stream()))
+    _same_dtype("spp_maxpool", x, y5, y9, y13)
+    fn = lib().sy_spp_maxpool_f16 if x.dtype == torch.float16 else lib().sy_spp_maxpool
+    _check(fn(x.st(), y5.st(), y9.st(), y13.st(), _stream()))
 
 
 def copy(x: View, y: View):
+    """(moves 16-bit values: bf16 and fp16 views alike)"""
+    _same_dtype("copy", x, y)
     _check(lib().sy_copy(x.st(), y.st(), _stream()))
 
 
 def head_pred_decode(cls_feat: View, reg_feat: View, w_reg, b_reg, w_obj, b_obj, w_cls, b_cls, stride,
                      anchor_offset, a_total, out, origin, sigmoid, decode):
+    _same_dtype("head_pred_decode", cls_feat, reg_feat)
     d = SyHeadPredDesc()
     d.cls_feat, d.reg_feat = cls_feat.st(), reg_feat.st()
+    d.storage = STORAGE[cls_feat.dtype]
     d.w_reg, d.b_reg, d.w_obj, d.b_obj = w_reg.data_ptr(), b_reg.data_ptr(), w_obj.data_ptr(), b_obj.data_ptr()
     d.w_cls, d.b_cls = w_cls.data_ptr(), b_cls.data_ptr()
     d.num_classes = w_cls.shape[0]

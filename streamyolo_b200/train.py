@@ -313,6 +313,7 @@ class Trainer:
     def __init__(self, model, lr=0.01, momentum=0.9, weight_decay=5e-4, ema_decay=0.9998, use_ema=True,
                  bucket_bytes=25 << 20, overlap=True):
         assert model.training and model.head.use_l1
+        engine.require_bf16_training(model)
         self.model = model
         self.fs = FlatState(model, ema=use_ema)
         self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
