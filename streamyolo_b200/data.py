@@ -91,6 +91,33 @@ def frame_transform(frames, ann, counts, mirror, input_size, max_labels=50, flip
     return x, labels
 
 
+def preprocess(x, labels, tsize, input_size, out=None):
+    """``Exp.preprocess(x, labels, tsize)`` (StreamYOLO's cfgs/s_s50_onex_dfp_tal_flip.py:160-171, the same in every
+    cfg) on the device: at a multi-scale size ``tsize`` other than ``input_size`` a bilinear resize (sy_resize_bilinear) and
+    ``labels[0][..., 1::2] *= sx``, ``labels[0][..., 2::2] *= sy``, the same for ``labels[1]`` (sy_scale_labels).  As in
+    the cfgs, ``labels`` is the (future, current) pair, or for a still model one label tensor whose images 0 and 1 are
+    rescaled.  At ``input_size`` nothing runs and ``(x, labels)`` come back as they are.
+
+    out  ``(x, labels)`` static buffers of size ``tsize`` (a CUDA graph's inputs): the resize writes there and the labels are
+         copied there before they are scaled, so ``labels`` is left unchanged.  Without it the labels are scaled in place,
+         like the cfgs do."""
+    scale_y, scale_x = tsize[0] / input_size[0], tsize[1] / input_size[1]
+    if scale_x == 1 and scale_y == 1:
+        return x, labels
+    if out is not None:
+        l_out = out[1]
+        if torch.is_tensor(labels):
+            l_out.copy_(labels)
+        else:
+            for dst, src in zip(l_out, labels):
+                dst.copy_(src)
+        labels = l_out
+    x = ops.resize_bilinear(x, tuple(tsize), out=None if out is None else out[0])
+    for t in (labels[0], labels[1]):
+        ops.scale_labels_(t, scale_x, scale_y)
+    return x, labels
+
+
 def stream_frame(frame, size=(600, 960), out=None):
     """streamyolo_det.preproc(frame, size) followed by torch.from_numpy(.).float()[None]: uint8 CUDA [h, w, 3] BGR ->
     fp32 [1, 3, H, W], a plain (possibly non-uniform) cv2-exact resize without pad or mirror."""

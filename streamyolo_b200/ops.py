@@ -659,11 +659,17 @@ def sgd_nesterov_ema_step(param, grad, momentum_buf, ema, n_param, decay_begin, 
     _check(lib().sy_sgd_nesterov_ema_step(C.byref(d), _stream()))
 
 
-def resize_bilinear(x, size):
-    """F.interpolate(x, size=size, mode="bilinear", align_corners=False) of an NCHW fp32 batch on the device."""
+def resize_bilinear(x, size, out=None):
+    """F.interpolate(x, size=size, mode="bilinear", align_corners=False) of an NCHW fp32 batch on the device.  ``out``: a
+    contiguous fp32 [B, C, size] tensor to write into (the static input of a CUDA graph) instead of a new one."""
     assert x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4
     b, c, hi, wi = x.shape
-    y = torch.empty((b, c, size[0], size[1]), dtype=torch.float32, device=x.device)
+    if out is None:
+        y = torch.empty((b, c, size[0], size[1]), dtype=torch.float32, device=x.device)
+    else:
+        _require(out.dtype == torch.float32 and out.is_contiguous() and tuple(out.shape) == (b, c, size[0], size[1])
+                 and out.device == x.device, f"resize_bilinear: out must be contiguous fp32 {(b, c, size[0], size[1])}")
+        y = out
     _check(lib().sy_resize_bilinear(x.data_ptr(), b * c, hi, wi, y.data_ptr(), size[0], size[1], _stream()))
     return y
 

@@ -105,3 +105,25 @@ def synth_labels(batch: int, height: int = 600, width: int = 960, n_obj: int = 1
             fut[b] = 0
             cur[b] = 0
     return torch.from_numpy(fut), torch.from_numpy(cur)
+
+
+def synth_uint8_pairs(batch: int, height: int = 600, width: int = 960, rows: int = 60, seed: int = 1):
+    """What the data loader hands ``data.pair_transform`` for ``batch`` pairs already at ``(height, width)``: uint8 BGR
+    frames ``[B, 2, h, w, 3]``, float64 annotations ``[B, 2, rows, 5]`` (x1, y1, x2, y2, cls; zero padded), int32 counts
+    ``[B, 2]`` and int32 mirror bits ``[B]``, as CPU tensors."""
+    g = _rng("uint8_pairs", seed)
+    lo = g.integers(0, 256, (batch, 2, height // 16 + 1, width // 16 + 1, 3)).astype(np.uint8)
+    frames = np.repeat(np.repeat(lo, 16, 2), 16, 3)[:, :, :height, :width] ^ g.integers(0, 64, (batch, 2, height, width, 3),
+                                                                                         dtype=np.uint8)
+    ann = np.zeros((batch, 2, rows, 5))
+    counts = g.integers(4, 20, (batch, 2)).astype(np.int32)
+    for i in range(batch):
+        for f in range(2):
+            n = counts[i, f]
+            x1, y1 = g.uniform(0, 0.9 * width, n), g.uniform(0, 0.9 * height, n)
+            bw, bh = g.uniform(8, 0.2 * width, n), g.uniform(8, 0.2 * height, n)
+            ann[i, f, :n] = np.stack([x1, y1, np.minimum(x1 + bw, width - 1), np.minimum(y1 + bh, height - 1),
+                                      g.integers(0, 8, n)], 1)
+    mirror = g.integers(0, 2, batch).astype(np.int32)
+    return (torch.from_numpy(np.ascontiguousarray(frames)), torch.from_numpy(ann), torch.from_numpy(counts),
+            torch.from_numpy(mirror))

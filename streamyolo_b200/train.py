@@ -16,6 +16,8 @@
       - ONE launch (``sy_sgd_nesterov_ema_step``) then does unscale (1 / (world x loss scale)) + weight decay + momentum +
         nesterov + parameter update + EMA over the whole state;
       - conv operands are re-packed from the fp32 masters by ``sy_pack_conv_weight`` launches (engine.WEIGHT_EPOCH).
+  * multi-scale training (``Exp.random_resize`` every 10 iterations): ``multiscale_sizes`` lists the sizes,
+    ``Trainer.capture_sizes`` captures one step per size into one graph memory pool, ``Trainer.replay_size`` runs one.
 """
 import copy
 import math
@@ -78,6 +80,21 @@ def train_step(model, optimizer, x, targets, ema=None, grad_scale=1.0):
     if ema is not None:
         ema.update(model)
     return losses
+
+
+def multiscale_sizes(input_size=(600, 960), random_size=(50, 70)):
+    """The distinct input sizes (h, w) multi-scale training runs at: what ``Exp.random_resize`` can draw
+    (StreamYOLO's cfgs/s_s50_onex_dfp_tal_flip.py:138-157: ``size = randint(*random_size)``,
+    ``(16 * int(size * h / w), 16 * size)``, every 10 iterations) plus ``input_size`` (the last epoch), in drawing order."""
+    size_factor = input_size[0] * 1.0 / input_size[1]
+    out = []
+    for size in range(random_size[0], random_size[1] + 1):
+        hw = (16 * int(size * size_factor), int(16 * size))
+        if hw not in out:
+            out.append(hw)
+    if tuple(input_size) not in out:
+        out.append(tuple(input_size))
+    return out
 
 
 # ------------------------------------------------------------------------------------------------ flat state
@@ -452,15 +469,132 @@ class Trainer:
 
     def replay(self, lr=None):
         self._set_hyper(lr)
+        self._replay_plan(self._plan)
+        return backward._loss_dict(self._graph_loss)
+
+    def _replay_plan(self, plan):
         works = []
-        for i, (g, bucket) in enumerate(self._plan):
-            if i == len(self._plan) - 1:
+        for i, (g, bucket) in enumerate(plan):
+            if i == len(plan) - 1:
                 for w in works:
                     w.wait()
             g.replay()
             if bucket is not None:
                 works.append(dist.all_reduce(self.fs.grad[bucket[0]:bucket[1]], op=dist.ReduceOp.SUM, async_op=True))
-        return backward._loss_dict(self._graph_loss)
+
+    # ---- multi-scale training: one captured step per input size, all in one graph memory pool
+    def capture_sizes(self, sizes, make_inputs, prologue=None, loss_scale=1.0):
+        """Capture one whole step (as ``capture``) per input size (``multiscale_sizes()``), for ``replay_size``.
+
+        make_inputs(size) -> (x, targets)   the static input buffers of that size's graph; called for every size before
+                                            anything is captured, so they live outside the graphs' memory pool;
+                                            the sizes' inputs may be views of one buffer (one graph runs at a time)
+        prologue(size, x, targets)          captured at the front of that size's graph, fills its inputs: e.g.
+                                            ``data.pair_transform(frames, ..., out=stage)`` into a buffer at ``input_size``
+                                            followed by ``data.preprocess(*stage, size, input_size, out=(x, targets))``
+
+        The capture leaves the training state as it found it: parameters, BatchNorm statistics (and
+        ``num_batches_tracked``), momentum, the EMA copy and ``updates`` are restored after the eager warm-up step that
+        each size runs before its capture.  The graphs share ONE memory pool (a step's intermediates are freed when its
+        capture ends, so the next capture reuses them: the pool is about one step of the largest size); the loss vector of
+        each graph stays referenced, so no capture takes it over.  Replays must therefore run one at a time, on the current
+        stream, which ``replay_size`` does.  Several ranks: the graphs are cut at the same gradient buckets for every size
+        (the flat gradient layout does not depend on the input size)."""
+        dev = self.fs.state.device
+        sizes = sorted({tuple(int(v) for v in s) for s in sizes}, key=lambda s: -s[0] * s[1])   # largest first: the
+        inputs = {s: make_inputs(s) for s in sizes}                                          # pool grows once
+        self._ms_hyper = torch.zeros(8, dtype=torch.float32, device=dev)
+        self._ms_host = [torch.zeros(8, dtype=torch.float32).pin_memory() for _ in range(2)]
+        self._ms_copied = [None, None]
+        self._ms_slot = 0
+        self._ms_loss_scale = loss_scale
+        state = (self.fs.state.clone(), self.fs.mom.clone(), None if self.fs.ema is None else self.fs.ema.clone())
+        counters = [(b, b.clone()) for b in self.model.buffers() if not b.dtype.is_floating_point]
+        updates = self.updates
+        self._stage_hyper(None)
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):                      # warm-up at every size (allocator, lazy module attributes)
+            for s in sizes:
+                x, targets = inputs[s]
+                if prologue is not None:
+                    prologue(s, x, targets)
+                self.forward_backward(x, targets, loss_scale)
+                self.optimizer_step(hyper=self._ms_hyper)
+            self.fs.state.copy_(state[0])                  # ... and back to the state before the call
+            self.fs.mom.copy_(state[1])
+            if state[2] is not None:
+                self.fs.ema.copy_(state[2])
+            for b, v in counters:
+                b.copy_(v)
+            engine.WEIGHT_EPOCH += 1
+            self._repack()                                 # conv operands of the restored parameters
+        self.updates = updates
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()                           # the warm-up's blocks: device memory for the graphs' pool
+        pool = torch.cuda.graph_pool_handle()
+        self._ms = {}                                      # size -> (plan, loss vector)
+        for s in sizes:
+            x, targets = inputs[s]
+            plan = []
+            cur = [None]
+
+            def begin():
+                g = torch.cuda.CUDAGraph()
+                g.capture_begin(pool=pool)
+                cur[0] = g
+
+            def cut(a, b):
+                cur[0].capture_end()
+                plan.append((cur[0], (a, b)))
+                begin()
+
+            self.sink.on_bucket = cut if self.world > 1 else None
+            with torch.cuda.stream(side):
+                begin()
+                if prologue is not None:
+                    prologue(s, x, targets)
+                loss = self.forward_backward(x, targets, loss_scale)
+                if self.world > 1:
+                    cur[0].capture_end()
+                    plan.append((cur[0], None))
+                    begin()
+                self.optimizer_step(hyper=self._ms_hyper)
+                cur[0].capture_end()
+                plan.append((cur[0], None))
+            self.sink.on_bucket = None
+            self._ms[s] = (plan, loss)
+            torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        buckets = {s: [b for _, b in plan] for s, (plan, _) in self._ms.items()}
+        first = buckets[sizes[0]]
+        assert all(b == first for b in buckets.values()), "the gradient buckets differ between input sizes"
+        return {s: len(plan) for s, (plan, _) in self._ms.items()}
+
+    def replay_size(self, size, lr=None):
+        """One captured step at ``size`` (a size given to ``capture_sizes``); returns its loss dict.  Several ranks: every rank
+        must replay the same size, as the reference's ``Exp.random_resize`` ensures (rank 0 draws it and broadcasts it)."""
+        size = tuple(int(v) for v in size)
+        if size not in self._ms:
+            raise KeyError(f"replay_size: no graph captured for {size} (captured: {sorted(self._ms)})")
+        plan, loss = self._ms[size]
+        self.updates += 1
+        self._stage_hyper(lr)
+        self._replay_plan(plan)
+        return backward._loss_dict(loss)
+
+    def _stage_hyper(self, lr):
+        """the hyper-parameter block of the size graphs for the step ``updates``, through two pinned slots: a slot is written
+        again only after the copy that read it last has run (the host runs ahead of the device)"""
+        i = self._ms_slot = (self._ms_slot + 1) % len(self._ms_host)
+        if self._ms_copied[i] is not None:
+            self._ms_copied[i].synchronize()
+        host = self._ms_host[i]
+        host[:6] = torch.tensor(self._hyper_values(lr, self._ms_loss_scale))
+        self._ms_hyper.copy_(host, non_blocking=True)
+        self._ms_copied[i] = torch.cuda.Event()
+        self._ms_copied[i].record()
 
     def ema_state_dict(self):
         return self.fs.ema_state_dict(self.model)
