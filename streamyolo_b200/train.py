@@ -18,6 +18,9 @@
       - conv operands are re-packed from the fp32 masters by ``sy_pack_conv_weight`` launches (engine.WEIGHT_EPOCH).
   * multi-scale training (``Exp.random_resize`` every 10 iterations): ``multiscale_sizes`` lists the sizes,
     ``Trainer.capture_sizes`` captures one step per size into one graph memory pool, ``Trainer.replay_size`` runs one.
+  * checkpoints (double_trainer.py:221-226, 285-318, 353-371): ``Trainer.state_dict`` / ``load_state_dict`` (exact
+    continuation), ``reference_checkpoint`` / ``load_reference_checkpoint`` (the reference's file and ``--resume``),
+    ``optimizer_state_dict`` in torch.optim.SGD format, ``all_reduce_norm`` (BatchNorm statistics averaged over the ranks).
 """
 import copy
 import math
@@ -201,16 +204,21 @@ class FlatState:
         o, n = self.offset[id(p)]
         return self.grad[o:o + n]
 
-    def ema_state_dict(self, model):
-        """state_dict of the EMA model ([yolox] ModelEMA.ema.state_dict()): float entries from the flat EMA copy, the rest
-        (num_batches_tracked) as in the live model."""
+    def views(self, model, buf):
+        """``model.state_dict()`` with every entry that lives in the flat state taken from ``buf`` (a buffer laid out like
+        ``state``, e.g. ``ema``) as a view; the rest (num_batches_tracked) are the module's own tensors."""
         base = self.state.data_ptr()
         index = {base + 4 * o: (o, n) for (o, n) in self.offset.values()}
         out = {}
         for k, t in model.state_dict().items():
             hit = index.get(t.data_ptr()) if t.dtype == torch.float32 else None
-            out[k] = self.ema[hit[0]:hit[0] + hit[1]].view(t.shape).clone() if hit else t.clone()
+            out[k] = buf[hit[0]:hit[0] + hit[1]].view(t.shape) if hit else t
         return out
+
+    def ema_state_dict(self, model):
+        """state_dict of the EMA model ([yolox] ModelEMA.ema.state_dict()): float entries from the flat EMA copy, the rest
+        (num_batches_tracked) as in the live model."""
+        return {k: t.clone() for k, t in self.views(model, self.ema).items()}
 
 
 class FlatSink:
@@ -508,9 +516,7 @@ class Trainer:
         self._ms_copied = [None, None]
         self._ms_slot = 0
         self._ms_loss_scale = loss_scale
-        state = (self.fs.state.clone(), self.fs.mom.clone(), None if self.fs.ema is None else self.fs.ema.clone())
-        counters = [(b, b.clone()) for b in self.model.buffers() if not b.dtype.is_floating_point]
-        updates = self.updates
+        snapshot = copy.deepcopy(self.state_dict())
         self._stage_hyper(None)
         side = torch.cuda.Stream()
         side.wait_stream(torch.cuda.current_stream())
@@ -521,15 +527,7 @@ class Trainer:
                     prologue(s, x, targets)
                 self.forward_backward(x, targets, loss_scale)
                 self.optimizer_step(hyper=self._ms_hyper)
-            self.fs.state.copy_(state[0])                  # ... and back to the state before the call
-            self.fs.mom.copy_(state[1])
-            if state[2] is not None:
-                self.fs.ema.copy_(state[2])
-            for b, v in counters:
-                b.copy_(v)
-            engine.WEIGHT_EPOCH += 1
-            self._repack()                                 # conv operands of the restored parameters
-        self.updates = updates
+            self.load_state_dict(snapshot)                 # ... and back to the state before the call
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         torch.cuda.empty_cache()                           # the warm-up's blocks: device memory for the graphs' pool
@@ -598,3 +596,144 @@ class Trainer:
 
     def ema_state_dict(self):
         return self.fs.ema_state_dict(self.model)
+
+    # ---- training state: save, resume, BatchNorm statistics over the ranks
+    # Loading copies into the buffers the step reads (fs.state, fs.mom, fs.ema, the modules' integer buffers) and never
+    # rebinds them: graphs captured by capture / capture_sizes keep reading those addresses, and the modules' tensors are
+    # views into the flat state.
+    def state_dict(self):
+        """The whole training state, for an EXACT continuation with ``load_state_dict``:
+
+            "model"         model.state_dict() (parameters, BatchNorm statistics, num_batches_tracked)
+            "optimizer"     optimizer_state_dict(): momentum in torch.optim.SGD format
+            "ema"           the EMA model's state_dict (as ema_state_dict()), None without EMA
+            "updates"       optimiser steps so far (the EMA decay ramp)
+            "lr", "momentum", "weight_decay"
+                            the Trainer's hyper-parameters (``lr`` is the default of steps that are given none)
+
+        As with ``nn.Module.state_dict`` the tensors are views of the live buffers: the weights, the momentum and the EMA
+        copy each share one storage, so ``torch.save`` writes each of them once.  ``copy.deepcopy`` it for a snapshot in
+        memory.  BatchNorm statistics are per rank, so with several ranks each rank saves its own."""
+        return {"model": self.model.state_dict(), "optimizer": self.optimizer_state_dict(),
+                "ema": None if self.fs.ema is None else self.fs.views(self.model, self.fs.ema),
+                "updates": self.updates, "lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay}
+
+    def load_state_dict(self, sd):
+        """Continue from a ``state_dict()`` of a Trainer of the same architecture and EMA setting: the next step computes
+        bit for bit what the saving Trainer's next step would have."""
+        if (sd["ema"] is None) != (self.fs.ema is None):
+            raise ValueError(f"load_state_dict: the state was saved {'without' if sd['ema'] is None else 'with'} EMA, "
+                             f"this Trainer runs {'with' if self.fs.ema is not None else 'without'} it")
+        self._check_entries(sd["model"], "model")
+        if self.fs.ema is not None:
+            self._check_entries(sd["ema"], "ema")
+        self.load_optimizer_state_dict(sd["optimizer"])
+        self._load_model(sd["model"])
+        if self.fs.ema is not None:
+            with torch.no_grad():
+                for k, t in self.fs.views(self.model, self.fs.ema).items():
+                    if t.dtype == torch.float32:
+                        t.copy_(sd["ema"][k])
+        self.updates = int(sd["updates"])
+        self.lr, self.momentum, self.weight_decay = sd["lr"], sd["momentum"], sd["weight_decay"]
+        self._state_changed()
+
+    def optimizer_state_dict(self):
+        """What ``build_optimizer(model, lr, momentum, weight_decay).state_dict()`` holds after the same updates (yolox's
+        three groups, BN weights | decayed weights | biases, indices in group order), with each parameter's
+        ``momentum_buffer`` a view of its slice of the flat momentum.  Before the first update there is no per-parameter
+        state, as in torch."""
+        opt = build_optimizer(self.model, self.lr, self.momentum, self.weight_decay)
+        if self.updates > 0:
+            for g in opt.param_groups:
+                for p in g["params"]:
+                    o, n = self.fs.offset[id(p)]
+                    opt.state[p]["momentum_buffer"] = self.fs.mom[o:o + n].view(p.shape)
+        return opt.state_dict()
+
+    def load_optimizer_state_dict(self, sd):
+        """Momentum and hyper-parameters from a torch.optim.SGD state_dict of ``build_optimizer``'s groups (the reference's
+        ``ckpt["optimizer"]`` or ``optimizer_state_dict()``).  A parameter without ``momentum_buffer`` gets zeros, which
+        is what torch's first step amounts to.  The fused step runs one lr and momentum, nesterov, and weight decay on the
+        decayed group only: other hyper-parameters raise ``ValueError``."""
+        opt = build_optimizer(self.model, self.lr, self.momentum, self.weight_decay)
+        opt.load_state_dict(sd)                            # torch checks the group count and sizes
+        g = opt.param_groups
+        lr, momentum, wd = g[0]["lr"], g[0]["momentum"], g[1]["weight_decay"]
+        if (any(x["lr"] != lr or x["momentum"] != momentum or not x["nesterov"] or x["dampening"] != 0
+                or x.get("maximize", False) for x in g) or g[0]["weight_decay"] != 0 or g[2]["weight_decay"] != 0):
+            raise ValueError("load_optimizer_state_dict: hyper-parameters the fused SGD-nesterov step cannot run: "
+                             + str([{k: v for k, v in x.items() if k != "params"} for x in g]))
+        bufs = [(p, opt.state.get(p, {}).get("momentum_buffer")) for x in g for p in x["params"]]
+        bad = [(tuple(b.shape), tuple(p.shape)) for p, b in bufs if b is not None and b.shape != p.shape]
+        if bad:
+            raise ValueError(f"load_optimizer_state_dict: momentum_buffer shapes do not match the parameters: {bad[:3]}")
+        with torch.no_grad():
+            for p, b in bufs:
+                o, n = self.fs.offset[id(p)]
+                if b is None:
+                    self.fs.mom[o:o + n].zero_()
+                else:
+                    self.fs.mom[o:o + n].copy_(b.reshape(-1))
+        self.lr, self.momentum, self.weight_decay = lr, momentum, wd
+
+    def reference_checkpoint(self, start_epoch, best_ap=0.0):
+        """The dict the reference trainer's ``save_ckpt`` writes (exps/train_utils/double_trainer.py:353-371):
+        ``{"start_epoch", "model", "optimizer", "best_ap"}`` with "model" the EMA weights when EMA is on, otherwise the live
+        weights, and "optimizer" in torch.optim.SGD format.  ``torch.save`` it on rank 0 after ``all_reduce_norm()``.
+        Resuming from it (``load_reference_checkpoint`` or the reference's ``--resume``) is lossy by the reference's own
+        design; ``state_dict()`` is the exact path."""
+        model = self.model.state_dict() if self.fs.ema is None else self.fs.views(self.model, self.fs.ema)
+        return {"start_epoch": start_epoch, "model": model, "optimizer": self.optimizer_state_dict(), "best_ap": best_ap}
+
+    def load_reference_checkpoint(self, ckpt, updates):
+        """The reference's ``--resume`` (``resume_train``, double_trainer.py:285-318, and the ModelEMA built after it,
+        :173-175) on a checkpoint its ``save_ckpt`` or ``reference_checkpoint`` wrote: ckpt["model"] becomes the live
+        weights and BatchNorm buffers, the momentum and hyper-parameters come from ckpt["optimizer"], the EMA copy restarts
+        from the loaded weights and ``updates`` is set to ``updates`` (the reference passes ``max_iter * start_epoch``).
+        Lossy: when the file was saved with EMA the live weights are replaced by the EMA weights, as in the reference;
+        ``load_state_dict`` is the exact path.  Returns ``(start_epoch, best_ap)``.
+
+        Fine-tuning from a yolox checkpoint (``-c yolox_l.pth``: a shape-tolerant load of ckpt["model"] only) is done on
+        the model before the Trainer is built."""
+        self._check_entries(ckpt["model"], "ckpt['model']")
+        self.load_optimizer_state_dict(ckpt["optimizer"])
+        self._load_model(ckpt["model"])
+        if self.fs.ema is not None:
+            self.fs.ema.copy_(self.fs.state)
+        self.updates = int(updates)
+        self._state_changed()
+        return ckpt["start_epoch"], ckpt.get("best_ap", 0)
+
+    def all_reduce_norm(self):
+        """[yolox] ``all_reduce_norm(model)``, which the reference runs before every evaluation and ``last_epoch`` checkpoint
+        (double_trainer.py:223-226): every BatchNorm state entry becomes its mean over the ranks.  The statistics are per
+        rank during training (``broadcast_buffers=False``); they are the flat state's float-buffer region, so this is ONE
+        all-reduce (SUM, then / world: yolox's ``op="mean"``).  BatchNorm weights and biases (parameters, updated with the
+        mean gradient) and num_batches_tracked are equal on all ranks already.  Runs on the current stream and is not meant
+        for a captured graph.  No-op in one process."""
+        if self.world == 1:
+            return
+        stats = self.fs.state[self.fs.n_param:self.fs.n_total]
+        dist.all_reduce(stats, op=dist.ReduceOp.SUM)
+        stats.div_(self.world)
+        self._state_changed()
+
+    def _check_entries(self, sd, what):
+        want = self.model.state_dict()
+        missing = [k for k in want if k not in sd]
+        extra = [k for k in sd if k not in want]
+        shape = [k for k in want if k in sd and tuple(sd[k].shape) != tuple(want[k].shape)]
+        if missing or extra or shape:
+            raise ValueError(f"{what}: not a state of this model's architecture: {len(missing)} keys missing {missing[:3]}, "
+                             f"{len(extra)} unexpected {extra[:3]}, {len(shape)} of another shape {shape[:3]}")
+
+    def _load_model(self, sd):
+        with torch.no_grad():
+            for k, t in self.model.state_dict().items():       # views of the flat state, and the integer buffers
+                t.copy_(sd[k])
+
+    def _state_changed(self):
+        """the flat state was written outside the fused step: new operand cache keys, conv operands re-packed in place"""
+        engine.WEIGHT_EPOCH += 1
+        self._repack()
