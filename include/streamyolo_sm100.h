@@ -194,6 +194,18 @@ int sy_spp_maxpool_f16(SyTensor x, SyTensor y5, SyTensor y9, SyTensor y13, sy_st
 /* strided copy of a view (used for 3-channel duplicates and buffers).  sy_upsample_nearest and sy_copy only move
  * 16-bit values, so they serve fp16 views unchanged. */
 int sy_copy(SyTensor x, SyTensor y, sy_stream_t stream);
+/* Per-stream first frame of a batched on_pipe tick: the star node of exps/model/dfp_pafpn.py:177-228 (no buffer: the
+ * support features are the current ones, sup = cur) for the streams that start a sequence, the carried buffer for the
+ * others.  For every image i with flags[i] != 0, image i of src[k] is copied into image i of dst[k], k < n_pairs (the
+ * three FPN levels in ONE launch); images whose flag is clear are not touched.  The flags live in device memory, so a
+ * CUDA graph that captured the launch follows what the host writes there before each replay.  Moves 16-bit values: bf16
+ * and fp16 views alike. */
+typedef struct {
+  SyTensor src[3], dst[3];   /* pair k: [n][h][w][c] views of the same shape; pairs k >= n_pairs are ignored */
+  int32_t n_pairs;           /* 1..3 */
+  const int32_t* flags;      /* [n], device memory */
+} SySelectImagesDesc;
+int sy_select_images(const SySelectImagesDesc* d, sy_stream_t stream);
 
 /* -------- head: prediction convs + decode (exps/model/tal_head.py:105-131,167-171,
  * 174,197-199,225-260) ------------------------------------------------------------ */

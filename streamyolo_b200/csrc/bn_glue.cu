@@ -1,6 +1,6 @@
-// BatchNorm(train) finalize / apply+SiLU, nearest upsample, SPP max pools, strided copy:
-// vectorised (16-byte) HBM-bound kernels over NHWC bf16 views.  The upsample and the copy only move 16-bit values and
-// serve fp16 views unchanged; the SPP max pools compare values and have an fp16 instantiation (sy_spp_maxpool_f16).
+// BatchNorm(train) finalize / apply+SiLU, nearest upsample, SPP max pools, strided copy, per-image select:
+// vectorised (16-byte) HBM-bound kernels over NHWC bf16 views.  The upsample, the copy and the select only move 16-bit
+// values and serve fp16 views unchanged; the SPP max pools compare values and have an fp16 instantiation (sy_spp_maxpool_f16).
 #include <math.h>
 #include <stdlib.h>
 
@@ -273,6 +273,50 @@ __global__ void copy_kernel(const __nv_bfloat16* __restrict__ x, long long xp, _
   }
 }
 
+// Per-image select of up to three views in one launch (the FPN levels of a streaming tick): blockIdx.z = view pair,
+// blockIdx.y = image.  The flag is read on the device, so a captured launch follows the flags the host writes before each
+// replay; every block of an image whose flag is clear returns at once.  Inside an image it is copy_kernel's walk.
+struct SelectPair {
+  const __nv_bfloat16* x;
+  __nv_bfloat16* y;
+  long long xp, yp;            // pixel pitches (elements)
+  long long x_img, y_img;      // image strides (elements)
+  long long npix;              // pixels per image
+  int C;
+};
+struct SelectArgs {
+  SelectPair p[3];
+};
+
+__global__ void __launch_bounds__(256) select_images_kernel(const __grid_constant__ SelectArgs a,
+                                                            const int32_t* __restrict__ flags) {
+  if (flags[blockIdx.y] == 0) return;
+  const SelectPair& p = a.p[blockIdx.z];
+  const __nv_bfloat16* x = p.x + (long long)blockIdx.y * p.x_img;
+  __nv_bfloat16* y = p.y + (long long)blockIdx.y * p.y_img;
+  const long long npix = p.npix;
+  const int G = p.C / 8;
+  if (G <= (int)blockDim.x) {
+    const int ppb = (int)blockDim.x / G;
+    const int prow = (int)threadIdx.x / G, g = (int)threadIdx.x - prow * G;
+    if (prow >= ppb) return;
+    const long long step = (long long)gridDim.x * ppb;
+    for (long long pix0 = (long long)blockIdx.x * ppb + prow; pix0 < npix; pix0 += 4 * step) {
+      uint4 v[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (pix0 + j * step < npix) v[j] = *reinterpret_cast<const uint4*>(x + (pix0 + j * step) * p.xp + g * 8);
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (pix0 + j * step < npix) *reinterpret_cast<uint4*>(y + (pix0 + j * step) * p.yp + g * 8) = v[j];
+    }
+  } else {                                        // more than 2048 channels: one pixel per block pass
+    for (long long pix = blockIdx.x; pix < npix; pix += gridDim.x)
+      for (int g = threadIdx.x; g < G; g += blockDim.x)
+        *reinterpret_cast<uint4*>(y + pix * p.yp + g * 8) = *reinterpret_cast<const uint4*>(x + pix * p.xp + g * 8);
+  }
+}
+
 static inline int grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
   const long long cap = (long long)sm_count() * 16;
@@ -390,4 +434,29 @@ extern "C" int sy_copy(SyTensor x, SyTensor y, sy_stream_t stream_) {
                                                                                           npix, x.c);
   }
   return launch_status("copy_kernel");
+}
+
+extern "C" int sy_select_images(const SySelectImagesDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr && d->flags != nullptr && d->n_pairs >= 1 && d->n_pairs <= 3, SY_EINVAL,
+             "select_images: needs device flags and 1-3 view pairs");
+  SelectArgs a{};
+  const int n = d->src[0].n;
+  SY_REQUIRE(n >= 1 && n <= 65535, SY_EINVAL, "select_images: %d images (1..65535)", n);
+  long long most = 1;                               // 16-byte chunks per image of the largest pair
+  for (int k = 0; k < d->n_pairs; ++k) {
+    const SyTensor s = d->src[k], t = d->dst[k];
+    SY_REQUIRE(view_ok(s) && view_ok(t) && s.n == n && t.n == n && s.h == t.h && s.w == t.w && s.c == t.c, SY_EINVAL,
+               "select_images: pair %d: bad or mismatched views", k);
+    const long long npix = (long long)s.h * s.w;
+    a.p[k] = SelectPair{CBF(s.ptr), BF(t.ptr), (long long)s.pitch, (long long)t.pitch, npix * s.pitch, npix * t.pitch,
+                        npix, s.c};
+    const long long chunks = npix * (s.c / 8);
+    most = chunks > most ? chunks : most;
+  }
+  // one pass of 4 chunks per thread over the largest image; the smaller pairs' surplus blocks return at once
+  const long long want = (most + 4LL * 256 - 1) / (4LL * 256);
+  const int gx = (int)(want < 1024 ? want : 1024);
+  select_images_kernel<<<dim3(gx, n, d->n_pairs), 256, 0, stream>>>(a, d->flags);
+  return launch_status("select_images_kernel");
 }

@@ -133,6 +133,10 @@ class SyLetterboxDesc(C.Structure):
                 ("out_w", C.c_int32), ("flags", C.c_void_p), ("out", C.c_void_p)]
 
 
+class SySelectImagesDesc(C.Structure):
+    _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
+
+
 # every symbol include/streamyolo_sm100.h declares: (restype, argtypes)
 _SIG = {
     "sy_last_error_string": (C.c_char_p, []),
@@ -158,6 +162,7 @@ _SIG = {
     "sy_spp_maxpool": (C.c_int, [SyTensor, SyTensor, SyTensor, SyTensor, C.c_void_p]),
     "sy_spp_maxpool_f16": (C.c_int, [SyTensor, SyTensor, SyTensor, SyTensor, C.c_void_p]),
     "sy_copy": (C.c_int, [SyTensor, SyTensor, C.c_void_p]),
+    "sy_select_images": (C.c_int, [C.POINTER(SySelectImagesDesc), C.c_void_p]),
     "sy_head_pred_decode": (C.c_int, [C.POINTER(SyHeadPredDesc), C.c_void_p]),
     "sy_tal_loss_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "sy_tal_loss": (C.c_int, [C.POINTER(SyTalLossDesc), C.c_void_p]),
@@ -461,6 +466,22 @@ def copy(x: View, y: View):
     """(moves 16-bit values: bf16 and fp16 views alike)"""
     _same_dtype("copy", x, y)
     _check(lib().sy_copy(x.st(), y.st(), _stream()))
+
+
+def select_images(srcs, dsts, flags):
+    """Image i of ``dsts[k]`` = image i of ``srcs[k]`` for every i whose int32 device flag ``flags[i]`` is set, for up to
+    three view pairs in ONE launch (sy_select_images); images whose flag is clear are not touched.  The flags are read on
+    the device: a captured launch follows what is written there before each replay.  (Moves 16-bit values: bf16 and fp16
+    views alike.)"""
+    _require(1 <= len(srcs) == len(dsts) <= 3, "select_images: 1 to 3 (src, dst) view pairs")
+    _same_dtype("select_images", *srcs, *dsts)
+    _require(torch.is_tensor(flags) and flags.dtype == torch.int32 and flags.is_contiguous()
+             and flags.numel() == srcs[0].n, "select_images: flags must be int32 [n]")
+    d = SySelectImagesDesc()
+    for k, (s, t) in enumerate(zip(srcs, dsts)):
+        d.src[k], d.dst[k] = s.st(), t.st()
+    d.n_pairs, d.flags = len(srcs), flags.data_ptr()
+    _check(lib().sy_select_images(C.byref(d), _stream()))
 
 
 def head_pred_decode(cls_feat: View, reg_feat: View, w_reg, b_reg, w_obj, b_obj, w_cls, b_cls, stride,
