@@ -473,6 +473,41 @@ typedef struct SyLetterboxDesc {
 } SyLetterboxDesc;
 int sy_letterbox(const SyLetterboxDesc* d, sy_stream_t stream);
 
+/* ---- JPEG decode ----
+ * Batched decode of the training frames' JPEG files into what cv2.imread(path) returns for them (uint8 BGR, bit-identical),
+ * replacing the host decodes of exps/dataset/tal_flip_one_future_argoversedataset.py:195,216,
+ * tal_flip_two_future_argoversedataset.py:207,228 and still_argoversedataset.py:160.  Reads only device memory and never
+ * synchronises, so it can be captured in a CUDA graph in front of sy_letterbox.
+ * Decoded streams: baseline (SOF0) or extended sequential (SOF1) 8-bit Huffman JPEG with three YCbCr components in one
+ * interleaved scan, luma sampling 1x1, 2x1 or 2x2 (chroma 1x1), any Huffman tables, 8- or 16-bit quantisation tables, with
+ * or without restart intervals, any size.  Everything else, and every damaged stream, gets a non-zero status[i] and image
+ * i's output is left untouched; the other images of the batch decode as usual.  The decoder reads no input byte at or past
+ * lengths[i] and writes nothing outside image i's output row.
+ * Descriptor errors return SY_EINVAL; problems with the stream contents go only to status[]. */
+enum {
+  SY_JPEG_OK = 0,
+  SY_JPEG_EHEADER = 1,       /* not a JPEG, malformed or truncated marker segments, undefined or invalid tables, or
+                              * lengths[i] outside [4, max_bytes] */
+  SY_JPEG_EUNSUPPORTED = 2,  /* progressive, arithmetic, lossless, hierarchical, 12-bit, not 3 components, RGB (Adobe
+                              * transform 0), other sampling factors or more than one scan */
+  SY_JPEG_EORIENTATION = 3,  /* an EXIF orientation other than 1 (cv2.imread would rotate the image) */
+  SY_JPEG_ESIZE = 4,         /* the frame's size differs from the descriptor's h x w */
+  SY_JPEG_EDATA = 5          /* corrupt or truncated entropy-coded data */
+};
+typedef struct SyJpegDecodeDesc {
+  const uint8_t* bytes;     /* [n][max_bytes] file bytes, image i in the first lengths[i] bytes of row i */
+  const int32_t* lengths;   /* [n] device int32 */
+  int32_t n;
+  int64_t max_bytes;        /* row pitch of bytes (1 .. 2^28) */
+  int32_t h, w;             /* the size every image must have */
+  uint8_t* out;             /* [n][h][w][3] BGR */
+  int32_t* status;          /* [n] device int32, SY_JPEG_* */
+  void* workspace;          /* sy_jpeg_decode_workspace_bytes(n, max_bytes, h, w) bytes, 256-byte aligned */
+  size_t workspace_bytes;
+} SyJpegDecodeDesc;
+size_t sy_jpeg_decode_workspace_bytes(int32_t n, int64_t max_bytes, int32_t h, int32_t w);
+int sy_jpeg_decode(const SyJpegDecodeDesc* d, sy_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,9 +6,16 @@ TrainTransform / ValTransform (:170-263) for a batch of single frames, ``stream_
 driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60, 176-181).  Both are bit-identical to the cv2 / numpy host code
 they replace (sy_pair_labels, sy_frame_labels, sy_letterbox); INTEGRATION.md shows where they plug in.
 """
+import numpy as np
 import torch
 
 from . import ops
+
+# per-image status of decode_jpeg (SY_JPEG_* of include/streamyolo_sm100.h)
+JPEG_STATUS = {0: "ok", 1: "malformed or truncated header, or invalid tables", 2: "unsupported JPEG variant "
+               "(progressive, arithmetic, lossless, 12-bit, not YCbCr 4:2:0 / 4:2:2 / 4:4:4, or several scans)",
+               3: "EXIF orientation other than 1", 4: "image size differs from the batch size",
+               5: "corrupt or truncated entropy-coded data"}
 
 
 def _fit(h, w, size):
@@ -129,3 +136,60 @@ def stream_frame(frame, size=(600, 960), out=None):
     ops._require(tuple(out.shape) == (1, 3, size[0], size[1]), "stream_frame: out must be [1, 3, H, W]")
     ops.letterbox(frame.view(1, h, w, 3), (h, w), size, out)
     return out
+
+
+def pack_jpeg(files, max_bytes):
+    """Host side of device JPEG decoding: the file contents ``files`` (``bytes`` or uint8 numpy arrays, e.g.
+    ``np.fromfile(path, np.uint8)``) -> (uint8 [N, max_bytes] zero-padded rows, int32 [N] lengths), both numpy, for the
+    dataset's ``pull_item`` / collate.  A file longer than ``max_bytes`` raises ValueError."""
+    rows = np.zeros((len(files), max_bytes), np.uint8)
+    lengths = np.zeros(len(files), np.int32)
+    for i, f in enumerate(files):
+        a = np.frombuffer(f, np.uint8) if isinstance(f, (bytes, bytearray, memoryview)) else np.asarray(f, np.uint8).ravel()
+        if a.size > max_bytes:
+            raise ValueError(f"pack_jpeg: file {i} has {a.size} bytes, more than max_bytes = {max_bytes}")
+        rows[i, :a.size] = a
+        lengths[i] = a.size
+    return rows, lengths
+
+
+_JPEG_WS = {}
+
+
+def decode_jpeg(streams, lengths, hw, out=None, status=None, workspace=None):
+    """Decode a batch of JPEG files on the device into what cv2.imread returns for them (sy_jpeg_decode).
+
+    streams   uint8 CUDA [N, max_bytes] file bytes (pack_jpeg's rows, copied to the device)
+    lengths   int32 CUDA [N]
+    hw        (H, W) every frame must have
+    out, status, workspace   uint8 [N, H, W, 3], int32 [N] and the uint8 workspace to write into (static buffers for
+              CUDA-graph capture); new ones when omitted (the workspace is then cached per device and shape)
+
+    -> ``(frames, status)``: frames uint8 [N, H, W, 3] BGR, the ``raw=True`` input of pair_transform (viewed as
+    [N / 2, 2, H, W, 3]) and frame_transform; status int32 [N], 0 where the frame decoded, else a JPEG_STATUS code and
+    that frame is left as it was.  Nothing is read back: check_jpeg_status is the synchronising check."""
+    ops._require(torch.is_tensor(streams) and streams.dim() == 2 and streams.is_cuda,
+                 "decode_jpeg: streams must be a CUDA uint8 [N, max_bytes] tensor")
+    n, max_bytes = streams.shape
+    h, w = hw
+    dev = streams.device
+    if out is None:
+        out = torch.empty((n, h, w, 3), dtype=torch.uint8, device=dev)
+    if status is None:
+        status = torch.empty((n,), dtype=torch.int32, device=dev)
+    ops._require(tuple(out.shape) == (n, h, w, 3), f"decode_jpeg: out must be [{n}, {h}, {w}, 3]")
+    if workspace is None:
+        key = (dev, n, max_bytes, h, w)
+        if key not in _JPEG_WS:
+            _JPEG_WS[key] = torch.empty(ops.jpeg_decode_workspace_bytes(n, max_bytes, h, w), dtype=torch.uint8, device=dev)
+        workspace = _JPEG_WS[key]
+    ops.jpeg_decode(streams, lengths, out, status, workspace)
+    return out, status
+
+
+def check_jpeg_status(status):
+    """Synchronising check of decode_jpeg's status: raises RuntimeError naming the first frame that did not decode and why."""
+    st = status.cpu().tolist()
+    for i, s in enumerate(st):
+        if s != 0:
+            raise RuntimeError(f"decode_jpeg: frame {i} did not decode: {JPEG_STATUS.get(s, f'status {s}')}")

@@ -133,6 +133,12 @@ class SyLetterboxDesc(C.Structure):
                 ("out_w", C.c_int32), ("flags", C.c_void_p), ("out", C.c_void_p)]
 
 
+class SyJpegDecodeDesc(C.Structure):
+    _fields_ = [("bytes", C.c_void_p), ("lengths", C.c_void_p), ("n", C.c_int32), ("max_bytes", C.c_int64),
+                ("h", C.c_int32), ("w", C.c_int32), ("out", C.c_void_p), ("status", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
 class SySelectImagesDesc(C.Structure):
     _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
 
@@ -192,6 +198,8 @@ _SIG = {
     "sy_pair_labels": (C.c_int, [C.POINTER(SyPairLabelsDesc), C.c_void_p]),
     "sy_frame_labels": (C.c_int, [C.POINTER(SyFrameLabelsDesc), C.c_void_p]),
     "sy_letterbox": (C.c_int, [C.POINTER(SyLetterboxDesc), C.c_void_p]),
+    "sy_jpeg_decode_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
+    "sy_jpeg_decode": (C.c_int, [C.POINTER(SyJpegDecodeDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
 
@@ -790,3 +798,30 @@ class PackBatch:
             arr = (SyPackItem * len(self.items))(*self.items)
             self.table = torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(self.device)
         _check(lib().sy_pack_conv_weights_batch(self.table.data_ptr(), len(self.items), self.total, _stream()))
+
+
+def jpeg_decode_workspace_bytes(n, max_bytes, h, w):
+    """bytes of the sy_jpeg_decode workspace for n frames of h x w stored in rows of max_bytes (host-only)"""
+    need = load_library().sy_jpeg_decode_workspace_bytes(n, max_bytes, h, w)
+    _require(need > 0, f"jpeg_decode: bad sizes (n {n}, max_bytes {max_bytes}, {h}x{w})")
+    return need
+
+
+def jpeg_decode(streams, lengths, out, status, workspace):
+    """Decode n JPEG files into uint8 BGR frames (sy_jpeg_decode): ``streams`` uint8 [n, max_bytes] file bytes, ``lengths``
+    int32 [n], ``out`` uint8 [n, h, w, 3], ``status`` int32 [n] (SY_JPEG_*), ``workspace`` uint8 of at least
+    jpeg_decode_workspace_bytes(n, max_bytes, h, w) bytes, all on one CUDA device.  Nothing is read back."""
+    _require(_tensor_ok(streams, torch.uint8, 2), "jpeg_decode: streams must be contiguous uint8 [n, max_bytes]")
+    n, max_bytes = streams.shape
+    _require(_tensor_ok(lengths, torch.int32, 1) and lengths.shape[0] == n, "jpeg_decode: lengths must be int32 [n]")
+    _require(_tensor_ok(out, torch.uint8, 4) and out.shape[0] == n and out.shape[3] == 3,
+             "jpeg_decode: out must be contiguous uint8 [n, h, w, 3]")
+    _require(_tensor_ok(status, torch.int32, 1) and status.shape[0] == n, "jpeg_decode: status must be int32 [n]")
+    need = jpeg_decode_workspace_bytes(n, max_bytes, out.shape[1], out.shape[2])
+    _require(_tensor_ok(workspace, torch.uint8, 1) and workspace.numel() >= need,
+             f"jpeg_decode: workspace must be contiguous uint8 of at least {need} bytes")
+    _require(len({t.device for t in (streams, lengths, out, status, workspace)}) == 1 and streams.is_cuda,
+             "jpeg_decode: all tensors must be on one CUDA device")
+    d = SyJpegDecodeDesc(streams.data_ptr(), lengths.data_ptr(), n, max_bytes, out.shape[1], out.shape[2], out.data_ptr(),
+                         status.data_ptr(), workspace.data_ptr(), workspace.numel())
+    _check(lib().sy_jpeg_decode(C.byref(d), _stream()), kernels=5)
