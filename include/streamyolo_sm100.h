@@ -45,6 +45,15 @@ enum {
 /* 16-bit activation storage of a launch (SyConvDesc.storage, SyHeadPredDesc.storage) */
 enum { SY_STORAGE_BF16 = 0, SY_STORAGE_F16 = 1 };
 
+/* Activation after BatchNorm ([yolox] get_activation: "silu" / "relu" / "lrelu"), the `act` argument of sy_conv2d_tc,
+ * sy_conv2d_simt, sy_dwconv2d (FUSED mode), sy_bn_act_apply and sy_bn_act_backward; any other value: SY_EINVAL.
+ *   SY_ACT_NONE   identity
+ *   SY_ACT_SILU   v * sigmoid(v)                    (nn.SiLU)
+ *   SY_ACT_RELU   v > 0 ? v : 0                     (nn.ReLU;  derivative z > 0 ? 1 : 0)
+ *   SY_ACT_LRELU  v > 0 ? v : 0.1f * v              (nn.LeakyReLU(0.1);  derivative z > 0 ? 1 : 0.1f)
+ * The derivatives at z = 0 (0 for ReLU, 0.1 for LeakyReLU) are autograd's for the in-place modules yolox builds. */
+enum { SY_ACT_NONE = 0, SY_ACT_SILU = 1, SY_ACT_RELU = 2, SY_ACT_LRELU = 3 };
+
 typedef struct {
   void* ptr;      /* bf16 (fp16 where the entry point stores fp16) */
   int32_t n, h, w, c;
@@ -73,12 +82,12 @@ typedef struct {
 
 typedef struct {
   SyTensor x;            /* input  */
-  SyTensor y;            /* output: RAW -> conv result; FUSED -> silu(acc*scale+shift)(+res) */
+  SyTensor y;            /* output: RAW -> conv result; FUSED -> act(acc*scale+shift)(+res) */
   const void* w;         /* bf16 [Cout][kh*kw][Cin] */
   int32_t kh, kw;        /* 1 or 3 each, padding (k-1)/2 */
   int32_t stride;        /* 1 or 2 */
   int32_t mode;          /* SY_CONV_RAW / SY_CONV_FUSED */
-  int32_t act;           /* FUSED: 1 = SiLU, 0 = identity */
+  int32_t act;           /* FUSED: SY_ACT_* (checked in every mode) */
   const float* scale;    /* FUSED: [Cout] (folded BatchNorm), may be NULL = 1 */
   const float* shift;    /* FUSED: [Cout], may be NULL = 0 */
   SyTensor res;          /* FUSED: optional residual added after the activation (ptr NULL = none) */
@@ -159,7 +168,7 @@ int sy_focus_pack(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w
 int sy_focus_pack_f16(const float* x, int32_t b, int32_t in_ch, int32_t h, int32_t w_px, int32_t frames,
                       SyTensor y, sy_stream_t stream);
 
-/* -------- BatchNorm (train mode) + SiLU (replaces nn.BatchNorm2d + nn.SiLU inside
+/* -------- BatchNorm (train mode) + activation (replaces nn.BatchNorm2d + nn.SiLU / ReLU / LeakyReLU inside
  * [yolox] BaseConv; eps/momentum from cfgs/s_s50_onex_dfp_tal_flip.py:40-44) ---------- */
 /* Per-(row-chunk, channel) partial sums of a stored tensor: partials [P][2][c],
  * P = sy_stats_num_partials(n, h*w) image-major. */
@@ -174,7 +183,7 @@ int sy_bn_finalize(const float* partials, int32_t n_partials, int32_t p_split, i
                    const float* gamma, const float* beta, float* running_mean, float* running_var,
                    int64_t* num_batches_tracked, float momentum, float eps,
                    float* scale_out, float* shift_out, sy_stream_t stream);
-/* y = act(x*scale[g]+shift[g]) (+ res), g = (image >= split_n); single bf16 rounding.
+/* y = act(x*scale[g]+shift[g]) (+ res), g = (image >= split_n), act = SY_ACT_*; single bf16 rounding.
  * y_group1_offset / res_group1_offset: element offsets added to the y / res addresses of the images of
  * statistics group 1 (0 = plain views).  The DFP fusion (exps/model/dfp_pafpn.py:168-170) uses them to
  * write jian(support frame n) into channels [c, 2c) of output image n - split_n, next to jian(current). */
@@ -265,7 +274,7 @@ typedef struct SyConvWgradDesc {
 size_t sy_conv2d_wgrad_workspace_bytes(const SyConvWgradDesc* d);
 int sy_conv2d_wgrad_tc(const SyConvWgradDesc* d, sy_stream_t stream);
 
-/* Backward of BatchNorm(train) + SiLU behind a [yolox] BaseConv (autograd of nn.BatchNorm2d + nn.SiLU under
+/* Backward of BatchNorm(train) + activation behind a [yolox] BaseConv (autograd of nn.BatchNorm2d + the act module under
  * loss.backward(), exps/train_utils/double_trainer.py:114).  raw = the conv output the forward stored, dy = gradient w.r.t.
  * the BaseConv output; scale / shift / mean / invstd = [2 groups][c] as published by the forward (scale = gamma * invstd,
  * shift = beta - mean * scale; images >= split_n form statistics group 1).  Writes draw (bf16, gradient w.r.t. the conv
@@ -275,7 +284,7 @@ typedef struct SyBnActBwdDesc {
   SyTensor raw, dy, draw;
   const float* scale; const float* shift; const float* mean; const float* invstd;
   int32_t split_n;
-  int32_t act;             /* 1: SiLU, 0: identity */
+  int32_t act;             /* SY_ACT_* of the forward */
   float* dgamma; float* dbeta;
   int32_t accumulate;
   float* partials; int32_t n_partials;

@@ -1,16 +1,19 @@
-// Backward of BatchNorm(train) + SiLU behind every [yolox] BaseConv (what autograd runs for loss.backward(),
-// /root/reference/exps/train_utils/double_trainer.py:114):   y = silu(z),  z = gamma * xhat + beta,
+// Backward of BatchNorm(train) + activation behind every [yolox] BaseConv (what autograd runs for loss.backward(),
+// /root/reference/exps/train_utils/double_trainer.py:114):   y = act(z),  z = gamma * xhat + beta,
 // xhat = (raw - mean_g) * invstd_g  with the batch statistics of the pixel's statistics group g (current / support frames,
 // see DESIGN.md section 3), raw = the conv output.
 //
-//   dz      = dy * silu'(z)                      silu'(z) = s (1 + z (1 - s)),  s = sigmoid(z)
+//   dz      = dy * act'(z)        SiLU:  s (1 + z (1 - s)),  s = sigmoid(z)
+//                                 ReLU:  z > 0 ? 1 : 0       LeakyReLU(0.1):  z > 0 ? 1 : 0.1     identity: 1
 //   dbeta   = sum dz             dgamma = sum dz * xhat               (over both groups)
 //   draw    = gamma * invstd_g * (dz - mean_g(dz) - xhat * mean_g(dz * xhat))
 //
 // Three launches: partial sums (up to 296 rows per statistics group so that the pass fills the GPU whatever the map size;
 // deterministic, fixed order), a finalize (one warp per channel) that produces dgamma, dbeta and the per-(group, channel)
 // coefficients, and the element-wise pass that writes draw in bf16 for the conv's data / weight gradient kernels.
-// HBM-bound 16-byte accesses over NHWC bf16 views.
+// HBM-bound 16-byte accesses over NHWC bf16 views.  The reduce and apply kernels come in two instantiations: KINK = false
+// (identity / SiLU, the element loop of the SiLU-only kernels unchanged) and KINK = true (ReLU / LeakyReLU: the
+// derivative is a select on z > 0 with the launch's code, uniform across the grid; no SFU work).
 #include <math.h>
 
 #include "common.cuh"
@@ -25,14 +28,6 @@ __device__ __forceinline__ void unpack8b(const uint4& v, float* f) {
   f[0] = bf16_lo(v.x); f[1] = bf16_hi(v.x); f[2] = bf16_lo(v.y); f[3] = bf16_hi(v.y);
   f[4] = bf16_lo(v.z); f[5] = bf16_hi(v.z); f[6] = bf16_lo(v.w); f[7] = bf16_hi(v.w);
 }
-// silu'(z) = s (1 + z (1 - s)), s = sigmoid(z) on the approximate SFU ops (ex2 / rcp, ~2 ulp fp32; the result is stored as bf16)
-__device__ __forceinline__ float dsilu(float z) {
-  float e, s;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(z * -1.4426950408889634f));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(s) : "f"(1.0f + e));
-  return s * (1.0f + z * (1.0f - s));
-}
-
 struct BwdArgs {
   const __nv_bfloat16* raw; long long raw_pitch;
   const __nv_bfloat16* dy; long long dy_pitch;
@@ -45,6 +40,7 @@ struct BwdArgs {
 // Partial rows [rows0 + rows1][2 (sum dz | sum dz * xhat)][C].  Row r of a group covers an equal share of the group's
 // pixels; inside the block a thread owns one 8-channel chunk and every (256 / G)-th pixel (kBwdUnroll 16-byte load pairs in
 // flight), then the pixel lanes are combined through shared memory in a fixed order (deterministic).
+template <bool KINK>
 __global__ void __launch_bounds__(kBwdThreads, 2) bn_act_bwd_reduce_kernel(const BwdArgs q, float* partials) {
   __shared__ float red[kBwdThreads][17];
   const int grp = (int)blockIdx.x >= q.rows0 ? 1 : 0;
@@ -89,7 +85,8 @@ __global__ void __launch_bounds__(kBwdThreads, 2) bn_act_bwd_reduce_kernel(const
           unpack8b(dv[j], d);
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            const float dz = q.act ? d[i] * dsilu(r[i] * sc[i] + sh[i]) : d[i];
+            const float z = r[i] * sc[i] + sh[i];
+            const float dz = KINK ? d[i] * dact_f(q.act, z) : (q.act ? d[i] * dsilu(z) : d[i]);
             s[i] += dz;
             s[8 + i] += dz * (r[i] * k1[i] + k0[i]);
           }
@@ -175,8 +172,9 @@ __global__ void __launch_bounds__(256) bn_act_bwd_finalize_kernel(const float* _
   dgamma[c] = accumulate ? dgamma[c] + dg : dg;
 }
 
-// draw = A * dz + C1 * r + C0 (bf16), dz = dy * silu'(r * A + B).  Same thread mapping as the forward normalise pass: a
+// draw = A * dz + C1 * r + C0 (bf16), dz = dy * act'(r * A + B).  Same thread mapping as the forward normalise pass: a
 // thread owns one 8-channel chunk for its whole life (coefficients in registers), kBwdUnroll load pairs in flight.
+template <bool KINK>
 __global__ void __launch_bounds__(kBwdThreads, 2) bn_act_bwd_apply_kernel(const BwdArgs q, const float* __restrict__ coef,
                                                                        __nv_bfloat16* draw, long long draw_pitch) {
   const int C = q.C, G = C >> 3;
@@ -218,7 +216,8 @@ __global__ void __launch_bounds__(kBwdThreads, 2) bn_act_bwd_apply_kernel(const 
       unpack8b(dv[j], d);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        const float dz = q.act ? d[i] * dsilu(r[i] * A[i] + B[i]) : d[i];
+        const float z = r[i] * A[i] + B[i];
+        const float dz = KINK ? d[i] * dact_f(q.act, z) : (q.act ? d[i] * dsilu(z) : d[i]);
         o[i] = A[i] * dz + (C1[i] * r[i] + C0[i]);
       }
       *reinterpret_cast<uint4*>(op + pix * draw_pitch) =
@@ -262,6 +261,7 @@ extern "C" int sy_bn_act_backward(const SyBnActBwdDesc* d, sy_stream_t stream_) 
   SY_REQUIRE(d->scale && d->shift && d->mean && d->invstd && d->dgamma && d->dbeta && d->partials && d->coef, SY_EINVAL,
              "bn_act_backward: null pointer");
   SY_REQUIRE(raw.c <= 8 * kBwdThreads, SY_EINVAL, "bn_act_backward: C=%d > %d", raw.c, 8 * kBwdThreads);
+  SY_REQUIRE(act_ok(d->act), SY_EINVAL, "bn_act_backward: act=%d is not an SY_ACT_* code", d->act);
   const int hw = raw.h * raw.w;
   const int split = (d->split_n > 0 && d->split_n < raw.n) ? d->split_n : raw.n;
   BwdArgs q{};
@@ -273,7 +273,10 @@ extern "C" int sy_bn_act_backward(const SyBnActBwdDesc* d, sy_stream_t stream_) 
   q.rows0 = bwd_rows_for(q.split_pix, raw.c); q.rows1 = bwd_rows_for(q.npix - q.split_pix, raw.c);
   const int rows = q.rows0 + q.rows1;
   SY_REQUIRE(d->n_partials >= rows, SY_EWORKSPACE, "bn_act_backward: %d partial rows, need %d", d->n_partials, rows);
-  bn_act_bwd_reduce_kernel<<<rows, kBwdThreads, 0, stream>>>(q, d->partials);
+  auto reduce = [&](auto kernel) { kernel<<<rows, kBwdThreads, 0, stream>>>(q, d->partials); };
+  const bool kink = d->act == SY_ACT_RELU || d->act == SY_ACT_LRELU;
+  if (kink) reduce(bn_act_bwd_reduce_kernel<true>);
+  else reduce(bn_act_bwd_reduce_kernel<false>);
   const double inv0 = q.split_pix > 0 ? 1.0 / (double)q.split_pix : 0.0;
   const double inv1 = q.npix - q.split_pix > 0 ? 1.0 / (double)(q.npix - q.split_pix) : 0.0;
   // (plain launches: programmatic dependent launch of the backward kernels was measured SLOWER -- 17.16 vs 16.39 ms per
@@ -283,7 +286,10 @@ extern "C" int sy_bn_act_backward(const SyBnActBwdDesc* d, sy_stream_t stream_) 
   const int G = raw.c / 8, ppb = kBwdThreads / G;
   long long blocks = (q.npix + (long long)ppb * kBwdUnroll - 1) / ((long long)ppb * kBwdUnroll);
   if (blocks > sm_count() * 8) blocks = sm_count() * 8;
-  bn_act_bwd_apply_kernel<<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, reinterpret_cast<__nv_bfloat16*>(dr.ptr),
-                                                                 dr.pitch);
+  auto apply = [&](auto kernel) {
+    kernel<<<(int)blocks, kBwdThreads, 0, stream>>>(q, d->coef, reinterpret_cast<__nv_bfloat16*>(dr.ptr), dr.pitch);
+  };
+  if (kink) apply(bn_act_bwd_apply_kernel<true>);
+  else apply(bn_act_bwd_apply_kernel<false>);
   return launch_status("bn_act_backward kernels");
 }

@@ -67,15 +67,15 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
   return make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
 }
 
-// y = act(x * scale[grp] + shift[grp]) (+ res), 16 bytes (8 channels) per thread and pixel.
+// y = act(x * scale[grp] + shift[grp]) (+ res), act = the SY_ACT_* code ACT, 16 bytes (8 channels) per thread and pixel.
 // A thread keeps ONE channel chunk for its whole life (scale/shift of both statistics groups live in registers, no
 // per-element index division) and walks the pixels with kApplyUnroll independent 16-byte loads in flight.
 constexpr int kApplyThreads = 256;
 constexpr int kApplyUnroll = 4;
-template <bool ACT, bool RES>
+template <int ACT, bool RES>
 __global__ void __launch_bounds__(kApplyThreads, 3)
 bn_act_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xp, const float* __restrict__ scale,
-                    const float* __restrict__ shift, long long split_pix, int act,
+                    const float* __restrict__ shift, long long split_pix,
                     const __nv_bfloat16* res, long long rp, __nv_bfloat16* y, long long yp,
                     long long npix, int C, long long y_goff1, long long r_goff1) {
   pdl_launch_dependents();
@@ -125,7 +125,7 @@ bn_act_apply_kernel(const __nv_bfloat16* __restrict__ x, long long xp, const flo
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         const float t = f[i] * sc[i] + sh[i];
-        f[i] = ACT ? silu_f(t) : t;
+        f[i] = act_f(ACT, t);
       }
       if (RES) {
         float r[8];
@@ -353,6 +353,7 @@ extern "C" int sy_bn_act_apply(SyTensor x, const float* scale, const float* shif
   SY_REQUIRE(x.n == y.n && x.h == y.h && x.w == y.w && x.c == y.c, SY_EINVAL, "bn_act_apply: x/y shape mismatch");
   SY_REQUIRE(((uintptr_t)scale % 16) == 0 && ((uintptr_t)shift % 16) == 0, SY_EINVAL, "bn_act_apply: scale/shift alignment");
   SY_REQUIRE((y_goff1 % 8) == 0 && (r_goff1 % 8) == 0, SY_EINVAL, "bn_act_apply: group offsets must be multiples of 8");
+  SY_REQUIRE(act_ok(act), SY_EINVAL, "bn_act_apply: act=%d is not an SY_ACT_* code", act);
   const __nv_bfloat16* rp = nullptr;
   long long rpitch = 0;
   if (res.ptr) {
@@ -374,13 +375,21 @@ extern "C" int sy_bn_act_apply(SyTensor x, const float* scale, const float* shif
     // 100 (all shared, the conv kernels' split) 6.51 ms.
     SY_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 0));
     SY_CUDA(launch_pdl(kernel, dim3(grid), dim3(kApplyThreads), 0, stream, CBF(x.ptr), (long long)x.pitch, scale, shift,
-                       split_pix, act, rp, rpitch, BF(y.ptr), (long long)y.pitch, npix, x.c, (long long)y_goff1,
+                       split_pix, rp, rpitch, BF(y.ptr), (long long)y.pitch, npix, x.c, (long long)y_goff1,
                        (long long)r_goff1));
     return SY_OK;
   };
+  auto go = [&](auto code) -> int {
+    constexpr int A = decltype(code)::value;
+    return has_res ? launch(bn_act_apply_kernel<A, true>) : launch(bn_act_apply_kernel<A, false>);
+  };
   int rc;
-  if (act) rc = has_res ? launch(bn_act_apply_kernel<true, true>) : launch(bn_act_apply_kernel<true, false>);
-  else rc = has_res ? launch(bn_act_apply_kernel<false, true>) : launch(bn_act_apply_kernel<false, false>);
+  switch (act) {
+    case SY_ACT_NONE: rc = go(std::integral_constant<int, SY_ACT_NONE>{}); break;
+    case SY_ACT_SILU: rc = go(std::integral_constant<int, SY_ACT_SILU>{}); break;
+    case SY_ACT_RELU: rc = go(std::integral_constant<int, SY_ACT_RELU>{}); break;
+    default: rc = go(std::integral_constant<int, SY_ACT_LRELU>{}); break;
+  }
   if (rc != SY_OK) return rc;
   return launch_status("bn_act_apply_kernel");
 }

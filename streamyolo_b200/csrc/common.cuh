@@ -130,5 +130,32 @@ __device__ __forceinline__ float silu_f(float v) {
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
   return v * r;
 }
+// silu'(z) = s (1 + z (1 - s)), s = sigmoid(z) on the approximate SFU ops (ex2 / rcp, ~2 ulp fp32; the result is stored as bf16)
+__device__ __forceinline__ float dsilu(float z) {
+  float e, s;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(z * -1.4426950408889634f));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(s) : "f"(1.0f + e));
+  return s * (1.0f + z * (1.0f - s));
+}
+
+constexpr float kLreluSlope = 0.1f;     // nn.LeakyReLU(0.1), what [yolox] get_activation("lrelu") builds
+
+// act(v) for an SY_ACT_* code.  ReLU / LeakyReLU are PyTorch's expressions (v > 0 ? v : 0 / v * 0.1f): -0 and NaN map like
+// theirs.  A compile-time code folds to one branch; a run-time one (the FUSED epilogues) is a short select chain in front
+// of the unchanged SiLU.
+__device__ __forceinline__ float act_f(int code, float v) {
+  if (code == SY_ACT_SILU) return silu_f(v);
+  if (code == SY_ACT_RELU) return v > 0.f ? v : 0.f;
+  if (code == SY_ACT_LRELU) return v > 0.f ? v : v * kLreluSlope;
+  return v;
+}
+// d act / dz at the pre-activation z, autograd's convention at z = 0: 0 for ReLU, 0.1 for LeakyReLU
+__device__ __forceinline__ float dact_f(int code, float z) {
+  if (code == SY_ACT_SILU) return dsilu(z);
+  if (code == SY_ACT_RELU) return z > 0.f ? 1.f : 0.f;
+  if (code == SY_ACT_LRELU) return z > 0.f ? 1.f : kLreluSlope;
+  return 1.f;
+}
+inline bool act_ok(int code) { return code >= SY_ACT_NONE && code <= SY_ACT_LRELU; }
 
 }  // namespace sy

@@ -53,7 +53,7 @@ __global__ void conv_simt_kernel(const SimtConvParams p) {
       for (int o = 0; o < 8; ++o) {
         const int c = g * 8 + o;
         float t = acc[o] * (p.scale ? p.scale[c] : 1.f) + (p.shift ? p.shift[c] : 0.f);
-        acc[o] = p.act ? silu_f(t) : t;
+        acc[o] = act_f(p.act, t);
       }
       if (p.res) {
         const uint4 rv = *reinterpret_cast<const uint4*>(p.res + pix * p.res_pitch + g * 8);
@@ -160,6 +160,7 @@ extern "C" int sy_conv2d_simt(const SyConvDesc* d, sy_stream_t stream_) {
   SY_REQUIRE((d->kh == 1 || d->kh == 3) && (d->kw == 1 || d->kw == 3) && (d->stride == 1 || d->stride == 2), SY_EINVAL,
              "conv2d_simt: kernel %dx%d stride %d unsupported", d->kh, d->kw, d->stride);
   SY_REQUIRE(d->storage == SY_STORAGE_BF16, SY_EINVAL, "conv2d_simt: bf16 storage only (storage %d)", d->storage);
+  SY_REQUIRE(act_ok(d->act), SY_EINVAL, "conv2d_simt: act=%d is not an SY_ACT_* code", d->act);
   SimtConvParams p{};
   p.pad_h = (d->kh - 1) / 2; p.pad_w = (d->kw - 1) / 2;
   p.N = x.n; p.H = x.h; p.W = x.w; p.Cin = x.c; p.Cout = y.c; p.kh = d->kh; p.kw = d->kw; p.stride = d->stride;

@@ -584,7 +584,7 @@ __device__ __forceinline__ void statistics(const Params& p, const Smem& sm, int 
 // registers), then converts its rows of every 64-column slab into the staging tile.  A ring stage is handed back to the
 // producers one commit group late (wgmma.wait_group 1), so the next group's MMAs are queued while the last ones drain.
 // Returns the debug-timeline cursor of thread 0, which the kernel tail carries on.  F16: fp16 operands and output.
-template <int BN, bool TL, int AM, bool F16>
+template <int BN, bool TL, int AM, bool F16, bool KINK>
 __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int tid) {
   // the compiler knows this range for threadIdx.x but not for the argument; with it the FUSED scale/shift fill below is
   // one guarded pass instead of a loop
@@ -702,7 +702,7 @@ __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int 
     wgmma_fence_operand(acc);
     release();
     tl_rec<TL>(p, tl_n, 2, 1, tile, 0);
-    // ---- epilogue: per 64-column slab, registers -> (raw | folded BN + SiLU + residual) -> bf16 | fp16 -> staging tile
+    // ---- epilogue: per 64-column slab, registers -> (raw | folded BN + act + residual) -> bf16 | fp16 -> staging tile
 #pragma unroll
     for (int slab = 0; slab < BN / kSlabCols; ++slab, sbuf ^= sflip) {
       tl_rec<TL>(p, tl_n, 2, 2, tile, slab);
@@ -743,7 +743,11 @@ __device__ __forceinline__ int mma_convert(const Params& p, const Smem& sm, int 
             if (p.mode != SY_CONV_RAW) {
               v0 = v0 * sScale[cl] + sShift[cl];
               v1 = v1 * sScale[cl + 1] + sShift[cl + 1];
-              if (p.act) { v0 = silu_f(v0); v1 = silu_f(v1); }
+              if constexpr (KINK) {                      // ReLU / LeakyReLU: conv_tc_kink_kernel only
+                v0 = act_f(p.act, v0); v1 = act_f(p.act, v1);
+              } else if (p.act) {                        // SiLU (SY_ACT_NONE: the backward's data-gradient convs)
+                v0 = silu_f(v0); v1 = silu_f(v1);
+              }
               if (p.res != nullptr && inb) {
                 const uint32_t rv = *reinterpret_cast<const uint32_t*>(p.res + pix[h] * p.res_pitch + n0 + cl);
                 v0 += st_lo<F16>(rv);
@@ -906,7 +910,7 @@ __device__ __forceinline__ void bn_tail(const Params& p, const Smem& sm, int tid
 //              shared-memory descriptors into that halo (every 8-pixel swizzle atom of a tap view is one halo row).
 //              3x3 stride-1 only.  Each input pixel crosses L2 -> SM once per tile instead of nine times.
 // The body of both kernels below: carves up shared memory, initialises the barriers, dispatches the warp roles.
-template <int BN, bool TL, int AM, bool F16>
+template <int BN, bool TL, int AM, bool F16, bool KINK>
 __device__ __forceinline__ void conv_tc_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmY,
                                              const Params& p) {
   constexpr bool HALO = (AM == 2);
@@ -969,7 +973,7 @@ __device__ __forceinline__ void conv_tc_body(const CUtensorMap& tmA, const CUten
     bn_tail<TL>(p, sm, threadIdx.x, tl);
   } else {
     reg_alloc<kRegsMma>();
-    int tl = mma_convert<BN, TL, AM, F16>(p, sm, threadIdx.x);
+    int tl = mma_convert<BN, TL, AM, F16, KINK>(p, sm, threadIdx.x);
     bn_tail<TL>(p, sm, threadIdx.x, tl);
   }
   __syncthreads();
@@ -981,7 +985,7 @@ template <int BN, bool TL, int AM>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                const __grid_constant__ CUtensorMap tmY, const Params p) {
-  conv_tc_body<BN, TL, AM, false>(tmA, tmB, tmY, p);
+  conv_tc_body<BN, TL, AM, false, false>(tmA, tmB, tmY, p);
 }
 
 // fp16 activations and weights, FUSED mode only (a kernel of its own: the bf16 kernel's name and instantiations stay as
@@ -990,7 +994,17 @@ template <int BN, int AM>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_f16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                    const __grid_constant__ CUtensorMap tmY, const Params p) {
-  conv_tc_body<BN, false, AM, true>(tmA, tmB, tmY, p);
+  conv_tc_body<BN, false, AM, true, false>(tmA, tmB, tmY, p);
+}
+
+// FUSED mode with SY_ACT_RELU / SY_ACT_LRELU, bf16 or fp16: the same roles with the activation switch compiled into the
+// epilogue.  A kernel of its own so that the SiLU / identity epilogue of the two kernels above (every eval conv, the
+// backward's data-gradient convs) stays the code it was.
+template <int BN, int AM, bool F16>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_tc_kink_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                    const __grid_constant__ CUtensorMap tmY, const Params p) {
+  conv_tc_body<BN, false, AM, F16, true>(tmA, tmB, tmY, p);
 }
 
 // ------------------------------------------------------------------ host side
@@ -1069,6 +1083,8 @@ static bool set_smem_attr() {
     else
       ok = cudaFuncSetAttribute(conv_tc_kernel<BN, false, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess &&
            cudaFuncSetAttribute(conv_tc_kernel<BN, true, AM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) == cudaSuccess;
+    ok = ok && cudaFuncSetAttribute(conv_tc_kink_kernel<BN, AM, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    kSmemLimit) == cudaSuccess;
     if (!ok) cudaGetLastError();
     state = ok ? 1 : -1;
   }
@@ -1131,6 +1147,10 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
       for (int i = 0; i < 8; ++i)
         if (ok_smem[i] == 0) { ok_smem[i] = smem; break; }
     }
+  }
+  if (p.mode == SY_CONV_FUSED && (p.act == SY_ACT_RELU || p.act == SY_ACT_LRELU)) {     // (no timeline: refused)
+    SY_CUDA(launch_pdl(conv_tc_kink_kernel<BN, AM, F16>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
+    return launch_status("conv_tc_kink_kernel");
   }
   if constexpr (F16) {                  // (no statistics, no timeline: the host side refused them)
     SY_CUDA(launch_pdl(conv_tc_f16_kernel<BN, AM>, dim3(grid), dim3(kThreads), (size_t)smem, stream, ta, tb, ty, p));
@@ -1216,6 +1236,9 @@ extern "C" int sy_conv2d_tc(const SyConvDesc* d, sy_stream_t stream_) {
              d->tile_mode, d->tile_bn);
   SY_REQUIRE(d->storage == SY_STORAGE_BF16 || d->storage == SY_STORAGE_F16, SY_EINVAL, "conv2d_tc: storage %d unsupported",
              d->storage);
+  SY_REQUIRE(act_ok(d->act), SY_EINVAL, "conv2d_tc: act=%d is not an SY_ACT_* code", d->act);
+  SY_REQUIRE(!(d->mode == SY_CONV_FUSED && d->act >= SY_ACT_RELU && d->debug_timeline != nullptr), SY_EINVAL,
+             "conv2d_tc: the debug timeline is not recorded for ReLU / LeakyReLU FUSED launches");
   const bool f16 = d->storage == SY_STORAGE_F16;
   SY_REQUIRE(!f16 || (d->mode == SY_CONV_FUSED && d->stat_partials == nullptr && d->bn[0].gamma == nullptr &&
                       d->debug_timeline == nullptr),

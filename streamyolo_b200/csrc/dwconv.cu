@@ -53,7 +53,7 @@ __global__ void __launch_bounds__(256) dwconv_kernel(const DwParams p) {
       for (int i = 0; i < 8; ++i) {
         const int c = g * 8 + i;
         const float t = acc[i] * (p.scale ? p.scale[c] : 1.f) + (p.shift ? p.shift[c] : 0.f);
-        acc[i] = p.act ? silu_f(t) : t;
+        acc[i] = act_f(p.act, t);
       }
       if (p.res != nullptr) {
         const uint4 rv = *reinterpret_cast<const uint4*>(p.res + pix * p.res_pitch + g * 8);
@@ -88,6 +88,7 @@ extern "C" int sy_dwconv2d(const SyConvDesc* d, sy_stream_t stream_) {
   SY_REQUIRE(((uintptr_t)d->w % 16) == 0, SY_EINVAL, "dwconv2d: weights not 16B aligned");
   SY_REQUIRE(d->storage == SY_STORAGE_BF16 || (d->storage == SY_STORAGE_F16 && d->mode == SY_CONV_FUSED), SY_EINVAL,
              "dwconv2d: storage %d in mode %d unsupported (fp16: FUSED only)", d->storage, d->mode);
+  SY_REQUIRE(act_ok(d->act), SY_EINVAL, "dwconv2d: act=%d is not an SY_ACT_* code", d->act);
   DwParams p{};
   p.x = reinterpret_cast<const uint16_t*>(x.ptr); p.x_pitch = x.pitch;
   p.w = reinterpret_cast<const uint16_t*>(d->w);

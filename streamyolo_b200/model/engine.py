@@ -2,14 +2,15 @@
 
 Train mode (``model.training``): every BaseConv = wgmma conv writing the raw bf16 result + per-tile
 statistic partials  ->  bn_finalize (batch statistics, running-stat update)  ->  bn_act_apply
-(normalise + SiLU + optional residual, written straight into its consumer's concat slice).
+(normalise + activation + optional residual, written straight into its consumer's concat slice).
 The two frames of a pair are batched through the shared-weight backbone as 2B images with
 *grouped* statistics (group 0 = current frames, group 1 = support frames), which reproduces the
 reference's two sequential passes (/root/reference/exps/model/dfp_pafpn.py:120,145) exactly,
 including the order of the two running-statistic updates.
 
 Eval mode: BatchNorm is folded into a per-channel scale/shift applied in the conv epilogue
-together with SiLU and the residual (what yolox ``fuse_model`` + ``fuseforward`` achieve).
+together with the activation and the residual (what yolox ``fuse_model`` + ``fuseforward`` achieve).  The activation is
+each BaseConv's own (``act_code``: SiLU, ReLU or LeakyReLU(0.1), as its ``act`` name says).
 
 The recording forward of a training step (model/backward.py) is this same walk with a tape in the ``Ctx``: nothing is
 updated in place, every op keeps what its backward needs and is recorded on the tape.
@@ -193,9 +194,15 @@ def graph_capture_stream(device):
     return _CAPTURE_STREAMS[key]
 
 
-def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, act=1, y_goff1=0, res_goff1=0, impl=None,
-                kind="normal"):
-    """Train mode: conv -> batch statistics -> BatchNorm (running-stat update) -> act (+res) into ``y``.
+def act_code(m):
+    """the kernels' SY_ACT_* code of a BaseConv's activation (its ``act`` name: "silu" / "relu" / "lrelu")"""
+    return ops.ACT_CODES[m.act_name]
+
+
+def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, act=None, y_goff1=0, res_goff1=0,
+                impl=None, kind="normal"):
+    """Train mode: conv -> batch statistics -> BatchNorm (running-stat update) -> act (+res) into ``y``.  ``act``: the
+    SY_ACT_* code, by default that of ``mods`` (which share one activation).
     Tensor-core path = 2 launches: the conv writes the raw bf16 result, accumulates the statistics and
     (grid barrier + parallel reduce in its tail) publishes scale/shift; then the normalise pass.  ``mods``: one BaseConv, or two whose
     outputs are concatenated along channels (CSPLayer conv1 | conv2).  With a tape the conv also writes the batch mean /
@@ -214,6 +221,8 @@ def conv_bn_act(ctx: Ctx, mods, x: View, wpk, k, s, y: View, res: View = None, a
     for m in mods:
         m._stats_epoch = getattr(m, "_stats_epoch", 0) + 1
     impl = impl or ctx.impl
+    if act is None:
+        act = act_code(mods[0])
     if impl == "tc":
         partials = torch.empty((ops.conv_stat_rows(), 4 * cout), dtype=torch.float32, device=ctx.device)
         segs, c0 = [], 0
@@ -277,7 +286,7 @@ def base_conv(ctx: Ctx, m, x: View, y: View = None, res: View = None) -> View:
     dw = m.conv.groups > 1
     wpk = packed_operand(m, ctx.slot("_pk"), [m.conv.weight], ctx.pack(ops.pack_dw_weight if dw else ops.pack_conv_weight))
     impl = "dw" if dw else ctx.impl
-    act = 1 if m.act_name == "silu" else 0
+    act = act_code(m)
     if not ctx.train:
         scale, shift = _folded(m)
         ops.conv2d(x, wpk, y, k, s, ops.SY_CONV_FUSED, impl=impl, scale=scale, shift=shift, act=act, res=res)
@@ -298,9 +307,10 @@ def _folded_pair(m1, m2):
 
 def conv_pair(ctx: Ctx, m1, m2, x: View) -> View:
     """Two BaseConvs with the same geometry reading the same input as ONE launch: [.., c1 + c2] output, one BatchNorm
-    parameter segment per module (CSPLayer conv1 | conv2; the first cls / reg tower convs of a head level)."""
-    if hasattr(m1, "dconv") or hasattr(m2, "dconv"):          # depthwise variants: two ordinary launches into one buffer
-        c1, c2 = m1.pconv.conv.out_channels, m2.pconv.conv.out_channels
+    parameter segment per module (CSPLayer conv1 | conv2; the first cls / reg tower convs of a head level).  Depthwise
+    variants, and two modules with different activations, take two ordinary launches into the one buffer."""
+    if hasattr(m1, "dconv") or hasattr(m2, "dconv") or m1.act_name != m2.act_name:
+        c1, c2 = (getattr(m, "pconv", m).conv.out_channels for m in (m1, m2))
         u = ctx.empty(x.n, x.h, x.w, c1 + c2)
         base_conv(ctx, m1, x, u.ch(0, c1))
         base_conv(ctx, m2, x, u.ch(c1, c2))
@@ -313,7 +323,7 @@ def conv_pair(ctx: Ctx, m1, m2, x: View) -> View:
     wpk = packed_operand(m1, ctx.slot("_pk2"), [m1.conv.weight, m2.conv.weight], ctx.pack(ops.pack_conv_weight))
     if not ctx.train:
         scale, shift = _folded_pair(m1, m2)
-        ops.conv2d(x, wpk, u, k, s, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=1)
+        ops.conv2d(x, wpk, u, k, s, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=act_code(m1))
     else:
         conv_bn_act(ctx, (m1, m2), x, wpk, k, s, u)
     _trace(m1, u.ch(0, c1))
@@ -366,7 +376,8 @@ def focus_stem(ctx: Ctx, m, x, frames) -> View:
     y = ctx.empty(n, h // 2, w // 2, cout)
     if not ctx.train:
         scale, shift = _folded(bc)
-        ops.conv2d(xin, wpk, y, ops.STEM_K, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift, act=1)
+        ops.conv2d(xin, wpk, y, ops.STEM_K, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift,
+                   act=act_code(bc))
     else:
         conv_bn_act(ctx, (bc,), xin, wpk, ops.STEM_K, 1, y, kind="stem")
     _trace(bc, y)
@@ -447,12 +458,13 @@ def dfp_fuse(ctx: Ctx, net, cur, sup):
         half = m.conv.out_channels
         out = ctx.empty(nb, c.h, c.w, 2 * half)
         wpk = packed_operand(m, ctx.slot("_pk"), [m.conv.weight], ctx.pack(ops.pack_conv_weight))
+        act = act_code(m)
         if not ctx.train:
             scale, shift = _folded(m)
             ops.conv2d(c, wpk, out.ch(0, half), 1, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale, shift=shift,
-                       act=1, res=c.ch(0, half))
+                       act=act, res=c.ch(0, half))
             ops.conv2d(s, wpk, out.ch(half, half), 1, 1, ops.SY_CONV_FUSED, impl=ctx.impl, scale=scale,
-                       shift=shift, act=1, res=c.ch(half, half))
+                       shift=shift, act=act, res=c.ch(half, half))
         else:
             # the reference runs jian(cur) then jian(sup): two BN batches, two running-stat updates.
             # Batched here (grouped statistics) when cur/sup are the two halves of one buffer -- not with a tape: the
@@ -464,12 +476,12 @@ def dfp_fuse(ctx: Ctx, net, cur, sup):
                 # group 1 (support frames, images nb..2nb-1) lands in channels [half, 2*half) of image n - nb
                 yv = View(out.buf, 0, half, 0, 2 * nb)
                 rv = View(c.buf, c.c0, half, c.n0, 2 * nb)
-                conv_bn_act(sub, (m,), both, wpk, 1, 1, yv, rv, 1,
+                conv_bn_act(sub, (m,), both, wpk, 1, 1, yv, rv, act,
                             y_goff1=half - nb * yv.img_elems(), res_goff1=half - nb * rv.img_elems())
             else:
                 sub = Ctx(True, nb, nb, ctx.device, ctx.tape)
                 for src, dst, r in ((c, out.ch(0, half), c.ch(0, half)), (s, out.ch(half, half), c.ch(half, half))):
-                    conv_bn_act(sub, (m,), src, wpk, 1, 1, dst, r, 1)
+                    conv_bn_act(sub, (m,), src, wpk, 1, 1, dst, r, act)
         outs.append(out)
     return tuple(outs)
 

@@ -19,18 +19,24 @@ def _run_standalone(module, fn, x):
         return engine.as_nchw(fn(ctx, v))
 
 
+# [yolox] get_activation: the module each ``act`` name builds (and so the module type, repr and state dict of ``self.act``)
+ACTIVATIONS = {"silu": lambda: nn.SiLU(inplace=True), "relu": lambda: nn.ReLU(inplace=True),
+               "lrelu": lambda: nn.LeakyReLU(0.1, inplace=True)}
+
+
 class BaseConv(nn.Module):
-    """Conv2d(bias=False, pad=(k-1)//2) -> BatchNorm2d -> SiLU."""
+    """Conv2d(bias=False, pad=(k-1)//2) -> BatchNorm2d -> act, act = "silu" (SiLU), "relu" (ReLU) or "lrelu"
+    (LeakyReLU(0.1))."""
 
     def __init__(self, in_channels, out_channels, ksize, stride, groups=1, bias=False, act="silu"):
         super().__init__()
         if bias or groups not in (1, in_channels) or (groups > 1 and in_channels != out_channels):
             raise NotImplementedError("streamyolo_b200: BaseConv is dense (groups=1) or depthwise (groups=in=out), without bias")
-        if act not in ("silu",):
-            raise NotImplementedError(f"activation {act!r}: only 'silu' is used by the StreamYOLO cfgs")
+        if act not in ACTIVATIONS:
+            raise NotImplementedError(f"activation {act!r}: the kernels implement 'silu', 'relu' and 'lrelu'")
         self.conv = nn.Conv2d(in_channels, out_channels, ksize, stride, (ksize - 1) // 2, groups=groups, bias=False)
         self.bn = nn.BatchNorm2d(out_channels)
-        self.act = nn.SiLU(inplace=True)
+        self.act = ACTIVATIONS[act]()
         self.ksize, self.stride, self.act_name = ksize, stride, act
 
     def forward(self, x):
@@ -43,8 +49,8 @@ class BaseConv(nn.Module):
 class DWConv(nn.Module):
     """[yolox] DWConv: depthwise k x k BaseConv (groups = in_channels) then 1x1 pointwise BaseConv.  Forward only (train-mode
     BatchNorm and eval): the depthwise half runs on sy_dwconv2d (coalesced CUDA-core kernel, HBM-bound), the pointwise half
-    on the tensor-core kernel.  The training backward (model/backward.py) does not cover depthwise layers -- no shipped cfg
-    sets depthwise=True."""
+    on the tensor-core kernel.  Both halves apply ``act`` (silu / relu / lrelu, see BaseConv).  The training backward
+    (model/backward.py) does not cover depthwise layers -- no shipped cfg sets depthwise=True."""
 
     def __init__(self, in_channels, out_channels, ksize, stride=1, act="silu"):
         super().__init__()
@@ -85,6 +91,8 @@ class CSPLayer(nn.Module):
 
 
 class Focus(nn.Module):
+    """[yolox] Focus: space-to-depth, then a 3x3 BaseConv with activation ``act`` (silu / relu / lrelu)."""
+
     def __init__(self, in_channels, out_channels, ksize=1, stride=1, act="silu"):
         super().__init__()
         if in_channels != 3 or ksize != 3 or stride != 1:
@@ -99,6 +107,9 @@ class Focus(nn.Module):
 
 
 class SPPBottleneck(nn.Module):
+    """[yolox] SPPBottleneck: conv1, max pools 5 / 9 / 13, conv2; both BaseConvs apply ``activation`` (silu / relu / lrelu),
+    which may differ from the rest of the network's ``act``."""
+
     def __init__(self, in_channels, out_channels, kernel_sizes=(5, 9, 13), activation="silu"):
         super().__init__()
         if tuple(kernel_sizes) != (5, 9, 13):

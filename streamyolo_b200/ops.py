@@ -14,6 +14,8 @@ LIB_PATH = os.path.join(_HERE, "lib", "libstreamyolo_sm100.so")
 SY_CONV_RAW, SY_CONV_FUSED = 0, 1
 SY_STORAGE_BF16, SY_STORAGE_F16 = 0, 1
 SY_PACK_F16 = 0x100
+SY_ACT_NONE, SY_ACT_SILU, SY_ACT_RELU, SY_ACT_LRELU = 0, 1, 2, 3
+ACT_CODES = {"silu": SY_ACT_SILU, "relu": SY_ACT_RELU, "lrelu": SY_ACT_LRELU}    # [yolox] act name -> the kernels' act code
 STORAGE = {torch.bfloat16: SY_STORAGE_BF16, torch.float16: SY_STORAGE_F16}    # activation dtype -> SyConvDesc.storage
 
 
