@@ -329,6 +329,12 @@ typedef struct SyHeadPredBwdDesc {
 } SyHeadPredBwdDesc;
 int sy_head_pred_bwd_rows(int32_t b, int32_t h, int32_t w);
 int sy_head_pred_backward(const SyHeadPredBwdDesc* d, sy_stream_t stream);
+/* The same backward for 1 <= num_classes <= 251 with (5 + num_classes) * c * 4 <= 200 KiB, the limits of
+ * sy_head_pred_decode (what the reference's TALHead / PIPEHead take, exps/model/tal_head.py:27, 101-131, 163-171, under
+ * loss.backward(), exps/train_utils/double_trainer.py:114).  Same descriptor, same partials (sy_head_pred_bwd_rows rows),
+ * fixed-order reduction: deterministic.  sy_head_pred_backward keeps its 27-class limit; the trainer uses this entry
+ * point above it. */
+int sy_head_pred_backward_wide(const SyHeadPredBwdDesc* d, sy_stream_t stream);
 
 /* Backward of the loss: what autograd computes for loss.backward() (exps/train_utils/double_trainer.py:114)
  * through TALHead.get_losses (exps/model/tal_head.py:426-461): the SimOTA assignment, the class targets and the

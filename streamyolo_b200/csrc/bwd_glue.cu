@@ -6,6 +6,8 @@
 //                           the destination pixels that read it (same fp32 index expression as the forward)
 //   * sy_head_pred_backward the three 1x1 prediction convs of a head level (tal_head.py:101-131): data gradient into the
 //                           cls / reg tower outputs, weight + bias gradients (two-stage, fixed-order reduction)
+//   * sy_head_pred_backward_wide    the same for any class count the forward takes (COCO's 80 included): shared-memory
+//                           weight tile, outputs tiled in groups of 32 so that no accumulator array grows with the class count
 #include <math.h>
 
 #include "common.cuh"
@@ -175,6 +177,138 @@ __global__ void head_pred_bwd_finalize_kernel(const float* __restrict__ partial,
   if (c < C) dst = (o < 4) ? dw_reg + (size_t)o * C + c : (o == 4 ? dw_obj + c : dw_cls + (size_t)(o - 5) * C + c);
   else dst = (o < 4) ? db_reg + o : (o == 4 ? db_obj : db_cls + (o - 5));
   *dst = accumulate ? *dst + s : s;
+}
+
+// ---- the same backward for any class count the forward takes (sy_head_pred_backward_wide): nothing grows with NO except
+// the grid.  The data gradient keeps the whole [NO][C] weight tile in shared memory (the forward's own limit,
+// (5 + nc) * C * 4 <= 200 KiB, sy_head_pred_decode) and gives each thread kWidePT pixels of one 8-channel chunk, so one
+// shared-memory read of eight weights serves kWidePT pixels; the sums run over o = 0 .. NO-1 in the order of
+// head_pred_bwd_data_kernel.
+constexpr int kWidePT = 2;            // pixels per thread of the data gradient
+constexpr int kWideOG = 32;           // outputs per block of the weight gradient
+__global__ void __launch_bounds__(256) head_pred_bwd_data_wide_kernel(const HeadBwdArgs q) {
+  extern __shared__ float wsm[];       // [NO][C]: reg(4), obj(1), cls(NO - 5)
+  const int NO = q.NO, C = q.C;
+  for (int i = threadIdx.x; i < NO * C; i += blockDim.x) {
+    const int o = i / C, c = i - o * C;
+    wsm[i] = (o < 4) ? q.w_reg[(size_t)o * C + c] : (o == 4 ? q.w_obj[c] : q.w_cls[(size_t)(o - 5) * C + c]);
+  }
+  __syncthreads();
+  const int G = C / 8;
+  const int HW = q.H * q.W;
+  const int npix = q.B * HW;
+  const int ppb = (int)blockDim.x / G;             // G <= 256 (C <= 2048, checked by the host)
+  const int prow = (int)threadIdx.x / G, cg = (int)threadIdx.x - prow * G;
+  if (prow >= ppb) return;
+  const int step = gridDim.x * ppb * kWidePT;
+  for (int pix0 = (blockIdx.x * ppb + prow) * kWidePT; pix0 < npix; pix0 += step) {
+    const float* g[kWidePT];
+#pragma unroll
+    for (int j = 0; j < kWidePT; ++j) {
+      const int pix = min(pix0 + j, npix - 1);     // past the end: recompute the last pixel, not stored
+      const int b = pix / HW;
+      g[j] = q.g + ((long long)b * q.a_total + q.anchor_offset + (pix - b * HW)) * NO;
+    }
+    float dr[kWidePT][8], dc[kWidePT][8];
+#pragma unroll
+    for (int j = 0; j < kWidePT; ++j)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) { dr[j][i] = 0.f; dc[j][i] = 0.f; }
+#pragma unroll
+    for (int o = 0; o < 5; ++o) {
+      const float4 w0 = *reinterpret_cast<const float4*>(wsm + o * C + cg * 8);
+      const float4 w1 = *reinterpret_cast<const float4*>(wsm + o * C + cg * 8 + 4);
+      const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+      for (int j = 0; j < kWidePT; ++j) {
+        const float gv = g[j][o];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) dr[j][i] += gv * w[i];
+      }
+    }
+    for (int o = 5; o < NO; ++o) {
+      const float4 w0 = *reinterpret_cast<const float4*>(wsm + o * C + cg * 8);
+      const float4 w1 = *reinterpret_cast<const float4*>(wsm + o * C + cg * 8 + 4);
+      const float w[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+      for (int j = 0; j < kWidePT; ++j) {
+        const float gv = g[j][o];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) dc[j][i] += gv * w[i];
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < kWidePT; ++j) {
+      if (pix0 + j >= npix) break;
+      const long long pix = pix0 + j;
+      *reinterpret_cast<uint4*>(q.drf + pix * q.drfp + cg * 8) =
+          make_uint4(pack_bf16(dr[j][0], dr[j][1]), pack_bf16(dr[j][2], dr[j][3]), pack_bf16(dr[j][4], dr[j][5]),
+                     pack_bf16(dr[j][6], dr[j][7]));
+      *reinterpret_cast<uint4*>(q.dcf + pix * q.dcfp + cg * 8) =
+          make_uint4(pack_bf16(dc[j][0], dc[j][1]), pack_bf16(dc[j][2], dc[j][3]), pack_bf16(dc[j][4], dc[j][5]),
+                     pack_bf16(dc[j][6], dc[j][7]));
+    }
+  }
+}
+
+// Weight gradient: block (x, y) = 256-pixel row x, outputs y * kWideOG ...; thread t owns channels t, t + 256, ... and
+// kWideOG accumulators whatever NO is.  partial[x][o][c] as head_pred_bwd_weight_kernel writes it: each sum runs over the
+// row's pixels in order, so head_pred_bwd_finalize_kernel's fixed-order reduction makes the result deterministic.
+__global__ void __launch_bounds__(256) head_pred_bwd_weight_wide_kernel(const HeadBwdArgs q) {
+  __shared__ __align__(16) float gsm[kHeadBwdPix][kWideOG];
+  const int NO = q.NO;
+  const int o0 = blockIdx.y * kWideOG;
+  const int no = min(kWideOG, NO - o0);
+  const long long npix = (long long)q.B * q.H * q.W;
+  const long long p0 = (long long)blockIdx.x * kHeadBwdPix;
+  const int np = (int)min((long long)kHeadBwdPix, npix - p0);
+  for (int i = threadIdx.x; i < np * kWideOG; i += blockDim.x) {
+    const int pp = i / kWideOG, o = i - pp * kWideOG;
+    const long long pix = p0 + pp;
+    const int b = (int)(pix / ((long long)q.H * q.W));
+    const long long a = (long long)b * q.a_total + q.anchor_offset + (pix - (long long)b * q.H * q.W);
+    gsm[pp][o] = o < no ? q.g[a * NO + o0 + o] : 0.f;
+  }
+  __syncthreads();
+  const int n_reg = max(0, min(5 - o0, kWideOG));  // outputs of this group that read the reg tower (group 0 only)
+  float* out = q.partial + (size_t)blockIdx.x * NO * (q.C + 1);
+  for (int c = threadIdx.x; c < q.C; c += blockDim.x) {
+    float acc[kWideOG];
+#pragma unroll
+    for (int o = 0; o < kWideOG; ++o) acc[o] = 0.f;
+    // eight pixels per pass, their feature loads issued before the first FMA (head_pred_bwd_weight_kernel)
+    constexpr int kPB = 8;
+    for (int pp = 0; pp < np; pp += kPB) {
+      float r[kPB], cv[kPB];
+#pragma unroll
+      for (int j = 0; j < kPB; ++j) {
+        const bool in = pp + j < np;
+        r[j] = in && n_reg > 0 ? __bfloat162float(q.rf[(p0 + pp + j) * q.rfp + c]) : 0.f;
+        cv[j] = in ? __bfloat162float(q.cf[(p0 + pp + j) * q.cfp + c]) : 0.f;
+      }
+#pragma unroll
+      for (int j = 0; j < kPB; ++j) {
+        if (pp + j < np) {
+          const float4* g4 = reinterpret_cast<const float4*>(gsm[pp + j]);
+#pragma unroll
+          for (int o4 = 0; o4 < kWideOG / 4; ++o4) {
+            const float4 gv = g4[o4];
+            const float gg[4] = {gv.x, gv.y, gv.z, gv.w};
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[4 * o4 + i] += gg[i] * (4 * o4 + i < n_reg ? r[j] : cv[j]);
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int o = 0; o < kWideOG; ++o)
+      if (o < no) out[(size_t)(o0 + o) * (q.C + 1) + c] = acc[o];
+  }
+  if (threadIdx.x < no) {              // bias gradient of this row
+    float s = 0.f;
+    for (int pp = 0; pp < np; ++pp) s += gsm[pp][threadIdx.x];
+    out[(size_t)(o0 + threadIdx.x) * (q.C + 1) + q.C] = s;
+  }
 }
 
 // y += x (bf16, fp32 add, one rounding): gradient accumulation where a tensor feeds several consumers (residual
@@ -377,6 +511,53 @@ extern "C" int sy_head_pred_backward(const SyHeadPredBwdDesc* d, sy_stream_t str
   head_pred_bwd_finalize_kernel<<<cdiv(n_out, 256), 256, 0, stream>>>(d->partials, rows, q.NO, f.c, d->dw_reg, d->dw_obj, d->dw_cls,
                                                                      d->db_reg, d->db_obj, d->db_cls, d->accumulate);
   return launch_status("head_pred_backward kernels");
+}
+
+extern "C" int sy_head_pred_backward_wide(const SyHeadPredBwdDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr, SY_EINVAL, "null descriptor");
+  const SyTensor& f = d->cls_feat;
+  SY_REQUIRE(view_ok(f) && view_ok(d->reg_feat) && view_ok(d->d_cls_feat) && view_ok(d->d_reg_feat), SY_EINVAL,
+             "head_pred_backward_wide: bad views");
+  SY_REQUIRE(d->reg_feat.n == f.n && d->reg_feat.h == f.h && d->reg_feat.w == f.w && d->reg_feat.c == f.c &&
+                 d->d_cls_feat.n == f.n && d->d_cls_feat.h == f.h && d->d_cls_feat.w == f.w && d->d_cls_feat.c == f.c &&
+                 d->d_reg_feat.n == f.n && d->d_reg_feat.h == f.h && d->d_reg_feat.w == f.w && d->d_reg_feat.c == f.c,
+             SY_EINVAL, "head_pred_backward_wide: shape mismatch");
+  SY_REQUIRE(d->num_classes >= 1 && d->num_classes <= 251, SY_EINVAL, "head_pred_backward_wide: num_classes out of range");
+  SY_REQUIRE(f.c % 8 == 0 && sizeof(float) * (5 + d->num_classes) * f.c <= 200 * 1024, SY_EINVAL,
+             "head_pred_backward_wide: %d channels x %d outputs do not fit the shared-memory weight tile", f.c,
+             5 + d->num_classes);
+  SY_REQUIRE(f.c <= 2048 && (long long)f.n * f.h * f.w <= (1ll << 30), SY_EINVAL,
+             "head_pred_backward_wide: %d channels / %d x %d x %d pixels unsupported", f.c, f.n, f.h, f.w);
+  SY_REQUIRE(d->grad_raw && d->w_reg && d->w_obj && d->w_cls && d->dw_reg && d->dw_obj && d->dw_cls && d->db_reg && d->db_obj &&
+                 d->db_cls && d->partials,
+             SY_EINVAL, "head_pred_backward_wide: null pointer");
+  SY_REQUIRE(d->anchor_offset >= 0 && d->anchor_offset + f.h * f.w <= d->a_total, SY_EINVAL,
+             "head_pred_backward_wide: anchor range");
+  const int rows = sy_head_pred_bwd_rows(f.n, f.h, f.w);
+  SY_REQUIRE(d->n_partials >= rows, SY_EWORKSPACE, "head_pred_backward_wide: %d partial rows, need %d", d->n_partials, rows);
+  HeadBwdArgs q{};
+  q.g = d->grad_raw;
+  q.cf = reinterpret_cast<const __nv_bfloat16*>(f.ptr); q.cfp = f.pitch;
+  q.rf = reinterpret_cast<const __nv_bfloat16*>(d->reg_feat.ptr); q.rfp = d->reg_feat.pitch;
+  q.w_reg = d->w_reg; q.w_obj = d->w_obj; q.w_cls = d->w_cls;
+  q.B = f.n; q.H = f.h; q.W = f.w; q.C = f.c; q.NO = 5 + d->num_classes; q.a_total = d->a_total; q.anchor_offset = d->anchor_offset;
+  q.dcf = reinterpret_cast<__nv_bfloat16*>(d->d_cls_feat.ptr); q.dcfp = d->d_cls_feat.pitch;
+  q.drf = reinterpret_cast<__nv_bfloat16*>(d->d_reg_feat.ptr); q.drfp = d->d_reg_feat.pitch;
+  q.partial = d->partials;
+  // data gradient: a resident grid (the weight tile is loaded once per block) walking groups of kWidePT pixels
+  const size_t smem = sizeof(float) * q.NO * f.c;
+  if (smem > 48 * 1024)
+    SY_CUDA(cudaFuncSetAttribute(head_pred_bwd_data_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const int per_sm = (int)((227 * 1024) / (smem + 1024));
+  const int groups = cdiv(f.n * f.h * f.w, kWidePT * (256 / (f.c / 8)));
+  const int blocks = min(groups, sm_count() * max(1, min(per_sm, 8)));
+  head_pred_bwd_data_wide_kernel<<<blocks, 256, smem, stream>>>(q);
+  head_pred_bwd_weight_wide_kernel<<<dim3(rows, cdiv(q.NO, kWideOG)), 256, 0, stream>>>(q);
+  const int n_out = q.NO * (f.c + 1);
+  head_pred_bwd_finalize_kernel<<<cdiv(n_out, 256), 256, 0, stream>>>(d->partials, rows, q.NO, f.c, d->dw_reg, d->dw_obj, d->dw_cls,
+                                                                     d->db_reg, d->db_obj, d->db_cls, d->accumulate);
+  return launch_status("head_pred_backward_wide kernels");
 }
 
 extern "C" int sy_add(SyTensor x, SyTensor y, sy_stream_t stream_) {

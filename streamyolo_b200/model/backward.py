@@ -328,18 +328,22 @@ def _one_zero(T, c):
     return cache[c]
 
 
+NARROW_HEAD_CLASSES = 27     # sy_head_pred_backward's register accumulators; above it sy_head_pred_backward_wide
+
+
 def _head_backward(T: Tape, head, r, grad_scale, sink):
     out, origin = r["out"], r["origin"]
     g_raw = torch.empty_like(out)
     ops.tal_loss_backward(out, origin, r["fut"], r["hw"], head.strides, float(head.gamma), True, r["ws"], grad_scale,
                           grad_raw=g_raw)
+    pred_backward = ops.head_pred_backward if head.num_classes <= NARROW_HEAD_CLASSES else ops.head_pred_backward_wide
     for k, cf, rf, off in r["levels"]:
         regp, objp, clsp = head.reg_preds[k], head.obj_preds[k], head.cls_preds[k]
         dws, dbs, acc = sink.head(head, k)
         gcf, grf = T.g(cf), T.g(rf)
         assert T.first(cf) and T.first(rf), "the prediction convs are the only consumers of the tower outputs"
-        ops.head_pred_backward(g_raw, cf, rf, gcf, grf, _f32(regp.weight), _f32(objp.weight), _f32(clsp.weight),
-                               r["a_total"], off, dws[0], dws[1], dws[2], dbs[0], dbs[1], dbs[2], accumulate=acc)
+        pred_backward(g_raw, cf, rf, gcf, grf, _f32(regp.weight), _f32(objp.weight), _f32(clsp.weight),
+                      r["a_total"], off, dws[0], dws[1], dws[2], dbs[0], dbs[1], dbs[2], accumulate=acc)
         sink.done([regp.weight, objp.weight, clsp.weight, regp.bias, objp.bias, clsp.bias])
 
 

@@ -13,7 +13,8 @@ from .network_blocks import BaseConv, DWConv
 
 
 MAX_NUM_CLASSES = 251     # sy_head_pred_decode: compiled instantiations for 8 / 1 / 20 classes, a generic kernel for any other count
-                          # (the reference head takes num_classes freely, tal_head.py:27); training backward: <= 27 classes
+                          # (the reference head takes num_classes freely, tal_head.py:27); the training backward takes the same
+                          # counts: sy_head_pred_backward up to 27 classes, sy_head_pred_backward_wide above (model/backward.py)
 
 
 class TALHead(nn.Module):

@@ -183,6 +183,7 @@ _SIG = {
     "sy_upsample_nearest_backward": (C.c_int, [SyTensor, SyTensor, C.c_void_p]),
     "sy_head_pred_bwd_rows": (C.c_int, [C.c_int32, C.c_int32, C.c_int32]),
     "sy_head_pred_backward": (C.c_int, [C.POINTER(SyHeadPredBwdDesc), C.c_void_p]),
+    "sy_head_pred_backward_wide": (C.c_int, [C.POINTER(SyHeadPredBwdDesc), C.c_void_p]),
     "sy_bn_act_bwd_rows": (C.c_int, [C.c_int32, C.c_int32]),
     "sy_bn_act_backward": (C.c_int, [C.POINTER(SyBnActBwdDesc), C.c_void_p]),
     "sy_postprocess_nms_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
@@ -638,6 +639,21 @@ def upsample_nearest_backward(dy: View, dx: View):
 
 def head_pred_backward(grad_raw, cls_feat: View, reg_feat: View, d_cls_feat: View, d_reg_feat: View, w_reg, w_obj, w_cls,
                        a_total, anchor_offset, dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate=False):
+    """Backward of one head level's three prediction convs, 1 <= classes <= 27 (sy_head_pred_backward)."""
+    _head_pred_bwd("sy_head_pred_backward", grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls,
+                   a_total, anchor_offset, dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate)
+
+
+def head_pred_backward_wide(grad_raw, cls_feat: View, reg_feat: View, d_cls_feat: View, d_reg_feat: View, w_reg, w_obj,
+                            w_cls, a_total, anchor_offset, dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate=False):
+    """The same for any class count the forward takes (sy_head_pred_backward_wide: 1 ... 251 classes, (5 + classes) x
+    channels x 4 bytes <= 200 KiB)."""
+    _head_pred_bwd("sy_head_pred_backward_wide", grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls,
+                   a_total, anchor_offset, dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate)
+
+
+def _head_pred_bwd(entry, grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls, a_total, anchor_offset,
+                   dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate):
     nc = w_cls.shape[0]
     rows = load_library().sy_head_pred_bwd_rows(cls_feat.n, cls_feat.h, cls_feat.w)
     partials = torch.empty((rows, (5 + nc) * (cls_feat.c + 1)), dtype=torch.float32, device=grad_raw.device)
@@ -649,7 +665,7 @@ def head_pred_backward(grad_raw, cls_feat: View, reg_feat: View, d_cls_feat: Vie
     d.dw_reg, d.dw_obj, d.dw_cls = dw_reg.data_ptr(), dw_obj.data_ptr(), dw_cls.data_ptr()
     d.db_reg, d.db_obj, d.db_cls = db_reg.data_ptr(), db_obj.data_ptr(), db_cls.data_ptr()
     d.accumulate, d.partials, d.n_partials = int(accumulate), partials.data_ptr(), rows
-    _check(lib().sy_head_pred_backward(C.byref(d), _stream()), kernels=3)
+    _check(getattr(lib(), entry)(C.byref(d), _stream()), kernels=3)
 
 
 def add_(x: View, y: View):
