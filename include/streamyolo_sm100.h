@@ -379,6 +379,19 @@ typedef struct SyNmsDesc {
 size_t sy_postprocess_nms_workspace_bytes(int32_t b, int32_t a_total);
 int sy_postprocess_nms(const SyNmsDesc* d, sy_stream_t stream);
 
+/* Per-stream gating of a batched streaming tick whose frames were decoded on the device (sy_jpeg_decode_sized): the
+ * driver's loop (sAP/streamyolo/streamyolo_det.py:150-195) only runs the model on a frame it has.  For every stream i,
+ * start[i] = (status[i] == SY_JPEG_OK && flags[i] != 0) and keep[i] = (status[i] == SY_JPEG_OK); status NULL counts every
+ * stream as decoded.  start feeds sy_select_images' first-frame choice and keep the buffer update, so a stream without a
+ * decoded frame keeps its carried features.  All arrays [n] int32 in device memory; no host synchronisation. */
+int sy_stream_gate(const int32_t* status, const int32_t* flags, int32_t n, int32_t* start, int32_t* keep, sy_stream_t stream);
+/* Per-stream box rescale of sy_postprocess_nms' rows, replacing the host's `detections[:, :4] / in_scale` of the driver's
+ * inference() (streamyolo_det.py:82) and the evaluators' `bboxes /= scale` (exps/evaluators/onex_stream_evaluator.py:182):
+ * det [n][max_det][7], rows < count[i] of stream i get x1, y1, x2, y2 divided by ratio[i] (fp32, IEEE division), and
+ * count[i] = 0 where status[i] != SY_JPEG_OK (status may be NULL). */
+int sy_stream_rescale(float* det, int32_t n, int32_t max_det, int32_t* count, const int32_t* status, const float* ratio,
+                      sy_stream_t stream);
+
 /* -------- training step glue (streamyolo_b200/csrc/train_glue.cu) ---------------------------------------------- */
 /* fp32 OIHW conv parameter -> bf16 GEMM operand, on the device (one launch per parameter per optimiser step):
  *   mode 0  out[o][r*kw+s][i] = w[o][i][r][s]                          forward B operand of sy_conv2d_tc
@@ -487,6 +500,20 @@ typedef struct SyLetterboxDesc {
   float* out;              /* [n][3][out_h][out_w] */
 } SyLetterboxDesc;
 int sy_letterbox(const SyLetterboxDesc* d, sy_stream_t stream);
+/* The same resize with a size per frame: frame k (uint8 BGR at the top-left of slot k of slot_h x slot_w, e.g. the output of
+ * sy_jpeg_decode_sized) of sizes[k] = (h, w, dst_h, dst_w) is resized h x w -> dst_h x dst_w (none when equal) with
+ * sy_letterbox's arithmetic and placed top-left on a canvas of 114: the evaluation preproc of data_augment_flip.py:151-167
+ * (dst = (int(h * r), int(w * r)), r = min(out_h / h, out_w / w)) or the driver's plain resize (dst = out) per stream.
+ * With every row equal to (h, w, dst_h, dst_w) the output is sy_letterbox's.  A row that does not fit the slot or the canvas
+ * leaves image k untouched. */
+typedef struct SyLetterboxSizedDesc {
+  const uint8_t* src;      /* [n][slot_h][slot_w][3] */
+  int32_t n, slot_h, slot_w;
+  const int32_t* sizes;    /* [n][4] device int32: h, w, dst_h, dst_w */
+  int32_t out_h, out_w;
+  float* out;              /* [n][3][out_h][out_w] */
+} SyLetterboxSizedDesc;
+int sy_letterbox_sized(const SyLetterboxSizedDesc* d, sy_stream_t stream);
 
 /* ---- JPEG decode ----
  * Batched decode of the training frames' JPEG files into what cv2.imread(path) returns for them (uint8 BGR, bit-identical),
@@ -522,6 +549,24 @@ typedef struct SyJpegDecodeDesc {
 } SyJpegDecodeDesc;
 size_t sy_jpeg_decode_workspace_bytes(int32_t n, int64_t max_bytes, int32_t h, int32_t w);
 int sy_jpeg_decode(const SyJpegDecodeDesc* d, sy_stream_t stream);
+/* The same decoder with a size per image, for camera streams of different sizes (the frames cv2.imread gives the driver's
+ * loop, sAP/streamyolo/streamyolo_det.py:176-181): image i must be sizes[i] = (h, w) with h <= max_h and w <= max_w, else
+ * it gets SY_JPEG_ESIZE and is left untouched; it is written at the top-left of slot i of out [n][max_h][max_w][3] (row
+ * pitch max_w * 3; the rest of the slot is not written).  The workspace is sized by the slot. */
+typedef struct SyJpegDecodeSizedDesc {
+  const uint8_t* bytes;     /* [n][max_bytes] file bytes, image i in the first lengths[i] bytes of row i */
+  const int32_t* lengths;   /* [n] device int32 */
+  int32_t n;
+  int64_t max_bytes;        /* row pitch of bytes (1 .. 2^28) */
+  const int32_t* sizes;     /* [n][2] device int32: the (h, w) image i must have */
+  int32_t max_h, max_w;     /* slot size */
+  uint8_t* out;             /* [n][max_h][max_w][3] BGR */
+  int32_t* status;          /* [n] device int32, SY_JPEG_* */
+  void* workspace;          /* sy_jpeg_decode_sized_workspace_bytes(n, max_bytes, max_h, max_w) bytes, 256-byte aligned */
+  size_t workspace_bytes;
+} SyJpegDecodeSizedDesc;
+size_t sy_jpeg_decode_sized_workspace_bytes(int32_t n, int64_t max_bytes, int32_t max_h, int32_t max_w);
+int sy_jpeg_decode_sized(const SyJpegDecodeSizedDesc* d, sy_stream_t stream);
 
 #ifdef __cplusplus
 }

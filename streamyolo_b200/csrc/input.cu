@@ -7,6 +7,8 @@
 //                      mirror, the 114 pad and HWC uint8 -> CHW fp32; optionally preceded by load_resized_img's resize
 //                      (tal_flip_one_future_argoversedataset.py:179-187).  With no pad and no flags it is the streaming
 //                      driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60).
+//   * sy_letterbox_sized  the same resize with a source size and a resized extent per frame, the frames in slots of one
+//                      size: the evaluation preproc (data_augment_flip.py:151-167) of camera streams of different sizes.
 // Built with -fmad=false: the tap positions (x + 0.5) * scale - 0.5 and the fp64 label arithmetic must round every
 // operation separately, as OpenCV and numpy do.  The output is then bit-identical to cv2 / numpy.
 #include <math.h>
@@ -67,25 +69,12 @@ __device__ __forceinline__ void stage1_px(const uint8_t* __restrict__ img, const
   }
 }
 
-// One thread per output pixel (three planes): blockIdx.z = frame, blockIdx.y = output row, x along the row (coalesced fp32
-// stores, no index divisions).  Value at (y, x) of the dst_h x dst_w region: stage b applied to the (mirrored) first-stage
-// image, or, without a second stage, the first-stage image at the mirrored column.  Outside the region: 114.
+// Value at (y, x) of the dst region of one frame: stage b applied to the (mirrored) first-stage image, or, without a
+// second stage, the first-stage image at the mirrored column.  Shared by letterbox_kernel and letterbox_sized_kernel.
 template <bool FIRST, bool SECOND>
-__global__ void __launch_bounds__(128) letterbox_kernel(const uint8_t* __restrict__ src, ResizeStage a, ResizeStage b,
-                                                        int out_h, int out_w, const int32_t* __restrict__ flags,
-                                                        float* __restrict__ out) {
-  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, k = blockIdx.z;
-  if (x >= out_w) return;
-  const long long plane = (long long)out_h * out_w;
-  float* o = out + 3 * plane * k + (long long)y * out_w + x;
-  if (y >= b.dst_h || x >= b.dst_w) {
-    o[0] = o[plane] = o[2 * plane] = (float)kPadValue;
-    return;
-  }
-  const uint8_t* img = src + (long long)a.src_h * a.src_w * 3 * k;
-  const bool mir = flags != nullptr && flags[k] != 0;
+__device__ __forceinline__ void letterbox_px(const uint8_t* __restrict__ img, const ResizeStage& a, const ResizeStage& b,
+                                             bool mir, int y, int x, int p[3]) {
   const int mid_w = b.src_w;                       // width of the first-stage image (the mirror axis)
-  int p[3];
   if constexpr (!SECOND) {
     stage1_px<FIRST>(img, a, y, mir ? mid_w - 1 - x : x, p);
   } else {
@@ -101,6 +90,53 @@ __global__ void __launch_bounds__(128) letterbox_kernel(const uint8_t* __restric
 #pragma unroll
     for (int ch = 0; ch < 3; ++ch) p[ch] = vmix(p00[ch] * a0 + p01[ch] * a1, p10[ch] * a0 + p11[ch] * a1, b0, b1);
   }
+}
+
+// One thread per output pixel (three planes): blockIdx.z = frame, blockIdx.y = output row, x along the row (coalesced fp32
+// stores, no index divisions).  Inside the dst_h x dst_w region: letterbox_px.  Outside: 114.
+template <bool FIRST, bool SECOND>
+__global__ void __launch_bounds__(128) letterbox_kernel(const uint8_t* __restrict__ src, ResizeStage a, ResizeStage b,
+                                                        int out_h, int out_w, const int32_t* __restrict__ flags,
+                                                        float* __restrict__ out) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, k = blockIdx.z;
+  if (x >= out_w) return;
+  const long long plane = (long long)out_h * out_w;
+  float* o = out + 3 * plane * k + (long long)y * out_w + x;
+  if (y >= b.dst_h || x >= b.dst_w) {
+    o[0] = o[plane] = o[2 * plane] = (float)kPadValue;
+    return;
+  }
+  const uint8_t* img = src + (long long)a.src_h * a.src_w * 3 * k;
+  const bool mir = flags != nullptr && flags[k] != 0;
+  int p[3];
+  letterbox_px<FIRST, SECOND>(img, a, b, mir, y, x, p);
+  o[0] = (float)p[0];
+  o[plane] = (float)p[1];
+  o[2 * plane] = (float)p[2];
+}
+
+// The same per frame k of slots of slot_h x slot_w: sizes[k] = (h, w, dst_h, dst_w), the frame at the slot's top-left, its
+// resize to dst_h x dst_w (none when equal) and the 114 pad.  The tap scales are OpenCV's 1 / (dst / src), in fp64 as the
+// host computes them for sy_letterbox.  A row that does not fit the slot or the canvas leaves image k untouched.
+__global__ void __launch_bounds__(128) letterbox_sized_kernel(const uint8_t* __restrict__ src, int slot_h, int slot_w,
+                                                              const int32_t* __restrict__ sizes, int out_h, int out_w,
+                                                              float* __restrict__ out) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, k = blockIdx.z;
+  if (x >= out_w) return;
+  const int h = sizes[4 * k], w = sizes[4 * k + 1], dh = sizes[4 * k + 2], dw = sizes[4 * k + 3];
+  if (h < 1 || w < 1 || h > slot_h || w > slot_w || dh < 1 || dw < 1 || dh > out_h || dw > out_w) return;
+  const long long plane = (long long)out_h * out_w;
+  float* o = out + 3 * plane * k + (long long)y * out_w + x;
+  if (y >= dh || x >= dw) {
+    o[0] = o[plane] = o[2 * plane] = (float)kPadValue;
+    return;
+  }
+  const ResizeStage a{h, slot_w, h, w, 1.0, 1.0};  // no first stage: only the row pitch (slot_w pixels) is read
+  const ResizeStage b{h, w, dh, dw, 1.0 / ((double)dh / h), 1.0 / ((double)dw / w)};
+  const uint8_t* img = src + (long long)slot_h * slot_w * 3 * k;
+  int p[3];
+  if (dh != h || dw != w) letterbox_px<false, true>(img, a, b, false, y, x, p);
+  else letterbox_px<false, false>(img, a, b, false, y, x, p);
   o[0] = (float)p[0];
   o[plane] = (float)p[1];
   o[2 * plane] = (float)p[2];
@@ -227,4 +263,16 @@ extern "C" int sy_letterbox(const SyLetterboxDesc* d, sy_stream_t stream_) {
                  : (second ? letterbox_kernel<false, true> : letterbox_kernel<false, false>);
   k<<<grid, 128, 0, stream>>>(d->src, a, b, d->out_h, d->out_w, d->flags, d->out);
   return launch_status("letterbox_kernel");
+}
+
+extern "C" int sy_letterbox_sized(const SyLetterboxSizedDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr && d->src != nullptr && d->sizes != nullptr && d->out != nullptr, SY_EINVAL,
+             "letterbox_sized: null pointer");
+  SY_REQUIRE(d->n > 0 && d->n <= 65535 && d->slot_h > 0 && d->slot_w > 0 && d->out_h > 0 && d->out_w > 0 &&
+                 d->out_h <= 65535, SY_EINVAL, "letterbox_sized: bad sizes");
+  SY_REQUIRE((long long)d->slot_h * d->slot_w * 3 < (1ll << 31), SY_EINVAL, "letterbox_sized: slot too large");
+  const dim3 grid(cdiv(d->out_w, 128), d->out_h, d->n);
+  letterbox_sized_kernel<<<grid, 128, 0, stream>>>(d->src, d->slot_h, d->slot_w, d->sizes, d->out_h, d->out_w, d->out);
+  return launch_status("letterbox_sized_kernel");
 }

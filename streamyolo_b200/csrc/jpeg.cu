@@ -17,6 +17,9 @@
 //   5. jpeg_color_kernel     jdsample.c's chroma upsampling ("fancy" triangle filter for 2x1 / 2x2, plain replication when
 //                            the chroma plane is at most 2 samples wide) and jdcolor.c's fixed-point YCbCr -> BGR; it also
 //                            publishes each image's status.
+// sy_jpeg_decode gives every image the batch's size; sy_jpeg_decode_sized gives image i its own expected size and a slot of
+// max_h x max_w in the output.  Both run the same five kernels: each image's MCU geometry, restart bookkeeping, upsampling
+// and colour conversion read the size stored in its JpegImage by the parse.
 // oracle/jpeg_oracle.py restates every stage in numpy; tests/test_jpeg_decode.py pins it to cv2.imdecode.
 #include <cooperative_groups.h>
 #include <cub/block/block_scan.cuh>
@@ -45,6 +48,7 @@ struct HuffTab {
 
 struct JpegImage {
   int32_t status, done;
+  int32_t h, w;         // the image's own size (SOF)
   int32_t h0, v0, mcux, mcuy, bpm, total_blocks;
   int32_t ri, n_units, unit_bits, ecs_bits;
   int32_t scan_begin;
@@ -124,8 +128,11 @@ __device__ bool build_huff(HuffTab* t, const uint8_t* counts, const uint8_t* val
   return true;
 }
 
+// h x w: the size every image must have, or with ``sizes`` the output slot, and image i must be sizes[i] = (h_i, w_i) and
+// fit the slot
 __global__ void __launch_bounds__(32) jpeg_parse_kernel(const uint8_t* __restrict__ bytes, const int32_t* __restrict__ lengths,
-                                                        int64_t max_bytes, int h, int w, uint8_t* ws, Layout L) {
+                                                        int64_t max_bytes, int h, int w, const int32_t* __restrict__ sizes,
+                                                        uint8_t* ws, Layout L) {
   if (threadIdx.x != 0) return;
   const int i = blockIdx.x;
   JpegImage* im = image_of(ws, L, i);
@@ -218,7 +225,9 @@ __global__ void __launch_bounds__(32) jpeg_parse_kernel(const uint8_t* __restric
     }
     // APPn, COM and other segments: skipped
   }
-  if (ih != h || iw != w) return finish(SY_JPEG_ESIZE);
+  const int eh = sizes != nullptr ? sizes[2 * i] : h, ew = sizes != nullptr ? sizes[2 * i + 1] : w;
+  if (ih != eh || iw != ew || ih > h || iw > w) return finish(SY_JPEG_ESIZE);
+  im->h = ih, im->w = iw;
   im->h0 = ch[0], im->v0 = cv[0];
   im->mcux = cdiv(iw, 8 * ch[0]), im->mcuy = cdiv(ih, 8 * cv[0]);
   im->bpm = ch[0] * cv[0] + 2;
@@ -633,12 +642,15 @@ __device__ __forceinline__ int chroma(const uint8_t* __restrict__ p, int cw, int
   return (3 * near + far + (odd ? 7 : 8)) >> 4;
 }
 
-__global__ void __launch_bounds__(128) jpeg_color_kernel(uint8_t* ws, Layout L, int h, int w, uint8_t* __restrict__ out,
-                                                          int32_t* __restrict__ status) {
+// out: slots of slot_h x slot_w pixels, image img top-left in slot img
+__global__ void __launch_bounds__(128) jpeg_color_kernel(uint8_t* ws, Layout L, int slot_h, int slot_w,
+                                                          uint8_t* __restrict__ out, int32_t* __restrict__ status) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, img = blockIdx.z;
   const JpegImage* im = image_of(ws, L, img);
   if (x == 0 && y == 0) status[img] = im->status;
-  if (x >= w || im->status != SY_JPEG_OK) return;
+  if (im->status != SY_JPEG_OK) return;
+  const int h = im->h, w = im->w;
+  if (x >= w || y >= h) return;
   const int h0 = im->h0, v0 = im->v0, mcux = im->mcux;
   const uint8_t* planes = ws + L.image_stride * img + L.off_planes;
   const int yw = mcux * h0 * 8, yh = im->mcuy * v0 * 8, cw = mcux * 8, chh = im->mcuy * 8;
@@ -649,7 +661,7 @@ __global__ void __launch_bounds__(128) jpeg_color_kernel(uint8_t* ws, Layout L, 
   const int R = Y + ((91881 * cr + 32768) >> 16);
   const int G = Y + ((-22554 * cb + 32768 - 46802 * cr) >> 16);
   const int B = Y + ((116130 * cb + 32768) >> 16);
-  uint8_t* o = out + (((size_t)img * h + y) * w + x) * 3;
+  uint8_t* o = out + (((size_t)img * slot_h + y) * slot_w + x) * 3;
   o[0] = (uint8_t)min(max(B, 0), 255);
   o[1] = (uint8_t)min(max(G, 0), 255);
   o[2] = (uint8_t)min(max(R, 0), 255);
@@ -675,6 +687,24 @@ Layout make_layout(int64_t max_bytes, int h, int w) {
   return L;
 }
 
+// the five kernels over n images in slots of h x w (sizes: each image's own size, or NULL for h x w)
+int jpeg_launch(const uint8_t* bytes, const int32_t* lengths, int n, int64_t max_bytes, int h, int w, const int32_t* sizes,
+                uint8_t* out, int32_t* status, void* workspace, cudaStream_t stream) {
+  const Layout L = make_layout(max_bytes, h, w);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  jpeg_parse_kernel<<<n, 32, 0, stream>>>(bytes, lengths, max_bytes, h, w, sizes, ws, L);
+  SY_CUDA(cudaGetLastError());
+  jpeg_ecs_kernel<<<n, kEcsThreads, 0, stream>>>(bytes, lengths, max_bytes, ws, L);
+  SY_CUDA(cudaGetLastError());
+  jpeg_huffman_kernel<<<dim3(kClusterCtas, n), kHuffThreads, 0, stream>>>(ws, L);
+  SY_CUDA(cudaGetLastError());
+  const int max_blocks = (int)((L.off_planes - L.off_coef) / 128);
+  jpeg_idct_kernel<<<dim3(cdiv(max_blocks, kIdctBlocksPerCta), n), 8 * kIdctBlocksPerCta, 0, stream>>>(ws, L);
+  SY_CUDA(cudaGetLastError());
+  jpeg_color_kernel<<<dim3(cdiv(w, 128), h, n), 128, 0, stream>>>(ws, L, h, w, out, status);
+  return launch_status("jpeg_color_kernel");
+}
+
 }  // namespace
 }  // namespace sy
 
@@ -695,17 +725,24 @@ extern "C" int sy_jpeg_decode(const SyJpegDecodeDesc* d, sy_stream_t stream_) {
   const size_t need = sy_jpeg_decode_workspace_bytes(d->n, d->max_bytes, d->h, d->w);
   SY_REQUIRE(d->workspace_bytes >= need && ((uintptr_t)d->workspace % 256) == 0, SY_EINVAL,
              "jpeg_decode: workspace of %zu bytes (need %zu, 256-byte aligned)", d->workspace_bytes, need);
-  const Layout L = make_layout(d->max_bytes, d->h, d->w);
-  uint8_t* ws = static_cast<uint8_t*>(d->workspace);
-  jpeg_parse_kernel<<<d->n, 32, 0, stream>>>(d->bytes, d->lengths, d->max_bytes, d->h, d->w, ws, L);
-  SY_CUDA(cudaGetLastError());
-  jpeg_ecs_kernel<<<d->n, kEcsThreads, 0, stream>>>(d->bytes, d->lengths, d->max_bytes, ws, L);
-  SY_CUDA(cudaGetLastError());
-  jpeg_huffman_kernel<<<dim3(kClusterCtas, d->n), kHuffThreads, 0, stream>>>(ws, L);
-  SY_CUDA(cudaGetLastError());
-  const int max_blocks = (int)((L.off_planes - L.off_coef) / 128);
-  jpeg_idct_kernel<<<dim3(cdiv(max_blocks, kIdctBlocksPerCta), d->n), 8 * kIdctBlocksPerCta, 0, stream>>>(ws, L);
-  SY_CUDA(cudaGetLastError());
-  jpeg_color_kernel<<<dim3(cdiv(d->w, 128), d->h, d->n), 128, 0, stream>>>(ws, L, d->h, d->w, d->out, d->status);
-  return launch_status("jpeg_color_kernel");
+  return jpeg_launch(d->bytes, d->lengths, d->n, d->max_bytes, d->h, d->w, nullptr, d->out, d->status, d->workspace, stream);
+}
+
+extern "C" size_t sy_jpeg_decode_sized_workspace_bytes(int32_t n, int64_t max_bytes, int32_t max_h, int32_t max_w) {
+  return sy_jpeg_decode_workspace_bytes(n, max_bytes, max_h, max_w);
+}
+
+extern "C" int sy_jpeg_decode_sized(const SyJpegDecodeSizedDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr && d->bytes != nullptr && d->lengths != nullptr && d->sizes != nullptr && d->out != nullptr &&
+                 d->status != nullptr && d->workspace != nullptr, SY_EINVAL, "jpeg_decode_sized: null pointer");
+  SY_REQUIRE(d->n > 0 && d->n <= 65535 && d->max_bytes > 0 && d->max_bytes <= (1ll << 28) && d->max_h > 0 &&
+                 d->max_w > 0 && d->max_h <= 65535 && d->max_w <= 65535, SY_EINVAL,
+             "jpeg_decode_sized: bad sizes (n %d, max_bytes %lld, slot %dx%d)", d->n, (long long)d->max_bytes, d->max_h,
+             d->max_w);
+  const size_t need = sy_jpeg_decode_sized_workspace_bytes(d->n, d->max_bytes, d->max_h, d->max_w);
+  SY_REQUIRE(d->workspace_bytes >= need && ((uintptr_t)d->workspace % 256) == 0, SY_EINVAL,
+             "jpeg_decode_sized: workspace of %zu bytes (need %zu, 256-byte aligned)", d->workspace_bytes, need);
+  return jpeg_launch(d->bytes, d->lengths, d->n, d->max_bytes, d->max_h, d->max_w, d->sizes, d->out, d->status,
+                     d->workspace, stream);
 }

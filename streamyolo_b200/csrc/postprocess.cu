@@ -193,6 +193,38 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
   if (tid == 0) q.count[b] = base < q.max_det ? base : q.max_det;
 }
 
+// Per-stream gating of a streaming tick (see sy_stream_gate): a stream whose frame did not decode starts nothing and
+// keeps its buffer.
+__global__ void __launch_bounds__(128) stream_gate_kernel(const int32_t* __restrict__ status,
+                                                          const int32_t* __restrict__ flags, int n,
+                                                          int32_t* __restrict__ start, int32_t* __restrict__ keep) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const bool ok = status == nullptr || status[i] == SY_JPEG_OK;
+  start[i] = ok && flags[i] != 0;
+  keep[i] = ok;
+}
+
+// One CTA per stream: the boxes of its count rows / ratio (IEEE fp32 division, as numpy divides the float32 rows by the
+// ratio), or no rows when its frame did not decode.
+__global__ void __launch_bounds__(128) stream_rescale_kernel(float* __restrict__ det, int max_det, int32_t* __restrict__ count,
+                                                             const int32_t* __restrict__ status,
+                                                             const float* __restrict__ ratio) {
+  const int b = blockIdx.x;
+  const int n = min(max(count[b], 0), max_det);
+  __syncthreads();                                 // every thread has read count[b] before thread 0 may clear it
+  if (status != nullptr && status[b] != SY_JPEG_OK) {
+    if (threadIdx.x == 0) count[b] = 0;
+    return;
+  }
+  const float r = ratio[b];
+  float* rows = det + (size_t)b * max_det * 7;
+  for (int e = threadIdx.x; e < 4 * n; e += blockDim.x) {
+    float* v = rows + (e >> 2) * 7 + (e & 3);
+    *v = __fdiv_rn(*v, r);
+  }
+}
+
 static inline size_t nms_ws_bytes(int B, int A) { return ((size_t)B * A * 4 * sizeof(float) + 255) / 256 * 256 + (size_t)B * A * sizeof(int); }
 
 }  // namespace sy
@@ -225,4 +257,22 @@ extern "C" int sy_postprocess_nms(const SyNmsDesc* d, sy_stream_t stream_) {
   q.det = d->det_out; q.count = d->count_out;
   nms_kernel<<<d->b, kNmsThreads, smem, stream>>>(q);
   return launch_status("nms_kernel");
+}
+
+extern "C" int sy_stream_gate(const int32_t* status, const int32_t* flags, int32_t n, int32_t* start, int32_t* keep,
+                              sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(flags != nullptr && start != nullptr && keep != nullptr, SY_EINVAL, "stream_gate: null pointer");
+  SY_REQUIRE(n > 0, SY_EINVAL, "stream_gate: %d streams", n);
+  stream_gate_kernel<<<cdiv(n, 128), 128, 0, stream>>>(status, flags, n, start, keep);
+  return launch_status("stream_gate_kernel");
+}
+
+extern "C" int sy_stream_rescale(float* det, int32_t n, int32_t max_det, int32_t* count, const int32_t* status,
+                                 const float* ratio, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(det != nullptr && count != nullptr && ratio != nullptr, SY_EINVAL, "stream_rescale: null pointer");
+  SY_REQUIRE(n > 0 && n <= 65535 && max_det > 0, SY_EINVAL, "stream_rescale: bad sizes (%d streams, max_det %d)", n, max_det);
+  stream_rescale_kernel<<<n, 128, 0, stream>>>(det, max_det, count, status, ratio);
+  return launch_status("stream_rescale_kernel");
 }

@@ -3,7 +3,8 @@
 ``pair_transform`` = DoubleTrainTransform(max_labels, hsv=False, flip) / DoubleValTransform
 (/root/reference/exps/data/data_augment_flip.py:141-234) for a batch of frame pairs, ``frame_transform`` =
 TrainTransform / ValTransform (:170-263) for a batch of single frames, ``stream_frame`` = the streaming
-driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60, 176-181).  Both are bit-identical to the cv2 / numpy host code
+driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60, 176-181), ``stream_frames_sized`` the same for frames of
+different sizes (the evaluation preproc, data_augment_flip.py:151-167, per frame).  They are bit-identical to the cv2 / numpy host code
 they replace (sy_pair_labels, sy_frame_labels, sy_letterbox); INTEGRATION.md shows where they plug in.
 """
 import numpy as np
@@ -138,6 +139,58 @@ def stream_frame(frame, size=(600, 960), out=None):
     return out
 
 
+def _sizes_list(sizes, who):
+    """``sizes`` ([(h, w), ...] or an int [n, 2] array) as a list of int pairs, each at least 1x1"""
+    out = [tuple(int(v) for v in s) for s in np.asarray(sizes).reshape(-1, 2).tolist()]
+    ops._require(len(out) > 0 and all(h >= 1 and w >= 1 for h, w in out), f"{who}: sizes must be (h, w) pairs of at least 1")
+    return out
+
+
+def sized_table(sizes, input_size, in_scale=None):
+    """The per-frame transform of frames of different sizes into one ``input_size`` (H, W) model input.
+
+    A frame whose driver size (int(h * in_scale), int(w * in_scale)) is ``input_size`` gets the streaming driver's plain
+    resize to H x W and the ratio ``in_scale`` (streamyolo_det.py:57-60, 176-181, 82); every other frame (all of them without
+    ``in_scale``) the evaluation preproc: r = min(H / h, W / w), a resize to (int(h * r), int(w * r)) and the 114 pad, with
+    the ratio r its boxes are divided by (data_augment_flip.py:151-167, onex_stream_evaluator.py:182).
+
+    -> (int32 numpy [n, 4] rows h, w, dst_h, dst_w -- sy_letterbox_sized's table -- and the n ratios as Python floats)."""
+    rows, ratios = [], []
+    for h, w in _sizes_list(sizes, "sized_table"):
+        if in_scale is not None and (int(h * in_scale), int(w * in_scale)) == tuple(input_size):
+            r, dst = in_scale, tuple(input_size)
+        else:
+            r, dst = _fit(h, w, input_size)
+        ops._require(min(dst) >= 1, f"sized_table: a {h}x{w} frame fitted into {tuple(input_size)} is empty")
+        rows.append((h, w, dst[0], dst[1]))
+        ratios.append(r)
+    return np.array(rows, np.int32), ratios
+
+
+def stream_frames_sized(frames, sizes, input_size, out=None, in_scale=None):
+    """``preproc`` per frame for frames of different sizes (sy_letterbox_sized).
+
+    frames  uint8 CUDA [n, max_h, max_w, 3] slots (decode_jpeg_sized's output): frame i BGR at the top-left of slot i
+    sizes   the n frames' (h, w), each within the slot
+    in_scale  with it, a frame of driver size ``input_size`` takes the driver's plain resize (see sized_table)
+
+    -> ``(x, ratios)``: x fp32 [n, 3, H, W], what ``preproc(frame_i, input_size)`` gives with the 114 pad, and each frame's
+    ratio (the r its boxes are divided by)."""
+    sizes = _sizes_list(sizes, "stream_frames_sized")
+    ops._require(torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+                 and frames.is_contiguous() and frames.shape[0] == len(sizes),
+                 f"stream_frames_sized: frames must be contiguous uint8 [{len(sizes)}, max_h, max_w, 3]")
+    n, sh, sw, _ = frames.shape
+    for i, (h, w) in enumerate(sizes):
+        ops._require(h <= sh and w <= sw, f"stream_frames_sized: frame {i} of {h}x{w} is larger than the {sh}x{sw} slot")
+    table, ratios = sized_table(sizes, input_size, in_scale)
+    if out is None:
+        out = torch.empty((n, 3, input_size[0], input_size[1]), dtype=torch.float32, device=frames.device)
+    ops._require(tuple(out.shape) == (n, 3, input_size[0], input_size[1]), "stream_frames_sized: out must be [n, 3, H, W]")
+    ops.letterbox_sized(frames, torch.from_numpy(table).to(frames.device), out)
+    return out, ratios
+
+
 def pack_jpeg(files, max_bytes):
     """Host side of device JPEG decoding: the file contents ``files`` (``bytes`` or uint8 numpy arrays, e.g.
     ``np.fromfile(path, np.uint8)``) -> (uint8 [N, max_bytes] zero-padded rows, int32 [N] lengths), both numpy, for the
@@ -193,3 +246,43 @@ def check_jpeg_status(status):
     for i, s in enumerate(st):
         if s != 0:
             raise RuntimeError(f"decode_jpeg: frame {i} did not decode: {JPEG_STATUS.get(s, f'status {s}')}")
+
+
+def decode_jpeg_sized(streams, lengths, sizes, max_hw, out=None, status=None, workspace=None):
+    """Decode a batch of JPEG files of different sizes on the device (sy_jpeg_decode_sized).
+
+    streams, lengths  as decode_jpeg
+    sizes     the (h, w) each frame must have: host pairs (checked against ``max_hw`` here) or an int32 CUDA [N, 2] tensor
+              (static for CUDA-graph capture; a frame larger than the slot then gets status 4)
+    max_hw    (max_h, max_w) of the output slots
+    out, status, workspace   uint8 [N, max_h, max_w, 3], int32 [N] and the workspace to write into, as decode_jpeg
+
+    -> ``(frames, status)``: frame i what cv2.imread returns for file i, at the top-left of slot i (the rest of the slot is
+    not written); status as decode_jpeg.  Nothing is read back."""
+    mh, mw = (int(v) for v in max_hw)
+    if not torch.is_tensor(sizes):
+        hw = _sizes_list(sizes, "decode_jpeg_sized")
+        for i, (h, w) in enumerate(hw):
+            ops._require(h <= mh and w <= mw, f"decode_jpeg_sized: frame {i} of {h}x{w} is larger than the {mh}x{mw} slot")
+        sizes = torch.tensor(hw, dtype=torch.int32)
+    ops._require(sizes.dtype == torch.int32 and tuple(sizes.shape) == (sizes.shape[0], 2),
+                 "decode_jpeg_sized: sizes must be int32 [N, 2]")
+    ops._require(torch.is_tensor(streams) and streams.dim() == 2 and streams.dtype == torch.uint8 and streams.is_cuda,
+                 "decode_jpeg_sized: streams must be a CUDA uint8 [N, max_bytes] tensor")
+    n, max_bytes = streams.shape
+    ops._require(sizes.shape[0] == n, f"decode_jpeg_sized: {sizes.shape[0]} sizes for {n} files")
+    dev = streams.device
+    sizes = sizes.to(dev)
+    if out is None:
+        out = torch.empty((n, mh, mw, 3), dtype=torch.uint8, device=dev)
+    if status is None:
+        status = torch.empty((n,), dtype=torch.int32, device=dev)
+    ops._require(tuple(out.shape) == (n, mh, mw, 3), f"decode_jpeg_sized: out must be [{n}, {mh}, {mw}, 3]")
+    if workspace is None:
+        key = (dev, n, max_bytes, mh, mw)
+        if key not in _JPEG_WS:
+            _JPEG_WS[key] = torch.empty(ops.jpeg_decode_sized_workspace_bytes(n, max_bytes, mh, mw), dtype=torch.uint8,
+                                        device=dev)
+        workspace = _JPEG_WS[key]
+    ops.jpeg_decode_sized(streams, lengths, sizes, out, status, workspace)
+    return out, status

@@ -141,6 +141,17 @@ class SyJpegDecodeDesc(C.Structure):
                 ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
+class SyJpegDecodeSizedDesc(C.Structure):
+    _fields_ = [("bytes", C.c_void_p), ("lengths", C.c_void_p), ("n", C.c_int32), ("max_bytes", C.c_int64),
+                ("sizes", C.c_void_p), ("max_h", C.c_int32), ("max_w", C.c_int32), ("out", C.c_void_p),
+                ("status", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
+class SyLetterboxSizedDesc(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("n", C.c_int32), ("slot_h", C.c_int32), ("slot_w", C.c_int32),
+                ("sizes", C.c_void_p), ("out_h", C.c_int32), ("out_w", C.c_int32), ("out", C.c_void_p)]
+
+
 class SySelectImagesDesc(C.Structure):
     _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
 
@@ -188,6 +199,8 @@ _SIG = {
     "sy_bn_act_backward": (C.c_int, [C.POINTER(SyBnActBwdDesc), C.c_void_p]),
     "sy_postprocess_nms_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "sy_postprocess_nms": (C.c_int, [C.POINTER(SyNmsDesc), C.c_void_p]),
+    "sy_stream_gate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sy_stream_rescale": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sy_conv2d_wgrad_workspace_bytes": (C.c_size_t, [C.POINTER(SyConvWgradDesc)]),
     "sy_conv2d_wgrad_tc": (C.c_int, [C.POINTER(SyConvWgradDesc), C.c_void_p]),
     "sy_pack_conv_weight": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
@@ -201,8 +214,11 @@ _SIG = {
     "sy_pair_labels": (C.c_int, [C.POINTER(SyPairLabelsDesc), C.c_void_p]),
     "sy_frame_labels": (C.c_int, [C.POINTER(SyFrameLabelsDesc), C.c_void_p]),
     "sy_letterbox": (C.c_int, [C.POINTER(SyLetterboxDesc), C.c_void_p]),
+    "sy_letterbox_sized": (C.c_int, [C.POINTER(SyLetterboxSizedDesc), C.c_void_p]),
     "sy_jpeg_decode_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
     "sy_jpeg_decode": (C.c_int, [C.POINTER(SyJpegDecodeDesc), C.c_void_p]),
+    "sy_jpeg_decode_sized_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
+    "sy_jpeg_decode_sized": (C.c_int, [C.POINTER(SyJpegDecodeSizedDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
 
@@ -493,6 +509,29 @@ def select_images(srcs, dsts, flags):
         d.src[k], d.dst[k] = s.st(), t.st()
     d.n_pairs, d.flags = len(srcs), flags.data_ptr()
     _check(lib().sy_select_images(C.byref(d), _stream()))
+
+
+def stream_gate(status, flags, start, keep):
+    """start[i] = flags[i] != 0 and status[i] == 0, keep[i] = status[i] == 0 (sy_stream_gate): int32 [n] device arrays;
+    ``status`` None counts every stream as decoded."""
+    n = flags.numel()
+    for name, t in (("flags", flags), ("start", start), ("keep", keep)) + ((("status", status),) if status is not None else ()):
+        _require(_tensor_ok(t, torch.int32, 1) and t.numel() == n and t.is_cuda, f"stream_gate: {name} must be CUDA int32 [n]")
+    _check(lib().sy_stream_gate(status.data_ptr() if status is not None else None, flags.data_ptr(), n, start.data_ptr(),
+                                keep.data_ptr(), _stream()))
+
+
+def stream_rescale(det, count, status, ratio):
+    """In place: the boxes of rows < count[i] of ``det`` [n, max_det, 7] divided by fp32 ``ratio[i]``, and count[i] = 0 where
+    ``status[i]`` != 0 (sy_stream_rescale; ``status`` may be None)."""
+    _require(_tensor_ok(det, torch.float32, 3) and det.shape[2] == 7, "stream_rescale: det must be float32 [n, max_det, 7]")
+    n = det.shape[0]
+    _require(_tensor_ok(count, torch.int32, 1) and count.numel() == n, "stream_rescale: count must be int32 [n]")
+    _require(_tensor_ok(ratio, torch.float32, 1) and ratio.numel() == n, "stream_rescale: ratio must be float32 [n]")
+    _require(status is None or (_tensor_ok(status, torch.int32, 1) and status.numel() == n),
+             "stream_rescale: status must be int32 [n]")
+    _check(lib().sy_stream_rescale(det.data_ptr(), n, det.shape[1], count.data_ptr(),
+                                   status.data_ptr() if status is not None else None, ratio.data_ptr(), _stream()))
 
 
 def head_pred_decode(cls_feat: View, reg_feat: View, w_reg, b_reg, w_obj, b_obj, w_cls, b_cls, stride,
@@ -797,6 +836,20 @@ def letterbox(src, mid, dst, out, flags=None):
     _check(lib().sy_letterbox(C.byref(d), _stream()))
 
 
+def letterbox_sized(src, sizes, out):
+    """uint8 [n, slot_h, slot_w, 3] slots -> fp32 [n, 3, H, W] ``out`` (sy_letterbox_sized): frame k of ``sizes[k]`` = (h, w,
+    dst_h, dst_w) (int32 [n, 4] on the device) at the slot's top-left, cv2-exact resize to dst, top-left on a canvas of 114."""
+    _require(_tensor_ok(src, torch.uint8, 4) and src.shape[3] == 3 and src.is_cuda,
+             "letterbox_sized: frames must be contiguous CUDA uint8 [n, slot_h, slot_w, 3]")
+    n, sh, sw, _ = src.shape
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 4) and sizes.device == src.device,
+             f"letterbox_sized: sizes must be int32 [{n}, 4] on the frames' device")
+    _require(_tensor_ok(out, torch.float32, 4) and out.shape[0] == n and out.shape[1] == 3 and out.device == src.device,
+             f"letterbox_sized: out must be contiguous float32 [{n}, 3, H, W] on the frames' device")
+    d = SyLetterboxSizedDesc(src.data_ptr(), n, sh, sw, sizes.data_ptr(), out.shape[2], out.shape[3], out.data_ptr())
+    _check(lib().sy_letterbox_sized(C.byref(d), _stream()))
+
+
 class PackBatch:
     """Every conv operand of a model re-packed in ONE launch (sy_pack_conv_weights_batch).  ``add`` the (fp32 parameter,
     bf16 destination, layout) pairs once -- the tensors must keep their addresses -- then ``run()`` after every update."""
@@ -843,3 +896,30 @@ def jpeg_decode(streams, lengths, out, status, workspace):
     d = SyJpegDecodeDesc(streams.data_ptr(), lengths.data_ptr(), n, max_bytes, out.shape[1], out.shape[2], out.data_ptr(),
                          status.data_ptr(), workspace.data_ptr(), workspace.numel())
     _check(lib().sy_jpeg_decode(C.byref(d), _stream()), kernels=5)
+
+
+def jpeg_decode_sized_workspace_bytes(n, max_bytes, max_h, max_w):
+    """bytes of the sy_jpeg_decode_sized workspace for n frames in slots of max_h x max_w, stored in rows of max_bytes"""
+    need = load_library().sy_jpeg_decode_sized_workspace_bytes(n, max_bytes, max_h, max_w)
+    _require(need > 0, f"jpeg_decode_sized: bad sizes (n {n}, max_bytes {max_bytes}, slot {max_h}x{max_w})")
+    return need
+
+
+def jpeg_decode_sized(streams, lengths, sizes, out, status, workspace):
+    """Decode n JPEG files of their own sizes (sy_jpeg_decode_sized): ``sizes`` int32 [n, 2] expected (h, w), ``out`` uint8
+    [n, max_h, max_w, 3] slots, the rest as jpeg_decode.  Nothing is read back."""
+    _require(_tensor_ok(streams, torch.uint8, 2), "jpeg_decode_sized: streams must be contiguous uint8 [n, max_bytes]")
+    n, max_bytes = streams.shape
+    _require(_tensor_ok(lengths, torch.int32, 1) and lengths.shape[0] == n, "jpeg_decode_sized: lengths must be int32 [n]")
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 2), "jpeg_decode_sized: sizes must be int32 [n, 2]")
+    _require(_tensor_ok(out, torch.uint8, 4) and out.shape[0] == n and out.shape[3] == 3,
+             "jpeg_decode_sized: out must be contiguous uint8 [n, max_h, max_w, 3]")
+    _require(_tensor_ok(status, torch.int32, 1) and status.shape[0] == n, "jpeg_decode_sized: status must be int32 [n]")
+    need = jpeg_decode_sized_workspace_bytes(n, max_bytes, out.shape[1], out.shape[2])
+    _require(_tensor_ok(workspace, torch.uint8, 1) and workspace.numel() >= need,
+             f"jpeg_decode_sized: workspace must be contiguous uint8 of at least {need} bytes")
+    _require(len({t.device for t in (streams, lengths, sizes, out, status, workspace)}) == 1 and streams.is_cuda,
+             "jpeg_decode_sized: all tensors must be on one CUDA device")
+    d = SyJpegDecodeSizedDesc(streams.data_ptr(), lengths.data_ptr(), n, max_bytes, sizes.data_ptr(), out.shape[1],
+                              out.shape[2], out.data_ptr(), status.data_ptr(), workspace.data_ptr(), workspace.numel())
+    _check(lib().sy_jpeg_decode_sized(C.byref(d), _stream()), kernels=5)

@@ -11,13 +11,27 @@ that starts a sequence -- the star node of dfp_pafpn.py:177-228 -- the carried b
 buffer update, the head and the NMS (``sy_postprocess_nms`` with room for every anchor).  Around the replay ``step``
 copies the frames in and the detections out through pinned host memory and synchronises once.
 
+Streams of different sizes, fed JPEG bytes (a camera rig):
+
+    det = StreamDetector(model, frame_sizes=[(1200, 1920), (2048, 1550), (1550, 2048)], input_size=(600, 960),
+                         in_scale=0.5, jpeg_max_bytes=1 << 20)
+    for (bboxes, scores, labels) in det.step_jpeg([jpeg0, jpeg1, None]):   # None: no frame from that camera this tick
+        ...
+    det.last_status()                             # per stream: 0 decoded, a data.JPEG_STATUS code, or NO_FRAME
+
+Then the tick also decodes the S files (sy_jpeg_decode_sized) into slots of the largest size and resizes each frame with
+its own transform (data.sized_table: the driver's plain resize for a frame of driver size ``input_size``, the evaluation
+letterbox otherwise; sy_letterbox_sized), and divides each stream's boxes by its own ratio on the device.  A stream whose
+frame did not decode, or that got none, keeps its carried features, starts no sequence and returns no detections
+(sy_stream_gate, sy_stream_rescale): all decided on the device, still one replay and one synchronisation per tick.
+
 The graph reads the weights and the folded BatchNorm as they were at capture: after ``load_state_dict`` (or any other
 change of the weights or running statistics) call ``capture()`` again.  Nothing checks this per frame.
 """
 import numpy as np
 import torch
 
-from . import ops
+from . import data, ops
 from .model import engine
 
 
@@ -55,6 +69,98 @@ class StreamTick:
                                                        max_det=self.raw.shape[1])
 
 
+class SizedStreamTick(StreamTick):
+    """The tick of streams with a size each: ``frames`` is uint8 [S, max_h, max_w, 3] slots (stream i's frame at the top-left
+    of slot i), ``table`` the static int32 [S, 4] rows of data.sized_table and ``ratio`` fp32 [S] each stream's box ratio.
+    With ``jpeg_max_bytes`` the inputs are ``bytes`` (uint8 [S, jpeg_max_bytes]) and ``lengths`` (int32 [S], 0 = no frame),
+    decoded inside the tick into ``frames`` with a per-stream ``status``."""
+
+    def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None):
+        table = np.asarray(table, np.int32)
+        slot = (int(table[:, 0].max()), int(table[:, 1].max()))
+        super().__init__(model, slot, size, streams, conf_thre, nms_thre, device)
+        self.table = torch.from_numpy(table).to(device)
+        self.ratio = torch.tensor(ratios, dtype=torch.float32, device=device)
+        self.start = torch.zeros((streams,), dtype=torch.int32, device=device)
+        self.keep = torch.ones((streams,), dtype=torch.int32, device=device)
+        self.status = None
+        if jpeg_max_bytes is not None:
+            self.bytes = torch.zeros((streams, jpeg_max_bytes), dtype=torch.uint8, device=device)
+            self.lengths = torch.zeros((streams,), dtype=torch.int32, device=device)
+            self.status = torch.zeros((streams,), dtype=torch.int32, device=device)
+            self.sizes = self.table[:, :2].contiguous()
+            self.workspace = torch.empty(ops.jpeg_decode_sized_workspace_bytes(streams, jpeg_max_bytes, *slot),
+                                         dtype=torch.uint8, device=device)
+
+    def run(self):
+        ctx, net, head = self.ctx, self.model.backbone, self.model.head
+        if self.status is not None:
+            ops.jpeg_decode_sized(self.bytes, self.lengths, self.sizes, self.frames, self.status, self.workspace)
+        ops.stream_gate(self.status, self.flags, self.start, self.keep)
+        ops.letterbox_sized(self.frames, self.table, self.x)
+        with torch.no_grad(), engine.forward_scope(ctx.device):
+            cur = engine.pafpn_frames(ctx, net, self.x, 1)
+            if self.buffer is None:
+                self.buffer = tuple(ctx.empty(v.n, v.h, v.w, v.c) for v in cur)
+            ops.select_images(cur, self.buffer, self.start)
+            fused = engine.dfp_fuse(ctx, net, cur, self.buffer)
+            ops.select_images(cur, self.buffer, self.keep)
+            self.raw = head.run(ctx, fused)
+            self.det, self.count = ops.postprocess_nms(self.raw, head.num_classes, self.conf_thre, self.nms_thre,
+                                                       max_det=self.raw.shape[1])
+            ops.stream_rescale(self.det, self.count, self.status, self.ratio)
+
+
+NO_FRAME = -1     # last_status() of a stream that was given no frame
+
+
+def input_size_for(frame_sizes, in_scale, input_size=None):
+    """The model input size of a rig: ``input_size`` when given, else the driver's (int(h * in_scale), int(w * in_scale))
+    of the largest frame (by area; the first of equal ones)."""
+    if input_size is not None:
+        return tuple(int(v) for v in input_size)
+    h, w = max(frame_sizes, key=lambda s: s[0] * s[1])
+    return int(h * in_scale), int(w * in_scale)
+
+
+def jpeg_files(files, streams, max_bytes):
+    """step_jpeg's inputs as S uint8 numpy arrays (``None``: no frame this tick, an empty array), or an error: a list of S
+    entries, each ``bytes`` / ``bytearray`` / ``memoryview``, a uint8 numpy array or CPU tensor, or None, and at most
+    ``max_bytes`` long."""
+    if not isinstance(files, (list, tuple)) or len(files) != streams:
+        raise ValueError(f"StreamDetector.step_jpeg: give a list of {streams} files (None for no frame)")
+    out = []
+    for i, f in enumerate(files):
+        if f is None:
+            a = np.zeros(0, np.uint8)
+        elif isinstance(f, (bytes, bytearray, memoryview)):
+            a = np.frombuffer(f, np.uint8)
+        else:
+            a = f.numpy() if torch.is_tensor(f) and not f.is_cuda else f
+            if not isinstance(a, np.ndarray) or a.dtype != np.uint8:
+                raise TypeError(f"StreamDetector.step_jpeg: file {i} must be bytes or a uint8 array, not "
+                                f"{getattr(a, 'dtype', type(a).__name__)}")
+            a = np.ascontiguousarray(a).reshape(-1)
+        if a.size > max_bytes:
+            raise ValueError(f"StreamDetector.step_jpeg: file {i} has {a.size} bytes, more than jpeg_max_bytes = {max_bytes}")
+        out.append(a)
+    return out
+
+
+def route_status(status, present, flags):
+    """The host's bookkeeping after a JPEG tick: -> (the per-stream status last_status() reports -- NO_FRAME for a stream
+    given no frame --, the start flags of the next tick).  A stream whose frame decoded has started (or continued) its
+    sequence, so its flag clears; one that was gated keeps its flag, so that a sequence starts at its next decoded frame."""
+    st = np.where(np.asarray(present, bool), np.asarray(status, np.int32), NO_FRAME).astype(np.int32)
+    return st, np.where(st == 0, 0, np.asarray(flags, np.int32)).astype(np.int32)
+
+
+def sized_output(det):
+    """one stream's NMS rows (numpy fp32 [n, 7]) whose boxes the device already divided by the stream's ratio -> the
+    driver's (bboxes, scores, labels)"""
+    return det[:, :4].copy(), det[:, 4] * det[:, 5], det[:, 6].astype(np.int32)
+
+
 def step_frames(frames, streams, frame_hw):
     """``frames`` (numpy, CPU or CUDA tensor) as a uint8 [S, h, w, 3] tensor, or RuntimeError; [h, w, 3] for one stream."""
     s, (h, w) = streams, frame_hw
@@ -75,13 +181,31 @@ class StreamDetector:
     """``model`` (YOLOX with a DFPPAFPN backbone, in eval mode, weights loaded) on ``streams`` camera streams of
     ``frame_hw`` uint8 BGR frames, at the driver's input size ``(int(h * in_scale), int(w * in_scale))``.  The activation
     storage is ``model.activation_dtype`` (``torch.float16`` for the driver's ``model.half()``).  The constructor captures
-    the tick (after one warm-up run); every stream starts a sequence at the first ``step``."""
+    the tick (after one warm-up run); every stream starts a sequence at the first ``step``.
 
-    def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65):
+    Streams of their own sizes and JPEG input (``frame_sizes`` or ``jpeg_max_bytes`` selects this mode):
+      frame_sizes     [(h, w), ...], one per stream (default: ``frame_hw`` for every stream); with the default
+                      ``streams=1`` it also sets the number of streams
+      input_size      the model's (H, W); default: the driver's size of the largest frame (input_size_for).  Only with
+                      one of the two other keywords: without them the input size is the driver's, as above
+      jpeg_max_bytes  the longest JPEG file ``step_jpeg`` takes.  The replay then starts with the decode of the streams'
+                      files, so such a detector takes files only (``step_jpeg``); without it, it takes decoded frames only
+                      (``step`` with a list of S frames, frame i of stream i's size)
+    Each stream's frame is transformed as data.sized_table says and its boxes divided by its own ratio (``ratios``)."""
+
+    def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
+                 frame_sizes=None, input_size=None, jpeg_max_bytes=None):
         if model.training:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
             raise ValueError(f"StreamDetector: streams must be a positive integer, not {streams}")
+        self.sized = frame_sizes is not None or jpeg_max_bytes is not None
+        if input_size is not None and not self.sized:
+            raise ValueError("StreamDetector: input_size takes frame_sizes or jpeg_max_bytes; without them the input size "
+                             "is the driver's (int(h * in_scale), int(w * in_scale))")
+        if self.sized:
+            return self._init_sized(model, frame_hw, in_scale, int(streams), conf_thre, nms_thre, frame_sizes, input_size,
+                                    jpeg_max_bytes)
         h, w = (int(v) for v in frame_hw)
         size = (int(h * in_scale), int(w * in_scale))
         if min(h, w, *size) < 1:
@@ -92,6 +216,40 @@ class StreamDetector:
         self._tick = StreamTick(model, (h, w), size, self.streams, conf_thre, nms_thre, dev)
         self._stage = torch.empty((self.streams, h, w, 3), dtype=torch.uint8).pin_memory()
         self._flags = torch.ones((self.streams,), dtype=torch.int32).pin_memory()
+        self._graph = None
+        self.capture()
+
+    def _init_sized(self, model, frame_hw, in_scale, streams, conf_thre, nms_thre, frame_sizes, input_size, jpeg_max_bytes):
+        sizes = [tuple(int(v) for v in frame_hw)] * streams if frame_sizes is None else \
+            [tuple(int(v) for v in s) for s in frame_sizes]
+        if len(sizes) != streams and frame_sizes is not None and streams == 1:
+            streams = len(sizes)                      # streams defaults to one: frame_sizes then sets the count
+        if len(sizes) != streams or any(len(s) != 2 or min(s) < 1 for s in sizes):
+            raise ValueError(f"StreamDetector: frame_sizes must hold {streams} (h, w) pairs, not {frame_sizes}")
+        size = input_size_for(sizes, in_scale, input_size)
+        if min(size) < 1:
+            raise ValueError(f"StreamDetector: frames {sizes} at in_scale {in_scale} give input size {size}")
+        if jpeg_max_bytes is not None and (int(jpeg_max_bytes) != jpeg_max_bytes or not 4 <= jpeg_max_bytes <= 1 << 28):
+            raise ValueError(f"StreamDetector: jpeg_max_bytes must be an integer in [4, 2^28], not {jpeg_max_bytes}")
+        try:
+            table, ratios = data.sized_table(sizes, size, in_scale)
+        except RuntimeError as e:
+            raise ValueError(f"StreamDetector: {e}") from None
+        dev = next(model.parameters()).device
+        ops.lib()
+        self.model, self.streams, self.in_scale, self.size = model, streams, in_scale, size
+        self.frame_sizes, self.ratios = sizes, ratios
+        self.jpeg_max_bytes = None if jpeg_max_bytes is None else int(jpeg_max_bytes)
+        self._tick = SizedStreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes)
+        self.frame_hw = tuple(self._tick.frames.shape[1:3])          # the slot: the largest height and width
+        if self.jpeg_max_bytes is None:           # one pinned staging frame per stream, of the stream's own size
+            self._stage = [torch.empty((h, w, 3), dtype=torch.uint8).pin_memory() for h, w in sizes]
+        else:
+            self._jstage = torch.empty((streams, self.jpeg_max_bytes), dtype=torch.uint8).pin_memory()
+            self._jlen = torch.zeros((streams,), dtype=torch.int32).pin_memory()
+            self._status = torch.zeros((streams,), dtype=torch.int32).pin_memory()
+        self._last_status = None
+        self._flags = torch.ones((streams,), dtype=torch.int32).pin_memory()
         self._graph = None
         self.capture()
 
@@ -127,7 +285,11 @@ class StreamDetector:
     def step(self, frames):
         """One frame per stream -> a list of S ``(bboxes, scores, labels)`` numpy tuples, what the driver's inference()
         returns (boxes in frame pixels, float32 [n, 4]; scores float32 [n]; labels int32 [n]).  ``frames``: uint8 BGR
-        [S, h, w, 3] ([h, w, 3] for one stream), a numpy array, a CPU tensor or a CUDA tensor."""
+        [S, h, w, 3] ([h, w, 3] for one stream), a numpy array, a CPU tensor or a CUDA tensor.  With ``frame_sizes``: a list
+        of S frames, frame i uint8 [h_i, w_i, 3] of stream i's size (numpy, CPU or CUDA).  A detector built with
+        ``jpeg_max_bytes`` takes files only: ``step`` raises RuntimeError there, use ``step_jpeg``."""
+        if self.sized:
+            return self._step_sized(frames)
         t = self._tick
         src = step_frames(frames, self.streams, self.frame_hw)
         if src.is_cuda:
@@ -147,3 +309,63 @@ class StreamDetector:
     def last_raw(self):
         """A device copy of the last tick's head outputs [S, A, 5 + nc] (what the driver keeps as ``results_raw``)."""
         return self._tick.raw.clone()
+
+    def _step_sized(self, frames):
+        t = self._tick
+        if self.jpeg_max_bytes is not None:
+            raise RuntimeError("StreamDetector.step: this detector was built with jpeg_max_bytes, and its replay decodes the "
+                               "streams' files: feed it with step_jpeg (build one with frame_sizes alone for decoded frames)")
+        if not isinstance(frames, (list, tuple)) or len(frames) != self.streams:
+            raise RuntimeError(f"StreamDetector.step: give a list of {self.streams} frames, one per stream")
+        for i, (f, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
+            src = f if torch.is_tensor(f) else torch.from_numpy(np.ascontiguousarray(f))
+            ops._require(src.dtype == torch.uint8 and tuple(src.shape) == (h, w, 3),
+                         f"StreamDetector.step: frame {i} must be uint8 [{h}, {w}, 3], not {src.dtype} {list(src.shape)}")
+            if src.is_cuda:
+                t.frames[i, :h, :w].copy_(src)
+            else:                                     # only the frame's h x w pixels cross, not the whole slot
+                self._stage[i].copy_(src)
+                t.frames[i, :h, :w].copy_(self._stage[i], non_blocking=True)
+        return self._run_sized(None)
+
+    def step_jpeg(self, files):
+        """One JPEG file per stream -> a list of S ``(bboxes, scores, labels)`` tuples as ``step`` returns them, with one
+        host synchronisation.  ``files``: a list of S entries, each the file's bytes (``bytes``, or a uint8 numpy array or
+        CPU tensor, e.g. ``np.fromfile(path, np.uint8)``) of at most ``jpeg_max_bytes``, or None when the stream has no
+        frame this tick.  A stream whose file did not decode (see ``last_status``) or that got None returns empty arrays,
+        keeps its carried features and, if it was to start a sequence, starts it at its next decoded frame."""
+        if self.jpeg_max_bytes is None:
+            raise RuntimeError("StreamDetector.step_jpeg: construct the detector with jpeg_max_bytes")
+        t = self._tick
+        files = jpeg_files(files, self.streams, self.jpeg_max_bytes)
+        stage = self._jstage.numpy()
+        for i, a in enumerate(files):
+            stage[i, :a.size] = a
+            self._jlen[i] = a.size
+            if a.size:
+                t.bytes[i, :a.size].copy_(self._jstage[i, :a.size], non_blocking=True)
+        t.lengths.copy_(self._jlen, non_blocking=True)
+        return self._run_sized([a.size > 0 for a in files])
+
+    def _run_sized(self, present):
+        t = self._tick
+        flags = self._flags.numpy().copy()
+        t.flags.copy_(self._flags, non_blocking=True)
+        self._graph.replay()
+        self._det.copy_(t.det, non_blocking=True)
+        self._count.copy_(t.count, non_blocking=True)
+        if present is not None:
+            self._status.copy_(t.status, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        if present is None:
+            self._flags.zero_()
+        else:
+            self._last_status, nxt = route_status(self._status.numpy(), present, flags)
+            self._flags.copy_(torch.from_numpy(nxt))
+        det = self._det.numpy()
+        return [sized_output(det[i, :n]) for i, n in enumerate(self._count.tolist())]
+
+    def last_status(self):
+        """Per-stream int32 status of the last ``step_jpeg``: 0 where the frame decoded, a data.JPEG_STATUS code where it
+        did not, NO_FRAME (-1) where the stream got no file; None before the first ``step_jpeg``."""
+        return None if self._last_status is None else self._last_status.copy()
