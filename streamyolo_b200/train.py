@@ -16,8 +16,12 @@
       - ONE launch (``sy_sgd_nesterov_ema_step``) then does unscale (1 / (world x loss scale)) + weight decay + momentum +
         nesterov + parameter update + EMA over the whole state;
       - conv operands are re-packed from the fp32 masters by ``sy_pack_conv_weight`` launches (engine.WEIGHT_EPOCH).
-  * multi-scale training (``Exp.random_resize`` every 10 iterations): ``multiscale_sizes`` lists the sizes,
-    ``Trainer.capture_sizes`` captures one step per size into one graph memory pool, ``Trainer.replay_size`` runs one.
+  * the step as CUDA graph(s): ``Trainer.capture`` / ``replay`` at one input size; for multi-scale training
+    (``Exp.random_resize`` every 10 iterations) ``multiscale_sizes`` lists the sizes, ``Trainer.capture_sizes`` captures
+    one step per size into one graph memory pool, ``Trainer.replay_size`` runs one.  Every graph of a Trainer reads lr,
+    weight decay, momentum, 1 / (world x loss scale) and the EMA decay from ONE device block; each replay refills it from
+    one of two pinned host slots, and a slot is rewritten only after the copy that last read it has run, because the
+    host runs ahead of the device.
   * checkpoints (double_trainer.py:221-226, 285-318, 353-371): ``Trainer.state_dict`` / ``load_state_dict`` (exact
     continuation), ``reference_checkpoint`` / ``load_reference_checkpoint`` (the reference's file and ``--resume``),
     ``optimizer_state_dict`` in torch.optim.SGD format, ``all_reduce_norm`` (BatchNorm statistics averaged over the ranks).
@@ -346,6 +350,8 @@ class Trainer:
         self.bucket_bytes, self.overlap = bucket_bytes, overlap
         self.sink = None
         self.world = dist.get_world_size() if dist.is_initialized() else 1
+        self._hyper, self._hyper_slot = None, 0            # the captured graphs' hyper-parameter block (_capture)
+        self._graph, self._sized = None, {}                # what capture / capture_sizes captured
         engine.WEIGHT_EPOCH += 1
         self._build_repack()
         self._repack()
@@ -422,63 +428,95 @@ class Trainer:
         into one graph segment per gradient bucket; between two segments the host enqueues that bucket's NCCL all-reduce on the
         communication stream, where it overlaps the following segments (the collectives themselves stay outside the
         captured graphs); a last segment holds the optimiser step.  ``prologue``: a callable captured at the front of the
-        graph, e.g. ``data.pair_transform(..., out=(x, targets))`` so that the static inputs are the uint8 frames."""
-        dev = self.fs.state.device
-        self._hyper = torch.zeros(8, dtype=torch.float32, device=dev)
-        self._hyper_host = torch.zeros(8, dtype=torch.float32).pin_memory()
-        self._loss_scale = loss_scale
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):                      # warm-up on a side stream (allocator, lazy module attributes)
-            if prologue is not None:
-                prologue()
-            self._set_hyper(None)
-            self.forward_backward(x, targets, loss_scale)
-            self.optimizer_step(hyper=self._hyper)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        pool = torch.cuda.graph_pool_handle()
-        self._plan = []                                    # [(graph, bucket range or None)]
-        cur = [None]
+        graph, e.g. ``data.pair_transform(..., out=(x, targets))`` so that the static inputs are the uint8 frames.
 
-        def begin():
-            g = torch.cuda.CUDAGraph()
-            g.capture_begin(pool=pool)
-            cur[0] = g
-
-        def cut(a, b):
-            cur[0].capture_end()
-            self._plan.append((cur[0], (a, b)))
-            begin()
-
-        self.sink.on_bucket = cut if self.world > 1 else None
-        with torch.cuda.stream(side):
-            begin()
-            if prologue is not None:
-                prologue()
-            loss = self.forward_backward(x, targets, loss_scale)
-            if self.world > 1:                             # the optimiser step waits for the collectives: its own segment
-                cur[0].capture_end()
-                self._plan.append((cur[0], None))
-                begin()
-            self.optimizer_step(hyper=self._hyper)
-            cur[0].capture_end()
-            self._plan.append((cur[0], None))
-        self.sink.on_bucket = None
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        self._graph_loss = loss
-        return len(self._plan)
-
-    def _set_hyper(self, lr):
-        self.updates += 1
-        self._hyper_host[:6] = torch.tensor(self._hyper_values(lr, self._loss_scale))
-        self._hyper.copy_(self._hyper_host, non_blocking=True)
+        Before capturing, the step runs once eagerly on the inputs as they stand: that warm-up is a real training step at
+        ``self.lr`` (``updates`` goes up by one; parameters, BatchNorm statistics, momentum and the EMA copy advance), so
+        the first ``replay`` is the second step.  Returns the number of graph segments."""
+        self._graph = None                                 # a second call replaces the first: its graph goes first
+        keyed = None if prologue is None else lambda *_: prologue()
+        self._graph = self._capture({None: (x, targets)}, keyed, loss_scale, restore=False)[None]
+        return len(self._graph[0])
 
     def replay(self, lr=None):
-        self._set_hyper(lr)
-        self._replay_plan(self._plan)
-        return backward._loss_dict(self._graph_loss)
+        return self._replay(self._graph, lr)
+
+    def _capture(self, inputs, prologue, loss_scale, restore):
+        """Capture one step per entry of ``inputs`` ({key: (x, targets)}; ``prologue(key, x, targets)`` at the front of
+        each) into ONE graph memory pool, after one eager warm-up step per entry on a side stream (allocator, lazy module
+        attributes).  ``restore``: the warm-up steps are undone, the training state is as before the call.  Returns
+        {key: (plan, loss vector, loss_scale)}, a plan being [(graph segment, bucket all-reduced after it, or None)].  The
+        loss vectors stay referenced, so no later capture in the pool takes them over."""
+        if self._hyper is None:          # ONE block per Trainer, never reallocated: every captured graph reads its address
+            self._hyper = torch.zeros(8, dtype=torch.float32, device=self.fs.state.device)
+            self._hyper_slots = [(torch.zeros(8, dtype=torch.float32).pin_memory(), torch.cuda.Event()) for _ in range(2)]
+        snapshot = copy.deepcopy(self.state_dict()) if restore else None
+        self.updates += 1
+        self._stage_hyper(None, loss_scale)
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):
+            for key, (x, targets) in inputs.items():
+                if prologue is not None:
+                    prologue(key, x, targets)
+                self.forward_backward(x, targets, loss_scale)
+                self.optimizer_step(hyper=self._hyper)
+            if restore:
+                self.load_state_dict(snapshot)
+        torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        torch.cuda.empty_cache()                           # the warm-up's blocks: device memory for the graphs' pool
+        pool = torch.cuda.graph_pool_handle()
+        graphs = {}
+        for key, (x, targets) in inputs.items():
+            plan, cur = [], None
+
+            def begin():
+                nonlocal cur
+                cur = torch.cuda.CUDAGraph()
+                cur.capture_begin(pool=pool)
+
+            def end(bucket=None):
+                cur.capture_end()
+                plan.append((cur, bucket))
+
+            def cut(a, b):
+                end((a, b))
+                begin()
+
+            self.sink.on_bucket = cut if self.world > 1 else None
+            with torch.cuda.stream(side):
+                begin()
+                if prologue is not None:
+                    prologue(key, x, targets)
+                loss = self.forward_backward(x, targets, loss_scale)
+                if self.world > 1:                         # the optimiser step waits for the collectives: its own segment
+                    end()
+                    begin()
+                self.optimizer_step(hyper=self._hyper)
+                end()
+            self.sink.on_bucket = None
+            graphs[key] = (plan, loss, loss_scale)
+            torch.cuda.current_stream().wait_stream(side)
+        torch.cuda.synchronize()
+        return graphs
+
+    def _replay(self, graph, lr):
+        plan, loss, loss_scale = graph
+        self.updates += 1
+        self._stage_hyper(lr, loss_scale)
+        self._replay_plan(plan)
+        return backward._loss_dict(loss)
+
+    def _stage_hyper(self, lr, loss_scale):
+        """the hyper-parameter block of the captured graphs for the step ``updates``, through two pinned slots: a slot is
+        written again only after the copy that read it last has run (the host runs ahead of the device)"""
+        self._hyper_slot ^= 1
+        host, copied = self._hyper_slots[self._hyper_slot]
+        copied.synchronize()
+        host[:6] = torch.tensor(self._hyper_values(lr, loss_scale))
+        self._hyper.copy_(host, non_blocking=True)
+        copied.record()
 
     def _replay_plan(self, plan):
         works = []
@@ -508,91 +546,21 @@ class Trainer:
         each graph stays referenced, so no capture takes it over.  Replays must therefore run one at a time, on the current
         stream, which ``replay_size`` does.  Several ranks: the graphs are cut at the same gradient buckets for every size
         (the flat gradient layout does not depend on the input size)."""
-        dev = self.fs.state.device
         sizes = sorted({tuple(int(v) for v in s) for s in sizes}, key=lambda s: -s[0] * s[1])   # largest first: the
         inputs = {s: make_inputs(s) for s in sizes}                                          # pool grows once
-        self._ms_hyper = torch.zeros(8, dtype=torch.float32, device=dev)
-        self._ms_host = [torch.zeros(8, dtype=torch.float32).pin_memory() for _ in range(2)]
-        self._ms_copied = [None, None]
-        self._ms_slot = 0
-        self._ms_loss_scale = loss_scale
-        snapshot = copy.deepcopy(self.state_dict())
-        self._stage_hyper(None)
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):                      # warm-up at every size (allocator, lazy module attributes)
-            for s in sizes:
-                x, targets = inputs[s]
-                if prologue is not None:
-                    prologue(s, x, targets)
-                self.forward_backward(x, targets, loss_scale)
-                self.optimizer_step(hyper=self._ms_hyper)
-            self.load_state_dict(snapshot)                 # ... and back to the state before the call
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        torch.cuda.empty_cache()                           # the warm-up's blocks: device memory for the graphs' pool
-        pool = torch.cuda.graph_pool_handle()
-        self._ms = {}                                      # size -> (plan, loss vector)
-        for s in sizes:
-            x, targets = inputs[s]
-            plan = []
-            cur = [None]
-
-            def begin():
-                g = torch.cuda.CUDAGraph()
-                g.capture_begin(pool=pool)
-                cur[0] = g
-
-            def cut(a, b):
-                cur[0].capture_end()
-                plan.append((cur[0], (a, b)))
-                begin()
-
-            self.sink.on_bucket = cut if self.world > 1 else None
-            with torch.cuda.stream(side):
-                begin()
-                if prologue is not None:
-                    prologue(s, x, targets)
-                loss = self.forward_backward(x, targets, loss_scale)
-                if self.world > 1:
-                    cur[0].capture_end()
-                    plan.append((cur[0], None))
-                    begin()
-                self.optimizer_step(hyper=self._ms_hyper)
-                cur[0].capture_end()
-                plan.append((cur[0], None))
-            self.sink.on_bucket = None
-            self._ms[s] = (plan, loss)
-            torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        buckets = {s: [b for _, b in plan] for s, (plan, _) in self._ms.items()}
-        first = buckets[sizes[0]]
-        assert all(b == first for b in buckets.values()), "the gradient buckets differ between input sizes"
-        return {s: len(plan) for s, (plan, _) in self._ms.items()}
+        self._sized = {}                                   # a second call replaces the first: its graphs go first
+        self._sized = self._capture(inputs, prologue, loss_scale, restore=True)
+        buckets = [[b for _, b in plan] for plan, _, _ in self._sized.values()]
+        assert all(b == buckets[0] for b in buckets), "the gradient buckets differ between input sizes"
+        return {s: len(plan) for s, (plan, _, _) in self._sized.items()}
 
     def replay_size(self, size, lr=None):
         """One captured step at ``size`` (a size given to ``capture_sizes``); returns its loss dict.  Several ranks: every rank
         must replay the same size, as the reference's ``Exp.random_resize`` ensures (rank 0 draws it and broadcasts it)."""
         size = tuple(int(v) for v in size)
-        if size not in self._ms:
-            raise KeyError(f"replay_size: no graph captured for {size} (captured: {sorted(self._ms)})")
-        plan, loss = self._ms[size]
-        self.updates += 1
-        self._stage_hyper(lr)
-        self._replay_plan(plan)
-        return backward._loss_dict(loss)
-
-    def _stage_hyper(self, lr):
-        """the hyper-parameter block of the size graphs for the step ``updates``, through two pinned slots: a slot is written
-        again only after the copy that read it last has run (the host runs ahead of the device)"""
-        i = self._ms_slot = (self._ms_slot + 1) % len(self._ms_host)
-        if self._ms_copied[i] is not None:
-            self._ms_copied[i].synchronize()
-        host = self._ms_host[i]
-        host[:6] = torch.tensor(self._hyper_values(lr, self._ms_loss_scale))
-        self._ms_hyper.copy_(host, non_blocking=True)
-        self._ms_copied[i] = torch.cuda.Event()
-        self._ms_copied[i].record()
+        if size not in self._sized:
+            raise KeyError(f"replay_size: no graph captured for {size} (captured: {sorted(self._sized)})")
+        return self._replay(self._sized[size], lr)
 
     def ema_state_dict(self):
         return self.fs.ema_state_dict(self.model)
