@@ -1,15 +1,17 @@
 """The streaming detector: the sAP driver's per-frame loop (sAP/streamyolo/streamyolo_det.py:150-195) as ONE CUDA graph
-replay per frame, for one camera stream or several batched together.
+replay per frame, for one camera stream or several batched together, each stream with a frame size of its own.
 
     det = StreamDetector(model, frame_hw=(1200, 1920), in_scale=0.5, streams=1)   # model in eval(), weights loaded
     det.reset()                                   # every stream starts a sequence (det.reset(i): stream i only)
     bboxes, scores, labels = det.step(frame)[0]   # what the driver's inference() returns for that frame
 
-One tick runs, for the S streams at once: the driver's resize of the S uint8 frames (``data.stream_frame`` at batch S), the
-backbone + PAFPN on the current frames, the per-stream choice of the support features (the current ones for a stream
-that starts a sequence -- the star node of dfp_pafpn.py:177-228 -- the carried buffer otherwise), the DFP fusion, the
-buffer update, the head and the NMS (``sy_postprocess_nms`` with room for every anchor).  Around the replay ``step``
-copies the frames in and the detections out through pinned host memory and synchronises once.
+One tick runs, for the S streams at once: the resize of each stream's uint8 frame with its own transform (data.sized_table:
+the driver's plain resize, ``data.stream_frame``, for a frame whose driver size is the input size, the evaluation
+letterbox otherwise; sy_letterbox_sized), the backbone + PAFPN on the current frames, the per-stream choice of the support features
+(the current ones for a stream that starts a sequence -- the star node of dfp_pafpn.py:177-228 -- the carried buffer
+otherwise), the DFP fusion, the buffer update, the head, the NMS (``sy_postprocess_nms`` with room for every anchor) and
+the division of each stream's boxes by its own ratio (``in_scale`` for the driver's resize; sy_stream_rescale).  Around
+the replay ``step`` copies the frames in and the detections out through pinned host memory and synchronises once.
 
 Streams of different sizes, fed JPEG bytes (a camera rig):
 
@@ -19,9 +21,7 @@ Streams of different sizes, fed JPEG bytes (a camera rig):
         ...
     det.last_status()                             # per stream: 0 decoded, a data.JPEG_STATUS code, or NO_FRAME
 
-Then the tick also decodes the S files (sy_jpeg_decode_sized) into slots of the largest size and resizes each frame with
-its own transform (data.sized_table: the driver's plain resize for a frame of driver size ``input_size``, the evaluation
-letterbox otherwise; sy_letterbox_sized), and divides each stream's boxes by its own ratio on the device.  A stream whose
+Then the tick starts with the decode of the S files (sy_jpeg_decode_sized) into slots of the largest size.  A stream whose
 frame did not decode, or that got none, keeps its carried features, starts no sequence and returns no detections
 (sy_stream_gate, sy_stream_rescale): all decided on the device, still one replay and one synchronisation per tick.
 
@@ -37,52 +37,29 @@ from .model import engine
 
 class StreamTick:
     """The work of one tick on static buffers -- what ``StreamDetector`` captures as a CUDA graph.  ``frames`` (uint8
-    [S, h, w, 3]) and ``flags`` (int32 [S], set = the stream starts a sequence) are the inputs; ``raw`` ([S, A, 5 + nc] head
-    outputs), ``det`` ([S, A, 7] rows x1, y1, x2, y2, obj, class_conf, class_pred) and ``count`` ([S] rows of ``det``) are
-    the outputs; ``buffer`` holds each stream's features carried to the next tick."""
-
-    def __init__(self, model, frame_hw, size, streams, conf_thre, nms_thre, device):
-        self.model, self.size = model, tuple(size)
-        self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
-        h, w = frame_hw
-        self.frames = torch.zeros((streams, h, w, 3), dtype=torch.uint8, device=device)
-        self.flags = torch.ones((streams,), dtype=torch.int32, device=device)
-        self.x = torch.empty((streams, 3, size[0], size[1]), dtype=torch.float32, device=device)
-        self.ctx = engine.Ctx(False, streams, streams, torch.device(device), dtype=model.activation_dtype)
-        self.buffer = None
-        self.raw = self.det = self.count = None
-
-    def run(self):
-        ctx, net, head = self.ctx, self.model.backbone, self.model.head
-        s, h, w, _ = self.frames.shape
-        ops.letterbox(self.frames, (h, w), self.size, self.x)
-        with torch.no_grad(), engine.forward_scope(ctx.device):
-            cur = engine.pafpn_frames(ctx, net, self.x, 1)
-            if self.buffer is None:
-                self.buffer = tuple(ctx.empty(v.n, v.h, v.w, v.c) for v in cur)
-            ops.select_images(cur, self.buffer, self.flags)
-            fused = engine.dfp_fuse(ctx, net, cur, self.buffer)
-            for c, b in zip(cur, self.buffer):
-                ops.copy(c, b)
-            self.raw = head.run(ctx, fused)
-            self.det, self.count = ops.postprocess_nms(self.raw, head.num_classes, self.conf_thre, self.nms_thre,
-                                                       max_det=self.raw.shape[1])
-
-
-class SizedStreamTick(StreamTick):
-    """The tick of streams with a size each: ``frames`` is uint8 [S, max_h, max_w, 3] slots (stream i's frame at the top-left
-    of slot i), ``table`` the static int32 [S, 4] rows of data.sized_table and ``ratio`` fp32 [S] each stream's box ratio.
-    With ``jpeg_max_bytes`` the inputs are ``bytes`` (uint8 [S, jpeg_max_bytes]) and ``lengths`` (int32 [S], 0 = no frame),
-    decoded inside the tick into ``frames`` with a per-stream ``status``."""
+    [S, max_h, max_w, 3] slots, stream i's frame at the top-left of slot i) and ``flags`` (int32 [S], set = the stream
+    starts a sequence) are the inputs; ``table`` holds the static int32 [S, 4] rows of data.sized_table and ``ratio`` (fp32
+    [S]) each stream's box ratio.  With ``jpeg_max_bytes`` the inputs are ``bytes`` (uint8 [S, jpeg_max_bytes]) and
+    ``lengths`` (int32 [S], 0 = no frame) instead of ``frames``, decoded inside the tick into ``frames`` with a per-stream
+    ``status``.  ``raw`` ([S, A, 5 + nc] head outputs), ``det`` ([S, A, 7] rows x1, y1, x2, y2 -- divided by the stream's
+    ratio --, obj, class_conf, class_pred) and ``count`` ([S] rows of ``det``) are the outputs; ``buffer`` holds each
+    stream's features carried to the next tick."""
 
     def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None):
+        self.model, self.size = model, tuple(size)
+        self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
         table = np.asarray(table, np.int32)
         slot = (int(table[:, 0].max()), int(table[:, 1].max()))
-        super().__init__(model, slot, size, streams, conf_thre, nms_thre, device)
+        self.frames = torch.zeros((streams, slot[0], slot[1], 3), dtype=torch.uint8, device=device)
+        self.flags = torch.ones((streams,), dtype=torch.int32, device=device)
         self.table = torch.from_numpy(table).to(device)
         self.ratio = torch.tensor(ratios, dtype=torch.float32, device=device)
         self.start = torch.zeros((streams,), dtype=torch.int32, device=device)
         self.keep = torch.ones((streams,), dtype=torch.int32, device=device)
+        self.x = torch.empty((streams, 3, size[0], size[1]), dtype=torch.float32, device=device)
+        self.ctx = engine.Ctx(False, streams, streams, torch.device(device), dtype=model.activation_dtype)
+        self.buffer = None
+        self.raw = self.det = self.count = None
         self.status = None
         if jpeg_max_bytes is not None:
             self.bytes = torch.zeros((streams, jpeg_max_bytes), dtype=torch.uint8, device=device)
@@ -171,27 +148,23 @@ def step_frames(frames, streams, frame_hw):
     return src.reshape(s, h, w, 3)
 
 
-def driver_output(det, in_scale):
-    """The driver's inference() conversion of one frame's NMS rows (numpy fp32 [n, 7]): boxes / in_scale,
-    obj * class_conf, the class as int32."""
-    return det[:, :4] / in_scale, det[:, 4] * det[:, 5], det[:, 6].astype(np.int32)
-
-
 class StreamDetector:
     """``model`` (YOLOX with a DFPPAFPN backbone, in eval mode, weights loaded) on ``streams`` camera streams of
     ``frame_hw`` uint8 BGR frames, at the driver's input size ``(int(h * in_scale), int(w * in_scale))``.  The activation
     storage is ``model.activation_dtype`` (``torch.float16`` for the driver's ``model.half()``).  The constructor captures
     the tick (after one warm-up run); every stream starts a sequence at the first ``step``.
 
-    Streams of their own sizes and JPEG input (``frame_sizes`` or ``jpeg_max_bytes`` selects this mode):
+    Streams of their own sizes and JPEG input:
       frame_sizes     [(h, w), ...], one per stream (default: ``frame_hw`` for every stream); with the default
                       ``streams=1`` it also sets the number of streams
       input_size      the model's (H, W); default: the driver's size of the largest frame (input_size_for).  Only with
-                      one of the two other keywords: without them the input size is the driver's, as above
+                      ``frame_sizes`` or ``jpeg_max_bytes``: without them the input size is the driver's, as above
       jpeg_max_bytes  the longest JPEG file ``step_jpeg`` takes.  The replay then starts with the decode of the streams'
                       files, so such a detector takes files only (``step_jpeg``); without it, it takes decoded frames only
-                      (``step`` with a list of S frames, frame i of stream i's size)
-    Each stream's frame is transformed as data.sized_table says and its boxes divided by its own ratio (``ratios``)."""
+                      (``step``)
+    Each stream's frame is transformed as data.sized_table says and its boxes divided by its own ratio (``ratios``): a frame
+    of driver size ``input_size`` gets the driver's plain resize and ``in_scale``.  ``frame_hw`` is the slot the frames are
+    stored in: the largest height and width (the frame size when every stream has one size)."""
 
     def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
                  frame_sizes=None, input_size=None, jpeg_max_bytes=None):
@@ -199,35 +172,17 @@ class StreamDetector:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
             raise ValueError(f"StreamDetector: streams must be a positive integer, not {streams}")
-        self.sized = frame_sizes is not None or jpeg_max_bytes is not None
-        if input_size is not None and not self.sized:
+        if input_size is not None and frame_sizes is None and jpeg_max_bytes is None:
             raise ValueError("StreamDetector: input_size takes frame_sizes or jpeg_max_bytes; without them the input size "
                              "is the driver's (int(h * in_scale), int(w * in_scale))")
-        if self.sized:
-            return self._init_sized(model, frame_hw, in_scale, int(streams), conf_thre, nms_thre, frame_sizes, input_size,
-                                    jpeg_max_bytes)
-        h, w = (int(v) for v in frame_hw)
-        size = (int(h * in_scale), int(w * in_scale))
-        if min(h, w, *size) < 1:
-            raise ValueError(f"StreamDetector: frame {frame_hw} at in_scale {in_scale} gives input size {size}")
-        dev = next(model.parameters()).device
-        ops.lib()
-        self.model, self.streams, self.frame_hw, self.in_scale, self.size = model, int(streams), (h, w), in_scale, size
-        self._tick = StreamTick(model, (h, w), size, self.streams, conf_thre, nms_thre, dev)
-        self._stage = torch.empty((self.streams, h, w, 3), dtype=torch.uint8).pin_memory()
-        self._flags = torch.ones((self.streams,), dtype=torch.int32).pin_memory()
-        self._graph = None
-        self.capture()
-
-    def _init_sized(self, model, frame_hw, in_scale, streams, conf_thre, nms_thre, frame_sizes, input_size, jpeg_max_bytes):
-        sizes = [tuple(int(v) for v in frame_hw)] * streams if frame_sizes is None else \
-            [tuple(int(v) for v in s) for s in frame_sizes]
+        streams = int(streams)
+        sizes = [tuple(int(v) for v in s) for s in ([frame_hw] * streams if frame_sizes is None else frame_sizes)]
         if len(sizes) != streams and frame_sizes is not None and streams == 1:
             streams = len(sizes)                      # streams defaults to one: frame_sizes then sets the count
-        if len(sizes) != streams or any(len(s) != 2 or min(s) < 1 for s in sizes):
+        if len(sizes) != streams or any(len(s) != 2 for s in sizes):
             raise ValueError(f"StreamDetector: frame_sizes must hold {streams} (h, w) pairs, not {frame_sizes}")
         size = input_size_for(sizes, in_scale, input_size)
-        if min(size) < 1:
+        if min(size) < 1 or min(min(s) for s in sizes) < 1:
             raise ValueError(f"StreamDetector: frames {sizes} at in_scale {in_scale} give input size {size}")
         if jpeg_max_bytes is not None and (int(jpeg_max_bytes) != jpeg_max_bytes or not 4 <= jpeg_max_bytes <= 1 << 28):
             raise ValueError(f"StreamDetector: jpeg_max_bytes must be an integer in [4, 2^28], not {jpeg_max_bytes}")
@@ -240,10 +195,10 @@ class StreamDetector:
         self.model, self.streams, self.in_scale, self.size = model, streams, in_scale, size
         self.frame_sizes, self.ratios = sizes, ratios
         self.jpeg_max_bytes = None if jpeg_max_bytes is None else int(jpeg_max_bytes)
-        self._tick = SizedStreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes)
+        self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes)
         self.frame_hw = tuple(self._tick.frames.shape[1:3])          # the slot: the largest height and width
-        if self.jpeg_max_bytes is None:           # one pinned staging frame per stream, of the stream's own size
-            self._stage = [torch.empty((h, w, 3), dtype=torch.uint8).pin_memory() for h, w in sizes]
+        if self.jpeg_max_bytes is None:           # stream i's frame is staged at the start of slot i (see step)
+            self._stage = torch.empty(tuple(self._tick.frames.shape), dtype=torch.uint8).pin_memory()
         else:
             self._jstage = torch.empty((streams, self.jpeg_max_bytes), dtype=torch.uint8).pin_memory()
             self._jlen = torch.zeros((streams,), dtype=torch.int32).pin_memory()
@@ -284,49 +239,40 @@ class StreamDetector:
 
     def step(self, frames):
         """One frame per stream -> a list of S ``(bboxes, scores, labels)`` numpy tuples, what the driver's inference()
-        returns (boxes in frame pixels, float32 [n, 4]; scores float32 [n]; labels int32 [n]).  ``frames``: uint8 BGR
-        [S, h, w, 3] ([h, w, 3] for one stream), a numpy array, a CPU tensor or a CUDA tensor.  With ``frame_sizes``: a list
-        of S frames, frame i uint8 [h_i, w_i, 3] of stream i's size (numpy, CPU or CUDA).  A detector built with
+        returns (boxes in frame pixels, float32 [n, 4]; scores float32 [n]; labels int32 [n]).  ``frames``: a list of S
+        frames, frame i uint8 BGR [h_i, w_i, 3] of stream i's size; or, when every stream has the same size, uint8
+        [S, h, w, 3] ([h, w, 3] for one stream).  Each a numpy array, a CPU tensor or a CUDA tensor.  A detector built with
         ``jpeg_max_bytes`` takes files only: ``step`` raises RuntimeError there, use ``step_jpeg``."""
-        if self.sized:
-            return self._step_sized(frames)
-        t = self._tick
-        src = step_frames(frames, self.streams, self.frame_hw)
-        if src.is_cuda:
-            t.frames.copy_(src)
-        else:
-            self._stage.copy_(src)
-            t.frames.copy_(self._stage, non_blocking=True)
-        t.flags.copy_(self._flags, non_blocking=True)
-        self._graph.replay()
-        self._det.copy_(t.det, non_blocking=True)
-        self._count.copy_(t.count, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
-        self._flags.zero_()
-        det = self._det.numpy()
-        return [driver_output(det[i, :n], self.in_scale) for i, n in enumerate(self._count.tolist())]
-
-    def last_raw(self):
-        """A device copy of the last tick's head outputs [S, A, 5 + nc] (what the driver keeps as ``results_raw``)."""
-        return self._tick.raw.clone()
-
-    def _step_sized(self, frames):
         t = self._tick
         if self.jpeg_max_bytes is not None:
             raise RuntimeError("StreamDetector.step: this detector was built with jpeg_max_bytes, and its replay decodes the "
                                "streams' files: feed it with step_jpeg (build one with frame_sizes alone for decoded frames)")
-        if not isinstance(frames, (list, tuple)) or len(frames) != self.streams:
-            raise RuntimeError(f"StreamDetector.step: give a list of {self.streams} frames, one per stream")
-        for i, (f, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
-            src = f if torch.is_tensor(f) else torch.from_numpy(np.ascontiguousarray(f))
-            ops._require(src.dtype == torch.uint8 and tuple(src.shape) == (h, w, 3),
-                         f"StreamDetector.step: frame {i} must be uint8 [{h}, {w}, 3], not {src.dtype} {list(src.shape)}")
+        if isinstance(frames, (list, tuple)):
+            ops._require(len(frames) == self.streams, f"StreamDetector.step: give a list of {self.streams} frames, one per stream")
+            for i, (f, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
+                src = f if torch.is_tensor(f) else torch.from_numpy(np.ascontiguousarray(f))
+                ops._require(src.dtype == torch.uint8 and tuple(src.shape) == (h, w, 3),
+                             f"StreamDetector.step: frame {i} must be uint8 [{h}, {w}, 3], not {src.dtype} {list(src.shape)}")
+                if src.is_cuda:
+                    t.frames[i, :h, :w].copy_(src)
+                else:                                 # only the frame's h x w pixels cross, not the whole slot
+                    stage = self._stage[i].view(-1)[:h * w * 3].view(h, w, 3)
+                    stage.copy_(src)
+                    t.frames[i, :h, :w].copy_(stage, non_blocking=True)
+        else:
+            ops._require(all(s == self.frame_hw for s in self.frame_sizes),
+                         f"StreamDetector.step: give a list of {self.streams} frames, one per stream")
+            src = step_frames(frames, self.streams, self.frame_hw)
             if src.is_cuda:
-                t.frames[i, :h, :w].copy_(src)
-            else:                                     # only the frame's h x w pixels cross, not the whole slot
-                self._stage[i].copy_(src)
-                t.frames[i, :h, :w].copy_(self._stage[i], non_blocking=True)
-        return self._run_sized(None)
+                t.frames.copy_(src)
+            else:
+                self._stage.copy_(src)
+                t.frames.copy_(self._stage, non_blocking=True)
+        return self._run(None)
+
+    def last_raw(self):
+        """A device copy of the last tick's head outputs [S, A, 5 + nc] (what the driver keeps as ``results_raw``)."""
+        return self._tick.raw.clone()
 
     def step_jpeg(self, files):
         """One JPEG file per stream -> a list of S ``(bboxes, scores, labels)`` tuples as ``step`` returns them, with one
@@ -345,11 +291,12 @@ class StreamDetector:
             if a.size:
                 t.bytes[i, :a.size].copy_(self._jstage[i, :a.size], non_blocking=True)
         t.lengths.copy_(self._jlen, non_blocking=True)
-        return self._run_sized([a.size > 0 for a in files])
+        return self._run([a.size > 0 for a in files])
 
-    def _run_sized(self, present):
+    def _run(self, present):
+        """Replay the tick on the staged inputs and return the detections; ``present`` (JPEG ticks only): which streams
+        were given a file."""
         t = self._tick
-        flags = self._flags.numpy().copy()
         t.flags.copy_(self._flags, non_blocking=True)
         self._graph.replay()
         self._det.copy_(t.det, non_blocking=True)
@@ -360,7 +307,7 @@ class StreamDetector:
         if present is None:
             self._flags.zero_()
         else:
-            self._last_status, nxt = route_status(self._status.numpy(), present, flags)
+            self._last_status, nxt = route_status(self._status.numpy(), present, self._flags.numpy())
             self._flags.copy_(torch.from_numpy(nxt))
         det = self._det.numpy()
         return [sized_output(det[i, :n]) for i, n in enumerate(self._count.tolist())]

@@ -1,10 +1,11 @@
 """The streaming detector (streamyolo_b200.stream): the sAP driver's per-frame loop as one CUDA graph per tick.
 
 CPU (no GPU needed):
-  * the tick the graph captures, run under the torch emulation of the kernels (tests/emul_ops.py, fp32 storage) with
-    letterbox, the per-image select and the NMS emulated here, reproduces the fp32 oracle's on_pipe forward per stream --
-    the star call for a stream that starts a sequence, the buffered call otherwise -- over a sequence with mixed resets;
-  * the driver's output conversion and the argument checks;
+  * the tick the graph captures, run under the torch emulation of the kernels (tests/emul_ops.py, fp32 storage) with the
+    per-stream resize, the start / keep gate, the per-image select, the NMS and the box division emulated here, reproduces
+    the fp32 oracle's on_pipe forward per stream -- the star call for a stream that starts a sequence, the buffered call
+    otherwise -- over a sequence with mixed resets;
+  * the host's output conversion and the argument checks;
   * select_images_kernel compiles without spills.
 
 GPU (H100):
@@ -53,11 +54,27 @@ def same_dets(a, b):
 TINY = CASES["tiny_120x160"]
 
 
-def _letterbox(src, mid, dst, out, flags=None):
-    """what sy_letterbox does for the streaming driver's preproc (no intermediate size, no mirror)"""
-    assert flags is None and tuple(mid) == tuple(src.shape[1:3])
-    for i in range(src.shape[0]):
-        out[i] = torch.from_numpy(input_oracle.stream_frame(src[i].numpy(), dst)[0])
+def _letterbox_sized(src, table, out):
+    """what sy_letterbox_sized does for rows of the driver's size: the streaming driver's preproc of each frame"""
+    for i, (h, w, dh, dw) in enumerate(table.tolist()):
+        assert (dh, dw) == tuple(out.shape[2:])
+        out[i] = torch.from_numpy(input_oracle.stream_frame(src[i, :h, :w].numpy(), (dh, dw))[0])
+
+
+def _stream_gate(status, flags, start, keep):
+    """what sy_stream_gate does"""
+    ok = torch.ones_like(flags) if status is None else (status == 0).to(torch.int32)
+    start.copy_(ok * (flags != 0).to(torch.int32))
+    keep.copy_(ok)
+
+
+def _stream_rescale(det, count, status, ratio):
+    """what sy_stream_rescale does"""
+    for i in range(det.shape[0]):
+        if status is not None and int(status[i]) != 0:
+            count[i] = 0
+        else:
+            det[i, :int(count[i]), :4] /= ratio[i]
 
 
 def _select_images(srcs, dsts, flags):
@@ -82,15 +99,17 @@ def _postprocess_nms(pred, num_classes, conf_thre, nms_thre, class_agnostic=Fals
     return det, count
 
 
-def test_tick_follows_oracle_on_pipe_per_stream(monkeypatch):
+def test_tick_follows_oracle_on_pipe_per_stream_and_divides_boxes(monkeypatch):
     """three streams over four ticks (tick 0: every stream starts; tick 2: stream 1 restarts; tick 3: streams 0 and 2): each
     stream's head outputs equal the fp32 oracle's on_pipe call on that stream alone -- star after a reset, buffered on the
     stream's previous frame otherwise -- to float roundoff, and the buffered streams really differ from a star call"""
     from test_fp16_storage import calibrated_oracle, product_from
     emul_ops.install(monkeypatch, exact=True)
-    monkeypatch.setattr(ops, "letterbox", _letterbox)
+    monkeypatch.setattr(ops, "letterbox_sized", _letterbox_sized)
+    monkeypatch.setattr(ops, "stream_gate", _stream_gate)
     monkeypatch.setattr(ops, "select_images", _select_images)
     monkeypatch.setattr(ops, "postprocess_nms", _postprocess_nms)
+    monkeypatch.setattr(ops, "stream_rescale", _stream_rescale)
     x = synth.synth_frames(TINY["B"], TINY["H"], TINY["W"])
     o = calibrated_oracle(TINY, x, synth.synth_labels(TINY["B"], TINY["H"], TINY["W"]), None)
     m = product_from(o, TINY)
@@ -98,7 +117,9 @@ def test_tick_follows_oracle_on_pipe_per_stream(monkeypatch):
     # nothing about the routing
     o.decode_in_inference = m.head.decode_in_inference = False
     S, size, fhw = 3, (TINY["H"], TINY["W"]), (2 * TINY["H"], 2 * TINY["W"])
-    tick = stream.StreamTick(m, fhw, size, S, CONF, NMS, "cpu")
+    table, ratios = data.sized_table([fhw] * S, size, 0.5)          # every frame of driver size: the plain resize
+    assert table.tolist() == [[fhw[0], fhw[1], size[0], size[1]]] * S and ratios == [0.5] * S
+    tick = stream.StreamTick(m, table, ratios, size, S, CONF, NMS, "cpu")
     resets = [(0, 1, 2), (), (1,), (0, 2)]
     bufs = [None] * S
     for t, rs in enumerate(resets):
@@ -119,17 +140,21 @@ def test_tick_follows_oracle_on_pipe_per_stream(monkeypatch):
                 assert float((star - want).norm() / want.norm()) > 100 * err, f"tick {t} stream {i}: buffer had no effect"
             d = postprocess_oracle(got, 8, CONF, NMS)[0]
             n = 0 if d is None else len(d)
+            if n:
+                d[:, :4] /= 0.5                                       # the boxes divided by the stream's ratio
             assert int(tick.count[i]) == n and (n == 0 or torch.equal(tick.det[i, :n], d))
 
 
-def test_driver_output_conversion():
-    """boxes / in_scale, obj * class_conf, the class as int32: the driver's inference() on its numpy rows"""
+def test_sized_output_conversion():
+    """the boxes as the device left them (divided by the stream's ratio, see test_stream_rescale_is_numpys_division),
+    obj * class_conf, the class as int32: the driver's inference() on its numpy rows, in arrays of their own (the rows
+    are the pinned buffer the next tick overwrites)"""
     rows = np.array([[10.5, 20.25, 110.0, 220.75, 0.9, 0.5, 3.0], [0.0, 1.0, 2.0, 3.0, 0.25, 0.75, 7.0]], np.float32)
-    b, s, lab = stream.driver_output(rows, 0.5)
-    assert b.dtype == np.float32 and np.array_equal(b, rows[:, :4] * 2)
+    b, s, lab = stream.sized_output(rows)
+    assert b.dtype == np.float32 and np.array_equal(b, rows[:, :4]) and not np.shares_memory(b, rows)
     assert s.dtype == np.float32 and np.array_equal(s, np.array([0.9 * 0.5, 0.25 * 0.75], np.float32))
     assert lab.dtype == np.int32 and lab.tolist() == [3, 7]
-    b, s, lab = stream.driver_output(np.zeros((0, 7), np.float32), 0.5)
+    b, s, lab = stream.sized_output(np.zeros((0, 7), np.float32))
     assert b.shape == (0, 4) and s.shape == (0,) and lab.shape == (0,)
 
 

@@ -12,6 +12,7 @@ GPU (H100):
     frames bit for bit; a damaged file and a file of the wrong size get their status and leave their slot untouched;
   * stream_frames_sized: the driver's preproc and the evaluation preproc of every fixture, bit for bit, with r;
   * with every size equal, both equal decode_jpeg / stream_frame;
+  * stream_rescale divides the boxes as numpy divides the driver's float32 rows by a Python float, bit for bit;
   * StreamYOLO-s (synthetic weights, fp16 storage) over a sequence with a damaged file, a stream without a frame and resets:
     one stream of each size is bit-identical to its own eager driver loop (transform, model(x, buffer, mode='on_pipe'), the
     driver's inference() with that stream's ratio); the three sizes in one detector are bit-identical, stream by stream,
@@ -222,6 +223,31 @@ def test_equal_sizes_match_the_single_size_paths():
     xb, _ = data.stream_frames_sized(big, [(1200, 1920)] * SEQ, SIZE)
     want = torch.cat([data.stream_frame(ref[k], SIZE) for k in range(SEQ)])
     assert torch.equal(x, want) and torch.equal(xb, want) and ratios == [0.5] * SEQ
+
+
+@pytest.mark.gpu
+def test_stream_rescale_is_numpys_division():
+    """the boxes of each stream's count rows equal numpy's ``rows[:, :4] / ratio`` (the driver's ``det[:, :4] / in_scale``:
+    float32 rows divided by a Python float) bit for bit, for ratios that are powers of two and ratios that are not; the
+    other columns and the rows past the count keep their bits; a stream whose status is not 0 gets count 0"""
+    rng = np.random.default_rng(3)
+    ratios = [0.5, 0.3, 1 / 3, float(G["b444.r"]), float(G["c420_r16.r"])]
+    n, max_det = len(ratios), 64
+    rows = (rng.random((n, max_det, 7)) * rng.choice([1.0, 100.0, 2000.0], (n, max_det, 7))).astype(np.float32)
+    counts = np.array([64, 37, 50, 1, 0], np.int32)
+    assert (rows[0, :, :4] / 0.3).dtype == np.float32
+    for status in (None, np.array([0, 0, 4, 0, 5], np.int32)):
+        det, count = torch.from_numpy(rows).to(DEV), torch.from_numpy(counts).to(DEV)
+        ops.stream_rescale(det, count, None if status is None else torch.from_numpy(status).to(DEV),
+                           torch.tensor(ratios, dtype=torch.float32, device=DEV))
+        got, got_n = det.cpu().numpy(), count.cpu().numpy()
+        for i, r in enumerate(ratios):
+            ok = status is None or status[i] == 0
+            want = rows[i].copy()
+            if ok:
+                want[:counts[i], :4] = rows[i, :counts[i], :4] / r
+            assert got_n[i] == (counts[i] if ok else 0), (i, status)
+            assert np.array_equal(got[i].view(np.int32), want.view(np.int32)), (i, r, status)
 
 
 def _model_s():

@@ -78,7 +78,7 @@ def eager_frame(model, frame, buffer, ev=None):
         d = np.zeros((0, 7), np.float32) if d is None else d.cpu().numpy()
     if ev is not None:
         ev[1].record()
-    out = stream.driver_output(d, IN_SCALE)
+    out = d[:, :4] / IN_SCALE, d[:, 4] * d[:, 5], d[:, 6].astype(np.int32)     # the driver's inference() conversion
     torch.cuda.synchronize()
     return out, buffer
 

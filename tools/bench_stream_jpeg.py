@@ -3,7 +3,7 @@ storage, synthetic weights with BatchNorm calibrated as in tools/bench_stream.py
 NMS 0.65).  The files are the fixtures of tests/golden/stream_jpeg_files.npz (1200x1920 4:2:0, 2048x1550 4:4:4, 1550x2048
 4:2:0 with restart markers), requantised into SEQ distinct frames each.
 
-  (a) step        today's StreamDetector.step on decoded 1200x1920 numpy frames (cv2.imread's output), host clock per frame
+  (a) step        StreamDetector.step on decoded 1200x1920 numpy frames (cv2.imread's output), host clock per frame
   (b) step_jpeg   StreamDetector(jpeg_max_bytes=...).step_jpeg on the same frames' files, host clock per frame
   (c) replay      the JPEG detector's graph alone, CUDA events
   (d) rigs        step_jpeg and the replay alone for 3 streams (1200x1920, 2048x1550, 1550x2048) and 6 (each twice)
