@@ -391,6 +391,32 @@ int sy_stream_gate(const int32_t* status, const int32_t* flags, int32_t n, int32
  * count[i] = 0 where status[i] != SY_JPEG_OK (status may be NULL). */
 int sy_stream_rescale(float* det, int32_t n, int32_t max_det, int32_t* count, const int32_t* status, const float* ratio,
                       sy_stream_t stream);
+/* Device half of the validation evaluators' convert_to_coco_format (exps/evaluators/onex_stream_evaluator.py:167-209,
+ * twox_stream_evaluator.py:165-217, still_stream_evaluator.py:137-169) for a batch of b images: the first count[i] rows
+ * of image i of sy_postprocess_nms' det [b][max_det][7] become COCO detection rows, compacted image-major in NMS order:
+ * bbox_out [N][4] = x1 / r, y1 / r, x2 / r - x1 / r, y2 / r - y1 / r (`bboxes /= scale; xyxy2xywh(bboxes)`, fp32, one
+ * rounding per operation, r = ratio[i]), score_out [N] = obj * class_conf (fp32), category_out [N] =
+ * class_ids[(int)class_pred] (-1 for a class outside [0, num_classes)), image_id_out [N] = image_id[i], and
+ * total_out [1] = N.  An image emits nothing when image_id[i] < 0 (the evaluator's frame-id rules drop it), or, with
+ * status given, when any of its frames_per_image frames status[i * frames_per_image + f] is not SY_JPEG_OK.  The outputs
+ * hold room for b * max_det rows; rows past N are not written.  All arrays in device memory; b <= 4096. */
+typedef struct SyCocoRowsDesc {
+  const float* det;
+  int32_t b, max_det;
+  const int32_t* count;        /* [b] */
+  const float* ratio;          /* [b] */
+  const int32_t* image_id;     /* [b], < 0: emit nothing */
+  const int32_t* status;       /* [b * frames_per_image] SY_JPEG_*, or NULL */
+  int32_t frames_per_image;
+  int32_t num_classes;
+  const int32_t* class_ids;    /* [num_classes] */
+  float* bbox_out;
+  float* score_out;
+  int32_t* image_id_out;
+  int32_t* category_out;
+  int32_t* total_out;
+} SyCocoRowsDesc;
+int sy_coco_rows(const SyCocoRowsDesc* d, sy_stream_t stream);
 
 /* -------- training step glue (streamyolo_b200/csrc/train_glue.cu) ---------------------------------------------- */
 /* fp32 OIHW conv parameter -> bf16 GEMM operand, on the device (one launch per parameter per optimiser step):

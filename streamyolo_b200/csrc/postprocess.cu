@@ -1,4 +1,5 @@
-// Detection post-processing on the device: confidence threshold + class-aware greedy NMS.
+// Detection post-processing on the device: confidence threshold + class-aware greedy NMS; the streaming tick's gating and
+// box division; the evaluators' COCO detection rows (coco_rows_kernel).
 //
 // Replaces [yolox 0.3.0] yolox.utils.postprocess (called at /root/reference/exps/evaluators/onex_stream_evaluator.py:148,
 // sAP/streamyolo/streamyolo_det.py:62-83): cxcywh -> xyxy, class_conf / class_pred = max over the class scores,
@@ -225,6 +226,55 @@ __global__ void __launch_bounds__(128) stream_rescale_kernel(float* __restrict__
   }
 }
 
+// Device half of the evaluators' convert_to_coco_format (see sy_coco_rows).  One CTA per image: its first output row is
+// the sum of the emitted counts of the images before it (image-major order; B is a batch, so the O(B) sum is short),
+// then one thread per row.  Block 0 also writes the total.  Explicit _rn intrinsics: the reference's fp32 torch CPU ops,
+// one rounding each.
+__device__ __forceinline__ int coco_rows_n(const int32_t* count, const int32_t* image_id, const int32_t* status, int fpi,
+                                           int max_det, int b) {
+  if (image_id[b] < 0) return 0;
+  if (status != nullptr)
+    for (int f = 0; f < fpi; ++f)
+      if (status[b * fpi + f] != SY_JPEG_OK) return 0;
+  return min(max(count[b], 0), max_det);
+}
+
+__global__ void __launch_bounds__(256) coco_rows_kernel(const SyCocoRowsDesc q) {
+  __shared__ int s_base, s_total;
+  const int b = blockIdx.x;
+  if (threadIdx.x == 0) {
+    int base = 0, total = 0;
+    for (int k = 0; k < q.b; ++k) {
+      const int n = coco_rows_n(q.count, q.image_id, q.status, q.frames_per_image, q.max_det, k);
+      if (k < b) base += n;
+      total += n;
+    }
+    s_base = base;
+    s_total = total;
+  }
+  __syncthreads();
+  if (b == 0 && threadIdx.x == 0) *q.total_out = s_total;
+  const int n = coco_rows_n(q.count, q.image_id, q.status, q.frames_per_image, q.max_det, b);
+  const float r = q.ratio[b];
+  const int id = q.image_id[b];
+  const float* rows = q.det + (size_t)b * q.max_det * 7;
+  for (int j = threadIdx.x; j < n; j += blockDim.x) {
+    const float* d = rows + (size_t)j * 7;
+    const int o = s_base + j;
+    // bboxes /= scale (fp32 tensor / Python float: torch divides by the float-rounded scale), then xyxy2xywh in place
+    const float x1 = __fdiv_rn(d[0], r), y1 = __fdiv_rn(d[1], r);
+    const float x2 = __fdiv_rn(d[2], r), y2 = __fdiv_rn(d[3], r);
+    q.bbox_out[(size_t)o * 4 + 0] = x1;
+    q.bbox_out[(size_t)o * 4 + 1] = y1;
+    q.bbox_out[(size_t)o * 4 + 2] = __fsub_rn(x2, x1);
+    q.bbox_out[(size_t)o * 4 + 3] = __fsub_rn(y2, y1);
+    q.score_out[o] = __fmul_rn(d[4], d[5]);                    // output[:, 4] * output[:, 5]
+    const int c = (int)d[6];                                    // class_ids[int(cls)]
+    q.category_out[o] = (c >= 0 && c < q.num_classes) ? q.class_ids[c] : -1;
+    q.image_id_out[o] = id;
+  }
+}
+
 static inline size_t nms_ws_bytes(int B, int A) { return ((size_t)B * A * 4 * sizeof(float) + 255) / 256 * 256 + (size_t)B * A * sizeof(int); }
 
 }  // namespace sy
@@ -275,4 +325,17 @@ extern "C" int sy_stream_rescale(float* det, int32_t n, int32_t max_det, int32_t
   SY_REQUIRE(n > 0 && n <= 65535 && max_det > 0, SY_EINVAL, "stream_rescale: bad sizes (%d streams, max_det %d)", n, max_det);
   stream_rescale_kernel<<<n, 128, 0, stream>>>(det, max_det, count, status, ratio);
   return launch_status("stream_rescale_kernel");
+}
+
+extern "C" int sy_coco_rows(const SyCocoRowsDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr, SY_EINVAL, "null descriptor");
+  SY_REQUIRE(d->det && d->count && d->ratio && d->image_id && d->class_ids && d->bbox_out && d->score_out &&
+             d->image_id_out && d->category_out && d->total_out, SY_EINVAL, "coco_rows: null pointer");
+  SY_REQUIRE(d->b > 0 && d->b <= 4096 && d->max_det > 0 && d->num_classes > 0, SY_EINVAL,
+             "coco_rows: bad sizes (%d images, max_det %d, %d classes)", d->b, d->max_det, d->num_classes);
+  SY_REQUIRE(d->status == nullptr || d->frames_per_image >= 1, SY_EINVAL, "coco_rows: frames_per_image %d",
+             d->frames_per_image);
+  coco_rows_kernel<<<d->b, 256, 0, stream>>>(*d);
+  return launch_status("coco_rows_kernel");
 }

@@ -12,9 +12,18 @@ import types
 _NAMES = ("yolox", "dfp_pafpn", "darknet", "tal_head", "pipe_head")      # every module of the reference's exps/model/
 
 
-def install(postprocess: bool = True) -> None:
+_EVALUATORS = (("onex_stream_evaluator", "ONEX_COCOEvaluator", "onex"), ("twox_stream_evaluator", "TWOX_COCOEvaluator", "twox"),
+               ("still_stream_evaluator", "STILL_COCOEvaluator", "still"))
+
+
+def install(postprocess: bool = True, evaluators: bool = False) -> None:
     """``postprocess=True`` also points ``yolox.utils.postprocess`` (imported by the reference's evaluators,
-    exps/evaluators/onex_stream_evaluator.py:14,148) at the device NMS when the yolox package is importable."""
+    exps/evaluators/onex_stream_evaluator.py:14,148) at the device NMS when the yolox package is importable.
+
+    ``evaluators=True`` replaces ``ONEX_COCOEvaluator``, ``TWOX_COCOEvaluator`` and ``STILL_COCOEvaluator`` in their
+    ``exps.evaluators.*`` modules by subclasses whose ``evaluate`` runs the batch loop on the device
+    (``streamyolo_b200.evaluate``); ``evaluate_prediction`` (COCOeval, per-class AP) stays the reference's.  Nothing
+    happens when the reference's evaluators, yolox or pycocotools cannot be imported."""
     pkg = importlib.import_module("streamyolo_b200.model")
     if "exps" not in sys.modules:
         root = types.ModuleType("exps")
@@ -33,3 +42,23 @@ def install(postprocess: bool = True) -> None:
                 yu.boxes.postprocess = device_postprocess
         except ImportError:
             pass
+    if evaluators:
+        install_evaluators()
+
+
+def install_evaluators() -> None:
+    """The ``evaluators=True`` part of ``install``."""
+    try:
+        import pycocotools  # noqa: F401
+        import yolox.utils  # noqa: F401
+    except ImportError:
+        return
+    from .evaluate import DeviceEvaluator, device_evaluator
+    for mod, name, rule in _EVALUATORS:
+        try:
+            m = importlib.import_module(f"exps.evaluators.{mod}")
+        except ImportError:
+            continue
+        base = getattr(m, name, None)
+        if base is not None and not issubclass(base, DeviceEvaluator):
+            setattr(m, name, device_evaluator(base, rule))

@@ -156,6 +156,14 @@ class SySelectImagesDesc(C.Structure):
     _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
 
 
+class SyCocoRowsDesc(C.Structure):
+    _fields_ = [("det", C.c_void_p), ("b", C.c_int32), ("max_det", C.c_int32), ("count", C.c_void_p), ("ratio", C.c_void_p),
+                ("image_id", C.c_void_p), ("status", C.c_void_p), ("frames_per_image", C.c_int32),
+                ("num_classes", C.c_int32), ("class_ids", C.c_void_p), ("bbox_out", C.c_void_p),
+                ("score_out", C.c_void_p), ("image_id_out", C.c_void_p), ("category_out", C.c_void_p),
+                ("total_out", C.c_void_p)]
+
+
 # every symbol include/streamyolo_sm100.h declares: (restype, argtypes)
 _SIG = {
     "sy_last_error_string": (C.c_char_p, []),
@@ -201,6 +209,7 @@ _SIG = {
     "sy_postprocess_nms": (C.c_int, [C.POINTER(SyNmsDesc), C.c_void_p]),
     "sy_stream_gate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sy_stream_rescale": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sy_coco_rows": (C.c_int, [C.POINTER(SyCocoRowsDesc), C.c_void_p]),
     "sy_conv2d_wgrad_workspace_bytes": (C.c_size_t, [C.POINTER(SyConvWgradDesc)]),
     "sy_conv2d_wgrad_tc": (C.c_int, [C.POINTER(SyConvWgradDesc), C.c_void_p]),
     "sy_pack_conv_weight": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
@@ -532,6 +541,42 @@ def stream_rescale(det, count, status, ratio):
              "stream_rescale: status must be int32 [n]")
     _check(lib().sy_stream_rescale(det.data_ptr(), n, det.shape[1], count.data_ptr(),
                                    status.data_ptr() if status is not None else None, ratio.data_ptr(), _stream()))
+
+
+def coco_rows(det, count, ratio, image_id, class_ids, status=None, out=None):
+    """COCO detection rows of a batch of NMS outputs (sy_coco_rows): ``det`` fp32 [B, max_det, 7] and ``count`` int32 [B]
+    of postprocess_nms, ``ratio`` fp32 [B], ``image_id`` int32 [B] (< 0: the image emits nothing), ``class_ids`` int32
+    [num_classes]; ``status`` int32 [B * F] decode status of each image's F frames (an image with a frame not decoded emits
+    nothing), or None.  -> ``(bbox fp32 [B * max_det, 4] xywh, score fp32 [B * max_det], image_id int32 [B * max_det],
+    category int32 [B * max_det], total int32 [1])``: the first ``total`` rows are valid.  ``out``: those five tensors of an
+    earlier call to write into (static buffers for CUDA-graph capture).  Nothing is read back."""
+    _require(_tensor_ok(det, torch.float32, 3) and det.shape[2] == 7 and det.is_cuda,
+             "coco_rows: det must be contiguous CUDA float32 [B, max_det, 7]")
+    b, max_det, _ = det.shape
+    for name, t, dt in (("count", count, torch.int32), ("ratio", ratio, torch.float32), ("image_id", image_id, torch.int32)):
+        _require(_tensor_ok(t, dt, 1) and t.numel() == b and t.device == det.device, f"coco_rows: {name} must be {dt} [{b}]")
+    _require(_tensor_ok(class_ids, torch.int32, 1) and class_ids.numel() > 0 and class_ids.device == det.device,
+             "coco_rows: class_ids must be int32 [num_classes]")
+    _require(status is None or (_tensor_ok(status, torch.int32, 1) and status.numel() % b == 0 and status.numel() > 0
+                                and status.device == det.device), f"coco_rows: status must be int32 [{b} * frames]")
+    cap = b * max_det
+    if out is None:
+        out = (torch.empty((cap, 4), dtype=torch.float32, device=det.device),
+               torch.empty((cap,), dtype=torch.float32, device=det.device),
+               torch.empty((cap,), dtype=torch.int32, device=det.device),
+               torch.empty((cap,), dtype=torch.int32, device=det.device),
+               torch.empty((1,), dtype=torch.int32, device=det.device))
+    bbox, score, ids, cat, total = out
+    _require(_tensor_ok(bbox, torch.float32, 2) and tuple(bbox.shape) == (cap, 4) and _tensor_ok(score, torch.float32, 1)
+             and _tensor_ok(ids, torch.int32, 1) and _tensor_ok(cat, torch.int32, 1) and _tensor_ok(total, torch.int32, 1)
+             and score.numel() == ids.numel() == cat.numel() == cap and total.numel() == 1,
+             f"coco_rows: out must be fp32 [{cap}, 4], fp32 [{cap}], int32 [{cap}], int32 [{cap}], int32 [1]")
+    d = SyCocoRowsDesc(det.data_ptr(), b, max_det, count.data_ptr(), ratio.data_ptr(), image_id.data_ptr(),
+                       status.data_ptr() if status is not None else None,
+                       status.numel() // b if status is not None else 1, class_ids.numel(), class_ids.data_ptr(),
+                       bbox.data_ptr(), score.data_ptr(), ids.data_ptr(), cat.data_ptr(), total.data_ptr())
+    _check(lib().sy_coco_rows(C.byref(d), _stream()))
+    return out
 
 
 def head_pred_decode(cls_feat: View, reg_feat: View, w_reg, b_reg, w_obj, b_obj, w_cls, b_cls, stride,
