@@ -1,14 +1,19 @@
-// Detection post-processing on the device: confidence threshold + class-aware greedy NMS; the streaming tick's gating and
-// box division; the evaluators' COCO detection rows (coco_rows_kernel).
+// Detection post-processing on the device: confidence threshold + greedy NMS; the streaming tick's gating and box
+// division; the evaluators' COCO detection rows (coco_rows_kernel).
 //
 // Replaces [yolox 0.3.0] yolox.utils.postprocess (called at /root/reference/exps/evaluators/onex_stream_evaluator.py:148,
 // sAP/streamyolo/streamyolo_det.py:62-83): cxcywh -> xyxy, class_conf / class_pred = max over the class scores,
-// keep obj * class_conf >= conf_thre, torchvision.ops.batched_nms(boxes, obj * class_conf, class, nms_thre), rows
-// [x1, y1, x2, y2, obj, class_conf, class_pred] in decreasing score order.  The reference does this per image in Python
-// with torchvision's NMS; here one CTA per image: composite-key bitonic sort in shared memory (score descending, anchor
-// index ascending on ties: deterministic), greedy suppression with the IoU arithmetic of torchvision's kernel
-// (inter / (area_i + area_j - inter) > thr, no +1), compaction.  Compiled with -fmad=false: every decision is bit-exact
-// against the fp32 restatement in oracle/postprocess_oracle.py.
+// keep obj * class_conf >= conf_thre, torchvision.ops.batched_nms(boxes, obj * class_conf, class, nms_thre) (class-
+// agnostic: torchvision.ops.nms), rows [x1, y1, x2, y2, obj, class_conf, class_pred] in decreasing score order.  The
+// reference runs it per image on CUDA tensors, where torchvision 0.26's batched_nms takes _batched_nms_coordinate_trick
+// (up to 100 000 box coordinates; this kernel takes at most 16 384 anchors): every candidate box is shifted by
+// class * (max candidate coordinate + 1) in fp32 (a NaN coordinate makes every offset NaN), then one class-agnostic nms
+// runs on the shifted boxes, so boxes of different classes can suppress each other when their shifted boxes overlap.
+// Here one CTA per image: composite-key bitonic sort in shared memory (score descending, anchor index ascending on ties,
+// as torchvision's stable sort), the same offsets, greedy suppression with the IoU arithmetic of torchvision's CUDA
+// kernel (devIoU as compiled for sm_90: inter / (fma(w_b, h_b, w_a * h_a) - inter) > float(thr), a the earlier box, b
+// the later one, no +1), compaction of the unshifted boxes.  Compiled with -fmad=false and explicit _rn intrinsics:
+// every decision is bit-exact against the fp32 restatement in oracle/postprocess_oracle.py (nms_reference).
 #include "common.cuh"
 
 namespace sy {
@@ -25,6 +30,29 @@ struct NmsArgs {
   float* det;              // [B][max_det][7]
   int* count;              // [B]
 };
+
+// xyxy of one prediction row, as yolox: cx - w / 2, cy - h / 2, cx + w / 2, cy + h / 2, one rounding each (w * 0.5 is
+// w / 2 exactly)
+__device__ __forceinline__ void box_corners(const float* r, float c[4]) {
+  const float hw = __fmul_rn(r[2], 0.5f), hh = __fmul_rn(r[3], 0.5f);
+  c[0] = __fsub_rn(r[0], hw); c[1] = __fsub_rn(r[1], hh); c[2] = __fadd_rn(r[0], hw); c[3] = __fadd_rn(r[1], hh);
+}
+
+// max that propagates NaN, like torch.max (fmaxf ignores it)
+__device__ __forceinline__ float max_nan(float a, float b) { return (b > a || b != b) ? b : a; }
+
+// torchvision's devIoU(a, b) > thr as compiled for sm_90 (nms_kernel_impl<float>): a is the earlier box (cur_box), its
+// area a plain product; the later box's area is fused into the sum; fmaxf / fminf for the intersection.  inter == 0
+// makes the ratio +-0 or NaN, which is never > a threshold >= 0: the division is skipped then.
+__device__ __forceinline__ bool iou_above(float ax1, float ay1, float ax2, float ay2, float a_area, float bx1, float by1,
+                                          float bx2, float by2, float thr) {
+  const float w = fmaxf(__fsub_rn(fminf(ax2, bx2), fmaxf(ax1, bx1)), 0.f);
+  const float h = fmaxf(__fsub_rn(fminf(ay2, by2), fmaxf(ay1, by1)), 0.f);
+  const float inter = __fmul_rn(w, h);
+  if (!(inter > 0.f) && thr >= 0.f) return false;
+  const float den = __fsub_rn(__fmaf_rn(__fsub_rn(bx2, bx1), __fsub_rn(by2, by1), a_area), inter);
+  return __fdiv_rn(inter, den) > thr;
+}
 
 __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
   extern __shared__ unsigned long long keys[];                 // [Apad], then removed flags [Apad] bytes, then scan scratch
@@ -62,7 +90,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
       __syncthreads();
     }
   }
-  // ---- 3. number of candidates (keys are sorted: first zero key), sorted boxes / classes
+  // ---- 3. number of candidates (keys are sorted: first zero key), sorted boxes / classes, the max candidate coordinate
   if (tid == 0) s_n = 0;
   __syncthreads();
   for (int i = tid; i < q.Apad; i += kNmsThreads)
@@ -71,11 +99,16 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
   const int n = s_n;
   float* BX = q.boxes + (size_t)b * q.A * 4;
   int* CL = q.cls + (size_t)b * q.A;
+  float mx = -INFINITY;
   for (int j = tid; j < n; j += kNmsThreads) {
     const int a = (int)(0xFFFFFFFFu - (unsigned)(keys[j] & 0xFFFFFFFFull));
     const float* r = P + (size_t)a * no;
-    const float hw = r[2] / 2.f, hh = r[3] / 2.f;
-    BX[j * 4 + 0] = r[0] - hw; BX[j * 4 + 1] = r[1] - hh; BX[j * 4 + 2] = r[0] + hw; BX[j * 4 + 3] = r[1] + hh;
+    float c[4];
+    box_corners(r, c);
+    for (int e = 0; e < 4; ++e) {
+      BX[j * 4 + e] = c[e];
+      mx = max_nan(mx, c[e]);
+    }
     int best = 0;
     float bv = r[5];
     for (int k = 1; k < q.NC; ++k)
@@ -83,45 +116,51 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
     CL[j] = best;
     removed[j] = 0;
   }
+  // batched_nms's offsets: boxes + class * (boxes.max() + 1), fp32, NaN propagating like torch.max.  Each thread shifts
+  // the boxes it wrote.
+  __shared__ float s_max[kNmsThreads / 32];
+  for (int m = 16; m > 0; m >>= 1) mx = max_nan(mx, __shfl_xor_sync(0xffffffffu, mx, m));
+  if ((tid & 31) == 0) s_max[tid >> 5] = mx;
+  __syncthreads();
+  if (!q.class_agnostic) {
+    mx = s_max[0];
+    for (int w = 1; w < kNmsThreads / 32; ++w) mx = max_nan(mx, s_max[w]);
+    const float step = __fadd_rn(mx, 1.f);
+    for (int j = tid; j < n; j += kNmsThreads) {
+      const float off = __fmul_rn((float)CL[j], step);
+      for (int e = 0; e < 4; ++e) BX[j * 4 + e] = __fadd_rn(BX[j * 4 + e], off);
+    }
+  }
   __syncthreads();
   // ---- 4. greedy suppression in score order, 32 candidates at a time.  (One block-wide barrier per candidate -- the first
   //         version -- cost ~0.25 ms for 2000 candidates; now two barriers per 32.)
   //   (a) warp 0 settles the chunk among its own members: lane l owns candidate c0 + l; for i = 0..31 in order, if candidate
-  //       i is still alive, the later lanes of the same class test their box against it (the box of i comes by shuffle);
+  //       i is still alive, the later lanes test their box against it (the box of i comes by shuffle);
   //   (b) all threads apply the chunk's survivors to the candidates behind the chunk.
-  //   Same decisions as the sequential loop: a candidate is removed iff a kept earlier candidate of its class overlaps it.
+  //   Same decisions as the sequential loop: a candidate is removed iff a kept earlier candidate overlaps it, the earlier
+  //   one in devIoU's first place.  No class test: the offsets keep classes apart exactly as far as the reference does.
   __shared__ float s_kbox[32][4];
   __shared__ float s_karea[32];
-  __shared__ int s_kcls[32];
   __shared__ int s_nk;
+  const float thr = q.nms_thre;
   for (int c0 = 0; c0 < n; c0 += 32) {
     if (tid < 32) {
       const int j = c0 + tid;
       const bool in = j < n;
       float x1 = 0.f, y1 = 0.f, x2 = 0.f, y2 = 0.f;
-      int cl = -1;
       bool alive = false;
       if (in) {
         x1 = BX[j * 4]; y1 = BX[j * 4 + 1]; x2 = BX[j * 4 + 2]; y2 = BX[j * 4 + 3];
-        cl = CL[j];
         alive = removed[j] == 0;
       }
-      const float area = (x2 - x1) * (y2 - y1);
+      const float area = __fmul_rn(__fsub_rn(x2, x1), __fsub_rn(y2, y1));
       for (int i = 0; i < 32; ++i) {
         const unsigned live = __ballot_sync(0xffffffffu, alive);
         if (!((live >> i) & 1u)) continue;                   // candidate i was removed (or lies past n): uniform
         const float ix1 = __shfl_sync(0xffffffffu, x1, i), iy1 = __shfl_sync(0xffffffffu, y1, i);
         const float ix2 = __shfl_sync(0xffffffffu, x2, i), iy2 = __shfl_sync(0xffffffffu, y2, i);
         const float iarea = __shfl_sync(0xffffffffu, area, i);
-        const int ic = __shfl_sync(0xffffffffu, cl, i);
-        if (alive && tid > i && (q.class_agnostic || cl == ic)) {
-          const float xx1 = fmaxf(ix1, x1), yy1 = fmaxf(iy1, y1);
-          const float xx2 = fminf(ix2, x2), yy2 = fminf(iy2, y2);
-          const float w = fmaxf(0.f, xx2 - xx1), h = fmaxf(0.f, yy2 - yy1);
-          const float inter = w * h;
-          const float ovr = inter / (iarea + area - inter);
-          if (ovr > q.nms_thre) alive = false;
-        }
+        if (alive && tid > i && iou_above(ix1, iy1, ix2, iy2, iarea, x1, y1, x2, y2, thr)) alive = false;
       }
       if (in && !alive) removed[j] = 1;
       // survivors of the chunk, compacted (order irrelevant for step (b))
@@ -130,7 +169,6 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
         const int k = __popc(live & ((1u << tid) - 1u));
         s_kbox[k][0] = x1; s_kbox[k][1] = y1; s_kbox[k][2] = x2; s_kbox[k][3] = y2;
         s_karea[k] = area;
-        s_kcls[k] = cl;
       }
       if (tid == 0) s_nk = __popc(live);
     }
@@ -140,16 +178,11 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
       for (int j = c0 + 32 + tid; j < n; j += kNmsThreads) {
         if (removed[j]) continue;
         const float x1 = BX[j * 4], y1 = BX[j * 4 + 1], x2 = BX[j * 4 + 2], y2 = BX[j * 4 + 3];
-        const float jarea = (x2 - x1) * (y2 - y1);
-        const int cl = CL[j];
         for (int k = 0; k < nk; ++k) {
-          if (!q.class_agnostic && s_kcls[k] != cl) continue;
-          const float xx1 = fmaxf(s_kbox[k][0], x1), yy1 = fmaxf(s_kbox[k][1], y1);
-          const float xx2 = fminf(s_kbox[k][2], x2), yy2 = fminf(s_kbox[k][3], y2);
-          const float w = fmaxf(0.f, xx2 - xx1), h = fmaxf(0.f, yy2 - yy1);
-          const float inter = w * h;
-          const float ovr = inter / (s_karea[k] + jarea - inter);
-          if (ovr > q.nms_thre) { removed[j] = 1; break; }
+          if (iou_above(s_kbox[k][0], s_kbox[k][1], s_kbox[k][2], s_kbox[k][3], s_karea[k], x1, y1, x2, y2, thr)) {
+            removed[j] = 1;
+            break;
+          }
         }
       }
     }
@@ -185,7 +218,7 @@ __global__ void __launch_bounds__(kNmsThreads) nms_kernel(const NmsArgs q) {
       float bv = r[5];
       for (int k = 1; k < q.NC; ++k) bv = r[5 + k] > bv ? r[5 + k] : bv;
       float* o = q.det + ((size_t)b * q.max_det + pos) * 7;
-      o[0] = BX[j * 4]; o[1] = BX[j * 4 + 1]; o[2] = BX[j * 4 + 2]; o[3] = BX[j * 4 + 3];
+      box_corners(r, o);                                       // the unshifted corners
       o[4] = r[4]; o[5] = bv; o[6] = (float)CL[j];
     }
     base += s_scan[kNmsThreads / 32 - 1];

@@ -72,12 +72,13 @@ def test_cuda_postprocess_matches_oracle(b, a, conf, thr, agn):
 
 @pytest.mark.parametrize("seed", [11, 12, 13])
 def test_oracle_postprocess_matches_torchvision_golden(seed):
-    """The committed fixtures (oracle/make_nms_golden.py, generated with torchvision's NMS) pin the oracle without needing
-    torchvision at test time: same kept anchors, same order, rows assembled like yolox.utils.postprocess."""
+    """The committed fixtures (oracle/make_nms_golden.py, generated with torchvision's per-class NMS on the CPU: batched_nms's
+    vanilla path) pin nms_greedy without needing torchvision at test time: same kept anchors, same order, rows assembled
+    like yolox.utils.postprocess."""
     import os
     g = np.load(os.path.join(os.path.dirname(__file__), "golden", f"nms_{seed}.npz"))
     pred = torch.from_numpy(g["pred"])[None]
-    out = postprocess_oracle(pred, 8, float(g["conf"]), float(g["thr"]))[0]
+    out = postprocess_oracle(pred, 8, float(g["conf"]), float(g["thr"]), nms=nms_greedy)[0]
     keep = torch.from_numpy(g["keep"])
     p = pred[0]
     want = torch.cat([torch.stack([p[keep, 0] - p[keep, 2] / 2, p[keep, 1] - p[keep, 3] / 2, p[keep, 0] + p[keep, 2] / 2,
