@@ -450,7 +450,9 @@ int sy_pack_conv_weights_batch(const SyPackItem* items_dev, int32_t n_items, int
  * only + [yolox] ModelEMA.update (exps/train_utils/double_trainer.py:113-123, 173-175).  Elements [0, n_param) are
  * parameters in the order (BatchNorm weights, biases | decayed weights from decay_begin); [n_param, n_total) are the
  * floating-point buffers (BatchNorm running statistics) that only the EMA follows.  Step-by-step the same roundings as
- * torch.optim.SGD / ModelEMA in fp32.  found_inf (device float, may be NULL): non-zero skips the whole update. */
+ * torch.optim.SGD / ModelEMA in fp32.  found_inf (device float, may be NULL): non-zero skips the whole update, or with
+ * found_inf_ema non-zero only the parameter and momentum update: the EMA still runs ema = d * ema + (1 - d) * param, as
+ * ModelEMA.update does after a step GradScaler skipped (double_trainer.py:115-119). */
 typedef struct SySgdEmaDesc {
   float* param;              /* [n_total] model state (parameters then float buffers) */
   const float* grad;         /* [n_param] (the all-reduced flat gradient buffer) */
@@ -465,8 +467,16 @@ typedef struct SySgdEmaDesc {
    * six scalars above, so that a step captured in a CUDA graph follows the LR schedule / EMA ramp / loss scale of the
    * iteration it is replayed in (the host rewrites the 24 bytes before each replay). */
   const float* hyper;
+  int32_t found_inf_ema;     /* 0: a non-zero *found_inf skips the EMA too; else the EMA still runs (see above) */
 } SySgdEmaDesc;
 int sy_sgd_nesterov_ema_step(const SySgdEmaDesc* d, sy_stream_t stream);
+
+/* GradScaler's inf / NaN check of the gradients (torch._amp_foreach_non_finite_check_and_unscale_, behind
+ * GradScaler.step at exps/train_utils/double_trainer.py:115), over one flat fp32 buffer x[0, n) (16-byte aligned):
+ * *flag = 1.0 if any element is NaN or +-inf, else 0.0, and *count += 1 when it is 1.0 (a device counter of skipped
+ * steps).  The flag is reset by this call (a memset, then one vectorised pass), so it can be captured in a CUDA graph and
+ * replayed.  flag then goes to SySgdEmaDesc.found_inf. */
+int sy_nonfinite_flag(const float* x, int64_t n, float* flag, int32_t* count, sy_stream_t stream);
 
 /* Input pipeline on the device (SURVEY section 8 f4): Exp.preprocess (cfgs/s_s50_onex_dfp_tal_flip.py:160-171) =
  * F.interpolate(inputs, size=tsize, mode="bilinear", align_corners=False) on the NCHW fp32 frame-pair batch

@@ -7,6 +7,8 @@
 //                              GradScaler unscale + weight decay + SGD momentum (nesterov) + ModelEMA
 //                              (/root/reference/exps/train_utils/double_trainer.py:113-123, 173-175; [yolox 0.3.0]
 //                              Exp.get_optimizer, ModelEMA)
+//   * sy_nonfinite_flag        GradScaler's inf / NaN check of the flat gradient (double_trainer.py:115), feeding the
+//                              step's skip-with-EMA mode
 //   * sy_resize_bilinear       the multi-scale resize of Exp.preprocess (/root/reference/cfgs/s_s50_onex_dfp_tal_flip.py:160-171:
 //                              F.interpolate(mode="bilinear", align_corners=False)) + sy_scale_labels for the box rescale
 #include <math.h>
@@ -166,14 +168,20 @@ __global__ void __launch_bounds__(256) pack_weights_batch_kernel(const SyPackIte
 __global__ void sgd_ema_kernel(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ mbuf,
                                float* __restrict__ ema, long long n_param, long long n_total, long long decay_begin, float lr,
                                float momentum, float wd, float inv_scale, int nesterov, float ema_d, float ema_1md,
-                               const float* __restrict__ found_inf, const float* __restrict__ hyper) {
-  if (found_inf != nullptr && *found_inf != 0.f) return;          // GradScaler.step skips the update on inf / nan
+                               const float* __restrict__ found_inf, int found_inf_ema, const float* __restrict__ hyper) {
+  // GradScaler.step skips the optimiser update on inf / nan.  found_inf_ema = 0: the whole launch is skipped, EMA included;
+  // otherwise parameters and momentum stay, and the EMA still moves towards them (ModelEMA.update runs on a skipped step)
+  bool skip = false;
+  if (found_inf != nullptr && *found_inf != 0.f) {
+    if (!found_inf_ema) return;
+    skip = true;
+  }
   if (hyper != nullptr) {                                          // graph-replay safe hyper-parameters
     lr = hyper[0]; momentum = hyper[1]; wd = hyper[2]; inv_scale = hyper[3]; ema_d = hyper[4]; ema_1md = hyper[5];
   }
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n_total; i += (long long)gridDim.x * blockDim.x) {
     float v = p[i];
-    if (i < n_param) {
+    if (i < n_param && !skip) {
       float d = g[i];
       if (inv_scale != 1.0f) d = __fmul_rn(d, inv_scale);         // GradScaler.unscale_: grad.mul_(inv_scale)
       if (i >= decay_begin && wd != 0.f) d = fmaf(wd, v, d);      // grad.add(param, alpha=wd)
@@ -185,6 +193,25 @@ __global__ void sgd_ema_kernel(float* __restrict__ p, const float* __restrict__ 
     }
     if (ema != nullptr) ema[i] = __fadd_rn(__fmul_rn(ema[i], ema_d), __fmul_rn(ema_1md, v));   // v *= d; v += (1 - d) * model
   }
+}
+
+// Any NaN / +-inf among x[0, n) -> *flag = 1 and ++*count, once per launch: the block that turns the flag from 0 to 1
+// counts.  The flag is zeroed by the host entry point (a memset node in a captured graph) before this runs.  Four floats
+// per load (x 16-byte aligned), the n % 4 tail by the first threads.  Non-finite = all exponent bits set (FLT_MAX and
+// subnormals are finite), tested on the bits so that no compiler flag changes it.
+__device__ __forceinline__ bool nonfinite_bits(float v) { return (__float_as_uint(v) & 0x7f800000u) == 0x7f800000u; }
+
+__global__ void __launch_bounds__(256) nonfinite_flag_kernel(const float* __restrict__ x, long long n, float* flag,
+                                                             int* count) {
+  const long long n4 = n >> 2;
+  const float4* x4 = reinterpret_cast<const float4*>(x);
+  bool bad = false;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+    const float4 v = __ldg(x4 + i);
+    bad |= nonfinite_bits(v.x) | nonfinite_bits(v.y) | nonfinite_bits(v.z) | nonfinite_bits(v.w);
+  }
+  if (blockIdx.x == 0 && threadIdx.x < (n & 3)) bad |= nonfinite_bits(x[(n4 << 2) + threadIdx.x]);
+  if (__syncthreads_or(bad) && threadIdx.x == 0 && atomicExch(flag, 1.f) == 0.f) atomicAdd(count, 1);
 }
 
 // F.interpolate(x, size=(Ho, Wo), mode="bilinear", align_corners=False) on NCHW fp32 (ATen upsample_bilinear2d:
@@ -269,8 +296,17 @@ extern "C" int sy_sgd_nesterov_ema_step(const SySgdEmaDesc* d, sy_stream_t strea
   sgd_ema_kernel<<<grid_for(d->n_total, 256), 256, 0, stream>>>(d->param, d->grad, d->momentum_buf, d->ema, d->n_param, d->n_total,
                                                                d->decay_begin, d->lr, d->momentum, d->weight_decay,
                                                                d->inv_scale, d->nesterov, d->ema_decay, d->ema_one_minus_decay,
-                                                               d->found_inf, d->hyper);
+                                                               d->found_inf, d->found_inf_ema, d->hyper);
   return launch_status("sgd_ema_kernel");
+}
+
+extern "C" int sy_nonfinite_flag(const float* x, int64_t n, float* flag, int32_t* count, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(x != nullptr && flag != nullptr && count != nullptr && n > 0, SY_EINVAL, "nonfinite_flag: bad arguments");
+  SY_REQUIRE(reinterpret_cast<uintptr_t>(x) % 16 == 0, SY_EINVAL, "nonfinite_flag: x must be 16-byte aligned");
+  if (cudaMemsetAsync(flag, 0, sizeof(float), stream) != cudaSuccess) return launch_status("nonfinite_flag memset");
+  nonfinite_flag_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, stream>>>(x, n, flag, count);
+  return launch_status("nonfinite_flag_kernel");
 }
 
 extern "C" int sy_resize_bilinear(const float* x, int32_t nc, int32_t hi, int32_t wi, float* y, int32_t ho, int32_t wo,

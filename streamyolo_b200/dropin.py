@@ -3,9 +3,12 @@
 
     import streamyolo_b200.dropin; streamyolo_b200.dropin.install()     # before get_exp(...)
 
-Registers ``exps``, ``exps.model`` and the five model modules (yolox, dfp_pafpn, darknet, tal_head, pipe_head) in ``sys.modules`` (existing ``exps`` packages are
-kept: only the ``exps.model.*`` names are redirected)."""
+Registers ``exps.model`` and the five model modules (yolox, dfp_pafpn, darknet, tal_head, pipe_head) in ``sys.modules``.
+An ``exps`` package that is importable (the reference checkout's, when ``tools/train.py`` runs from its root) is imported
+and kept, so that ``exps.train_utils`` and ``exps.evaluators`` stay its own; only the ``exps.model.*`` names are
+redirected.  Without one, an empty ``exps`` package is registered."""
 import importlib
+import importlib.util
 import sys
 import types
 
@@ -16,19 +19,27 @@ _EVALUATORS = (("onex_stream_evaluator", "ONEX_COCOEvaluator", "onex"), ("twox_s
                ("still_stream_evaluator", "STILL_COCOEvaluator", "still"))
 
 
-def install(postprocess: bool = True, evaluators: bool = False) -> None:
+def install(postprocess: bool = True, evaluators: bool = False, trainer: bool = False) -> None:
     """``postprocess=True`` also points ``yolox.utils.postprocess`` (imported by the reference's evaluators,
     exps/evaluators/onex_stream_evaluator.py:14,148) at the device NMS when the yolox package is importable.
 
     ``evaluators=True`` replaces ``ONEX_COCOEvaluator``, ``TWOX_COCOEvaluator`` and ``STILL_COCOEvaluator`` in their
     ``exps.evaluators.*`` modules by subclasses whose ``evaluate`` runs the batch loop on the device
     (``streamyolo_b200.evaluate``); ``evaluate_prediction`` (COCOeval, per-class AP) stays the reference's.  Nothing
-    happens when the reference's evaluators, yolox or pycocotools cannot be imported."""
+    happens when the reference's evaluators, yolox or pycocotools cannot be imported.
+
+    ``trainer=True`` replaces ``exps.train_utils.double_trainer.Trainer`` (what every shipped cfg's ``get_trainer``
+    imports) by a subclass whose loop runs on the device (``streamyolo_b200.train_loop``): JPEG files in, one CUDA graph
+    replay per iteration.  Nothing happens when that module or yolox cannot be imported.  ``install(trainer=True,
+    evaluators=True)`` is the recommended pair for ``tools/train.py``: the per-epoch evaluation then runs on the device too."""
     pkg = importlib.import_module("streamyolo_b200.model")
     if "exps" not in sys.modules:
-        root = types.ModuleType("exps")
-        root.__path__ = []
-        sys.modules["exps"] = root
+        if importlib.util.find_spec("exps") is not None:   # the reference checkout's own package: its exps.train_utils,
+            importlib.import_module("exps")                 # exps.evaluators, ... must stay importable
+        else:
+            root = types.ModuleType("exps")
+            root.__path__ = []
+            sys.modules["exps"] = root
     sys.modules["exps.model"] = pkg
     setattr(sys.modules["exps"], "model", pkg)
     for n in _NAMES:
@@ -44,6 +55,8 @@ def install(postprocess: bool = True, evaluators: bool = False) -> None:
             pass
     if evaluators:
         install_evaluators()
+    if trainer:
+        install_trainer()
 
 
 def install_evaluators() -> None:
@@ -62,3 +75,16 @@ def install_evaluators() -> None:
         base = getattr(m, name, None)
         if base is not None and not issubclass(base, DeviceEvaluator):
             setattr(m, name, device_evaluator(base, rule))
+
+
+def install_trainer() -> None:
+    """The ``trainer=True`` part of ``install``; a second call changes nothing."""
+    try:
+        import yolox  # noqa: F401
+        m = importlib.import_module("exps.train_utils.double_trainer")
+    except ImportError:
+        return
+    from .train_loop import DeviceTrainer, device_trainer
+    base = getattr(m, "Trainer", None)
+    if base is not None and not issubclass(base, DeviceTrainer):
+        m.Trainer = device_trainer(base)

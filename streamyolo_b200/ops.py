@@ -94,7 +94,7 @@ class SySgdEmaDesc(C.Structure):
                 ("n_param", C.c_int64), ("n_total", C.c_int64), ("decay_begin", C.c_int64),
                 ("lr", C.c_float), ("momentum", C.c_float), ("weight_decay", C.c_float), ("inv_scale", C.c_float),
                 ("nesterov", C.c_int32), ("ema_decay", C.c_float), ("ema_one_minus_decay", C.c_float),
-                ("found_inf", C.c_void_p), ("hyper", C.c_void_p)]
+                ("found_inf", C.c_void_p), ("hyper", C.c_void_p), ("found_inf_ema", C.c_int32)]
 
 
 class SyPackItem(C.Structure):
@@ -217,6 +217,7 @@ _SIG = {
     "sy_pack_item_tiles": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32]),
     "sy_pack_conv_weights_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_void_p]),
     "sy_sgd_nesterov_ema_step": (C.c_int, [C.POINTER(SySgdEmaDesc), C.c_void_p]),
+    "sy_nonfinite_flag": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sy_resize_bilinear": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32,
                                      C.c_void_p]),
     "sy_scale_labels": (C.c_int, [C.c_void_p, C.c_int64, C.c_int32, C.c_float, C.c_float, C.c_void_p]),
@@ -776,9 +777,11 @@ def conv2d_plan(n, h, w, cin, cout, k, s, tile_mode=0, tile_bn=0):
 
 
 def sgd_nesterov_ema_step(param, grad, momentum_buf, ema, n_param, decay_begin, lr, momentum=0.9, weight_decay=5e-4,
-                          inv_scale=1.0, nesterov=True, ema_decay=0.0, found_inf=None, hyper=None):
+                          inv_scale=1.0, nesterov=True, ema_decay=0.0, found_inf=None, hyper=None, found_inf_ema=False):
     """One fused optimiser step over flat fp32 state (sy_sgd_nesterov_ema_step); ``ema`` may be None.  ``hyper``: device
-    fp32 [lr, momentum, weight_decay, inv_scale, ema_decay, 1 - ema_decay] replacing the scalars (CUDA-graph replays)."""
+    fp32 [lr, momentum, weight_decay, inv_scale, ema_decay, 1 - ema_decay] replacing the scalars (CUDA-graph replays).
+    ``found_inf``: device fp32 [1]; non-zero skips the step, and with ``found_inf_ema`` only the parameter and momentum
+    update (the EMA still follows the unchanged parameters, as ModelEMA.update does on a step GradScaler skipped)."""
     d = SySgdEmaDesc()
     d.param, d.grad, d.momentum_buf = param.data_ptr(), grad.data_ptr(), momentum_buf.data_ptr()
     d.ema = ema.data_ptr() if ema is not None else None
@@ -787,7 +790,19 @@ def sgd_nesterov_ema_step(param, grad, momentum_buf, ema, n_param, decay_begin, 
     d.ema_decay, d.ema_one_minus_decay = ema_decay, 1.0 - ema_decay
     d.found_inf = found_inf.data_ptr() if found_inf is not None else None
     d.hyper = hyper.data_ptr() if hyper is not None else None
+    d.found_inf_ema = int(found_inf_ema)
     _check(lib().sy_sgd_nesterov_ema_step(C.byref(d), _stream()))
+
+
+def nonfinite_flag(x, flag, count):
+    """GradScaler's inf / NaN check (sy_nonfinite_flag) of a flat fp32 CUDA tensor ``x``: ``flag`` (fp32 [1]) becomes 1.0
+    if any element is NaN or +-inf, else 0.0, and ``count`` (int32 [1]) goes up by one when it is 1.0.  Nothing is read
+    back; capturable."""
+    _require(x.dtype == torch.float32 and x.is_cuda and x.is_contiguous() and x.numel() > 0 and x.data_ptr() % 16 == 0,
+             "nonfinite_flag: x must be a non-empty contiguous 16-byte aligned fp32 CUDA tensor")
+    _require(flag.dtype == torch.float32 and flag.numel() == 1 and count.dtype == torch.int32 and count.numel() == 1
+             and flag.device == x.device == count.device, "nonfinite_flag: flag must be fp32 [1], count int32 [1], on x's device")
+    _check(lib().sy_nonfinite_flag(x.data_ptr(), x.numel(), flag.data_ptr(), count.data_ptr(), _stream()))
 
 
 def resize_bilinear(x, size, out=None):

@@ -340,11 +340,22 @@ class Trainer:
     [B, 3, H, W] and one label tensor (one backbone pass, model/backward.py ``_record``)."""
 
     def __init__(self, model, lr=0.01, momentum=0.9, weight_decay=5e-4, ema_decay=0.9998, use_ema=True,
-                 bucket_bytes=25 << 20, overlap=True):
+                 bucket_bytes=25 << 20, overlap=True, skip_nonfinite=False):
+        """``skip_nonfinite``: what ``GradScaler.step`` does for the reference's ``--fp16`` (double_trainer.py:113-119).
+        Every optimiser step first checks the all-reduced flat gradient for NaN / +-inf on the device (sy_nonfinite_flag;
+        every rank sees the same sums, so every rank decides the same); a flagged step leaves the parameters and momentum
+        as they are, while the EMA copy still moves towards them with that step's decay and ``updates`` still counts, as
+        ModelEMA.update does after a skipped step.  ``skipped_steps()`` reads the device counter (a synchronisation).
+        The check reads the gradient before the unscale: with a loss scale of 1 or more the unscaled gradient is finite
+        exactly when it is."""
         assert model.training and model.head.use_l1
         engine.require_bf16_training(model)
         self.model = model
         self.fs = FlatState(model, ema=use_ema)
+        self.skip_nonfinite = bool(skip_nonfinite)
+        dev = self.fs.state.device
+        self._found_inf = torch.zeros(1, dtype=torch.float32, device=dev) if self.skip_nonfinite else None
+        self._skipped = torch.zeros(1, dtype=torch.int32, device=dev) if self.skip_nonfinite else None
         self.lr, self.momentum, self.weight_decay = lr, momentum, weight_decay
         self.ema_decay, self.updates = ema_decay, 0
         self.bucket_bytes, self.overlap = bucket_bytes, overlap
@@ -410,9 +421,17 @@ class Trainer:
         if hyper is None:
             self.updates += 1
         h = self._hyper_values(lr, loss_scale)
+        guard = {}
+        if self.skip_nonfinite and found_inf is not None:
+            raise ValueError("optimizer_step: found_inf is not taken by a Trainer built with skip_nonfinite=True (it "
+                             "computes its own flag)")
+        if self.skip_nonfinite:
+            ops.nonfinite_flag(self.fs.grad, self._found_inf, self._skipped)
+            guard = {"found_inf": self._found_inf, "found_inf_ema": True}
+        elif found_inf is not None:
+            guard = {"found_inf": found_inf}
         ops.sgd_nesterov_ema_step(self.fs.state, self.fs.grad, self.fs.mom, self.fs.ema, self.fs.n_param, self.fs.decay_begin,
-                                  h[0], h[1], h[2], inv_scale=h[3], nesterov=True, ema_decay=h[4], found_inf=found_inf,
-                                  hyper=hyper)
+                                  h[0], h[1], h[2], inv_scale=h[3], nesterov=True, ema_decay=h[4], hyper=hyper, **guard)
         engine.WEIGHT_EPOCH += 1            # the conv operands follow the new masters: one batched re-pack launch
         self._repack()
 
@@ -444,13 +463,16 @@ class Trainer:
     def _capture(self, inputs, prologue, loss_scale, restore):
         """Capture one step per entry of ``inputs`` ({key: (x, targets)}; ``prologue(key, x, targets)`` at the front of
         each) into ONE graph memory pool, after one eager warm-up step per entry on a side stream (allocator, lazy module
-        attributes).  ``restore``: the warm-up steps are undone, the training state is as before the call.  Returns
-        {key: (plan, loss vector, loss_scale)}, a plan being [(graph segment, bucket all-reduced after it, or None)].  The
-        loss vectors stay referenced, so no later capture in the pool takes them over."""
+        attributes).  ``restore``: the warm-up steps are undone, the training state (and the skipped-step counter) is as
+        before the call.  Returns {key: (plan, loss vector, loss_scale, (x, targets))}, a plan being [(graph segment, bucket
+        all-reduced after it, or None)].  The loss vectors stay referenced, so no later capture in the pool takes them over;
+        so do the static inputs, which every replay writes (prologue) and reads: freed while the graph lives, their memory
+        would go to other tensors that each replay then overwrites."""
         if self._hyper is None:          # ONE block per Trainer, never reallocated: every captured graph reads its address
             self._hyper = torch.zeros(8, dtype=torch.float32, device=self.fs.state.device)
             self._hyper_slots = [(torch.zeros(8, dtype=torch.float32).pin_memory(), torch.cuda.Event()) for _ in range(2)]
         snapshot = copy.deepcopy(self.state_dict()) if restore else None
+        skipped = self._skipped.clone() if restore and self._skipped is not None else None
         self.updates += 1
         self._stage_hyper(None, loss_scale)
         side = torch.cuda.Stream()
@@ -463,6 +485,8 @@ class Trainer:
                 self.optimizer_step(hyper=self._hyper)
             if restore:
                 self.load_state_dict(snapshot)
+                if skipped is not None:
+                    self._skipped.copy_(skipped)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         torch.cuda.empty_cache()                           # the warm-up's blocks: device memory for the graphs' pool
@@ -496,13 +520,13 @@ class Trainer:
                 self.optimizer_step(hyper=self._hyper)
                 end()
             self.sink.on_bucket = None
-            graphs[key] = (plan, loss, loss_scale)
+            graphs[key] = (plan, loss, loss_scale, (x, targets))
             torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         return graphs
 
     def _replay(self, graph, lr):
-        plan, loss, loss_scale = graph
+        plan, loss, loss_scale, _ = graph
         self.updates += 1
         self._stage_hyper(lr, loss_scale)
         self._replay_plan(plan)
@@ -534,7 +558,8 @@ class Trainer:
 
         make_inputs(size) -> (x, targets)   the static input buffers of that size's graph; called for every size before
                                             anything is captured, so they live outside the graphs' memory pool;
-                                            the sizes' inputs may be views of one buffer (one graph runs at a time)
+                                            the sizes' inputs may be views of one buffer (one graph runs at a time);
+                                            the Trainer keeps them referenced as long as their graphs
         prologue(size, x, targets)          captured at the front of that size's graph, fills its inputs: e.g.
                                             ``data.pair_transform(frames, ..., out=stage)`` into a buffer at ``input_size``
                                             followed by ``data.preprocess(*stage, size, input_size, out=(x, targets))``
@@ -550,9 +575,9 @@ class Trainer:
         inputs = {s: make_inputs(s) for s in sizes}                                          # pool grows once
         self._sized = {}                                   # a second call replaces the first: its graphs go first
         self._sized = self._capture(inputs, prologue, loss_scale, restore=True)
-        buckets = [[b for _, b in plan] for plan, _, _ in self._sized.values()]
+        buckets = [[b for _, b in plan] for plan, _, _, _ in self._sized.values()]
         assert all(b == buckets[0] for b in buckets), "the gradient buckets differ between input sizes"
-        return {s: len(plan) for s, (plan, _, _) in self._sized.items()}
+        return {s: len(plan) for s, (plan, _, _, _) in self._sized.items()}
 
     def replay_size(self, size, lr=None):
         """One captured step at ``size`` (a size given to ``capture_sizes``); returns its loss dict.  Several ranks: every rank
@@ -564,6 +589,11 @@ class Trainer:
 
     def ema_state_dict(self):
         return self.fs.ema_state_dict(self.model)
+
+    def skipped_steps(self):
+        """How many optimiser steps ``skip_nonfinite`` has skipped so far (reads the device counter: a synchronisation);
+        0 without ``skip_nonfinite``."""
+        return 0 if self._skipped is None else int(self._skipped.item())
 
     # ---- training state: save, resume, BatchNorm statistics over the ranks
     # Loading copies into the buffers the step reads (fs.state, fs.mom, fs.ema, the modules' integer buffers) and never
