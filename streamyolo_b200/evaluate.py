@@ -20,14 +20,13 @@ evaluator's own ``evaluate_prediction`` (COCOeval and the per-class table stay t
 combined with (``device_evaluator(ONEX_COCOEvaluator, "onex")``; ``dropin.install(evaluators=True)`` does this for the
 three reference evaluators).
 """
-import os
 import time
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
-from . import data, ops
+from . import feed, ops
 from .model import engine
 
 RULES = {"onex": 2, "twox": 2, "still": 1}            # rule -> frames per sample
@@ -94,45 +93,37 @@ def coco_dicts(rows):
 
 class EvalBatch:
     """The work of one batch on static buffers -- what ``DeviceEvaluator`` captures as a CUDA graph per batch size.
-    Inputs: ``bytes`` uint8 [F * B, max_bytes] and ``lengths`` int32 [F * B] (the files of the B samples, F = 2 frames
-    per sample for pairs, current frame first, 1 for still), ``image_id`` int32 [B] (the output id of each sample, -1 to
-    emit nothing).  Outputs: ``status`` int32 [F * B] (data.JPEG_STATUS) and ``rows`` (ops.coco_rows' five tensors)."""
+    Inputs (``jpeg.inputs``): ``bytes`` uint8 [F * B, max_bytes] and ``lengths`` int32 [F * B] (the files of the B samples,
+    F = 2 frames per sample for pairs, current frame first, 1 for still), ``image_id`` int32 [B] (-1: emit nothing).
+    Outputs: ``jpeg.status`` int32 [F * B] (data.JPEG_STATUS) and ``rows`` (ops.coco_rows' five tensors)."""
 
     def __init__(self, model, batch, frames, frame_hw, input_size, max_bytes, conf_thre, nms_thre, class_ids, ratio, device):
-        self.model, self.batch, self.frames_per_image = model, batch, frames
-        self.hw, self.size = tuple(frame_hw), tuple(input_size)
-        self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
-        n = batch * frames
-        self.bytes = torch.zeros((n, max_bytes), dtype=torch.uint8, device=device)
-        self.lengths = torch.zeros((n,), dtype=torch.int32, device=device)
-        self.frames = torch.zeros((n, self.hw[0], self.hw[1], 3), dtype=torch.uint8, device=device)
-        self.status = torch.zeros((n,), dtype=torch.int32, device=device)
-        self.workspace = torch.empty(ops.jpeg_decode_workspace_bytes(n, max_bytes, *self.hw), dtype=torch.uint8, device=device)
-        self.x = torch.empty((batch, 3 * frames, self.size[0], self.size[1]), dtype=torch.float32, device=device)
-        self.image_id = torch.full((batch,), -1, dtype=torch.int32, device=device)
+        self.model, self.conf_thre, self.nms_thre = model, float(conf_thre), float(nms_thre)
+        self.jpeg = feed.JpegBatch(batch_spec(batch, frames, max_bytes), frames, frame_hw, input_size, device)
+        self.x = torch.empty((batch, 3 * frames, input_size[0], input_size[1]), dtype=torch.float32, device=device)
         self.ratio = torch.full((batch,), ratio, dtype=torch.float32, device=device)
         self.class_ids = class_ids
         self.rows = None
 
     def run(self):
-        data.decode_jpeg(self.bytes, self.lengths, self.hw, out=self.frames, status=self.status, workspace=self.workspace)
-        if self.frames_per_image == 2:
-            data.pair_transform(self.frames.view(self.batch, 2, self.hw[0], self.hw[1], 3), None, None, None, self.size,
-                                flip=False, raw=True, out=(self.x, None))
-        else:
-            data.frame_transform(self.frames, None, None, None, self.size, flip=False, raw=True, out=(self.x, None))
+        self.jpeg.run((self.x, None))
         with torch.no_grad():
             raw = self.model(self.x)
         det, count = ops.postprocess_nms(raw, self.model.head.num_classes, self.conf_thre, self.nms_thre,
                                          max_det=raw.shape[1])
-        self.rows = ops.coco_rows(det, count, self.ratio, self.image_id, self.class_ids, status=self.status, out=self.rows)
+        self.rows = ops.coco_rows(det, count, self.ratio, self.jpeg.inputs["image_id"], self.class_ids,
+                                  status=self.jpeg.status, out=self.rows)
 
 
 def _sample(dataset, index, frames):
-    """(file paths, (h, w)) of a dataset index: onex / twox annotations (res, support_res, img_info, resized_info, file,
-    support_file), still (res, img_info, resized_info, file)"""
-    a = dataset.annotations[index]
-    return ((a[4], a[5]), tuple(a[2])) if frames == 2 else ((a[3],), tuple(a[1]))
+    """(file paths, (h, w)) of a dataset index (the layout of feed.sample)"""
+    files, _, hw = feed.sample(dataset.annotations[index], frames)
+    return files, hw
+
+
+def batch_spec(batch, frames, max_bytes):
+    """the fields of an evaluated batch (feed.jpeg_spec and the output ids)"""
+    return dict(feed.jpeg_spec(batch, frames, max_bytes), image_id=((batch,), torch.int32))
 
 
 class DeviceEvaluator:
@@ -158,9 +149,7 @@ class DeviceEvaluator:
         self.rule = rule if rule is not None else self.rule
         if self.rule not in RULES:
             raise ValueError(f"DeviceEvaluator: rule must be one of {sorted(RULES)}, not {self.rule!r}")
-        if max_bytes is not None and (int(max_bytes) != max_bytes or not 4 <= max_bytes <= 1 << 28):
-            raise ValueError(f"DeviceEvaluator: max_bytes must be an integer in [4, 2^28], not {max_bytes}")
-        self.max_bytes = None if max_bytes is None else int(max_bytes)
+        self.max_bytes = None if max_bytes is None else feed.check_max_bytes(max_bytes, "DeviceEvaluator: max_bytes")
         ds = dataloader.dataset
         if len(ds.class_ids) != num_classes:
             raise ValueError(f"DeviceEvaluator: the dataset's class table has {len(ds.class_ids)} entries for "
@@ -170,11 +159,7 @@ class DeviceEvaluator:
         self.frames_per_image = RULES[self.rule]
         self.batches = sampler_batches(dataloader)
         used = sorted({i for b in self.batches for i in b})
-        sizes = {i: _sample(ds, i, self.frames_per_image)[1] for i in used}
-        hw = {s for s in sizes.values()}
-        if len(hw) != 1:
-            raise ValueError(f"DeviceEvaluator: one frame size per evaluator; the evaluated samples have {sorted(hw)}")
-        self.frame_hw = tuple(int(v) for v in hw.pop())
+        self.frame_hw = feed.frame_size([ds.annotations[i] for i in used], self.frames_per_image, "DeviceEvaluator")
         self.ratio = min(self.img_size[0] / float(self.frame_hw[0]), self.img_size[1] / float(self.frame_hw[1]))
         images = None if self.rule == "still" else ds.coco.dataset["images"]
         self.table = dict(zip(used, image_id_table(images, [ds.ids[i] for i in used], self.rule).tolist()))
@@ -186,10 +171,6 @@ class DeviceEvaluator:
         [N, 4] xywh in frame pixels, ``score`` fp32 [N], ``image_id`` int64 [N], ``category_id`` int64 [N]; None before."""
         return None if self._rows is None else {k: v.copy() for k, v in self._rows.items()}
 
-    def _files(self, batch):
-        ds = self.dataloader.dataset
-        return [p for i in batch for p in _sample(ds, i, self.frames_per_image)[0]]
-
     def _capture(self, model, sizes, max_bytes, device):
         """one EvalBatch and its graph per batch size, the graphs in one memory pool (they replay one at a time)"""
         class_ids = torch.tensor([int(c) for c in self.dataloader.dataset.class_ids], dtype=torch.int32, device=device)
@@ -197,16 +178,7 @@ class DeviceEvaluator:
         for b in sorted(sizes, reverse=True):
             t = EvalBatch(model, b, self.frames_per_image, self.frame_hw, self.img_size, max_bytes, self.confthre,
                           self.nmsthre, class_ids, self.ratio, device)
-            side = torch.cuda.Stream(device=device)
-            side.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(side):
-                t.run()                               # packs the conv operands and folds BatchNorm outside the graph
-            torch.cuda.current_stream().wait_stream(side)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, pool=pool, stream=engine.graph_capture_stream(device)):
-                t.run()
-            out[b] = (t, g)
+            out[b] = (t, engine.capture_graph(t.run, device, pool))
         return out
 
     def evaluate(self, model, distributed=False, half=False, trt_file=None, decoder=None, test_size=None):
@@ -229,10 +201,8 @@ class DeviceEvaluator:
         if model.head.num_classes != self.num_classes:
             raise ValueError(f"DeviceEvaluator: the model has {model.head.num_classes} classes, the evaluator "
                              f"{self.num_classes}")
-        max_bytes = self.max_bytes
-        if max_bytes is None:
-            longest = max(os.path.getsize(p) for b in self.batches for p in self._files(b))
-            max_bytes = max(4096, -(-longest // 4096) * 4096)
+        ds, fpi = self.dataloader.dataset, self.frames_per_image
+        max_bytes = self.max_bytes or feed.default_max_bytes(p for i in self.table for p in _sample(ds, i, fpi)[0])
         ops.lib()
         t0 = time.perf_counter()
         graphs = self._capture(model, {len(b) for b in self.batches}, max_bytes, device)
@@ -259,54 +229,32 @@ class DeviceEvaluator:
         batch i replays.  -> (rows, device ms of every replay but the last)."""
         n_batches, fpi = len(self.batches), self.frames_per_image
         b_max = max(len(b) for b in self.batches)
-        cur, copy = torch.cuda.current_stream(device), torch.cuda.Stream(device=device)
-        h_bytes = [torch.zeros((b_max * fpi, max_bytes), dtype=torch.uint8).pin_memory() for _ in range(2)]
-        h_len = [torch.zeros((b_max * fpi,), dtype=torch.int32).pin_memory() for _ in range(2)]
-        h_ids = [torch.zeros((b_max,), dtype=torch.int32).pin_memory() for _ in range(2)]
-        d_bytes = [torch.zeros((b_max * fpi, max_bytes), dtype=torch.uint8, device=device) for _ in range(2)]
-        d_len = [torch.zeros((b_max * fpi,), dtype=torch.int32, device=device) for _ in range(2)]
-        d_ids = [torch.zeros((b_max,), dtype=torch.int32, device=device) for _ in range(2)]
+        ds, cur = self.dataloader.dataset, torch.cuda.current_stream(device)
+        buf = feed.DoubleBuffer(batch_spec(b_max, fpi, max_bytes), b_max, device)
         cap = graphs[b_max][0].rows[0].shape[0]
-        h_rows = [(torch.empty((cap, 4), dtype=torch.float32).pin_memory(), torch.empty((cap,), dtype=torch.float32).pin_memory(),
-                   torch.empty((cap,), dtype=torch.int32).pin_memory(), torch.empty((cap,), dtype=torch.int32).pin_memory(),
-                   torch.empty((1,), dtype=torch.int32).pin_memory(), torch.empty((b_max * fpi,), dtype=torch.int32).pin_memory())
+        h_rows = [(feed.pinned((cap, 4), torch.float32), feed.pinned((cap,), torch.float32), feed.pinned((cap,), torch.int32),
+                   feed.pinned((cap,), torch.int32), feed.pinned((1,), torch.int32), feed.pinned((b_max * fpi,), torch.int32))
                   for _ in range(2)]
-        h2d_done, in_used, out_done = ([torch.cuda.Event() for _ in range(2)] for _ in range(3))
+        out_done = [torch.cuda.Event() for _ in range(2)]
         timing = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(n_batches)]
         parts = []
 
-        def read(i):                                  # host thread: files of batch i -> pinned slot i % 2
+        def read(i):                                  # host thread: files of batch i -> host slot i % 2
             s, batch = i % 2, self.batches[i]
-            h2d_done[s].synchronize()                 # the slot's previous batch has crossed
-            stage = h_bytes[s].numpy()
-            for k, path in enumerate(self._files(batch)):
-                a = np.fromfile(path, np.uint8)
-                if a.size > max_bytes:
-                    raise ValueError(f"DeviceEvaluator: dataset index {batch[k // fpi]}: {path} has {a.size} bytes, more "
-                                     f"than max_bytes = {max_bytes}")
-                stage[k, :a.size] = a
-                h_len[s][k] = a.size
-            h_ids[s][:len(batch)] = torch.tensor([self.table[i] for i in batch], dtype=torch.int32)
+            buf.slot_free(s)
+            for b, k in enumerate(batch):
+                feed.read_sample(buf.host[s], b, k, _sample(ds, k, fpi)[0], "DeviceEvaluator")
+            buf.host[s]["image_id"][:len(batch)] = [self.table[k] for k in batch]
 
         def h2d(i, fut):
             fut.result()
-            s, n = i % 2, len(self.batches[i]) * fpi
-            copy.wait_event(in_used[s])               # the device slot's previous batch has been taken in
-            with torch.cuda.stream(copy):
-                d_bytes[s][:n].copy_(h_bytes[s][:n], non_blocking=True)
-                d_len[s][:n].copy_(h_len[s][:n], non_blocking=True)
-                d_ids[s].copy_(h_ids[s], non_blocking=True)
-            h2d_done[s].record(copy)
+            buf.h2d(i % 2, len(self.batches[i]))
 
         def collect(i):                               # rows of batch i, out of pinned slot i % 2
             s, batch = i % 2, self.batches[i]
             out_done[s].synchronize()
             bbox, score, ids, cat, total, status = h_rows[s]
-            for k, st in enumerate(status[:len(batch) * fpi].tolist()):
-                if st != 0:
-                    raise RuntimeError(f"DeviceEvaluator: dataset index {batch[k // fpi]} (file "
-                                       f"{self._files([batch[k // fpi]])[k % fpi]}) did not decode: "
-                                       f"{data.JPEG_STATUS.get(st, f'status {st}')}")
+            feed.check_decoded(status, batch, ds.annotations, fpi, "DeviceEvaluator")
             n = int(total[0])
             parts.append({"bbox": bbox[:n].numpy().copy(), "score": score[:n].numpy().copy(),
                           "image_id": ids[:n].numpy().astype(np.int64), "category_id": cat[:n].numpy().astype(np.int64)})
@@ -318,11 +266,7 @@ class DeviceEvaluator:
                 for i, batch in enumerate(self.batches):
                     s, b = i % 2, len(batch)
                     t, g = graphs[b]
-                    cur.wait_event(h2d_done[s])
-                    t.bytes.copy_(d_bytes[s][:b * fpi])
-                    t.lengths.copy_(d_len[s][:b * fpi])
-                    t.image_id.copy_(d_ids[s][:b])
-                    in_used[s].record(cur)
+                    buf.take(s, t.jpeg.inputs, b)
                     timing[i][0].record(cur)
                     g.replay()
                     timing[i][1].record(cur)
@@ -331,7 +275,7 @@ class DeviceEvaluator:
                     for dst, src in zip(h_rows[s][:4], rows[:4]):
                         dst[:m].copy_(src, non_blocking=True)
                     h_rows[s][4].copy_(rows[4], non_blocking=True)
-                    h_rows[s][5][:b * fpi].copy_(t.status, non_blocking=True)
+                    h_rows[s][5][:b * fpi].copy_(t.jpeg.status, non_blocking=True)
                     out_done[s].record(cur)
                     if i + 1 < n_batches:
                         h2d(i + 1, reads.pop(i + 1))
@@ -341,8 +285,7 @@ class DeviceEvaluator:
                         collect(i - 1)
                 collect(n_batches - 1)
             finally:
-                cur.synchronize()
-                copy.synchronize()
+                buf.close()
         infer_ms = sum(a.elapsed_time(e) for a, e in timing[:-1])
         return (merge_ranks(parts) if parts else empty_rows()), infer_ms
 

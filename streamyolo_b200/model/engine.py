@@ -194,6 +194,21 @@ def graph_capture_stream(device):
     return _CAPTURE_STREAMS[key]
 
 
+def capture_graph(fn, device, pool=None):
+    """``fn`` as a CUDA graph: run once on a side stream (which packs the conv operands and folds BatchNorm outside the
+    graph), synchronised, then captured on ``graph_capture_stream(device)``, in ``pool`` if given."""
+    side = torch.cuda.Stream(device=device)
+    side.wait_stream(torch.cuda.current_stream(device))
+    with torch.cuda.stream(side):
+        fn()
+    torch.cuda.current_stream(device).wait_stream(side)
+    torch.cuda.synchronize(device)
+    g = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(g, pool=pool, stream=graph_capture_stream(device)):
+        fn()
+    return g
+
+
 def act_code(m):
     """the kernels' SY_ACT_* code of a BaseConv's activation (its ``act`` name: "silu" / "relu" / "lrelu")"""
     return ops.ACT_CODES[m.act_name]

@@ -31,7 +31,7 @@ change of the weights or running statistics) call ``capture()`` again.  Nothing 
 import numpy as np
 import torch
 
-from . import data, ops
+from . import data, feed, ops
 from .model import engine
 
 
@@ -184,8 +184,8 @@ class StreamDetector:
         size = input_size_for(sizes, in_scale, input_size)
         if min(size) < 1 or min(min(s) for s in sizes) < 1:
             raise ValueError(f"StreamDetector: frames {sizes} at in_scale {in_scale} give input size {size}")
-        if jpeg_max_bytes is not None and (int(jpeg_max_bytes) != jpeg_max_bytes or not 4 <= jpeg_max_bytes <= 1 << 28):
-            raise ValueError(f"StreamDetector: jpeg_max_bytes must be an integer in [4, 2^28], not {jpeg_max_bytes}")
+        if jpeg_max_bytes is not None:
+            jpeg_max_bytes = feed.check_max_bytes(jpeg_max_bytes, "StreamDetector: jpeg_max_bytes")
         try:
             table, ratios = data.sized_table(sizes, size, in_scale)
         except RuntimeError as e:
@@ -194,17 +194,17 @@ class StreamDetector:
         ops.lib()
         self.model, self.streams, self.in_scale, self.size = model, streams, in_scale, size
         self.frame_sizes, self.ratios = sizes, ratios
-        self.jpeg_max_bytes = None if jpeg_max_bytes is None else int(jpeg_max_bytes)
+        self.jpeg_max_bytes = jpeg_max_bytes
         self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes)
         self.frame_hw = tuple(self._tick.frames.shape[1:3])          # the slot: the largest height and width
         if self.jpeg_max_bytes is None:           # stream i's frame is staged at the start of slot i (see step)
-            self._stage = torch.empty(tuple(self._tick.frames.shape), dtype=torch.uint8).pin_memory()
+            self._stage = feed.pinned(tuple(self._tick.frames.shape), torch.uint8)
         else:
-            self._jstage = torch.empty((streams, self.jpeg_max_bytes), dtype=torch.uint8).pin_memory()
-            self._jlen = torch.zeros((streams,), dtype=torch.int32).pin_memory()
-            self._status = torch.zeros((streams,), dtype=torch.int32).pin_memory()
+            self._jstage = feed.pinned((streams, self.jpeg_max_bytes), torch.uint8)
+            self._jlen = feed.pinned((streams,), torch.int32)
+            self._status = feed.pinned((streams,), torch.int32)
         self._last_status = None
-        self._flags = torch.ones((streams,), dtype=torch.int32).pin_memory()
+        self._flags = feed.pinned((streams,), torch.int32)
         self._graph = None
         self.capture()
 
@@ -213,19 +213,9 @@ class StreamDetector:
         ``load_state_dict``.  Every stream starts a sequence at the next ``step``."""
         self._graph = None
         t = self._tick
-        side = torch.cuda.Stream()
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            t.run()                                   # packs the conv operands and folds BatchNorm outside the graph
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g, stream=engine.graph_capture_stream(t.frames.device)):
-            t.run()
-        self._graph = g
-        a = t.raw.shape[1]
-        self._det = torch.empty((self.streams, a, 7), dtype=torch.float32).pin_memory()
-        self._count = torch.empty((self.streams,), dtype=torch.int32).pin_memory()
+        self._graph = engine.capture_graph(t.run, t.frames.device)
+        self._det = feed.pinned((self.streams, t.raw.shape[1], 7), torch.float32)
+        self._count = feed.pinned((self.streams,), torch.int32)
         self.reset()
 
     def reset(self, stream=None):
@@ -277,9 +267,9 @@ class StreamDetector:
     def step_jpeg(self, files):
         """One JPEG file per stream -> a list of S ``(bboxes, scores, labels)`` tuples as ``step`` returns them, with one
         host synchronisation.  ``files``: a list of S entries, each the file's bytes (``bytes``, or a uint8 numpy array or
-        CPU tensor, e.g. ``np.fromfile(path, np.uint8)``) of at most ``jpeg_max_bytes``, or None when the stream has no
-        frame this tick.  A stream whose file did not decode (see ``last_status``) or that got None returns empty arrays,
-        keeps its carried features and, if it was to start a sequence, starts it at its next decoded frame."""
+        CPU tensor) of at most ``jpeg_max_bytes``, or None when the stream has no frame this tick.  A stream whose file
+        did not decode (see ``last_status``) or that got None returns empty arrays, keeps its carried features and, if it
+        was to start a sequence, starts it at its next decoded frame."""
         if self.jpeg_max_bytes is None:
             raise RuntimeError("StreamDetector.step_jpeg: construct the detector with jpeg_max_bytes")
         t = self._tick

@@ -24,8 +24,8 @@ the files and labels come from the wrapped dataset's ``annotations`` and ``max_l
 ``preproc``.  A pair's mirror bit is one draw with p = 1/2 (``DoubleTrainTransform``'s ``random.randrange(2)``) from a
 generator seeded by ``exp.seed`` and the rank; a still frame's is 0 (``TrainTransform``'s default ``mirror=False``).
 
-Feeding.  A host thread reads the files of iteration i + 2 into a pinned slot (``np.fromfile``) while the copy of
-iteration i + 1 (copy stream, ordered by events) and the replay of iteration i run.  The host synchronises only where
+Feeding.  A host thread reads the files of iteration i + 2 into a pinned slot while the copy of iteration i + 1 (copy
+stream, ordered by events) and the replay of iteration i run (feed.DoubleBuffer).  The host synchronises only where
 the reference does: at the print iteration (the losses), at ``exp.random_resize`` every 10 iterations (its ``.item()``)
 and at the end of an epoch.  Each iteration's JPEG status goes into a device ring that is read at those points; a frame
 that did not decode then raises ``RuntimeError`` with its dataset index, file and ``data.JPEG_STATUS`` reason, so up to
@@ -56,7 +56,7 @@ from concurrent.futures import ThreadPoolExecutor
 import numpy as np
 import torch
 
-from . import data, train
+from . import data, feed, train
 
 RING = 10                     # iterations between two synchronisations at most: random_resize syncs every 10
 
@@ -74,10 +74,8 @@ def _index(item):
 
 class BatchTable:
     """What the loop needs of the training dataset (``loader.dataset``, yolox's MosaicDetection wrapper, around
-    ``_dataset``): per dataset index the files, the float64 [n, 5] label arrays (x1, y1, x2, y2, cls, as ``pull_item``
-    returns them) and the frame size.  Pair annotations (onex / twox): ``(res, support_res, img_info, resized_info, file,
-    support_file)``, frame 0 being ``file`` and label 0 ``res`` (the future boxes); still: ``(res, img_info,
-    resized_info, file)``."""
+    ``_dataset``): its ``annotations`` (feed.sample: the files, labels and frame size of a dataset index), the frames per
+    sample, the one frame size, the most label rows of a frame and the transform's ``max_labels`` and ``flip``."""
 
     def __init__(self, loader):
         wrapper = loader.dataset
@@ -87,61 +85,32 @@ class BatchTable:
         if hsv:
             raise NotImplementedError("DeviceTrainer: the cfg's preproc sets hsv=True; HSV augmentation has no device "
                                       "implementation")
-        first = self.annotations[0]
-        self.frames = 2 if len(first) == 6 else 1
-        sizes = {tuple(int(v) for v in (a[2] if self.frames == 2 else a[1])) for a in self.annotations}
-        if len(sizes) != 1:
-            raise ValueError(f"DeviceTrainer: one frame size per training set; the dataset's img_info hold {sorted(sizes)}")
-        self.frame_hw = sizes.pop()
-        self.max_rows = max(1, max(len(a[k]) for a in self.annotations for k in range(self.frames)))
-
-    def __len__(self):
-        return len(self.annotations)
-
-    def files(self, i):
-        a = self.annotations[i]
-        return (a[4], a[5]) if self.frames == 2 else (a[3],)
-
-    def labels(self, i):
-        a = self.annotations[i]
-        return (a[0], a[1]) if self.frames == 2 else (a[0],)
-
-    def longest_file(self):
-        return max(os.path.getsize(p) for i in range(len(self)) for p in self.files(i))
+        self.frames = 2 if len(self.annotations[0]) == 6 else 1
+        self.frame_hw = feed.frame_size(self.annotations, self.frames, "DeviceTrainer")
+        self.max_rows = max(1, max(len(lab) for a in self.annotations for lab in feed.sample(a, self.frames)[1]))
 
 
 class DeviceStep:
-    """The device half of the loop: the static inputs, one captured step per multi-scale size (``Trainer.capture_sizes``
-    in one memory pool), the pinned host slots and device slots of the double buffer, the copy stream and the status
-    ring.  ``DeviceTrainer`` drives it through ``host``, ``slot_free``, ``h2d``, ``replay`` and ``sync``; tests put a
-    stand-in with the same methods in its place."""
+    """The device half of the loop: the static inputs and their decode + transform, one captured step per multi-scale
+    size (``Trainer.capture_sizes`` in one memory pool), the double buffer and the status ring.  ``DeviceTrainer`` drives
+    it through ``host``, ``slot_free``, ``h2d``, ``replay`` and ``sync``; tests put a stand-in with the same methods in its
+    place."""
 
     def __init__(self, tr, table, batch, input_size, sizes, max_bytes, device):
         self.tr, self.batch, self.fpi = tr, batch, table.frames
-        self.hw, self.input_size, self.max_labels, self.flip = table.frame_hw, tuple(input_size), table.max_labels, table.flip
+        self.input_size, self.max_labels = tuple(input_size), table.max_labels
         n, R, dev = batch * self.fpi, table.max_rows, device
         lab = (batch, self.fpi, R, 5) if self.fpi == 2 else (batch, R, 5)
         cnt = (batch, self.fpi) if self.fpi == 2 else (batch,)
-
-        def slot(make):
-            return {"bytes": make((n, max_bytes), torch.uint8), "lengths": make((n,), torch.int32),
-                    "ann": make(lab, torch.float64), "counts": make(cnt, torch.int32), "mirror": make((batch,), torch.int32)}
-
-        self.static = slot(lambda s, t: torch.zeros(s, dtype=t, device=dev))
-        self.dev_slots = [slot(lambda s, t: torch.zeros(s, dtype=t, device=dev)) for _ in range(2)]
-        self._host = [slot(lambda s, t: torch.zeros(s, dtype=t).pin_memory()) for _ in range(2)]
-        self.host = [{k: v.numpy() for k, v in h.items()} for h in self._host]
-        self.frames = torch.zeros((n, self.hw[0], self.hw[1], 3), dtype=torch.uint8, device=dev)
-        self.status = torch.zeros((n,), dtype=torch.int32, device=dev)
+        spec = dict(feed.jpeg_spec(batch, self.fpi, max_bytes), ann=(lab, torch.float64), counts=(cnt, torch.int32),
+                    mirror=((batch,), torch.int32))
+        self.buffer = feed.DoubleBuffer(spec, batch, dev)
+        self.host = self.buffer.host
+        self.jpeg = feed.JpegBatch(spec, self.fpi, table.frame_hw, self.input_size, dev, table.max_labels, table.flip)
         self.ring = torch.zeros((RING, n), dtype=torch.int32, device=dev)
-        self.workspace = torch.empty(train.ops.jpeg_decode_workspace_bytes(n, max_bytes, *self.hw), dtype=torch.uint8,
-                                     device=dev)
         c = 3 * self.fpi
         self.stage = self._buffers(self.input_size, dev)
         self.shared = torch.empty(batch * c * max(h * w for h, w in sizes), dtype=torch.float32, device=dev)
-        self.copy = torch.cuda.Stream(device=dev)
-        self.h2d_done = [torch.cuda.Event() for _ in range(2)]
-        self.in_used = [torch.cuda.Event() for _ in range(2)]
         self.sizes, self.dev, self.n_ring, self.losses = sizes, dev, 0, None
 
     def _buffers(self, size, dev, x=None):
@@ -159,47 +128,27 @@ class DeviceStep:
         return self._buffers(size, self.dev, self.shared[:b * c * size[0] * size[1]].view((b, c) + tuple(size)))
 
     def _prologue(self, size, x, targets):
-        st = self.static
-        data.decode_jpeg(st["bytes"], st["lengths"], self.hw, out=self.frames, status=self.status, workspace=self.workspace)
-        if self.fpi == 2:
-            data.pair_transform(self.frames.view(self.batch, 2, self.hw[0], self.hw[1], 3), st["ann"], st["counts"],
-                                st["mirror"], self.input_size, max_labels=self.max_labels, flip=self.flip, raw=True,
-                                out=self.stage)
-        else:
-            data.frame_transform(self.frames, st["ann"], st["counts"], st["mirror"], self.input_size,
-                                 max_labels=self.max_labels, flip=self.flip, raw=True, out=self.stage)
+        self.jpeg.run(self.stage)
         data.preprocess(self.stage[0], self.stage[1], size, self.input_size, out=(x, targets))
-
-    def _take(self, s):
-        """device slot s -> the static inputs, on the current stream after its copy"""
-        cur = torch.cuda.current_stream(self.dev)
-        cur.wait_event(self.h2d_done[s])
-        for k, v in self.static.items():
-            v.copy_(self.dev_slots[s][k])
-        self.in_used[s].record(cur)
 
     def capture(self, s):
         """capture every size on the batch in slot s (the capture trains nothing: Trainer.capture_sizes restores the state)"""
-        self._take(s)
+        self.buffer.take(s, self.jpeg.inputs, self.batch)
         self.tr.capture_sizes(self.sizes, self._make_inputs, self._prologue)
 
     def slot_free(self, s):
         """(reader thread) block until the last copy out of host slot s has run"""
-        self.h2d_done[s].synchronize()
+        self.buffer.slot_free(s)
 
     def h2d(self, s):
-        self.copy.wait_event(self.in_used[s])          # the device slot's previous batch has been taken in
-        with torch.cuda.stream(self.copy):
-            for k, v in self.dev_slots[s].items():
-                v.copy_(self._host[s][k], non_blocking=True)
-        self.h2d_done[s].record(self.copy)
+        self.buffer.h2d(s, self.batch)
 
     def replay(self, s, size, lr):
         """one step on the batch in slot s at ``size`` with learning rate ``lr``; its status goes into the ring.  Returns
         the graph's loss dict: device tensors that the next replay overwrites."""
-        self._take(s)
+        self.buffer.take(s, self.jpeg.inputs, self.batch)
         self.losses = self.tr.replay_size(size, lr)
-        self.ring[self.n_ring % RING].copy_(self.status)
+        self.ring[self.n_ring % RING].copy_(self.jpeg.status)
         self.n_ring += 1
         return self.losses
 
@@ -210,8 +159,7 @@ class DeviceStep:
         return [rows[(self.n_ring - pending + j) % RING] for j in range(pending)]
 
     def close(self):
-        torch.cuda.current_stream(self.dev).synchronize()
-        self.copy.synchronize()
+        self.buffer.close()
 
 
 class DeviceTrainer:
@@ -327,17 +275,17 @@ class DeviceTrainer:
         """the batch iterator, the reader thread, the device step (its graphs captured on the first batch), and the
         reads of the first two iterations"""
         t = self.table
-        max_bytes = self.max_bytes
-        if max_bytes is None:
-            max_bytes = max(4096, -(-t.longest_file() // 4096) * 4096)
-        self._max_bytes = int(max_bytes)
+        if self.max_bytes is None:
+            max_bytes = feed.default_max_bytes(p for a in t.annotations for p in feed.sample(a, t.frames)[0])
+        else:
+            max_bytes = feed.check_max_bytes(self.max_bytes, "DeviceTrainer: max_bytes")
         self._batches = iter(self.train_loader.batch_sampler)
         self._rng = np.random.default_rng([int(self.exp.seed or 0), int(self.rank)])
         self._reader = ThreadPoolExecutor(max_workers=1)
         self._left = (self.max_epoch - self.start_epoch) * self.max_iter       # iterations still to be read
         batch = self.train_loader.batch_sampler.batch_size
         sizes = train.multiscale_sizes(self.exp.input_size, self.exp.random_size)
-        self.step = self.step_class(self.tr, t, batch, self.exp.input_size, sizes, self._max_bytes, self.device)
+        self.step = self.step_class(self.tr, t, batch, self.exp.input_size, sizes, max_bytes, self.device)
         self._reads, self._k, self._pending = [], 0, []
         self._submit()
         self._submit()
@@ -357,30 +305,21 @@ class DeviceTrainer:
 
     def _read(self, s, idx, mirror):
         """(reader thread) files, labels and mirror bits of one batch -> host slot s"""
-        t, fpi = self.table, self.table.frames
+        fpi = self.table.frames
         self.step.slot_free(s)
         h = self.step.host[s]
         if len(idx) != h["mirror"].shape[0]:
             raise ValueError(f"DeviceTrainer: the batch sampler yielded {len(idx)} indices, the step takes "
                              f"{h['mirror'].shape[0]} (drop_last=False with an uneven last batch is not supported)")
-        h["counts"][...] = 0
-        h["ann"][...] = 0
+        ann, counts = h["ann"].reshape(len(idx), fpi, -1, 5), h["counts"].reshape(len(idx), fpi)     # views
+        ann[...] = 0
+        counts[...] = 0
         for b, i in enumerate(idx):
-            for f, path in enumerate(t.files(i)):
-                a = np.fromfile(path, np.uint8)
-                if a.size > self._max_bytes:
-                    raise ValueError(f"DeviceTrainer: dataset index {i}: {path} has {a.size} bytes, more than "
-                                     f"max_bytes = {self._max_bytes}")
-                h["bytes"][b * fpi + f, :a.size] = a
-                h["lengths"][b * fpi + f] = a.size
-            for f, lab in enumerate(t.labels(i)):
-                n = len(lab)
-                if fpi == 2:
-                    h["ann"][b, f, :n] = lab
-                    h["counts"][b, f] = n
-                else:
-                    h["ann"][b, :n] = lab
-                    h["counts"][b] = n
+            files, labels, _ = feed.sample(self.table.annotations[i], fpi)
+            feed.read_sample(h, b, i, files, "DeviceTrainer")
+            for f, lab in enumerate(labels):
+                ann[b, f, :len(lab)] = lab
+                counts[b, f] = len(lab)
             h["mirror"][b] = mirror[b]
 
     def _wait_read(self):
@@ -398,11 +337,7 @@ class DeviceTrainer:
         rows = self.step.sync(n)
         now = time.time()
         for idx, st in zip(self._pending, rows):
-            for k, v in enumerate(np.asarray(st)[:len(idx) * self.table.frames].tolist()):
-                if v != 0:
-                    i = idx[k // self.table.frames]
-                    raise RuntimeError(f"DeviceTrainer: dataset index {i} (file {self.table.files(i)[k % self.table.frames]}) "
-                                       f"did not decode: {data.JPEG_STATUS.get(v, f'status {v}')}")
+            feed.check_decoded(st, idx, self.table.annotations, self.table.frames, "DeviceTrainer")
         it = (now - self._sync_time) / n
         for data_time, lr in self._meter_rows:
             self.meter.update(iter_time=it, data_time=data_time, lr=lr)

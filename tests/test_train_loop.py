@@ -404,11 +404,11 @@ def tiny_build():
 
 
 def run_loop(tmp_path, monkeypatch, layout="onex", n=13, world=1, rank=0, max_epoch=2, args=None, exp_kw=None,
-             step=FakeStep, table=None):
+             step=FakeStep, table=None, max_bytes=None):
     emul_ops.install(monkeypatch, exact=True)
     mod = helpers_module(monkeypatch)
     cls = train_loop.device_trainer(mod.Trainer)
-    cls.step_class = step
+    cls.step_class, cls.max_bytes = step, max_bytes
     table = make_table(str(tmp_path / "data"), n, layout) if table is None else table
     exp = Exp(table, layout, str(tmp_path / "out"), world=world, rank=rank, max_epoch=max_epoch, build=tiny_build,
               **(exp_kw or {}))
@@ -562,6 +562,14 @@ def test_refusals(tmp_path, monkeypatch):
     table[2] = table[2][:2] + ((100, 160),) + table[2][3:]
     with pytest.raises(ValueError, match="one frame size"):
         run_loop(tmp_path / "c", monkeypatch, table=table)
+
+
+def test_max_bytes_out_of_range_is_refused_before_the_step(tmp_path, monkeypatch):
+    """a DeviceTrainer.max_bytes outside [4, 2^28] is refused when the feed starts, before a step is built or a file read"""
+    FakeStep.log = None
+    with pytest.raises(ValueError, match=r"DeviceTrainer: max_bytes must be an integer in \[4, 2\^28\], not 3"):
+        run_loop(tmp_path, monkeypatch, n=6, max_bytes=3)
+    assert FakeStep.log is None
 
 
 def _mosaic(tmp_path, monkeypatch):
