@@ -418,6 +418,83 @@ typedef struct SyCocoRowsDesc {
 } SyCocoRowsDesc;
 int sy_coco_rows(const SyCocoRowsDesc* d, sy_stream_t stream);
 
+/* -------- forecast (streamyolo_b200/csrc/forecast.cu) ----------------------------------------------------------------
+ * The sAP toolkit's forecast of streaming detections to the query frame (sAP/forecast/pps_forecast_kf.py with
+ * --forecast-before-assoc and --assoc iou): on every new detection a constant-velocity Kalman predict of the tracks
+ * (F(dt), Q = dt^2 I, :175-184), greedy IoU association of the score-sorted detections with the tracks
+ * (sAP/track/__init__.py:90-133, no_unmatched1, pycocotools' fp64 bbIou, ties to the later track) and a Kalman update of
+ * the matched ones (R = 10 I, :81-97); at a query, the matched tracks extrapolated dt frames ahead and every track
+ * cleaned up by extrap_clean_up(..., lt=True) (sAP/forecast/__init__.py:33-56, min_size 75).  One CTA per stream or
+ * sequence; the state lives in caller-owned device buffers of S streams of at most T tracks.  Every entry point is
+ * capturable: no allocation, no synchronisation. */
+typedef struct SyForecastState {
+  float* x;          /* [S][T][8] Kalman mean: l, t, w, h and their velocities */
+  float* P;          /* [S][T][8][8] covariance */
+  int32_t* label;    /* [S][T] */
+  float* score;      /* [S][T] */
+  int32_t* track;    /* [S][T] track id */
+  int32_t* meta;     /* [S][4]: n_tracks, n_matched, next track id, overflow (set when a detection had more than T rows;
+                        that stream's state is then left as it was) */
+  int32_t S, T;      /* 1 <= S <= 65535, 1 <= T <= 2^20 */
+} SyForecastState;
+/* scratch bytes of sy_forecast_update / sy_forecast_sequences for S streams (sequences) of at most T tracks */
+size_t sy_forecast_workspace_bytes(int32_t streams, int32_t max_tracks);
+/* One new detection per stream (pps_forecast_kf.py:167-256): det [S][max_det][7] and count [S] as sy_postprocess_nms
+ * and sy_stream_rescale leave them (score = obj * class_conf, label = (int)class_pred); dt [S] the frames between this
+ * detection's input frame and the previous one's; start [S] (or NULL) != 0 clears the stream's tracks and restarts its
+ * track ids at 0 first; keep [S] (or NULL) == 0 leaves the stream untouched.  A new detection with no rows keeps the
+ * predicted tracks and n_matched. */
+typedef struct SyForecastUpdateDesc {
+  SyForecastState state;
+  const float* det;
+  int32_t max_det;
+  const int32_t* count;
+  const int32_t* dt;
+  const int32_t* start;
+  const int32_t* keep;
+  double match_iou_th;     /* inclusive */
+  void* workspace;
+  size_t workspace_bytes;
+} SyForecastUpdateDesc;
+int sy_forecast_update(const SyForecastUpdateDesc* d, sy_stream_t stream);
+/* Each stream's tracks extrapolated dt[s] frames ahead (:258-273): the first n_matched as x[:4] + dt * x[4:], the others
+ * as x[:4]; then extrap_clean_up with the stream's image size img_wh[s] = (W, H).  Rows compacted in track order at
+ * [s][0..count_out[s]) of box_out [S][T][4] (l, t, w, h), score_out, label_out, track_out [S][T]. */
+typedef struct SyForecastExtrapDesc {
+  SyForecastState state;
+  const int32_t* dt;       /* [S] */
+  const int32_t* img_wh;   /* [S][2] */
+  float* box_out;
+  float* score_out;
+  int32_t* label_out;
+  int32_t* track_out;
+  int32_t* count_out;      /* [S] */
+} SyForecastExtrapDesc;
+int sy_forecast_extrap(const SyForecastExtrapDesc* d, sy_stream_t stream);
+/* The offline pass (pps_forecast_kf.py:134-287) over S sequences, one CTA each, with the state of sy_forecast_update
+ * (cleared at each sequence's start).  Detection k has det_n[k] rows at det + 7 * det_start[k] (rows as in
+ * sy_forecast_update).  Sequence s owns the frames [seq_frames[s], seq_frames[s + 1]) of frames [F][6]: (index of the
+ * latest detection or -1, dt of the update when that detection is new, dt of the query, first output row, W, H).  A
+ * frame's rows go to its first output row on (room for its track count, which the host knows) and rows_out [F] counts
+ * them; a frame without a detection, or whose sequence has no track yet, emits nothing. */
+typedef struct SyForecastSequencesDesc {
+  SyForecastState state;
+  const float* det;
+  const int32_t* det_start;
+  const int32_t* det_n;
+  const int32_t* frames;
+  const int32_t* seq_frames;   /* [S + 1] */
+  double match_iou_th;
+  float* box_out;
+  float* score_out;
+  int32_t* label_out;
+  int32_t* track_out;
+  int32_t* rows_out;           /* [F] */
+  void* workspace;
+  size_t workspace_bytes;
+} SyForecastSequencesDesc;
+int sy_forecast_sequences(const SyForecastSequencesDesc* d, sy_stream_t stream);
+
 /* -------- training step glue (streamyolo_b200/csrc/train_glue.cu) ---------------------------------------------- */
 /* fp32 OIHW conv parameter -> bf16 GEMM operand, on the device (one launch per parameter per optimiser step):
  *   mode 0  out[o][r*kw+s][i] = w[o][i][r][s]                          forward B operand of sy_conv2d_tc

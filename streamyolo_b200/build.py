@@ -31,6 +31,7 @@ SOURCES = {
     "head_loss.cu": ["-fmad=false"],
     "postprocess.cu": ["-fmad=false"],
     "input.cu": ["-fmad=false"],
+    "forecast.cu": ["-fmad=false"],
     "jpeg.cu": [],
 }
 

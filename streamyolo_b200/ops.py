@@ -164,6 +164,29 @@ class SyCocoRowsDesc(C.Structure):
                 ("total_out", C.c_void_p)]
 
 
+class SyForecastState(C.Structure):
+    _fields_ = [("x", C.c_void_p), ("P", C.c_void_p), ("label", C.c_void_p), ("score", C.c_void_p), ("track", C.c_void_p),
+                ("meta", C.c_void_p), ("S", C.c_int32), ("T", C.c_int32)]
+
+
+class SyForecastUpdateDesc(C.Structure):
+    _fields_ = [("state", SyForecastState), ("det", C.c_void_p), ("max_det", C.c_int32), ("count", C.c_void_p),
+                ("dt", C.c_void_p), ("start", C.c_void_p), ("keep", C.c_void_p), ("match_iou_th", C.c_double),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
+class SyForecastExtrapDesc(C.Structure):
+    _fields_ = [("state", SyForecastState), ("dt", C.c_void_p), ("img_wh", C.c_void_p), ("box_out", C.c_void_p),
+                ("score_out", C.c_void_p), ("label_out", C.c_void_p), ("track_out", C.c_void_p), ("count_out", C.c_void_p)]
+
+
+class SyForecastSequencesDesc(C.Structure):
+    _fields_ = [("state", SyForecastState), ("det", C.c_void_p), ("det_start", C.c_void_p), ("det_n", C.c_void_p),
+                ("frames", C.c_void_p), ("seq_frames", C.c_void_p), ("match_iou_th", C.c_double), ("box_out", C.c_void_p),
+                ("score_out", C.c_void_p), ("label_out", C.c_void_p), ("track_out", C.c_void_p), ("rows_out", C.c_void_p),
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
 # every symbol include/streamyolo_sm100.h declares: (restype, argtypes)
 _SIG = {
     "sy_last_error_string": (C.c_char_p, []),
@@ -210,6 +233,10 @@ _SIG = {
     "sy_stream_gate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sy_stream_rescale": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sy_coco_rows": (C.c_int, [C.POINTER(SyCocoRowsDesc), C.c_void_p]),
+    "sy_forecast_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
+    "sy_forecast_update": (C.c_int, [C.POINTER(SyForecastUpdateDesc), C.c_void_p]),
+    "sy_forecast_extrap": (C.c_int, [C.POINTER(SyForecastExtrapDesc), C.c_void_p]),
+    "sy_forecast_sequences": (C.c_int, [C.POINTER(SyForecastSequencesDesc), C.c_void_p]),
     "sy_conv2d_wgrad_workspace_bytes": (C.c_size_t, [C.POINTER(SyConvWgradDesc)]),
     "sy_conv2d_wgrad_tc": (C.c_int, [C.POINTER(SyConvWgradDesc), C.c_void_p]),
     "sy_pack_conv_weight": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
@@ -578,6 +605,103 @@ def coco_rows(det, count, ratio, image_id, class_ids, status=None, out=None):
                        bbox.data_ptr(), score.data_ptr(), ids.data_ptr(), cat.data_ptr(), total.data_ptr())
     _check(lib().sy_coco_rows(C.byref(d), _stream()))
     return out
+
+
+class ForecastState:
+    """Device state of the sy_forecast_* entry points for ``streams`` streams (or sequences) of at most ``max_tracks``
+    tracks, with the update's workspace: x fp32 [S, T, 8], P fp32 [S, T, 8, 8], label / track int32 [S, T], score fp32
+    [S, T], meta int32 [S, 4] (n_tracks, n_matched, next track id, overflow).  Zeroed: no tracks."""
+
+    def __init__(self, streams, max_tracks, device):
+        _require(int(streams) == streams and 1 <= streams <= 65535, f"ForecastState: {streams} streams (1 to 65535)")
+        _require(int(max_tracks) == max_tracks and 1 <= max_tracks <= 1 << 20,
+                 f"ForecastState: max_tracks {max_tracks} (1 to 2^20)")
+        s, t = int(streams), int(max_tracks)
+        self.streams, self.max_tracks = s, t
+        self.x = torch.zeros((s, t, 8), dtype=torch.float32, device=device)
+        self.P = torch.zeros((s, t, 8, 8), dtype=torch.float32, device=device)
+        self.label = torch.zeros((s, t), dtype=torch.int32, device=device)
+        self.score = torch.zeros((s, t), dtype=torch.float32, device=device)
+        self.track = torch.zeros((s, t), dtype=torch.int32, device=device)
+        self.meta = torch.zeros((s, 4), dtype=torch.int32, device=device)
+        self.workspace = torch.empty(load_library().sy_forecast_workspace_bytes(s, t), dtype=torch.uint8, device=device)
+
+    def desc(self):
+        return SyForecastState(self.x.data_ptr(), self.P.data_ptr(), self.label.data_ptr(), self.score.data_ptr(),
+                               self.track.data_ptr(), self.meta.data_ptr(), self.streams, self.max_tracks)
+
+
+def _on(t, dtype, shape, device):
+    return _tensor_ok(t, dtype, len(shape)) and tuple(t.shape) == tuple(shape) and t.device == device
+
+
+def forecast_update(state, det, count, dt, start=None, keep=None, match_iou_th=0.3):
+    """One new detection per stream into ``state`` (sy_forecast_update): ``det`` fp32 [S, max_det, 7] and ``count`` int32
+    [S] as postprocess_nms / stream_rescale leave them, ``dt`` int32 [S] frames since each stream's previous detection,
+    ``start`` / ``keep`` int32 [S] or None.  Nothing is read back: a stream whose count exceeds max_tracks keeps its state
+    and gets state.meta[s, 3] = 1."""
+    dev = state.x.device
+    _require(_tensor_ok(det, torch.float32, 3) and det.shape[0] == state.streams and det.shape[2] == 7 and det.device == dev,
+             f"forecast_update: det must be float32 [{state.streams}, max_det, 7] on {dev}")
+    for name, t in (("count", count), ("dt", dt), ("start", start), ("keep", keep)):
+        _require(t is None and name in ("start", "keep") or (t is not None and _on(t, torch.int32, (state.streams,), dev)),
+                 f"forecast_update: {name} must be int32 [{state.streams}] on {dev}")
+    d = SyForecastUpdateDesc(state.desc(), det.data_ptr(), det.shape[1], count.data_ptr(), dt.data_ptr(),
+                             start.data_ptr() if start is not None else None, keep.data_ptr() if keep is not None else None,
+                             float(match_iou_th), state.workspace.data_ptr(), state.workspace.numel())
+    _check(lib().sy_forecast_update(C.byref(d), _stream()))
+
+
+def forecast_extrap(state, dt, img_wh, out=None):
+    """Each stream's tracks extrapolated ``dt`` (int32 [S]) frames ahead and cleaned up for its image size ``img_wh`` (int32
+    [S, 2], (W, H)) (sy_forecast_extrap) -> ``(box fp32 [S, T, 4] ltwh, score fp32 [S, T], label int32 [S, T], track int32
+    [S, T], count int32 [S])``: the first count[s] rows of stream s are valid.  ``out``: those five tensors of an earlier
+    call to write into."""
+    s, t, dev = state.streams, state.max_tracks, state.x.device
+    _require(_on(dt, torch.int32, (s,), dev), f"forecast_extrap: dt must be int32 [{s}] on {dev}")
+    _require(_on(img_wh, torch.int32, (s, 2), dev), f"forecast_extrap: img_wh must be int32 [{s}, 2] on {dev}")
+    if out is None:
+        out = (torch.empty((s, t, 4), dtype=torch.float32, device=dev), torch.empty((s, t), dtype=torch.float32, device=dev),
+               torch.empty((s, t), dtype=torch.int32, device=dev), torch.empty((s, t), dtype=torch.int32, device=dev),
+               torch.empty((s,), dtype=torch.int32, device=dev))
+    box, score, label, track, count = out
+    _require(_on(box, torch.float32, (s, t, 4), dev) and _on(score, torch.float32, (s, t), dev)
+             and _on(label, torch.int32, (s, t), dev) and _on(track, torch.int32, (s, t), dev)
+             and _on(count, torch.int32, (s,), dev), "forecast_extrap: out must be the five tensors of an earlier call")
+    d = SyForecastExtrapDesc(state.desc(), dt.data_ptr(), img_wh.data_ptr(), box.data_ptr(), score.data_ptr(),
+                             label.data_ptr(), track.data_ptr(), count.data_ptr())
+    _check(lib().sy_forecast_extrap(C.byref(d), _stream()))
+    return out
+
+
+def forecast_sequences(state, det, det_start, det_n, frames, seq_frames, n_rows, match_iou_th=0.3):
+    """The offline forecast of ``state.streams`` sequences (sy_forecast_sequences): ``det`` fp32 [R, 7] rows of every
+    detection, detection k at rows det_start[k] .. + det_n[k] (int32 [D]); ``frames`` int32 [F, 6] (latest detection or
+    -1, dt of its update, dt of the query, first output row, W, H); ``seq_frames`` int32 [S + 1]; ``n_rows`` the output
+    room (the sum of the frames' track counts) -> ``(box fp32 [n_rows, 4] ltwh, score fp32, label int32, track int32
+    [n_rows], rows int32 [F])``: frame f's rows start at frames[f, 3], rows[f] of them.  The state is cleared per sequence."""
+    dev = state.x.device
+    _require(_tensor_ok(det, torch.float32, 2) and det.shape[1] == 7 and det.shape[0] > 0 and det.device == dev,
+             "forecast_sequences: det must be float32 [R, 7]")
+    nd = det_start.shape[0] if torch.is_tensor(det_start) else -1
+    _require(nd > 0 and _on(det_start, torch.int32, (nd,), dev) and _on(det_n, torch.int32, (nd,), dev),
+             "forecast_sequences: det_start and det_n must be int32 [D]")
+    _require(_tensor_ok(frames, torch.int32, 2) and frames.shape[1] == 6 and frames.device == dev,
+             "forecast_sequences: frames must be int32 [F, 6]")
+    _require(_on(seq_frames, torch.int32, (state.streams + 1,), dev),
+             f"forecast_sequences: seq_frames must be int32 [{state.streams + 1}]")
+    n_rows = max(int(n_rows), 1)
+    box = torch.empty((n_rows, 4), dtype=torch.float32, device=dev)
+    score = torch.empty((n_rows,), dtype=torch.float32, device=dev)
+    label = torch.empty((n_rows,), dtype=torch.int32, device=dev)
+    track = torch.empty((n_rows,), dtype=torch.int32, device=dev)
+    rows = torch.empty((frames.shape[0],), dtype=torch.int32, device=dev)
+    d = SyForecastSequencesDesc(state.desc(), det.data_ptr(), det_start.data_ptr(), det_n.data_ptr(), frames.data_ptr(),
+                                seq_frames.data_ptr(), float(match_iou_th), box.data_ptr(), score.data_ptr(),
+                                label.data_ptr(), track.data_ptr(), rows.data_ptr(), state.workspace.data_ptr(),
+                                state.workspace.numel())
+    _check(lib().sy_forecast_sequences(C.byref(d), _stream()))
+    return box, score, label, track, rows
 
 
 def head_pred_decode(cls_feat: View, reg_feat: View, w_reg, b_reg, w_obj, b_obj, w_cls, b_cls, stride,

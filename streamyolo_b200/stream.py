@@ -45,7 +45,8 @@ class StreamTick:
     ratio --, obj, class_conf, class_pred) and ``count`` ([S] rows of ``det``) are the outputs; ``buffer`` holds each
     stream's features carried to the next tick."""
 
-    def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None):
+    def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None,
+                 forecast=None):
         self.model, self.size = model, tuple(size)
         self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
         table = np.asarray(table, np.int32)
@@ -61,6 +62,13 @@ class StreamTick:
         self.buffer = None
         self.raw = self.det = self.count = None
         self.status = None
+        # forecast = (match_iou_th, max_tracks): the tick ends with the tracks' update from its detections, each stream
+        # gated by start / keep; fc_dt (int32 [S], set by the host) is the frames since the stream's previous update
+        self.fc = self.fc_dt = None
+        if forecast is not None:
+            self.fc_th = float(forecast[0])
+            self.fc = ops.ForecastState(streams, forecast[1], device)
+            self.fc_dt = torch.zeros((streams,), dtype=torch.int32, device=device)
         if jpeg_max_bytes is not None:
             self.bytes = torch.zeros((streams, jpeg_max_bytes), dtype=torch.uint8, device=device)
             self.lengths = torch.zeros((streams,), dtype=torch.int32, device=device)
@@ -86,6 +94,8 @@ class StreamTick:
             self.det, self.count = ops.postprocess_nms(self.raw, head.num_classes, self.conf_thre, self.nms_thre,
                                                        max_det=self.raw.shape[1])
             ops.stream_rescale(self.det, self.count, self.status, self.ratio)
+            if self.fc is not None:
+                ops.forecast_update(self.fc, self.det, self.count, self.fc_dt, self.start, self.keep, self.fc_th)
 
 
 NO_FRAME = -1     # last_status() of a stream that was given no frame
@@ -162,12 +172,22 @@ class StreamDetector:
       jpeg_max_bytes  the longest JPEG file ``step_jpeg`` takes.  The replay then starts with the decode of the streams'
                       files, so such a detector takes files only (``step_jpeg``); without it, it takes decoded frames only
                       (``step``)
+    Forecast (the sAP toolkit's pps_forecast_kf.py online):
+      forecast        True: the tick ends with each stream's track update from its detections (sy_forecast_update:
+                      Kalman predict, greedy IoU association, Kalman update), gated as the feature buffer is: a stream
+                      that starts a sequence clears its tracks, one without a decoded frame keeps them.  ``step`` and
+                      ``step_jpeg`` then take ``fidx``, each stream's frame index, and ``forecast(fidx)`` extrapolates
+                      the tracks to a query frame.  The detections ``step`` returns do not change.
+      match_iou_th    the association's IoU threshold (inclusive)
+      max_tracks      the most detections one stream's update takes; a tick with more raises RuntimeError naming the
+                      stream, whose tracks are then left as they were
     Each stream's frame is transformed as data.sized_table says and its boxes divided by its own ratio (``ratios``): a frame
     of driver size ``input_size`` gets the driver's plain resize and ``in_scale``.  ``frame_hw`` is the slot the frames are
     stored in: the largest height and width (the frame size when every stream has one size)."""
 
     def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
-                 frame_sizes=None, input_size=None, jpeg_max_bytes=None):
+                 frame_sizes=None, input_size=None, jpeg_max_bytes=None, forecast=False, match_iou_th=0.3,
+                 max_tracks=1024):
         if model.training:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
@@ -186,6 +206,8 @@ class StreamDetector:
             raise ValueError(f"StreamDetector: frames {sizes} at in_scale {in_scale} give input size {size}")
         if jpeg_max_bytes is not None:
             jpeg_max_bytes = feed.check_max_bytes(jpeg_max_bytes, "StreamDetector: jpeg_max_bytes")
+        if forecast and (int(max_tracks) != max_tracks or not 1 <= max_tracks <= 1 << 20):
+            raise ValueError(f"StreamDetector: max_tracks must be an integer in [1, 2^20], not {max_tracks}")
         try:
             table, ratios = data.sized_table(sizes, size, in_scale)
         except RuntimeError as e:
@@ -195,7 +217,14 @@ class StreamDetector:
         self.model, self.streams, self.in_scale, self.size = model, streams, in_scale, size
         self.frame_sizes, self.ratios = sizes, ratios
         self.jpeg_max_bytes = jpeg_max_bytes
-        self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes)
+        self.forecasting = bool(forecast)
+        self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes,
+                                (match_iou_th, int(max_tracks)) if forecast else None)
+        if self.forecasting:
+            self._fc_dt = feed.pinned((streams,), torch.int32)
+            self._fc_meta = feed.pinned((streams, 4), torch.int32)
+            self._fc_wh = torch.tensor([(w, h) for h, w in sizes], dtype=torch.int32, device=dev)
+            self._fc_out = None
         self.frame_hw = tuple(self._tick.frames.shape[1:3])          # the slot: the largest height and width
         if self.jpeg_max_bytes is None:           # stream i's frame is staged at the start of slot i (see step)
             self._stage = feed.pinned(tuple(self._tick.frames.shape), torch.uint8)
@@ -216,6 +245,9 @@ class StreamDetector:
         self._graph = engine.capture_graph(t.run, t.frames.device)
         self._det = feed.pinned((self.streams, t.raw.shape[1], 7), torch.float32)
         self._count = feed.pinned((self.streams,), torch.int32)
+        if self.forecasting:                      # the warm-up run went through the update: no stream has tracks yet
+            t.fc.meta.zero_()
+            self._fc_last = [None] * self.streams         # each stream's frame index at its last update
         self.reset()
 
     def reset(self, stream=None):
@@ -227,13 +259,16 @@ class StreamDetector:
                 raise ValueError(f"StreamDetector.reset: stream {stream} not in [0, {self.streams})")
             self._flags[stream] = 1
 
-    def step(self, frames):
+    def step(self, frames, fidx=None):
         """One frame per stream -> a list of S ``(bboxes, scores, labels)`` numpy tuples, what the driver's inference()
         returns (boxes in frame pixels, float32 [n, 4]; scores float32 [n]; labels int32 [n]).  ``frames``: a list of S
         frames, frame i uint8 BGR [h_i, w_i, 3] of stream i's size; or, when every stream has the same size, uint8
         [S, h, w, 3] ([h, w, 3] for one stream).  Each a numpy array, a CPU tensor or a CUDA tensor.  A detector built with
-        ``jpeg_max_bytes`` takes files only: ``step`` raises RuntimeError there, use ``step_jpeg``."""
+        ``jpeg_max_bytes`` takes files only: ``step`` raises RuntimeError there, use ``step_jpeg``.  With ``forecast=True``,
+        ``fidx`` gives each stream's frame index (a list of S ints; an int for one stream), and the tick updates the
+        stream's tracks with its detections (see ``forecast``)."""
         t = self._tick
+        fidx = self._fidx(fidx, "step")
         if self.jpeg_max_bytes is not None:
             raise RuntimeError("StreamDetector.step: this detector was built with jpeg_max_bytes, and its replay decodes the "
                                "streams' files: feed it with step_jpeg (build one with frame_sizes alone for decoded frames)")
@@ -258,22 +293,24 @@ class StreamDetector:
             else:
                 self._stage.copy_(src)
                 t.frames.copy_(self._stage, non_blocking=True)
-        return self._run(None)
+        return self._run(None, fidx)
 
     def last_raw(self):
         """A device copy of the last tick's head outputs [S, A, 5 + nc] (what the driver keeps as ``results_raw``)."""
         return self._tick.raw.clone()
 
-    def step_jpeg(self, files):
+    def step_jpeg(self, files, fidx=None):
         """One JPEG file per stream -> a list of S ``(bboxes, scores, labels)`` tuples as ``step`` returns them, with one
         host synchronisation.  ``files``: a list of S entries, each the file's bytes (``bytes``, or a uint8 numpy array or
         CPU tensor) of at most ``jpeg_max_bytes``, or None when the stream has no frame this tick.  A stream whose file
         did not decode (see ``last_status``) or that got None returns empty arrays, keeps its carried features and, if it
-        was to start a sequence, starts it at its next decoded frame."""
+        was to start a sequence, starts it at its next decoded frame.  ``fidx``: as for ``step``; such a stream's tracks
+        are left as they were."""
         if self.jpeg_max_bytes is None:
             raise RuntimeError("StreamDetector.step_jpeg: construct the detector with jpeg_max_bytes")
         t = self._tick
         files = jpeg_files(files, self.streams, self.jpeg_max_bytes)
+        fidx = self._fidx(fidx, "step_jpeg")
         stage = self._jstage.numpy()
         for i, a in enumerate(files):
             stage[i, :a.size] = a
@@ -281,26 +318,86 @@ class StreamDetector:
             if a.size:
                 t.bytes[i, :a.size].copy_(self._jstage[i, :a.size], non_blocking=True)
         t.lengths.copy_(self._jlen, non_blocking=True)
-        return self._run([a.size > 0 for a in files])
+        return self._run([a.size > 0 for a in files], fidx)
 
-    def _run(self, present):
+    def _fidx(self, fidx, what):
+        """``fidx`` of step / step_jpeg as a list of S ints (None without forecast)"""
+        if not self.forecasting:
+            if fidx is not None:
+                raise ValueError(f"StreamDetector.{what}: fidx takes a detector built with forecast=True")
+            return None
+        if isinstance(fidx, (int, np.integer)) and self.streams == 1:
+            fidx = [fidx]
+        if not isinstance(fidx, (list, tuple, np.ndarray)) or len(fidx) != self.streams \
+                or any(int(v) != v for v in fidx):
+            raise ValueError(f"StreamDetector.{what}: with forecast=True give fidx, {self.streams} frame indices "
+                             "(an int for one stream)")
+        return [int(v) for v in fidx]
+
+    def _dt(self, fidx):
+        """frames from each stream's last update to ``fidx`` (0 for a stream without one), into the pinned dt"""
+        for i, (f, last) in enumerate(zip(fidx, self._fc_last)):
+            d = 0 if last is None else f - last
+            if not -2 ** 31 <= d < 2 ** 31:
+                raise ValueError(f"StreamDetector: stream {i}: frame index {f} is {d} frames from its last update")
+            self._fc_dt[i] = d
+
+    def _run(self, present, fidx=None):
         """Replay the tick on the staged inputs and return the detections; ``present`` (JPEG ticks only): which streams
-        were given a file."""
+        were given a file; ``fidx``: the streams' frame indices (forecast only)."""
         t = self._tick
         t.flags.copy_(self._flags, non_blocking=True)
+        if fidx is not None:
+            self._dt(fidx)
+            t.fc_dt.copy_(self._fc_dt, non_blocking=True)
         self._graph.replay()
         self._det.copy_(t.det, non_blocking=True)
         self._count.copy_(t.count, non_blocking=True)
         if present is not None:
             self._status.copy_(t.status, non_blocking=True)
+        if fidx is not None:
+            self._fc_meta.copy_(t.fc.meta, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         if present is None:
+            updated = [True] * self.streams
             self._flags.zero_()
         else:
             self._last_status, nxt = route_status(self._status.numpy(), present, self._flags.numpy())
+            updated = (self._last_status == 0).tolist()
             self._flags.copy_(torch.from_numpy(nxt))
+        if fidx is not None:
+            over = [i for i in range(self.streams) if self._fc_meta[i, 3] != 0]
+            if over:
+                raise RuntimeError(f"StreamDetector: stream {over[0]}'s detection has more rows than max_tracks = "
+                                   f"{t.fc.max_tracks}; its tracks were left as they were (build the detector with a "
+                                   "larger max_tracks)")
+            for i, u in enumerate(updated):
+                if u:
+                    self._fc_last[i] = fidx[i]
         det = self._det.numpy()
         return [sized_output(det[i, :n]) for i, n in enumerate(self._count.tolist())]
+
+    def forecast(self, fidx):
+        """Each stream's tracks extrapolated to its frame index ``fidx`` (a list of S ints; an int for one stream) ->
+        a list of S ``(ltwh, scores, labels, tracks)`` numpy tuples: float32 [n, 4] boxes in frame pixels, float32 [n],
+        int32 [n], int32 [n].  The sAP toolkit's forecast (sAP/forecast/pps_forecast_kf.py:258-273): the tracks matched
+        at the last update move by their Kalman velocity times the frames since that update, the others stay; boxes are
+        clipped to the stream's frame and dropped below 75 pixels (extrap_clean_up).  One launch, one synchronisation."""
+        if not self.forecasting:
+            raise RuntimeError("StreamDetector.forecast: build the detector with forecast=True")
+        fidx = self._fidx(fidx, "forecast")
+        t = self._tick
+        self._dt(fidx)
+        dt = self._fc_dt.to(t.fc.x.device, non_blocking=True)
+        out = ops.forecast_extrap(t.fc, dt, self._fc_wh)
+        if self._fc_out is None:
+            self._fc_out = tuple(feed.pinned(tuple(o.shape), o.dtype) for o in out)
+        for h, d in zip(self._fc_out, out):
+            h.copy_(d, non_blocking=True)
+        torch.cuda.current_stream().synchronize()
+        box, score, label, track, count = (h.numpy() for h in self._fc_out)
+        return [(box[i, :n].copy(), score[i, :n].copy(), label[i, :n].copy(), track[i, :n].copy())
+                for i, n in enumerate(count.tolist())]
 
     def last_status(self):
         """Per-stream int32 status of the last ``step_jpeg``: 0 where the frame decoded, a data.JPEG_STATUS code where it
