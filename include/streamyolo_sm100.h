@@ -443,7 +443,8 @@ size_t sy_forecast_workspace_bytes(int32_t streams, int32_t max_tracks);
  * and sy_stream_rescale leave them (score = obj * class_conf, label = (int)class_pred); dt [S] the frames between this
  * detection's input frame and the previous one's; start [S] (or NULL) != 0 clears the stream's tracks and restarts its
  * track ids at 0 first; keep [S] (or NULL) == 0 leaves the stream untouched.  A new detection with no rows keeps the
- * predicted tracks and n_matched. */
+ * predicted tracks and n_matched (pps_forecast_kf.py), or, with clear_on_empty != 0, leaves the stream without tracks
+ * (sAP/forecast/streamer.py:247-280); the track id counter continues either way. */
 typedef struct SyForecastUpdateDesc {
   SyForecastState state;
   const float* det;
@@ -455,6 +456,7 @@ typedef struct SyForecastUpdateDesc {
   double match_iou_th;     /* inclusive */
   void* workspace;
   size_t workspace_bytes;
+  int32_t clear_on_empty;  /* 0: pps_forecast_kf.py's rule for an empty detection; else streamer.py's */
 } SyForecastUpdateDesc;
 int sy_forecast_update(const SyForecastUpdateDesc* d, sy_stream_t stream);
 /* Each stream's tracks extrapolated dt[s] frames ahead (:258-273): the first n_matched as x[:4] + dt * x[4:], the others
@@ -471,6 +473,24 @@ typedef struct SyForecastExtrapDesc {
   int32_t* count_out;      /* [S] */
 } SyForecastExtrapDesc;
 int sy_forecast_extrap(const SyForecastExtrapDesc* d, sy_stream_t stream);
+/* Up to Q queries per stream in one launch: stream s's tracks extrapolated dt[s][k] frames ahead for k < n_query[s], each
+ * as sy_forecast_extrap does with an fp32 dt (the streamer's fractional query, sAP/forecast/streamer.py:287-297: numpy's
+ * fp32 x[:4] + dt * x[4:]); an integer dt gives sy_forecast_extrap's rows bit for bit.  Query (s, k) writes its rows at
+ * [s][k][0..count_out[s][k]) of box_out [S][Q][T][4] (l, t, w, h), score_out, label_out, track_out [S][Q][T];
+ * count_out [S][Q] is 0 for k >= n_query[s]. */
+typedef struct SyForecastExtrapQueriesDesc {
+  SyForecastState state;
+  const float* dt;         /* [S][Q] */
+  const int32_t* n_query;  /* [S] */
+  int32_t Q;               /* 1 <= Q <= 65535 */
+  const int32_t* img_wh;   /* [S][2] */
+  float* box_out;
+  float* score_out;
+  int32_t* label_out;
+  int32_t* track_out;
+  int32_t* count_out;      /* [S][Q] */
+} SyForecastExtrapQueriesDesc;
+int sy_forecast_extrap_queries(const SyForecastExtrapQueriesDesc* d, sy_stream_t stream);
 /* The offline pass (pps_forecast_kf.py:134-287) over S sequences, one CTA each, with the state of sy_forecast_update
  * (cleared at each sequence's start).  Detection k has det_n[k] rows at det + 7 * det_start[k] (rows as in
  * sy_forecast_update).  Sequence s owns the frames [seq_frames[s], seq_frames[s + 1]) of frames [F][6]: (index of the

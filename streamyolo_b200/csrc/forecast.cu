@@ -160,7 +160,7 @@ __device__ __forceinline__ void kf_update(const float* x, const float* P, const 
 // the whole CTA.  rows: sy_postprocess_nms rows [n][7] (x1, y1, x2, y2, obj, class_conf, class_pred); the score is
 // obj * class_conf and the label (int)class_pred.  n > T leaves the state as it was and sets the overflow flag.
 __device__ void forecast_update(const FcStream& S, const FcScratch& W, int T, const float* __restrict__ rows, int n,
-                                int dt_i, bool start, double th) {
+                                int dt_i, bool start, double th, bool clear_on_empty) {
   __shared__ double s_iou[2][kFcWarps];
   __shared__ int s_idx[2][kFcWarps], s_last[2][kFcWarps], s_nan[2][kFcWarps];
   __shared__ int s_meta[3];
@@ -182,7 +182,13 @@ __device__ void forecast_update(const FcStream& S, const FcScratch& W, int T, co
   const float dt = (float)dt_i;
   // predict every track before the association, on every new detection (:175-184)
   for (int i = tid; i < m; i += kFcThreads) kf_predict(S.x + (size_t)i * 8, S.P + (size_t)i * 64, dt);
-  if (n == 0) return;                               // an empty detection keeps the predicted tracks and n_matched
+  if (n == 0) {
+    // pps_forecast_kf.py keeps the predicted tracks and n_matched; the streamer (sAP/forecast/streamer.py:247-280)
+    // associates the tracks with nothing, matches none and starts from the empty detection: no track is left.  The
+    // id counter stays either way.  (The predict above only wrote the tracks' own slots.)
+    if (clear_on_empty && tid == 0) S.meta[0] = S.meta[1] = 0;
+    return;
+  }
   // sort by score (:204-207) by rank, convert ltrb -> ltwh (:209)
   for (int j = tid; j < n; j += kFcThreads) {
     const float* d = rows + (size_t)j * 7;
@@ -299,7 +305,9 @@ __device__ void forecast_update(const FcStream& S, const FcScratch& W, int T, co
 
 // The tracks extrapolated dt frames ahead (:258-273) and cleaned up as extrap_clean_up(..., lt=True) does
 // (forecast/__init__.py:33-56), compacted in track order into box [.][4] (ltwh), score, label, track.  -> rows written.
-__device__ int forecast_extrap(const FcStream& S, int dt_i, float W_img, float H_img, float* __restrict__ box,
+// dt is an fp32 frame count: the streamer's fractional query (its Python float rounded to fp32 by numpy's fp32
+// multiply), or an integer one converted exactly.
+__device__ int forecast_extrap(const FcStream& S, float dt, float W_img, float H_img, float* __restrict__ box,
                                float* __restrict__ score, int32_t* __restrict__ label, int32_t* __restrict__ track) {
   __shared__ int s_cnt[kFcWarps];
   __shared__ int s_mt[2];
@@ -307,7 +315,6 @@ __device__ int forecast_extrap(const FcStream& S, int dt_i, float W_img, float H
   if (tid == 0) s_mt[0] = S.meta[0], s_mt[1] = S.meta[1];
   __syncthreads();
   const int m = s_mt[0], n_matched = s_mt[1];
-  const float dt = (float)dt_i;
   int base = 0;
   for (int i0 = 0; i0 < m; i0 += kFcThreads) {
     const int i = i0 + tid;
@@ -357,15 +364,30 @@ __global__ void __launch_bounds__(kFcThreads) forecast_update_kernel(const SyFor
   }
   const int n = min(max(q.count[s], 0), q.max_det);
   forecast_update(fc_stream(q.state, s), fc_scratch(q.workspace, s, q.state.T), q.state.T,
-                  q.det + (size_t)s * q.max_det * 7, n, q.dt[s], q.start != nullptr && q.start[s] != 0, q.match_iou_th);
+                  q.det + (size_t)s * q.max_det * 7, n, q.dt[s], q.start != nullptr && q.start[s] != 0, q.match_iou_th,
+                  q.clear_on_empty != 0);
 }
 
 __global__ void __launch_bounds__(kFcThreads) forecast_extrap_kernel(const SyForecastExtrapDesc q) {
   const int s = blockIdx.x;
   const size_t T = q.state.T;
-  const int n = forecast_extrap(fc_stream(q.state, s), q.dt[s], (float)q.img_wh[s * 2], (float)q.img_wh[s * 2 + 1],
-                                q.box_out + s * T * 4, q.score_out + s * T, q.label_out + s * T, q.track_out + s * T);
+  const int n = forecast_extrap(fc_stream(q.state, s), (float)q.dt[s], (float)q.img_wh[s * 2],
+                                (float)q.img_wh[s * 2 + 1], q.box_out + s * T * 4, q.score_out + s * T,
+                                q.label_out + s * T, q.track_out + s * T);
   if (threadIdx.x == 0) q.count_out[s] = n;
+}
+
+// One CTA per (stream, query): blockIdx.x the stream, blockIdx.y the query; queries past n_query[s] write a count of 0.
+__global__ void __launch_bounds__(kFcThreads) forecast_extrap_queries_kernel(const SyForecastExtrapQueriesDesc q) {
+  const int s = blockIdx.x, k = blockIdx.y;
+  const size_t T = q.state.T, o = (size_t)s * q.Q + k;
+  if (k >= q.n_query[s]) {
+    if (threadIdx.x == 0) q.count_out[o] = 0;
+    return;
+  }
+  const int n = forecast_extrap(fc_stream(q.state, s), q.dt[o], (float)q.img_wh[s * 2], (float)q.img_wh[s * 2 + 1],
+                                q.box_out + o * T * 4, q.score_out + o * T, q.label_out + o * T, q.track_out + o * T);
+  if (threadIdx.x == 0) q.count_out[o] = n;
 }
 
 // One CTA per sequence: its annotated frames in order, each a table row (see SyForecastSequencesDesc).
@@ -383,12 +405,13 @@ __global__ void __launch_bounds__(kFcThreads) forecast_sequences_kernel(const Sy
       continue;
     }
     if (d != prev) {
-      forecast_update(S, W, q.state.T, q.det + (size_t)q.det_start[d] * 7, q.det_n[d], row[1], start, q.match_iou_th);
+      forecast_update(S, W, q.state.T, q.det + (size_t)q.det_start[d] * 7, q.det_n[d], row[1], start, q.match_iou_th,
+                      false);
       __syncthreads();
       prev = d, start = false;
     }
     const size_t o = (size_t)row[3];
-    const int n = forecast_extrap(S, row[2], (float)row[4], (float)row[5], q.box_out + o * 4, q.score_out + o,
+    const int n = forecast_extrap(S, (float)row[2], (float)row[4], (float)row[5], q.box_out + o * 4, q.score_out + o,
                                   q.label_out + o, q.track_out + o);
     if (threadIdx.x == 0) q.rows_out[f] = n;
   }
@@ -431,6 +454,17 @@ extern "C" int sy_forecast_extrap(const SyForecastExtrapDesc* d, sy_stream_t str
              "forecast_extrap: null pointer");
   forecast_extrap_kernel<<<d->state.S, kFcThreads, 0, stream>>>(*d);
   return launch_status("forecast_extrap_kernel");
+}
+
+extern "C" int sy_forecast_extrap_queries(const SyForecastExtrapQueriesDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr, SY_EINVAL, "null descriptor");
+  FC_STATE_CHECK(d->state, "forecast_extrap_queries");
+  SY_REQUIRE(d->Q >= 1 && d->Q <= 65535, SY_EINVAL, "forecast_extrap_queries: %d queries per stream (1 to 65535)", d->Q);
+  SY_REQUIRE(d->dt && d->n_query && d->img_wh && d->box_out && d->score_out && d->label_out && d->track_out &&
+             d->count_out, SY_EINVAL, "forecast_extrap_queries: null pointer");
+  forecast_extrap_queries_kernel<<<dim3(d->state.S, d->Q), kFcThreads, 0, stream>>>(*d);
+  return launch_status("forecast_extrap_queries_kernel");
 }
 
 extern "C" int sy_forecast_sequences(const SyForecastSequencesDesc* d, sy_stream_t stream_) {

@@ -172,12 +172,18 @@ class SyForecastState(C.Structure):
 class SyForecastUpdateDesc(C.Structure):
     _fields_ = [("state", SyForecastState), ("det", C.c_void_p), ("max_det", C.c_int32), ("count", C.c_void_p),
                 ("dt", C.c_void_p), ("start", C.c_void_p), ("keep", C.c_void_p), ("match_iou_th", C.c_double),
-                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+                ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t), ("clear_on_empty", C.c_int32)]
 
 
 class SyForecastExtrapDesc(C.Structure):
     _fields_ = [("state", SyForecastState), ("dt", C.c_void_p), ("img_wh", C.c_void_p), ("box_out", C.c_void_p),
                 ("score_out", C.c_void_p), ("label_out", C.c_void_p), ("track_out", C.c_void_p), ("count_out", C.c_void_p)]
+
+
+class SyForecastExtrapQueriesDesc(C.Structure):
+    _fields_ = [("state", SyForecastState), ("dt", C.c_void_p), ("n_query", C.c_void_p), ("Q", C.c_int32),
+                ("img_wh", C.c_void_p), ("box_out", C.c_void_p), ("score_out", C.c_void_p), ("label_out", C.c_void_p),
+                ("track_out", C.c_void_p), ("count_out", C.c_void_p)]
 
 
 class SyForecastSequencesDesc(C.Structure):
@@ -236,6 +242,7 @@ _SIG = {
     "sy_forecast_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32]),
     "sy_forecast_update": (C.c_int, [C.POINTER(SyForecastUpdateDesc), C.c_void_p]),
     "sy_forecast_extrap": (C.c_int, [C.POINTER(SyForecastExtrapDesc), C.c_void_p]),
+    "sy_forecast_extrap_queries": (C.c_int, [C.POINTER(SyForecastExtrapQueriesDesc), C.c_void_p]),
     "sy_forecast_sequences": (C.c_int, [C.POINTER(SyForecastSequencesDesc), C.c_void_p]),
     "sy_conv2d_wgrad_workspace_bytes": (C.c_size_t, [C.POINTER(SyConvWgradDesc)]),
     "sy_conv2d_wgrad_tc": (C.c_int, [C.POINTER(SyConvWgradDesc), C.c_void_p]),
@@ -635,11 +642,12 @@ def _on(t, dtype, shape, device):
     return _tensor_ok(t, dtype, len(shape)) and tuple(t.shape) == tuple(shape) and t.device == device
 
 
-def forecast_update(state, det, count, dt, start=None, keep=None, match_iou_th=0.3):
+def forecast_update(state, det, count, dt, start=None, keep=None, match_iou_th=0.3, clear_on_empty=False):
     """One new detection per stream into ``state`` (sy_forecast_update): ``det`` fp32 [S, max_det, 7] and ``count`` int32
     [S] as postprocess_nms / stream_rescale leave them, ``dt`` int32 [S] frames since each stream's previous detection,
     ``start`` / ``keep`` int32 [S] or None.  Nothing is read back: a stream whose count exceeds max_tracks keeps its state
-    and gets state.meta[s, 3] = 1."""
+    and gets state.meta[s, 3] = 1.  An empty detection keeps the predicted tracks (pps_forecast_kf.py), or with
+    ``clear_on_empty`` leaves the stream without tracks (the streamer, sAP/forecast/streamer.py)."""
     dev = state.x.device
     _require(_tensor_ok(det, torch.float32, 3) and det.shape[0] == state.streams and det.shape[2] == 7 and det.device == dev,
              f"forecast_update: det must be float32 [{state.streams}, max_det, 7] on {dev}")
@@ -648,7 +656,8 @@ def forecast_update(state, det, count, dt, start=None, keep=None, match_iou_th=0
                  f"forecast_update: {name} must be int32 [{state.streams}] on {dev}")
     d = SyForecastUpdateDesc(state.desc(), det.data_ptr(), det.shape[1], count.data_ptr(), dt.data_ptr(),
                              start.data_ptr() if start is not None else None, keep.data_ptr() if keep is not None else None,
-                             float(match_iou_th), state.workspace.data_ptr(), state.workspace.numel())
+                             float(match_iou_th), state.workspace.data_ptr(), state.workspace.numel(),
+                             1 if clear_on_empty else 0)
     _check(lib().sy_forecast_update(C.byref(d), _stream()))
 
 
@@ -671,6 +680,32 @@ def forecast_extrap(state, dt, img_wh, out=None):
     d = SyForecastExtrapDesc(state.desc(), dt.data_ptr(), img_wh.data_ptr(), box.data_ptr(), score.data_ptr(),
                              label.data_ptr(), track.data_ptr(), count.data_ptr())
     _check(lib().sy_forecast_extrap(C.byref(d), _stream()))
+    return out
+
+
+def forecast_extrap_queries(state, dt, n_query, img_wh, out=None):
+    """Up to Q queries per stream in one launch (sy_forecast_extrap_queries): stream s's tracks extrapolated ``dt[s, k]``
+    (fp32 [S, Q]) frames ahead for k < ``n_query[s]`` (int32 [S]), each cleaned up for ``img_wh`` (int32 [S, 2], (W, H)) ->
+    ``(box fp32 [S, Q, T, 4] ltwh, score fp32 [S, Q, T], label int32 [S, Q, T], track int32 [S, Q, T], count int32 [S, Q])``:
+    the first count[s, k] rows of query (s, k) are valid, count is 0 past n_query[s].  An integer dt gives forecast_extrap's
+    rows bit for bit.  ``out``: those five tensors of an earlier call to write into.  Capturable."""
+    s, t, dev = state.streams, state.max_tracks, state.x.device
+    q = dt.shape[1] if _tensor_ok(dt, torch.float32, 2) else 0
+    _require(q >= 1 and _on(dt, torch.float32, (s, q), dev), f"forecast_extrap_queries: dt must be float32 [{s}, Q] on {dev}")
+    _require(q <= 65535, f"forecast_extrap_queries: {q} queries per stream (at most 65535)")
+    _require(_on(n_query, torch.int32, (s,), dev), f"forecast_extrap_queries: n_query must be int32 [{s}] on {dev}")
+    _require(_on(img_wh, torch.int32, (s, 2), dev), f"forecast_extrap_queries: img_wh must be int32 [{s}, 2] on {dev}")
+    if out is None:
+        out = (torch.empty((s, q, t, 4), dtype=torch.float32, device=dev),
+               torch.empty((s, q, t), dtype=torch.float32, device=dev), torch.empty((s, q, t), dtype=torch.int32, device=dev),
+               torch.empty((s, q, t), dtype=torch.int32, device=dev), torch.empty((s, q), dtype=torch.int32, device=dev))
+    box, score, label, track, count = out
+    _require(_on(box, torch.float32, (s, q, t, 4), dev) and _on(score, torch.float32, (s, q, t), dev)
+             and _on(label, torch.int32, (s, q, t), dev) and _on(track, torch.int32, (s, q, t), dev)
+             and _on(count, torch.int32, (s, q), dev), "forecast_extrap_queries: out must be the five tensors of an earlier call")
+    d = SyForecastExtrapQueriesDesc(state.desc(), dt.data_ptr(), n_query.data_ptr(), q, img_wh.data_ptr(), box.data_ptr(),
+                                    score.data_ptr(), label.data_ptr(), track.data_ptr(), count.data_ptr())
+    _check(lib().sy_forecast_extrap_queries(C.byref(d), _stream()))
     return out
 
 

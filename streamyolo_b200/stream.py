@@ -28,6 +28,8 @@ frame did not decode, or that got none, keeps its carried features, starts no se
 The graph reads the weights and the folded BatchNorm as they were at capture: after ``load_state_dict`` (or any other
 change of the weights or running statistics) call ``capture()`` again.  Nothing checks this per frame.
 """
+import time
+
 import numpy as np
 import torch
 
@@ -46,7 +48,7 @@ class StreamTick:
     stream's features carried to the next tick."""
 
     def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None,
-                 forecast=None):
+                 forecast=None, clear_on_empty=False, queries=0):
         self.model, self.size = model, tuple(size)
         self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
         table = np.asarray(table, np.int32)
@@ -69,6 +71,15 @@ class StreamTick:
             self.fc_th = float(forecast[0])
             self.fc = ops.ForecastState(streams, forecast[1], device)
             self.fc_dt = torch.zeros((streams,), dtype=torch.int32, device=device)
+        self.fc_clear = bool(clear_on_empty)
+        # queries = Q > 0: the tick then extrapolates the updated tracks to up to Q queries per stream (sy_forecast_
+        # extrap_queries): fc_qdt (fp32 [S, Q]) and fc_nq (int32 [S]) are inputs set by the host, fc_qout the outputs
+        self.fc_q = int(queries)
+        if self.fc_q:
+            self.fc_qdt = torch.zeros((streams, self.fc_q), dtype=torch.float32, device=device)
+            self.fc_nq = torch.zeros((streams,), dtype=torch.int32, device=device)
+            self.fc_wh = torch.from_numpy(np.ascontiguousarray(table[:, [1, 0]])).to(device)   # (W, H)
+            self.fc_qout = None
         if jpeg_max_bytes is not None:
             self.bytes = torch.zeros((streams, jpeg_max_bytes), dtype=torch.uint8, device=device)
             self.lengths = torch.zeros((streams,), dtype=torch.int32, device=device)
@@ -95,7 +106,10 @@ class StreamTick:
                                                        max_det=self.raw.shape[1])
             ops.stream_rescale(self.det, self.count, self.status, self.ratio)
             if self.fc is not None:
-                ops.forecast_update(self.fc, self.det, self.count, self.fc_dt, self.start, self.keep, self.fc_th)
+                ops.forecast_update(self.fc, self.det, self.count, self.fc_dt, self.start, self.keep, self.fc_th,
+                                    clear_on_empty=self.fc_clear)
+            if self.fc_q:
+                self.fc_qout = ops.forecast_extrap_queries(self.fc, self.fc_qdt, self.fc_nq, self.fc_wh, self.fc_qout)
 
 
 NO_FRAME = -1     # last_status() of a stream that was given no frame
@@ -181,13 +195,21 @@ class StreamDetector:
       match_iou_th    the association's IoU threshold (inclusive)
       max_tracks      the most detections one stream's update takes; a tick with more raises RuntimeError naming the
                       stream, whose tracks are then left as they were
+    The sAP toolkit's streamer (sAP/forecast/streamer.py, see streamyolo_b200.streamer), with ``forecast=True``:
+      clear_on_empty  True: an empty detection leaves the stream without tracks, as the streamer's association does
+                      (the default keeps the predicted tracks, as pps_forecast_kf.py does)
+      queries         Q > 0: the tick ends with the extrapolation of each stream's updated tracks to up to Q queries
+                      (sy_forecast_extrap_queries), given to ``step`` / ``step_jpeg`` as ``query_dt`` and read back
+                      with the detections, one synchronisation per tick (``last_queries``)
+      ``submit`` / ``poll`` / ``receive`` run a tick without waiting for it, and ``publish`` / ``query`` extrapolate the
+      tracks of the last received tick while the next one is in flight (the wall-clock streamer)
     Each stream's frame is transformed as data.sized_table says and its boxes divided by its own ratio (``ratios``): a frame
     of driver size ``input_size`` gets the driver's plain resize and ``in_scale``.  ``frame_hw`` is the slot the frames are
     stored in: the largest height and width (the frame size when every stream has one size)."""
 
     def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
                  frame_sizes=None, input_size=None, jpeg_max_bytes=None, forecast=False, match_iou_th=0.3,
-                 max_tracks=1024):
+                 max_tracks=1024, clear_on_empty=False, queries=0):
         if model.training:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
@@ -208,6 +230,10 @@ class StreamDetector:
             jpeg_max_bytes = feed.check_max_bytes(jpeg_max_bytes, "StreamDetector: jpeg_max_bytes")
         if forecast and (int(max_tracks) != max_tracks or not 1 <= max_tracks <= 1 << 20):
             raise ValueError(f"StreamDetector: max_tracks must be an integer in [1, 2^20], not {max_tracks}")
+        if int(queries) != queries or not 0 <= queries <= 65535:
+            raise ValueError(f"StreamDetector: queries must be an integer in [0, 65535], not {queries}")
+        if (clear_on_empty or queries) and not forecast:
+            raise ValueError("StreamDetector: clear_on_empty and queries take forecast=True")
         try:
             table, ratios = data.sized_table(sizes, size, in_scale)
         except RuntimeError as e:
@@ -218,13 +244,21 @@ class StreamDetector:
         self.frame_sizes, self.ratios = sizes, ratios
         self.jpeg_max_bytes = jpeg_max_bytes
         self.forecasting = bool(forecast)
+        self.queries = int(queries)
         self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes,
-                                (match_iou_th, int(max_tracks)) if forecast else None)
+                                (match_iou_th, int(max_tracks)) if forecast else None, clear_on_empty, self.queries)
         if self.forecasting:
             self._fc_dt = feed.pinned((streams,), torch.int32)
             self._fc_meta = feed.pinned((streams, 4), torch.int32)
             self._fc_wh = torch.tensor([(w, h) for h, w in sizes], dtype=torch.int32, device=dev)
             self._fc_out = None
+        if self.queries:
+            self._q_dt = feed.pinned((streams, self.queries), torch.float32)
+            self._q_n = feed.pinned((streams,), torch.int32)
+            self._q_out = None
+            self._queries = None
+        self._pub = None                          # publish / query: the published tracks, their stream and events
+        self._inflight = None
         self.frame_hw = tuple(self._tick.frames.shape[1:3])          # the slot: the largest height and width
         if self.jpeg_max_bytes is None:           # stream i's frame is staged at the start of slot i (see step)
             self._stage = feed.pinned(tuple(self._tick.frames.shape), torch.uint8)
@@ -245,6 +279,9 @@ class StreamDetector:
         self._graph = engine.capture_graph(t.run, t.frames.device)
         self._det = feed.pinned((self.streams, t.raw.shape[1], 7), torch.float32)
         self._count = feed.pinned((self.streams,), torch.int32)
+        if self.queries:
+            self._q_out = tuple(feed.pinned(tuple(o.shape), o.dtype) for o in t.fc_qout)
+        self._inflight = None
         if self.forecasting:                      # the warm-up run went through the update: no stream has tracks yet
             t.fc.meta.zero_()
             self._fc_last = [None] * self.streams         # each stream's frame index at its last update
@@ -259,19 +296,28 @@ class StreamDetector:
                 raise ValueError(f"StreamDetector.reset: stream {stream} not in [0, {self.streams})")
             self._flags[stream] = 1
 
-    def step(self, frames, fidx=None):
+    def step(self, frames, fidx=None, query_dt=None):
         """One frame per stream -> a list of S ``(bboxes, scores, labels)`` numpy tuples, what the driver's inference()
         returns (boxes in frame pixels, float32 [n, 4]; scores float32 [n]; labels int32 [n]).  ``frames``: a list of S
         frames, frame i uint8 BGR [h_i, w_i, 3] of stream i's size; or, when every stream has the same size, uint8
         [S, h, w, 3] ([h, w, 3] for one stream).  Each a numpy array, a CPU tensor or a CUDA tensor.  A detector built with
         ``jpeg_max_bytes`` takes files only: ``step`` raises RuntimeError there, use ``step_jpeg``.  With ``forecast=True``,
         ``fidx`` gives each stream's frame index (a list of S ints; an int for one stream), and the tick updates the
-        stream's tracks with its detections (see ``forecast``)."""
-        t = self._tick
+        stream's tracks with its detections (see ``forecast``).  With ``queries``, ``query_dt`` gives each stream's query
+        offsets (a list of S sequences of at most Q frame counts, floats; None: none) that the tick extrapolates the
+        updated tracks to (see ``last_queries``)."""
         fidx = self._fidx(fidx, "step")
+        self._stage_frames(frames, "step")
+        self._queries_in(query_dt, "step")
+        return self._run(None, fidx)
+
+    def _stage_frames(self, frames, what):
+        """``frames`` of ``step`` copied (asynchronously) into the tick's frame slots"""
+        t = self._tick
         if self.jpeg_max_bytes is not None:
-            raise RuntimeError("StreamDetector.step: this detector was built with jpeg_max_bytes, and its replay decodes the "
-                               "streams' files: feed it with step_jpeg (build one with frame_sizes alone for decoded frames)")
+            raise RuntimeError(f"StreamDetector.{what}: this detector was built with jpeg_max_bytes, and its replay decodes "
+                               "the streams' files: feed it with step_jpeg (build one with frame_sizes alone for decoded "
+                               "frames)")
         if isinstance(frames, (list, tuple)):
             ops._require(len(frames) == self.streams, f"StreamDetector.step: give a list of {self.streams} frames, one per stream")
             for i, (f, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
@@ -293,13 +339,12 @@ class StreamDetector:
             else:
                 self._stage.copy_(src)
                 t.frames.copy_(self._stage, non_blocking=True)
-        return self._run(None, fidx)
 
     def last_raw(self):
         """A device copy of the last tick's head outputs [S, A, 5 + nc] (what the driver keeps as ``results_raw``)."""
         return self._tick.raw.clone()
 
-    def step_jpeg(self, files, fidx=None):
+    def step_jpeg(self, files, fidx=None, query_dt=None):
         """One JPEG file per stream -> a list of S ``(bboxes, scores, labels)`` tuples as ``step`` returns them, with one
         host synchronisation.  ``files``: a list of S entries, each the file's bytes (``bytes``, or a uint8 numpy array or
         CPU tensor) of at most ``jpeg_max_bytes``, or None when the stream has no frame this tick.  A stream whose file
@@ -318,7 +363,29 @@ class StreamDetector:
             if a.size:
                 t.bytes[i, :a.size].copy_(self._jstage[i, :a.size], non_blocking=True)
         t.lengths.copy_(self._jlen, non_blocking=True)
+        self._queries_in(query_dt, "step_jpeg")
         return self._run([a.size > 0 for a in files], fidx)
+
+    def _queries_in(self, query_dt, what):
+        """``query_dt`` of step / step_jpeg into the pinned query inputs, copied to the tick's"""
+        if not self.queries:
+            if query_dt is not None:
+                raise ValueError(f"StreamDetector.{what}: query_dt takes a detector built with queries > 0")
+            return
+        query_dt = [None] * self.streams if query_dt is None else query_dt
+        if not isinstance(query_dt, (list, tuple)) or len(query_dt) != self.streams \
+                or any(q is not None and len(q) > self.queries for q in query_dt):
+            raise ValueError(f"StreamDetector.{what}: query_dt must hold {self.streams} sequences of at most "
+                             f"{self.queries} frame counts (None for none)")
+        self._q_dt.zero_()
+        for i, q in enumerate(query_dt):
+            n = 0 if q is None else len(q)
+            self._q_n[i] = n
+            if n:
+                self._q_dt[i, :n] = torch.from_numpy(np.asarray(q, np.float32))
+        t = self._tick
+        t.fc_qdt.copy_(self._q_dt, non_blocking=True)
+        t.fc_nq.copy_(self._q_n, non_blocking=True)
 
     def _fidx(self, fidx, what):
         """``fidx`` of step / step_jpeg as a list of S ints (None without forecast)"""
@@ -345,11 +412,21 @@ class StreamDetector:
     def _run(self, present, fidx=None):
         """Replay the tick on the staged inputs and return the detections; ``present`` (JPEG ticks only): which streams
         were given a file; ``fidx``: the streams' frame indices (forecast only)."""
+        self._launch(present, fidx)
+        torch.cuda.current_stream().synchronize()
+        return self._finish(present, fidx)
+
+    def _launch(self, present, fidx):
+        """the replay and the copies out of ``_run``, queued on the current stream"""
+        if self._inflight is not None:
+            raise RuntimeError("StreamDetector: a submitted tick is still in flight: receive() it first")
         t = self._tick
         t.flags.copy_(self._flags, non_blocking=True)
         if fidx is not None:
             self._dt(fidx)
             t.fc_dt.copy_(self._fc_dt, non_blocking=True)
+        if self._pub is not None:                 # the tick rewrites the tracks a pending publish copies
+            torch.cuda.current_stream().wait_event(self._pub["copied"])
         self._graph.replay()
         self._det.copy_(t.det, non_blocking=True)
         self._count.copy_(t.count, non_blocking=True)
@@ -357,7 +434,13 @@ class StreamDetector:
             self._status.copy_(t.status, non_blocking=True)
         if fidx is not None:
             self._fc_meta.copy_(t.fc.meta, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
+        if self.queries:
+            for h, d in zip(self._q_out, t.fc_qout):
+                h.copy_(d, non_blocking=True)
+
+    def _finish(self, present, fidx):
+        """the host's side of ``_run`` once the tick and its copies are done -> the detections"""
+        t = self._tick
         if present is None:
             updated = [True] * self.streams
             self._flags.zero_()
@@ -374,8 +457,104 @@ class StreamDetector:
             for i, u in enumerate(updated):
                 if u:
                     self._fc_last[i] = fidx[i]
+        if self.queries:
+            box, score, label, track, count = (h.numpy() for h in self._q_out)
+            n_q, meta = self._q_n.tolist(), self._fc_meta.numpy()
+            self._queries = [[None if meta[i, 0] == 0 else
+                              (box[i, k, :n].copy(), score[i, k, :n].copy(), label[i, k, :n].copy(), track[i, k, :n].copy())
+                              for k, n in enumerate(count[i, :n_q[i]].tolist())] for i in range(self.streams)]
         det = self._det.numpy()
         return [sized_output(det[i, :n]) for i, n in enumerate(self._count.tolist())]
+
+    def last_queries(self):
+        """The extrapolations of the last ``step`` / ``step_jpeg`` (a detector built with ``queries``): per stream, one
+        entry per ``query_dt`` offset, ``(ltwh, scores, labels, tracks)`` as ``forecast`` returns them, or None where the
+        stream has no track after its update (the streamer then emits empty arrays of its own dtypes)"""
+        if not self.queries:
+            raise RuntimeError("StreamDetector.last_queries: build the detector with queries > 0")
+        return self._queries
+
+    def submit(self, frames, fidx=None):
+        """``step`` without the wait: stage ``frames`` and queue the replay and its copies, then return.  ``poll`` tells
+        when it is done and ``receive`` then returns what ``step`` returns.  One tick at a time."""
+        fidx = self._fidx(fidx, "submit")
+        if self._inflight is not None:
+            raise RuntimeError("StreamDetector.submit: a submitted tick is still in flight: receive() it first")
+        if self.queries:
+            raise RuntimeError("StreamDetector.submit: a detector built with queries runs its ticks with step / step_jpeg")
+        self._stage_frames(frames, "submit")
+        self._launch(None, fidx)
+        done = torch.cuda.Event()
+        done.record()
+        self._inflight = (done, fidx)
+
+    def poll(self, timeout):
+        """True once the submitted tick is done, waiting at most ``timeout`` seconds for it (the toolkit's
+        ``Pipe.poll(timeout)``); False when it is still running then"""
+        if self._inflight is None:
+            raise RuntimeError("StreamDetector.poll: no tick was submitted")
+        done = self._inflight[0]
+        end = time.perf_counter() + max(float(timeout), 0.0)
+        while not done.query():
+            if time.perf_counter() >= end:
+                return False
+        return True
+
+    def receive(self):
+        """The submitted tick's detections, as ``step`` returns them; waits for it when ``poll`` has not seen it done"""
+        if self._inflight is None:
+            raise RuntimeError("StreamDetector.receive: no tick was submitted")
+        done, fidx = self._inflight
+        done.synchronize()
+        self._inflight = None
+        return self._finish(None, fidx)
+
+    def publish(self):
+        """Copy the tracks of the last received tick to the buffers ``query`` reads, on a stream of their own: a tick
+        submitted after this waits for the copy, and no tick in flight writes what a query reads"""
+        if not self.forecasting:
+            raise RuntimeError("StreamDetector.publish: build the detector with forecast=True")
+        if self._inflight is not None:
+            raise RuntimeError("StreamDetector.publish: receive() the submitted tick first")
+        t = self._tick
+        if self._pub is None:
+            self._pub = {"state": ops.ForecastState(self.streams, t.fc.max_tracks, t.fc.x.device),
+                         "stream": torch.cuda.Stream(t.fc.x.device), "copied": torch.cuda.Event(), "out": None,
+                         "host": None, "dt": feed.pinned((self.streams, 1), torch.float32),
+                         "n": torch.ones((self.streams,), dtype=torch.int32, device=t.fc.x.device),
+                         "meta": feed.pinned((self.streams, 4), torch.int32)}
+        p = self._pub
+        p["stream"].wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(p["stream"]):
+            for name in ("x", "P", "label", "score", "track", "meta"):
+                getattr(p["state"], name).copy_(getattr(t.fc, name))
+            p["copied"].record()
+        p["meta"].copy_(self._fc_meta)
+
+    def query(self, dt):
+        """The published tracks extrapolated ``dt`` frames ahead (a list of S numbers, fp32 frame counts; a number for
+        one stream) -> per stream ``(ltwh, scores, labels, tracks)`` as ``forecast`` returns them, or None where the
+        stream had no track.  One launch (sy_forecast_extrap_queries) and one synchronisation of the publish stream: it
+        does not wait for a tick in flight."""
+        if self._pub is None:
+            raise RuntimeError("StreamDetector.query: publish() the tracks first")
+        p = self._pub
+        dt = [dt] if np.ndim(dt) == 0 else list(dt)
+        if len(dt) != self.streams:
+            raise ValueError(f"StreamDetector.query: give {self.streams} offsets")
+        p["dt"][:, 0] = torch.from_numpy(np.asarray(dt, np.float32))
+        with torch.cuda.stream(p["stream"]):
+            d = p["dt"].to(p["state"].x.device, non_blocking=True)
+            p["out"] = ops.forecast_extrap_queries(p["state"], d, p["n"], self._fc_wh, p["out"])
+            if p["host"] is None:
+                p["host"] = tuple(feed.pinned(tuple(o.shape), o.dtype) for o in p["out"])
+            for h, o in zip(p["host"], p["out"]):
+                h.copy_(o, non_blocking=True)
+        p["stream"].synchronize()
+        box, score, label, track, count = (h.numpy() for h in p["host"])
+        return [None if p["meta"][i, 0] == 0 else
+                (box[i, 0, :n].copy(), score[i, 0, :n].copy(), label[i, 0, :n].copy(), track[i, 0, :n].copy())
+                for i, n in enumerate(count[:, 0].tolist())]
 
     def forecast(self, fidx):
         """Each stream's tracks extrapolated to its frame index ``fidx`` (a list of S ints; an int for one stream) ->
