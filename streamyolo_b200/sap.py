@@ -5,17 +5,33 @@ pickles and time_info.pkl out, for the reference's streaming_eval.py to score.
     python -m streamyolo_b200.sap --data-root ... --annot-path .../val.json --fps 30 --in_scale 0.5 --no-mask \\
         --out-dir ... --overwrite --config cfgs/l_s50_onex_dfp_tal_flip.py --weights l_s50_one_x.pth     # wall clock
     python -m streamyolo_b200.sap ... --clock simulated --runtime-ms 33 --streams 8                       # simulated clock
+    python -m streamyolo_b200.sap ... --clock simulated --runtime rt.pkl --seed 0 --streams 8           # drawn runtimes
+    python -m streamyolo_b200.sap ... --clock infinite --runtime rt.pkl --seed 0 --streams 8            # infinite GPUs
 
-It takes the driver's arguments (``--cpu-pre`` and ``--no-class-mapping`` are ignored, as there) and three more:
+It takes the driver's arguments (``--cpu-pre`` and ``--no-class-mapping`` are ignored, as there) and these:
 
   --clock wall       (default) the driver's loop (:152-195) on ``time.perf_counter``, one sequence at a time.  Before a
                      sequence starts its files are decoded on the device (``data.decode_jpeg``, bit-exact against
                      cv2.imread) into one device tensor, outside the timed region as the driver's cv2.imread loop is;
                      each tick is one ``StreamDetector.step`` (one CUDA graph replay).
   --clock simulated  the simulated-time scheduler of sAP/det/srt_det.py:102-165 with a constant runtime of
-                     ``--runtime-ms`` per frame: the schedule no longer depends on the detector, so every sequence's
-                     frame list is computed first and up to ``--streams`` sequences run at once, one stream each, in one
-                     ``StreamDetector(jpeg_max_bytes=...)``.  ``runtime`` is the given constant for every frame.
+                     ``--runtime-ms`` per frame, or with each frame's runtime drawn from the ``--runtime`` distribution
+                     (scaled by ``--perf-factor``, seeded by ``--seed``) as srt_det.py draws it: the schedule no longer
+                     depends on the detector, so every sequence's frame list is computed first and up to ``--streams``
+                     sequences run at once, one stream each, in one ``StreamDetector(jpeg_max_bytes=...)``.  ``runtime``
+                     holds each kept frame's runtime.
+  --clock infinite   sAP/det/srt_det_inf.py, the same protocol with infinite GPUs: every frame ii is detected and its
+                     result is out at ``ii / fps + draw``; each pickle is then reordered by ``np.argsort(timestamps)``.
+                     The script runs single-frame detectors; here frame ii is fused with frame ii - 1 (frame 0 with
+                     itself), what the driver's loop gives when it detects every frame.  The frames run as on the
+                     simulated clock, a sequence's frames on one stream, up to ``--streams`` sequences at once.
+
+``--runtime`` is a pickled ``{'type': 'empirical', 'samples': [...]}``, what sAP/util/add_to_runtime_zoo.py makes of a
+run's time_info.pkl.  The draws are the scripts' bit for bit: ``np.random.RandomState(seed).choice(samples /
+perf_factor)``, one per frame that passes the stride / dynamic-schedule checks (the one that ends a sequence included),
+the generator carried from one sequence to the next in the annotation file's order.  The global numpy state is left
+alone.  ``--cached-res`` (replaying stored single-frame results) raises NotImplementedError: a StreamYOLO detection
+depends on the frame processed before it, so cached single-frame results cannot be re-scheduled.
 
 Boxes are in frame pixels: the detector divides by ``--in_scale``, which is what the driver's ``inference()`` divides by
 at the default 0.5 (it keeps its own default of 0.5 whatever ``--in_scale`` says).  Frames must be 1200 x 1920, the size
@@ -39,11 +55,12 @@ DECODE_BATCH = 16                 # files per decode_jpeg call when a sequence i
 
 
 def parse_args(argv=None):
-    """The driver's arguments (streamyolo_det.py:30-47) and ``--clock``, ``--runtime-ms``, ``--streams``."""
+    """The driver's arguments (streamyolo_det.py:30-47) and ``--clock``, ``--runtime-ms``, ``--streams``; srt_det.py's
+    ``--runtime``, ``--perf-factor``, ``--seed`` and ``--cached-res``."""
     p = argparse.ArgumentParser(prog="python -m streamyolo_b200.sap")
     p.add_argument("--data-root", type=str, required=True)
     p.add_argument("--annot-path", type=str, required=True)
-    p.add_argument("--det-stride", type=float, default=1)
+    p.add_argument("--det-stride", type=float, default=None)
     p.add_argument("--in_scale", type=float, default=0.5)
     p.add_argument("--fps", type=float, default=30)
     p.add_argument("--no-mask", action="store_true", default=False)
@@ -54,17 +71,67 @@ def parse_args(argv=None):
     p.add_argument("--config", type=str, required=True)
     p.add_argument("--weights", type=str, required=True)
     p.add_argument("--overwrite", action="store_true", default=False)
-    p.add_argument("--clock", choices=("wall", "simulated"), default="wall")
+    p.add_argument("--clock", choices=("wall", "simulated", "infinite"), default="wall")
     p.add_argument("--runtime-ms", type=float, default=None, help="simulated clock: the runtime of every frame")
-    p.add_argument("--streams", type=int, default=1, help="simulated clock: sequences run at once")
+    p.add_argument("--runtime", type=str, default=None, help="simulated and infinite clocks: a pickled runtime "
+                   "distribution ({'type': 'empirical', 'samples': [...]}) to draw each frame's runtime from")
+    p.add_argument("--perf-factor", type=float, default=None, help="with --runtime: samples are divided by it (default 1)")
+    p.add_argument("--seed", type=int, default=None, help="with --runtime: the draws' seed (default 0)")
+    p.add_argument("--cached-res", type=str, default=None, help="not supported (see the module doc)")
+    p.add_argument("--streams", type=int, default=1, help="simulated and infinite clocks: sequences run at once")
     opts = p.parse_args(argv)
-    if opts.clock == "wall" and (opts.runtime_ms is not None or opts.streams != 1):
-        p.error("--runtime-ms and --streams take --clock simulated; the wall clock runs one sequence at a time")
-    if opts.clock == "simulated" and (opts.runtime_ms is None or not opts.runtime_ms > 0):
-        p.error("--clock simulated needs a positive --runtime-ms")
+    if opts.clock == "wall" and (opts.runtime_ms is not None or opts.runtime is not None or opts.streams != 1):
+        p.error("--runtime-ms, --runtime and --streams take --clock simulated or infinite; the wall clock runs one "
+                "sequence at a time")
+    if opts.runtime_ms is not None and opts.runtime is not None:
+        p.error("--runtime-ms and --runtime are mutually exclusive")
+    if opts.clock == "simulated" and opts.runtime is None and (opts.runtime_ms is None or not opts.runtime_ms > 0):
+        p.error("--clock simulated needs a positive --runtime-ms or a --runtime distribution")
+    if opts.clock == "infinite":
+        if opts.runtime is None:
+            p.error("--clock infinite needs a --runtime distribution")
+        if opts.det_stride is not None or opts.dynamic_schedule:
+            p.error("--clock infinite detects every frame: it takes neither --det-stride nor --dynamic-schedule")
+    if opts.runtime is None and (opts.perf_factor is not None or opts.seed is not None):
+        p.error("--perf-factor and --seed take --runtime")
+    if opts.perf_factor is not None and not opts.perf_factor > 0:
+        p.error("--perf-factor must be positive")
     if opts.streams < 1:
         p.error("--streams must be at least 1")
+    opts.det_stride = 1 if opts.det_stride is None else opts.det_stride
+    opts.perf_factor = 1 if opts.perf_factor is None else opts.perf_factor
+    opts.seed = 0 if opts.seed is None else opts.seed
+    if opts.cached_res is not None:
+        raise NotImplementedError("--cached-res: a StreamYOLO detection depends on the frame processed before it, so "
+                                  "stored single-frame results cannot be re-scheduled")
     return opts
+
+
+class Empirical:
+    """srt_det.py's runtime distribution (util/runtime_dist.py ``Empirical``) on a generator of its own: ``samples /
+    perf_factor`` in float64 (the values of the script's in-place ``/=``), ``draw()`` is ``np.random.choice(samples)``
+    after ``np.random.seed(seed)``, and the global numpy state is left alone."""
+
+    def __init__(self, samples, perf_factor=1, seed=0):
+        if not perf_factor > 0:
+            raise ValueError(f"perf_factor must be positive, not {perf_factor}")
+        self.samples = np.asarray(samples, np.float64) / perf_factor
+        self.rng = np.random.RandomState(seed)
+
+    def draw(self):
+        return self.rng.choice(self.samples)
+
+    def mean(self):
+        return self.samples.mean()
+
+
+def load_runtime(path, perf_factor=1, seed=0):
+    """a pickled runtime distribution -> ``Empirical``; ValueError for any type but 'empirical', as dist_from_dict"""
+    with open(path, "rb") as f:
+        dist = pickle.load(f)
+    if dist["type"] != "empirical":
+        raise ValueError(f'Unknown distribution type "{dist["type"]}"')
+    return Empirical(dist["samples"], perf_factor, seed)
 
 
 def sequences(dataset):
@@ -119,13 +186,16 @@ def wall_sequence(det, frames, n_frame, fps, det_stride, dynamic_schedule, clock
 
 
 def simulated_schedule(n_frame, fps, det_stride, dynamic_schedule, runtime):
-    """srt_det.py:102-165 with every frame taking ``runtime`` seconds -> (input_fidx, timestamps).  Without detector
-    outputs in it, the schedule is a function of these five numbers."""
+    """srt_det.py:102-165.  ``runtime`` is a number, the seconds every frame takes -> (input_fidx, timestamps); or an
+    ``Empirical`` that each frame's runtime is drawn from -> (input_fidx, timestamps, runtime), the last the draws of
+    the frames kept.  The detector's outputs take no part in the schedule: it is a function of these arguments (and of
+    the generator's state, which moves on by one draw per frame run, the one that ends the sequence included)."""
+    draws = None if np.isscalar(runtime) else []
     input_fidx, timestamps = [], []
     last_fidx = None
     t_total = n_frame / fps
     t_elapsed = 0
-    mean_rtf = runtime * fps
+    mean_rtf = (runtime if draws is None else runtime.mean()) * fps
     stride_cnt = 0
     while t_elapsed < t_total:
         fidx_continuous = t_elapsed * fps
@@ -146,12 +216,24 @@ def simulated_schedule(n_frame, fps, det_stride, dynamic_schedule, runtime):
         else:
             stride_cnt += 1
             continue
-        t_elapsed += runtime
+        rt_this = runtime if draws is None else runtime.draw()
+        t_elapsed += rt_this
         if t_elapsed >= t_total:
             break
         timestamps.append(t_elapsed)
         input_fidx.append(fidx)
-    return input_fidx, timestamps
+        if draws is not None:
+            draws.append(rt_this)
+    return (input_fidx, timestamps) if draws is None else (input_fidx, timestamps, draws)
+
+
+def infinite_order(out):
+    """srt_det_inf.py:127-134: a sequence's pickle dict, its frames in detection order, reordered in place by
+    ``np.argsort(timestamps)`` (the default, unstable kind: ties fall as they fall in the script)"""
+    idx = np.argsort(out["timestamps"])
+    for k in ("timestamps", "results_raw", "results_parsed", "input_fidx", "runtime"):
+        out[k] = [out[k][i] for i in idx]
+    return out
 
 
 def pack_ticks(lengths, streams):
@@ -178,17 +260,18 @@ def pack_ticks(lengths, streams):
 
 def run_simulated(det, files, schedules, runtime, done):
     """Run every sequence's scheduled frames on the streams of ``det`` (a StreamDetector built with ``jpeg_max_bytes``),
-    packed by ``pack_ticks``.  ``files[q]`` are sequence q's file paths, ``schedules[q]`` its (input_fidx, timestamps);
+    packed by ``pack_ticks``.  ``files[q]`` are sequence q's file paths, ``schedules[q]`` its (input_fidx, timestamps)
+    with ``runtime`` the runtime of every frame, or its (input_fidx, timestamps, runtimes) with ``runtime`` None;
     ``done(q, out)`` gets sequence q's pickle dict as soon as its last frame has run (and every empty sequence first).
 
     A host thread reads the files of tick k + 1 while tick k runs.  Only the files are held: S decoded sequences (6.2 GB
     each at 900 frames of 1200 x 1920) would not fit, so each tick's replay decodes its S files itself."""
-    outs = [{"results_raw": [], "results_parsed": [], "timestamps": list(ts), "input_fidx": list(fi),
-             "runtime": [runtime] * len(fi)} for fi, ts in schedules]
-    for q, (fi, _) in enumerate(schedules):
+    outs = [{"results_raw": [], "results_parsed": [], "timestamps": list(s[1]), "input_fidx": list(s[0]),
+             "runtime": [runtime] * len(s[0]) if runtime is not None else list(s[2])} for s in schedules]
+    for q, (fi, *_) in enumerate(schedules):
         if not fi:
             done(q, outs[q])
-    lengths = [len(fi) for fi, _ in schedules]
+    lengths = [len(s[0]) for s in schedules]
     ticks = pack_ticks(lengths, det.streams) if any(lengths) else []
 
     def path(e):
@@ -298,13 +381,23 @@ def run(opts, model, clock=time.perf_counter, detector=stream.StreamDetector):
             done(q, wall_sequence(det, frames, len(p), opts.fps, opts.det_stride, opts.dynamic_schedule, clock))
             del frames
     else:
-        rt = opts.runtime_ms / 1000.0
-        schedules = [simulated_schedule(len(p), opts.fps, opts.det_stride, opts.dynamic_schedule, rt) for p in paths]
-        used = [p[i] for p, (fi, _) in zip(paths, schedules) for i in fi]
-        busy = sum(1 for fi, _ in schedules if fi)
+        # every schedule first, in the sequences' order: the draws carry the generator from one sequence to the next
+        rt = None if opts.runtime is None else load_runtime(opts.runtime, opts.perf_factor, opts.seed)
+        const = opts.runtime_ms / 1000.0 if rt is None else None
+        if opts.clock == "simulated":
+            schedules = [simulated_schedule(len(p), opts.fps, opts.det_stride, opts.dynamic_schedule,
+                                            const if rt is None else rt) for p in paths]
+        else:                                     # srt_det_inf.py:98-125: every frame, out at ii / fps + draw
+            schedules = []
+            for p in paths:
+                draws = [rt.draw() for _ in range(len(p))]
+                schedules.append((list(range(len(p))), [ii / opts.fps + d for ii, d in enumerate(draws)], draws))
+        finish = done if opts.clock == "simulated" else lambda q, out: done(q, infinite_order(out))
+        used = [p[i] for p, s in zip(paths, schedules) for i in s[0]]
+        busy = sum(1 for s in schedules if s[0])
         det = None if not used else detector(model, frame_sizes=[DRIVER_HW] * min(opts.streams, busy),
                                              in_scale=opts.in_scale, jpeg_max_bytes=feed.default_max_bytes(used))
-        run_simulated(det, paths, schedules, rt, done)
+        run_simulated(det, paths, schedules, const, finish)
     runtime_all = [r for rs in runtimes for r in rs]
     n_processed, n_total = len(runtime_all), sum(len(p) for p in paths)
     runtime_all_np = np.asarray(runtime_all)

@@ -13,7 +13,13 @@ Wall clock (one sequence, the legs alternating over ROUNDS rounds):
 Simulated clock: 16 sequences at a constant 40 ms runtime through sap.run_simulated at S = 1, 4, 8, 16 streams, total
 seconds (the pickles are built but not written), ROUNDS_SIM rounds alternating S.
 
-usage: python tools/bench_sap.py [rounds] [frames] [out path]"""
+Infinite clock (``infinite``, this leg alone): INF_SEQ sequences of [frames] frames (default INF_FRAMES), every frame
+detected with runtimes drawn from a synthetic distribution as ``--clock infinite`` draws them, through sap.run_simulated
+and srt_det_inf's reordering (sap.infinite_order) at S = 1, 8, 16 streams: detected frames per second, ROUNDS_SIM rounds
+alternating S after one warm-up pass per S.
+
+usage: python tools/bench_sap.py [rounds] [frames] [out path]
+       python tools/bench_sap.py infinite [frames] [out path]"""
 import os
 import statistics
 import sys
@@ -25,16 +31,21 @@ sys.path.insert(0, HERE)
 import numpy as np
 import torch
 
-from bench_stream import calibrated_l, card, eager_frame
+ARGV, sys.argv[1:] = sys.argv[1:], []        # bench_stream parses its own arguments when it is imported
+from bench_stream import calibrated_l, card, eager_frame  # noqa: E402
 from oracle.make_stream_jpeg_golden import SEQ, requant
 from streamyolo_b200 import sap, stream
 
-ROUNDS = int(sys.argv[1]) if len(sys.argv) > 1 else 3
-FRAMES = int(sys.argv[2]) if len(sys.argv) > 2 else 900
-OUT = sys.argv[3] if len(sys.argv) > 3 else None
+INFINITE = len(ARGV) > 0 and ARGV[0] == "infinite"
+ROUNDS = 0 if INFINITE else int(ARGV[0]) if len(ARGV) > 0 else 3
+FRAMES = int(ARGV[1]) if len(ARGV) > 1 else 150 if INFINITE else 900
+OUT = ARGV[2] if len(ARGV) > 2 else None
 ROUNDS_SIM = 2
 N_SEQ, RUNTIME, FPS = 16, 0.040, 30.0
 STREAMS = (1, 4, 8, 16)
+INF_SEQ, INF_STREAMS = 16, (1, 8, 16)
+# a synthetic runtime_all (seconds) for the infinite clock's draws; they set the timestamps, not the work
+INF_SAMPLES = [0.021, 0.034, 0.028, 0.061, 0.019, 0.045, 0.030, 0.083]
 G = np.load(os.path.join(os.path.dirname(HERE), "tests", "golden", "stream_jpeg_files.npz"))
 
 
@@ -67,6 +78,37 @@ def pct(v, q):
     return float(np.percentile(np.asarray(v) * 1e3, q))
 
 
+def infinite(model, files, lines):
+    """the infinite clock's leg: -> lines appended to ``lines``"""
+    paths = [[files[j % SEQ] for j in range(FRAMES)]] * INF_SEQ
+    dist = sap.Empirical(INF_SAMPLES, 1, 0)
+    schedules = []
+    for p in paths:
+        draws = [dist.draw() for _ in p]
+        schedules.append((list(range(len(p))), [ii / FPS + d for ii, d in enumerate(draws)], draws))
+    used = sum(len(p) for p in paths)
+    dets = {s: stream.StreamDetector(model, frame_sizes=[sap.DRIVER_HW] * s, in_scale=0.5,
+                                     jpeg_max_bytes=max(os.path.getsize(p) for p in files) + 4096) for s in INF_STREAMS}
+    done = lambda q, o: sap.infinite_order(o)            # noqa: E731
+    for s in INF_STREAMS:                                  # warm-up: every graph replayed, the file reader started
+        sap.run_simulated(dets[s], [p[:2 * s] for p in paths[:s]], [(f[:2 * s], t[:2 * s], r[:2 * s]) for f, t, r in
+                          schedules[:s]], None, done)
+    sec = {s: [] for s in INF_STREAMS}
+    for r in range(ROUNDS_SIM):
+        for s in INF_STREAMS:
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            sap.run_simulated(dets[s], paths, schedules, None, done)
+            torch.cuda.synchronize()
+            sec[s].append(time.perf_counter() - t0)
+            print(f"round {r}: infinite S={s} {sec[s][-1]:.2f} s", flush=True)
+    lines.append(f"infinite clock, {INF_SEQ} sequences of {FRAMES} frames, every frame run ({used} frames), total seconds "
+                 "(median, min-max), frames/s:")
+    for s in INF_STREAMS:
+        m = statistics.median(sec[s])
+        lines.append(f"  S={s:2d} {m:7.2f} s ({min(sec[s]):.2f}-{max(sec[s]):.2f}), {used / m:.0f} frames/s")
+
+
 def main():
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
@@ -90,6 +132,9 @@ def main():
     lines.append(f"sequence: {FRAMES} files, {mb:.1f} MB")
     model = calibrated_l(dev)
     model.activation_dtype = torch.float16
+    if INFINITE:
+        infinite(model, files, lines)
+        return finish(lines, files, tmp)
     det = stream.StreamDetector(model, frame_hw=sap.DRIVER_HW, in_scale=0.5)
     eager = EagerDriver(model)
     sap.decode_sequence(seq[:32], sap.DRIVER_HW, dev)                # warm-up: module load, workspace
@@ -156,6 +201,10 @@ def main():
     for s in STREAMS:
         m = statistics.median(sim[s])
         lines.append(f"  S={s:2d} {m:7.2f} s ({min(sim[s]):.2f}-{max(sim[s]):.2f}), {used / m:.0f} frames/s")
+    finish(lines, files, tmp)
+
+
+def finish(lines, files, tmp):
     text = "\n".join(lines)
     print(text)
     if OUT:
