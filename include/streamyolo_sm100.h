@@ -648,6 +648,35 @@ typedef struct SyLetterboxSizedDesc {
 } SyLetterboxSizedDesc;
 int sy_letterbox_sized(const SyLetterboxSizedDesc* d, sy_stream_t stream);
 
+/* ---- Raw camera frames ----
+ * YUV frames of camera streams of different sizes -> uint8 BGR frames at the top-left of slots of one size (the slots
+ * sy_jpeg_decode_sized writes and sy_letterbox_sized reads), bit-identical to cv2.cvtColor with the code named beside each
+ * format.  OpenCV's BT.601 limited-range fixed point: y = max(Y - 16, 0) * 1220542, u = U - 128, v = V - 128,
+ * B = clip((y + 2116026 u + 2^19) >> 20), G = clip((y - 852492 v - 409993 u + 2^19) >> 20), R = clip((y + 1673527 v + 2^19)
+ * >> 20); every pixel of a 2x2 (4:2:0) or 2x1 (4:2:2) group takes the group's chroma sample (replicated, not interpolated).
+ * Frame i is the first h * w * 3 / 2 (4:2:0) or h * w * 2 (4:2:2) bytes of row i of src, laid out as cv2 takes it: */
+enum {
+  SY_YUV_NV12 = 0,   /* COLOR_YUV2BGR_NV12: Y plane [h][w], then interleaved U, V [h / 2][w / 2][2] */
+  SY_YUV_NV21 = 1,   /* COLOR_YUV2BGR_NV21: Y plane, then interleaved V, U */
+  SY_YUV_I420 = 2,   /* COLOR_YUV2BGR_I420: Y plane, U plane [h / 2][w / 2], V plane [h / 2][w / 2] */
+  SY_YUV_YV12 = 3,   /* COLOR_YUV2BGR_YV12: Y plane, V plane, U plane */
+  SY_YUV_YUY2 = 4,   /* COLOR_YUV2BGR_YUY2 (YUYV): [h][w / 2] groups Y0 U Y1 V */
+  SY_YUV_UYVY = 5    /* COLOR_YUV2BGR_UYVY: [h][w / 2] groups U Y0 V Y1 */
+};
+/* sizes[i] = (h, w) of frame i.  A row with h = 0 means no frame this tick, and a row that is odd where the format
+ * subsamples (4:2:0: h or w; 4:2:2: w), does not fit the slot, or whose frame is longer than max_bytes, also leaves slot i
+ * untouched.  Reads no byte of row i past frame i's own bytes, only device memory; never synchronises (capturable). */
+typedef struct SyYuvToBgrSizedDesc {
+  const uint8_t* src;      /* [n][max_bytes] */
+  int32_t n;
+  int64_t max_bytes;       /* row pitch of src */
+  const int32_t* sizes;    /* [n][2] device int32: h, w */
+  int32_t format;          /* SY_YUV_* */
+  int32_t slot_h, slot_w;
+  uint8_t* out;            /* [n][slot_h][slot_w][3] BGR */
+} SyYuvToBgrSizedDesc;
+int sy_yuv_to_bgr_sized(const SyYuvToBgrSizedDesc* d, sy_stream_t stream);
+
 /* ---- JPEG decode ----
  * Batched decode of the training frames' JPEG files into what cv2.imread(path) returns for them (uint8 BGR, bit-identical),
  * replacing the host decodes of exps/dataset/tal_flip_one_future_argoversedataset.py:195,216,

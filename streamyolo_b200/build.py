@@ -33,6 +33,7 @@ SOURCES = {
     "input.cu": ["-fmad=false"],
     "forecast.cu": ["-fmad=false"],
     "jpeg.cu": [],
+    "yuv.cu": [],
 }
 
 

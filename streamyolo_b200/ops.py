@@ -152,6 +152,11 @@ class SyLetterboxSizedDesc(C.Structure):
                 ("sizes", C.c_void_p), ("out_h", C.c_int32), ("out_w", C.c_int32), ("out", C.c_void_p)]
 
 
+class SyYuvToBgrSizedDesc(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("n", C.c_int32), ("max_bytes", C.c_int64), ("sizes", C.c_void_p),
+                ("format", C.c_int32), ("slot_h", C.c_int32), ("slot_w", C.c_int32), ("out", C.c_void_p)]
+
+
 class SySelectImagesDesc(C.Structure):
     _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
 
@@ -263,6 +268,7 @@ _SIG = {
     "sy_jpeg_decode": (C.c_int, [C.POINTER(SyJpegDecodeDesc), C.c_void_p]),
     "sy_jpeg_decode_sized_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
     "sy_jpeg_decode_sized": (C.c_int, [C.POINTER(SyJpegDecodeSizedDesc), C.c_void_p]),
+    "sy_yuv_to_bgr_sized": (C.c_int, [C.POINTER(SyYuvToBgrSizedDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
 
@@ -1142,3 +1148,24 @@ def jpeg_decode_sized(streams, lengths, sizes, out, status, workspace):
     d = SyJpegDecodeSizedDesc(streams.data_ptr(), lengths.data_ptr(), n, max_bytes, sizes.data_ptr(), out.shape[1],
                               out.shape[2], out.data_ptr(), status.data_ptr(), workspace.data_ptr(), workspace.numel())
     _check(lib().sy_jpeg_decode_sized(C.byref(d), _stream()), kernels=5)
+
+
+# frame_format -> SY_YUV_* of sy_yuv_to_bgr_sized (each the cv2.cvtColor code it replaces: COLOR_YUV2BGR_NV12, ...)
+YUV_FORMATS = {"nv12": 0, "nv21": 1, "i420": 2, "yv12": 3, "yuyv": 4, "uyvy": 5}
+
+
+def yuv_to_bgr_sized(src, sizes, fmt, out):
+    """Raw YUV frames -> uint8 BGR slots (sy_yuv_to_bgr_sized), cv2.cvtColor(COLOR_YUV2BGR_*) bit for bit: ``src`` uint8
+    [n, max_bytes], frame i in the first bytes of row i in cv2's layout of ``fmt`` (a YUV_FORMATS key); ``sizes`` int32
+    [n, 2] (h, w), h = 0 for no frame; ``out`` uint8 [n, slot_h, slot_w, 3], frame i at the top-left of slot i.  A row
+    with no frame, an odd size where the format subsamples, or a frame that does not fit leaves its slot untouched."""
+    _require(fmt in YUV_FORMATS, f"yuv_to_bgr_sized: unknown format {fmt!r} (one of {', '.join(YUV_FORMATS)})")
+    _require(_tensor_ok(src, torch.uint8, 2) and src.is_cuda, "yuv_to_bgr_sized: src must be contiguous CUDA uint8 [n, max_bytes]")
+    n, max_bytes = src.shape
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 2) and sizes.device == src.device,
+             f"yuv_to_bgr_sized: sizes must be int32 [{n}, 2] on src's device")
+    _require(_tensor_ok(out, torch.uint8, 4) and out.shape[0] == n and out.shape[3] == 3 and out.device == src.device,
+             f"yuv_to_bgr_sized: out must be contiguous uint8 [{n}, slot_h, slot_w, 3] on src's device")
+    d = SyYuvToBgrSizedDesc(src.data_ptr(), n, max_bytes, sizes.data_ptr(), YUV_FORMATS[fmt], out.shape[1], out.shape[2],
+                            out.data_ptr())
+    _check(lib().sy_yuv_to_bgr_sized(C.byref(d), _stream()))

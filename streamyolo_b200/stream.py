@@ -25,6 +25,14 @@ Then the tick starts with the decode of the S files (sy_jpeg_decode_sized) into 
 frame did not decode, or that got none, keeps its carried features, starts no sequence and returns no detections
 (sy_stream_gate, sy_stream_rescale): all decided on the device, still one replay and one synchronisation per tick.
 
+Raw camera frames (YUV, as ISPs, hardware codecs, V4L2 and GMSL deliver them):
+
+    det = StreamDetector(model, frame_sizes=[(1200, 1920), (1080, 1920)], input_size=(600, 960), frame_format="nv12")
+    det.step([nv12_0, nv12_1])                    # uint8 [h * 3 // 2, w] each, what cv2.cvtColor(COLOR_YUV2BGR_NV12) takes
+
+Then the tick starts with the conversion of the S frames to BGR (sy_yuv_to_bgr_sized, cv2.cvtColor bit for bit) into the
+slots; only each frame's own bytes cross to the device.
+
 The graph reads the weights and the folded BatchNorm as they were at capture: after ``load_state_dict`` (or any other
 change of the weights or running statistics) call ``capture()`` again.  Nothing checks this per frame.
 """
@@ -45,10 +53,12 @@ class StreamTick:
     ``lengths`` (int32 [S], 0 = no frame) instead of ``frames``, decoded inside the tick into ``frames`` with a per-stream
     ``status``.  ``raw`` ([S, A, 5 + nc] head outputs), ``det`` ([S, A, 7] rows x1, y1, x2, y2 -- divided by the stream's
     ratio --, obj, class_conf, class_pred) and ``count`` ([S] rows of ``det``) are the outputs; ``buffer`` holds each
-    stream's features carried to the next tick."""
+    stream's features carried to the next tick.  With a YUV ``frame_format`` (an ops.YUV_FORMATS key) the input is ``yuv``
+    (uint8 [S, max_bytes], stream i's frame in cv2's layout in the first bytes of row i), converted inside the tick into
+    ``frames``."""
 
     def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None,
-                 forecast=None, clear_on_empty=False, queries=0):
+                 forecast=None, clear_on_empty=False, queries=0, frame_format="bgr"):
         self.model, self.size = model, tuple(size)
         self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
         table = np.asarray(table, np.int32)
@@ -64,6 +74,12 @@ class StreamTick:
         self.buffer = None
         self.raw = self.det = self.count = None
         self.status = None
+        self.yuv = None
+        if frame_format != "bgr":
+            self.yuv_format = frame_format
+            self.yuv = torch.zeros((streams, max(int(np.prod(frame_shape(frame_format, h, w))) for h, w in table[:, :2])),
+                                   dtype=torch.uint8, device=device)
+            self.yuv_sizes = self.table[:, :2].contiguous()
         # forecast = (match_iou_th, max_tracks): the tick ends with the tracks' update from its detections, each stream
         # gated by start / keep; fc_dt (int32 [S], set by the host) is the frames since the stream's previous update
         self.fc = self.fc_dt = None
@@ -92,6 +108,8 @@ class StreamTick:
         ctx, net, head = self.ctx, self.model.backbone, self.model.head
         if self.status is not None:
             ops.jpeg_decode_sized(self.bytes, self.lengths, self.sizes, self.frames, self.status, self.workspace)
+        if self.yuv is not None:
+            ops.yuv_to_bgr_sized(self.yuv, self.yuv_sizes, self.yuv_format, self.frames)
         ops.stream_gate(self.status, self.flags, self.start, self.keep)
         ops.letterbox_sized(self.frames, self.table, self.x)
         with torch.no_grad(), engine.forward_scope(ctx.device):
@@ -162,14 +180,26 @@ def sized_output(det):
     return det[:, :4].copy(), det[:, 4] * det[:, 5], det[:, 6].astype(np.int32)
 
 
-def step_frames(frames, streams, frame_hw):
-    """``frames`` (numpy, CPU or CUDA tensor) as a uint8 [S, h, w, 3] tensor, or RuntimeError; [h, w, 3] for one stream."""
-    s, (h, w) = streams, frame_hw
+FRAME_FORMATS = ("bgr",) + tuple(ops.YUV_FORMATS)
+
+
+def frame_shape(fmt, h, w):
+    """the uint8 array ``step`` takes for one h x w frame of ``fmt`` (a FRAME_FORMATS entry), in cv2's layout"""
+    if fmt == "bgr":
+        return h, w, 3
+    return (h * 3 // 2, w) if fmt in ("nv12", "nv21", "i420", "yv12") else (h, w, 2)
+
+
+def step_frames(frames, streams, frame_hw, fmt="bgr"):
+    """``frames`` (numpy, CPU or CUDA tensor) as a uint8 [S, *frame_shape] tensor, or RuntimeError; [*frame_shape] for
+    one stream."""
+    s, shape = streams, frame_shape(fmt, *frame_hw)
     src = frames if torch.is_tensor(frames) else torch.from_numpy(np.ascontiguousarray(frames))
-    ops._require(src.dtype == torch.uint8 and (tuple(src.shape) == (s, h, w, 3) or (s == 1 and tuple(src.shape) == (h, w, 3))),
-                 f"StreamDetector.step: frames must be uint8 [{s}, {h}, {w}, 3]" + (f" or [{h}, {w}, 3]" if s == 1 else "")
+    one = ", ".join(str(v) for v in shape)
+    ops._require(src.dtype == torch.uint8 and (tuple(src.shape) == (s, *shape) or (s == 1 and tuple(src.shape) == shape)),
+                 f"StreamDetector.step: frames must be uint8 [{s}, {one}]" + (f" or [{one}]" if s == 1 else "")
                  + f", not {src.dtype} {list(src.shape)}")
-    return src.reshape(s, h, w, 3)
+    return src.reshape(s, *shape)
 
 
 class StreamDetector:
@@ -195,6 +225,12 @@ class StreamDetector:
       match_iou_th    the association's IoU threshold (inclusive)
       max_tracks      the most detections one stream's update takes; a tick with more raises RuntimeError naming the
                       stream, whose tracks are then left as they were
+    Raw camera frames:
+      frame_format    "bgr" (the default): ``step`` and ``submit`` take uint8 BGR [h, w, 3] frames.  "nv12", "nv21",
+                      "i420", "yv12" (4:2:0: uint8 [h * 3 // 2, w], even h and w) or "yuyv", "uyvy" (4:2:2: uint8
+                      [h, w, 2], even w): they take the camera's frames in cv2's layout, and the replay starts with their
+                      conversion to BGR (sy_yuv_to_bgr_sized, cv2.cvtColor(COLOR_YUV2BGR_NV12, _NV21, _I420, _YV12,
+                      _YUY2, _UYVY) bit for bit).  Not with ``jpeg_max_bytes``
     The sAP toolkit's streamer (sAP/forecast/streamer.py, see streamyolo_b200.streamer), with ``forecast=True``:
       clear_on_empty  True: an empty detection leaves the stream without tracks, as the streamer's association does
                       (the default keeps the predicted tracks, as pps_forecast_kf.py does)
@@ -209,7 +245,7 @@ class StreamDetector:
 
     def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
                  frame_sizes=None, input_size=None, jpeg_max_bytes=None, forecast=False, match_iou_th=0.3,
-                 max_tracks=1024, clear_on_empty=False, queries=0):
+                 max_tracks=1024, clear_on_empty=False, queries=0, frame_format="bgr"):
         if model.training:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
@@ -228,6 +264,17 @@ class StreamDetector:
             raise ValueError(f"StreamDetector: frames {sizes} at in_scale {in_scale} give input size {size}")
         if jpeg_max_bytes is not None:
             jpeg_max_bytes = feed.check_max_bytes(jpeg_max_bytes, "StreamDetector: jpeg_max_bytes")
+        if frame_format not in FRAME_FORMATS:
+            raise ValueError(f"StreamDetector: unknown frame_format {frame_format!r} (one of {', '.join(FRAME_FORMATS)})")
+        if frame_format != "bgr":
+            if jpeg_max_bytes is not None:
+                raise ValueError(f"StreamDetector: frame_format {frame_format!r} takes raw frames, jpeg_max_bytes JPEG "
+                                 "files: give one or the other")
+            sub420 = len(frame_shape(frame_format, 2, 2)) == 2
+            odd = [s for s in sizes if s[1] % 2 or (sub420 and s[0] % 2)]
+            if odd:
+                raise ValueError(f"StreamDetector: {frame_format} frames need an even width"
+                                 + (" and height" if sub420 else "") + f", as cv2 requires; not {odd[0]}")
         if forecast and (int(max_tracks) != max_tracks or not 1 <= max_tracks <= 1 << 20):
             raise ValueError(f"StreamDetector: max_tracks must be an integer in [1, 2^20], not {max_tracks}")
         if int(queries) != queries or not 0 <= queries <= 65535:
@@ -243,10 +290,12 @@ class StreamDetector:
         self.model, self.streams, self.in_scale, self.size = model, streams, in_scale, size
         self.frame_sizes, self.ratios = sizes, ratios
         self.jpeg_max_bytes = jpeg_max_bytes
+        self.frame_format = frame_format
         self.forecasting = bool(forecast)
         self.queries = int(queries)
         self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes,
-                                (match_iou_th, int(max_tracks)) if forecast else None, clear_on_empty, self.queries)
+                                (match_iou_th, int(max_tracks)) if forecast else None, clear_on_empty, self.queries,
+                                frame_format)
         if self.forecasting:
             self._fc_dt = feed.pinned((streams,), torch.int32)
             self._fc_meta = feed.pinned((streams, 4), torch.int32)
@@ -260,8 +309,8 @@ class StreamDetector:
         self._pub = None                          # publish / query: the published tracks, their stream and events
         self._inflight = None
         self.frame_hw = tuple(self._tick.frames.shape[1:3])          # the slot: the largest height and width
-        if self.jpeg_max_bytes is None:           # stream i's frame is staged at the start of slot i (see step)
-            self._stage = feed.pinned(tuple(self._tick.frames.shape), torch.uint8)
+        if self.jpeg_max_bytes is None:
+            self._inputs()
         else:
             self._jstage = feed.pinned((streams, self.jpeg_max_bytes), torch.uint8)
             self._jlen = feed.pinned((streams,), torch.int32)
@@ -311,8 +360,16 @@ class StreamDetector:
         self._queries_in(query_dt, "step")
         return self._run(None, fidx)
 
+    def _inputs(self):
+        """the tick's buffer ``step`` copies the frames to (``frames``, or ``yuv`` for a YUV frame_format), each stream's
+        frame shape in it and the pinned stage (stream i's frame staged at the start of row i)"""
+        t = self._tick
+        self._in = t.frames if t.yuv is None else t.yuv
+        self._shapes = [frame_shape(self.frame_format, h, w) for h, w in self.frame_sizes]
+        self._stage = feed.pinned(tuple(self._in.shape), torch.uint8)
+
     def _stage_frames(self, frames, what):
-        """``frames`` of ``step`` copied (asynchronously) into the tick's frame slots"""
+        """``frames`` of ``step`` copied (asynchronously) into the tick's input buffer"""
         t = self._tick
         if self.jpeg_max_bytes is not None:
             raise RuntimeError(f"StreamDetector.{what}: this detector was built with jpeg_max_bytes, and its replay decodes "
@@ -320,25 +377,30 @@ class StreamDetector:
                                "frames)")
         if isinstance(frames, (list, tuple)):
             ops._require(len(frames) == self.streams, f"StreamDetector.step: give a list of {self.streams} frames, one per stream")
-            for i, (f, (h, w)) in enumerate(zip(frames, self.frame_sizes)):
+            for i, (f, shape, (h, w)) in enumerate(zip(frames, self._shapes, self.frame_sizes)):
+                ops._require(f is not None, f"StreamDetector.step: frame {i} is None: every stream takes a frame per tick")
                 src = f if torch.is_tensor(f) else torch.from_numpy(np.ascontiguousarray(f))
-                ops._require(src.dtype == torch.uint8 and tuple(src.shape) == (h, w, 3),
-                             f"StreamDetector.step: frame {i} must be uint8 [{h}, {w}, 3], not {src.dtype} {list(src.shape)}")
+                ops._require(src.dtype == torch.uint8 and tuple(src.shape) == shape, f"StreamDetector.step: frame {i} must "
+                             f"be uint8 {list(shape)}, not {src.dtype} {list(src.shape)}")
+                n = src.numel()
+                dst = t.frames[i, :h, :w] if t.yuv is None else t.yuv[i, :n].view(shape)
                 if src.is_cuda:
-                    t.frames[i, :h, :w].copy_(src)
-                else:                                 # only the frame's h x w pixels cross, not the whole slot
-                    stage = self._stage[i].view(-1)[:h * w * 3].view(h, w, 3)
+                    dst.copy_(src)
+                else:                                 # only the frame's own bytes cross, not the whole slot
+                    stage = self._stage[i].view(-1)[:n].view(shape)
                     stage.copy_(src)
-                    t.frames[i, :h, :w].copy_(stage, non_blocking=True)
+                    dst.copy_(stage, non_blocking=True)
         else:
             ops._require(all(s == self.frame_hw for s in self.frame_sizes),
                          f"StreamDetector.step: give a list of {self.streams} frames, one per stream")
-            src = step_frames(frames, self.streams, self.frame_hw)
+            src = step_frames(frames, self.streams, self.frame_hw, self.frame_format)
+            dst = self._in.view(src.shape)            # one size: each slot holds exactly one frame
             if src.is_cuda:
-                t.frames.copy_(src)
+                dst.copy_(src)
             else:
-                self._stage.copy_(src)
-                t.frames.copy_(self._stage, non_blocking=True)
+                stage = self._stage.view(src.shape)
+                stage.copy_(src)
+                dst.copy_(stage, non_blocking=True)
 
     def last_raw(self):
         """A device copy of the last tick's head outputs [S, A, 5 + nc] (what the driver keeps as ``results_raw``)."""
