@@ -730,6 +730,43 @@ typedef struct SyJpegDecodeSizedDesc {
 size_t sy_jpeg_decode_sized_workspace_bytes(int32_t n, int64_t max_bytes, int32_t max_h, int32_t max_w);
 int sy_jpeg_decode_sized(const SyJpegDecodeSizedDesc* d, sy_stream_t stream);
 
+/* ---- JPEG encode ----
+ * Batched encode of uint8 BGR images of their own sizes into the bytes cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY,
+ * quality]) returns for them, with cv2's other defaults (replacing the host cv2.imwrite of recorded camera frames):
+ * baseline SOF0, YCbCr 4:2:0, libjpeg's quality-scaled Annex K tables, the standard Huffman tables, no restart interval,
+ * JFIF 1.01 APP0 with density 1:1; segments SOI APP0 DQT DQT SOF0 DHT x 4 SOS, the scan, EOI.  Image i is sizes[i] =
+ * (h, w) at the top-left of slot i of src [n][max_h][max_w][3] (the slots sy_jpeg_decode_sized and sy_yuv_to_bgr_sized
+ * write); its file goes to the first lengths[i] bytes of row i of out.  Per image status: */
+enum {
+  SY_JPEG_ENCODE_OK = 0,
+  SY_JPEG_ENCODE_EOVERFLOW = 1,   /* the file does not fit in max_bytes: lengths[i] = 0, nothing written past max_bytes */
+  SY_JPEG_ENCODE_ESIZE = 2        /* sizes[i] has h or w below 1 or outside the slot: lengths[i] = 0, row i untouched */
+};
+/* The sizes are read on the device only, so a captured graph follows sizes written before each replay.  Never
+ * synchronises (capturable).  SY_EINVAL: quality outside 1..100, a slot or max_bytes outside the limits of
+ * sy_jpeg_encode_workspace_bytes, a null or misaligned pointer, or a short workspace. */
+typedef struct SyJpegEncodeDesc {
+  const uint8_t* src;       /* [n][max_h][max_w][3] BGR */
+  const int32_t* sizes;     /* [n][2] device int32: h, w (4-byte aligned) */
+  int32_t n;
+  int32_t max_h, max_w;     /* slot size */
+  int32_t quality;          /* 1..100 */
+  uint8_t* out;             /* [n][max_bytes] */
+  int64_t max_bytes;        /* row pitch of out (1 .. 2^31) */
+  int64_t* lengths;         /* [n] device int64 (8-byte aligned): the file's length, 0 where status != OK */
+  int32_t* status;          /* [n] device int32 (4-byte aligned), SY_JPEG_ENCODE_* */
+  void* workspace;          /* sy_jpeg_encode_workspace_bytes(n, max_h, max_w, max_bytes) bytes, 256-byte aligned */
+  size_t workspace_bytes;
+} SyJpegEncodeDesc;
+/* 0 for n outside 1..65535, a slot side outside 1..65535, max_bytes outside 1..2^31, or a slot of 2^32 / 1660 blocks or
+ * more */
+size_t sy_jpeg_encode_workspace_bytes(int32_t n, int32_t max_h, int32_t max_w, int64_t max_bytes);
+/* A length no h x w file exceeds, whatever its content and quality: 623 header bytes, EOI, and every one of the
+ * 6 * ceil(h / 16) * ceil(w / 16) blocks at 1660 bits (the longest DC code and its 11 bits, then 63 AC coefficients of
+ * the longest AC code and 10 bits each), every scan byte followed by a stuffed 00.  0 for a side outside 1..65535. */
+int64_t sy_jpeg_encode_max_bytes(int32_t h, int32_t w);
+int sy_jpeg_encode(const SyJpegEncodeDesc* d, sy_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -34,6 +34,7 @@ SOURCES = {
     "forecast.cu": ["-fmad=false"],
     "jpeg.cu": [],
     "yuv.cu": [],
+    "jpeg_encode.cu": [],
 }
 
 

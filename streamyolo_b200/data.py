@@ -7,6 +7,8 @@ driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60, 176-181), ``stream_fra
 different sizes (the evaluation preproc, data_augment_flip.py:151-167, per frame).  They are bit-identical to the cv2 / numpy host code
 they replace (sy_pair_labels, sy_frame_labels, sy_letterbox); INTEGRATION.md shows where they plug in.
 """
+import operator
+
 import numpy as np
 import torch
 
@@ -286,3 +288,95 @@ def decode_jpeg_sized(streams, lengths, sizes, max_hw, out=None, status=None, wo
         workspace = _JPEG_WS[key]
     ops.jpeg_decode_sized(streams, lengths, sizes, out, status, workspace)
     return out, status
+
+
+# per-image status of encode_jpeg (SY_JPEG_ENCODE_* of include/streamyolo_sm100.h)
+ENCODE_STATUS = {0: "ok", 1: "the file does not fit in max_bytes", 2: "its size is outside the slot"}
+_ENC_WS = {}
+
+
+def encode_jpeg(frames, quality=95, sizes=None, max_bytes=None, out=None, workspace=None):
+    """Encode uint8 BGR frames on the device into the files cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY,
+    quality]) returns, byte for byte (sy_jpeg_encode: baseline, 4:2:0, standard Huffman tables, JFIF), which
+    cv2.imwrite(path, frame, ...) would write.
+
+    frames    uint8 CUDA [n, h, w, 3]; or slots [n, max_h, max_w, 3] (decode_jpeg_sized's or the streaming detector's
+              ``frames``) with ``sizes``
+    sizes     each frame's (h, w) at the top-left of its slot: host pairs (checked here) or an int32 CUDA [n, 2] tensor
+              (read on the device only, static for CUDA-graph capture)
+    max_bytes the longest file to make room for (the row length of the output); default ``ops.jpeg_encode_max_bytes``
+              of the slot, which no frame of the slot's size exceeds
+    out       ``(buf, lengths, status)``: uint8 [n, max_bytes], int64 [n] and int32 [n] device buffers to write into.  The
+              call then only enqueues the encode (capturable) and returns ``out``; ``jpeg_files(*out)`` reads them back
+    workspace the uint8 workspace (ops.jpeg_encode_workspace_bytes) to use; cached per device and shape when omitted
+
+    -> a list of n ``bytes``, the files (one synchronisation).  A file longer than ``max_bytes`` raises ValueError
+    naming the frame."""
+    ops._require(torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+                 and frames.is_contiguous() and frames.is_cuda,
+                 "encode_jpeg: frames must be a contiguous CUDA uint8 [n, h, w, 3] tensor")
+    try:
+        quality = operator.index(quality)
+    except TypeError:
+        raise RuntimeError(f"encode_jpeg: quality must be an integer in 1..100, not {quality!r}") from None
+    ops._require(1 <= quality <= 100, f"encode_jpeg: quality must be an integer in 1..100, not {quality}")
+    n, mh, mw, _ = frames.shape
+    dev = frames.device
+    if sizes is None:
+        sizes = [(mh, mw)] * n
+    if not torch.is_tensor(sizes):
+        hw = _sizes_list(sizes, "encode_jpeg")
+        ops._require(len(hw) == n, f"encode_jpeg: {len(hw)} sizes for {n} frames")
+        for i, (h, w) in enumerate(hw):
+            ops._require(h <= mh and w <= mw, f"encode_jpeg: frame {i} of {h}x{w} is larger than the {mh}x{mw} slot")
+        sizes = torch.tensor(hw, dtype=torch.int32)
+    ops._require(sizes.dtype == torch.int32 and tuple(sizes.shape) == (n, 2), f"encode_jpeg: sizes must be int32 [{n}, 2]")
+    sizes = sizes.to(dev).contiguous()
+    if out is None:
+        if max_bytes is None:
+            max_bytes = ops.jpeg_encode_max_bytes(mh, mw)
+        buf = torch.empty((n, int(max_bytes)), dtype=torch.uint8, device=dev)
+        lengths = torch.empty((n,), dtype=torch.int64, device=dev)
+        status = torch.empty((n,), dtype=torch.int32, device=dev)
+    else:
+        buf, lengths, status = out
+        ops._require(torch.is_tensor(buf) and buf.dim() == 2 and (max_bytes is None or buf.shape[1] == max_bytes),
+                     "encode_jpeg: out's buffer must be uint8 [n, max_bytes]")
+    if workspace is None:
+        key = (dev, n, mh, mw, buf.shape[1])
+        if key not in _ENC_WS:
+            _ENC_WS[key] = torch.empty(ops.jpeg_encode_workspace_bytes(n, mh, mw, buf.shape[1]), dtype=torch.uint8,
+                                       device=dev)
+        workspace = _ENC_WS[key]
+    ops.jpeg_encode(frames, sizes, quality, buf, lengths, status, workspace)
+    if out is not None:
+        return out
+    return jpeg_files(buf, lengths, status)
+
+
+def jpeg_files(buf, lengths, status, present=None, stage=None):
+    """encode_jpeg's output -> a list of ``bytes``: exactly each file's length is copied back, with one synchronisation.
+    ``lengths`` / ``status`` may already be on the host; ``present``: which rows to read (None for the others, whose status
+    is not checked); ``stage``: a page-locked uint8 host tensor of at least the files' total length to copy through (a new
+    one otherwise).  A file that did not fit raises ValueError naming its frame."""
+    n = buf.shape[0]
+    present = [True] * n if present is None else [bool(p) for p in present]
+    st, ln = status.cpu().tolist(), lengths.cpu().tolist()
+    for i in range(n):
+        if present[i] and st[i] != 0:
+            raise ValueError(f"encode_jpeg: frame {i} was not encoded: {ENCODE_STATUS.get(st[i], f'status {st[i]}')}"
+                             + (f" (max_bytes = {buf.shape[1]})" if st[i] == 1 else ""))
+    total = sum(l for l, p in zip(ln, present) if p)
+    if stage is None or stage.numel() < total:
+        stage = torch.empty((max(total, 1),), dtype=torch.uint8, pin_memory=True)
+    spans, at = [], 0
+    for i in range(n):
+        if not present[i]:
+            spans.append(None)
+            continue
+        stage[at:at + ln[i]].copy_(buf[i, :ln[i]], non_blocking=True)
+        spans.append((at, at + ln[i]))
+        at += ln[i]
+    torch.cuda.current_stream(buf.device).synchronize()
+    host = stage.numpy()
+    return [None if sp is None else host[sp[0]:sp[1]].tobytes() for sp in spans]

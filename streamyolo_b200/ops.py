@@ -157,6 +157,12 @@ class SyYuvToBgrSizedDesc(C.Structure):
                 ("format", C.c_int32), ("slot_h", C.c_int32), ("slot_w", C.c_int32), ("out", C.c_void_p)]
 
 
+class SyJpegEncodeDesc(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("sizes", C.c_void_p), ("n", C.c_int32), ("max_h", C.c_int32), ("max_w", C.c_int32),
+                ("quality", C.c_int32), ("out", C.c_void_p), ("max_bytes", C.c_int64), ("lengths", C.c_void_p),
+                ("status", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
+
+
 class SySelectImagesDesc(C.Structure):
     _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
 
@@ -269,6 +275,9 @@ _SIG = {
     "sy_jpeg_decode_sized_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
     "sy_jpeg_decode_sized": (C.c_int, [C.POINTER(SyJpegDecodeSizedDesc), C.c_void_p]),
     "sy_yuv_to_bgr_sized": (C.c_int, [C.POINTER(SyYuvToBgrSizedDesc), C.c_void_p]),
+    "sy_jpeg_encode_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int64]),
+    "sy_jpeg_encode_max_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
+    "sy_jpeg_encode": (C.c_int, [C.POINTER(SyJpegEncodeDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
 
@@ -1169,3 +1178,45 @@ def yuv_to_bgr_sized(src, sizes, fmt, out):
     d = SyYuvToBgrSizedDesc(src.data_ptr(), n, max_bytes, sizes.data_ptr(), YUV_FORMATS[fmt], out.shape[1], out.shape[2],
                             out.data_ptr())
     _check(lib().sy_yuv_to_bgr_sized(C.byref(d), _stream()))
+
+
+def jpeg_encode_max_bytes(h, w):
+    """a file length no h x w JPEG of sy_jpeg_encode exceeds, for any content and quality"""
+    need = load_library().sy_jpeg_encode_max_bytes(h, w)
+    _require(need > 0, f"jpeg_encode_max_bytes: bad size {h}x{w}")
+    return need
+
+
+def jpeg_encode_workspace_bytes(n, max_h, max_w, max_bytes):
+    """bytes of the sy_jpeg_encode workspace for n images in slots of max_h x max_w and files of at most max_bytes"""
+    need = load_library().sy_jpeg_encode_workspace_bytes(n, max_h, max_w, max_bytes)
+    _require(need > 0, f"jpeg_encode: bad sizes (n {n}, slot {max_h}x{max_w}, max_bytes {max_bytes})")
+    return need
+
+
+def jpeg_encode(src, sizes, quality, out, lengths, status, workspace):
+    """Encode n BGR images of their own sizes into what cv2.imencode(".jpg", img, [IMWRITE_JPEG_QUALITY, quality])
+    returns (sy_jpeg_encode): ``src`` uint8 [n, max_h, max_w, 3], image i at the top-left of slot i; ``sizes`` int32
+    [n, 2] (h, w) on the device; ``out`` uint8 [n, max_bytes], file i in the first ``lengths[i]`` bytes of row i;
+    ``lengths`` int64 [n]; ``status`` int32 [n] (0 ok, 1 the file does not fit in max_bytes, 2 a size row outside the
+    slot); ``workspace`` uint8 of jpeg_encode_workspace_bytes.  Enqueues only (capturable)."""
+    _require(isinstance(quality, int) and 1 <= quality <= 100,
+             f"jpeg_encode: quality must be an integer in 1..100, not {quality!r}")
+    _require(_tensor_ok(src, torch.uint8, 4) and src.shape[3] == 3 and src.is_cuda,
+             "jpeg_encode: src must be contiguous CUDA uint8 [n, max_h, max_w, 3]")
+    n, mh, mw, _ = src.shape
+    dev = src.device
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 2) and sizes.device == dev,
+             f"jpeg_encode: sizes must be int32 [{n}, 2] on src's device")
+    _require(_tensor_ok(out, torch.uint8, 2) and out.shape[0] == n and out.device == dev,
+             f"jpeg_encode: out must be contiguous uint8 [{n}, max_bytes] on src's device")
+    _require(_tensor_ok(lengths, torch.int64, 1) and lengths.shape[0] == n and lengths.device == dev,
+             f"jpeg_encode: lengths must be int64 [{n}] on src's device")
+    _require(_tensor_ok(status, torch.int32, 1) and status.shape[0] == n and status.device == dev,
+             f"jpeg_encode: status must be int32 [{n}] on src's device")
+    need = jpeg_encode_workspace_bytes(n, mh, mw, out.shape[1])
+    _require(_tensor_ok(workspace, torch.uint8, 1) and workspace.numel() >= need and workspace.device == dev,
+             f"jpeg_encode: workspace must be contiguous uint8 of at least {need} bytes on src's device")
+    d = SyJpegEncodeDesc(src.data_ptr(), sizes.data_ptr(), n, mh, mw, int(quality), out.data_ptr(), out.shape[1],
+                         lengths.data_ptr(), status.data_ptr(), workspace.data_ptr(), workspace.numel())
+    _check(lib().sy_jpeg_encode(C.byref(d), _stream()), kernels=8)

@@ -55,10 +55,11 @@ class StreamTick:
     ratio --, obj, class_conf, class_pred) and ``count`` ([S] rows of ``det``) are the outputs; ``buffer`` holds each
     stream's features carried to the next tick.  With a YUV ``frame_format`` (an ops.YUV_FORMATS key) the input is ``yuv``
     (uint8 [S, max_bytes], stream i's frame in cv2's layout in the first bytes of row i), converted inside the tick into
-    ``frames``."""
+    ``frames``.  With ``record_quality`` the tick ends with the JPEG encode of the frames in ``frames`` (``rec_out``,
+    ``rec_len``, ``rec_status``)."""
 
     def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None,
-                 forecast=None, clear_on_empty=False, queries=0, frame_format="bgr"):
+                 forecast=None, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None):
         self.model, self.size = model, tuple(size)
         self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
         table = np.asarray(table, np.int32)
@@ -103,6 +104,17 @@ class StreamTick:
             self.sizes = self.table[:, :2].contiguous()
             self.workspace = torch.empty(ops.jpeg_decode_sized_workspace_bytes(streams, jpeg_max_bytes, *slot),
                                          dtype=torch.uint8, device=device)
+        # record_quality: the tick ends with the JPEG encode of every slot's frame (sy_jpeg_encode) into rec_out, file i
+        # in the first rec_len[i] bytes of row i, rec_status[i] its SY_JPEG_ENCODE_* status
+        self.rec_q = record_quality
+        if record_quality is not None:
+            rec_bytes = ops.jpeg_encode_max_bytes(*slot)
+            self.rec_sizes = self.table[:, :2].contiguous()
+            self.rec_out = torch.zeros((streams, rec_bytes), dtype=torch.uint8, device=device)
+            self.rec_len = torch.zeros((streams,), dtype=torch.int64, device=device)
+            self.rec_status = torch.zeros((streams,), dtype=torch.int32, device=device)
+            self.rec_ws = torch.empty(ops.jpeg_encode_workspace_bytes(streams, *slot, rec_bytes), dtype=torch.uint8,
+                                      device=device)
 
     def run(self):
         ctx, net, head = self.ctx, self.model.backbone, self.model.head
@@ -128,6 +140,9 @@ class StreamTick:
                                     clear_on_empty=self.fc_clear)
             if self.fc_q:
                 self.fc_qout = ops.forecast_extrap_queries(self.fc, self.fc_qdt, self.fc_nq, self.fc_wh, self.fc_qout)
+        if self.rec_q is not None:
+            ops.jpeg_encode(self.frames, self.rec_sizes, self.rec_q, self.rec_out, self.rec_len, self.rec_status,
+                            self.rec_ws)
 
 
 NO_FRAME = -1     # last_status() of a stream that was given no frame
@@ -239,13 +254,18 @@ class StreamDetector:
                       with the detections, one synchronisation per tick (``last_queries``)
       ``submit`` / ``poll`` / ``receive`` run a tick without waiting for it, and ``publish`` / ``query`` extrapolate the
       tracks of the last received tick while the next one is in flight (the wall-clock streamer)
+    Recording what the cameras saw:
+      record_quality  None (the default) or a JPEG quality 1..100: the tick ends with the encode of every stream's BGR
+                      frame -- the decoded, converted or given frame the resize reads -- into the file cv2.imencode(".jpg",
+                      frame, [cv2.IMWRITE_JPEG_QUALITY, record_quality]) makes (sy_jpeg_encode), and ``last_jpeg``
+                      reads the files back.  The detections do not change
     Each stream's frame is transformed as data.sized_table says and its boxes divided by its own ratio (``ratios``): a frame
     of driver size ``input_size`` gets the driver's plain resize and ``in_scale``.  ``frame_hw`` is the slot the frames are
     stored in: the largest height and width (the frame size when every stream has one size)."""
 
     def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
                  frame_sizes=None, input_size=None, jpeg_max_bytes=None, forecast=False, match_iou_th=0.3,
-                 max_tracks=1024, clear_on_empty=False, queries=0, frame_format="bgr"):
+                 max_tracks=1024, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None):
         if model.training:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
@@ -281,6 +301,9 @@ class StreamDetector:
             raise ValueError(f"StreamDetector: queries must be an integer in [0, 65535], not {queries}")
         if (clear_on_empty or queries) and not forecast:
             raise ValueError("StreamDetector: clear_on_empty and queries take forecast=True")
+        if record_quality is not None and (isinstance(record_quality, bool) or not isinstance(record_quality, (int, np.integer))
+                                           or not 1 <= record_quality <= 100):
+            raise ValueError(f"StreamDetector: record_quality must be None or an integer in 1..100, not {record_quality!r}")
         try:
             table, ratios = data.sized_table(sizes, size, in_scale)
         except RuntimeError as e:
@@ -295,7 +318,13 @@ class StreamDetector:
         self.queries = int(queries)
         self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes,
                                 (match_iou_th, int(max_tracks)) if forecast else None, clear_on_empty, self.queries,
-                                frame_format)
+                                frame_format, None if record_quality is None else int(record_quality))
+        self.record_quality = None if record_quality is None else int(record_quality)
+        if self.record_quality is not None:
+            self._rec_len = feed.pinned((streams,), torch.int64)
+            self._rec_status = feed.pinned((streams,), torch.int32)
+            self._rec_rows = None                 # the streams the last tick has a file for
+            self._rec_stage = None
         if self.forecasting:
             self._fc_dt = feed.pinned((streams,), torch.int32)
             self._fc_meta = feed.pinned((streams, 4), torch.int32)
@@ -499,6 +528,9 @@ class StreamDetector:
         if self.queries:
             for h, d in zip(self._q_out, t.fc_qout):
                 h.copy_(d, non_blocking=True)
+        if self.record_quality is not None:
+            self._rec_len.copy_(t.rec_len, non_blocking=True)
+            self._rec_status.copy_(t.rec_status, non_blocking=True)
 
     def _finish(self, present, fidx):
         """the host's side of ``_run`` once the tick and its copies are done -> the detections"""
@@ -510,6 +542,8 @@ class StreamDetector:
             self._last_status, nxt = route_status(self._status.numpy(), present, self._flags.numpy())
             updated = (self._last_status == 0).tolist()
             self._flags.copy_(torch.from_numpy(nxt))
+        if self.record_quality is not None:
+            self._rec_rows = list(updated)
         if fidx is not None:
             over = [i for i in range(self.streams) if self._fc_meta[i, 3] != 0]
             if over:
@@ -527,6 +561,21 @@ class StreamDetector:
                               for k, n in enumerate(count[i, :n_q[i]].tolist())] for i in range(self.streams)]
         det = self._det.numpy()
         return [sized_output(det[i, :n]) for i, n in enumerate(self._count.tolist())]
+
+    def last_jpeg(self):
+        """The last tick's frames as JPEG files (a detector built with ``record_quality``): per stream the ``bytes``
+        cv2.imencode(".jpg", frame, [cv2.IMWRITE_JPEG_QUALITY, record_quality]) returns for the BGR frame the tick
+        detected on, or None for a stream without a frame that tick (no file, or one that did not decode).  Copies exactly
+        each file's length back, with one synchronisation; None before the first tick."""
+        if self.record_quality is None:
+            raise RuntimeError("StreamDetector.last_jpeg: build the detector with record_quality")
+        if self._rec_rows is None:
+            return None
+        t = self._tick
+        total = sum(int(l) for l, r in zip(self._rec_len.tolist(), self._rec_rows) if r)
+        if self._rec_stage is None or self._rec_stage.numel() < total:
+            self._rec_stage = feed.pinned((max(2 * total, 1),), torch.uint8)
+        return data.jpeg_files(t.rec_out, self._rec_len, self._rec_status, self._rec_rows, self._rec_stage)
 
     def last_queries(self):
         """The extrapolations of the last ``step`` / ``step_jpeg`` (a detector built with ``queries``): per stream, one
