@@ -767,6 +767,59 @@ size_t sy_jpeg_encode_workspace_bytes(int32_t n, int32_t max_h, int32_t max_w, i
 int64_t sy_jpeg_encode_max_bytes(int32_t h, int32_t w);
 int sy_jpeg_encode(const SyJpegEncodeDesc* d, sy_stream_t stream);
 
+/* ---- detection drawing (the sAP toolkit's visualisation) ----
+ * sy_draw_boxes: the box branch of vis_obj_fancy (sAP/vis/vis_det_th.py:99-120, masks None, no text) on n uint8 images
+ * of their own sizes: image i is sizes[i] = (h, w) at the top-left of slot i of src [n][max_h][max_w][3] and is drawn
+ * into the same place of dst (dst == src draws in place).  With the first counts[i] boxes of row i (x1, y1, x2, y2,
+ * already rounded; corners in either order) and their labels, in list order:
+ *   1. fill (cv2.rectangle(img, ..., thickness=-1) then cv2.addWeighted(img_filled, 0.8, img, 0.2, 0), :101-110): a pixel
+ *      in at least one box's [min(x1,x2), max(x1,x2)] x [min(y1,y2), max(y1,y2)] (inclusive) becomes
+ *      rint(0.8f * v + 0.2f * p) per channel, p the palette colour of the last such box;
+ *   2. contours (cv2.rectangle(img, ..., thickness=2), :112-120): a pixel within Chebyshev distance 1 of at least one
+ *      box's border, except the four pixels diagonally outside its corners, becomes the palette colour of the last such
+ *      box.
+ * The palette is uint8 [P][3] in the images' channel order.  A box whose label is outside [0, P) is not drawn (the host
+ * refuses those); counts are clamped to [0, K]; an image whose size row is below 1 or outside the slot is left alone.
+ * Pixels outside an image and pixels no box touches are not written.  Boxes, labels, counts and sizes are read on the
+ * device only, so a captured graph follows what is written before each replay; the result does not depend on thread
+ * scheduling.  SY_EINVAL: a null pointer, n or a slot side outside 1..65535, K outside 1..2^24, P outside 1..65536, or a
+ * dst slot shape other than src's. */
+typedef struct SyDrawBoxesDesc {
+  const uint8_t* src;       /* [n][max_h][max_w][3] */
+  const int32_t* sizes;     /* [n][2] device int32: h, w */
+  int32_t n;
+  int32_t max_h, max_w;     /* src's slot size */
+  const int32_t* boxes;     /* [n][K][4] x1, y1, x2, y2 */
+  const int32_t* labels;    /* [n][K] */
+  const int32_t* counts;    /* [n] */
+  int32_t K;
+  const uint8_t* palette;   /* [P][3] */
+  int32_t P;
+  uint8_t* dst;             /* [n][dst_h][dst_w][3], may be src */
+  int32_t dst_h, dst_w;     /* must equal max_h, max_w */
+} SyDrawBoxesDesc;
+int sy_draw_boxes(const SyDrawBoxesDesc* d, sy_stream_t stream);
+
+/* sy_vis_det_boxes: a streaming tick's NMS rows -> sy_draw_boxes's boxes, labels and counts, as the host path from the
+ * driver's output to vis_obj_fancy computes them: the score obj * class_conf in fp32 (stream.sized_output), rows kept
+ * where score >= score_th in fp32 (vis_det_th.py:81-83; -inf keeps every row, the script's score_th <= 0), in order; the
+ * boxes through the ltrb -> ltwh -> ltrb round trip of streaming_eval.py and vis_det_th.py:232 (w = x2 - x1, then
+ * x1 + w, in fp32) and rounded half to even (.round().astype(np.int32), :97; NaN, infinities and values outside int32
+ * become INT_MIN, as that cast gives on x86-64); the label is class_pred.  det is
+ * [S][A][7] (x1, y1, x2, y2, obj, class_conf, class_pred), stream s's first count[s] rows valid (clamped to [0, A]);
+ * boxes [S][A][4], labels [S][A], counts [S] are written.  SY_EINVAL: a null pointer, S outside 1..65535 or A outside
+ * 1..2^24. */
+typedef struct SyVisDetBoxesDesc {
+  const float* det;         /* [S][A][7] */
+  const int32_t* count;     /* [S] */
+  int32_t S, A;
+  float score_th;
+  int32_t* boxes;           /* [S][A][4] */
+  int32_t* labels;          /* [S][A] */
+  int32_t* counts;          /* [S] */
+} SyVisDetBoxesDesc;
+int sy_vis_det_boxes(const SyVisDetBoxesDesc* d, sy_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

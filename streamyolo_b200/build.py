@@ -35,6 +35,7 @@ SOURCES = {
     "jpeg.cu": [],
     "yuv.cu": [],
     "jpeg_encode.cu": [],
+    "vis.cu": [],
 }
 
 

@@ -380,3 +380,74 @@ def jpeg_files(buf, lengths, status, present=None, stage=None):
     torch.cuda.current_stream(buf.device).synchronize()
     host = stage.numpy()
     return [None if sp is None else host[sp[0]:sp[1]].tobytes() for sp in spans]
+
+
+def _device_int32(v, dev, what):
+    """``v`` (numpy, a list or a tensor) as a contiguous int32 tensor on ``dev``"""
+    t = v if torch.is_tensor(v) else torch.from_numpy(np.ascontiguousarray(np.asarray(v)))
+    ops._require(not t.is_floating_point() and not t.is_complex(), f"draw_boxes: {what} must be integers, not {t.dtype}")
+    return t.to(device=dev, dtype=torch.int32).contiguous()
+
+
+def draw_boxes(frames, boxes, labels, counts, palette, sizes=None, out=None):
+    """Draw detections as the sAP toolkit's visualisation does (vis_obj_fancy of sAP/vis/vis_det_th.py with
+    show_label=False, show_score=False; sy_draw_boxes): each box filled at 0.8 / 0.2 over the frame, then outlined two
+    pixels wide, in its label's palette colour, later boxes over earlier ones.
+
+    frames    uint8 CUDA [n, h, w, 3]; or slots [n, max_h, max_w, 3] with ``sizes`` (decode_jpeg_sized's output)
+    boxes     int32 [n, K, 4] x1, y1, x2, y2, already rounded (vis_obj_fancy's ``bboxes.round().astype(np.int32)``); or a
+              list of n [k_i, 4] arrays, which sets ``counts``
+    labels    int32 [n, K] (or a list of n [k_i] arrays), each in [0, P)
+    counts    int32 [n]: the first counts[i] boxes of row i are drawn (None with lists)
+    palette   uint8 [P, 3] in the frames' channel order: (B, G, R) for BGR frames
+    sizes     each frame's (h, w) at the top-left of its slot: host pairs or an int32 CUDA [n, 2] tensor
+    out       None: draw in place on ``frames`` and return them.  A uint8 tensor of ``frames``' shape: draw ``frames``
+              into it, leaving ``frames`` alone; only the pixels a box touches are written, so ``out`` should hold a copy
+              of the frames.  With ``out`` every other argument must already be a CUDA tensor, and the call only enqueues
+              the kernel (capturable in a CUDA graph, which then follows the boxes and counts written before each replay)
+
+    Host arguments are copied to the device (no synchronisation); nothing is read back."""
+    ops._require(torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+                 and frames.is_contiguous() and frames.is_cuda,
+                 "draw_boxes: frames must be a contiguous CUDA uint8 [n, h, w, 3] tensor")
+    n, mh, mw, _ = frames.shape
+    dev = frames.device
+    if out is not None:
+        args = {"boxes": boxes, "labels": labels, "counts": counts, "palette": palette}
+        if sizes is not None:
+            args["sizes"] = sizes
+        for k, v in args.items():
+            ops._require(torch.is_tensor(v) and v.is_cuda, f"draw_boxes: with out=, {k} must be a CUDA tensor")
+    if isinstance(boxes, (list, tuple)):
+        ops._require(counts is None and isinstance(labels, (list, tuple)) and len(boxes) == n and len(labels) == n,
+                     f"draw_boxes: give {n} box arrays and {n} label arrays, and no counts")
+        bl = [np.asarray(b, np.int64).reshape(-1, 4) for b in boxes]
+        ll = [np.asarray(l, np.int64).reshape(-1) for l in labels]
+        ops._require(all(len(b) == len(l) for b, l in zip(bl, ll)), "draw_boxes: each frame needs one label per box")
+        k = max([1] + [len(b) for b in bl])
+        bx, lb = np.zeros((n, k, 4), np.int64), np.zeros((n, k), np.int64)
+        for i, (b, l) in enumerate(zip(bl, ll)):
+            bx[i, :len(b)], lb[i, :len(l)] = b, l
+        boxes, labels, counts = bx, lb, [len(b) for b in bl]
+    for name, v in (("boxes", boxes), ("labels", labels), ("counts", counts)):
+        if not torch.is_tensor(v):
+            a = np.asarray(v)
+            ops._require(a.dtype.kind in "iub" and (a.size == 0 or (a.min() >= -2 ** 31 and a.max() < 2 ** 31)),
+                         f"draw_boxes: {name} must be int32 values")
+    boxes, labels, counts = (_device_int32(v, dev, k) for v, k in ((boxes, "boxes"), (labels, "labels"),
+                                                                    (counts, "counts")))
+    pal = palette if torch.is_tensor(palette) else torch.from_numpy(np.ascontiguousarray(np.asarray(palette, np.uint8)))
+    pal = pal.to(dev).contiguous()
+    if sizes is None:
+        sizes = [(mh, mw)] * n
+    if not torch.is_tensor(sizes):
+        hw = _sizes_list(sizes, "draw_boxes")
+        ops._require(len(hw) == n, f"draw_boxes: {len(hw)} sizes for {n} frames")
+        for i, (h, w) in enumerate(hw):
+            ops._require(h <= mh and w <= mw, f"draw_boxes: frame {i} of {h}x{w} is larger than the {mh}x{mw} slot")
+        sizes = torch.tensor(hw, dtype=torch.int32)
+    ops._require(sizes.dtype == torch.int32 and tuple(sizes.shape) == (n, 2), f"draw_boxes: sizes must be int32 [{n}, 2]")
+    sizes = sizes.to(dev).contiguous()
+    if boxes.dim() == 3 and boxes.data_ptr() % 16:
+        boxes = boxes.clone()
+    return ops.draw_boxes(frames, sizes, boxes, labels, counts, pal, frames if out is None else out)

@@ -163,6 +163,17 @@ class SyJpegEncodeDesc(C.Structure):
                 ("status", C.c_void_p), ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t)]
 
 
+class SyDrawBoxesDesc(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("sizes", C.c_void_p), ("n", C.c_int32), ("max_h", C.c_int32), ("max_w", C.c_int32),
+                ("boxes", C.c_void_p), ("labels", C.c_void_p), ("counts", C.c_void_p), ("K", C.c_int32),
+                ("palette", C.c_void_p), ("P", C.c_int32), ("dst", C.c_void_p), ("dst_h", C.c_int32), ("dst_w", C.c_int32)]
+
+
+class SyVisDetBoxesDesc(C.Structure):
+    _fields_ = [("det", C.c_void_p), ("count", C.c_void_p), ("S", C.c_int32), ("A", C.c_int32), ("score_th", C.c_float),
+                ("boxes", C.c_void_p), ("labels", C.c_void_p), ("counts", C.c_void_p)]
+
+
 class SySelectImagesDesc(C.Structure):
     _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
 
@@ -278,6 +289,8 @@ _SIG = {
     "sy_jpeg_encode_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int64]),
     "sy_jpeg_encode_max_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "sy_jpeg_encode": (C.c_int, [C.POINTER(SyJpegEncodeDesc), C.c_void_p]),
+    "sy_draw_boxes": (C.c_int, [C.POINTER(SyDrawBoxesDesc), C.c_void_p]),
+    "sy_vis_det_boxes": (C.c_int, [C.POINTER(SyVisDetBoxesDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
 
@@ -1220,3 +1233,63 @@ def jpeg_encode(src, sizes, quality, out, lengths, status, workspace):
     d = SyJpegEncodeDesc(src.data_ptr(), sizes.data_ptr(), n, mh, mw, int(quality), out.data_ptr(), out.shape[1],
                          lengths.data_ptr(), status.data_ptr(), workspace.data_ptr(), workspace.numel())
     _check(lib().sy_jpeg_encode(C.byref(d), _stream()), kernels=8)
+
+
+def draw_boxes(src, sizes, boxes, labels, counts, palette, dst):
+    """Draw the boxes of the sAP toolkit's vis_obj_fancy (vis_det_th.py:99-120, no text) on n images of their own sizes
+    (sy_draw_boxes): ``src`` / ``dst`` uint8 [n, max_h, max_w, 3] (the same tensor draws in place), image i of
+    ``sizes[i]`` = (h, w) (int32 [n, 2]) at the top-left of slot i; ``boxes`` int32 [n, K, 4] (x1, y1, x2, y2, rounded),
+    ``labels`` int32 [n, K], ``counts`` int32 [n] (the first counts[i] boxes of row i are drawn); ``palette`` uint8
+    [P, 3] in the images' channel order.  Only pixels a box touches are written.  Enqueues only (capturable)."""
+    _require(_tensor_ok(src, torch.uint8, 4) and src.shape[3] == 3 and src.is_cuda,
+             "draw_boxes: src must be contiguous CUDA uint8 [n, max_h, max_w, 3]")
+    n, mh, mw, _ = src.shape
+    dev = src.device
+    _require(_tensor_ok(dst, torch.uint8, 4) and tuple(dst.shape) == tuple(src.shape) and dst.device == dev,
+             f"draw_boxes: dst must be contiguous uint8 {list(src.shape)} on src's device")
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 2) and sizes.device == dev,
+             f"draw_boxes: sizes must be int32 [{n}, 2] on src's device")
+    _require(_tensor_ok(boxes, torch.int32, 3) and boxes.shape[0] == n and boxes.shape[2] == 4 and boxes.shape[1] >= 1
+             and boxes.device == dev and boxes.data_ptr() % 16 == 0,
+             f"draw_boxes: boxes must be contiguous 16-byte aligned int32 [{n}, K, 4] on src's device")
+    k = boxes.shape[1]
+    _require(_tensor_ok(labels, torch.int32, 2) and tuple(labels.shape) == (n, k) and labels.device == dev,
+             f"draw_boxes: labels must be int32 [{n}, {k}] on src's device")
+    _require(_tensor_ok(counts, torch.int32, 1) and counts.shape[0] == n and counts.device == dev,
+             f"draw_boxes: counts must be int32 [{n}] on src's device")
+    _require(_tensor_ok(palette, torch.uint8, 2) and palette.shape[1] == 3 and 1 <= palette.shape[0] <= 65536
+             and palette.device == dev, "draw_boxes: palette must be contiguous uint8 [P, 3] (1 <= P <= 65536) on src's "
+             "device")
+    d = SyDrawBoxesDesc(src.data_ptr(), sizes.data_ptr(), n, mh, mw, boxes.data_ptr(), labels.data_ptr(),
+                        counts.data_ptr(), k, palette.data_ptr(), palette.shape[0], dst.data_ptr(), dst.shape[1],
+                        dst.shape[2])
+    _check(lib().sy_draw_boxes(C.byref(d), _stream()))
+    return dst
+
+
+def vis_det_boxes(det, count, score_th, boxes=None, labels=None, counts=None):
+    """A streaming tick's NMS rows (fp32 [S, A, 7]: x1, y1, x2, y2 already divided by the ratio, obj, class_conf,
+    class_pred; ``count`` int32 [S]) -> draw_boxes's (boxes int32 [S, A, 4], labels int32 [S, A], counts int32 [S]) for
+    the rows whose fp32 score obj * class_conf is >= ``score_th`` (fp32; -inf keeps every row), in order, the boxes taken
+    through the ltwh round trip and rounded half to even (sy_vis_det_boxes).  Writes into the given buffers (allocated
+    when None).  Enqueues only (capturable)."""
+    _require(_tensor_ok(det, torch.float32, 3) and det.shape[2] == 7 and det.is_cuda,
+             "vis_det_boxes: det must be contiguous CUDA float32 [S, A, 7]")
+    s, a, _ = det.shape
+    dev = det.device
+    _require(_tensor_ok(count, torch.int32, 1) and count.shape[0] == s and count.device == dev,
+             f"vis_det_boxes: count must be int32 [{s}] on det's device")
+    if boxes is None:
+        boxes = torch.empty((s, a, 4), dtype=torch.int32, device=dev)
+        labels = torch.empty((s, a), dtype=torch.int32, device=dev)
+        counts = torch.empty((s,), dtype=torch.int32, device=dev)
+    _require(_tensor_ok(boxes, torch.int32, 3) and tuple(boxes.shape) == (s, a, 4) and boxes.device == dev
+             and boxes.data_ptr() % 16 == 0, f"vis_det_boxes: boxes must be 16-byte aligned int32 [{s}, {a}, 4]")
+    _require(_tensor_ok(labels, torch.int32, 2) and tuple(labels.shape) == (s, a) and labels.device == dev,
+             f"vis_det_boxes: labels must be int32 [{s}, {a}]")
+    _require(_tensor_ok(counts, torch.int32, 1) and counts.shape[0] == s and counts.device == dev,
+             f"vis_det_boxes: counts must be int32 [{s}]")
+    d = SyVisDetBoxesDesc(det.data_ptr(), count.data_ptr(), s, a, float(score_th), boxes.data_ptr(),
+                          labels.data_ptr(), counts.data_ptr())
+    _check(lib().sy_vis_det_boxes(C.byref(d), _stream()))
+    return boxes, labels, counts

@@ -56,10 +56,13 @@ class StreamTick:
     stream's features carried to the next tick.  With a YUV ``frame_format`` (an ops.YUV_FORMATS key) the input is ``yuv``
     (uint8 [S, max_bytes], stream i's frame in cv2's layout in the first bytes of row i), converted inside the tick into
     ``frames``.  With ``record_quality`` the tick ends with the JPEG encode of the frames in ``frames`` (``rec_out``,
-    ``rec_len``, ``rec_status``)."""
+    ``rec_len``, ``rec_status``).  With ``record_boxes`` = (fp32 score threshold, uint8 [P, 3] BGR palette on the device)
+    the encode reads ``rec_frames`` instead: a copy of ``frames`` with the tick's detections drawn (sy_vis_det_boxes,
+    sy_draw_boxes), so ``frames``, which a later tick may read again, is never drawn on."""
 
     def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None,
-                 forecast=None, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None):
+                 forecast=None, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None,
+                 record_boxes=None):
         self.model, self.size = model, tuple(size)
         self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
         table = np.asarray(table, np.int32)
@@ -115,6 +118,13 @@ class StreamTick:
             self.rec_status = torch.zeros((streams,), dtype=torch.int32, device=device)
             self.rec_ws = torch.empty(ops.jpeg_encode_workspace_bytes(streams, *slot, rec_bytes), dtype=torch.uint8,
                                       device=device)
+        # record_boxes: the frames are copied to rec_frames and the detections drawn there before the encode; vb holds
+        # sy_vis_det_boxes's (boxes, labels, counts), allocated by the first (warm-up) run
+        self.rec_boxes = record_boxes
+        if record_boxes is not None:
+            self.vb_th, self.vb_palette = record_boxes
+            self.rec_frames = torch.zeros_like(self.frames)
+            self.vb = None
 
     def run(self):
         ctx, net, head = self.ctx, self.model.backbone, self.model.head
@@ -141,8 +151,13 @@ class StreamTick:
             if self.fc_q:
                 self.fc_qout = ops.forecast_extrap_queries(self.fc, self.fc_qdt, self.fc_nq, self.fc_wh, self.fc_qout)
         if self.rec_q is not None:
-            ops.jpeg_encode(self.frames, self.rec_sizes, self.rec_q, self.rec_out, self.rec_len, self.rec_status,
-                            self.rec_ws)
+            rec = self.frames
+            if self.rec_boxes is not None:
+                self.vb = ops.vis_det_boxes(self.det, self.count, self.vb_th, *(self.vb or ()))
+                self.rec_frames.copy_(self.frames)
+                ops.draw_boxes(self.rec_frames, self.rec_sizes, *self.vb, self.vb_palette, self.rec_frames)
+                rec = self.rec_frames
+            ops.jpeg_encode(rec, self.rec_sizes, self.rec_q, self.rec_out, self.rec_len, self.rec_status, self.rec_ws)
 
 
 NO_FRAME = -1     # last_status() of a stream that was given no frame
@@ -196,6 +211,29 @@ def sized_output(det):
 
 
 FRAME_FORMATS = ("bgr",) + tuple(ops.YUV_FORMATS)
+
+
+def record_boxes_args(record_boxes, record_quality, num_classes):
+    """``StreamDetector(record_boxes=(score_th, palette))`` -> (the fp32 threshold sy_vis_det_boxes takes, the uint8
+    [P, 3] palette in BGR order), or ValueError"""
+    if record_quality is None:
+        raise ValueError("StreamDetector: record_boxes draws on the recorded frames: it takes record_quality")
+    if not isinstance(record_boxes, (tuple, list)) or len(record_boxes) != 2:
+        raise ValueError(f"StreamDetector: record_boxes must be None or (score_th, palette), not {record_boxes!r}")
+    th, palette = record_boxes
+    if isinstance(th, bool) or not isinstance(th, (int, float, np.integer, np.floating)) or not np.isfinite(th):
+        raise ValueError(f"StreamDetector: record_boxes's score_th must be a finite number, not {th!r}")
+    try:
+        pal = np.asarray(palette)
+    except Exception:
+        pal = None
+    if pal is None or pal.dtype.kind not in "iu" or pal.ndim != 2 or pal.shape[1] != 3 or pal.size == 0 \
+            or pal.min() < 0 or pal.max() > 255:
+        raise ValueError("StreamDetector: record_boxes's palette must be a list of (R, G, B) integer triples in 0..255")
+    if len(pal) < num_classes:
+        raise ValueError(f"StreamDetector: record_boxes's palette has {len(pal)} colours for {num_classes} classes")
+    # vis_obj_fancy filters only when score_th > 0 (vis_det_th.py:81), then compares fp32 scores with it in fp32
+    return (float(np.float32(th)) if th > 0 else -np.inf), np.ascontiguousarray(pal[:, ::-1].astype(np.uint8))
 
 
 def frame_shape(fmt, h, w):
@@ -259,13 +297,20 @@ class StreamDetector:
                       frame -- the decoded, converted or given frame the resize reads -- into the file cv2.imencode(".jpg",
                       frame, [cv2.IMWRITE_JPEG_QUALITY, record_quality]) makes (sy_jpeg_encode), and ``last_jpeg``
                       reads the files back.  The detections do not change
+      record_boxes    None (the default) or ``(score_th, palette)``, with ``record_quality``: each recorded frame has the
+                      tick's own detections drawn on it first, as the sAP toolkit's vis_det_th.py draws a result file
+                      (vis_obj_fancy without text: boxes filled at 0.8 / 0.2 and outlined two pixels wide in their class
+                      colour), the rows with score >= score_th (``score_th`` <= 0: every row).  ``palette``: a list of
+                      (R, G, B) per class, in the order of the toolkit's ``color_palette``, at least ``num_classes`` long.
+                      Drawn on a copy: the detections, forecasts and every other output do not change
     Each stream's frame is transformed as data.sized_table says and its boxes divided by its own ratio (``ratios``): a frame
     of driver size ``input_size`` gets the driver's plain resize and ``in_scale``.  ``frame_hw`` is the slot the frames are
     stored in: the largest height and width (the frame size when every stream has one size)."""
 
     def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
                  frame_sizes=None, input_size=None, jpeg_max_bytes=None, forecast=False, match_iou_th=0.3,
-                 max_tracks=1024, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None):
+                 max_tracks=1024, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None,
+                 record_boxes=None):
         if model.training:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
@@ -304,6 +349,8 @@ class StreamDetector:
         if record_quality is not None and (isinstance(record_quality, bool) or not isinstance(record_quality, (int, np.integer))
                                            or not 1 <= record_quality <= 100):
             raise ValueError(f"StreamDetector: record_quality must be None or an integer in 1..100, not {record_quality!r}")
+        if record_boxes is not None:
+            record_boxes = record_boxes_args(record_boxes, record_quality, model.head.num_classes)
         try:
             table, ratios = data.sized_table(sizes, size, in_scale)
         except RuntimeError as e:
@@ -318,7 +365,9 @@ class StreamDetector:
         self.queries = int(queries)
         self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes,
                                 (match_iou_th, int(max_tracks)) if forecast else None, clear_on_empty, self.queries,
-                                frame_format, None if record_quality is None else int(record_quality))
+                                frame_format, None if record_quality is None else int(record_quality),
+                                None if record_boxes is None else (record_boxes[0],
+                                                                   torch.from_numpy(record_boxes[1]).to(dev)))
         self.record_quality = None if record_quality is None else int(record_quality)
         if self.record_quality is not None:
             self._rec_len = feed.pinned((streams,), torch.int64)
