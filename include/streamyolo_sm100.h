@@ -820,6 +820,31 @@ typedef struct SyVisDetBoxesDesc {
 } SyVisDetBoxesDesc;
 int sy_vis_det_boxes(const SyVisDetBoxesDesc* d, sy_stream_t stream);
 
+/* sy_splice_frames: the split screen of the sAP toolkit's vis_contrast.py (sAP/vis/vis_contrast.py:148-165) on n pairs of
+ * uint8 images of their own sizes, written into A in place: image i is sizes[i] = (h, w) at the top-left of slot i of a
+ * and of b, both [n][max_h][max_w][3].  With splits[i] = (split, band_start, band_end) and c a pixel's coordinate along
+ * the split axis (its column, or its row with horizontal = 1):
+ *   band_start <= c < band_end   the band colour (:158-165, img[:, line_start:line_end] = line_color)
+ *   otherwise c >= split         B's pixel (:148-156: B alone where split <= 0, img[:, split:] = img_B[:, split:])
+ *   otherwise                    A's pixel, not written.
+ * The host clamps split, band_start and band_end to [0, l] (l = w, or h with horizontal), an empty band being
+ * band_start >= band_end; the kernel takes any int32 values as the rules above.  The colour is in the images' channel
+ * order: (93, 159, 241) for BGR images is the script's RGB [241, 159, 93].  Pixels outside an image are not read or
+ * written; an image whose size row is below 1 or outside the slot is left alone.  Sizes and splits are read on the device
+ * only, so a captured graph follows what is written before each replay.  One launch, no synchronisation.  SY_EINVAL: a
+ * null pointer, a == b, n or a slot side outside 1..65535, or horizontal other than 0 or 1. */
+typedef struct SySpliceFramesDesc {
+  uint8_t* a;               /* [n][max_h][max_w][3], written in place */
+  const uint8_t* b;         /* [n][max_h][max_w][3] */
+  const int32_t* sizes;     /* [n][2] device int32: h, w */
+  const int32_t* splits;    /* [n][3] device int32: split, band_start, band_end */
+  int32_t n;
+  int32_t max_h, max_w;     /* slot size of a and b */
+  int32_t horizontal;       /* 0: split along x (columns, the script's default), 1: along y (--horizontal) */
+  uint8_t color[3];         /* the band colour */
+} SySpliceFramesDesc;
+int sy_splice_frames(const SySpliceFramesDesc* d, sy_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

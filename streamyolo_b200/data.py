@@ -451,3 +451,45 @@ def draw_boxes(frames, boxes, labels, counts, palette, sizes=None, out=None):
     if boxes.dim() == 3 and boxes.data_ptr() % 16:
         boxes = boxes.clone()
     return ops.draw_boxes(frames, sizes, boxes, labels, counts, pal, frames if out is None else out)
+
+
+# the band colour of the sAP toolkit's vis_contrast.py (RGB [241, 159, 93], :106) in BGR order
+CONTRAST_BAND_BGR = (93, 159, 241)
+
+
+def splice_frames(a, b, splits, sizes=None, horizontal=False, color=CONTRAST_BAND_BGR):
+    """Compose split-screen frames as the sAP toolkit's vis_contrast.py does (:148-165; sy_splice_frames): frame B from
+    the split line on, frame A before it, and a band of ``color`` over both, written into ``a`` in place.
+
+    a, b      uint8 CUDA [n, h, w, 3], or slots [n, max_h, max_w, 3] with ``sizes`` (decode_jpeg_sized's output); two
+              different tensors of one shape
+    splits    per frame (split, band_start, band_end): columns, or rows with ``horizontal``, at or past ``split`` take B's
+              pixels, and [band_start, band_end) takes the band colour.  Host triples or an int32 CUDA [n, 3] tensor
+    sizes     each pair's (h, w) at the top-left of its slots: host pairs (checked here) or an int32 CUDA [n, 2] tensor
+    color     the band colour in the frames' channel order: the script's, for BGR frames, by default
+
+    Host arguments are copied to the device (no synchronisation); with every argument a CUDA tensor the call only
+    enqueues the kernel, so it can be captured in a CUDA graph, which then follows the splits and sizes written before
+    each replay.  Pixels outside each frame, and A's pixels before the split outside the band, are not written."""
+    ops._require(torch.is_tensor(a) and a.dtype == torch.uint8 and a.dim() == 4 and a.shape[3] == 3
+                 and a.is_contiguous() and a.is_cuda, "splice_frames: a must be a contiguous CUDA uint8 [n, h, w, 3] tensor")
+    n, mh, mw, _ = a.shape
+    dev = a.device
+    if not torch.is_tensor(splits):
+        sp = np.asarray(splits, np.int64).reshape(-1, 3) if len(splits) else np.zeros((0, 3), np.int64)
+        ops._require(len(sp) == n, f"splice_frames: {len(sp)} splits for {n} frames")
+        ops._require(sp.size == 0 or (sp.min() >= -2 ** 31 and sp.max() < 2 ** 31), "splice_frames: splits must be "
+                     "int32 values")
+        splits = torch.from_numpy(sp.astype(np.int32))
+    ops._require(splits.dtype == torch.int32 and tuple(splits.shape) == (n, 3), f"splice_frames: splits must be int32 "
+                 f"[{n}, 3]")
+    if sizes is None:
+        sizes = [(mh, mw)] * n
+    if not torch.is_tensor(sizes):
+        hw = _sizes_list(sizes, "splice_frames")
+        ops._require(len(hw) == n, f"splice_frames: {len(hw)} sizes for {n} frames")
+        for i, (h, w) in enumerate(hw):
+            ops._require(h <= mh and w <= mw, f"splice_frames: frame {i} of {h}x{w} is larger than the {mh}x{mw} slot")
+        sizes = torch.tensor(hw, dtype=torch.int32)
+    ops._require(sizes.dtype == torch.int32 and tuple(sizes.shape) == (n, 2), f"splice_frames: sizes must be int32 [{n}, 2]")
+    return ops.splice_frames(a, b, sizes.to(dev).contiguous(), splits.to(dev).contiguous(), horizontal, color)

@@ -174,6 +174,11 @@ class SyVisDetBoxesDesc(C.Structure):
                 ("boxes", C.c_void_p), ("labels", C.c_void_p), ("counts", C.c_void_p)]
 
 
+class SySpliceFramesDesc(C.Structure):
+    _fields_ = [("a", C.c_void_p), ("b", C.c_void_p), ("sizes", C.c_void_p), ("splits", C.c_void_p), ("n", C.c_int32),
+                ("max_h", C.c_int32), ("max_w", C.c_int32), ("horizontal", C.c_int32), ("color", C.c_uint8 * 3)]
+
+
 class SySelectImagesDesc(C.Structure):
     _fields_ = [("src", SyTensor * 3), ("dst", SyTensor * 3), ("n_pairs", C.c_int32), ("flags", C.c_void_p)]
 
@@ -291,6 +296,7 @@ _SIG = {
     "sy_jpeg_encode": (C.c_int, [C.POINTER(SyJpegEncodeDesc), C.c_void_p]),
     "sy_draw_boxes": (C.c_int, [C.POINTER(SyDrawBoxesDesc), C.c_void_p]),
     "sy_vis_det_boxes": (C.c_int, [C.POINTER(SyVisDetBoxesDesc), C.c_void_p]),
+    "sy_splice_frames": (C.c_int, [C.POINTER(SySpliceFramesDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
 
@@ -1293,3 +1299,28 @@ def vis_det_boxes(det, count, score_th, boxes=None, labels=None, counts=None):
                           labels.data_ptr(), counts.data_ptr())
     _check(lib().sy_vis_det_boxes(C.byref(d), _stream()))
     return boxes, labels, counts
+
+
+def splice_frames(a, b, sizes, splits, horizontal, color):
+    """The split screen of the sAP toolkit's vis_contrast.py (:148-165) on n pairs of images of their own sizes
+    (sy_splice_frames), written into ``a`` in place: ``a`` / ``b`` uint8 [n, max_h, max_w, 3], pair i of ``sizes[i]`` =
+    (h, w) (int32 [n, 2]) at the top-left of slot i; ``splits`` int32 [n, 3] (split, band_start, band_end) along the
+    columns, or the rows with ``horizontal``: a pixel in [band_start, band_end) gets ``color`` (3 values in the images'
+    channel order), else one at or past ``split`` gets B's pixel, else it keeps A's.  Enqueues only (capturable)."""
+    _require(_tensor_ok(a, torch.uint8, 4) and a.shape[3] == 3 and a.is_cuda,
+             "splice_frames: a must be contiguous CUDA uint8 [n, max_h, max_w, 3]")
+    n, mh, mw, _ = a.shape
+    dev = a.device
+    _require(_tensor_ok(b, torch.uint8, 4) and tuple(b.shape) == tuple(a.shape) and b.device == dev,
+             f"splice_frames: b must be contiguous uint8 {list(a.shape)} on a's device")
+    _require(a.data_ptr() != b.data_ptr(), "splice_frames: a and b must be different buffers")
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 2) and sizes.device == dev,
+             f"splice_frames: sizes must be int32 [{n}, 2] on a's device")
+    _require(_tensor_ok(splits, torch.int32, 2) and tuple(splits.shape) == (n, 3) and splits.device == dev,
+             f"splice_frames: splits must be int32 [{n}, 3] on a's device")
+    col = [int(c) for c in color]
+    _require(len(col) == 3 and all(0 <= c <= 255 for c in col), "splice_frames: color must be 3 values in 0..255")
+    d = SySpliceFramesDesc(a.data_ptr(), b.data_ptr(), sizes.data_ptr(), splits.data_ptr(), n, mh, mw, int(bool(horizontal)),
+                           (C.c_uint8 * 3)(*col))
+    _check(lib().sy_splice_frames(C.byref(d), _stream()))
+    return a
