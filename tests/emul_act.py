@@ -56,9 +56,10 @@ def wrap(monkeypatch):
             return base_apply(x, scale_ptr, shift_ptr, split_n, act, res, y, y_goff1, res_goff1)
         scale, shift = ((scale_ptr, shift_ptr) if torch.is_tensor(scale_ptr)
                         else (emul_ops.PTRS[scale_ptr], emul_ops.PTRS[shift_ptr]))
+        scale, shift = scale.reshape(-1, x.c), shift.reshape(-1, x.c)
         t = emul_ops._nchw(x)
         n = t.shape[0]
-        sp = split_n if 0 < split_n < n else n
+        sp = min(max(split_n, 0), n)          # group 1 = the images >= split_n, as sy_bn_act_apply
         outs = []
         for gi, (a, b, yo, ro) in enumerate([(0, sp, 0, 0), (sp, n, y_goff1, res_goff1)]):
             if a >= b:
@@ -68,7 +69,7 @@ def wrap(monkeypatch):
                 out = out + emul_ops._strided(res, a, b - a, ro).permute(0, 3, 1, 2).float()
             outs.append((a, b, yo, out))
         for a, b, yo, out in outs:           # every residual is read before any output is written (in-place residuals)
-            emul_ops._strided(y, a, b - a, yo).copy_(emul_ops._bf(out.permute(0, 2, 3, 1)))
+            emul_ops._strided(y, a, b - a, yo).copy_(out.permute(0, 2, 3, 1))
 
     def bn_act_backward(raw, dy, draw, scale, shift, mean, invstd, split_n, act, dgamma, dbeta, accumulate=False):
         if act not in KINKS:

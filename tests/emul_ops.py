@@ -32,7 +32,39 @@ def _nchw(v: View):
 
 
 def _store(v: View, t_nchw):
-    v.torch().copy_(_bf(t_nchw.permute(0, 2, 3, 1)))
+    """one rounding to the view's storage (bf16, fp16, or fp32 in EXACT mode)"""
+    v.torch().copy_(t_nchw.permute(0, 2, 3, 1))
+
+
+def _require(cond, msg):
+    """the library's argument checks: it refuses before any launch, with ops._check's RuntimeError"""
+    if not cond:
+        raise RuntimeError("libstreamyolo_sm100 error 1: " + msg)
+
+
+ACTS = (ops.SY_ACT_NONE, ops.SY_ACT_SILU, ops.SY_ACT_RELU, ops.SY_ACT_LRELU)
+
+
+def _act(t, code):
+    """the SY_ACT_* activation (include/streamyolo_sm100.h)"""
+    _require(code in ACTS, f"act={code} is not an SY_ACT_* code")
+    if code == ops.SY_ACT_SILU:
+        return F.silu(t)
+    if code == ops.SY_ACT_RELU:
+        return F.relu(t)
+    return F.leaky_relu(t, 0.1) if code == ops.SY_ACT_LRELU else t
+
+
+def _dact(z, code):
+    """its derivative, autograd's value at z = 0 (0 for ReLU, 0.1 for LeakyReLU)"""
+    if code == ops.SY_ACT_SILU:
+        s = torch.sigmoid(z)
+        return s * (1 + z * (1 - s))
+    if code == ops.SY_ACT_RELU:
+        return (z > 0).to(z.dtype)
+    if code == ops.SY_ACT_LRELU:
+        return torch.where(z > 0, torch.ones_like(z), torch.full_like(z, 0.1))
+    return torch.ones_like(z)
 
 
 def _unpack(wpk, kh, kw):
@@ -42,13 +74,27 @@ def _unpack(wpk, kh, kw):
 
 
 def conv_stat_rows():
+    """the library's is the SM count (132 on an H100 SXM, 114 on a PCIe card); the host only sizes the partials of a RAW
+    launch with it and hands them back, so any count the conv below accepts serves"""
     return 132
 
 
 def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=None, partials=None, split_n=0,
            timeline=None, debug_flags=0, bn=None, momentum=0.03, eps=1e-3, scale_shift=None, sync=None, mean_invstd=None,
            debug_f32=None, tile_mode=0, tile_bn=0, stat_updates=1):
+    """Returns the number of partial rows written: one row per launch with ``partials`` (the sums of the whole batch,
+    [Cout][2 groups][2 (sum, sumsq)] as the library lays out each of its per-CTA rows), 0 without."""
     kh, kw = (k, k) if isinstance(k, int) else k
+    dtypes = {x.dtype, y.dtype, wpk.dtype} | ({res.dtype} if res is not None else set())
+    if len(dtypes) != 1:
+        raise ValueError(f"conv2d: x, y, res and the packed weights must share one storage dtype, got {sorted(map(str, dtypes))}")
+    _require(act in ACTS, f"conv2d: act={act} is not an SY_ACT_* code")
+    _require(x.dtype != torch.float16 or (mode == ops.SY_CONV_FUSED and not bn and partials is None and impl != "simt"),
+             "conv2d: fp16 storage is FUSED mode only, without statistics")
+    one_group = not 0 < split_n < x.n
+    _require(stat_updates in (0, 1, 2) and (stat_updates != 2 or (bn and one_group)),
+             f"conv2d: stat_updates={stat_updates} with split_n={split_n} of {x.n}")
+    _require(partials is None or partials.shape[0] >= conv_stat_rows(), "conv2d: too few statistic rows")
     if impl == "dw":                                # depthwise: wpk [kh*kw][C]
         c = wpk.shape[1]
         out = F.conv2d(_nchw(x), wpk.float().t().reshape(c, 1, kh, kw), None, s, ((kh - 1) // 2, (kw - 1) // 2), groups=c)
@@ -57,18 +103,22 @@ def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=
     if mode == ops.SY_CONV_FUSED:
         if scale is not None:
             out = out * scale.float()[None, :, None, None] + shift.float()[None, :, None, None]
-        if act:
-            out = F.silu(out)
+        out = _act(out, act)
         if res is not None:
             out = out + _nchw(res)
         _store(y, out)
         return 0
     _store(y, out)
+    stored = _nchw(y)
+    n = stored.shape[0]
+    sp = split_n if 0 < split_n < n else n
+    groups = [(0, sp), (sp, n)] if sp < n else [(0, n)]
+    if partials is not None:
+        row = partials[0].view(stored.shape[1], 2, 2)
+        for gi, (a, b) in enumerate(groups):
+            row[:, gi, 0] = stored[a:b].sum((0, 2, 3))
+            row[:, gi, 1] = stored[a:b].pow(2).sum((0, 2, 3))
     if bn:
-        stored = _nchw(y)
-        n = stored.shape[0]
-        sp = split_n if 0 < split_n < n else n
-        groups = [(0, sp), (sp, n)] if sp < n else [(0, n)]
         c0s = [seg[5] for seg in bn] + [stored.shape[1]]
         for gi, (a, b) in enumerate(groups):
             part = stored[a:b]
@@ -84,7 +134,7 @@ def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=
                 if mean_invstd is not None:
                     mean_invstd[0, gi, sl] = mean[sl]
                     mean_invstd[1, gi, sl] = invstd[sl]
-                for _ in range(stat_updates):
+                for _ in range(max(stat_updates, 1)):
                     if rm is not None:
                         rm.mul_(1 - momentum).add_(momentum * mean[sl])
                         rv.mul_(1 - momentum).add_(momentum * var[sl] * (cnt / max(cnt - 1, 1)))
@@ -92,7 +142,7 @@ def conv2d(x, wpk, y, k, s, mode, impl="tc", scale=None, shift=None, act=1, res=
                         nbt.add_(1)
         PTRS[scale_shift[0].data_ptr()] = scale_shift[0]
         PTRS[scale_shift[1].data_ptr()] = scale_shift[1]
-    return 132
+    return 1 if partials is not None else 0
 
 
 def _strided(v: View, img0, nimg, goff):
@@ -105,25 +155,33 @@ def _strided(v: View, img0, nimg, goff):
 
 
 def bn_act_apply(x, scale_ptr, shift_ptr, split_n, act, res, y, y_goff1=0, res_goff1=0):
+    """group 1 = the images >= split_n (split_n <= 0: every image, split_n >= n: none); a scale / shift of one row serves a
+    launch whose images are all in group 0"""
     scale, shift = (scale_ptr, shift_ptr) if torch.is_tensor(scale_ptr) else (PTRS[scale_ptr], PTRS[shift_ptr])   # [2 groups][C]
+    _require((x.n, x.h, x.w, x.c) == (y.n, y.h, y.w, y.c), "bn_act_apply: x/y shape mismatch")
+    _require(res is None or (res.n, res.h, res.w, res.c) == (x.n, x.h, x.w, x.c), "bn_act_apply: residual mismatch")
+    _require(y_goff1 % 8 == 0 and res_goff1 % 8 == 0, "bn_act_apply: group offsets must be multiples of 8")
+    _require(act in ACTS, f"bn_act_apply: act={act} is not an SY_ACT_* code")
+    scale, shift = scale.reshape(-1, x.c), shift.reshape(-1, x.c)
     t = _nchw(x)
     n = t.shape[0]
-    sp = split_n if 0 < split_n < n else n
+    sp = min(max(split_n, 0), n)
+    outs = []
     for gi, (a, b, yo, ro) in enumerate([(0, sp, 0, 0), (sp, n, y_goff1, res_goff1)]):
         if a >= b:
             continue
-        out = t[a:b] * scale[gi][None, :, None, None] + shift[gi][None, :, None, None]
-        if act:
-            out = F.silu(out)
+        out = _act(t[a:b] * scale[gi][None, :, None, None] + shift[gi][None, :, None, None], act)
         if res is not None:
             out = out + _strided(res, a, b - a, ro).permute(0, 3, 1, 2).float()
-        _strided(y, a, b - a, yo).copy_(_bf(out.permute(0, 2, 3, 1)))
+        outs.append((a, b, yo, out))
+    for a, b, yo, out in outs:           # every residual is read before any output is written (in-place residuals)
+        _strided(y, a, b - a, yo).copy_(out.permute(0, 2, 3, 1))
 
 
 def focus_pack(x, frames, y):
     b = x.shape[0]
     xs = torch.cat([x[:, 3 * f:3 * f + 3] for f in range(frames)], 0)
-    xs = xs.float() if EXACT else xs.to(torch.bfloat16).float()
+    xs = xs.float() if EXACT else xs.to(y.dtype).float()
     foc = torch.cat([xs[..., ::2, ::2], xs[..., 1::2, ::2], xs[..., ::2, 1::2], xs[..., 1::2, 1::2]], 1)   # [n,12,h,w]
     n, _, h, w = foc.shape
     out = torch.zeros(n, 64, h, w)
@@ -134,22 +192,34 @@ def focus_pack(x, frames, y):
     assert n == frames * b
 
 
+def _same_dtype(what, *views):
+    if len({v.dtype for v in views}) != 1:
+        raise ValueError(f"{what}: the views must share one storage dtype")
+
+
 def upsample_nearest(x, y):
+    _same_dtype("upsample_nearest", x, y)
     _store(y, F.interpolate(_nchw(x), size=(y.h, y.w), mode="nearest"))
 
 
 def spp_maxpool(x, y5, y9, y13):
+    _same_dtype("spp_maxpool", x, y5, y9, y13)
     t = _nchw(x)
     for k, v in ((5, y5), (9, y9), (13, y13)):
         _store(v, F.max_pool2d(t, k, 1, k // 2))
 
 
 def copy(x, y):
+    _same_dtype("copy", x, y)
+    _require((x.n, x.h, x.w, x.c) == (y.n, y.h, y.w, y.c), "copy: view mismatch")
     y.torch().copy_(x.torch())
 
 
 def head_pred_decode(cls_feat, reg_feat, w_reg, b_reg, w_obj, b_obj, w_cls, b_cls, stride, anchor_offset, a_total, out,
                      origin, sigmoid, decode):
+    if cls_feat.dtype != reg_feat.dtype:
+        raise ValueError("head_pred_decode: the views must share one storage dtype")
+    _require(0 <= anchor_offset and anchor_offset + cls_feat.h * cls_feat.w <= a_total, "head_pred: anchor range")
     cf, rf = _nchw(cls_feat), _nchw(reg_feat)
     o = torch.cat([F.conv2d(rf, w_reg[:, :, None, None], b_reg), F.conv2d(rf, w_obj[:, :, None, None], b_obj),
                    F.conv2d(cf, w_cls[:, :, None, None], b_cls)], 1)
@@ -169,6 +239,8 @@ def head_pred_decode(cls_feat, reg_feat, w_reg, b_reg, w_obj, b_obj, w_cls, b_cl
 
 
 def tal_loss_workspace_bytes(b, a_total, max_labels, num_classes):
+    """the host allocates this many bytes and hands the buffer to tal_loss / tal_loss_backward: here it only keys
+    LOSS_STATE"""
     return 256
 
 
@@ -180,6 +252,10 @@ def _loss_oracle(hw, strides, gamma, thr, val, nc):
 
 def tal_loss(outputs, origin, labels_fut, labels_cur, hw, strides, gamma, ignore_thr, ignore_value, use_l1, workspace,
              loss_out, fg_out=None, matched_out=None, pred_iou_out=None):
+    _require(sum(h * w for h, w in hw) == outputs.shape[1], "tal_loss: levels give the wrong anchor count")
+    _require(workspace.numel() * workspace.element_size() >= tal_loss_workspace_bytes(
+        outputs.shape[0], outputs.shape[1], labels_fut.shape[1], outputs.shape[2] - 5), "tal_loss: workspace too small")
+    _require(not use_l1 or origin is not None, "tal_loss: use_l1 needs origin preds")
     o, grid = _loss_oracle(hw, strides, gamma, ignore_thr, ignore_value, outputs.shape[2] - 5)
     with torch.enable_grad():
         out_l, org_l = outputs.clone().requires_grad_(True), origin.clone().requires_grad_(True)
@@ -207,13 +283,32 @@ def tal_loss_backward(outputs, origin, labels_fut, hw, strides, gamma, use_l1, w
 
 def head_pred_backward(grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls, a_total, anchor_offset,
                        dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate=False):
+    """1 <= classes <= 27, as sy_head_pred_backward"""
+    _require(1 <= w_cls.shape[0] <= 27, "head_pred_backward: num_classes out of range")
+    _head_pred_bwd(grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls, a_total, anchor_offset, dw_reg,
+                   dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate)
+
+
+def head_pred_backward_wide(grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls, a_total,
+                            anchor_offset, dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate=False):
+    """1 <= classes <= 251 with (5 + classes) x channels x 4 bytes <= 200 KiB, as sy_head_pred_backward_wide"""
+    nc = w_cls.shape[0]
+    _require(1 <= nc <= 251 and cls_feat.c % 8 == 0 and 4 * (5 + nc) * cls_feat.c <= 200 * 1024,
+             "head_pred_backward_wide: num_classes out of range")
+    _head_pred_bwd(grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls, a_total, anchor_offset, dw_reg,
+                   dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate)
+
+
+def _head_pred_bwd(grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_reg, w_obj, w_cls, a_total, anchor_offset,
+                   dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls, accumulate):
     h, w = cls_feat.h, cls_feat.w
+    _require(0 <= anchor_offset and anchor_offset + h * w <= a_total, "head_pred_backward: anchor range")
     g = grad_raw[:, anchor_offset:anchor_offset + h * w]                    # [b, hw, no]
     cf, rf = cls_feat.torch().float().flatten(1, 2), reg_feat.torch().float().flatten(1, 2)   # [b, hw, c]
     d_rf = g[..., 0:4] @ w_reg + g[..., 4:5] @ w_obj
     d_cf = g[..., 5:] @ w_cls
-    d_reg_feat.torch().copy_(_bf(d_rf.reshape(d_reg_feat.torch().shape)))
-    d_cls_feat.torch().copy_(_bf(d_cf.reshape(d_cls_feat.torch().shape)))
+    d_reg_feat.torch().copy_(d_rf.reshape(d_reg_feat.torch().shape))
+    d_cls_feat.torch().copy_(d_cf.reshape(d_cls_feat.torch().shape))
     res = [torch.einsum("bpo,bpc->oc", g[..., 0:4], rf), torch.einsum("bpo,bpc->oc", g[..., 4:5], rf),
            torch.einsum("bpo,bpc->oc", g[..., 5:], cf), g[..., 0:4].sum((0, 1)), g[..., 4:5].sum((0, 1)), g[..., 5:].sum((0, 1))]
     for dst, val in zip((dw_reg, dw_obj, dw_cls, db_reg, db_obj, db_cls), res):
@@ -221,6 +316,7 @@ def head_pred_backward(grad_raw, cls_feat, reg_feat, d_cls_feat, d_reg_feat, w_r
 
 
 def bn_act_backward(raw, dy, draw, scale, shift, mean, invstd, split_n, act, dgamma, dbeta, accumulate=False):
+    _require(act in ACTS, f"bn_act_backward: act={act} is not an SY_ACT_* code")
     r, d = _nchw(raw), _nchw(dy)
     n = r.shape[0]
     sp = split_n if 0 < split_n < n else n
@@ -228,9 +324,7 @@ def bn_act_backward(raw, dy, draw, scale, shift, mean, invstd, split_n, act, dga
     dg, db = torch.zeros_like(dgamma), torch.zeros_like(dbeta)
     for gi, (a, b) in enumerate([(0, sp), (sp, n)] if sp < n else [(0, n)]):
         sc, sh, mu, iv = (t[gi][None, :, None, None] for t in (scale, shift, mean, invstd))
-        z = r[a:b] * sc + sh
-        s = torch.sigmoid(z)
-        dz = d[a:b] * (s * (1 + z * (1 - s))) if act else d[a:b]
+        dz = d[a:b] * _dact(r[a:b] * sc + sh, act)
         xh = (r[a:b] - mu) * iv
         m1, m2 = dz.mean((0, 2, 3), keepdim=True), (dz * xh).mean((0, 2, 3), keepdim=True)
         out[a:b] = sc * (dz - m1 - xh * m2)
@@ -249,6 +343,7 @@ def conv2d_wgrad(x, dy, k, s, dw, accumulate=False, workspace=None):
 
 
 def dilate2(g, D):
+    _require(g.n == D.n and g.c == D.c and D.h in (2 * g.h - 1, 2 * g.h) and D.w in (2 * g.w - 1, 2 * g.w), "dilate2: bad views")
     D.torch().zero_()
     D.torch()[:, ::2, ::2, :][:, :g.h, :g.w] = g.torch()
 
@@ -269,16 +364,21 @@ def spp_maxpool_backward(x, d5, d9, d13, dx):
 
 
 def add_(x, y):
+    _require((x.n, x.h, x.w, x.c) == (y.n, y.h, y.w, y.c), "add: view mismatch")
     _store(y, _nchw(x) + _nchw(y))
 
 
 def sgd_nesterov_ema_step(param, grad, momentum_buf, ema, n_param, decay_begin, lr, momentum=0.9, weight_decay=5e-4,
-                          inv_scale=1.0, nesterov=True, ema_decay=0.0, found_inf=None, hyper=None):
-    """what sy_sgd_nesterov_ema_step does, in torch (same order of operations as torch.optim.SGD / yolox ModelEMA)"""
+                          inv_scale=1.0, nesterov=True, ema_decay=0.0, found_inf=None, hyper=None, found_inf_ema=False):
+    """what sy_sgd_nesterov_ema_step does, in torch (same order of operations as torch.optim.SGD / yolox ModelEMA); a
+    flagged step with ``found_inf_ema`` still moves the EMA towards the unchanged parameters (ModelEMA.update)"""
+    one_minus = 1.0 - ema_decay
+    if hyper is not None:             # 1 - ema_decay is hyper[5] as the host wrote it, not recomputed from hyper[4]
+        lr, momentum, weight_decay, inv_scale, ema_decay, one_minus = (float(v) for v in hyper[:6])
     if found_inf is not None and float(found_inf) != 0.0:
+        if found_inf_ema and ema is not None:
+            ema.mul_(ema_decay).add_(one_minus * param)
         return
-    if hyper is not None:
-        lr, momentum, weight_decay, inv_scale, ema_decay = (float(v) for v in hyper[:5])
     p = param[:n_param]
     g = grad[:n_param] * inv_scale if inv_scale != 1.0 else grad[:n_param].clone()
     g[decay_begin:] = g[decay_begin:].add(p[decay_begin:], alpha=weight_decay)
@@ -286,11 +386,21 @@ def sgd_nesterov_ema_step(param, grad, momentum_buf, ema, n_param, decay_begin, 
     g = g.add(momentum_buf, alpha=momentum) if nesterov else momentum_buf
     p.add_(g, alpha=-lr)
     if ema is not None:
-        ema.mul_(ema_decay).add_((1.0 - ema_decay) * param)
+        ema.mul_(ema_decay).add_(one_minus * param)
 
 
-def resize_bilinear(x, size):
-    return F.interpolate(x, size=size, mode="bilinear", align_corners=False)
+def nonfinite_flag(x, flag, count):
+    flag.fill_(float(not bool(torch.isfinite(x).all())))
+    count.add_(flag.to(torch.int32))
+
+
+def resize_bilinear(x, size, out=None):
+    y = F.interpolate(x, size=size, mode="bilinear", align_corners=False)
+    if out is None:
+        return y
+    _require(tuple(out.shape) == tuple(y.shape) and out.dtype == torch.float32 and out.is_contiguous(),
+             "resize_bilinear: bad out")
+    return out.copy_(y)
 
 
 def scale_labels_(labels, sx, sy):
@@ -318,11 +428,59 @@ class PackBatch:
                 out[:, :, co:co + w.shape[0]].copy_(pack_conv_weight_dgrad(w))
 
 
+def letterbox_sized(src, sizes, out):
+    """the streaming driver's preproc of each frame.  Deliberately narrower than the library: only rows whose
+    destination fills ``out`` (the library puts a smaller one top-left on a canvas of 114)"""
+    from oracle import input_oracle
+    for i, (h, w, dh, dw) in enumerate(sizes.tolist()):
+        assert (dh, dw) == tuple(out.shape[2:]), "emulated for destinations that fill out only"
+        out[i] = torch.from_numpy(input_oracle.stream_frame(src[i, :h, :w].numpy(), (dh, dw))[0])
+
+
+def stream_gate(status, flags, start, keep):
+    ok = torch.ones_like(flags) if status is None else (status == 0).to(torch.int32)
+    start.copy_(ok * (flags != 0).to(torch.int32))
+    keep.copy_(ok)
+
+
+def stream_rescale(det, count, status, ratio):
+    for i in range(det.shape[0]):
+        if status is not None and int(status[i]) != 0:
+            count[i] = 0
+        else:
+            det[i, :int(count[i]), :4] /= ratio[i]
+
+
+def select_images(srcs, dsts, flags):
+    _require(1 <= len(srcs) == len(dsts) <= 3, "select_images: 1 to 3 (src, dst) view pairs")
+    for s, d in zip(srcs, dsts):
+        for i in range(s.n):
+            if int(flags[i]):
+                d.torch()[i].copy_(s.torch()[i])
+
+
+def postprocess_nms(pred, num_classes, conf_thre, nms_thre, class_agnostic=False, max_det=None):
+    """what sy_postprocess_nms writes, from the NMS oracle; rows past count[i] are zero here and unspecified there"""
+    from oracle.postprocess_oracle import postprocess_oracle
+    b, a, _ = pred.shape
+    max_det = a if max_det is None else max_det
+    det = torch.zeros((b, max_det, 7))
+    count = torch.zeros((b,), dtype=torch.int32)
+    for i, d in enumerate(postprocess_oracle(pred, num_classes, conf_thre, nms_thre, class_agnostic)):
+        if d is not None:
+            d = d[:max_det]
+            det[i, :len(d)] = d
+            count[i] = len(d)
+    return det, count
+
+
 NAMES = ["conv_stat_rows", "conv2d", "bn_act_apply", "focus_pack", "upsample_nearest", "spp_maxpool", "copy",
          "head_pred_decode", "tal_loss_workspace_bytes", "tal_loss", "tal_loss_backward", "head_pred_backward",
-         "bn_act_backward", "conv2d_wgrad", "dilate2", "upsample_nearest_backward", "spp_maxpool_backward", "add_",
-         "pack_conv_weight", "pack_conv_weight_dgrad", "pack_stem_weight", "sgd_nesterov_ema_step", "resize_bilinear",
-         "scale_labels_", "pack_dw_weight", "stats_num_partials", "channel_stats", "bn_finalize", "PackBatch"]
+         "head_pred_backward_wide", "bn_act_backward", "conv2d_wgrad", "dilate2", "upsample_nearest_backward",
+         "spp_maxpool_backward", "add_", "pack_conv_weight", "pack_conv_weight_dgrad", "pack_stem_weight",
+         "sgd_nesterov_ema_step", "nonfinite_flag", "resize_bilinear", "scale_labels_", "pack_dw_weight",
+         "stats_num_partials", "channel_stats", "bn_finalize", "PackBatch", "letterbox_sized", "stream_gate",
+         "stream_rescale", "select_images", "postprocess_nms"]
 
 
 def _view_init(self, buf, c0=0, c=None, n0=0, n=None):
@@ -332,9 +490,13 @@ def _view_init(self, buf, c0=0, c=None, n0=0, n=None):
     self.n = buf.shape[0] - n0 if n is None else n
 
 
-def pack_conv_weight(*ws):
+def _pk(t, dtype):
+    return _bf(t) if dtype == torch.bfloat16 or EXACT else t.to(dtype)
+
+
+def pack_conv_weight(*ws, dtype=torch.bfloat16):
     """what sy_pack_conv_weight (mode 0) writes: [sum O][kh*kw][I] in the emulated storage type"""
-    return torch.cat([_bf(w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], w.shape[2] * w.shape[3], w.shape[1]))
+    return torch.cat([_pk(w.detach().permute(0, 2, 3, 1).reshape(w.shape[0], w.shape[2] * w.shape[3], w.shape[1]), dtype)
                       for w in ws], 0).contiguous()
 
 
@@ -344,9 +506,9 @@ def pack_conv_weight_dgrad(*ws):
     return pack_conv_weight(w.flip(2, 3).transpose(0, 1).contiguous())
 
 
-def pack_dw_weight(w):
+def pack_dw_weight(w, dtype=torch.bfloat16):
     c, _, kh, kw = w.shape
-    return _bf(w.detach().reshape(c, kh * kw).t()).contiguous()
+    return _pk(w.detach().reshape(c, kh * kw).t(), dtype).contiguous()
 
 
 def stats_num_partials(n, hw):
@@ -354,16 +516,22 @@ def stats_num_partials(n, hw):
 
 
 def channel_stats(x, partials):
+    """one partial row per image (stats_num_partials: image-major rows, the same number per image, as the library)"""
+    _require(partials.shape[0] >= stats_num_partials(x.n, x.h * x.w), "channel_stats: too few partial rows")
     t = _nchw(x)
-    partials[:, 0] = t.sum((2, 3))
-    partials[:, 1] = t.pow(2).sum((2, 3))
+    partials[:x.n, 0] = t.sum((2, 3))
+    partials[:x.n, 1] = t.pow(2).sum((2, 3))
 
 
 def bn_finalize(partials, p_split, groups, count, gamma, beta, rmean, rvar, nbt, momentum, eps, scale, shift):
+    """group 0 = partial rows [0, p_split), group 1 = the rest; ``count`` is the pixel count of EACH group"""
+    _require(groups in (1, 2), f"bn_finalize: groups={groups}")
+    _require(partials.shape[0] > 0 and count > 0 and gamma.numel() > 0, "bn_finalize: empty input")
+    _require(groups == 1 or 0 < p_split < partials.shape[0], f"bn_finalize: p_split={p_split} of {partials.shape[0]}")
     for gi in range(groups):
         rows = partials[:p_split] if (gi == 0 and groups == 2) else (partials[p_split:] if groups == 2 else partials)
         s1, s2 = rows[:, 0].sum(0), rows[:, 1].sum(0)
-        cnt = count if gi == 0 else count * (partials.shape[0] - p_split) / max(p_split, 1)
+        cnt = count
         mean = s1 / cnt
         var = (s2 / cnt - mean * mean).clamp_min(0)
         sc = gamma.detach().float() * (var + eps).rsqrt()
@@ -378,12 +546,12 @@ def bn_finalize(partials, p_split, groups, count, gamma, beta, rmean, rvar, nbt,
     PTRS[shift.data_ptr()] = shift
 
 
-def pack_stem_weight(w):
+def pack_stem_weight(w, dtype=torch.bfloat16):
     """mode 2"""
     o = w.shape[0]
     p = torch.zeros((o, 3, 4, 16), dtype=torch.float32)
     p[:, :, :3, :12] = w.detach().permute(0, 2, 3, 1).float()
-    return _bf(p.reshape(o, 3, 64)).contiguous()
+    return _pk(p.reshape(o, 3, 64), dtype).contiguous()
 
 
 def install(monkeypatch, exact=False):

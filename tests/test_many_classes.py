@@ -177,7 +177,7 @@ def install(monkeypatch):
     def wide(grad_raw, cf, rf, dcf, drf, w_reg, w_obj, w_cls, *a, **kw):
         assert 1 <= w_cls.shape[0] <= 251 and (5 + w_cls.shape[0]) * cf.c * 4 <= 200 * 1024
         calls.append(("wide", w_cls.shape[0]))
-        emul_ops.head_pred_backward(grad_raw, cf, rf, dcf, drf, w_reg, w_obj, w_cls, *a, **kw)
+        emul_ops.head_pred_backward_wide(grad_raw, cf, rf, dcf, drf, w_reg, w_obj, w_cls, *a, **kw)
 
     monkeypatch.setattr(ops, "head_pred_backward", narrow)
     monkeypatch.setattr(ops, "head_pred_backward_wide", wide)

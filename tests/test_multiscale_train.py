@@ -65,20 +65,11 @@ def test_eager_steps_at_two_sizes_match_fp32_oracle(monkeypatch):
     assert tr.updates == 3
 
 
-def _resize_emul(x, size, out=None):
-    y = F.interpolate(x, size=size, mode="bilinear", align_corners=False)
-    if out is None:
-        return y
-    out.copy_(y)
-    return out
-
-
 @pytest.mark.parametrize("still", [False, True], ids=["pair", "still"])
 def test_preprocess_is_the_cfg_preprocess(still, monkeypatch):
     """data.preprocess (resize into the static input, labels copied then rescaled) == the cfgs' Exp.preprocess
     (F.interpolate + in-place label scaling of targets[0] and targets[1]); at input_size nothing runs"""
     emul_ops.install(monkeypatch, exact=True)
-    monkeypatch.setattr(ops, "resize_bilinear", _resize_emul)
     b, inp = 3, (120, 192)
     x = synth.synth_frames(b, *inp)[:, :3 if still else 6].contiguous()
     fut, cur = synth.synth_labels(b, *inp)

@@ -2,7 +2,7 @@
 
 CPU (no GPU needed):
   * the tick the graph captures, run under the torch emulation of the kernels (tests/emul_ops.py, fp32 storage) with the
-    per-stream resize, the start / keep gate, the per-image select, the NMS and the box division emulated here, reproduces
+    per-stream resize, the start / keep gate, the per-image select, the NMS and the box division emulated too, reproduces
     the fp32 oracle's on_pipe forward per stream -- the star call for a stream that starts a sequence, the buffered call
     otherwise -- over a sequence with mixed resets;
   * the host's output conversion and the argument checks;
@@ -54,62 +54,12 @@ def same_dets(a, b):
 TINY = CASES["tiny_120x160"]
 
 
-def _letterbox_sized(src, table, out):
-    """what sy_letterbox_sized does for rows of the driver's size: the streaming driver's preproc of each frame"""
-    for i, (h, w, dh, dw) in enumerate(table.tolist()):
-        assert (dh, dw) == tuple(out.shape[2:])
-        out[i] = torch.from_numpy(input_oracle.stream_frame(src[i, :h, :w].numpy(), (dh, dw))[0])
-
-
-def _stream_gate(status, flags, start, keep):
-    """what sy_stream_gate does"""
-    ok = torch.ones_like(flags) if status is None else (status == 0).to(torch.int32)
-    start.copy_(ok * (flags != 0).to(torch.int32))
-    keep.copy_(ok)
-
-
-def _stream_rescale(det, count, status, ratio):
-    """what sy_stream_rescale does"""
-    for i in range(det.shape[0]):
-        if status is not None and int(status[i]) != 0:
-            count[i] = 0
-        else:
-            det[i, :int(count[i]), :4] /= ratio[i]
-
-
-def _select_images(srcs, dsts, flags):
-    """what sy_select_images does"""
-    assert 1 <= len(srcs) == len(dsts) <= 3
-    for s, d in zip(srcs, dsts):
-        for i in range(s.n):
-            if int(flags[i]):
-                d.torch()[i].copy_(s.torch()[i])
-
-
-def _postprocess_nms(pred, num_classes, conf_thre, nms_thre, class_agnostic=False, max_det=None):
-    """what sy_postprocess_nms writes, from the NMS oracle"""
-    b, a, _ = pred.shape
-    max_det = a if max_det is None else max_det
-    det = torch.zeros((b, max_det, 7))
-    count = torch.zeros((b,), dtype=torch.int32)
-    for i, d in enumerate(postprocess_oracle(pred, num_classes, conf_thre, nms_thre, class_agnostic)):
-        if d is not None:
-            det[i, :len(d)] = d
-            count[i] = len(d)
-    return det, count
-
-
 def test_tick_follows_oracle_on_pipe_per_stream_and_divides_boxes(monkeypatch):
     """three streams over four ticks (tick 0: every stream starts; tick 2: stream 1 restarts; tick 3: streams 0 and 2): each
     stream's head outputs equal the fp32 oracle's on_pipe call on that stream alone -- star after a reset, buffered on the
     stream's previous frame otherwise -- to float roundoff, and the buffered streams really differ from a star call"""
     from test_fp16_storage import calibrated_oracle, product_from
     emul_ops.install(monkeypatch, exact=True)
-    monkeypatch.setattr(ops, "letterbox_sized", _letterbox_sized)
-    monkeypatch.setattr(ops, "stream_gate", _stream_gate)
-    monkeypatch.setattr(ops, "select_images", _select_images)
-    monkeypatch.setattr(ops, "postprocess_nms", _postprocess_nms)
-    monkeypatch.setattr(ops, "stream_rescale", _stream_rescale)
     x = synth.synth_frames(TINY["B"], TINY["H"], TINY["W"])
     o = calibrated_oracle(TINY, x, synth.synth_labels(TINY["B"], TINY["H"], TINY["W"]), None)
     m = product_from(o, TINY)

@@ -631,33 +631,10 @@ def test_install_trainer_finds_an_exps_package_on_disk(tmp_path):
     assert r.returncode == 0 and "ok" in r.stdout, r.stderr
 
 
-def _emulated_guard(monkeypatch):
-    """the new kernel modes in torch: sy_nonfinite_flag and the step's skip-with-EMA (found_inf_ema)"""
-    base = emul_ops.sgd_nesterov_ema_step
-
-    def sgd(param, grad, momentum_buf, ema, n_param, decay_begin, lr, momentum=0.9, weight_decay=5e-4, inv_scale=1.0,
-            nesterov=True, ema_decay=0.0, found_inf=None, hyper=None, found_inf_ema=False):
-        if found_inf is not None and float(found_inf) != 0.0 and found_inf_ema:
-            d = float(hyper[4]) if hyper is not None else ema_decay
-            if ema is not None:
-                ema.mul_(d).add_((1.0 - d) * param)
-            return
-        base(param, grad, momentum_buf, ema, n_param, decay_begin, lr, momentum, weight_decay, inv_scale, nesterov,
-             ema_decay, found_inf, hyper)
-
-    def flag(x, f, count):
-        f.fill_(float(not bool(torch.isfinite(x).all())))
-        count.add_(f.to(torch.int32))
-
-    monkeypatch.setattr(ops, "sgd_nesterov_ema_step", sgd)
-    monkeypatch.setattr(ops, "nonfinite_flag", flag)
-
-
 def test_skip_with_ema_is_sgd_skipped_plus_model_ema_update(monkeypatch):
     """a flagged step: parameters and momentum as torch SGD leaves them when GradScaler skips it, the EMA as
     ModelEMA.update; a finite step with the guard as without it"""
-    emul_ops.install(monkeypatch, exact=True)
-    _emulated_guard(monkeypatch)
+    emul_ops.install(monkeypatch, exact=True)        # with sy_nonfinite_flag and the step's skip-with-EMA (found_inf_ema)
     from test_cpu_backward import build_product
     ref = build_product(TINY)
     opt = train.build_optimizer(ref, 0.01)
