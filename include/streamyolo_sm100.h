@@ -647,6 +647,20 @@ typedef struct SyLetterboxSizedDesc {
   float* out;              /* [n][3][out_h][out_w] */
 } SyLetterboxSizedDesc;
 int sy_letterbox_sized(const SyLetterboxSizedDesc* d, sy_stream_t stream);
+/* The same resize into uint8 frames: frame k of sizes[k] = (h, w, dst_h, dst_w) at the top-left of slot k of src is
+ * resized h x w -> dst_h x dst_w with sy_letterbox's arithmetic (cv2.resize INTER_LINEAR on uint8, bit for bit; a copy
+ * when equal) into the top-left of slot k of out [n][out_h][out_w][3], channel order kept: mmcv.imrescale(img, s,
+ * interpolation="bilinear") with dst = (int(h * s + 0.5), int(w * s + 0.5)).  The rest of each out slot is not written;
+ * a row that does not fit the slots leaves out slot k untouched.  SY_EINVAL: a null pointer, src == out, or a side
+ * outside 1..65535 or a slot of 2^31 bytes or more. */
+typedef struct SyResizeSizedDesc {
+  const uint8_t* src;      /* [n][slot_h][slot_w][3] */
+  int32_t n, slot_h, slot_w;
+  const int32_t* sizes;    /* [n][4] device int32: h, w, dst_h, dst_w */
+  int32_t out_h, out_w;
+  uint8_t* out;            /* [n][out_h][out_w][3] */
+} SyResizeSizedDesc;
+int sy_resize_sized(const SyResizeSizedDesc* d, sy_stream_t stream);
 
 /* ---- Raw camera frames ----
  * YUV frames of camera streams of different sizes -> uint8 BGR frames at the top-left of slots of one size (the slots
@@ -819,6 +833,35 @@ typedef struct SyVisDetBoxesDesc {
   int32_t* counts;          /* [S] */
 } SyVisDetBoxesDesc;
 int sy_vis_det_boxes(const SyVisDetBoxesDesc* d, sy_stream_t stream);
+
+/* sy_draw_outlines: the drawing of the sAP toolkit's vis_det (sAP/det/__init__.py:103-175, masks None) on n uint8
+ * images of their own sizes, in place: image i is sizes[i] = (h, w) at the top-left of slot i of img [n][max_h][max_w][3].
+ * Every pixel of
+ *   - the first counts[i] boxes of row i (x1, y1, x2, y2, already rounded; corners in any order): the four 1-pixel lines
+ *     cv2.rectangle(img, (x1, y1), (x2, y2), color, thickness=1) draws, [min x, max x] x {y1, y2} and
+ *     {x1, x2} x [min y, max y], clipped to the image;
+ *   - the first n_points[i] entries of row i of points: pixel y * w + x of image i (the host's cv2.putText strokes),
+ *     entries outside [0, h * w) ignored;
+ * becomes ``color`` (3 values in the images' channel order).  Every touched pixel gets the same colour, so the result is
+ * the union of the touched pixels whatever the order of the writes.  Pixels outside an image and pixels nothing touches
+ * are not written; counts and n_points are clamped to [0, K] and [0, M]; an image whose size row is below 1 or outside
+ * the slot is left alone.  Sizes, boxes, counts, points and n_points are read on the device only, so a captured graph
+ * follows what is written before each replay.  SY_EINVAL: a null pointer, n or a slot side outside 1..65535, a slot of
+ * 2^31 pixels or more, K or M outside 1..2^24. */
+typedef struct SyDrawOutlinesDesc {
+  uint8_t* img;             /* [n][max_h][max_w][3], drawn in place */
+  const int32_t* sizes;     /* [n][2] device int32: h, w */
+  int32_t n;
+  int32_t max_h, max_w;     /* slot size */
+  const int32_t* boxes;     /* [n][K][4] x1, y1, x2, y2 */
+  const int32_t* counts;    /* [n] */
+  int32_t K;
+  const int32_t* points;    /* [n][M] pixel indices y * w + x */
+  const int32_t* n_points;  /* [n] */
+  int32_t M;
+  uint8_t color[3];
+} SyDrawOutlinesDesc;
+int sy_draw_outlines(const SyDrawOutlinesDesc* d, sy_stream_t stream);
 
 /* sy_splice_frames: the split screen of the sAP toolkit's vis_contrast.py (sAP/vis/vis_contrast.py:148-165) on n pairs of
  * uint8 images of their own sizes, written into A in place: image i is sizes[i] = (h, w) at the top-left of slot i of a

@@ -36,6 +36,7 @@ SOURCES = {
     "yuv.cu": [],
     "jpeg_encode.cu": [],
     "vis.cu": [],
+    "vis_det.cu": [],
     "contrast.cu": [],
 }
 

@@ -9,6 +9,7 @@
 //                      driver's preproc (sAP/streamyolo/streamyolo_det.py:57-60).
 //   * sy_letterbox_sized  the same resize with a source size and a resized extent per frame, the frames in slots of one
 //                      size: the evaluation preproc (data_augment_flip.py:151-167) of camera streams of different sizes.
+//   * sy_resize_sized  that resize into uint8 slots, no pad: mmcv.imrescale(bilinear) of the sAP toolkit's vis_det.
 // Built with -fmad=false: the tap positions (x + 0.5) * scale - 0.5 and the fp64 label arithmetic must round every
 // operation separately, as OpenCV and numpy do.  The output is then bit-identical to cv2 / numpy.
 #include <math.h>
@@ -140,6 +141,27 @@ __global__ void __launch_bounds__(128) letterbox_sized_kernel(const uint8_t* __r
   o[0] = (float)p[0];
   o[plane] = (float)p[1];
   o[2 * plane] = (float)p[2];
+}
+
+// The same resize into uint8 slots (mmcv.imrescale of the sAP toolkit's vis_det): frame k resized to dst_h x dst_w at the
+// top-left of out slot k, channel order kept, the rest of the slot not written.
+__global__ void __launch_bounds__(128) resize_sized_kernel(const uint8_t* __restrict__ src, int slot_h, int slot_w,
+                                                           const int32_t* __restrict__ sizes, int out_h, int out_w,
+                                                           uint8_t* __restrict__ out) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y, k = blockIdx.z;
+  const int h = sizes[4 * k], w = sizes[4 * k + 1], dh = sizes[4 * k + 2], dw = sizes[4 * k + 3];
+  if (h < 1 || w < 1 || h > slot_h || w > slot_w || dh < 1 || dw < 1 || dh > out_h || dw > out_w) return;
+  if (y >= dh || x >= dw) return;
+  const ResizeStage a{h, slot_w, h, w, 1.0, 1.0};  // no first stage: only the row pitch (slot_w pixels) is read
+  const ResizeStage b{h, w, dh, dw, 1.0 / ((double)dh / h), 1.0 / ((double)dw / w)};
+  const uint8_t* img = src + (long long)slot_h * slot_w * 3 * k;
+  int p[3];
+  if (dh != h || dw != w) letterbox_px<false, true>(img, a, b, false, y, x, p);
+  else letterbox_px<false, false>(img, a, b, false, y, x, p);
+  uint8_t* o = out + (((long long)k * out_h + y) * out_w + x) * 3;
+  o[0] = (uint8_t)p[0];
+  o[1] = (uint8_t)p[1];
+  o[2] = (uint8_t)p[2];
 }
 
 // One warp per (pair, frame).  Rows are x1, y1, x2, y2, cls in fp64; output rows cls, cx, cy, w, h in fp32.
@@ -275,4 +297,19 @@ extern "C" int sy_letterbox_sized(const SyLetterboxSizedDesc* d, sy_stream_t str
   const dim3 grid(cdiv(d->out_w, 128), d->out_h, d->n);
   letterbox_sized_kernel<<<grid, 128, 0, stream>>>(d->src, d->slot_h, d->slot_w, d->sizes, d->out_h, d->out_w, d->out);
   return launch_status("letterbox_sized_kernel");
+}
+
+extern "C" int sy_resize_sized(const SyResizeSizedDesc* d, sy_stream_t stream_) {
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  SY_REQUIRE(d != nullptr && d->src != nullptr && d->sizes != nullptr && d->out != nullptr, SY_EINVAL,
+             "resize_sized: null pointer");
+  SY_REQUIRE(d->src != d->out, SY_EINVAL, "resize_sized: src and out must be different buffers");
+  SY_REQUIRE(d->n > 0 && d->n <= 65535 && d->slot_h > 0 && d->slot_w > 0 && d->slot_h <= 65535 && d->slot_w <= 65535 &&
+                 d->out_h > 0 && d->out_w > 0 && d->out_h <= 65535 && d->out_w <= 65535,
+             SY_EINVAL, "resize_sized: bad sizes");
+  SY_REQUIRE((long long)d->slot_h * d->slot_w * 3 < (1ll << 31) && (long long)d->out_h * d->out_w * 3 < (1ll << 31),
+             SY_EINVAL, "resize_sized: slot too large");
+  const dim3 grid(cdiv(d->out_w, 128), d->out_h, d->n);
+  resize_sized_kernel<<<grid, 128, 0, stream>>>(d->src, d->slot_h, d->slot_w, d->sizes, d->out_h, d->out_w, d->out);
+  return launch_status("resize_sized_kernel");
 }

@@ -453,6 +453,111 @@ def draw_boxes(frames, boxes, labels, counts, palette, sizes=None, out=None):
     return ops.draw_boxes(frames, sizes, boxes, labels, counts, pal, frames if out is None else out)
 
 
+def imrescale_size(h, w, scale):
+    """The (h, w) mmcv.imrescale(img, scale) gives an h x w image (mmcv.image.rescale_size with a number:
+    ``int(w * scale + 0.5), int(h * scale + 0.5)``); ValueError for a scale <= 0, as mmcv raises, and for an empty result,
+    which cv2.resize refuses."""
+    if not scale > 0:
+        raise ValueError(f"Invalid scale {scale}, must be positive.")
+    out = int(h * float(scale) + 0.5), int(w * float(scale) + 0.5)
+    if min(out) < 1:
+        raise ValueError(f"imrescale: a {h}x{w} image at scale {scale} is empty ({out[0]}x{out[1]})")
+    return out
+
+
+def resize_sized(frames, sizes, dst_sizes, out_hw=None, out=None):
+    """Resize frames of different sizes as cv2.resize(img, (dst_w, dst_h), interpolation=INTER_LINEAR) does, bit for bit
+    (sy_resize_sized; mmcv.imrescale's bilinear resize with ``dst_sizes`` from imrescale_size).
+
+    frames    uint8 CUDA [n, slot_h, slot_w, 3] slots (decode_jpeg_sized's output), channel order kept
+    sizes     each frame's (h, w) at the top-left of its slot; dst_sizes: each frame's (dst_h, dst_w)
+    out_hw    the output slots' (h, w): the largest dst size by default
+    out       uint8 [n, out_h, out_w, 3] to write into; with it and an int32 CUDA [n, 4] ``sizes`` table (h, w, dst_h,
+              dst_w; ``dst_sizes`` None) the call only enqueues (capturable)
+
+    -> ``out``: frame i at the top-left of slot i; the rest of each slot is not written."""
+    ops._require(torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+                 and frames.is_contiguous() and frames.is_cuda,
+                 "resize_sized: frames must be a contiguous CUDA uint8 [n, slot_h, slot_w, 3] tensor")
+    n, sh, sw, _ = frames.shape
+    dev = frames.device
+    if torch.is_tensor(sizes):
+        ops._require(dst_sizes is None, "resize_sized: with a sizes table, give no dst_sizes")
+        table = sizes
+    else:
+        src, dst = _sizes_list(sizes, "resize_sized"), _sizes_list(dst_sizes, "resize_sized")
+        ops._require(len(src) == n and len(dst) == n, f"resize_sized: give {n} sizes and {n} dst sizes")
+        for i, (h, w) in enumerate(src):
+            ops._require(h <= sh and w <= sw, f"resize_sized: frame {i} of {h}x{w} is larger than the {sh}x{sw} slot")
+        table = torch.tensor([s + d for s, d in zip(src, dst)], dtype=torch.int32)
+        if out_hw is None and out is None:
+            out_hw = (max(h for h, _ in dst), max(w for _, w in dst))
+        if out is not None:
+            out_hw = tuple(out.shape[1:3])
+        for i, (h, w) in enumerate(dst):
+            ops._require(h <= out_hw[0] and w <= out_hw[1], f"resize_sized: frame {i} resized to {h}x{w} is larger "
+                         f"than the {out_hw[0]}x{out_hw[1]} output slot")
+    if out is None:
+        ops._require(out_hw is not None, "resize_sized: give out_hw or out")
+        out = torch.empty((n, int(out_hw[0]), int(out_hw[1]), 3), dtype=torch.uint8, device=dev)
+    return ops.resize_sized(frames, table.to(dev).contiguous(), out)
+
+
+# vis_det's box and text colour (0, 255, 0): the same in RGB and BGR order
+VIS_DET_GREEN = (0, 255, 0)
+
+
+def draw_outlines(frames, boxes, points, sizes=None, counts=None, n_points=None, color=VIS_DET_GREEN):
+    """Draw detections as the sAP toolkit's vis_det does (sAP/det/__init__.py:152-174; sy_draw_outlines), in place:
+    each box as cv2.rectangle(img, (x1, y1), (x2, y2), color, thickness=1) draws it, and the listed pixels (the label
+    text the host rasterised with cv2.putText) in the same colour.
+
+    frames    uint8 CUDA [n, h, w, 3]; or slots [n, max_h, max_w, 3] with ``sizes``
+    boxes     int32 [n, K, 4] x1, y1, x2, y2, already rounded (vis_det's ``bboxes.round().astype(np.int32)``), with
+              ``counts``; or a list of n [k_i, 4] arrays
+    points    int32 [n, M] pixel indices y * w + x within each frame, with ``n_points``; or a list of n index arrays
+    sizes     each frame's (h, w) at the top-left of its slot: host pairs or an int32 CUDA [n, 2] tensor
+    color     3 values in the frames' channel order
+
+    With every argument a CUDA tensor the call only enqueues the kernel (capturable in a CUDA graph, which then follows
+    what is written to the tensors before each replay); host arguments are copied to the device (no synchronisation).
+    Only the pixels a box or a listed index touches are written.  -> ``frames``."""
+    ops._require(torch.is_tensor(frames) and frames.dtype == torch.uint8 and frames.dim() == 4 and frames.shape[3] == 3
+                 and frames.is_contiguous() and frames.is_cuda,
+                 "draw_outlines: frames must be a contiguous CUDA uint8 [n, h, w, 3] tensor")
+    n, mh, mw, _ = frames.shape
+    dev = frames.device
+
+    def rows(v, c, width, what):
+        if torch.is_tensor(v):
+            ops._require(torch.is_tensor(c), f"draw_outlines: give {what} counts with a {what} tensor")
+            return v, c
+        ops._require(c is None and len(v) == n, f"draw_outlines: give {n} {what} arrays and no counts")
+        arrs = [np.asarray(a, np.int64).reshape((-1, 4) if width == 4 else (-1,)) for a in v]
+        ops._require(all(a.size == 0 or (a.min() >= -2 ** 31 and a.max() < 2 ** 31) for a in arrs),
+                     f"draw_outlines: {what} must be int32 values")
+        k = max([1] + [len(a) for a in arrs])
+        packed = np.zeros((n, k, 4) if width == 4 else (n, k), np.int32)
+        for i, a in enumerate(arrs):
+            packed[i, :len(a)] = a
+        return torch.from_numpy(packed), torch.tensor([len(a) for a in arrs], dtype=torch.int32)
+
+    boxes, counts = rows(boxes, counts, 4, "box")
+    points, n_points = rows(points, n_points, 1, "point")
+    if sizes is None:
+        sizes = [(mh, mw)] * n
+    if not torch.is_tensor(sizes):
+        hw = _sizes_list(sizes, "draw_outlines")
+        ops._require(len(hw) == n, f"draw_outlines: {len(hw)} sizes for {n} frames")
+        for i, (h, w) in enumerate(hw):
+            ops._require(h <= mh and w <= mw, f"draw_outlines: frame {i} of {h}x{w} is larger than the {mh}x{mw} slot")
+        sizes = torch.tensor(hw, dtype=torch.int32)
+    boxes, counts, points, n_points, sizes = (t.to(dev).contiguous() for t in (boxes, counts, points, n_points, sizes))
+    if boxes.data_ptr() % 16:
+        boxes = boxes.clone()
+    return ops.draw_outlines(frames, sizes, boxes, counts, points, n_points, color)
+
+
 # the band colour of the sAP toolkit's vis_contrast.py (RGB [241, 159, 93], :106) in BGR order
 CONTRAST_BAND_BGR = (93, 159, 241)
 

@@ -152,6 +152,11 @@ class SyLetterboxSizedDesc(C.Structure):
                 ("sizes", C.c_void_p), ("out_h", C.c_int32), ("out_w", C.c_int32), ("out", C.c_void_p)]
 
 
+class SyResizeSizedDesc(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("n", C.c_int32), ("slot_h", C.c_int32), ("slot_w", C.c_int32), ("sizes", C.c_void_p),
+                ("out_h", C.c_int32), ("out_w", C.c_int32), ("out", C.c_void_p)]
+
+
 class SyYuvToBgrSizedDesc(C.Structure):
     _fields_ = [("src", C.c_void_p), ("n", C.c_int32), ("max_bytes", C.c_int64), ("sizes", C.c_void_p),
                 ("format", C.c_int32), ("slot_h", C.c_int32), ("slot_w", C.c_int32), ("out", C.c_void_p)]
@@ -167,6 +172,12 @@ class SyDrawBoxesDesc(C.Structure):
     _fields_ = [("src", C.c_void_p), ("sizes", C.c_void_p), ("n", C.c_int32), ("max_h", C.c_int32), ("max_w", C.c_int32),
                 ("boxes", C.c_void_p), ("labels", C.c_void_p), ("counts", C.c_void_p), ("K", C.c_int32),
                 ("palette", C.c_void_p), ("P", C.c_int32), ("dst", C.c_void_p), ("dst_h", C.c_int32), ("dst_w", C.c_int32)]
+
+
+class SyDrawOutlinesDesc(C.Structure):
+    _fields_ = [("img", C.c_void_p), ("sizes", C.c_void_p), ("n", C.c_int32), ("max_h", C.c_int32), ("max_w", C.c_int32),
+                ("boxes", C.c_void_p), ("counts", C.c_void_p), ("K", C.c_int32), ("points", C.c_void_p),
+                ("n_points", C.c_void_p), ("M", C.c_int32), ("color", C.c_uint8 * 3)]
 
 
 class SyVisDetBoxesDesc(C.Structure):
@@ -286,6 +297,7 @@ _SIG = {
     "sy_frame_labels": (C.c_int, [C.POINTER(SyFrameLabelsDesc), C.c_void_p]),
     "sy_letterbox": (C.c_int, [C.POINTER(SyLetterboxDesc), C.c_void_p]),
     "sy_letterbox_sized": (C.c_int, [C.POINTER(SyLetterboxSizedDesc), C.c_void_p]),
+    "sy_resize_sized": (C.c_int, [C.POINTER(SyResizeSizedDesc), C.c_void_p]),
     "sy_jpeg_decode_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
     "sy_jpeg_decode": (C.c_int, [C.POINTER(SyJpegDecodeDesc), C.c_void_p]),
     "sy_jpeg_decode_sized_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
@@ -296,6 +308,7 @@ _SIG = {
     "sy_jpeg_encode": (C.c_int, [C.POINTER(SyJpegEncodeDesc), C.c_void_p]),
     "sy_draw_boxes": (C.c_int, [C.POINTER(SyDrawBoxesDesc), C.c_void_p]),
     "sy_vis_det_boxes": (C.c_int, [C.POINTER(SyVisDetBoxesDesc), C.c_void_p]),
+    "sy_draw_outlines": (C.c_int, [C.POINTER(SyDrawOutlinesDesc), C.c_void_p]),
     "sy_splice_frames": (C.c_int, [C.POINTER(SySpliceFramesDesc), C.c_void_p]),
 }
 EXPORTED_SYMBOLS = tuple(_SIG)
@@ -1103,6 +1116,23 @@ def letterbox_sized(src, sizes, out):
     _check(lib().sy_letterbox_sized(C.byref(d), _stream()))
 
 
+def resize_sized(src, sizes, out):
+    """uint8 [n, slot_h, slot_w, 3] slots -> uint8 [n, out_h, out_w, 3] ``out`` slots (sy_resize_sized): frame k of
+    ``sizes[k]`` = (h, w, dst_h, dst_w) (int32 [n, 4] on the device) at the slot's top-left, cv2-exact INTER_LINEAR resize
+    to dst at the top-left of out slot k; the rest of ``out`` is not written.  Enqueues only (capturable)."""
+    _require(_tensor_ok(src, torch.uint8, 4) and src.shape[3] == 3 and src.is_cuda,
+             "resize_sized: frames must be contiguous CUDA uint8 [n, slot_h, slot_w, 3]")
+    n, sh, sw, _ = src.shape
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 4) and sizes.device == src.device,
+             f"resize_sized: sizes must be int32 [{n}, 4] on the frames' device")
+    _require(_tensor_ok(out, torch.uint8, 4) and out.shape[0] == n and out.shape[3] == 3 and out.device == src.device
+             and out.data_ptr() != src.data_ptr(), f"resize_sized: out must be another contiguous uint8 [{n}, H, W, 3] "
+             "on the frames' device")
+    d = SyResizeSizedDesc(src.data_ptr(), n, sh, sw, sizes.data_ptr(), out.shape[1], out.shape[2], out.data_ptr())
+    _check(lib().sy_resize_sized(C.byref(d), _stream()))
+    return out
+
+
 class PackBatch:
     """Every conv operand of a model re-packed in ONE launch (sy_pack_conv_weights_batch).  ``add`` the (fp32 parameter,
     bf16 destination, layout) pairs once -- the tensors must keep their addresses -- then ``run()`` after every update."""
@@ -1299,6 +1329,34 @@ def vis_det_boxes(det, count, score_th, boxes=None, labels=None, counts=None):
                           labels.data_ptr(), counts.data_ptr())
     _check(lib().sy_vis_det_boxes(C.byref(d), _stream()))
     return boxes, labels, counts
+
+
+def draw_outlines(img, sizes, boxes, counts, points, n_points, color):
+    """The drawing of the sAP toolkit's vis_det (sAP/det/__init__.py:152-174) on n images of their own sizes, in place
+    (sy_draw_outlines): ``img`` uint8 [n, max_h, max_w, 3], image i of ``sizes[i]`` = (h, w) (int32 [n, 2]) at the
+    top-left of slot i; the 1-pixel rectangles of the first counts[i] boxes of ``boxes`` (int32 [n, K, 4] x1, y1, x2, y2,
+    rounded) and the pixels y * w + x of the first n_points[i] entries of ``points`` (int32 [n, M]) become ``color`` (3
+    values in the images' channel order).  Only those pixels are written.  Enqueues only (capturable)."""
+    _require(_tensor_ok(img, torch.uint8, 4) and img.shape[3] == 3 and img.is_cuda,
+             "draw_outlines: img must be contiguous CUDA uint8 [n, max_h, max_w, 3]")
+    n, mh, mw, _ = img.shape
+    dev = img.device
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 2) and sizes.device == dev,
+             f"draw_outlines: sizes must be int32 [{n}, 2] on img's device")
+    _require(_tensor_ok(boxes, torch.int32, 3) and boxes.shape[0] == n and boxes.shape[2] == 4 and boxes.shape[1] >= 1
+             and boxes.device == dev and boxes.data_ptr() % 16 == 0,
+             f"draw_outlines: boxes must be contiguous 16-byte aligned int32 [{n}, K, 4] on img's device")
+    _require(_tensor_ok(points, torch.int32, 2) and points.shape[0] == n and points.shape[1] >= 1 and points.device == dev,
+             f"draw_outlines: points must be contiguous int32 [{n}, M] on img's device")
+    for name, t in (("counts", counts), ("n_points", n_points)):
+        _require(_tensor_ok(t, torch.int32, 1) and t.shape[0] == n and t.device == dev,
+                 f"draw_outlines: {name} must be int32 [{n}] on img's device")
+    col = [int(c) for c in color]
+    _require(len(col) == 3 and all(0 <= c <= 255 for c in col), "draw_outlines: color must be 3 values in 0..255")
+    d = SyDrawOutlinesDesc(img.data_ptr(), sizes.data_ptr(), n, mh, mw, boxes.data_ptr(), counts.data_ptr(),
+                           boxes.shape[1], points.data_ptr(), n_points.data_ptr(), points.shape[1], (C.c_uint8 * 3)(*col))
+    _check(lib().sy_draw_outlines(C.byref(d), _stream()))
+    return img
 
 
 def splice_frames(a, b, sizes, splits, horizontal, color):
