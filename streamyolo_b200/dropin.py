@@ -19,7 +19,7 @@ _EVALUATORS = (("onex_stream_evaluator", "ONEX_COCOEvaluator", "onex"), ("twox_s
                ("still_stream_evaluator", "STILL_COCOEvaluator", "still"))
 
 
-def install(postprocess: bool = True, evaluators: bool = False, trainer: bool = False) -> None:
+def install(postprocess: bool = True, evaluators: bool = False, trainer: bool = False, virtual_ranks: int = 1) -> None:
     """``postprocess=True`` also points ``yolox.utils.postprocess`` (imported by the reference's evaluators,
     exps/evaluators/onex_stream_evaluator.py:14,148) at the device NMS when the yolox package is importable.
 
@@ -31,7 +31,9 @@ def install(postprocess: bool = True, evaluators: bool = False, trainer: bool = 
     ``trainer=True`` replaces ``exps.train_utils.double_trainer.Trainer`` (what every shipped cfg's ``get_trainer``
     imports) by a subclass whose loop runs on the device (``streamyolo_b200.train_loop``): JPEG files in, one CUDA graph
     replay per iteration.  Nothing happens when that module or yolox cannot be imported.  ``install(trainer=True,
-    evaluators=True)`` is the recommended pair for ``tools/train.py``: the per-epoch evaluation then runs on the device too."""
+    evaluators=True)`` is the recommended pair for ``tools/train.py``: the per-epoch evaluation then runs on the device too.
+    ``virtual_ranks=K`` (with ``trainer=True``): every process runs K ranks of a W x K-rank run one after another, so
+    ``tools/train.py -d 1 -b 32`` with K = 8 trains as the README's ``-d 8 -b 32`` does (``train_loop.DeviceTrainer``)."""
     pkg = importlib.import_module("streamyolo_b200.model")
     if "exps" not in sys.modules:
         if importlib.util.find_spec("exps") is not None:   # the reference checkout's own package: its exps.train_utils,
@@ -56,7 +58,7 @@ def install(postprocess: bool = True, evaluators: bool = False, trainer: bool = 
     if evaluators:
         install_evaluators()
     if trainer:
-        install_trainer()
+        install_trainer(virtual_ranks)
 
 
 def install_evaluators() -> None:
@@ -77,8 +79,10 @@ def install_evaluators() -> None:
             setattr(m, name, device_evaluator(base, rule))
 
 
-def install_trainer() -> None:
-    """The ``trainer=True`` part of ``install``; a second call changes nothing."""
+def install_trainer(virtual_ranks: int = 1) -> None:
+    """The ``trainer=True`` part of ``install``; a second call only sets ``virtual_ranks``."""
+    if int(virtual_ranks) != virtual_ranks or virtual_ranks < 1:
+        raise ValueError(f"install: virtual_ranks must be a positive integer, got {virtual_ranks!r}")
     try:
         import yolox  # noqa: F401
         m = importlib.import_module("exps.train_utils.double_trainer")
@@ -88,3 +92,5 @@ def install_trainer() -> None:
     base = getattr(m, "Trainer", None)
     if base is not None and not issubclass(base, DeviceTrainer):
         m.Trainer = device_trainer(base)
+    if base is not None:
+        m.Trainer.virtual_ranks = int(virtual_ranks)

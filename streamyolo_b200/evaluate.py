@@ -157,14 +157,19 @@ class DeviceEvaluator:
         if not all(-2 ** 31 <= int(c) < 2 ** 31 for c in ds.class_ids):
             raise ValueError("DeviceEvaluator: class ids must fit in int32")
         self.frames_per_image = RULES[self.rule]
-        self.batches = sampler_batches(dataloader)
+        self._use_batches(sampler_batches(dataloader))
+        self._rows = None
+        self.capture_seconds = None
+
+    def _use_batches(self, batches):
+        """the batches (dataset indices) the next evaluation runs, their one frame size and image-id table"""
+        ds = self.dataloader.dataset
+        self.batches = batches
         used = sorted({i for b in self.batches for i in b})
         self.frame_hw = feed.frame_size([ds.annotations[i] for i in used], self.frames_per_image, "DeviceEvaluator")
         self.ratio = min(self.img_size[0] / float(self.frame_hw[0]), self.img_size[1] / float(self.frame_hw[1]))
         images = None if self.rule == "still" else ds.coco.dataset["images"]
         self.table = dict(zip(used, image_id_table(images, [ds.ids[i] for i in used], self.rule).tolist()))
-        self._rows = None
-        self.capture_seconds = None
 
     def detections(self):
         """The rows of the last ``evaluate`` (after the gather, on rank 0 with several ranks) as numpy arrays: ``bbox`` fp32
@@ -194,6 +199,36 @@ class DeviceEvaluator:
         COCO rows; "NMS" is 0.  The "Average forward / NMS / inference time" line keeps its format."""
         if trt_file is not None or decoder is not None:
             raise NotImplementedError("DeviceEvaluator: trt_file and decoder are not supported")
+        rows, infer_ms = self._rows_of(model, half)
+        return self._score(rows, infer_ms, len(self.dataloader) - 1, distributed, next(model.parameters()).device)
+
+    def evaluate_virtual_ranks(self, model, load_rank, virtual_ranks, batch_size, distributed=False, half=False):
+        """``evaluate`` as a run of W x K ranks does it when this process runs K of them (``virtual_ranks``, W processes
+        when ``distributed``): virtual rank g = rank * K + k evaluates the indices ``DistributedSampler(num_replicas=W * K,
+        rank=g, shuffle=False)`` gives it, in batches of ``batch_size``, after ``load_rank(k)`` has put its weights into
+        ``model``; the rows are concatenated in rank order (gathered over the W processes) and scored once, and the
+        statistics are the sums over the W x K ranks.  The loader's own batches are evaluated again by ``evaluate``."""
+        import torch.distributed as dist
+        world, rank = (dist.get_world_size(), dist.get_rank()) if distributed else (1, 0)
+        ds, own = self.dataloader.dataset, self.batches
+        parts, infer_ms, n_batches = [], 0.0, 0
+        try:
+            for k in range(virtual_ranks):
+                sampler = torch.utils.data.distributed.DistributedSampler(ds, num_replicas=world * virtual_ranks,
+                                                                          rank=rank * virtual_ranks + k, shuffle=False)
+                idx = [int(i) for i in sampler]
+                self._use_batches([idx[i:i + batch_size] for i in range(0, len(idx), batch_size)])
+                load_rank(k)
+                rows, ms = self._rows_of(model, half)
+                parts.append(rows)
+                infer_ms += ms
+                n_batches += len(self.batches) - 1
+        finally:
+            self._use_batches(own)
+        return self._score(merge_ranks(parts), infer_ms, n_batches, distributed, next(model.parameters()).device)
+
+    def _rows_of(self, model, half):
+        """the rows of ``self.batches`` -> (rows, device ms of every replay but the last)"""
         model = model.eval()
         if half:
             model = model.half()
@@ -210,7 +245,11 @@ class DeviceEvaluator:
         self.capture_seconds = time.perf_counter() - t0
         rows, infer_ms = self._loop(graphs, max_bytes, device)
         del graphs
-        statistics = torch.tensor([infer_ms / 1000.0, 0.0, len(self.dataloader) - 1], dtype=torch.float32, device=device)
+        return rows, infer_ms
+
+    def _score(self, rows, infer_ms, n_batches, distributed, device):
+        """gather the rows of every process to rank 0 in rank order and score them (evaluate_prediction)"""
+        statistics = torch.tensor([infer_ms / 1000.0, 0.0, n_batches], dtype=torch.float32, device=device)
         if distributed:
             import torch.distributed as dist
             parts = [None] * dist.get_world_size() if dist.get_rank() == 0 else None

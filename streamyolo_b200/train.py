@@ -145,7 +145,11 @@ class FlatState:
     """Flat fp32 buffers holding the model's parameters (walk order), their gradients, momentum, and the EMA copy; re-points
     the module's tensors into them."""
 
-    def __init__(self, model, ema=True):
+    def __init__(self, model, ema=True, copies=1):
+        """``copies``: how many copies of the BatchNorm buffers the state holds, one per virtual rank (``Trainer``'s
+        ``virtual_ranks``).  Copy k of a float buffer sits ``k * n_buf`` floats after copy 0, so the fused step's EMA
+        covers every copy; ``num_batches_tracked`` gets one int64 copy per rank in ``int_bufs``.  The module's buffers
+        are views of the copy ``select`` chose last, copy 0 outside a step."""
         dev = next(model.parameters()).device
         groups = list(reversed(conv_groups_forward_order(model)))        # the order the walk finishes them in
         head = model.head
@@ -188,7 +192,8 @@ class FlatState:
         for b in bufs:
             place(b)
         cur = (cur + _ALIGN - 1) // _ALIGN * _ALIGN
-        self.n_total = cur
+        self.copies, self.n_buf = copies, cur - self.n_param
+        self.n_total = self.n_param + copies * self.n_buf
         self.state = torch.zeros(self.n_total, dtype=torch.float32, device=dev)
         self.grad = torch.zeros(self.n_param, dtype=torch.float32, device=dev)
         self.mom = torch.zeros(self.n_param, dtype=torch.float32, device=dev)
@@ -201,8 +206,34 @@ class FlatState:
             for p in params:
                 o, n = self.offset[id(p)]
                 p.grad = self.grad[o:o + n].view(p.shape)
+            for k in range(1, copies):
+                self.buffer_copy(k).copy_(self.buffer_copy(0))
+        self.bufs = bufs
+        self.int_bufs, self.int_copies = [], None
+        if copies > 1:
+            self.int_bufs = [b for b in model.buffers() if not b.dtype.is_floating_point]
+            self.int_copies = torch.stack([b.detach() for b in self.int_bufs]).repeat(copies, 1)
+        self.selected = 0
+        self.select(0)
         self.ema = self.state.clone() if ema else None
         self.params = params
+
+    def buffer_copy(self, k, buf=None):
+        """copy ``k`` of the float-buffer region of ``buf`` (default: ``state``), flat"""
+        buf = self.state if buf is None else buf
+        return buf[self.n_param + k * self.n_buf:self.n_param + (k + 1) * self.n_buf]
+
+    def select(self, k):
+        """point the module's BatchNorm buffers (running statistics, ``num_batches_tracked``) at copy ``k``: the kernels
+        read the buffer addresses when a launch is issued or recorded"""
+        self.selected = k
+        if self.copies == 1:
+            return
+        for b in self.bufs:
+            o, n = self.offset[id(b)]
+            b.data = self.state[o + k * self.n_buf:o + k * self.n_buf + n].view(b.shape)
+        for i, b in enumerate(self.int_bufs):
+            b.data = self.int_copies[k, i]
 
     def gview(self, p):
         o, n = self.offset[id(p)]
@@ -213,6 +244,9 @@ class FlatState:
         ``state``, e.g. ``ema``) as a view; the rest (num_batches_tracked) are the module's own tensors."""
         base = self.state.data_ptr()
         index = {base + 4 * o: (o, n) for (o, n) in self.offset.values()}
+        if self.copies > 1:                                              # the buffers of the selected copy
+            shift = self.selected * self.n_buf
+            index.update({base + 4 * (o + shift): (o + shift, n) for (o, n) in (self.offset[id(b)] for b in self.bufs)})
         out = {}
         for k, t in model.state_dict().items():
             hit = index.get(t.data_ptr()) if t.dtype == torch.float32 else None
@@ -250,6 +284,8 @@ class FlatSink:
         self.work = []
         self.launched = []
         self.on_bucket = None
+        self.accumulate_all = False         # begin(accumulate=True): every kernel adds onto the flat gradient
+        self.complete = True                # begin(complete=False): no bucket completes in this walk
 
     def _close(self, a, b, members):
         if not members:
@@ -261,7 +297,7 @@ class FlatSink:
 
     # ---- buffers for the kernels
     def _first(self, key):
-        acc = key in self.touched
+        acc = self.accumulate_all or key in self.touched
         self.touched.add(key)
         return acc
 
@@ -282,7 +318,7 @@ class FlatSink:
         ws = [self.fs.gview(p).view(p.shape[0], p.shape[1]) for p in (head.reg_preds[k].weight, head.obj_preds[k].weight,
                                                                       head.cls_preds[k].weight)]
         bs = [self.fs.gview(p) for p in (head.reg_preds[k].bias, head.obj_preds[k].bias, head.cls_preds[k].bias)]
-        return ws, bs, False
+        return ws, bs, self.accumulate_all
 
     # ---- completion tracking / communication
     def done(self, params):
@@ -299,11 +335,16 @@ class FlatSink:
                 if b[2] == 0 and self.overlap:
                     self._launch(b)
 
-    def begin(self, model):
-        """per step: how many launches contribute to each parameter (a module recorded twice, e.g. DFP jian, finishes on its
-        last launch)"""
+    def begin(self, model, accumulate=False, complete=True):
+        """per walk: how many launches contribute to each parameter (a module recorded twice, e.g. DFP jian, finishes on its
+        last launch).  Virtual ranks: the walks after a step's first one ``accumulate`` into the gradient the earlier walks
+        left, and only the step's last walk is ``complete``: its launches finish the gradients and launch the buckets."""
         self.touched.clear()
+        self.accumulate_all, self.complete = accumulate, complete
         self.pending = {}
+        self.work, self.launched = [], []
+        if not complete:
+            return
         for g in conv_groups_forward_order(model):
             n = self.uses.get(id(g[0]), 1)
             for m in g:
@@ -316,7 +357,6 @@ class FlatSink:
                 self.pending[id(p)] = 1
         for i, b in enumerate(self.buckets):
             b[2] = sum(1 for k, v in self.bucket_of.items() if v == i)
-        self.work, self.launched = [], []
 
     def _launch(self, b):
         self.launched.append((b[0], b[1]))
@@ -327,6 +367,8 @@ class FlatSink:
                 self.work.append(dist.all_reduce(self.fs.grad[b[0]:b[1]], op=dist.ReduceOp.SUM, async_op=True))
 
     def finish(self):
+        if not self.complete:
+            return
         for b in self.buckets:
             if (b[0], b[1]) not in self.launched:
                 self._launch(b)
@@ -340,18 +382,31 @@ class Trainer:
     [B, 3, H, W] and one label tensor (one backbone pass, model/backward.py ``_record``)."""
 
     def __init__(self, model, lr=0.01, momentum=0.9, weight_decay=5e-4, ema_decay=0.9998, use_ema=True,
-                 bucket_bytes=25 << 20, overlap=True, skip_nonfinite=False):
+                 bucket_bytes=25 << 20, overlap=True, skip_nonfinite=False, virtual_ranks=1):
         """``skip_nonfinite``: what ``GradScaler.step`` does for the reference's ``--fp16`` (double_trainer.py:113-119).
         Every optimiser step first checks the all-reduced flat gradient for NaN / +-inf on the device (sy_nonfinite_flag;
         every rank sees the same sums, so every rank decides the same); a flagged step leaves the parameters and momentum
         as they are, while the EMA copy still moves towards them with that step's decay and ``updates`` still counts, as
         ModelEMA.update does after a skipped step.  ``skipped_steps()`` reads the device counter (a synchronisation).
         The check reads the gradient before the unscale: with a loss scale of 1 or more the unscaled gradient is finite
-        exactly when it is."""
+        exactly when it is.
+
+        ``virtual_ranks`` = K: this process runs K ranks of a data-parallel run one after another, so that W processes
+        train as W x K ranks would (the reference's ``-d 8`` on fewer GPUs).  Every input batch holds K x B samples;
+        virtual rank k owns rows k*B .. (k+1)*B - 1 of the frames and of the labels.  Each virtual rank has its own
+        BatchNorm running statistics, ``num_batches_tracked`` and EMA buffers (``broadcast_buffers=False``); a step runs
+        K recording forwards and reverse walks on the K shards with rank k's buffers, the walks accumulating into one
+        flat gradient (the buckets are all-reduced over the W processes during the last walk), and the fused step
+        applies the mean over W x K.  ``step`` / ``replay`` return virtual rank 0's losses, ``rank_losses`` all K;
+        outside a step the module's buffers are rank 0's."""
         assert model.training and model.head.use_l1
         engine.require_bf16_training(model)
+        if int(virtual_ranks) != virtual_ranks or virtual_ranks < 1:
+            raise ValueError(f"Trainer: virtual_ranks must be a positive integer, got {virtual_ranks!r}")
+        self.virtual_ranks = int(virtual_ranks)
         self.model = model
-        self.fs = FlatState(model, ema=use_ema)
+        self.fs = FlatState(model, ema=use_ema, copies=self.virtual_ranks)
+        self._rank_loss = None                             # the loss vector of every virtual rank in the last step
         self.skip_nonfinite = bool(skip_nonfinite)
         dev = self.fs.state.device
         self._found_inf = torch.zeros(1, dtype=torch.float32, device=dev) if self.skip_nonfinite else None
@@ -404,18 +459,49 @@ class Trainer:
             engine.packed_operand(g[0], "_pkd", ws, ops.pack_conv_weight_dgrad, value=dg)
 
     def forward_backward(self, x, targets, loss_scale=1.0):
-        T, loss = backward._record(self.model, x, targets)
-        if self.sink is None:
-            self.sink = FlatSink(self.fs, dict(T.uses), self.bucket_bytes, self.overlap, self.world)
-        self.sink.uses = dict(T.uses)
-        self.sink.begin(self.model)
-        with torch.no_grad():
-            backward._walk(T, self.model.head, loss_scale, self.sink)
-        return loss
+        """The recording forward and reverse walk of every virtual rank on its shard; returns virtual rank 0's loss
+        vector.  Each rank's tape (activations, gradient arena) is dropped before the next rank records, so a captured
+        step's pool holds the activations of one rank."""
+        shards = self._shards(x, targets)
+        losses = []
+        for k, (xk, tk) in enumerate(shards):
+            self.fs.select(k)
+            T, loss = backward._record(self.model, xk, tk)
+            if self.sink is None:
+                self.sink = FlatSink(self.fs, dict(T.uses), self.bucket_bytes, self.overlap, self.world)
+            self.sink.uses = dict(T.uses)
+            self.sink.begin(self.model, accumulate=k > 0, complete=k == len(shards) - 1)
+            with torch.no_grad():
+                backward._walk(T, self.model.head, loss_scale, self.sink)
+            del T
+            losses.append(loss)
+        self.fs.select(0)
+        self._rank_loss = losses
+        return losses[0]
+
+    def _shards(self, x, targets):
+        """[(frames, labels)] of the virtual ranks: rows k*B .. (k+1)*B - 1 of ``x`` and of each label tensor"""
+        K = self.virtual_ranks
+        if K == 1:
+            return [(x, targets)]
+        n = x.shape[0]
+        labels = [targets] if torch.is_tensor(targets) else list(targets)
+        if n % K or any(t.shape[0] != n for t in labels):
+            raise ValueError(f"Trainer: a batch of {n} samples (labels {[tuple(t.shape) for t in labels]}) cannot be cut "
+                             f"into {K} virtual ranks of equal size")
+        b = n // K
+        cut = [[t[k * b:(k + 1) * b] for t in labels] for k in range(K)]
+        return [(x[k * b:(k + 1) * b], cut[k][0] if torch.is_tensor(targets) else tuple(cut[k])) for k in range(K)]
+
+    def rank_losses(self):
+        """The loss dicts of every virtual rank in the last step or replay, in rank order (device tensors; a replay
+        overwrites those of the graph it replays)."""
+        return [backward._loss_dict(v) for v in self._rank_loss]
 
     def _hyper_values(self, lr, loss_scale):
         d = self.ema_decay * (1 - math.exp(-self.updates / 2000)) if self.fs.ema is not None else 0.0
-        return [self.lr if lr is None else lr, self.momentum, self.weight_decay, 1.0 / (self.world * loss_scale), d, 1.0 - d]
+        return [self.lr if lr is None else lr, self.momentum, self.weight_decay,
+                1.0 / (self.world * self.virtual_ranks * loss_scale), d, 1.0 - d]
 
     def optimizer_step(self, lr=None, loss_scale=1.0, found_inf=None, hyper=None):
         if hyper is None:
@@ -513,24 +599,25 @@ class Trainer:
                 begin()
                 if prologue is not None:
                     prologue(key, x, targets)
-                loss = self.forward_backward(x, targets, loss_scale)
+                self.forward_backward(x, targets, loss_scale)
                 if self.world > 1:                         # the optimiser step waits for the collectives: its own segment
                     end()
                     begin()
                 self.optimizer_step(hyper=self._hyper)
                 end()
             self.sink.on_bucket = None
-            graphs[key] = (plan, loss, loss_scale, (x, targets))
+            graphs[key] = (plan, self._rank_loss, loss_scale, (x, targets))
             torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         return graphs
 
     def _replay(self, graph, lr):
-        plan, loss, loss_scale, _ = graph
+        plan, losses, loss_scale, _ = graph
         self.updates += 1
         self._stage_hyper(lr, loss_scale)
         self._replay_plan(plan)
-        return backward._loss_dict(loss)
+        self._rank_loss = losses
+        return backward._loss_dict(losses[0])
 
     def _stage_hyper(self, lr, loss_scale):
         """the hyper-parameter block of the captured graphs for the step ``updates``, through two pinned slots: a slot is
@@ -587,8 +674,22 @@ class Trainer:
             raise KeyError(f"replay_size: no graph captured for {size} (captured: {sorted(self._sized)})")
         return self._replay(self._sized[size], lr)
 
-    def ema_state_dict(self):
-        return self.fs.ema_state_dict(self.model)
+    def ema_state_dict(self, rank=0):
+        """the EMA model's state_dict as virtual rank ``rank`` holds it (its own EMA BatchNorm buffers)"""
+        return self._at_rank(rank, lambda: self.fs.ema_state_dict(self.model))
+
+    def model_state_dict(self, rank=0):
+        """a copy of ``model.state_dict()`` as virtual rank ``rank`` holds it (its own BatchNorm buffers)"""
+        return self._at_rank(rank, lambda: {k: t.clone() for k, t in self.model.state_dict().items()})
+
+    def _at_rank(self, rank, fn):
+        if not 0 <= rank < self.virtual_ranks:
+            raise ValueError(f"virtual rank {rank} of {self.virtual_ranks}")
+        self.fs.select(rank)
+        try:
+            return fn()
+        finally:
+            self.fs.select(0)
 
     def skipped_steps(self):
         """How many optimiser steps ``skip_nonfinite`` has skipped so far (reads the device counter: a synchronisation);
@@ -611,10 +712,25 @@ class Trainer:
 
         As with ``nn.Module.state_dict`` the tensors are views of the live buffers: the weights, the momentum and the EMA
         copy each share one storage, so ``torch.save`` writes each of them once.  ``copy.deepcopy`` it for a snapshot in
-        memory.  BatchNorm statistics are per rank, so with several ranks each rank saves its own."""
-        return {"model": self.model.state_dict(), "optimizer": self.optimizer_state_dict(),
-                "ema": None if self.fs.ema is None else self.fs.views(self.model, self.fs.ema),
-                "updates": self.updates, "lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay}
+        memory.  BatchNorm statistics are per rank, so with several ranks each rank saves its own.
+
+        With ``virtual_ranks`` K > 1, "model" and "ema" hold virtual rank 0's buffers and one more entry holds every
+        rank's:
+
+            "virtual_ranks" [{"buffers": the model's buffer entries, "ema": the EMA model's, or None}] x K"""
+        sd = {"model": self.model.state_dict(), "optimizer": self.optimizer_state_dict(),
+              "ema": None if self.fs.ema is None else self.fs.views(self.model, self.fs.ema),
+              "updates": self.updates, "lr": self.lr, "momentum": self.momentum, "weight_decay": self.weight_decay}
+        if self.virtual_ranks > 1:
+            sd["virtual_ranks"] = [self._at_rank(k, self._rank_buffers) for k in range(self.virtual_ranks)]
+        return sd
+
+    def _rank_buffers(self):
+        """the selected virtual rank's buffer entries of the model and of the EMA model, as views"""
+        names = [n for n, _ in self.model.named_buffers()]
+        ema = None if self.fs.ema is None else self.fs.views(self.model, self.fs.ema)
+        return {"buffers": {n: t.detach() for n, t in self.model.named_buffers()},
+                "ema": None if ema is None else {n: ema[n].detach() for n in names}}
 
     def load_state_dict(self, sd):
         """Continue from a ``state_dict()`` of a Trainer of the same architecture and EMA setting: the next step computes
@@ -622,6 +738,10 @@ class Trainer:
         if (sd["ema"] is None) != (self.fs.ema is None):
             raise ValueError(f"load_state_dict: the state was saved {'without' if sd['ema'] is None else 'with'} EMA, "
                              f"this Trainer runs {'with' if self.fs.ema is not None else 'without'} it")
+        ranks = sd.get("virtual_ranks")
+        if (1 if ranks is None else len(ranks)) != self.virtual_ranks:
+            raise ValueError(f"load_state_dict: the state holds {1 if ranks is None else len(ranks)} virtual ranks, this "
+                             f"Trainer runs {self.virtual_ranks}")
         self._check_entries(sd["model"], "model")
         if self.fs.ema is not None:
             self._check_entries(sd["ema"], "ema")
@@ -632,6 +752,9 @@ class Trainer:
                 for k, t in self.fs.views(self.model, self.fs.ema).items():
                     if t.dtype == torch.float32:
                         t.copy_(sd["ema"][k])
+        if ranks is not None:
+            for k in range(self.virtual_ranks):
+                self._at_rank(k, lambda: self._load_rank_buffers(ranks[k]))
         self.updates = int(sd["updates"])
         self.lr, self.momentum, self.weight_decay = sd["lr"], sd["momentum"], sd["weight_decay"]
         self._state_changed()
@@ -697,6 +820,10 @@ class Trainer:
         self._check_entries(ckpt["model"], "ckpt['model']")
         self.load_optimizer_state_dict(ckpt["optimizer"])
         self._load_model(ckpt["model"])
+        with torch.no_grad():                              # every reference rank loads the same file
+            for k in range(1, self.virtual_ranks):
+                self.fs.buffer_copy(k).copy_(self.fs.buffer_copy(0))
+                self.fs.int_copies[k].copy_(self.fs.int_copies[0])
         if self.fs.ema is not None:
             self.fs.ema.copy_(self.fs.state)
         self.updates = int(updates)
@@ -709,13 +836,30 @@ class Trainer:
         rank during training (``broadcast_buffers=False``); they are the flat state's float-buffer region, so this is ONE
         all-reduce (SUM, then / world: yolox's ``op="mean"``).  BatchNorm weights and biases (parameters, updated with the
         mean gradient) and num_batches_tracked are equal on all ranks already.  Runs on the current stream and is not meant
-        for a captured graph.  No-op in one process."""
-        if self.world == 1:
+        for a captured graph.  No-op in one process of one virtual rank.
+
+        With ``virtual_ranks`` K the mean is over W x K ranks: the K copies are summed in rank order, the sum is
+        all-reduced over the W processes and divided by W x K, and every copy receives the mean."""
+        if self.world * self.virtual_ranks == 1:
             return
-        stats = self.fs.state[self.fs.n_param:self.fs.n_total]
-        dist.all_reduce(stats, op=dist.ReduceOp.SUM)
-        stats.div_(self.world)
+        stats = self.fs.buffer_copy(0)
+        for k in range(1, self.virtual_ranks):
+            stats.add_(self.fs.buffer_copy(k))
+        if self.world > 1:
+            dist.all_reduce(stats, op=dist.ReduceOp.SUM)
+        stats.div_(self.world * self.virtual_ranks)
+        for k in range(1, self.virtual_ranks):
+            self.fs.buffer_copy(k).copy_(stats)
         self._state_changed()
+
+    def _load_rank_buffers(self, entry):
+        live = self._rank_buffers()
+        with torch.no_grad():
+            for which in ("buffers", "ema"):
+                if live[which] is None:
+                    continue
+                for n, t in live[which].items():
+                    t.copy_(entry[which][n])
 
     def _check_entries(self, sd, what):
         want = self.model.state_dict()

@@ -166,6 +166,7 @@ class DeviceTrainer:
     """The loop of the reference trainer (module docstring); combined with the reference class by ``device_trainer``."""
 
     step_class = DeviceStep   # the device half (a stand-in in the CPU tests)
+    virtual_ranks = 1         # ranks run one after another in this process (dropin.install(trainer=True, virtual_ranks=K))
     max_bytes = None          # the longest JPEG file a batch takes; default: the longest training file, rounded up to 4 KiB
     _helpers = None           # the module whose yolox helpers the loop calls (the reference class's)
 
@@ -219,15 +220,17 @@ class DeviceTrainer:
         self.train_loader = exp.get_data_loader(batch_size=args.batch_size, is_distributed=self.is_distributed,
                                                 no_aug=self.no_aug, cache_img=args.cache)
         self.table = BatchTable(self.train_loader)
-        self.max_iter = len(self.train_loader)
+        self._virtual = self._virtual_samplers()
+        self.max_iter = len(self.train_loader) if self._virtual is None else len(self._virtual[0])
         self.lr_scheduler = exp.get_lr_scheduler(exp.basic_lr_per_img * args.batch_size, self.max_iter)
         if args.occupy:
             self._h("occupy_mem")(self.local_rank)
         model.head.use_l1 = True                        # before_epoch's switch (no mosaic epoch is left), :209-217
         exp.eval_interval = 1
         self.eval_model = copy.deepcopy(model)          # before the Trainer turns the parameters into views
+        vr = {} if self._virtual is None else {"virtual_ranks": self.virtual_ranks}
         self.tr = self.make_trainer(model, lr=lr0, momentum=exp.momentum, weight_decay=exp.weight_decay,
-                                    use_ema=exp.ema, skip_nonfinite=bool(args.fp16))
+                                    use_ema=exp.ema, skip_nonfinite=bool(args.fp16), **vr)
         if self._resume is not None:
             self.tr.load_reference_checkpoint(self._resume, self.max_iter * self.start_epoch)
             self._resume = None
@@ -235,6 +238,9 @@ class DeviceTrainer:
         self.model = model
         self._start_feed()
         self.evaluator = exp.get_evaluator(batch_size=args.batch_size, is_distributed=self.is_distributed)
+        if self._virtual is not None and not hasattr(self.evaluator, "evaluate_virtual_ranks"):
+            raise ValueError(f"DeviceTrainer: virtual ranks evaluate one shard per rank through the device evaluator "
+                             f"(dropin.install(evaluators=True)); the cfg's evaluator is a {type(self.evaluator).__name__}")
         if self.rank == 0:
             if args.logger == "tensorboard":
                 self.tblogger = self._h("SummaryWriter")(os.path.join(self.file_name, "tensorboard"))
@@ -248,6 +254,31 @@ class DeviceTrainer:
                 raise ValueError("logger must be either 'tensorboard' or 'wandb'")
         logger.info("Training start...")
         logger.info("\n{}".format(model))
+
+    def _virtual_samplers(self):
+        """Virtual ranks (K > 1): the batch sampler of every virtual rank g = rank * K + k of a W x K-rank run, what
+        ``get_data_loader`` builds for rank g of W x K (a batch of ``args.batch_size // (W x K)``), rebuilt from the
+        loader's own yolox InfiniteSampler (its size, shuffle and seed) and YoloBatchSampler (drop_last, mosaic).  None
+        for K = 1: the loader's own batch sampler is iterated."""
+        K = self.virtual_ranks
+        if K == 1:
+            return None
+        bs = self.train_loader.batch_sampler
+        sampler = getattr(bs, "sampler", None)
+        if type(sampler).__name__ != "InfiniteSampler" or type(bs).__name__ != "YoloBatchSampler":
+            raise ValueError(f"DeviceTrainer: virtual ranks rebuild yolox's InfiniteSampler inside a YoloBatchSampler; the "
+                             f"loader has a {type(sampler).__name__} inside a {type(bs).__name__}")
+        G = sampler._world_size * K
+        B = self.args.batch_size // G
+        if B == 0:
+            raise ValueError(f"DeviceTrainer: a batch of {self.args.batch_size} leaves no sample for each of {G} ranks "
+                             f"({sampler._world_size} processes x {K} virtual ranks)")
+        out = []
+        for k in range(K):
+            s = type(sampler)(sampler._size, shuffle=sampler._shuffle, seed=sampler._seed)
+            s._rank, s._world_size = self.rank * K + k, G      # it takes them from torch.distributed when initialised
+            out.append(type(bs)(sampler=s, batch_size=B, drop_last=bs.drop_last, mosaic=bs.mosaic))
+        return out
 
     def resume_train(self, model):
         """double_trainer.py:285-318.  ``--resume``: the checkpoint is read here and loaded into the native Trainer once
@@ -279,11 +310,16 @@ class DeviceTrainer:
             max_bytes = feed.default_max_bytes(p for a in t.annotations for p in feed.sample(a, t.frames)[0])
         else:
             max_bytes = feed.check_max_bytes(self.max_bytes, "DeviceTrainer: max_bytes")
-        self._batches = iter(self.train_loader.batch_sampler)
-        self._rng = np.random.default_rng([int(self.exp.seed or 0), int(self.rank)])
+        K = self.virtual_ranks
+        if self._virtual is None:
+            self._batches = iter(self.train_loader.batch_sampler)
+            batch = self.train_loader.batch_sampler.batch_size
+        else:                                           # the virtual ranks' batches side by side, in rank order
+            self._batches = ([i for part in parts for i in part] for parts in zip(*self._virtual))
+            batch = K * self._virtual[0].batch_size
+        self._rngs = [np.random.default_rng([int(self.exp.seed or 0), int(self.rank) * K + k]) for k in range(K)]
         self._reader = ThreadPoolExecutor(max_workers=1)
         self._left = (self.max_epoch - self.start_epoch) * self.max_iter       # iterations still to be read
-        batch = self.train_loader.batch_sampler.batch_size
         sizes = train.multiscale_sizes(self.exp.input_size, self.exp.random_size)
         self.step = self.step_class(self.tr, t, batch, self.exp.input_size, sizes, max_bytes, self.device)
         self._reads, self._k, self._pending = [], 0, []
@@ -300,7 +336,10 @@ class DeviceTrainer:
         self._left -= 1
         s = (self._k + len(self._reads)) % 2
         idx = [_index(i) for i in next(self._batches)]
-        mirror = self._rng.integers(0, 2, len(idx)) if self.table.frames == 2 else np.zeros(len(idx), np.int64)
+        if self.table.frames == 2:                      # each (virtual) rank draws its own samples' bits
+            mirror = np.concatenate([r.integers(0, 2, len(idx) // len(self._rngs)) for r in self._rngs])
+        else:
+            mirror = np.zeros(len(idx), np.int64)
         self._reads.append((idx, self._reader.submit(self._read, s, idx, mirror)))
 
     def _read(self, s, idx, mirror):
@@ -406,11 +445,21 @@ class DeviceTrainer:
 
     def evaluate_and_save_model(self):
         """The evaluator gets ``eval_model``, a copy taken before the Trainer was built, holding the EMA weights
-        (``tr.ema_state_dict()``), or the live weights without EMA; never the training model itself."""
-        sd = self.tr.ema_state_dict() if self.use_model_ema else self.model.state_dict()
-        self.eval_model.load_state_dict(sd)
+        (``tr.ema_state_dict()``), or the live weights without EMA; never the training model itself.  Virtual ranks:
+        ``DeviceEvaluator.evaluate_virtual_ranks`` evaluates rank g's ``DistributedSampler`` shard of a W x K-rank run
+        with rank g's weights (its EMA BatchNorm buffers), in batches of ``args.batch_size // (W x K)``, and scores
+        the rows of all ranks once, in rank order, as the reference's ranks and its gather do."""
+        def load(k):
+            sd = self.tr.ema_state_dict(k) if self.use_model_ema else self.tr.model_state_dict(k)
+            self.eval_model.load_state_dict(sd)
+
         with self._h("adjust_status")(self.eval_model, training=False):
-            ap50_95, ap50, summary = self.exp.eval(self.eval_model, self.evaluator, self.is_distributed)
+            if self._virtual is None:
+                load(0)
+                ap50_95, ap50, summary = self.exp.eval(self.eval_model, self.evaluator, self.is_distributed)
+            else:       # every virtual rank's DistributedSampler shard with its own weights, scored once
+                ap50_95, ap50, summary = self.evaluator.evaluate_virtual_ranks(
+                    self.eval_model, load, self.virtual_ranks, self._virtual[0].batch_size, self.is_distributed)
         update_best_ckpt = ap50_95 > self.best_ap
         self.best_ap = max(self.best_ap, ap50_95)
         if self.rank == 0:
