@@ -691,6 +691,40 @@ typedef struct SyYuvToBgrSizedDesc {
 } SyYuvToBgrSizedDesc;
 int sy_yuv_to_bgr_sized(const SyYuvToBgrSizedDesc* d, sy_stream_t stream);
 
+/* 8-bit Bayer mosaics of camera streams of different sizes -> uint8 BGR frames at the top-left of the same slots,
+ * bit-identical to cv2.cvtColor(raw, COLOR_Bayer<pattern>2BGR) (bilinear) or COLOR_Bayer<pattern>2BGR_EA (edge-aware).
+ * Off the border (rows 1..h-2, columns 1..w-2) a pixel keeps its own colour; at a green site the colour of the left and
+ * right neighbours is their mean (a + b + 1) >> 1 and that of the upper and lower neighbours theirs; at a red or blue
+ * site the other of the two is the mean of the four diagonals (a + b + c + d + 2) >> 2 and green is the mean of the four
+ * edge neighbours (bilinear) or, edge-aware, of the vertical pair where |left - right| > |up - down|, else of the
+ * horizontal pair.  Column 0 copies column 1 and column w-1 column w-2, then row 0 copies row 1 and row h-1 row h-2.  A
+ * frame of fewer than 3 rows or columns is black, as cv2 makes it.  Frame i is the first h * w bytes of row i of src,
+ * row-major [h][w]; the pattern is the colour order of its top-left 2x2 (cv2's RGGB codes alias its BG ones): */
+enum {
+  SY_BAYER_RGGB = 0,   /* COLOR_BayerRGGB2BGR[_EA] = COLOR_BayerBG2BGR[_EA] */
+  SY_BAYER_BGGR = 1,   /* COLOR_BayerBGGR2BGR[_EA] = COLOR_BayerRG2BGR[_EA] */
+  SY_BAYER_GBRG = 2,   /* COLOR_BayerGBRG2BGR[_EA] = COLOR_BayerGR2BGR[_EA] */
+  SY_BAYER_GRBG = 3    /* COLOR_BayerGRBG2BGR[_EA] = COLOR_BayerGB2BGR[_EA] */
+};
+enum {
+  SY_DEMOSAIC_BILINEAR = 0,   /* COLOR_Bayer*2BGR */
+  SY_DEMOSAIC_EA = 1          /* COLOR_Bayer*2BGR_EA (value 2 is kept for VNG, not built) */
+};
+/* sizes[i] = (h, w) of frame i.  A row with h = 0 means no frame this tick; a row that does not fit the slot, or whose
+ * h * w is more than max_bytes, also leaves slot i untouched.  Nothing of slot i outside frame i's h x w is written.
+ * Reads no byte of row i past frame i's own h * w, only device memory; never synchronises (capturable). */
+typedef struct SyBayerToBgrSizedDesc {
+  const uint8_t* src;      /* [n][max_bytes] */
+  int32_t n;
+  int64_t max_bytes;       /* row pitch of src */
+  const int32_t* sizes;    /* [n][2] device int32: h, w */
+  int32_t pattern;         /* SY_BAYER_* */
+  int32_t algo;            /* SY_DEMOSAIC_* */
+  int32_t slot_h, slot_w;
+  uint8_t* out;            /* [n][slot_h][slot_w][3] BGR */
+} SyBayerToBgrSizedDesc;
+int sy_bayer_to_bgr_sized(const SyBayerToBgrSizedDesc* d, sy_stream_t stream);
+
 /* ---- JPEG decode ----
  * Batched decode of the training frames' JPEG files into what cv2.imread(path) returns for them (uint8 BGR, bit-identical),
  * replacing the host decodes of exps/dataset/tal_flip_one_future_argoversedataset.py:195,216,

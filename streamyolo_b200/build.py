@@ -34,6 +34,7 @@ SOURCES = {
     "forecast.cu": ["-fmad=false"],
     "jpeg.cu": [],
     "yuv.cu": [],
+    "bayer.cu": [],
     "jpeg_encode.cu": [],
     "vis.cu": [],
     "vis_det.cu": [],

@@ -162,6 +162,12 @@ class SyYuvToBgrSizedDesc(C.Structure):
                 ("format", C.c_int32), ("slot_h", C.c_int32), ("slot_w", C.c_int32), ("out", C.c_void_p)]
 
 
+class SyBayerToBgrSizedDesc(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("n", C.c_int32), ("max_bytes", C.c_int64), ("sizes", C.c_void_p),
+                ("pattern", C.c_int32), ("algo", C.c_int32), ("slot_h", C.c_int32), ("slot_w", C.c_int32),
+                ("out", C.c_void_p)]
+
+
 class SyJpegEncodeDesc(C.Structure):
     _fields_ = [("src", C.c_void_p), ("sizes", C.c_void_p), ("n", C.c_int32), ("max_h", C.c_int32), ("max_w", C.c_int32),
                 ("quality", C.c_int32), ("out", C.c_void_p), ("max_bytes", C.c_int64), ("lengths", C.c_void_p),
@@ -303,6 +309,7 @@ _SIG = {
     "sy_jpeg_decode_sized_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int64, C.c_int32, C.c_int32]),
     "sy_jpeg_decode_sized": (C.c_int, [C.POINTER(SyJpegDecodeSizedDesc), C.c_void_p]),
     "sy_yuv_to_bgr_sized": (C.c_int, [C.POINTER(SyYuvToBgrSizedDesc), C.c_void_p]),
+    "sy_bayer_to_bgr_sized": (C.c_int, [C.POINTER(SyBayerToBgrSizedDesc), C.c_void_p]),
     "sy_jpeg_encode_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int64]),
     "sy_jpeg_encode_max_bytes": (C.c_int64, [C.c_int32, C.c_int32]),
     "sy_jpeg_encode": (C.c_int, [C.POINTER(SyJpegEncodeDesc), C.c_void_p]),
@@ -1227,6 +1234,32 @@ def yuv_to_bgr_sized(src, sizes, fmt, out):
     d = SyYuvToBgrSizedDesc(src.data_ptr(), n, max_bytes, sizes.data_ptr(), YUV_FORMATS[fmt], out.shape[1], out.shape[2],
                             out.data_ptr())
     _check(lib().sy_yuv_to_bgr_sized(C.byref(d), _stream()))
+
+
+# the colour order of a mosaic's top-left 2x2 -> SY_BAYER_* of sy_bayer_to_bgr_sized (cv2's COLOR_BayerRGGB2BGR, ... --
+# the aliases of COLOR_BayerBG2BGR, _RG, _GR, _GB), and the demosaicing -> SY_DEMOSAIC_* (COLOR_Bayer*2BGR, ..._EA)
+BAYER_PATTERNS = {"rggb": 0, "bggr": 1, "gbrg": 2, "grbg": 3}
+DEMOSAIC = {"bilinear": 0, "ea": 1}
+
+
+def bayer_to_bgr_sized(src, sizes, pattern, algo, out):
+    """8-bit Bayer mosaics -> uint8 BGR slots (sy_bayer_to_bgr_sized), cv2.cvtColor(COLOR_Bayer*2BGR[_EA]) bit for bit:
+    ``src`` uint8 [n, max_bytes], frame i the first h * w bytes of row i, row-major [h, w]; ``pattern`` a BAYER_PATTERNS
+    key (the colour order of the top-left 2x2), ``algo`` a DEMOSAIC key; ``sizes`` int32 [n, 2] (h, w), h = 0 for no
+    frame; ``out`` uint8 [n, slot_h, slot_w, 3], frame i at the top-left of slot i.  A row with no frame, or a frame that
+    does not fit, leaves its slot untouched."""
+    _require(pattern in BAYER_PATTERNS,
+             f"bayer_to_bgr_sized: unknown pattern {pattern!r} (one of {', '.join(BAYER_PATTERNS)})")
+    _require(algo in DEMOSAIC, f"bayer_to_bgr_sized: unknown demosaicing {algo!r} (one of {', '.join(DEMOSAIC)})")
+    _require(_tensor_ok(src, torch.uint8, 2) and src.is_cuda, "bayer_to_bgr_sized: src must be contiguous CUDA uint8 [n, max_bytes]")
+    n, max_bytes = src.shape
+    _require(_tensor_ok(sizes, torch.int32, 2) and tuple(sizes.shape) == (n, 2) and sizes.device == src.device,
+             f"bayer_to_bgr_sized: sizes must be int32 [{n}, 2] on src's device")
+    _require(_tensor_ok(out, torch.uint8, 4) and out.shape[0] == n and out.shape[3] == 3 and out.device == src.device,
+             f"bayer_to_bgr_sized: out must be contiguous uint8 [{n}, slot_h, slot_w, 3] on src's device")
+    d = SyBayerToBgrSizedDesc(src.data_ptr(), n, max_bytes, sizes.data_ptr(), BAYER_PATTERNS[pattern], DEMOSAIC[algo],
+                              out.shape[1], out.shape[2], out.data_ptr())
+    _check(lib().sy_bayer_to_bgr_sized(C.byref(d), _stream()))
 
 
 def jpeg_encode_max_bytes(h, w):

@@ -31,7 +31,13 @@ Raw camera frames (YUV, as ISPs, hardware codecs, V4L2 and GMSL deliver them):
     det.step([nv12_0, nv12_1])                    # uint8 [h * 3 // 2, w] each, what cv2.cvtColor(COLOR_YUV2BGR_NV12) takes
 
 Then the tick starts with the conversion of the S frames to BGR (sy_yuv_to_bgr_sized, cv2.cvtColor bit for bit) into the
-slots; only each frame's own bytes cross to the device.
+slots; only each frame's own bytes cross to the device.  Raw sensor frames (8-bit Bayer mosaics, before any ISP) likewise:
+
+    det = StreamDetector(model, frame_sizes=[(1200, 1920)] * 8, input_size=(600, 960), frame_format="bayer_rggb",
+                         demosaic="ea")
+    det.step(raws)                                # uint8 [h, w] each, what cv2.cvtColor(COLOR_BayerRGGB2BGR_EA) takes
+
+and the tick starts with their demosaicing (sy_bayer_to_bgr_sized, cv2.cvtColor bit for bit).
 
 The graph reads the weights and the folded BatchNorm as they were at capture: after ``load_state_dict`` (or any other
 change of the weights or running statistics) call ``capture()`` again.  Nothing checks this per frame.
@@ -55,14 +61,16 @@ class StreamTick:
     ratio --, obj, class_conf, class_pred) and ``count`` ([S] rows of ``det``) are the outputs; ``buffer`` holds each
     stream's features carried to the next tick.  With a YUV ``frame_format`` (an ops.YUV_FORMATS key) the input is ``yuv``
     (uint8 [S, max_bytes], stream i's frame in cv2's layout in the first bytes of row i), converted inside the tick into
-    ``frames``.  With ``record_quality`` the tick ends with the JPEG encode of the frames in ``frames`` (``rec_out``,
-    ``rec_len``, ``rec_status``).  With ``record_boxes`` = (fp32 score threshold, uint8 [P, 3] BGR palette on the device)
+    ``frames``; with a Bayer one (BAYER_FORMATS) it is ``bayer`` (uint8 [S, max_bytes], stream i's [h, w] mosaic in the
+    first h * w bytes of row i), demosaiced inside the tick into ``frames`` with ``demosaic`` (an ops.DEMOSAIC key).
+    With ``record_quality`` the tick ends with the JPEG encode of the frames in ``frames`` (``rec_out``, ``rec_len``,
+    ``rec_status``).  With ``record_boxes`` = (fp32 score threshold, uint8 [P, 3] BGR palette on the device)
     the encode reads ``rec_frames`` instead: a copy of ``frames`` with the tick's detections drawn (sy_vis_det_boxes,
     sy_draw_boxes), so ``frames``, which a later tick may read again, is never drawn on."""
 
     def __init__(self, model, table, ratios, size, streams, conf_thre, nms_thre, device, jpeg_max_bytes=None,
                  forecast=None, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None,
-                 record_boxes=None):
+                 record_boxes=None, demosaic="bilinear"):
         self.model, self.size = model, tuple(size)
         self.conf_thre, self.nms_thre = float(conf_thre), float(nms_thre)
         table = np.asarray(table, np.int32)
@@ -78,8 +86,12 @@ class StreamTick:
         self.buffer = None
         self.raw = self.det = self.count = None
         self.status = None
-        self.yuv = None
-        if frame_format != "bgr":
+        self.yuv = self.bayer = None
+        if frame_format in BAYER_FORMATS:
+            self.bayer_pattern, self.demosaic = frame_format[len("bayer_"):], demosaic
+            self.bayer = torch.zeros((streams, int((table[:, 0] * table[:, 1]).max())), dtype=torch.uint8, device=device)
+            self.bayer_sizes = self.table[:, :2].contiguous()
+        elif frame_format != "bgr":
             self.yuv_format = frame_format
             self.yuv = torch.zeros((streams, max(int(np.prod(frame_shape(frame_format, h, w))) for h, w in table[:, :2])),
                                    dtype=torch.uint8, device=device)
@@ -132,6 +144,8 @@ class StreamTick:
             ops.jpeg_decode_sized(self.bytes, self.lengths, self.sizes, self.frames, self.status, self.workspace)
         if self.yuv is not None:
             ops.yuv_to_bgr_sized(self.yuv, self.yuv_sizes, self.yuv_format, self.frames)
+        if self.bayer is not None:
+            ops.bayer_to_bgr_sized(self.bayer, self.bayer_sizes, self.bayer_pattern, self.demosaic, self.frames)
         ops.stream_gate(self.status, self.flags, self.start, self.keep)
         ops.letterbox_sized(self.frames, self.table, self.x)
         with torch.no_grad(), engine.forward_scope(ctx.device):
@@ -211,6 +225,11 @@ def sized_output(det):
 
 
 FRAME_FORMATS = ("bgr",) + tuple(ops.YUV_FORMATS)
+# raw 8-bit Bayer mosaics, named by the colour order of their top-left 2x2 (ops.BAYER_PATTERNS)
+BAYER_FORMATS = tuple("bayer_" + p for p in ops.BAYER_PATTERNS)
+# the smallest Bayer frame: one whole 2x2 colour cell.  cv2 is reproducible at every size on a contiguous frame; below
+# 3 rows or columns it is black (and so is the device's)
+BAYER_MIN_HW = (2, 2)
 
 
 def record_boxes_args(record_boxes, record_quality, num_classes):
@@ -237,9 +256,12 @@ def record_boxes_args(record_boxes, record_quality, num_classes):
 
 
 def frame_shape(fmt, h, w):
-    """the uint8 array ``step`` takes for one h x w frame of ``fmt`` (a FRAME_FORMATS entry), in cv2's layout"""
+    """the uint8 array ``step`` takes for one h x w frame of ``fmt`` (a FRAME_FORMATS or BAYER_FORMATS entry), in cv2's
+    layout"""
     if fmt == "bgr":
         return h, w, 3
+    if fmt in BAYER_FORMATS:
+        return h, w
     return (h * 3 // 2, w) if fmt in ("nv12", "nv21", "i420", "yv12") else (h, w, 2)
 
 
@@ -283,7 +305,13 @@ class StreamDetector:
                       "i420", "yv12" (4:2:0: uint8 [h * 3 // 2, w], even h and w) or "yuyv", "uyvy" (4:2:2: uint8
                       [h, w, 2], even w): they take the camera's frames in cv2's layout, and the replay starts with their
                       conversion to BGR (sy_yuv_to_bgr_sized, cv2.cvtColor(COLOR_YUV2BGR_NV12, _NV21, _I420, _YV12,
-                      _YUY2, _UYVY) bit for bit).  Not with ``jpeg_max_bytes``
+                      _YUY2, _UYVY) bit for bit).  "bayer_rggb", "bayer_bggr", "bayer_gbrg", "bayer_grbg" (BAYER_FORMATS:
+                      8-bit sensor mosaics, uint8 [h, w], named by the colour order of the top-left 2x2; h and w at least
+                      2): the replay starts with their demosaicing (sy_bayer_to_bgr_sized, cv2.cvtColor(COLOR_BayerRGGB2BGR,
+                      _BGGR2BGR, _GBRG2BGR, _GRBG2BGR, with the _EA codes for ``demosaic="ea"``) bit for bit).  Not with
+                      ``jpeg_max_bytes``
+      demosaic        with a Bayer frame_format: "bilinear" (the default, cv2's COLOR_Bayer*2BGR) or "ea" (edge-aware,
+                      COLOR_Bayer*2BGR_EA)
     The sAP toolkit's streamer (sAP/forecast/streamer.py, see streamyolo_b200.streamer), with ``forecast=True``:
       clear_on_empty  True: an empty detection leaves the stream without tracks, as the streamer's association does
                       (the default keeps the predicted tracks, as pps_forecast_kf.py does)
@@ -310,7 +338,7 @@ class StreamDetector:
     def __init__(self, model, frame_hw=(1200, 1920), in_scale=0.5, streams=1, conf_thre=0.01, nms_thre=0.65,
                  frame_sizes=None, input_size=None, jpeg_max_bytes=None, forecast=False, match_iou_th=0.3,
                  max_tracks=1024, clear_on_empty=False, queries=0, frame_format="bgr", record_quality=None,
-                 record_boxes=None):
+                 record_boxes=None, demosaic="bilinear"):
         if model.training:
             raise ValueError("StreamDetector: the model must be in eval mode (model.eval())")
         if int(streams) != streams or streams < 1:
@@ -329,12 +357,23 @@ class StreamDetector:
             raise ValueError(f"StreamDetector: frames {sizes} at in_scale {in_scale} give input size {size}")
         if jpeg_max_bytes is not None:
             jpeg_max_bytes = feed.check_max_bytes(jpeg_max_bytes, "StreamDetector: jpeg_max_bytes")
-        if frame_format not in FRAME_FORMATS:
-            raise ValueError(f"StreamDetector: unknown frame_format {frame_format!r} (one of {', '.join(FRAME_FORMATS)})")
-        if frame_format != "bgr":
-            if jpeg_max_bytes is not None:
-                raise ValueError(f"StreamDetector: frame_format {frame_format!r} takes raw frames, jpeg_max_bytes JPEG "
-                                 "files: give one or the other")
+        if frame_format not in FRAME_FORMATS + BAYER_FORMATS:
+            raise ValueError(f"StreamDetector: unknown frame_format {frame_format!r} (one of "
+                             f"{', '.join(FRAME_FORMATS + BAYER_FORMATS)})")
+        if demosaic not in ops.DEMOSAIC:
+            raise ValueError(f"StreamDetector: unknown demosaic {demosaic!r} (one of {', '.join(ops.DEMOSAIC)})")
+        if demosaic != "bilinear" and frame_format not in BAYER_FORMATS:
+            raise ValueError(f"StreamDetector: demosaic={demosaic!r} takes a Bayer frame_format "
+                             f"({', '.join(BAYER_FORMATS)}), not {frame_format!r}")
+        if frame_format != "bgr" and jpeg_max_bytes is not None:
+            raise ValueError(f"StreamDetector: frame_format {frame_format!r} takes raw frames, jpeg_max_bytes JPEG "
+                             "files: give one or the other")
+        if frame_format in BAYER_FORMATS:
+            small = [s for s in sizes if s[0] < BAYER_MIN_HW[0] or s[1] < BAYER_MIN_HW[1]]
+            if small:
+                raise ValueError(f"StreamDetector: {frame_format} frames need at least {BAYER_MIN_HW[0]} rows and "
+                                 f"{BAYER_MIN_HW[1]} columns (one whole colour cell); not {small[0]}")
+        elif frame_format != "bgr":
             sub420 = len(frame_shape(frame_format, 2, 2)) == 2
             odd = [s for s in sizes if s[1] % 2 or (sub420 and s[0] % 2)]
             if odd:
@@ -360,14 +399,15 @@ class StreamDetector:
         self.model, self.streams, self.in_scale, self.size = model, streams, in_scale, size
         self.frame_sizes, self.ratios = sizes, ratios
         self.jpeg_max_bytes = jpeg_max_bytes
-        self.frame_format = frame_format
+        self.frame_format, self.demosaic = frame_format, demosaic
         self.forecasting = bool(forecast)
         self.queries = int(queries)
         self._tick = StreamTick(model, table, ratios, size, streams, conf_thre, nms_thre, dev, self.jpeg_max_bytes,
                                 (match_iou_th, int(max_tracks)) if forecast else None, clear_on_empty, self.queries,
                                 frame_format, None if record_quality is None else int(record_quality),
                                 None if record_boxes is None else (record_boxes[0],
-                                                                   torch.from_numpy(record_boxes[1]).to(dev)))
+                                                                   torch.from_numpy(record_boxes[1]).to(dev)),
+                                demosaic)
         self.record_quality = None if record_quality is None else int(record_quality)
         if self.record_quality is not None:
             self._rec_len = feed.pinned((streams,), torch.int64)
@@ -439,10 +479,10 @@ class StreamDetector:
         return self._run(None, fidx)
 
     def _inputs(self):
-        """the tick's buffer ``step`` copies the frames to (``frames``, or ``yuv`` for a YUV frame_format), each stream's
-        frame shape in it and the pinned stage (stream i's frame staged at the start of row i)"""
+        """the tick's buffer ``step`` copies the frames to (``frames``, ``yuv`` for a YUV frame_format or ``bayer`` for a
+        Bayer one), each stream's frame shape in it and the pinned stage (stream i's frame staged at the start of row i)"""
         t = self._tick
-        self._in = t.frames if t.yuv is None else t.yuv
+        self._in = t.yuv if t.yuv is not None else t.bayer if t.bayer is not None else t.frames
         self._shapes = [frame_shape(self.frame_format, h, w) for h, w in self.frame_sizes]
         self._stage = feed.pinned(tuple(self._in.shape), torch.uint8)
 
@@ -461,7 +501,7 @@ class StreamDetector:
                 ops._require(src.dtype == torch.uint8 and tuple(src.shape) == shape, f"StreamDetector.step: frame {i} must "
                              f"be uint8 {list(shape)}, not {src.dtype} {list(src.shape)}")
                 n = src.numel()
-                dst = t.frames[i, :h, :w] if t.yuv is None else t.yuv[i, :n].view(shape)
+                dst = t.frames[i, :h, :w] if self._in is t.frames else self._in[i, :n].view(shape)
                 if src.is_cuda:
                     dst.copy_(src)
                 else:                                 # only the frame's own bytes cross, not the whole slot
